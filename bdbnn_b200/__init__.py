@@ -1,4 +1,4 @@
-"""bdbnn_b200 — B200-native (sm_100a) implementation of BD-BNN's training hot path:
+"""bdbnn_b200 — H100-native (sm_90a) implementation of BD-BNN's training hot path:
 binarised conv2d fwd/bwd, kurtosis regulariser, KD losses (see DESIGN.md)."""
 from .modules import BinarizeConv2d, HardBinaryConv, HardBinaryConv_react, HardBinaryConv_cifar
 from .losses import (KurtosisWeight, DistributionLoss, DistributionLoss_layer,

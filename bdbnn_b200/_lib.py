@@ -89,7 +89,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 f"bdbnn_b200: {LIB_PATH} not found. Build it with `python -m bdbnn_b200.build` "
-                "(nvcc, sm_100a). There is no CPU / eager fallback.")
+                "(nvcc, sm_90a). There is no CPU / eager fallback.")
         h = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in SIGNATURES.items():
             fn = getattr(h, name)

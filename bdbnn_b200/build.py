@@ -1,4 +1,4 @@
-"""Build libbdbnn_b200.so in-tree with nvcc for sm_100a (no torch involved: the library is a plain
+"""Build libbdbnn_b200.so in-tree with nvcc for sm_90a (no torch involved: the library is a plain
 C-ABI shared object, see include/bdbnn.h).  `python -m bdbnn_b200.build [--force]`."""
 import hashlib
 import os
@@ -10,9 +10,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libbdbnn_b200.so")
 STAMP = os.path.join(HERE, ".libbdbnn_b200.stamp")
-SOURCES = ["api.cu", "pack.cu", "binconv.cu", "losses.cu", "tc_conv.cu", "tc_conv2.cu", "tc_conv64.cu", "tc_wgrad.cu", "pool.cu", "bn.cu", "stem.cu", "step_ops.cu", "real_conv.cu"]
+SOURCES = ["api.cu", "pack.cu", "binconv.cu", "losses.cu", "tc_conv.cu", "tc_wgrad.cu", "pool.cu", "bn.cu", "stem.cu", "step_ops.cu", "real_conv.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--use_fast_math=false", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
     "--cudart", "static", "-Xptxas", "-v",
 ]
@@ -37,7 +37,7 @@ def _digest():
 
 
 def build(force=False, verbose=False):
-    """Compile every .cu for sm_100a and link the shared library. Returns the library path."""
+    """Compile every .cu for sm_90a and link the shared library. Returns the library path."""
     dig = _digest()
     if not force and os.path.exists(LIB) and os.path.exists(STAMP):
         with open(STAMP) as fh:
@@ -66,7 +66,7 @@ def build(force=False, verbose=False):
         raise RuntimeError("nvcc failed:\n" + "\n".join(log))
     if verbose:
         print("\n".join(log))
-    cmd = [nvcc, "-shared", "--cudart", "static", "-gencode", "arch=compute_100a,code=sm_100a",
+    cmd = [nvcc, "-shared", "--cudart", "static", "-gencode", "arch=compute_90a,code=sm_90a",
            *objs, "-o", LIB, "-ldl", "-lpthread", "-lrt"]
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:

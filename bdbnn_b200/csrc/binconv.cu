@@ -1,5 +1,5 @@
 // Binary convolution on CUDA cores: XNOR-popcount forward + generic (any-shape) backward kernels.
-// The tensor-core (tcgen05) implicit-GEMM versions live in tc_conv.cu; the kernels here are the
+// The tensor-core (wgmma) implicit-GEMM versions live in tc_conv.cu; the kernels here are the
 // bit-serial path BASELINE.json:north_star prescribes and the shape-generic fallback.
 #include "common.cuh"
 
@@ -129,7 +129,7 @@ static int launch_fwd_xnor(const uint32_t* xs, const uint32_t* ws, const float* 
 // -------------------------------------------------------------------------------------------------
 // Generic data gradient (any kernel size / stride / channel count).  One thread per (input pixel,
 // channel); lanes of a warp share the pixel (when Cin >= 32) so gy / alpha / weight-word reads are
-// warp-broadcast.  Correctness baseline and fallback for shapes the tcgen05 path does not take.
+// warp-broadcast.  Correctness baseline and fallback for shapes the tensor-core path does not take.
 // -------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 binconv_dgrad_generic_kernel(const float* __restrict__ gy, const uint32_t* __restrict__ ws,

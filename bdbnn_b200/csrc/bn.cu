@@ -48,15 +48,17 @@ __device__ __forceinline__ float4 load_y4(const void* __restrict__ y, int64_t i)
 }
 
 // Per-channel (sum a, sum b, max c) over pixels; thread = one float4 channel group, strided over pixels.
-// Block partials go through shared-memory atomics, then one double atomicAdd per channel per block.
+// Each block adds its threads' partials of a channel in thread order and writes them to its row of `part`
+// ([gridDim.x][2C], summed in block order by det_sums_finish): the sums are the same in every run.
 template <bool BWD, bool I16 = false>
 __global__ void __launch_bounds__(kBnThreads)
 bn_reduce_kernel(const float4* __restrict__ p0, const void* __restrict__ p1, const float* __restrict__ mean,
-                 const float* __restrict__ invstd, int64_t n_pix, int C4, double* __restrict__ sums,
+                 const float* __restrict__ invstd, int64_t n_pix, int C4, double* __restrict__ part,
                  uint32_t* __restrict__ maxbits, const float* __restrict__ alpha = nullptr) {
-  extern __shared__ float sh[];               // [3][C]
+  extern __shared__ float4 shs[];             // [2][blockDim] per-thread partials, then [C] max bits
   const int C = C4 * 4;
-  for (int i = threadIdx.x; i < 3 * C; i += blockDim.x) sh[i] = 0.f;
+  uint32_t* shm = reinterpret_cast<uint32_t*>(shs + 2 * blockDim.x);   // non-negative floats order like uints
+  for (int i = threadIdx.x; i < C; i += blockDim.x) shm[i] = 0u;
   __syncthreads();
   const int64_t gtid = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
   const int64_t nthreads = int64_t(gridDim.x) * blockDim.x;   // multiple of C4 (host guarantees)
@@ -95,18 +97,101 @@ bn_reduce_kernel(const float4* __restrict__ p0, const void* __restrict__ p1, con
     mx.z = fmaxf(mx.z, fabsf(u.z)); mx.w = fmaxf(mx.w, fabsf(u.w));
   }
   const int c = c4 * 4;
-  atomicAdd(&sh[c + 0], sa.x); atomicAdd(&sh[c + 1], sa.y); atomicAdd(&sh[c + 2], sa.z); atomicAdd(&sh[c + 3], sa.w);
-  atomicAdd(&sh[C + c + 0], sb.x); atomicAdd(&sh[C + c + 1], sb.y);
-  atomicAdd(&sh[C + c + 2], sb.z); atomicAdd(&sh[C + c + 3], sb.w);
-  uint32_t* shm = reinterpret_cast<uint32_t*>(sh + 2 * C);   // non-negative floats order like uints
+  shs[threadIdx.x] = sa;
+  shs[blockDim.x + threadIdx.x] = sb;
   atomicMax(&shm[c + 0], __float_as_uint(mx.x)); atomicMax(&shm[c + 1], __float_as_uint(mx.y));
   atomicMax(&shm[c + 2], __float_as_uint(mx.z)); atomicMax(&shm[c + 3], __float_as_uint(mx.w));
   __syncthreads();
-  for (int i = threadIdx.x; i < C; i += blockDim.x) {
-    atomicAdd(sums + i, double(sh[i]));
-    atomicAdd(sums + C + i, double(sh[C + i]));
-    atomicMax(maxbits + i, shm[i]);
+  const int first = int((int64_t(blockIdx.x) * blockDim.x) % C4);     // channel group of thread 0
+  double* row = part + int64_t(blockIdx.x) * 2 * C;
+  for (int g = threadIdx.x; g < C4; g += blockDim.x) {
+    float4 a = make_float4(0, 0, 0, 0), b = a;
+    for (int t = (g - first + C4) % C4; t < int(blockDim.x); t += C4) {
+      const float4 u = shs[t], v = shs[blockDim.x + t];
+      a.x += u.x; a.y += u.y; a.z += u.z; a.w += u.w;
+      b.x += v.x; b.y += v.y; b.z += v.z; b.w += v.w;
+    }
+    row[4 * g + 0] = a.x; row[4 * g + 1] = a.y; row[4 * g + 2] = a.z; row[4 * g + 3] = a.w;
+    row[C + 4 * g + 0] = b.x; row[C + 4 * g + 1] = b.y; row[C + 4 * g + 2] = b.z; row[C + 4 * g + 3] = b.w;
   }
+  for (int i = threadIdx.x; i < C; i += blockDim.x) atomicMax(maxbits + i, shm[i]);
+}
+
+// ---- run-to-run deterministic sums across blocks ----------------------------------------------------
+// out[col] (+)= sum over parts p in [p0, p1) of in[p][col]: 32 columns x 32 part lanes per block; each lane adds its
+// parts in order, the lanes are then added in lane order.  gridDim.y > 1: one output row per part chunk.
+constexpr int kDetChunk = 1024;
+__global__ void __launch_bounds__(1024)
+det_reduce_kernel(const double* __restrict__ in, int64_t nparts, int width, double* __restrict__ out, int add) {
+  __shared__ double red[32][33];
+  const int col = blockIdx.x * 32 + threadIdx.x, lane = threadIdx.y;
+  const int64_t p0 = int64_t(blockIdx.y) * kDetChunk;
+  const int64_t p1 = p0 + kDetChunk < nparts ? p0 + kDetChunk : nparts;
+  double acc = 0.0;
+  if (col < width)
+    for (int64_t p = p0 + lane; p < p1; p += 32) acc += in[p * width + col];
+  red[lane][threadIdx.x] = acc;
+  __syncthreads();
+  if (lane == 0 && col < width) {
+    double t = 0.0;
+    for (int l = 0; l < 32; ++l) t += red[l][threadIdx.x];
+    if (add) out[col] += t;
+    else out[int64_t(blockIdx.y) * width + col] = t;
+  }
+}
+
+int det_sums_alloc(double** part, int64_t nparts, int width, cudaStream_t st) {
+  // keep freed scratch in the device's default pool instead of returning it at every synchronisation (release
+  // threshold 0 would make each eager call map fresh memory)
+  static const bool pool_ready = [] {
+    int dev = 0;
+    cudaMemPool_t pool;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetDefaultMemPool(&pool, dev) != cudaSuccess) return false;
+    uint64_t keep = UINT64_MAX;
+    return cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep) == cudaSuccess;
+  }();
+  (void)pool_ready;
+  BDBNN_CUDA(cudaMallocAsync(reinterpret_cast<void**>(part), size_t(nparts) * width * sizeof(double), st));
+  return BDBNN_OK;
+}
+
+int det_sums_finish(double* part, int64_t nparts, int width, double* sums, cudaStream_t st) {
+  double* cur = part;
+  while (nparts > kDetChunk) {
+    const int64_t m = (nparts + kDetChunk - 1) / kDetChunk;
+    double* next = nullptr;
+    const cudaError_t ea = cudaMallocAsync(reinterpret_cast<void**>(&next), size_t(m) * width * sizeof(double), st);
+    if (ea != cudaSuccess) {
+      cudaFreeAsync(cur, st);
+      set_error("det_sums_finish: cudaMallocAsync failed: %s", cudaGetErrorString(ea));
+      return BDBNN_ERR_CUDA;
+    }
+    det_reduce_kernel<<<dim3(unsigned((width + 31) / 32), unsigned(m)), dim3(32, 32), 0, st>>>(cur, nparts, width, next, 0);
+    const int rc = check_launch("det_reduce_kernel");
+    cudaFreeAsync(cur, st);
+    if (rc) { cudaFreeAsync(next, st); return rc; }
+    cur = next;
+    nparts = m;
+  }
+  det_reduce_kernel<<<dim3(unsigned((width + 31) / 32), 1), dim3(32, 32), 0, st>>>(cur, nparts, width, sums, 1);
+  const int rc = check_launch("det_reduce_kernel");
+  BDBNN_CUDA(cudaFreeAsync(cur, st));
+  return rc;
+}
+
+// bn_reduce_kernel over `grid` blocks with its partials summed into sums[2C] (pre-zeroed or accumulated)
+template <bool BWD, bool I16 = false>
+static int bn_reduce_launch(int grid, const float4* p0, const void* p1, const float* mean, const float* invstd,
+                            int64_t n_pix, int C4, double* sums, uint32_t* maxbits, const float* alpha,
+                            cudaStream_t st) {
+  double* part = nullptr;
+  int rc = det_sums_alloc(&part, grid, 8 * C4, st);
+  if (rc) return rc;
+  bn_reduce_kernel<BWD, I16><<<grid, kBnThreads, 2 * kBnThreads * sizeof(float4) + size_t(4 * C4) * sizeof(uint32_t),
+                               st>>>(p0, p1, mean, invstd, n_pix, C4, part, maxbits, alpha);
+  rc = check_launch(BWD ? "bn_reduce_kernel<bwd>" : "bn_reduce_kernel<fwd>");
+  if (rc) { cudaFreeAsync(part, st); return rc; }
+  return det_sums_finish(part, grid, 8 * C4, sums, st);
 }
 
 // [C] math of the forward: mean, invstd, a = gamma*invstd, b = beta - mean*a, running statistics
@@ -300,10 +385,9 @@ static int bn_grid(int64_t work, int C4, int per_sm = 8) {
 int bn_stats_launch(const float* y, int64_t n_pix, int C, double* sums, uint32_t* ymax, cudaStream_t st) {
   BDBNN_REQUIRE(C > 0 && (C & 3) == 0 && C <= 4096, "bn_stats: C must be a multiple of 4, <= 4096");
   const int C4 = C / 4;
-  bn_reduce_kernel<false><<<bn_grid(n_pix * C4 / 8, C4, n_pix * C4 > (int64_t(16) << 20) ? 8 : 3), kBnThreads,
-                            size_t(3 * C) * sizeof(float), st>>>(reinterpret_cast<const float4*>(y), nullptr, nullptr,
-                                                                 nullptr, n_pix, C4, sums, ymax);
-  return check_launch("bn_reduce_kernel<fwd>");
+  return bn_reduce_launch<false>(bn_grid(n_pix * C4 / 8, C4, n_pix * C4 > (int64_t(16) << 20) ? 8 : 3),
+                                 reinterpret_cast<const float4*>(y), nullptr, nullptr, nullptr, n_pix, C4, sums, ymax,
+                                 nullptr, st);
 }
 
 }  // namespace bdbnn
@@ -352,7 +436,7 @@ static int bn_fwd_impl(const void* y, const float* alpha_i16, const float* resid
     const uint32_t one16 = fmt == BDBNN_FMT_FP16 ? 0x3C00u : 0x3F80u;
     uint2* xb2 = reinterpret_cast<uint2*>(xb);
     uint32_t* xb8 = reinterpret_cast<uint32_t*>(xb_fp8);
-    // four float4 per thread and iteration (measured: bn_fwd 1.13 -> 1.04 ms per ResNet-18 step vs two); BDBNN_BN_UNROLL=2
+    // four float4 per thread and iteration (more loads in flight than two); BDBNN_BN_UNROLL=2
     static const int unroll2 = [] { const char* e = getenv("BDBNN_BN_UNROLL"); return e ? atoi(e) == 2 : 0; }();
     if (i16 && unroll2)
       bn_apply_add_pack_kernel<true, true, 2><<<grid, kBnThreads, 0, st>>>(y, r4, a, b, n4, C4, z4, sign_bits, mask_bits,
@@ -412,12 +496,11 @@ static int bn_bwd_pack_impl(const float* gz, const void* y, const float* alpha_i
     BDBNN_CUDA(cudaMemsetAsync(gmax_bits, 0, size_t(C) * sizeof(uint32_t), st));
     const int rgrid = bn_grid(n_pix * C4 / 8, C4, n_pix * C4 > (int64_t(16) << 20) ? 8 : 3);
     if (i16)
-      bn_reduce_kernel<true, true><<<rgrid, kBnThreads, size_t(3 * C) * sizeof(float), st>>>(
-          reinterpret_cast<const float4*>(gz), y, mean, invstd, n_pix, C4, sums_ws, gmax_bits, alpha_i16);
+      rc = bn_reduce_launch<true, true>(rgrid, reinterpret_cast<const float4*>(gz), y, mean, invstd, n_pix, C4, sums_ws,
+                                        gmax_bits, alpha_i16, st);
     else
-      bn_reduce_kernel<true, false><<<rgrid, kBnThreads, size_t(3 * C) * sizeof(float), st>>>(
-          reinterpret_cast<const float4*>(gz), y, mean, invstd, n_pix, C4, sums_ws, gmax_bits, nullptr);
-    rc = check_launch("bn_reduce_kernel<bwd>");
+      rc = bn_reduce_launch<true, false>(rgrid, reinterpret_cast<const float4*>(gz), y, mean, invstd, n_pix, C4,
+                                         sums_ws, gmax_bits, nullptr, st);
     if (rc) return rc;
   }
   bn_bwd_bound_kernel<<<1, 256, 0, st>>>(sums_ws, gmax_bits, ymax_bits, n_pix, C, mean, invstd, gamma, gscale,
@@ -550,7 +633,7 @@ bn_pool_fwd_kernel(const float4* __restrict__ y, const float* __restrict__ a, co
 // 3x3 / stride-2 / pad-1 forward (the stem's pool) with one block per output row (n, ho): the three input
 // row pointers and the row validity are per block, the tap loop is unrolled, and the winner index is kept
 // as four small integers instead of read-modify-write byte lanes — about half the instructions of the
-// generic kernel, which ncu showed issue-bound (55-60 % issue-slot utilisation at 2.4 TB/s).
+// generic kernel, which is bound by instruction issue rather than by memory.
 // Same scan order and NaN rule, so outputs are bit-identical.  blockDim.x is a multiple of C4.
 template <bool PACK>
 __global__ void __launch_bounds__(kBnThreads)
@@ -838,10 +921,9 @@ extern "C" int bdbnn_bn_pool_bwd(const float* g_pool, const uint8_t* idx, const 
   const int64_t n_pool = int64_t(N) * Ho * Wo, n_full = int64_t(N) * H * W;
   BDBNN_CUDA(cudaMemsetAsync(sums_ws, 0, size_t(2 * C) * sizeof(double), st));
   BDBNN_CUDA(cudaMemsetAsync(gmax_bits, 0, size_t(C) * sizeof(uint32_t), st));
-  bn_reduce_kernel<true><<<bn_grid(n_pool * C4 / 8, C4, 3), kBnThreads, size_t(3 * C) * sizeof(float), st>>>(
-      reinterpret_cast<const float4*>(g_pool), reinterpret_cast<const float4*>(y_sel), mean, invstd, n_pool, C4,
-      sums_ws, gmax_bits);
-  rc = check_launch("bn_reduce_kernel<bwd,pool>");
+  rc = bn_reduce_launch<true>(bn_grid(n_pool * C4 / 8, C4, 3), reinterpret_cast<const float4*>(g_pool),
+                              reinterpret_cast<const float4*>(y_sel), mean, invstd, n_pool, C4, sums_ws, gmax_bits,
+                              nullptr, st);
   if (rc) return rc;
   // means are over the FULL-resolution element count; gscale = 1 (`ones`)
   const int per_dim = (k + stride - 1) / stride;          // pooling windows covering one position, per axis

@@ -1,4 +1,4 @@
-// Shared helpers for libbdbnn_b200 (sm_100a only).
+// Shared helpers for libbdbnn_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -56,7 +56,7 @@ inline int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
@@ -80,6 +80,12 @@ __host__ __device__ inline float amax_pow2_scale(uint32_t amax_bits, bool invers
 
 // bn.cu: sum y, sum y^2, max|y| per channel of an NHWC fp32 tensor into (pre-zeroed) sums / ymax.
 int bn_stats_launch(const float* y, int64_t n_pix, int C, double* sums, uint32_t* ymax, cudaStream_t st);
+// bn.cu: run-to-run deterministic sums across blocks.  Block b writes its partial row part[b][0, width) (no
+// atomics); det_sums_finish adds the column sums, taken in a fixed order, to sums[0, width) and frees `part`
+// (also when it fails).
+// Stream-ordered allocation, so both may be captured into a CUDA graph.
+int det_sums_alloc(double** part, int64_t nparts, int width, cudaStream_t st);
+int det_sums_finish(double* part, int64_t nparts, int width, double* sums, cudaStream_t st);
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

@@ -17,8 +17,10 @@ struct TensorTable {
 constexpr int kLossThreads = 256;
 constexpr int kMomentStride = 8;  // doubles per tensor in the `moments` scratch
 
-__device__ __forceinline__ void block_atomic_add4(double v0, double v1, double v2, double v3,
-                                                  double* dst) {
+// Block sums of four values, stored to dst[0..3] (each block owns its dst: the cross-block sum is taken in a
+// fixed order by det_sums_finish, so results are the same in every run).
+__device__ __forceinline__ void block_store_sum4(double v0, double v1, double v2, double v3,
+                                                 double* dst) {
   __shared__ double red[4][kLossThreads / 32];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   v0 = warp_sum(v0); v1 = warp_sum(v1); v2 = warp_sum(v2); v3 = warp_sum(v3);
@@ -30,14 +32,14 @@ __device__ __forceinline__ void block_atomic_add4(double v0, double v1, double v
     double t2 = lane < nw ? red[2][lane] : 0.0, t3 = lane < nw ? red[3][lane] : 0.0;
     t0 = warp_sum(t0); t1 = warp_sum(t1); t2 = warp_sum(t2); t3 = warp_sum(t3);
     if (lane == 0) {
-      atomicAdd(dst + 0, t0); atomicAdd(dst + 1, t1); atomicAdd(dst + 2, t2); atomicAdd(dst + 3, t3);
+      dst[0] = t0; dst[1] = t1; dst[2] = t2; dst[3] = t3;
     }
   }
 }
 
 // Pass 1: shifted raw power sums S_k = sum (w - w[0])^k, k=1..4, fp64 accumulation.
 __global__ void __launch_bounds__(kLossThreads)
-kurt_moments_kernel(TensorTable tab, double* __restrict__ moments) {
+kurt_moments_kernel(TensorTable tab, double* __restrict__ part) {   // part: [gridDim.x][L][kMomentStride]
   const int l = blockIdx.y;
   const float* __restrict__ w = tab.a[l];
   const int64_t n = tab.n[l];
@@ -49,7 +51,7 @@ kurt_moments_kernel(TensorTable tab, double* __restrict__ moments) {
     const double d2 = d * d;
     s1 += d; s2 += d2; s3 += d2 * d; s4 += d2 * d2;
   }
-  block_atomic_add4(s1, s2, s3, s4, moments + l * kMomentStride);
+  block_store_sum4(s1, s2, s3, s4, part + (int64_t(blockIdx.x) * gridDim.y + l) * kMomentStride);
 }
 
 // Pass 2 (one thread per tensor): central moments -> mu, s (unbiased), K, mean z^3, loss.
@@ -174,7 +176,7 @@ mean_rows_kernel(const float* __restrict__ row_loss, int32_t N, float* __restric
 
 // ---- KD per-layer ------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kLossThreads)
-kd_layer_fwd_kernel(TensorTable tab, double* __restrict__ partial) {
+kd_layer_fwd_kernel(TensorTable tab, double* __restrict__ part) {   // part: [gridDim.x][L]
   __shared__ double red[kLossThreads / 32];
   const int l = blockIdx.y;
   const float* __restrict__ wt = tab.a[l];
@@ -192,7 +194,7 @@ kd_layer_fwd_kernel(TensorTable tab, double* __restrict__ partial) {
   if (threadIdx.x == 0) {
     double t = 0.0;
     for (int i = 0; i < int(blockDim.x >> 5); ++i) t += red[i];
-    atomicAdd(partial + l, t);
+    part[int64_t(blockIdx.x) * gridDim.y + l] = t;
   }
 }
 
@@ -265,8 +267,16 @@ extern "C" int bdbnn_kurtosis_multi_fwd(const float* const* w_ptrs_host, const i
   cudaStream_t st = cudaStream_t(stream);
   BDBNN_CUDA(cudaMemsetAsync(moments, 0, size_t(L) * kMomentStride * sizeof(double), st));
   dim3 grid(blocks_for(max_n, L), unsigned(L));
-  kurt_moments_kernel<<<grid, kLossThreads, 0, st>>>(tab, moments);
-  rc = check_launch("kurt_moments_kernel");
+  const int width = L * kMomentStride;
+  double* part = nullptr;
+  rc = det_sums_alloc(&part, grid.x, width, st);
+  if (rc) return rc;
+  const cudaError_t em = cudaMemsetAsync(part, 0, size_t(grid.x) * width * sizeof(double), st);
+  kurt_moments_kernel<<<grid, kLossThreads, 0, st>>>(tab, part);
+  rc = em != cudaSuccess ? (set_error("kurtosis: cudaMemsetAsync failed: %s", cudaGetErrorString(em)), BDBNN_ERR_CUDA)
+                         : check_launch("kurt_moments_kernel");
+  if (rc) { cudaFreeAsync(part, st); return rc; }
+  rc = det_sums_finish(part, grid.x, width, moments, st);
   if (rc) return rc;
   kurt_finalize_kernel<<<1, BDBNN_MAX_TENSORS, 0, st>>>(tab, moments, kurt_out, loss_out);
   return check_launch("kurt_finalize_kernel");
@@ -319,8 +329,13 @@ extern "C" int bdbnn_kd_layer_multi_fwd(const float* const* ws_ptrs_host,
   for (int l = 0; l < L; ++l) BDBNN_REQUIRE(tab.b[l] != nullptr, "student pointer %d is NULL", l);
   BDBNN_CUDA(cudaMemsetAsync(partial, 0, size_t(L) * sizeof(double), st));
   dim3 grid(blocks_for(max_n, L), unsigned(L));
-  kd_layer_fwd_kernel<<<grid, kLossThreads, 0, st>>>(tab, partial);
+  double* part = nullptr;
+  rc = det_sums_alloc(&part, grid.x, L, st);
+  if (rc) return rc;
+  kd_layer_fwd_kernel<<<grid, kLossThreads, 0, st>>>(tab, part);
   rc = check_launch("kd_layer_fwd_kernel");
+  if (rc) { cudaFreeAsync(part, st); return rc; }
+  rc = det_sums_finish(part, grid.x, L, partial, st);
   if (rc) return rc;
   kd_layer_finalize_kernel<<<1, 32, 0, st>>>(tab, partial, loss_out);
   return check_launch("kd_layer_finalize_kernel");

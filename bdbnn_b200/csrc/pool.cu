@@ -1,6 +1,6 @@
 // NHWC max-pool forward / backward (fp32).  Not part of the binary-conv maths, but it sits on the
 // timed train step right after the stem (822 MB activation at ResNet-18 N=256), where ATen's
-// max_pool_backward_nhwc is 10x off the HBM roofline (1.75 ms measured, profiles/r1_step3_*).
+// max_pool_backward_nhwc scatters with atomics instead of reading each input position once.
 //   forward : y = max over the k x k window (first maximum in scan order wins, NaN propagates — the
 //             torch.nn.MaxPool2d rule), idx = winning tap (r*k+s) as one byte per element
 //   backward: gather form, no atomics: gx[h,w] = sum of gy[ho,wo] over the (<= ceil(k/s)^2) windows

@@ -1,4 +1,4 @@
-// fp32 1x1 shortcut convolutions (ResNet `downsample`: 1x1, stride 2, no bias) on the tcgen05 kernels.
+// fp32 1x1 shortcut convolutions (ResNet `downsample`: 1x1, stride 2, no bias) on the tensor-core kernels.
 //
 // The reference keeps these convs real-valued (fp32 nn.Conv2d; cuDNN runs them on TF32 tensor cores).
 // Like the stem (stem.cu) both operands are rounded to fp16 after per-call power-of-two scales (11-bit

@@ -1,4 +1,4 @@
-// Stem convolution (7x7, stride 2, pad 3, 3 -> 64 channels, fp32 in / fp32 out) on tcgen05.
+// Stem convolution (7x7, stride 2, pad 3, 3 -> 64 channels, fp32 in / fp32 out) on wgmma.
 //
 // The reference runs this layer as an fp32 nn.Conv2d, which cuDNN executes on TF32 tensor cores by
 // default (11-bit significands, fp32 accumulate).  Here both operands are rounded to fp16 after a

@@ -1,4 +1,4 @@
-// Shared tcgen05 / TMA / mbarrier PTX wrappers and tensor-map helpers (sm_100a).
+// Shared wgmma / TMA / mbarrier PTX wrappers and tensor-map helpers (sm_90a).
 #pragma once
 #include <cuda.h>
 #include <stdlib.h>
@@ -59,260 +59,142 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_alloc(uint32_t slot_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(slot_smem),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16 inputs, fp32 accumulate.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrives when every previously issued tcgen05.mma of this thread has completed.
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, "
-      "%13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]),
-        "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// K-major shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout): start address >>4
-// in [0,14), LBO>>4 in [16,30), SBO>>4 in [32,46), version=1 in [46,48), layout type in [61,64).
-// For swizzled K-major tiles LBO is unused; SBO = bytes between 8-row groups = 8 * row_bytes.
-// NOTE (measured on B200): a start address that is a whole number of 128-byte rows into a
-// 1024B-aligned SWIZZLE_128B tile needs base_offset = 0 — the hardware applies the swizzle XOR to the
-// absolute shared-memory address bits, so row-shifted views of one TMA-written tile are valid operands.
-__device__ __forceinline__ uint64_t make_kmajor_desc(uint32_t saddr, uint32_t row_bytes) {
-  const uint32_t layout = row_bytes == 128 ? 2u : (row_bytes == 64 ? 4u : 6u);  // SW128 / SW64 / SW32
-  uint64_t d = 0;
-  d |= uint64_t((saddr & 0x3FFFFu) >> 4);
-  d |= uint64_t(1) << 16;                          // LBO (ignored for swizzled K-major)
-  d |= uint64_t((8u * row_bytes) >> 4) << 32;      // SBO
-  d |= uint64_t(1) << 46;                          // descriptor version (Blackwell)
-  d |= uint64_t(layout) << 61;
-  return d;
-}
-// Instruction descriptor (cute::UMMA::InstrDescriptor): c_format F32 (1) @4, a/b format BF16 (1) @7/@10,
-// K-major A and B (0) @15/@16, N>>3 @17, M>>4 @24.
-// fmt: BDBNN_FMT_FP16 (0) or BDBNN_FMT_BF16 (1) for both A and B (kind::f16).
-__host__ __device__ inline uint32_t make_idesc_bf16(uint32_t M, uint32_t N, uint32_t fmt = 1u) {
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-
-constexpr int kTcThreads = 192;
-constexpr int kMaxStages = 8;
-constexpr int kTileM = 128;
-constexpr int kMaxTaps = 49;
-
-// Four K=16 steps of one 64-element (128-byte, SWIZZLE_128B K-major) K block in a single asm block:
-// the MMA-issuing thread is a lone scalar thread, so per-MMA instruction count is what bounds the
-// issue rate (a generic descriptor rebuild per MMA costs ~80 clk, more than a 128x64x16 MMA takes).
-// a_lo/b_lo are the low descriptor words (address>>4 | LBO), desc_hi the shared high word.
-__device__ __forceinline__ void umma_bf16_k4(uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo, uint32_t desc_hi,
-                                             uint32_t idesc, uint32_t accumulate_first) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p, q;\n\t"
-      ".reg .b64 da, db;\n\t"
-      ".reg .b32 al, bl;\n\t"
-      "setp.ne.b32 p, %5, 0;\n\t"
-      "setp.eq.b32 q, 0, 0;\n\t"
-      "mov.b64 da, {%1, %3};\n\t"
-      "mov.b64 db, {%2, %3};\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, p;\n\t"
-      "add.u32 al, %1, 2;\n\t"
-      "add.u32 bl, %2, 2;\n\t"
-      "mov.b64 da, {al, %3};\n\t"
-      "mov.b64 db, {bl, %3};\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, q;\n\t"
-      "add.u32 al, %1, 4;\n\t"
-      "add.u32 bl, %2, 4;\n\t"
-      "mov.b64 da, {al, %3};\n\t"
-      "mov.b64 db, {bl, %3};\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, q;\n\t"
-      "add.u32 al, %1, 6;\n\t"
-      "add.u32 bl, %2, 6;\n\t"
-      "mov.b64 da, {al, %3};\n\t"
-      "mov.b64 db, {bl, %3};\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, q;\n\t"
-      "}" ::"r"(tmem_d),
-      "r"(a_lo), "r"(b_lo), "r"(desc_hi), "r"(idesc), "r"(accumulate_first)
-      : "memory");
-}
-// One MMA from pre-split descriptor words (cheap to advance: only the low words change per K step).
-__device__ __forceinline__ void umma_bf16_split(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo,
-                                                uint32_t b_hi, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      ".reg .b64 da, db;\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "mov.b64 da, {%1, %2};\n\t"
-      "mov.b64 db, {%3, %4};\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// fp8 (e4m3 x e4m3 -> f32) MMA, K = 32 per instruction; +-1 is exact in e4m3.
-__device__ __forceinline__ void umma_f8_split(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo,
-                                              uint32_t b_hi, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      ".reg .b64 da, db;\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "mov.b64 da, {%1, %2};\n\t"
-      "mov.b64 db, {%3, %4};\n\t"
-      "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], da, db, %5, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// e4m3 A and B (format code 0), f32 accumulate, K-major
-__host__ __device__ inline uint32_t make_idesc_f8(uint32_t M, uint32_t N) {
-  return (1u << 4) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-// Low / high descriptor words of a swizzled K-major tile with rows of `row_bytes` (64 or 128)
-__device__ __forceinline__ uint32_t kmajor_lo(uint32_t saddr) { return ((saddr & 0x3FFFFu) >> 4) | (1u << 16); }
-__device__ __forceinline__ uint32_t kmajor_hi(uint32_t row_bytes) {
-  return ((8u * row_bytes) >> 4) | (1u << 14) | ((row_bytes == 128 ? 2u : 4u) << 29);
-}
-// Low / high words of a SWIZZLE_128B K-major descriptor (see make_kmajor_desc).
-__device__ __forceinline__ uint32_t kmajor128_lo(uint32_t saddr) { return ((saddr & 0x3FFFFu) >> 4) | (1u << 16); }
-__device__ __forceinline__ uint32_t kmajor128_hi() { return (1024u >> 4) | (1u << 14) | (2u << 29); }
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, "
-      "%14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]),
-        "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]),
-        "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]),
-        "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 
-// ---------------------------------------------------------------------------------------------------
-// CTA-pair (cta_group::2) helpers: two CTAs of a 2-CTA cluster (same TPC) execute ONE tcgen05.mma of M = 256 —
-// each SM multiplies its own 128 A rows (its own shared memory, same descriptor offsets in both CTAs) with the
-// full B tile, of which each CTA holds half the rows (N/2) — so every SM fetches half as many B bytes from its
-// shared memory per unit of work.  Only the leader CTA (cluster rank 0) issues MMAs and commits; barriers that the
-// MMA thread waits on live in the leader, and the peer signals them through shared::cluster addresses.
-// ---------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
+
+// Warpgroup MMA (wgmma, sm_90a).  A warpgroup is four consecutive warps whose first warp index is a multiple of 4;
+// all 128 threads issue each wgmma together and the accumulator lives in their registers.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+// Keeps the compiler from moving accumulator reads/writes across an in-flight wgmma.
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// shared::cluster address of the same shared-memory offset in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t saddr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(rank));
-  return r;
+
+// Shared-memory matrix descriptor (sm_90 GMMA layout): start address >> 4 in [0,14), LBO >> 4 in [16,30),
+// SBO >> 4 in [32,46), layout type in [62,64) (1 = SWIZZLE_128B, 2 = SWIZZLE_64B, 3 = SWIZZLE_32B).
+// K-major swizzled tiles: LBO unused, SBO = bytes between 8-row groups = 8 * row_bytes; a K step inside a
+// swizzled row advances the start address by its byte width (the swizzle XOR is applied to address bits).
+// MN-major swizzled tiles: LBO = bytes between swizzle-row-wide MN chunks, SBO = bytes between 8-row K groups.
+__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t row_bytes) {
+  const uint32_t layout = row_bytes == 128 ? 1u : (row_bytes == 64 ? 2u : 3u);
+  uint64_t d = 0;
+  d |= uint64_t((saddr & 0x3FFFFu) >> 4);
+  d |= uint64_t((lbo_bytes >> 4) & 0x3FFFu) << 16;
+  d |= uint64_t(((8u * row_bytes) >> 4) & 0x3FFFu) << 32;
+  d |= uint64_t(layout) << 62;
+  return d;
 }
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_bar) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar) : "memory");
+__device__ __forceinline__ uint64_t make_kmajor_desc(uint32_t saddr, uint32_t row_bytes) {
+  return make_smem_desc(saddr, 16u, row_bytes);
 }
-// TMA loads whose completion is signalled on a barrier that may live in the PEER CTA (the leader's full barrier)
-__device__ __forceinline__ void tma_load_4d_cg2(uint32_t dst, const CUtensorMap* map, uint32_t cluster_bar, int c0,
-                                                int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, "
-      "%4, %5, %6}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(cluster_bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_cg2(uint32_t dst, const CUtensorMap* map, uint32_t cluster_bar, int c0,
-                                                int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, "
-      "%4}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(cluster_bar), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_cg2(uint32_t slot_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(slot_smem), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_cg2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// arrives on the barrier at this shared-memory offset in BOTH CTAs of the pair once all prior MMAs completed
-__device__ __forceinline__ void umma_commit_cg2(uint32_t bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-      "h"(uint16_t(3))
-      : "memory");
-}
-// One M=256 MMA of the pair from pre-split descriptor words; KIND 0 = f16/bf16 (K = 16), 1 = f8f6f4 (K = 32)
-template <int KIND>
-__device__ __forceinline__ void umma_split_cg2(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo,
-                                               uint32_t b_hi, uint32_t idesc, uint32_t accumulate) {
-  if (KIND == 0) {
+
+// D[64 x N] (+)= A[64 x K] * B[N x K]^T, fp32 accumulate in the warpgroup's registers (d: N/2 per thread).
+// KIND 0: fp16, 1: bf16 (K = 16; TA/TB = 1 for MN-major operands), 2: fp8 e4m3 (K = 32, K-major only).
+// Accumulator layout: thread t (warp w = t/32, lane l) holds rows 16w + l/4 (+8) and columns
+// 8j + 2(l%4) (+1): d[4j + 0/1] = row 16w + l/4, d[4j + 2/3] = row 16w + l/4 + 8.
+template <int N, int KIND, int TA = 0, int TB = 0>
+__device__ __forceinline__ void wgmma_ss(float (&d)[N / 2], uint64_t da, uint64_t db) {
+  static_assert(N == 16 || N == 32 || N == 64, "wgmma_ss: N in {16, 32, 64}");
+  static_assert(KIND >= 0 && KIND <= 2, "wgmma_ss: KIND in {0, 1, 2}");
+  if constexpr (N == 16 && KIND == 0) {
     asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        ".reg .b64 da, db;\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "mov.b64 da, {%1, %2};\n\t"
-        "mov.b64 db, {%3, %4};\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %5, p;\n\t"
-        "}" ::"r"(tmem_d),
-        "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %10, %11;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(da), "l"(db), "n"(TA), "n"(TB)
         : "memory");
-  } else {
+  }
+  if constexpr (N == 16 && KIND == 1) {
     asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        ".reg .b64 da, db;\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "mov.b64 da, {%1, %2};\n\t"
-        "mov.b64 db, {%3, %4};\n\t"
-        "tcgen05.mma.cta_group::2.kind::f8f6f4 [%0], da, db, %5, p;\n\t"
-        "}" ::"r"(tmem_d),
-        "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %10, %11;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(da), "l"(db), "n"(TA), "n"(TB)
+        : "memory");
+  }
+  if constexpr (N == 16 && KIND == 2) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k32.f32.e4m3.e4m3 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(da), "l"(db)
+        : "memory");
+  }
+  if constexpr (N == 32 && KIND == 0) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %18, %19;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "n"(TA), "n"(TB)
+        : "memory");
+  }
+  if constexpr (N == 32 && KIND == 1) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %18, %19;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "n"(TA), "n"(TB)
+        : "memory");
+  }
+  if constexpr (N == 32 && KIND == 2) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k32.f32.e4m3.e4m3 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db)
+        : "memory");
+  }
+  if constexpr (N == 64 && KIND == 0) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %34, %35;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "n"(TA), "n"(TB)
+        : "memory");
+  }
+  if constexpr (N == 64 && KIND == 1) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %34, %35;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "n"(TA), "n"(TB)
+        : "memory");
+  }
+  if constexpr (N == 64 && KIND == 2) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k32.f32.e4m3.e4m3 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db)
         : "memory");
   }
 }
+
+// Tensor-core kernels: warpgroups 0 and 1 issue the wgmmas for rows [0, 64) and [64, 128) of every 128-row
+// M tile and run the epilogue from their registers; warp 8 (lane 0) is the TMA producer.
+constexpr int kTcThreads = 288;
+constexpr int kProducerWarp = 8;
+constexpr int kMaxStages = 8;
+constexpr int kTileM = 128;
+constexpr int kMaxTaps = 49;
 
 // ---------------------------------------------------------------------------------------------------
 // Host side: tensor-map construction and launch
@@ -406,7 +288,7 @@ struct TcConvLaunch {
   int n_taps; int8_t dh[kMaxTaps], dw[kMaxTaps]; uint8_t tb[kMaxTaps];
   int out_step, off_h, off_w, OHf, OWf;
   const float* alpha; const uint32_t* mask; float* out;
-  int16_t* out_i16;              // forward (persistent kernel only): write the integer accumulator as int16 instead of out
+  int16_t* out_i16;              // forward, wide GEMMs only: write the integer accumulator as int16 instead of out
   int fmt;                       // operand format (BDBNN_FMT_*); -1 = fp8 e4m3 bytes (forward only)
   const uint32_t* amax_bits;     // FP16S gradient: device word with max|A|; epilogue multiplies by 2^-e
   const float* add;              // dgrad: optional tensor added to the result (shortcut gradient), or NULL
@@ -414,7 +296,7 @@ struct TcConvLaunch {
   // (sum y, sum y^2 as doubles [2*Nout]; max|y| bits [Nout]); NULL = off.  Zeroed by the caller.
   double* bn_sums;
   uint32_t* bn_ymax;
-  // dgrad only (persistent kernel, stride 1): bn_sums / bn_ymax receive the BACKWARD statistics of the BatchNorm
+  // dgrad only (wide GEMMs, stride 1): bn_sums / bn_ymax receive the BACKWARD statistics of the BatchNorm
   // unit that produced this conv's input — sum gz, sum gz*yhat, max|gz| with gz = this launch's result — using
   // that unit's int16 conv result st_y [pixels][Nout] and per-channel alpha / mean / invstd
   const int16_t* st_y; const float* st_alpha; const float* st_mean; const float* st_invstd;
@@ -456,16 +338,7 @@ size_t stem_wgrad_workspace_bytes(const StemGeom& g);
 int launch_stem_wgrad(const uint16_t* gys, const uint16_t* xw, float* ws, size_t ws_bytes, int* ksplit_out,
                       const StemGeom& g, cudaStream_t st);
 
-// Persistent multi-accumulator kernel (tc_conv2.cu). Returns BDBNN_ERR_UNSUPPORTED if the geometry
-// does not qualify (caller falls back to the one-tile-per-CTA kernel in tc_conv.cu).
-int launch_tc_conv2(const TcConvLaunch& L, int mode, cudaStream_t st);
-// Pixel-N kernel for the 64-channel layers (tc_conv64.cu): forward and stride-1 dgrad with Kc = Nout = 64 on images
-// of more than 256 pixels; BDBNN_ERR_UNSUPPORTED otherwise (callers then use launch_tc_conv2).
-int launch_tc_conv64(const TcConvLaunch& L, int mode, cudaStream_t st);
-bool tc_conv64_eligible(const TcConvLaunch& L);
-int launch_tc_conv64_stem(const TcConvLaunch& L, cudaStream_t st);
 void set_tc_trace(long long* buf);
-void set_conv_plan_sink(int32_t* sink);   // host-only planning probe, see tc_conv2.cu
 long long* get_tc_trace();
 bool wgrad_tc_ok(const bdbnn_conv_shape* s);
 

@@ -1,29 +1,31 @@
-// tcgen05 / TMA implicit-GEMM kernels for the binary convolution (sm_100a only).
+// wgmma / TMA implicit-GEMM kernel for the binary convolution (sm_90a).
 //
 //   tc_conv_kernel  : D[pix, n] = sum_{tap t} sum_{k} A[pix shifted by t, k] * B[n, t*Kc + k]
-//                     forward : A = sign(x)  (+-1 bf16, NHWC), B = sign(W)  [Cout][T][Cin]; epilogue * alpha[n]
-//                     dgrad   : A = gy*gscale (bf16,  NHWC), B = sign(W)^T [Cin][T'][Cout]; epilogue * STE mask bit
+//                     forward : A = sign(x)  (+-1 fp16/bf16/fp8, NHWC), B = sign(W) [Cout][T][Cin]; epilogue * alpha[n]
+//                     dgrad   : A = gy*gscale (bf16/fp16,  NHWC), B = sign(W)^T [Cin][T'][Cout]; epilogue * STE mask bit
 //
-// Dataflow per CTA (one 128-row output tile, one N tile):
-//   warp 4 lane 0 : TMA producer. For every (tap, K-block) loads the activation box
+// Dataflow per CTA (one 128-row output tile, one N tile of BN <= 128 columns):
+//   warp 8 lane 0 : TMA producer. For every (tap, K-block) loads the activation box
 //                   [BNI images][BH rows][BW=OW cols][KB channels] at coordinates shifted by the tap —
 //                   TMA zero-fills out-of-image coordinates, which IS the conv's zero padding — and the
-//                   matching [BN x KB] weight box, into a `stages`-deep ring of 128B-swizzled K-major tiles.
-//   warp 5 lane 0 : issues tcgen05.mma (kind::f16, bf16 x bf16 -> fp32 in TMEM), M=128, N=BN, K=16 per
-//                   instruction; tcgen05.commit releases ring slots / signals the epilogue.
-//   warps 0..3    : epilogue. tcgen05.ld the accumulator (warp w owns TMEM lanes 32w..32w+31 = tile rows),
-//                   apply alpha / STE mask, store fp32 NHWC rows (each thread writes whole 64-byte runs).
+//                   matching [BN x KB] weight box, into a `stages`-deep ring of swizzled K-major tiles.
+//   warpgroups 0/1: wgmma (fp32 accumulate in registers) for tile rows [0, 64) / [64, 128), one wgmma group in
+//                   flight: a ring slot is released once the group after it was issued and the one reading it retired.
+//                   Then the epilogue from the same registers: alpha or STE mask, optional int16 result, additive
+//                   tensor, and the per-channel BatchNorm statistics of the result (forward: sum y, sum y^2,
+//                   max|y|; dgrad: the backward sums of the BatchNorm unit that produced the conv input).
 // +-1 operands and fp32 accumulation make the forward integer-exact (|sum| <= 9*512 < 2^24).
 #include "tc_common.cuh"
 
 namespace bdbnn {
 
+constexpr int kMaxBN = 128;
 
 struct TcConvParams {
   int32_t OW, OH, NIMG;      // output pixel grid (one GEMM row per output pixel)
   int32_t BW, BH, BNI;       // tile = BNI images x BH rows x BW(=OW) cols  (<= 128 pixels)
   int32_t tiles_h;           // tiles per image group along h
-  int32_t Kc, KB, n_kb;      // contraction channels, K-block elements (16/32/64), Kc/KB
+  int32_t Kc, KB, n_kb;      // contraction channels, K-block elements, Kc/KB
   int32_t a_halves;          // 1: A has Kc channels; 2: A = [hi | lo] bf16 split, 2*Kc channels, B reused
   int32_t in_step;           // input coordinate = out coordinate * in_step + tap offset (2 for stride-2 fwd)
   int32_t n_taps;            // taps actually visited (subset for the stride-2 dgrad phases)
@@ -31,116 +33,61 @@ struct TcConvParams {
   uint8_t tap_b[kMaxTaps];   // K-block row of B for tap i (B column = tap_b * Kc + k)
   int32_t out_step, out_off_h, out_off_w, OHf, OWf;  // out pixel = (oh*out_step+off_h, ow*out_step+off_w) in OHf x OWf
   int32_t Nout, BN;          // GEMM N total / per CTA
-  // halo mode: ONE activation patch [PH][PW][64ch] per K block serves all taps; tap (dh,dw) is the same
-  // swizzled patch read from row offset (dh-dh_min)*PW + (dw-dw_min) (descriptor start + 128*shift)
-  int32_t halo, PW, PH, dh_min, dw_min, patch_bytes;
   int32_t stages;
-  int32_t row_bytes;         // KB * 2 = swizzle span (32/64/128)
-  int32_t fmt;               // operand format
+  int32_t row_bytes;         // KB * element size = swizzle span (32/64/128)
   const uint32_t* amax_bits; // FP16S: post-scale 2^-e (NULL otherwise)
   const float* add;          // dgrad: optional additive tensor
   const float* alpha;        // MODE 0: per-output-channel scale
   const uint32_t* mask;      // MODE 1: STE mask words [pix][Nout/32 (ceil)]
   float* out;                // [pix][Nout] fp32
+  int16_t* out_i16;          // MODE 0: the exact integer accumulator as int16 instead of out (y = alpha * int)
+  double* bn_sums;           // per-channel statistics [2*Nout] (NULL = off), see TcConvLaunch
+  double* stat_part;         // this launch's per-CTA statistics rows [gridDim.x][2*Nout] (det_sums_finish adds them)
+  uint32_t* bn_ymax;
+  const int16_t* st_y; const float* st_alpha; const float* st_mean; const float* st_invstd;   // MODE 1 statistics
 };
 
-template <int MODE>
+// KIND: 0 fp16, 1 bf16, 2 fp8 e4m3 operands; NW: wgmma N (16, 32, or 64 with BN/64 chunks)
+template <int MODE, int KIND, int NW>
 __global__ void __launch_bounds__(kTcThreads)
 tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const TcConvParams p) {
+  constexpr int NCH = NW == 64 ? kMaxBN / 64 : 1;
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[kMaxStages];
   __shared__ __align__(8) uint64_t empty_bar[kMaxStages];
-  __shared__ __align__(8) uint64_t accum_bar;
-  __shared__ __align__(8) uint64_t pfull_bar[2], pempty_bar[2];   // halo patch ring
-  __shared__ uint32_t tmem_slot;
+  // per-warp statistics partials, summed in a fixed order at the end (run-to-run deterministic)
+  __shared__ float stat_sum[kTcThreads / 32 - 1][kMaxBN], stat_sq[kTcThreads / 32 - 1][kMaxBN];
+  __shared__ float stat_max[kTcThreads / 32 - 1][kMaxBN];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t tiles_base = smem_base + (p.halo ? 2u * uint32_t(p.patch_bytes) : 0u);
-  const uint32_t a_bytes = p.halo ? 0u : kTileM * p.row_bytes;   // ring slot: [A tile] then B tile
-  const uint32_t b_bytes = p.BN * p.row_bytes;
-  const uint32_t stage_bytes = (a_bytes + b_bytes + 1023u) & ~1023u;
-  const uint32_t tmem_cols = p.BN < 32 ? 32u : uint32_t(p.BN);   // power of two >= 32
-
+  const uint32_t tiles_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t a_bytes = kTileM * p.row_bytes;   // ring slot: A tile, then B tile
+  const uint32_t stage_bytes = (a_bytes + uint32_t(p.BN) * p.row_bytes + 1023u) & ~1023u;
   const int tile_n = blockIdx.x / p.tiles_h, tile_h = blockIdx.x - tile_n * p.tiles_h;
   const int n0 = tile_n * p.BNI, h0 = tile_h * p.BH;
   const int nn0 = blockIdx.y * p.BN;
   const int kb_total = p.n_kb * p.a_halves;
   const int n_iters = p.n_taps * kb_total;
+  const bool do_stats = p.bn_sums != nullptr;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(smem_u32(&full_bar[s]), 1);
-      mbar_init(smem_u32(&empty_bar[s]), 1);
-    }
-    mbar_init(smem_u32(&accum_bar), 1);
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(smem_u32(&pfull_bar[s]), 1);
-      mbar_init(smem_u32(&pempty_bar[s]), 1);
+      mbar_init(smem_u32(&empty_bar[s]), 2);      // one arrival per consumer warpgroup
     }
     fence_barrier_init();
   }
-  if (warp == 4 && lane == 0) {
+  for (int i = threadIdx.x; i < (kTcThreads / 32 - 1) * kMaxBN; i += blockDim.x) {
+    (&stat_sum[0][0])[i] = 0.f; (&stat_sq[0][0])[i] = 0.f; (&stat_max[0][0])[i] = 0.f;
+  }
+  if (warp == kProducerWarp && lane == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
   }
-  if (warp == 5) tmem_alloc(smem_u32(&tmem_slot), tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_d = tmem_slot;
 
-  if (p.halo) {
-    if (warp == 4) {
-      if (lane == 0) {
-        int it = 0;
-        for (int kb = 0; kb < kb_total; ++kb) {
-          const int pa = kb & 1;
-          mbar_wait(smem_u32(&pempty_bar[pa]), (uint32_t(kb >> 1) & 1u) ^ 1u);
-          const uint32_t pb = smem_u32(&pfull_bar[pa]);
-          mbar_expect_tx(pb, uint32_t(p.PW * p.PH) * 128u);
-          tma_load_4d(smem_base + pa * p.patch_bytes, &tmA, pb, kb * p.KB, p.dw_min, h0 + p.dh_min, n0);
-          const int kbb = kb >= p.n_kb ? kb - p.n_kb : kb;
-          for (int ti = 0; ti < p.n_taps; ++ti, ++it) {
-            const int stage = it % p.stages;
-            const uint32_t phase = uint32_t(it / p.stages) & 1u;
-            mbar_wait(smem_u32(&empty_bar[stage]), phase ^ 1u);
-            const uint32_t fb = smem_u32(&full_bar[stage]);
-            mbar_expect_tx(fb, uint32_t(p.BN) * 128u);
-            tma_load_2d(tiles_base + stage * stage_bytes, &tmB, fb, p.tap_b[ti] * p.Kc + kbb * p.KB, nn0);
-          }
-        }
-      }
-    } else if (warp == 5) {
-      if (lane == 0) {
-        const uint32_t idesc = make_idesc_bf16(kTileM, uint32_t(p.BN), uint32_t(p.fmt));
-        int it = 0;
-        for (int kb = 0; kb < kb_total; ++kb) {
-          const int pa = kb & 1;
-          mbar_wait(smem_u32(&pfull_bar[pa]), uint32_t(kb >> 1) & 1u);
-          tc_fence_after();
-          const uint32_t patch = smem_base + pa * p.patch_bytes;
-          for (int ti = 0; ti < p.n_taps; ++ti, ++it) {
-            const int stage = it % p.stages;
-            const uint32_t phase = uint32_t(it / p.stages) & 1u;
-            mbar_wait(smem_u32(&full_bar[stage]), phase);
-            tc_fence_after();
-            const uint32_t shift = uint32_t((p.tap_dh[ti] - p.dh_min) * p.PW + (p.tap_dw[ti] - p.dw_min));
-            const uint32_t b_src = tiles_base + stage * stage_bytes;
-            for (int k = 0; k < 4; ++k) {
-              const uint64_t ad = make_kmajor_desc(patch + shift * 128u + k * 32, 128);
-              const uint64_t bd = make_kmajor_desc(b_src + k * 32, 128);
-              umma_bf16(tmem_d, ad, bd, idesc, (it > 0 || k > 0) ? 1u : 0u);
-            }
-            umma_commit(smem_u32(&empty_bar[stage]));
-          }
-          umma_commit(smem_u32(&pempty_bar[pa]));
-        }
-        umma_commit(smem_u32(&accum_bar));
-      }
-    }
-  } else if (warp == 4) {
+  if (warp == kProducerWarp) {
     if (lane == 0) {
       const uint32_t tx = uint32_t(p.BNI * p.BH * p.BW + p.BN) * uint32_t(p.row_bytes);
       int it = 0;
@@ -159,74 +106,132 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
-  } else if (warp == 5) {
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc_bf16(kTileM, uint32_t(p.BN), uint32_t(p.fmt));
-      const int k_steps = p.KB / 16;                  // UMMA K = 16 bf16 = 32 bytes
-      for (int it = 0; it < n_iters; ++it) {
-        const int stage = it % p.stages;
-        const uint32_t phase = uint32_t(it / p.stages) & 1u;
-        mbar_wait(smem_u32(&full_bar[stage]), phase);
-        tc_fence_after();
-        const uint32_t a_src = tiles_base + stage * stage_bytes;
-        for (int k = 0; k < k_steps; ++k) {
-          const uint64_t ad = make_kmajor_desc(a_src + k * 32, p.row_bytes);
-          const uint64_t bd = make_kmajor_desc(a_src + a_bytes + k * 32, p.row_bytes);
-          umma_bf16(tmem_d, ad, bd, idesc, (it > 0 || k > 0) ? 1u : 0u);
-        }
-        umma_commit(smem_u32(&empty_bar[stage]));     // slot reusable once these MMAs retire
+  } else {
+    const int wg = warp >> 2, wq = warp & 3;
+    const int nch = p.BN / NW;
+    float acc[NCH][NW / 2];
+#pragma unroll
+    for (int c = 0; c < NCH; ++c)
+#pragma unroll
+      for (int i = 0; i < NW / 2; ++i) acc[c][i] = 0.f;
+    const int k_steps = p.row_bytes / 32;          // one wgmma consumes 32 bytes of every row
+    for (int it = 0; it < n_iters; ++it) {
+      const int stage = it % p.stages;
+      mbar_wait(smem_u32(&full_bar[stage]), uint32_t(it / p.stages) & 1u);
+      const uint32_t a_src = tiles_base + stage * stage_bytes + uint32_t(wg * 64 * p.row_bytes);
+      const uint32_t b_src = tiles_base + stage * stage_bytes + a_bytes;
+      wgmma_fence();
+      for (int k = 0; k < k_steps; ++k) {
+        const uint64_t ad = make_kmajor_desc(a_src + k * 32, p.row_bytes);
+#pragma unroll
+        for (int c = 0; c < NCH; ++c)
+          if (c < nch)
+            wgmma_ss<NW, KIND>(acc[c], ad, make_kmajor_desc(b_src + uint32_t(c * NW * p.row_bytes) + k * 32, p.row_bytes));
       }
-      umma_commit(smem_u32(&accum_bar));
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (it > 0 && (threadIdx.x & 127) == 0) mbar_arrive(smem_u32(&empty_bar[(it - 1) % p.stages]));
     }
-  }
-  if (warp < 4) {
-    // ---- epilogue: warp w <-> TMEM lanes [32w, 32w+32) <-> tile rows ----
-    const int m = warp * 32 + lane;
-    const int rw = p.halo ? p.PW : p.BW;               // halo tiles live in padded-width pixel space
-    const int wi = m % rw;
-    const int q = m / rw;
-    const int hi = q % p.BH, ni = (p.halo && wi >= p.BW) ? p.BNI : q / p.BH;
-    const int oh = (h0 + hi) * p.out_step + p.out_off_h, ow = wi * p.out_step + p.out_off_w;
-    const bool valid = (ni < p.BNI) && (h0 + hi < p.OH) && (n0 + ni < p.NIMG) && oh < p.OHf && ow < p.OWf;
-    const int64_t pix = (int64_t(n0 + ni) * p.OHf + oh) * p.OWf + ow;
-    float* orow = p.out + pix * p.Nout + nn0;
-    const int mask_words = (p.Nout + 31) >> 5;
+    wgmma_wait<0>();
+#pragma unroll
+    for (int c = 0; c < NCH; ++c) wgmma_fence_regs(acc[c]);
 
-    mbar_wait(smem_u32(&accum_bar), 0);
-    tc_fence_after();
-    const float post = p.amax_bits ? amax_pow2_scale(__ldg(p.amax_bits), true) : 1.0f;
-    const uint32_t lane_base = tmem_d + (uint32_t(warp * 32) << 16);
-    for (int c0 = 0; c0 < p.BN; c0 += 16) {
-      uint32_t v[16];
-      tmem_ld16(lane_base + uint32_t(c0), v);
-      tmem_ld_wait();
-      if (valid) {
-        float f[16];
+    // ---- epilogue: this thread holds rows r and r + 8 (r = 64 wg + 16 wq + lane/4), column pairs 8j + 2(lane%4) ----
+    const float post = (MODE == 1 && p.amax_bits) ? amax_pow2_scale(__ldg(p.amax_bits), true) : 1.0f;
+    const int mask_words = (p.Nout + 31) >> 5;
+    int64_t pix[2];
+    bool valid[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int m = wg * 64 + wq * 16 + (lane >> 2) + 8 * h;
+      const int wi = m % p.BW;
+      const int q = m / p.BW;
+      const int hi = q % p.BH, ni = q / p.BH;
+      const int oh = (h0 + hi) * p.out_step + p.out_off_h, ow = wi * p.out_step + p.out_off_w;
+      valid[h] = (ni < p.BNI) && (h0 + hi < p.OH) && (n0 + ni < p.NIMG) && oh < p.OHf && ow < p.OWf;
+      pix[h] = (int64_t(n0 + ni) * p.OHf + oh) * p.OWf + ow;
+    }
+#pragma unroll
+    for (int c = 0; c < NCH; ++c) {
+      if (c >= nch) break;
+#pragma unroll
+      for (int j = 0; j < NW / 8; ++j) {
+        const int col = c * NW + 8 * j + 2 * (lane & 3);
+        const int ch = nn0 + col;
+        float a0 = 1.f, a1 = 1.f, sa0 = 0.f, sa1 = 0.f, sb0 = 0.f, sb1 = 0.f;
         if (MODE == 0) {
+          a0 = __ldg(p.alpha + ch); a1 = __ldg(p.alpha + ch + 1);
+        } else if (do_stats) {               // yhat = y_int * alpha * invstd - mean * invstd of the producing unit
+          const float is0 = __ldg(p.st_invstd + ch), is1 = __ldg(p.st_invstd + ch + 1);
+          sa0 = __ldg(p.st_alpha + ch) * is0; sa1 = __ldg(p.st_alpha + ch + 1) * is1;
+          sb0 = __ldg(p.st_mean + ch) * is0; sb1 = __ldg(p.st_mean + ch + 1) * is1;
+        }
+        float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f, m0 = 0.f, m1 = 0.f;
 #pragma unroll
-          for (int j = 0; j < 16; ++j) f[j] = __uint_as_float(v[j]) * __ldg(p.alpha + nn0 + c0 + j);
-        } else {
-          const int col = nn0 + c0;
-          const uint32_t word = __ldg(p.mask + pix * mask_words + (col >> 5)) >> (col & 31);
-#pragma unroll
-          for (int j = 0; j < 16; ++j) f[j] = ((word >> j) & 1u) ? __uint_as_float(v[j]) * post : 0.0f;
-          if (p.add != nullptr) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) f[j] += p.add[pix * p.Nout + nn0 + c0 + j];   // plain load: add may alias out
+        for (int h = 0; h < 2; ++h) {
+          if (!valid[h]) continue;
+          const float v0 = acc[c][4 * j + 2 * h], v1 = acc[c][4 * j + 2 * h + 1];
+          const int64_t off = pix[h] * p.Nout + ch;
+          float o0, o1;
+          if (MODE == 0) {
+            o0 = v0 * a0; o1 = v1 * a1;
+            if (p.out_i16 != nullptr)        // exact: |v| <= taps * Kc <= 32767
+              *reinterpret_cast<uint32_t*>(p.out_i16 + off) = (uint32_t(int(v0)) & 0xffffu) | (uint32_t(int(v1)) << 16);
+            else
+              *reinterpret_cast<float2*>(p.out + off) = make_float2(o0, o1);
+          } else {
+            const uint32_t word = __ldg(p.mask + pix[h] * mask_words + (ch >> 5)) >> (ch & 31);
+            o0 = (word & 1u) ? v0 * post : 0.0f;
+            o1 = (word & 2u) ? v1 * post : 0.0f;
+            if (p.add != nullptr) {          // plain load: add may alias out
+              const float2 ad = *reinterpret_cast<const float2*>(p.add + off);
+              o0 += ad.x; o1 += ad.y;
+            }
+            *reinterpret_cast<float2*>(p.out + off) = make_float2(o0, o1);
+          }
+          if (do_stats) {
+            s0 += o0; s1 += o1;
+            if (MODE == 1) {
+              const uint32_t yr = __ldg(reinterpret_cast<const uint32_t*>(p.st_y + off));
+              q0 += o0 * fmaf(float(int16_t(yr & 0xffffu)), sa0, -sb0);
+              q1 += o1 * fmaf(float(int16_t(yr >> 16)), sa1, -sb1);
+            } else {
+              q0 += o0 * o0; q1 += o1 * o1;
+            }
+            m0 = fmaxf(m0, fabsf(o0)); m1 = fmaxf(m1, fabsf(o1));
           }
         }
+        if (do_stats) {
+          // lanes with the same lane % 4 hold the same two channels for different rows
 #pragma unroll
-        for (int j = 0; j < 16; j += 4)
-          *reinterpret_cast<float4*>(orow + c0 + j) = make_float4(f[j], f[j + 1], f[j + 2], f[j + 3]);
+          for (int d = 4; d <= 16; d <<= 1) {
+            s0 += __shfl_xor_sync(0xffffffffu, s0, d); s1 += __shfl_xor_sync(0xffffffffu, s1, d);
+            q0 += __shfl_xor_sync(0xffffffffu, q0, d); q1 += __shfl_xor_sync(0xffffffffu, q1, d);
+            m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, d)); m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, d));
+          }
+          if (lane < 4) {            // each warp owns distinct rows: one writer per (warp, channel)
+            stat_sum[warp][col] = s0; stat_sum[warp][col + 1] = s1;
+            stat_sq[warp][col] = q0; stat_sq[warp][col + 1] = q1;
+            stat_max[warp][col] = m0; stat_max[warp][col + 1] = m1;
+          }
+        }
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_d, tmem_cols);
+  if (do_stats) {
+    __syncthreads();
+    // this CTA's row of the statistics partials (summed over CTAs in a fixed order after the kernel)
+    double* row = p.stat_part + int64_t(blockIdx.x) * 2 * p.Nout;
+    for (int i = threadIdx.x; i < p.BN; i += blockDim.x) {
+      double su = 0.0, sq = 0.0;
+      float mx = 0.f;
+      for (int w = 0; w < kTcThreads / 32 - 1; ++w) {
+        su += double(stat_sum[w][i]); sq += double(stat_sq[w][i]); mx = fmaxf(mx, stat_max[w][i]);
+      }
+      row[nn0 + i] = su;
+      row[p.Nout + nn0 + i] = sq;
+      atomicMax(p.bn_ymax + nn0 + i, __float_as_uint(mx));
+    }
   }
 }
 
@@ -242,19 +247,23 @@ static bool tc_shape_ok(const bdbnn_conv_shape* s) {
   return true;
 }
 
-template <int MODE>
-static int launch_tc_conv(const TcConvLaunch& L, cudaStream_t st) {
-  // Persistent multi-accumulator kernel first (tc_conv2.cu); BDBNN_TC_V2=0 forces the simple kernel.
-  static const int v2_env = [] { const char* e = getenv("BDBNN_TC_V2"); return e ? atoi(e) : 1; }();
-  if (v2_env) {
-    const int rc64 = launch_tc_conv64(L, MODE, st);        // 64-channel layers: pixels as the N = 256 dimension
-    if (rc64 != BDBNN_ERR_UNSUPPORTED) return rc64;
-    const int rc2 = launch_tc_conv2(L, MODE, st);
-    if (rc2 != BDBNN_ERR_UNSUPPORTED) return rc2;
-  }
-  if (L.out_i16) return BDBNN_ERR_UNSUPPORTED;      // int16 output exists in the persistent kernel only
-  TcConvParams p;
+// GEMMs whose contraction is a whole number of 64-channel K blocks (stem windows: 32 halves) and whose N is 64 or a
+// multiple of 128: the launches that may ask for the int16 result or for the dgrad's BatchNorm statistics.
+static bool wide_gemm(const TcConvLaunch& L) {
+  if (L.n_taps <= 0) return false;
+  if (L.win ? (L.Kc != 32 || L.fmt < 0) : (L.Kc % 64 != 0)) return false;
+  return L.Nout == 64 || L.Nout % 128 == 0;
+}
+
+// Tiling of one launch; returns false when the launch asks for something this kernel cannot give.
+static bool plan_tc_conv(const TcConvLaunch& L, int mode, TcConvParams* pp, size_t* smem_out, int* tiles_out) {
+  if (L.n_taps <= 0 || L.OW > kTileM) return false;
+  if ((L.out_i16 || (mode == 1 && L.bn_sums)) && !wide_gemm(L)) return false;
+  if (L.out_i16 && (mode != 0 || L.n_taps * L.Kc * L.a_halves > 32767)) return false;
+  if (mode == 1 && L.bn_sums && !(L.st_y && L.st_alpha && L.st_mean && L.st_invstd && L.out_step == 1)) return false;
+  TcConvParams& p = *pp;
   memset(&p, 0, sizeof(p));
+  const int esize = L.fmt < 0 ? 1 : 2;
   p.OW = L.OW; p.OH = L.OH; p.NIMG = L.NIMG;
   p.BW = L.OW;
   if (L.OH * L.OW <= kTileM) {
@@ -267,13 +276,13 @@ static int launch_tc_conv(const TcConvLaunch& L, cudaStream_t st) {
     p.BNI = 1;
   }
   p.tiles_h = (L.OH + p.BH - 1) / p.BH;
-  const int tiles_n = (L.NIMG + p.BNI - 1) / p.BNI;
   p.Kc = L.Kc;
-  p.KB = L.Kc >= 64 ? 64 : L.Kc;
+  p.KB = L.Kc * esize >= 128 ? 128 / esize : L.Kc;
+  if (L.Kc % p.KB != 0) return false;
   p.n_kb = L.Kc / p.KB;
   p.a_halves = L.a_halves;
   p.in_step = L.in_step;
-  p.row_bytes = p.KB * 2;
+  p.row_bytes = p.KB * esize;
   p.n_taps = L.n_taps;
   memcpy(p.tap_dh, L.dh, sizeof(p.tap_dh));
   memcpy(p.tap_dw, L.dw, sizeof(p.tap_dw));
@@ -281,62 +290,75 @@ static int launch_tc_conv(const TcConvLaunch& L, cudaStream_t st) {
   p.out_step = L.out_step; p.out_off_h = L.off_h; p.out_off_w = L.off_w; p.OHf = L.OHf; p.OWf = L.OWf;
   p.Nout = L.Nout;
   p.BN = pick_bn(L.Nout);
-  p.alpha = L.alpha; p.mask = L.mask; p.out = L.out;
-  p.fmt = L.fmt; p.amax_bits = L.amax_bits; p.add = L.add;
-  // Halo mode (stride-1 launches with >128-pixel images and 64-channel K blocks): see TcConvParams.
-  static const int halo_env = [] { const char* e = getenv("BDBNN_TC_HALO"); return e ? atoi(e) : 1; }();
-  if (halo_env > 0 && !L.win && L.in_step == 1 && p.KB == 64 && L.OH * L.OW > kTileM && p.n_taps > 0) {
-    int dh0 = 127, dh1 = -127, dw0 = 127, dw1 = -127;
-    for (int i = 0; i < p.n_taps; ++i) {
-      dh0 = min(dh0, int(p.tap_dh[i])); dh1 = max(dh1, int(p.tap_dh[i]));
-      dw0 = min(dw0, int(p.tap_dw[i])); dw1 = max(dw1, int(p.tap_dw[i]));
-    }
-    const int PW = L.OW + (dw1 - dw0);
-    if (PW <= kTileM) {
-      p.halo = 1;
-      p.PW = PW; p.dh_min = dh0; p.dw_min = dw0;
-      p.BNI = 1;
-      p.BH = kTileM / PW;
-      p.PH = p.BH + (dh1 - dh0);
-      p.tiles_h = (L.OH + p.BH - 1) / p.BH;
-      const int rows = kTileM + (dh1 - dh0) * PW + (dw1 - dw0);
-      p.patch_bytes = int((uint32_t(rows) * 128u + 1023u) & ~1023u);
-    }
-  }
-  const int tiles_n_eff = (L.NIMG + p.BNI - 1) / p.BNI;
-  const uint32_t stage_bytes = p.halo ? ((uint32_t(p.BN) * 128u + 1023u) & ~1023u)
-                                      : ((uint32_t(kTileM + p.BN) * p.row_bytes + 1023u) & ~1023u);
+  if (L.fmt < 0 && p.BN < 64) return false;
+  p.alpha = L.alpha; p.mask = L.mask; p.out = L.out; p.out_i16 = mode == 0 ? L.out_i16 : nullptr;
+  p.amax_bits = L.amax_bits; p.add = L.add;
+  p.bn_sums = L.bn_sums; p.bn_ymax = L.bn_ymax;
+  p.st_y = L.st_y; p.st_alpha = L.st_alpha; p.st_mean = L.st_mean; p.st_invstd = L.st_invstd;
+  const uint32_t stage_bytes = (uint32_t(kTileM + p.BN) * p.row_bytes + 1023u) & ~1023u;
   const int n_iters = p.n_taps * p.n_kb * p.a_halves;
-  const uint32_t ring_budget = 96u * 1024u - (p.halo ? 2u * uint32_t(p.patch_bytes) : 0u);
-  int stages = int(ring_budget / stage_bytes);
+  // a 96 KB ring leaves room for two CTAs per SM
+  int stages = int((96u * 1024u) / stage_bytes);
   if (stages > kMaxStages) stages = kMaxStages;
   if (stages > n_iters) stages = n_iters;
   if (stages < 2) stages = 2;
   p.stages = stages;
-  const size_t smem = size_t(stages) * stage_bytes + (p.halo ? 2u * size_t(p.patch_bytes) : 0u) + 1024;
+  *smem_out = size_t(stages) * stage_bytes + 1024;
+  *tiles_out = p.tiles_h * ((L.NIMG + p.BNI - 1) / p.BNI);
+  return true;
+}
 
+template <int MODE, int KIND>
+static int launch_kind(const CUtensorMap& tmA, const CUtensorMap& tmB, const TcConvParams& p, size_t smem, dim3 grid,
+                       cudaStream_t st) {
+  auto kern = p.BN == 16 ? tc_conv_kernel<MODE, KIND, 16>
+                         : (p.BN == 32 ? tc_conv_kernel<MODE, KIND, 32> : tc_conv_kernel<MODE, KIND, 64>);
+  BDBNN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+  if (p.bn_sums == nullptr) {
+    kern<<<grid, kTcThreads, smem, st>>>(tmA, tmB, p);
+    return check_launch("tc_conv_kernel");
+  }
+  TcConvParams q = p;
+  int rc = det_sums_alloc(&q.stat_part, grid.x, 2 * p.Nout, st);
+  if (rc) return rc;
+  kern<<<grid, kTcThreads, smem, st>>>(tmA, tmB, q);
+  rc = check_launch("tc_conv_kernel");
+  if (rc) { cudaFreeAsync(q.stat_part, st); return rc; }
+  return det_sums_finish(q.stat_part, grid.x, 2 * p.Nout, p.bn_sums, st);
+}
+
+template <int MODE>
+static int launch_tc_conv(const TcConvLaunch& L, cudaStream_t st) {
+  TcConvParams p;
+  size_t smem = 0;
+  int tiles = 0;
+  if (!plan_tc_conv(L, MODE, &p, &smem, &tiles)) {
+    set_error("tc_conv: launch geometry not supported");
+    return BDBNN_ERR_UNSUPPORTED;
+  }
+  const int esize = L.fmt < 0 ? 1 : 2;
   CUtensorMap tmA, tmB;
   int rc;
   if (L.win)   // stem: overlapping windows, row step in_step, window step 1
     rc = make_window_map(&tmA, L.A, L.NIMG, L.IH, L.IW, p.KB, L.win_stride, L.win_row_stride, L.win_img_stride,
                          p.BW, p.BH, p.BNI, L.in_step);
   else
-    rc = p.halo ? make_act_map(&tmA, L.A, L.NIMG, L.IH, L.IW, L.Kc * L.a_halves, 64, p.PW, p.PH, 1, 1)
-                : make_act_map(&tmA, L.A, L.NIMG, L.IH, L.IW, L.Kc * L.a_halves, p.KB, p.BW, p.BH, p.BNI,
-                               L.in_step);
+    rc = make_act_map(&tmA, L.A, L.NIMG, L.IH, L.IW, L.Kc * L.a_halves, p.KB, p.BW, p.BH, p.BNI, L.in_step, esize);
   if (rc) return rc;
-  rc = make_weight_map(&tmB, L.B, L.Nout, L.b_taps * L.Kc, p.KB, p.BN);
+  rc = make_weight_map(&tmB, L.B, L.Nout, L.b_taps * L.Kc, p.KB, p.BN, esize);
   if (rc) return rc;
-  auto kern = tc_conv_kernel<MODE>;
-  BDBNN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
-  dim3 grid(unsigned(p.tiles_h * tiles_n_eff), unsigned(L.Nout / p.BN));
-  kern<<<grid, kTcThreads, smem, st>>>(tmA, tmB, p);
-  rc = check_launch("tc_conv_kernel");
-  if (rc) return rc;
-  // this kernel has no statistics epilogue: one extra pass over the result when they were asked for
-  if (MODE == 0 && L.bn_sums != nullptr)
-    return bn_stats_launch(L.out, int64_t(L.NIMG) * L.OHf * L.OWf, L.Nout, L.bn_sums, L.bn_ymax, st);
-  return BDBNN_OK;
+  const dim3 grid(unsigned(tiles), unsigned(L.Nout / p.BN));
+  // forward statistics of the narrow (16/32-channel) GEMMs: one pass over the fp32 result after the kernel
+  const bool stats_pass = MODE == 0 && L.bn_sums != nullptr && !wide_gemm(L) && L.out != nullptr;
+  if (stats_pass) { p.bn_sums = nullptr; p.bn_ymax = nullptr; }
+  if (L.fmt < 0) {
+    if (MODE != 0) { set_error("tc_conv: fp8 operands are forward only"); return BDBNN_ERR_UNSUPPORTED; }
+    return launch_kind<0, 2>(tmA, tmB, p, smem, grid, st);
+  }
+  rc = L.fmt == BDBNN_FMT_BF16 ? launch_kind<MODE, 1>(tmA, tmB, p, smem, grid, st)
+                               : launch_kind<MODE, 0>(tmA, tmB, p, smem, grid, st);
+  if (rc || !stats_pass) return rc;
+  return bn_stats_launch(L.out, int64_t(L.NIMG) * L.OHf * L.OWf, L.Nout, L.bn_sums, L.bn_ymax, st);
 }
 
 // Stem conv forward (7x7 / stride 2 / pad 3 on 3 channels) as a 7-tap implicit GEMM over the packed
@@ -356,10 +378,12 @@ int launch_stem_fwd(const uint16_t* xw, const uint16_t* wf, const float* alpha, 
   L.bn_sums = bn_sums; L.bn_ymax = bn_ymax;
   int rc = bn_stats_zero(bn_sums, bn_ymax, kStemCout, st);
   if (rc) return rc;
-  rc = launch_tc_conv64_stem(L, st);            // pixel-N kernel (tc_conv64.cu); falls back to the pixel-M kernels
-  if (rc != BDBNN_ERR_UNSUPPORTED) return rc;
   return launch_tc_conv<0>(L, st);
 }
+
+static long long* g_trace = nullptr;
+void set_tc_trace(long long* buf) { g_trace = buf; }
+long long* get_tc_trace() { return g_trace; }
 
 }  // namespace bdbnn
 
@@ -370,9 +394,10 @@ extern "C" int bdbnn_debug_trace(long long* device_buf) {
   return BDBNN_OK;
 }
 
-// Host-only: the persistent kernel's tiling for the forward (mode 0: 16-bit operands, 2: fp8) or the first
-// dgrad phase (mode 1) of a shape.  out[12] = {planned, halo, TS, NB, BN, n_tiles, supers, stages, dynamic smem,
-// grid, stage bytes, patch bytes}; planned = 0 when the shape goes to the one-tile kernel.  No CUDA call.
+// Host-only: the kernel's tiling for the forward (mode 0: 16-bit operands, 2: fp8) or the first dgrad phase
+// (mode 1) of a shape.  out[12] = {planned, halo, TS, NB, BN, n_tiles, supers, stages, dynamic smem, grid,
+// stage bytes, patch bytes}; halo = 0, TS = NB = 1 (one 128-row tile per CTA, no patch), supers = M tiles.
+// planned = 0 when the GEMM is not eligible for the int16 result / fused dgrad statistics.  No CUDA call.
 extern "C" int bdbnn_debug_conv_plan(const bdbnn_conv_shape* s, int32_t mode, int32_t grad_halves, int32_t* out,
                                      int32_t n_out) {
   int rc = validate_shape(s);
@@ -413,21 +438,23 @@ extern "C" int bdbnn_debug_conv_plan(const bdbnn_conv_shape* s, int32_t mode, in
     L.fmt = mode == 2 ? -1 : BDBNN_FMT_FP16;
     if (mode == 2 && s->Cin % 128 != 0) return BDBNN_OK;
   }
-  if (L.n_taps == 0) return BDBNN_OK;
-  set_conv_plan_sink(out);
-  rc = launch_tc_conv2(L, mode == 1 ? 1 : 0, nullptr);
-  set_conv_plan_sink(nullptr);
-  if (rc == BDBNN_ERR_UNSUPPORTED) { memset(out, 0, 12 * sizeof(int32_t)); return BDBNN_OK; }
-  return rc;
+  if (L.n_taps == 0 || !wide_gemm(L)) return BDBNN_OK;
+  TcConvParams p;
+  size_t smem = 0;
+  int tiles = 0;
+  if (!plan_tc_conv(L, mode == 1 ? 1 : 0, &p, &smem, &tiles)) return BDBNN_OK;
+  const int32_t v[12] = {1, 0, 1, 1, p.BN, L.Nout / p.BN, tiles, p.stages, int32_t(smem), tiles * (L.Nout / p.BN),
+                         int32_t((uint32_t(kTileM + p.BN) * p.row_bytes + 1023u) & ~1023u), 0};
+  memcpy(out, v, sizeof(v));
+  return BDBNN_OK;
 }
 
 extern "C" int bdbnn_tc_supported(const bdbnn_conv_shape* s) {
   if (!tc_shape_ok(s)) return 0;
-  // fp8 forward only with 128-byte K rows (Cin % 128 == 0): with 64-channel (64-byte, SWIZZLE_64B) rows
-  // each K=32 MMA took ~240 clk on B200 (vs ~105 clk for the 16-bit K=16 MMA), i.e. no gain for layer1
+  // fp8 forward only with 128-byte K rows (Cin % 128 == 0)
   const bool v2 = s->Cin % 128 == 0 && (s->Cout == 64 || s->Cout % 128 == 0);
-  // int16 forward output: the persistent kernel must take the 16-bit-operand forward of this shape, and the
-  // integer result must fit (|y_int| <= kh*kw*Cin)
+  // int16 forward output: the forward GEMM must be eligible (bdbnn_debug_conv_plan) and the integer result
+  // must fit (|y_int| <= kh*kw*Cin)
   bool i16 = s->kh * s->kw * s->Cin <= 32767 && s->Cout <= 512;
   if (i16) {
     int32_t plan[12] = {0};
@@ -468,10 +495,7 @@ extern "C" int bdbnn_binconv_fwd_tc_i16(const void* xb, const void* wf, int32_t 
   L.bn_sums = bn_sums; L.bn_ymax = bn_ymax;
   rc = bn_stats_zero(bn_sums, bn_ymax, s->Cout, cudaStream_t(stream));
   if (rc) return rc;
-  rc = launch_tc_conv64(L, 0, cudaStream_t(stream));
-  if (rc == BDBNN_ERR_UNSUPPORTED) rc = launch_tc_conv2(L, 0, cudaStream_t(stream));
-  if (rc == BDBNN_ERR_UNSUPPORTED) set_error("binconv_fwd_tc_i16: geometry not supported by the persistent kernel");
-  return rc;
+  return launch_tc_conv<0>(L, cudaStream_t(stream));
 }
 
 extern "C" int bdbnn_binconv_fwd_tc(const uint16_t* xb_bf16, const uint16_t* wf_bf16, int32_t fmt,
@@ -481,7 +505,7 @@ extern "C" int bdbnn_binconv_fwd_tc(const uint16_t* xb_bf16, const uint16_t* wf_
   int rc = validate_shape(s);
   if (rc) return rc;
   BDBNN_REQUIRE(xb_bf16 && wf_bf16 && alpha && y, "binconv_fwd_tc: NULL pointer");
-  if (!tc_shape_ok(s)) { set_error("binconv_fwd_tc: shape not supported by the tcgen05 path"); return BDBNN_ERR_UNSUPPORTED; }
+  if (!tc_shape_ok(s)) { set_error("binconv_fwd_tc: shape not supported by the tensor-core path"); return BDBNN_ERR_UNSUPPORTED; }
   TcConvLaunch L;
   memset(&L, 0, sizeof(L));
   L.A = xb_bf16; L.IH = s->H; L.IW = s->W; L.Kc = s->Cin; L.a_halves = 1; L.in_step = s->stride;
@@ -509,7 +533,7 @@ extern "C" int bdbnn_binconv_fwd_tc8(const uint8_t* xb_fp8, const uint8_t* wf_fp
   if (rc) return rc;
   BDBNN_REQUIRE(xb_fp8 && wf_fp8 && alpha && y, "binconv_fwd_tc8: NULL pointer");
   if (!tc_shape_ok(s) || s->Cin % 128 != 0) {
-    set_error("binconv_fwd_tc8: shape not supported by the fp8 tcgen05 path");
+    set_error("binconv_fwd_tc8: shape not supported by the fp8 tensor-core path");
     return BDBNN_ERR_UNSUPPORTED;
   }
   TcConvLaunch L;
@@ -531,9 +555,7 @@ extern "C" int bdbnn_binconv_fwd_tc8(const uint8_t* xb_fp8, const uint8_t* wf_fp
   L.bn_sums = bn_sums; L.bn_ymax = bn_ymax;
   rc = bn_stats_zero(bn_sums, bn_ymax, s->Cout, cudaStream_t(stream));
   if (rc) return rc;
-  rc = launch_tc_conv2(L, 0, cudaStream_t(stream));
-  if (rc == BDBNN_ERR_UNSUPPORTED) set_error("binconv_fwd_tc8: geometry not supported by the persistent kernel");
-  return rc;
+  return launch_tc_conv<0>(L, cudaStream_t(stream));
 }
 
 struct DgradStats {      // backward statistics of the BatchNorm unit that produced this conv's input (see tc_common.cuh)
@@ -550,7 +572,7 @@ static int dgrad_tc_impl(const uint16_t* gys_bf16, int32_t grad_mode, const uint
   BDBNN_REQUIRE(grad_mode >= BDBNN_GRAD_BF16 && grad_mode <= BDBNN_GRAD_FP16S, "binconv_dgrad_tc: bad grad_mode");
   BDBNN_REQUIRE(grad_mode != BDBNN_GRAD_FP16S || amax_bits, "binconv_dgrad_tc: FP16S needs amax_bits");
   const int grad_halves = grad_mode == BDBNN_GRAD_BF16X2 ? 2 : 1;
-  if (!tc_shape_ok(s)) { set_error("binconv_dgrad_tc: shape not supported by the tcgen05 path"); return BDBNN_ERR_UNSUPPORTED; }
+  if (!tc_shape_ok(s)) { set_error("binconv_dgrad_tc: shape not supported by the tensor-core path"); return BDBNN_ERR_UNSUPPORTED; }
   cudaStream_t st = cudaStream_t(stream);
   const int T = s->kh * s->kw, sd = s->stride;
   // gx[h,w,c] = sum over taps (r,q) with (h+p-r) % sd == 0 (same in w) of
@@ -597,20 +619,11 @@ static int dgrad_tc_impl(const uint16_t* gys_bf16, int32_t grad_mode, const uint
     else if (add == nullptr) BDBNN_CUDA(cudaMemsetAsync(gx, 0, bytes, st));
   }
   if (stats) {
-    // one phase (stride 1), persistent kernel only: its epilogue owns the statistics
+    // one phase (stride 1): the epilogue owns the statistics
     if (n_launch != 1 || empty_phase) { set_error("binconv_dgrad_tc_stats: needs stride 1"); return BDBNN_ERR_UNSUPPORTED; }
-    static const int c64_env = [] { const char* e = getenv("BDBNN_TC_C64"); return e ? atoi(e) : 1; }();
-    if (c64_env < 2 && tc_conv64_eligible(Ls[0])) {
-      // 64-channel layers: the plain pixel-N dgrad + the separate reduction pass is faster (see tc_conv64.cu)
-      set_error("binconv_dgrad_tc_stats: declined for this shape (pixel-N kernel without statistics is faster)");
-      return BDBNN_ERR_UNSUPPORTED;
-    }
     rc = bn_stats_zero(stats->sums, stats->gmax, s->Cin, st);
     if (rc) return rc;
-    rc = launch_tc_conv64(Ls[0], 1, st);
-    if (rc == BDBNN_ERR_UNSUPPORTED) rc = launch_tc_conv2(Ls[0], 1, st);
-    if (rc == BDBNN_ERR_UNSUPPORTED) set_error("binconv_dgrad_tc_stats: geometry not supported by the persistent kernel");
-    return rc;
+    return launch_tc_conv<1>(Ls[0], st);
   }
   for (int i = 0; i < n_launch; ++i) {
     rc = launch_tc_conv<1>(Ls[i], st);

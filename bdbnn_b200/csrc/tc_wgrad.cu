@@ -1,48 +1,40 @@
-// Weight gradient on tensor cores (tcgen05 + TMA, sm_100a).
+// Weight gradient on tensor cores (wgmma + TMA, sm_90a).
 //
 //   D[(t,c), o] = sum_pix  xb[pix shifted by tap t, c] * gys[pix, o]          (K = output pixels)
 //
 // Both operands are "MN-major" for this GEMM: for a fixed pixel the M index (c) / N index (o) is the
 // contiguous one in NHWC memory, so a TMA box [pixels][64 channels] lands in shared memory exactly in
 // the canonical MN-major SWIZZLE_128B layout (8 pixel rows x 128 B per swizzle atom; SBO = 1024 B
-// between 8-row K groups; LBO = distance between the two 64-channel chunks of an M tile).
+// between 8-row K groups; LBO = distance between MN chunks).
 // An M tile of 128 rows is two 64-channel "units" (tap, channel-chunk); unit u = tap * (Cin/64) + chunk.
+// Per K stage one TMA box per unit is loaded (plus the gys boxes); warpgroup 0 multiplies rows [0, 64) of
+// every M tile, warpgroup 1 rows [64, 128).
 //
-// HALO mode (stride 1, images larger than 128 pixels): per K stage ONE activation patch per
-// 64-channel chunk is loaded — BH(+halo) image rows in padded-width raster order — and every tap is
-// that patch viewed from row offset (dh-dh_min)*PW + (dw-dw_min) (descriptor start + 128 B * shift;
-// the swizzle XOR is taken from absolute smem address bits, so row-shifted views are valid operands).
-// The gys box uses the same padded raster: its columns >= Wo fall outside the tensor and TMA zero-fills
-// them, so the padded K rows contribute exactly 0.  L2->SM traffic drops ~3x versus one box per tap.
-// BOX mode (small images, stride 2): one TMA box per unit, as before.
-//
-// Each CTA owns up to G accumulators (G*BN <= 512 TMEM columns) that share the gys stage, walks a
-// contiguous range of K stages (split-K across CTAs) and writes its partial tiles to its own slice of
-// an fp32 workspace [ksplit][T*Cin][Cout] (plain stores: a red.global.add flush of 148 CTAs onto the
-// same 37 K addresses cost 57 K cycles, 30 % of the layer-1 kernel); the finalize kernel sums the
+// Each CTA owns up to G accumulators (G*BN <= 256: 128 fp32 registers per thread) that share the gys stage,
+// walks a contiguous range of K stages (split-K across CTAs) and writes its partial tiles to its own slice of
+// an fp32 workspace [ksplit][T*Cin][Cout] (plain stores, no atomics); the finalize kernel sums the
 // slices in a fixed order (run-to-run deterministic), applies 1/gscale[o], the FP16S 2^-e, the
 // |W|<=1 STE mask and the [t][c][o] -> OIHW transposition.
 #include "tc_common.cuh"
 
 namespace bdbnn {
 
-constexpr int kMaxUnits = 16;      // units per CTA (G <= 5 M tiles of 2 units, or 2 tiles of 8 16-wide units)
+constexpr int kWgradWaves = 3;
+constexpr int kMaxUnits = 16;      // units per CTA (G <= 4 M tiles of 2 units, or 2 tiles of 8 16-wide units)
 
 struct TcWgradParams {
   int32_t OW, OH, NIMG;          // gy pixel grid
-  int32_t halo;
-  int32_t BW, BH, BNI, tiles_h;  // K stage = BNI x BH x (BW | PW) output pixels
-  int32_t PW, PH, dh_min, dw_min;
-  int32_t rows_a, rows_b;        // rows TMA writes per A box/patch and per B box
+  int32_t BW, BH, BNI, tiles_h;  // K stage = BNI x BH x BW output pixels
+  int32_t rows_a, rows_b;        // rows TMA writes per A box and per B box
   int32_t k_stage;               // K rows consumed per stage (multiple of 16)
-  uint32_t a_box_bytes;          // smem footprint of one A box/patch (1024-aligned)
+  uint32_t a_box_bytes;          // smem footprint of one A box (1024-aligned)
   uint32_t b_box_bytes;
-  int32_t n_a_boxes;             // A boxes/patches per stage
+  int32_t n_a_boxes;             // A boxes per stage
   int32_t n_kboxes, kboxes_per_cta;
   int32_t Cin, Cout, kh, kw, pad, stride;
   int32_t g_halves;              // 1: gys = bf16(g); 2: gys = [hi | lo] split, both accumulated
-  int32_t UW;                    // unit width in channels: 64 (128-byte rows, SWIZZLE_128B) or 32 (stem
-                                 // windows: 64-byte rows, SWIZZLE_64B); an M tile is 128/UW units
+  int32_t UW;                    // unit width in channels: 64 (128-byte rows, SWIZZLE_128B), 32 (64-byte rows,
+                                 // SWIZZLE_64B; stem windows) or 16 (SWIZZLE_32B); an M tile is 128/UW units
   int32_t chunks_per_tap;        // Cin / 64
   int32_t n_units, G;            // (tap, chunk) units; M tiles (accumulators) per CTA
   int32_t BN;                    // N tile (output channels per CTA)
@@ -61,32 +53,22 @@ struct TcWgradParams {
     }                                                                                            \
   } while (0)
 
-// row_bytes 128: SWIZZLE_128B atoms of 8 K rows x 64 MN elements; 64: SWIZZLE_64B, 8 x 32; 32: SWIZZLE_32B, 8 x 16.
-__device__ __forceinline__ uint64_t make_mnmajor_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t row_bytes = 128u) {
-  uint64_t d = 0;
-  d |= uint64_t((saddr & 0x3FFFFu) >> 4);
-  d |= uint64_t((lbo_bytes >> 4) & 0x3FFFu) << 16;   // LBO: stride between MN chunks (one swizzle row each)
-  d |= uint64_t((8u * row_bytes) >> 4) << 32;        // SBO: stride between 8-row K groups
-  d |= uint64_t(1) << 46;
-  d |= uint64_t(row_bytes == 128u ? 2u : (row_bytes == 64u ? 4u : 6u)) << 61;  // SWIZZLE_128B / _64B / _32B
-  return d;
-}
-
+// NW: wgmma N (16 or 32 for the narrow N tiles, else 64 with BN/64 chunks).  Accumulator slot s = g * (BN/NW) + chunk.
+template <int KIND, int NW>
 __global__ void __launch_bounds__(kTcThreads)
 tc_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmG,
                 const TcWgradParams p) {
+  constexpr int kSlots = 256 / NW;                               // 128 accumulator floats per thread
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[kMaxStages];
   __shared__ __align__(8) uint64_t empty_bar[kMaxStages];
-  __shared__ __align__(8) uint64_t accum_bar;
-  __shared__ uint32_t tmem_slot;
-  __shared__ uint32_t unit_off[kMaxUnits];   // byte offset of unit i's operand view inside a stage
-  __shared__ int32_t unit_c[kMaxUnits], unit_dw[kMaxUnits], unit_dh[kMaxUnits];   // box mode: TMA coordinates of unit i
+  __shared__ uint32_t unit_off[kMaxUnits];   // byte offset of unit i's operand box inside a stage
+  __shared__ int32_t unit_c[kMaxUnits], unit_dw[kMaxUnits], unit_dh[kMaxUnits];   // TMA coordinates of unit i
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t tiles_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const int mt0 = blockIdx.y * p.G;                               // first M tile of this CTA
-  const int upt = kTileM / p.UW;                                  // units per M tile (2 or 4)
+  const int upt = kTileM / p.UW;                                  // units per M tile (2, 4 or 8)
   const uint32_t a_row = uint32_t(p.UW) * 2u;                     // bytes per A row
   const int n_mtiles = (p.n_units + upt - 1) / upt;
   const int g_cta = min(p.G, n_mtiles - mt0);
@@ -98,27 +80,13 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
   const int nn0 = blockIdx.z * p.BN;
   const int kb_begin = blockIdx.x * p.kboxes_per_cta;
   const int kb_end = min(kb_begin + p.kboxes_per_cta, p.n_kboxes);
-  uint32_t tmem_cols = 32;
-  while (tmem_cols < uint32_t(p.G * p.BN)) tmem_cols <<= 1;
 
   if (threadIdx.x < g_cta * upt) {
     int u = mt0 * upt + threadIdx.x;
-    bool dup = false;
-    if (u >= p.n_units) { u = p.n_units - 1; dup = true; }        // odd unit count: rows ignored
+    if (u >= p.n_units) u = p.n_units - 1;                         // odd unit count: rows ignored
     const int t = u / p.chunks_per_tap, j = u - t * p.chunks_per_tap;
-    uint32_t off;
-    if (p.halo) {
-      const int r = t / p.kw, s = t - r * p.kw;
-      off = uint32_t(j) * p.a_box_bytes +
-            uint32_t((r - p.pad - p.dh_min) * p.PW + (s - p.pad - p.dw_min)) * 128u;
-      if (dup) off += 128u;                                        // keep LBO > 0
-    } else {
-      off = threadIdx.x * p.a_box_bytes;
-    }
-    unit_off[threadIdx.x] = off;
-    // the producer is ONE thread: everything per unit that needs a division is computed here, once (ncu of the
-    // layer4 launch showed the per-stage address arithmetic of 8 loads — ~750 dependent instructions — at 4.4 K
-    // cycles per stage, four times the MMA time)
+    unit_off[threadIdx.x] = threadIdx.x * p.a_box_bytes;
+    // the producer is ONE thread: everything per unit that needs a division is computed here, once
     const int r = t / p.kw, sx = t - r * p.kw;
     unit_c[threadIdx.x] = j * 64;
     unit_dw[threadIdx.x] = sx - p.pad;
@@ -127,9 +95,8 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(smem_u32(&full_bar[s]), 1);
-      mbar_init(smem_u32(&empty_bar[s]), 1);
+      mbar_init(smem_u32(&empty_bar[s]), 2);                       // one arrival per consumer warpgroup
     }
-    mbar_init(smem_u32(&accum_bar), 1);
     fence_barrier_init();
   }
   // Zero every row TMA never writes (A rows >= rows_a, B rows >= rows_b): they are read as K rows.
@@ -159,26 +126,21 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
     }
     fence_proxy_async();
   }
-  if (warp == 4 && lane == 0) {
+  if (warp == kProducerWarp && lane == 0) {
     prefetch_tmap(&tmX);
     prefetch_tmap(&tmG);
   }
-  if (warp == 5) tmem_alloc(smem_u32(&tmem_slot), tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_d = tmem_slot;
 
-  if (warp == 4) {
+  if (warp == kProducerWarp) {
     if (lane == 0) {
-      const int n_a_loads = p.halo ? p.n_a_boxes : g_cta * upt;
-      const uint32_t tx = uint32_t(n_a_loads) * uint32_t(p.rows_a) * a_row +
+      const int n_units_cta = g_cta * upt;
+      const uint32_t tx = uint32_t(n_units_cta) * uint32_t(p.rows_a) * a_row +
                           uint32_t(nb_boxes) * uint32_t(p.rows_b) * b_row;
       int tr_n = 0;
       int stage = 0;
       uint32_t phase = 0;
       int tile_n = kb_begin / p.tiles_h, tile_h = kb_begin - tile_n * p.tiles_h;   // advanced incrementally
-      const int n_units_cta = g_cta * upt;
       for (int kb = kb_begin; kb < kb_end; ++kb) {
         BDBNN_WTR(0, 0);
         mbar_wait(smem_u32(&empty_bar[stage]), phase ^ 1u);
@@ -187,14 +149,9 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
         mbar_expect_tx(fb, tx);
         const int n0 = tile_n * p.BNI, h0 = tile_h * p.BH;
         const uint32_t dst0 = tiles_base + stage * stage_bytes;
-        if (p.halo) {
-          for (int j = 0; j < p.n_a_boxes; ++j)
-            tma_load_4d(dst0 + j * p.a_box_bytes, &tmX, fb, j * 64, p.dw_min, h0 + p.dh_min, n0);
-        } else {
-          const int hs = h0 * p.stride;
-          for (int i = 0; i < n_units_cta; ++i)
-            tma_load_4d(dst0 + i * p.a_box_bytes, &tmX, fb, unit_c[i], unit_dw[i], hs + unit_dh[i], n0);
-        }
+        const int hs = h0 * p.stride;
+        for (int i = 0; i < n_units_cta; ++i)
+          tma_load_4d(dst0 + unit_off[i], &tmX, fb, unit_c[i], unit_dw[i], hs + unit_dh[i], n0);
         uint32_t bdst = dst0 + a_bytes;
         for (int hf = 0; hf < p.g_halves; ++hf)
           for (int jb = 0; jb < nb_chunks; ++jb, bdst += p.b_box_bytes)
@@ -203,79 +160,80 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
         if (++tile_h == p.tiles_h) { tile_h = 0; ++tile_n; }
       }
     }
-  } else if (warp == 5) {
-    if (lane == 0) {
-      // M=128, N=BN, A and B MN-major (bits 15/16)
-      const uint32_t idesc = make_idesc_bf16(kTileM, uint32_t(p.BN), uint32_t(p.fmt)) | (1u << 15) | (1u << 16);
-      const int k_steps = p.k_stage / 16;
-      int it = 0, tr_n = 0;
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int kb = kb_begin; kb < kb_end; ++kb, ++it) {
-        BDBNN_WTR(1, 0);
-        mbar_wait(smem_u32(&full_bar[stage]), phase);
-        tc_fence_after();
-        BDBNN_WTR(1, 1);
-        const uint32_t a0 = tiles_base + stage * stage_bytes;
-        const uint32_t b0 = a0 + a_bytes;
-        for (int g = 0; g < g_cta; ++g) {
-          const uint32_t ua = unit_off[upt * g], ub = unit_off[upt * g + 1];
-          const uint64_t ad0 = make_mnmajor_desc(a0 + ua, ub - ua, a_row);
-          const uint32_t a_kstep = a_row;                           // 16 K rows x a_row bytes, >> 4
-          const uint32_t a_lo0 = uint32_t(ad0), a_hi = uint32_t(ad0 >> 32);
-          const uint32_t acc = tmem_d + uint32_t(g * p.BN);
-          for (int hf = 0; hf < p.g_halves; ++hf) {
-            const uint64_t bd0 = make_mnmajor_desc(b0 + hf * nb_chunks * p.b_box_bytes, p.b_box_bytes, b_row);
-            const uint32_t b_kstep = b_row;                           // 16 K rows x b_row bytes, >> 4
-            const uint32_t b_lo0 = uint32_t(bd0), b_hi = uint32_t(bd0 >> 32);
-            // 16 pixel rows per K step: +2048 B (128-byte rows) = +128 in the low word's address field
-            umma_bf16_split(acc, a_lo0, a_hi, b_lo0, b_hi, idesc, (it > 0 || hf > 0) ? 1u : 0u);
-#pragma unroll 4
-            for (int k = 1; k < k_steps; ++k)
-              umma_bf16_split(acc, a_lo0 + uint32_t(k) * a_kstep, a_hi, b_lo0 + uint32_t(k) * b_kstep, b_hi, idesc, 1u);
+  } else if (kb_end > kb_begin) {
+    const int wg = warp >> 2, wq = warp & 3;
+    const int nch = p.BN / NW;                                     // wgmma chunks per M tile
+    const int n_slots = g_cta * nch;
+    const int u_wg = 64 / p.UW;                                    // units in this warpgroup's 64 rows
+    float acc[kSlots][NW / 2];
+#pragma unroll
+    for (int s = 0; s < kSlots; ++s)
+#pragma unroll
+      for (int i = 0; i < NW / 2; ++i) acc[s][i] = 0.f;
+    const int k_steps = p.k_stage / 16;
+    const uint32_t lbo_a = p.a_box_bytes;                          // MN stride between the units of one wgmma
+    int stage = 0;
+    uint32_t phase = 0;
+    int prev_stage = -1;
+    for (int kb = kb_begin; kb < kb_end; ++kb) {
+      mbar_wait(smem_u32(&full_bar[stage]), phase);
+      const uint32_t a0 = tiles_base + stage * stage_bytes;
+      const uint32_t b0 = a0 + a_bytes;
+      wgmma_fence();
+      for (int hf = 0; hf < p.g_halves; ++hf) {
+        for (int k = 0; k < k_steps; ++k) {
+          // 16 pixel rows per K step: 2 swizzle atoms of 8 rows
+#pragma unroll
+          for (int s = 0; s < kSlots; ++s) {
+            if (s < n_slots) {
+              const int g = s / nch, c = s - g * nch;
+              const uint64_t ad = make_smem_desc(a0 + unit_off[g * upt + wg * u_wg] + uint32_t(k) * 16u * a_row, lbo_a, a_row);
+              const uint64_t bd = make_smem_desc(b0 + uint32_t(hf * nb_chunks + c) * p.b_box_bytes + uint32_t(k) * 16u * b_row,
+                                                 p.b_box_bytes, b_row);
+              wgmma_ss<NW, KIND, 1, 1>(acc[s], ad, bd);
+            }
           }
         }
-        umma_commit(smem_u32(&empty_bar[stage]));
-        BDBNN_WTR(1, 4);
-        if (++stage == p.stages) { stage = 0; phase ^= 1u; }
       }
-      umma_commit(smem_u32(&accum_bar));
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev_stage >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(smem_u32(&empty_bar[prev_stage]));
+      prev_stage = stage;
+      if (++stage == p.stages) { stage = 0; phase ^= 1u; }
     }
-  } else if (kb_end > kb_begin) {
-    const int m = warp * 32 + lane;
-    int tr_n = threadIdx.x == 0 ? 0 : 100000;
-    BDBNN_WTR(2, 0);
-    mbar_wait(smem_u32(&accum_bar), 0);
-    tc_fence_after();
-    BDBNN_WTR(2, 1);
-    const uint32_t lane_base = tmem_d + (uint32_t(warp * 32) << 16);
-    for (int g = 0; g < g_cta; ++g) {
-      const int u = (mt0 + g) * upt + m / p.UW;
-      const bool valid = u < p.n_units;
-      float* wrow = p.ws + int64_t(blockIdx.x) * (int64_t(p.n_units) * p.UW * p.Cout) +
-                    (int64_t(u) * p.UW + (m % p.UW)) * p.Cout + nn0;       // slice, row (t*Cin + c)
-      for (int c0 = 0; c0 < p.BN; c0 += 16) {
-        uint32_t v[16];
-        tmem_ld16(lane_base + uint32_t(g * p.BN + c0), v);
-        tmem_ld_wait();
-        if (valid) {
+    wgmma_wait<0>();
 #pragma unroll
-          for (int j = 0; j < 16; j += 4)
-            *reinterpret_cast<float4*>(wrow + c0 + j) =
-                make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]),
-                            __uint_as_float(v[j + 3]));
-        }
+    for (int s = 0; s < kSlots; ++s) wgmma_fence_regs(acc[s]);
+    // ---- epilogue: rows m (and m + 8) of every M tile, column pairs 8j + 2(lane%4) of every chunk ----
+    float* slice = p.ws + int64_t(blockIdx.x) * (int64_t(p.n_units) * p.UW * p.Cout);
+#pragma unroll
+    for (int s = 0; s < kSlots; ++s) {
+      if (s >= n_slots) break;
+      const int g = s / nch, c = s - g * nch;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int m = wg * 64 + wq * 16 + (lane >> 2) + 8 * h;
+        const int u = (mt0 + g) * upt + m / p.UW;
+        if (u >= p.n_units) continue;
+        float* wrow = slice + (int64_t(u) * p.UW + (m % p.UW)) * p.Cout + nn0 + c * NW + 2 * (lane & 3);   // row t*Cin + c
+#pragma unroll
+        for (int j = 0; j < NW / 8; ++j)
+          *reinterpret_cast<float2*>(wrow + 8 * j) = make_float2(acc[s][4 * j + 2 * h], acc[s][4 * j + 2 * h + 1]);
       }
     }
-    BDBNN_WTR(2, 2);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_d, tmem_cols);
-  }
+}
+
+// Launch with the template arguments of the plan (operand format, wgmma N).
+static int launch_wgrad_kernel(const CUtensorMap& tmX, const CUtensorMap& tmG, const TcWgradParams& p, size_t smem,
+                               dim3 grid, cudaStream_t st) {
+  const int nw = p.BN >= 64 ? 64 : p.BN;
+  auto pick = [&](auto k16, auto k32, auto k64) { return nw == 16 ? k16 : (nw == 32 ? k32 : k64); };
+  auto kern = p.fmt == BDBNN_FMT_BF16 ? pick(tc_wgrad_kernel<1, 16>, tc_wgrad_kernel<1, 32>, tc_wgrad_kernel<1, 64>)
+                                      : pick(tc_wgrad_kernel<0, 16>, tc_wgrad_kernel<0, 32>, tc_wgrad_kernel<0, 64>);
+  BDBNN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+  kern<<<grid, kTcThreads, smem, st>>>(tmX, tmG, p);
+  return check_launch("tc_wgrad_kernel");
 }
 
 // gW[o][c][t] = wmask ? inv_gscale[o] * 2^-e * sum_k ws[k][(t*Cin + c)*Cout + o] : 0
@@ -327,7 +285,6 @@ static WgradPlan plan_wgrad(const bdbnn_conv_shape* s, int halves) {
   if (s->Cin % 64 != 0 || s->Cout % 64 != 0) return pl;
   if (s->Cout > 128 && s->Cout % 256 != 0) return pl;
   if (s->Wo > 128 || s->W > 128 * s->stride) return pl;
-  static const int halo_env = [] { const char* e = getenv("BDBNN_WGRAD_HALO"); return e ? atoi(e) : 1; }();
   TcWgradParams& p = pl.p;
   const int T = s->kh * s->kw;
   p.OW = s->Wo; p.OH = s->Ho; p.NIMG = s->N;
@@ -338,41 +295,16 @@ static WgradPlan plan_wgrad(const bdbnn_conv_shape* s, int halves) {
   p.n_units = T * p.chunks_per_tap;
   const int n_mtiles = (p.n_units + 1) / 2;
   p.BN = s->Cout >= 256 ? 256 : s->Cout;
-  p.G = 512 / p.BN;
+  p.G = 256 / p.BN;                                               // accumulator registers
   if (p.G > n_mtiles) p.G = n_mtiles;
-  if (p.G > 5) p.G = 5;
   {  // balance the M groups (e.g. 9 M tiles with G<=4 -> 3 groups of 3, not 4+4+1)
     const int groups = (n_mtiles + p.G - 1) / p.G;
     p.G = (n_mtiles + groups - 1) / groups;
   }
   p.stages = 2;
   const uint32_t budget = 222u * 1024u;
-  const int span = s->kh - 1;                                     // tap offsets span [-pad, k-1-pad]
-  const int PW = s->Wo + span;
-  bool planned = false;
-  if (halo_env && s->stride == 1 && s->Ho * s->Wo > kTileM && PW <= 256) {
-    // halo mode: patches hold (BH + span) x PW pixels; pick the largest BH whose 2-stage ring fits
-    for (int bh = (s->Ho < 16 ? s->Ho : 16); bh >= 1 && !planned; --bh) {
-      const int k_stage = (bh * PW + 15) & ~15;
-      if (k_stage > 512) continue;
-      const int rows_a = (bh + span) * PW;
-      const int view_rows = k_stage + span * PW + span + 1;       // rows a shifted view can touch
-      const uint32_t a_box = (uint32_t(max(rows_a, view_rows)) * 128u + 1023u) & ~1023u;
-      const uint32_t b_box = uint32_t(k_stage) * 128u;
-      const uint32_t stage = uint32_t(p.chunks_per_tap) * a_box + uint32_t(p.BN / 64 * halves) * b_box;
-      if (2u * stage > budget) continue;
-      // prefer row counts that waste little of the last stage of an image
-      const int tiles_h = (s->Ho + bh - 1) / bh;
-      if (tiles_h * bh - s->Ho > bh / 2 && bh > 1) continue;
-      p.halo = 1; p.PW = PW; p.PH = bh + span; p.dh_min = -s->pad; p.dw_min = -s->pad;
-      p.BW = PW; p.BH = bh; p.BNI = 1; p.tiles_h = tiles_h;
-      p.rows_a = rows_a; p.rows_b = bh * PW; p.k_stage = k_stage;
-      p.a_box_bytes = a_box; p.b_box_bytes = b_box; p.n_a_boxes = p.chunks_per_tap;
-      planned = true;
-    }
-  }
-  if (!planned) {
-    // box mode: one [rows][64ch] box per unit
+  {
+    // one [rows][64ch] box per unit
     const int row_bytes_all = p.G * 256 + p.BN * 2 * halves;      // smem bytes per pixel row per stage
     const int k_cap = int(budget / (unsigned(p.stages) * unsigned(row_bytes_all))) & ~15;
     if (k_cap < 16) return pl;
@@ -404,19 +336,19 @@ static WgradPlan plan_wgrad(const bdbnn_conv_shape* s, int halves) {
   p.n_kboxes = p.tiles_h * ((s->N + p.BNI - 1) / p.BNI);
   pl.mgroups = (n_mtiles + p.G - 1) / p.G;
   pl.ntiles = s->Cout / p.BN;
-  // split K so that the whole grid is ONE wave (<= #SMs CTAs): 1 CTA/SM by shared-memory size, and a
-  // second partial wave would double the kernel time
-  int ks = num_sms() / (pl.mgroups * pl.ntiles);
+  // split K over up to kWgradWaves waves of CTAs (1 CTA/SM by shared memory and registers): the register
+  // accumulators hold at most 256 columns per CTA, so one wave would leave fp32 accumulation chains of up to a
+  // whole layer's pixels in one CTA (bf16x2 wgrad error above 2e-5 of the L2 norm at N=256)
+  int ks = kWgradWaves * num_sms() / (pl.mgroups * pl.ntiles);
   if (ks < 1) ks = 1;
   pl.ks_cap = ks;                       // upper bound of ksplit for any gradient mode (workspace sizing)
   if (ks > p.n_kboxes) ks = p.n_kboxes;
   p.kboxes_per_cta = (p.n_kboxes + ks - 1) / ks;
   pl.ksplit = (p.n_kboxes + p.kboxes_per_cta - 1) / p.kboxes_per_cta;
   const size_t stage_bytes = size_t(p.n_a_boxes) * p.a_box_bytes + size_t(p.BN / 64 * halves) * p.b_box_bytes;
-  // Box-mode stages are small (32-64 K rows) and the loop is bound by the TMA round trip, not by bytes: use every
-  // stage the shared memory holds (BDBNN_WG_STAGES=2 restores the two-stage ring for A/B runs).
-  static const int stages_env = [] { const char* e = getenv("BDBNN_WG_STAGES"); return e ? atoi(e) : 0; }();
-  int stages = stages_env > 0 ? stages_env : int(budget / stage_bytes);
+  // stages are small (32-128 K rows) and the loop is bound by the TMA round trip, not by bytes: use every
+  // stage the shared memory holds
+  int stages = int(budget / stage_bytes);
   if (stages > kMaxStages) stages = kMaxStages;
   if (stages > p.kboxes_per_cta) stages = p.kboxes_per_cta;
   if (stages < 2) stages = 2;
@@ -449,8 +381,7 @@ static WgradPlan plan_wgrad_small(const bdbnn_conv_shape* s, int halves) {
   p.BN = s->Cout;
   p.G = kMaxUnits / upt;
   if (p.G > n_mtiles) p.G = n_mtiles;
-  if (p.G * p.BN > 512) p.G = 512 / p.BN;
-  p.halo = 0;
+  if (p.G * p.BN > 256) p.G = 256 / p.BN;
   p.BW = s->Wo;
   const int a_row = p.UW * 2, b_row = p.BN >= 64 ? 128 : p.BN * 2;
   // K stage: whole images when they are small, else rows of one image; <= 128 pixel rows
@@ -479,7 +410,7 @@ static WgradPlan plan_wgrad_small(const bdbnn_conv_shape* s, int halves) {
   if (p.stages > 4) p.stages = 4;
   pl.mgroups = (n_mtiles + p.G - 1) / p.G;
   pl.ntiles = 1;
-  int ks = num_sms() / pl.mgroups;
+  int ks = kWgradWaves * num_sms() / pl.mgroups;
   if (ks < 1) ks = 1;
   pl.ks_cap = ks;
   if (ks > p.n_kboxes) ks = p.n_kboxes;
@@ -563,11 +494,8 @@ int launch_stem_wgrad(const uint16_t* gys, const uint16_t* xw, float* ws, size_t
   if (rc) return rc;
   rc = make_act_map(&tmG, gys, g.N, g.Ho, g.Wo, kStemCout, 64, pl.p.BW, pl.p.BH, pl.p.BNI);
   if (rc) return rc;
-  BDBNN_CUDA(cudaFuncSetAttribute(tc_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(pl.smem)));
-  dim3 grid(unsigned(pl.ksplit), 1, 1);
-  tc_wgrad_kernel<<<grid, kTcThreads, pl.smem, st>>>(tmX, tmG, pl.p);
   *ksplit_out = pl.ksplit;
-  return check_launch("tc_wgrad_kernel(stem)");
+  return launch_wgrad_kernel(tmX, tmG, pl.p, pl.smem, dim3(unsigned(pl.ksplit), 1, 1), st);
 }
 
 }  // namespace bdbnn
@@ -580,7 +508,7 @@ extern "C" int bdbnn_debug_wgrad_plan(const bdbnn_conv_shape* s, int32_t grad_ha
   BDBNN_REQUIRE(grad_halves == 1 || grad_halves == 2, "debug_wgrad_plan: grad_halves must be 1 or 2");
   const WgradPlan pl = plan_wgrad(s, grad_halves);
   const int32_t v[12] = {pl.ok ? 1 : 0, pl.ksplit, pl.ks_cap, pl.mgroups, pl.ntiles, int32_t(pl.smem), pl.p.G, pl.p.BN,
-                         pl.p.UW, pl.p.halo, pl.p.k_stage, pl.p.stages};
+                         pl.p.UW, 0, pl.p.k_stage, pl.p.stages};
   memcpy(out, v, sizeof(v));
   return BDBNN_OK;
 }
@@ -608,7 +536,7 @@ extern "C" int bdbnn_binconv_wgrad_tc(const uint16_t* gys_bf16, int32_t grad_mod
   const int grad_halves = grad_mode == BDBNN_GRAD_BF16X2 ? 2 : 1;
   WgradPlan pl = plan_wgrad(s, grad_halves);
   pl.p.fmt = grad_mode == BDBNN_GRAD_FP16S ? BDBNN_FMT_FP16 : BDBNN_FMT_BF16;
-  if (!pl.ok) { set_error("binconv_wgrad_tc: shape not supported by the tcgen05 path"); return BDBNN_ERR_UNSUPPORTED; }
+  if (!pl.ok) { set_error("binconv_wgrad_tc: shape not supported by the tensor-core path"); return BDBNN_ERR_UNSUPPORTED; }
   const size_t need = bdbnn_wgrad_tc_workspace_bytes(s);
   if (workspace_bytes < need) {
     set_error("binconv_wgrad_tc: workspace %zu B < required %zu B", workspace_bytes, need);
@@ -618,18 +546,13 @@ extern "C" int bdbnn_binconv_wgrad_tc(const uint16_t* gys_bf16, int32_t grad_mod
   pl.p.ws = static_cast<float*>(workspace);
   pl.p.trace = get_tc_trace();
   CUtensorMap tmX, tmG;
-  if (pl.p.halo)
-    rc = make_act_map(&tmX, xb_bf16, s->N, s->H, s->W, s->Cin, 64, pl.p.PW, pl.p.PH, 1, 1);
-  else
-    rc = make_act_map(&tmX, xb_bf16, s->N, s->H, s->W, s->Cin, pl.p.UW, pl.p.BW, pl.p.BH, pl.p.BNI, s->stride);
+  rc = make_act_map(&tmX, xb_bf16, s->N, s->H, s->W, s->Cin, pl.p.UW, pl.p.BW, pl.p.BH, pl.p.BNI, s->stride);
   if (rc) return rc;
   rc = make_act_map(&tmG, gys_bf16, s->N, s->Ho, s->Wo, s->Cout * grad_halves, pl.p.BN < 64 ? pl.p.BN : 64, pl.p.BW,
                     pl.p.BH, pl.p.BNI);
   if (rc) return rc;
-  BDBNN_CUDA(cudaFuncSetAttribute(tc_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(pl.smem)));
-  dim3 grid(unsigned(pl.ksplit), unsigned(pl.mgroups), unsigned(pl.ntiles));
-  tc_wgrad_kernel<<<grid, kTcThreads, pl.smem, st>>>(tmX, tmG, pl.p);
-  rc = check_launch("tc_wgrad_kernel");
+  rc = launch_wgrad_kernel(tmX, tmG, pl.p, pl.smem, dim3(unsigned(pl.ksplit), unsigned(pl.mgroups), unsigned(pl.ntiles)),
+                           st);
   if (rc) return rc;
   const int64_t n = int64_t(s->Cout) * s->Cin * s->kh * s->kw;
   int64_t blocks = (n + 255) / 256;

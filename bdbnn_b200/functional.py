@@ -139,7 +139,7 @@ def _p(t):
 def _require_cuda(t, what):
     if not t.is_cuda:
         raise RuntimeError(f"bdbnn_b200.{what}: expected a CUDA tensor, got device={t.device}. "
-                           "The B200 path has no CPU fallback (use oracle/ for CPU checking).")
+                           "The CUDA path has no CPU fallback (use oracle/ for CPU checking).")
     if t.dtype != torch.float32:
         raise RuntimeError(f"bdbnn_b200.{what}: expected float32, got {t.dtype}")
 
@@ -167,7 +167,7 @@ def resolve_impl(impl, shape):
         raise ValueError(f"impl must be one of {_VALID_IMPL}, got {impl!r}")
     caps = int(_lib.lib().bdbnn_tc_supported(ctypes.byref(shape)))
     if impl == "tc" and not (caps & 1):
-        raise RuntimeError("bdbnn_b200: impl='tc' requested but the tcgen05 path does not support this shape")
+        raise RuntimeError("bdbnn_b200: impl='tc' requested but the wgmma path does not support this shape")
     return caps if (impl in ("auto", "tc") and (caps & 1)) else 0
 
 
@@ -296,7 +296,7 @@ class _BinConv2d(torch.autograd.Function):
                                                         ctypes.byref(sh), st), "binconv_dgrad_tc")
                 _lib.count(_dgrad_launches(sh))
             if need_w and not (ctx.use & 4):
-                # wgrad on CUDA cores from the saved sign bits (tcgen05 wgrad not available for this shape)
+                # wgrad on CUDA cores from the saved sign bits (wgmma wgrad not available for this shape)
                 gw = torch.empty(ctx.w_shape, dtype=torch.float32, device=dev)
                 with _timed("binconv_wgrad_generic", key, algorithmic_bytes("wgrad", sh)):
                     _lib.check(L.bdbnn_binconv_wgrad(_p(g), _p(sign_bits), _p(wmask), _p(gw),
@@ -800,7 +800,7 @@ def _side_launch(param, keep):
 
 
 def unit_supported(x_shape, w_shape, stride, padding):
-    """The fused unit needs all three tcgen05 kernels for the conv shape."""
+    """The fused unit needs all three wgmma kernels for the conv shape."""
     sh = conv_shape(x_shape, w_shape, stride, padding)
     return (int(_lib.lib().bdbnn_tc_supported(ctypes.byref(sh))) & 7) == 7
 
@@ -1097,7 +1097,7 @@ def shortcut_tc_enabled():
 
 
 def shortcut_supported(x, weight, stride):
-    """fp32 1x1 shortcut conv + BN on the tcgen05 kernels: CUDA fp32 NHWC-able x, [Cout,Cin,1,1] weight,
+    """fp32 1x1 shortcut conv + BN on the wgmma kernels: CUDA fp32 NHWC-able x, [Cout,Cin,1,1] weight,
     fp16s gradient mode (the operands are fp16), and all three kernels available for the 1x1 geometry."""
     if not (x.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and weight.dim() == 4):
         return False
@@ -1228,7 +1228,7 @@ class _RealConvBN(torch.autograd.Function):
 
 
 def shortcut_conv_bn(x, weight, gamma, beta, running_mean, running_var, momentum, eps, stride):
-    """BN_train(conv2d(x, weight[Cout,Cin,1,1], stride)) on the tcgen05 kernels (see shortcut_supported)."""
+    """BN_train(conv2d(x, weight[Cout,Cin,1,1], stride)) on the wgmma kernels (see shortcut_supported)."""
     return _RealConvBN.apply(x, weight, gamma, beta, running_mean, running_var, momentum, eps, int(stride))
 
 
@@ -1333,7 +1333,7 @@ def stem_tc_enabled():
 
 
 def stem_conv_supported(x, weight, stride, padding):
-    """tcgen05 stem: fp32 CUDA [N,3,H,W] (dense NCHW or channels_last) x [64,3,7,7], stride 2, pad 3,
+    """wgmma stem: fp32 CUDA [N,3,H,W] (dense NCHW or channels_last) x [64,3,7,7], stride 2, pad 3,
     output width <= 128, and no gradient w.r.t. the images."""
     if not (x.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and x.shape[1] == 3):
         return False
@@ -1400,8 +1400,8 @@ def _stem_wgrad_impl(gys, g_amax, xw, x_amax, n, h, w, w_param=None):
 
 class _StemConv(torch.autograd.Function):
     """y = conv2d(x, W, stride 2, pad 3) for the 3 -> 64 channel 7x7 stem (csrc/stem.cu).
-    forward : stem_pack (amax, fp16 window image, fp16 weights) -> stem_conv_fwd (tcgen05, 7-tap implicit GEMM)
-    backward: grad_pack (fp16 x 2^e) -> stem_conv_wgrad (tcgen05, split-K) ; no input gradient."""
+    forward : stem_pack (amax, fp16 window image, fp16 weights) -> stem_conv_fwd (wgmma, 7-tap implicit GEMM)
+    backward: grad_pack (fp16 x 2^e) -> stem_conv_wgrad (wgmma, split-K) ; no input gradient."""
 
     @staticmethod
     @_on_device
@@ -1474,7 +1474,7 @@ def stem_conv_bn_pool(x, weight, gamma, beta, running_mean, running_var, momentu
 
 
 def stem_conv(x, weight):
-    """7x7 / stride-2 / pad-3 stem convolution on tcgen05 (see stem_conv_supported)."""
+    """7x7 / stride-2 / pad-3 stem convolution on wgmma (see stem_conv_supported)."""
     _require_cuda(x, "stem_conv(x)")
     _require_cuda(weight, "stem_conv(weight)")
     return _StemConv.apply(x, weight)

@@ -220,7 +220,13 @@ class ResNetCifar(nn.Module):
     def forward(self, x):
         packed = _prepack(self, x)
         try:
-            x = self.bn1(self.conv1(x))
+            # fp32 stem on cuDNN: TF32 off, or cuDNN may pick a TF32 algorithm for some batch sizes (on the H100 at
+            # batch 8 but not 16), and the binary layers behind it amplify that 1e-3 difference into different signs
+            cudnn = torch.backends.cudnn
+            with cudnn.flags(enabled=cudnn.enabled, benchmark=cudnn.benchmark, deterministic=cudnn.deterministic,
+                             allow_tf32=False):
+                x = self.conv1(x)
+            x = self.bn1(x)
             x = self.layer3(self.layer2(self.layer1(x)))
         finally:
             if packed:

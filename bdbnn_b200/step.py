@@ -305,7 +305,7 @@ class GraphedTrainStep:
         opt.enable_graph_mode()
         cur = torch.cuda.current_stream()
         # the capture stream, by default above the second stream's priority: where both have blocks pending, the
-        # chain the step waits for goes first (BDBNN_GRAPH_PRIO=0: 8.80 ms, -1: 8.73 ms per ResNet-18 step)
+        # chain the step waits for goes first (BDBNN_GRAPH_PRIO=0: equal priorities)
         side = torch.cuda.Stream(priority=int(os.environ.get("BDBNN_GRAPH_PRIO", "-1")))
         side.wait_stream(cur)
         with torch.cuda.stream(side):

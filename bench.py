@@ -1,9 +1,10 @@
 #!/usr/bin/env python
-"""bench.py — ResNet-18 1W/1A training throughput (images/sec) on N B200s of one node.
+"""bench.py — ResNet-18 1W/1A training throughput (images/sec) on N H100s of one node.
 
     python bench.py --gpus 1 --steps 20 --warmup 5            # this repo (CUDA kernels)
     torchrun ... bench.py --gpus N --steps K --warmup W       # one rank per GPU, NCCL
     python bench.py --impl reference ...                      # reference arm: the CPU oracle step
+    python bench.py --gpus 1 --steps 20 --warmup 5 --dump-outputs DIR   # + the last timed step's outputs as .npy
 
 A "step" = one full optimisation step of the restated train.py body (bdbnn_b200.step.TrainStep:
 forward, losses, backward, gradient all-reduce, optimizer) on one synthetic batch.  Workload at N=1 is
@@ -14,6 +15,11 @@ step fed from pinned host memory (H2D copy of every batch + D2H read of the loss
 region); `roofline` = achieved algorithmic GB/s of the dominant CUDA kernel family measured with CUDA
 events on the launching stream inside the timed region; `cpu_baseline` = the CPU oracle step timed on
 this box's host cores on a bounded sample.
+
+--dump-outputs DIR writes what the last timed step computed (rank 0): the loss terms, the logits, and the
+updated parameters (`param.<name>.npy`), float32, at most 64 MB in all (a parameter too large for its share is
+replaced by a fixed, seeded sample of its entries).  Model weights and batch are seeded, so two builds run with
+the same arguments can be compared output for output.
 """
 import argparse
 import gc
@@ -54,35 +60,11 @@ def parse():
     ap.add_argument("--no-secondary", action="store_true", help="skip the bf16x2 gradient-mode secondary value")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's outputs to DIR/<name>.npy (float32, <= 64 MB in all)")
     ap.add_argument("--profile-mode", action="store_true",
                     help="for runs under ncu: 1 warm-up step, no e2e / cpu legs (numbers printed are not bench values)")
     return ap.parse_args()
-
-
-TRAFFIC_KERNEL = {  # KernelTimer family -> kernel-name prefixes in profiles/*_dram_traffic.json (ncu --set full)
-    "binconv_dgrad_tc": ("tc_conv2_kernel<1", "tc_conv64_kernel<1"),
-    "binconv_fwd_tc": ("tc_conv2_kernel<0", "tc_conv64_kernel<0, 0, 1, 0"),
-    "binconv_fwd_tc8": ("tc_conv2_kernel<0",), "binconv_wgrad_tc": ("tc_wgrad_kernel",),
-    "bn_fwd": ("bn_apply_add_pack_kernel<1",), "bn_bwd_pack": ("bn_bwd_pack_kernel<3",),
-}
-
-
-def ncu_traffic(family, calls_per_step):
-    """dram__bytes_read+write of the family's kernels over ONE step of the newest committed ncu capture, divided by
-    the family's API calls per step (a stride-2 dgrad is four phase launches; the three 1x1 shortcut dgrads run the
-    same kernel and are included, so the figure is an upper bound for the family)."""
-    import glob
-    import re
-    nat = lambda f: [int(t) if t.isdigit() else t for t in re.split(r"(\d+)", os.path.basename(f))]
-    files = sorted((f for f in glob.glob(os.path.join(ROOT, "profiles", "*_dram_traffic.json")) if "losses" not in f),
-                   key=nat)                                                     # r1_step9 < r1_step10 < r2_final
-    if not files or family not in TRAFFIC_KERNEL or not calls_per_step:
-        return None, None
-    with open(files[-1]) as fh:
-        d = json.load(fh)
-    tot = sum(e["launches"] * e["dram_bytes_per_launch"] for k, e in d.items()
-              if any(k.startswith(pre) for pre in TRAFFIC_KERNEL[family]))
-    return (round(tot / calls_per_step), os.path.basename(files[-1])) if tot else (None, None)
 
 
 def peaks():
@@ -91,7 +73,7 @@ def peaks():
         with open(p) as fh:
             d = json.load(fh)
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 class ClockSampler:
@@ -276,6 +258,7 @@ def eager_gpu_run(args, steps, warmup, batch, dev):
     torch.optim, cudnn.benchmark=True as train.py:368.  None of this repo's kernels run on this path."""
     from oracle import step_ref as S
     torch.backends.cudnn.benchmark = True
+    torch.backends.cudnn.deterministic = False       # cuDNN defaults otherwise (the timed path turns it on)
     torch.manual_seed(0)
     ishape, ncls, dataset = shapes(args.model, batch)
     model = build_model(args.model, ref=True).to(dev).to(memory_format=torch.channels_last)
@@ -314,6 +297,29 @@ def finish(world):
         os._exit(0)
 
 
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(path, out, model):
+    """DIR/<name>.npy (float32) of the step's tensor outputs and the updated parameters, <= DUMP_BYTES in all."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    arrays = {k: v for k, v in out.items() if torch.is_tensor(v)}
+    arrays.update({f"param.{n}": p for n, p in model.named_parameters()})
+    arrays = {k: v.detach().float().reshape(-1).cpu().numpy() if v.dim() else v.detach().float().reshape(1).cpu().numpy()
+              for k, v in arrays.items()}
+    total = sum(a.size for a in arrays.values()) * 4
+    if total > DUMP_BYTES:
+        # shrink every array above its fair share to a fixed seeded sample of its entries
+        share = DUMP_BYTES // 4 // len(arrays)
+        rng = np.random.default_rng(0)
+        for k, a in arrays.items():
+            if a.size > share:
+                arrays[k] = a[np.sort(rng.choice(a.size, share, replace=False))]
+    for k, a in arrays.items():
+        np.save(os.path.join(path, f"{k}.npy"), a.astype(np.float32))
+
+
 def main():
     args = parse()
     rank = int(os.environ.get("RANK", "0"))
@@ -348,7 +354,7 @@ def main():
         return
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device; the B200 path has no CPU fallback "
+        raise SystemExit("bench.py: no CUDA device; the CUDA path has no CPU fallback "
                          "(use --impl reference for the CPU arm)")
     if args.impl == "reference-gpu":
         if rank != 0:
@@ -379,7 +385,11 @@ def main():
         if os.environ.get("NCCL_DEBUG", "").upper() == "VERSION":
             os.environ["NCCL_DEBUG"] = "WARN"
         dist.init_process_group("nccl", device_id=dev)
-    torch.backends.cudnn.benchmark = True            # train.py:368
+    # train.py:368 turns cuDNN autotuning on; here it stays off: autotuning picks convolution algorithms by timing,
+    # so two runs could compute the cuDNN layers (the fp32 teacher, the ResNet-20 stem) with different algorithms
+    # and different rounding.  With the same arguments every run computes the same outputs.
+    torch.backends.cudnn.benchmark = False
+    torch.backends.cudnn.deterministic = True
     torch.manual_seed(0)
     ishape, ncls, dataset = shapes(args.model, batch)
     # parameters stay in their native dense (OIHW) layout: the kernels of this repo read and write weights and
@@ -467,12 +477,15 @@ def main():
     gc.disable()                 # a generation-2 collection inside the loop stalls the launch thread for tens of ms
     sampler.mark_begin()
     e0.record()
+    out = None
     for _ in range(args.steps):
-        step(x_dev, y_dev)
+        out = step(x_dev, y_dev)
     e1.record()
     barrier()
     sampler.mark_end()
     gc.enable()
+    if args.dump_outputs and rank == 0 and out is not None:
+        dump_outputs(args.dump_outputs, out, model)
     if args.profile_mode:
         torch.cuda.profiler.stop()
     ms_total = max_over_ranks(e0.elapsed_time(e1))
@@ -506,7 +519,7 @@ def main():
         ready = [torch.cuda.Event(), torch.cuda.Event()]
         consumed = [torch.cuda.Event(), torch.cuda.Event()]
 
-        diag = os.environ.get("BDBNN_E2E_DIAG", "")      # attribution runs only (scripts/): "noh2d", "nod2d"
+        diag = os.environ.get("BDBNN_E2E_DIAG", "")      # attribution runs only: "noh2d", "nod2d"
 
         def prefetch(i):
             b = i % 2
@@ -629,10 +642,8 @@ def main():
     timed = [k for k in kernels if k["achieved_gbs"]]       # families with algorithmic bytes (not the cuDNN teacher)
     if timed:
         top = timed[0]
-        traffic, traffic_src = ncu_traffic(top["kernel"], top["launches_per_step"])
         roofline = {"bound": "hbm", "kernel": top["kernel"], "achieved": top["achieved_gbs"], "peak": peak,
-                    "unit": "GB/s", "frac": round(top["achieved_gbs"] / peak, 4), "traffic": traffic,
-                    "traffic_source": traffic_src,
+                    "unit": "GB/s", "frac": round(top["achieved_gbs"] / peak, 4),
                     "peak_source": peak_src,
                     "how": "sum of per-launch algorithmic bytes (DESIGN.md §4) / sum of CUDA-event durations "
                            "of that kernel family over " + ("the timed region" if not use_graph else
@@ -663,7 +674,7 @@ def main():
                        else "SGD (train.py:319-321)", "conv_impl": args.conv_impl or "auto", "grad_mode": gname,
                        "launch": "CUDA graph replay (whole step captured once)" if use_graph else
                                  (graph_note or "eager (Python/ctypes per kernel)"),
-                       "l2_policy": "per-step working set (>3 GB of activations) exceeds the 126 MB L2; no flush"},
+                       "l2_policy": "per-step working set (>3 GB of activations) exceeds the 50 MB L2; no flush"},
             "clocks": clocks, "e2e": e2e, "gpu_launches": launches, "roofline": roofline,
             "kernels": kernels, "cpu_baseline": cpu, "eager_gpu": eager, "secondary": secondary}
     print(json.dumps(line))

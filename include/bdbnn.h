@@ -1,5 +1,5 @@
 /*
- * bdbnn.h — C ABI of libbdbnn_b200.so (sm_100a).
+ * bdbnn.h — C ABI of libbdbnn_b200.so (sm_90a).
  *
  * The reference (BlueAnon/BD-BNN) ships no native code: its hot path is Python calling
  * ATen/cuDNN.  Each entry point below therefore replaces a *Python* call site of the reference
@@ -13,7 +13,9 @@
  *   - bit tensors are uint32 words; bit j of word k covers channel 32*k+j (LSB first);
  *     bit value 1 encodes +1 (x >= 0), bit value 0 encodes -1 (x < 0); channel padding bits are 0;
  *   - stream is a cudaStream_t passed as void*; all work is enqueued on it, nothing synchronises;
- *   - the library never allocates device memory: the caller owns every buffer incl. workspaces;
+ *   - the caller owns every buffer incl. workspaces; the only device memory the library allocates is the
+ *     scratch of its cross-block reductions (per-block partials summed in a fixed order, so results are
+ *     the same in every run), stream-ordered (cudaMallocAsync / cudaFreeAsync on `stream`, capturable);
  *   - return value 0 = ok, negative = error (bdbnn_last_error_string() describes the last one on
  *     the calling thread).  Nothing throws across the ABI.
  */
@@ -59,10 +61,11 @@ typedef struct bdbnn_conv_shape {
 BDBNN_API int bdbnn_version(void);
 /* Thread-local description of the last error returned on this thread ("" if none). */
 BDBNN_API const char* bdbnn_last_error_string(void);
-/* Developer aid: when device_buf != NULL (3*2048 int64), CTA 0 of the persistent conv kernel records
- * (event id, clock64) pairs per warp role into it (scripts/trace_tc.py decodes). NULL disables. */
+/* Developer aid: when device_buf != NULL (3*2048 int64), CTA (0,0,0) of the weight-gradient kernel records
+ * (event id, clock64) pairs of its TMA producer warp (row 0: ring-slot wait begin / end) into it.  NULL
+ * disables. */
 BDBNN_API int bdbnn_debug_trace(long long* device_buf);
-/* Which tcgen05/TMA implicit-GEMM kernels can serve this shape: bitmask
+/* Which wgmma/TMA implicit-GEMM kernels can serve this shape: bitmask
  * BDBNN_TC_FWD | BDBNN_TC_DGRAD | BDBNN_TC_WGRAD (0 = none: the CUDA-core kernels do all three). */
 #define BDBNN_TC_FWD 1
 #define BDBNN_TC_DGRAD 2
@@ -119,7 +122,7 @@ BDBNN_API int bdbnn_ede_scale(float* g, const float* v, const float* k, const fl
 BDBNN_API int bdbnn_binconv_fwd_xnor(const uint32_t* sign_bits, const uint32_t* wsign_bits,
                            const float* alpha, float* y, const bdbnn_conv_shape* s, void* stream);
 
-/* ---- binary conv forward, tcgen05 implicit GEMM on +-1 bf16 operands (exact, fp32 accumulate) --
+/* ---- binary conv forward, wgmma implicit GEMM on +-1 bf16 operands (exact, fp32 accumulate) --
  * Same result as bdbnn_binconv_fwd_xnor.  Requires bdbnn_tc_supported(s).
  * bn_sums / bn_ymax (both or neither; also on fwd_tc8 and stem_conv_fwd): if non-NULL the kernel's
  * epilogue also accumulates the BatchNorm batch statistics of y — bn_sums = double[2*Cout] (sum y, then
@@ -139,7 +142,7 @@ BDBNN_API int bdbnn_binconv_fwd_tc8(const uint8_t* xb_fp8, const uint8_t* wf_fp8
  * fused BatchNorm units (bdbnn_bn_fwd_i16 / bdbnn_bn_bwd_pack_i16) read once in the forward and twice in the
  * backward.  fmt = BDBNN_FMT_FP16 / BDBNN_FMT_BF16 (16-bit +-1 operands) or -1 (fp8 e4m3 operands, needs
  * BDBNN_TC_FWD8).  The statistics (bn_sums / bn_ymax) are those of y = alpha * y_int, as in fwd_tc.
- * Requires bdbnn_tc_supported(s) & BDBNN_TC_FWD_I16 (persistent kernel only). */
+ * Requires bdbnn_tc_supported(s) & BDBNN_TC_FWD_I16 (GEMMs eligible in bdbnn_debug_conv_plan only). */
 BDBNN_API int bdbnn_binconv_fwd_tc_i16(const void* xb, const void* wf, int32_t fmt, const float* alpha,
                              int16_t* y_int, const bdbnn_conv_shape* s, double* bn_sums, uint32_t* bn_ymax,
                              void* stream);
@@ -159,7 +162,7 @@ BDBNN_API int bdbnn_binconv_dgrad(const float* gy, const uint32_t* wsign_bits, c
 BDBNN_API int bdbnn_binconv_wgrad(const float* gy, const uint32_t* sign_bits, const uint32_t* wmask_bits,
                         float* gW, const bdbnn_conv_shape* s, void* stream);
 
-/* ---- backward on tensor cores (tcgen05, 16-bit operands, fp32 accumulate) -----------------------
+/* ---- backward on tensor cores (wgmma, 16-bit operands, fp32 accumulate) -----------------------
  * grad_pack: v = gy[p*Cout+o] * gscale[o], written per `mode` (BDBNN_GRAD_*):
  *              BF16   gys[p*Cout+o]             = bf16_rn(v)
  *              BF16X2 gys[p*2Cout+o] = hi = bf16_rn(v), gys[p*2Cout+Cout+o] = bf16_rn(v - hi)
@@ -180,10 +183,10 @@ BDBNN_API int bdbnn_binconv_dgrad_tc(const uint16_t* gys, int32_t grad_mode, con
                            const uint16_t* wt, const uint32_t* mask_bits, const float* add, float* gx,
                            const bdbnn_conv_shape* s, void* stream);
 BDBNN_API size_t bdbnn_wgrad_tc_workspace_bytes(const bdbnn_conv_shape* s);
-/* Host-only: the persistent forward/dgrad kernel's tiling for a shape (mode 0 = forward, 1 = first dgrad
- * phase, 2 = fp8 forward).  out[12] = {planned (0 = one-tile kernel), halo mode, M tiles per super tile,
- * TMEM buffers, N tile, N tiles, super tiles, ring stages, dynamic smem bytes, grid, stage bytes, patch
- * bytes}.  Makes no CUDA call. */
+/* Host-only: the forward/dgrad kernel's tiling for a shape (mode 0 = forward, 1 = first dgrad phase,
+ * 2 = fp8 forward).  out[12] = {planned (0 = not eligible for the int16 result / fused dgrad statistics),
+ * halo mode (0), M tiles per CTA (1), accumulator buffers (1), N tile, N tiles, M tiles, ring stages,
+ * dynamic smem bytes, grid, stage bytes, patch bytes (0)}.  Makes no CUDA call. */
 BDBNN_API int bdbnn_debug_conv_plan(const bdbnn_conv_shape* s, int32_t mode, int32_t grad_halves, int32_t* out,
                           int32_t n_out);
 /* Host-only: the tiling bdbnn_binconv_wgrad_tc would use, for tests.  out[12] = {supported, ksplit, ks_cap,
@@ -273,7 +276,7 @@ BDBNN_API int bdbnn_bn_bwd_pack_i16(const float* gz, const int16_t* y_int, const
 /* bdbnn_bn_bwd_pack_i16(stats_ready = 1): sums_ws (sum gz | sum gz*yhat) and gmax_bits were already accumulated by
  * the kernel that PRODUCED gz — bdbnn_binconv_dgrad_tc_stats, the data-gradient kernel of the next unit, whose
  * result (dgrad + shortcut gradient) is this unit's gz: the separate reduction pass over gz and y is skipped.
- * dgrad_tc_stats = bdbnn_binconv_dgrad_tc (stride 1, persistent kernel, Cin <= 512) + those statistics of the
+ * dgrad_tc_stats = bdbnn_binconv_dgrad_tc (stride 1, eligible GEMMs, Cin <= 512) + those statistics of the
  * producing unit: prod_y_int int16 [N,H,W,Cin], prod_alpha / prod_mean / prod_invstd float[Cin];
  * prod_sums double[2*Cin] and prod_gmax u32[Cin] are zeroed here. */
 BDBNN_API int bdbnn_binconv_dgrad_tc_stats(const uint16_t* gys_bf16, int32_t grad_mode, const uint32_t* amax_bits,
@@ -316,7 +319,7 @@ BDBNN_API int bdbnn_maxpool_bwd(const float* gy, const uint8_t* idx, float* gx, 
                       int32_t W, int32_t C, int32_t k, int32_t stride, int32_t pad, int32_t Ho, int32_t Wo,
                       void* stream);
 
-/* ---- stem convolution: 7x7 / stride 2 / pad 3, 3 -> 64 channels, fp32 in / fp32 out, on tcgen05 ------
+/* ---- stem convolution: 7x7 / stride 2 / pad 3, 3 -> 64 channels, fp32 in / fp32 out, on wgmma --------
  * Replaces the fp32 nn.Conv2d `conv1` of the torchvision-style ResNet the reference trains
  * (model(images), train.py:492,602; its weight gradient under loss.backward(), train.py:528,650), which
  * cuDNN runs on TF32 tensor cores.  Operands here are fp16 after a per-call power-of-two scale
@@ -383,7 +386,7 @@ BDBNN_API int bdbnn_optim_sgd_multi_graph(float* const* params_host, const float
                                 const float* weight_decay_host, int32_t count, float momentum,
                                 const float* lr_dev, float grad_scale, void* stream);
 
-/* ---- fp32 1x1 shortcut convolution (`downsample` of the ResNet shells) on the tcgen05 kernels -----------
+/* ---- fp32 1x1 shortcut convolution (`downsample` of the ResNet shells) on the wgmma kernels -------------
  * Packing only (bdbnn_b200/csrc/real_conv.cu): xh = fp16(x[:, ::stride, ::stride, :] * 2^ex) dense NHWC
  * [N,Ho,Wo,Cin], wf = fp16(W * 2^ew) [Cout][Cin], wt = its transpose [Cin][Cout], and the scale vectors
  * alpha[o] = 2^-ew 2^-ex, gscale[o] = 2^-ew, inv_gscale[o] = 2^ew 2^-ex.  The convolution itself is

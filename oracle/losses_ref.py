@@ -1,7 +1,7 @@
 """ORACLE (test infrastructure, NOT product code) — CPU restatement of the reference loss terms.
 
-PINNED: checked against the reference's own code executed in the build container
-(tests/golden/make_golden.py imports /root/reference/kurtosis.py and utils/KD_loss.py and stores
+PINNED: checked against the reference's own code
+(tests/golden/make_golden.py imports the reference's kurtosis.py and utils/KD_loss.py and stores
 inputs + outputs under tests/golden/*.pt; tests/test_oracle_golden.py replays them).
 
   kurtosis_ref          <- KurtosisWeight.kurtosis_calc           kurtosis.py:23-39

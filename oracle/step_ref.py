@@ -6,10 +6,9 @@ loops, restated WITHOUT any product import:
     ref_train_step         <- train.py:457-529   (`train`)  and  train.py:573-651 (`train_teacher_student`)
 
 PINNED: tests/test_ref_train.py executes the reference's own `train()` / `train_teacher_student()`
-(imported unmodified from /root/reference/train.py by tests/ref_launcher.py, build container only) on the
+(imported unmodified from the reference's train.py by tests/ref_launcher.py when the fixtures are made) on the
 same model, batch and optimizer and requires the same loss terms, gradients and updated parameters; the
-fixtures that script stored (tests/golden/train_step_*.pt) replay the comparison where the reference is
-not mounted (the GPU box).
+fixtures that script stored (tests/golden/train_step_*.pt) replay the comparison.
 
 The reference's loop cannot run as shipped (SURVEY.md §0.3): `args.w_l2_reg`, `args.w_wr_reg` and (without
 --react) `args.w_lambda_ce` are read but never defined, and `args.w_kurtosis_target` is re-wrapped in a

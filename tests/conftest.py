@@ -10,7 +10,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box via gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -1,11 +1,11 @@
-"""Generate golden fixtures by running the REFERENCE's own code (only possible in the build
-container, where /root/reference is mounted).  Output: tests/golden/*.pt (committed, small).
+"""Generate golden fixtures by running the REFERENCE's own code (needs a checkout of the reference,
+named by BDBNN_REFERENCE_ROOT).  Output: tests/golden/*.pt (committed, small).
 
-    python tests/golden/make_golden.py
+    BDBNN_REFERENCE_ROOT=<reference checkout> python tests/golden/make_golden.py
 
 Reference entry points executed:
-  /root/reference/kurtosis.py            KurtosisWeight(...).fn_regularization()
-  /root/reference/utils/KD_loss.py       DistributionLoss()(s, t); DistributionLoss_layer()(...)
+  kurtosis.py            KurtosisWeight(...).fn_regularization()
+  utils/KD_loss.py       DistributionLoss()(s, t); DistributionLoss_layer()(...)
 KD_loss.py imports `models.imagenet...HardBinaryConv*` (absent upstream, SURVEY.md §0.1); stub modules
 exposing empty nn.Module subclasses of those names are installed in sys.modules for the import only.
 """
@@ -17,7 +17,7 @@ import types
 import torch
 import torch.nn as nn
 
-REF = "/root/reference"
+REF = os.environ.get("BDBNN_REFERENCE_ROOT", "")
 OUT = os.path.dirname(os.path.abspath(__file__))
 
 

@@ -1,14 +1,16 @@
 """Generate whole-step golden fixtures by executing the REFERENCE's own `train()` and
-`train_teacher_student()` (/root/reference/train.py:441-554, 556-675), imported unmodified through
+`train_teacher_student()` (the reference's train.py:441-554, 556-675), imported unmodified through
 tests/ref_launcher.py in "reference" mode: train.py, kurtosis.py, utils/utils.py and utils/KD_loss.py are
 the reference's files; only the `models` package (absent upstream) and the network under test (oracle
-modules, CPU) come from this repo.  Build container only.
+modules, CPU) come from this repo.  Needs a checkout of the reference (BDBNN_REFERENCE_ROOT).
 
-    python tests/golden/make_train_golden.py        ->  tests/golden/train_step_<case>.pt
+    BDBNN_REFERENCE_ROOT=<reference checkout> python tests/golden/make_train_golden.py
+        ->  tests/golden/train_step_<case>.pt
 
-Per case: the batch, the initial state (small nets) or its checksum (ResNet-18, regenerated from the
-seed), every value the loop fed to its AverageMeters (loss, CE, kurtosis, KL terms, top-1/5), every
-parameter gradient and every updated parameter (tensors for the small nets, summaries for ResNet-18)."""
+Per case: checksums of the batch and of the initial student / teacher states (all regenerated from the
+seeds of tests/train_cases.py by the tests), every value the loop fed to its AverageMeters (loss, CE,
+kurtosis, KL terms, top-1/5), every parameter gradient, every updated parameter and buffer (tensors for
+the small nets, summaries for ResNet-18)."""
 import os
 import sys
 
@@ -58,12 +60,13 @@ def run_case(case):
     after = {n: p.detach().clone() for n, p in stud.named_parameters()}
     buffers = {n: b.detach().clone() for n, b in stud.named_buffers()}
     rec = {"case": case, "config": c, "x_checksum": float(x.double().sum()), "y": y, "meters": log, "scalars": out["scalars"],
-           "hooked": list(out["hooked"].keys()), "sources": train.__bdbnn_sources__,
-           "init_checksum": TC.state_checksum_from(init), "torch": torch.__version__}
+           "hooked": list(out["hooked"].keys()), "init_checksum": TC.state_checksum_from(init), "torch": torch.__version__}
+    if t_state is not None:
+        rec["teacher_checksum"] = TC.state_checksum_from(t_state)
     if case in TC.SUMMARY_ONLY:
         rec.update(grads=TC.summarize(grads), after=TC.summarize(after), buffers=TC.summarize(buffers))
     else:
-        rec.update(x=x, init=init, teacher_state=t_state, grads=grads, after=after, buffers=buffers)
+        rec.update(grads=grads, after=after, buffers=buffers)
     torch.save(rec, os.path.join(os.environ.get("BDBNN_GOLDEN_OUT", HERE), f"train_step_{case}.pt"))
     print(case, {k: v for k, v in log.items() if k not in ("Time", "Data")}, out["scalars"])
 

@@ -4,7 +4,8 @@
     train = RL.import_reference_train(mode="dropin" | "reference")
     out = RL.run_reference_loop(train, model, optimizer, batches, args, teacher=None)
 
-`/root/reference/train.py` is imported as it is (never copied, never edited).  What it needs and the
+The reference's `train.py` (a checkout named by BDBNN_REFERENCE_ROOT) is imported as it is (never copied, never
+edited).  What it needs and the
 snapshot lacks is supplied from outside, exactly as SURVEY.md §0.3 / INTEGRATION.md §2 prescribe:
   * `tensorboardX`, `matplotlib` — stub modules in sys.modules when the real ones are not installed
     (train.py:23,38-40; logging only);
@@ -15,10 +16,10 @@ snapshot lacks is supplied from outside, exactly as SURVEY.md §0.3 / INTEGRATIO
   * the three `args` fields train.py reads but never defines (B1/B2): w_l2_reg, w_wr_reg = False,
     w_lambda_ce = 1.0;
   * the module globals `writer` / `msglogger` that main_worker() would have set (train.py:158-168).
-On a machine without CUDA (the build container) `Tensor.cuda()` / `Module.cuda()` are patched to
+On a machine without CUDA `Tensor.cuda()` / `Module.cuda()` are patched to
 identity for the duration of the call so that train.py:487-491 runs on the CPU; nothing else is touched.
 
-Test infrastructure: only tests/ and tests/golden/make_train_golden.py import this."""
+Fixture tooling: only tests/golden/make_train_golden.py imports this."""
 import contextlib
 import importlib
 import logging
@@ -28,13 +29,13 @@ import types
 
 import torch
 
-REF_ROOT = os.environ.get("BDBNN_REFERENCE_ROOT", "/root/reference")
+REF_ROOT = os.environ.get("BDBNN_REFERENCE_ROOT", "")
 REPO_ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 _SHADOWED = ("train", "kurtosis", "utils", "utils.utils", "utils.KD_loss", "loader")
 
 
 def reference_available():
-    return os.path.isfile(os.path.join(REF_ROOT, "train.py"))
+    return bool(REF_ROOT) and os.path.isfile(os.path.join(REF_ROOT, "train.py"))
 
 
 class ScalarWriter:
@@ -68,10 +69,10 @@ def _install_stubs():
 
 
 def import_reference_train(mode="dropin"):
-    """Import /root/reference/train.py as module `train` with the search order of `mode` and return it.
+    """Import the reference's train.py as module `train` with the search order of `mode` and return it.
     The module keeps `train.__bdbnn_mode__` and the resolved files in `train.__bdbnn_sources__`."""
     if not reference_available():
-        raise FileNotFoundError(f"{REF_ROOT}/train.py not found (the reference is only mounted in the build container)")
+        raise FileNotFoundError(f"reference train.py not found under BDBNN_REFERENCE_ROOT={REF_ROOT!r}")
     if mode not in ("dropin", "reference"):
         raise ValueError(mode)
     _install_stubs()

@@ -378,6 +378,6 @@ def test_ede_module_cifar_follows_assigned_k_t():
         y.backward(gy.cuda())
         yr.backward(gy)
         torch.testing.assert_close(y.detach().cpu(), yr.detach(), rtol=1e-5, atol=1e-6)
-        # 16/32-channel shapes run on the tcgen05 path: fp16s gradient operand -> 1.5e-3 of max|ref|
+        # 16/32-channel shapes run on the wgmma path: fp16s gradient operand -> 1.5e-3 of max|ref|
         for got, want in ((xd.grad.cpu(), xr.grad), (conv.weight.grad.cpu(), ref.weight.grad)):
             assert (got - want).abs().max().item() <= 1.5e-3 * want.abs().max().item()

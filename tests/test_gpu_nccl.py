@@ -90,7 +90,7 @@ def _single(outdir, init_flat):
     return torch.cat([p.grad.reshape(-1) for p in m.parameters()]).cpu()
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
 @pytest.mark.parametrize("use_shim", [True, False])
 def test_nccl_world2_grads_and_params_identical_and_match_single_process(tmp_path, use_shim):
     import torch.multiprocessing as mp

@@ -1,4 +1,4 @@
-"""GPU: tcgen05/TMA implicit-GEMM kernels vs the CUDA-core kernels and the CPU oracle."""
+"""GPU: wgmma/TMA implicit-GEMM kernels vs the CUDA-core kernels and the CPU oracle."""
 import ctypes
 
 import pytest
@@ -107,7 +107,7 @@ def test_tc_supported_rejects_unsupported_shapes():
     assert _caps((1, 64, 9, 9, 64, 3, 3, 1)) == 0       # stride 3
     assert _caps((1, 64, 8, 200, 64, 3, 1, 1)) == 0     # row wider than one tile
     from bdbnn_b200.functional import binconv2d
-    with pytest.raises(RuntimeError, match="tcgen05"):
+    with pytest.raises(RuntimeError, match="wgmma"):
         binconv2d(torch.randn(1, 40, 8, 8, device="cuda"), torch.randn(64, 40, 3, 3, device="cuda"), 1, 1, "tc")
 
 
@@ -274,7 +274,7 @@ def test_stem_bn_pool_fused_vs_torch(geom):
 @pytest.mark.parametrize("geom,layout", [((2, 32, 32), "nchw"), ((3, 33, 47), "nhwc"), ((5, 16, 16), "nchw"),
                                          ((2, 224, 224), "nhwc"), ((1, 64, 255), "nchw"), ((3, 150, 130), "nhwc")])
 def test_stem_conv_tc_vs_fp64_conv(geom, layout):
-    """7x7/2 stem conv on tcgen05 (fp16 operands with power-of-two scales = TF32-class significands, fp32
+    """7x7/2 stem conv on wgmma (fp16 operands with power-of-two scales = TF32-class significands, fp32
     accumulate) vs an fp64 convolution: forward and weight gradient within 2e-3 of max|ref|
     (cuDNN's TF32 stem, which the reference runs, has the same operand rounding)."""
     from bdbnn_b200 import functional as F_
@@ -304,7 +304,7 @@ def test_stem_conv_tc_vs_fp64_conv(geom, layout):
 
 
 def test_stem_conv_module_path_and_fallback(monkeypatch):
-    """ResNetImageNet._stem takes the tcgen05 stem by default and cuDNN with BDBNN_STEM_TC=0; both agree."""
+    """ResNetImageNet._stem takes the wgmma stem by default and cuDNN with BDBNN_STEM_TC=0; both agree."""
     from bdbnn_b200 import _lib
     from bdbnn_b200.resnet import resnet18
     torch.manual_seed(0)
@@ -372,7 +372,7 @@ def test_stem_fused_conv_bn_pool(geom):
 @pytest.mark.parametrize("geom", [(4, 64, 128, 16, 16, 2), (2, 64, 128, 56, 56, 2), (3, 128, 256, 28, 28, 2),
                                   (5, 256, 512, 14, 14, 2), (2, 64, 64, 9, 11, 1)])
 def test_shortcut_conv_bn_vs_fp64(geom):
-    """fp32 1x1 `downsample` conv + BN(train) on the tcgen05 kernels (fp16 operands with power-of-two scales,
+    """fp32 1x1 `downsample` conv + BN(train) on the wgmma kernels (fp16 operands with power-of-two scales,
     TF32-class like the cuDNN kernels the reference runs) vs conv2d + BatchNorm2d in fp64: output, running
     statistics and the gradients of x, W, gamma, beta."""
     import torch.nn as nn
@@ -492,7 +492,7 @@ def test_backward_tc_full_size_vs_fp64_conv_on_gpu(geom, mode, monkeypatch):
 
 
 @pytest.mark.parametrize("mode", ["fp16s", "bf16x2"])
-@pytest.mark.parametrize("geom", [(3, 64, 16, 16), (2, 128, 14, 14), (4, 256, 7, 7)])   # (64 ch on > 256-pixel images: pixel-N kernel, no fused sums)
+@pytest.mark.parametrize("geom", [(3, 64, 16, 16), (2, 128, 14, 14), (4, 256, 7, 7)])   # 64, 128 and 256 channels
 def test_bn_backward_sums_from_next_units_dgrad_epilogue(geom, mode, monkeypatch):
     """Two chained identity units (z1 = BN(conv(x)) + x; z2 = BN(conv(z1)) + z1): with BDBNN_BWD_STATS=1 the dgrad
     kernel of unit 2 accumulates unit 1's BatchNorm backward sums (sum gz1, sum gz1*yhat1, max|gz1|) in its epilogue

@@ -97,11 +97,11 @@ def test_capi_library_exports_every_declared_symbol():
     assert exported == set(syms), exported ^ set(syms)
 
 
-def test_library_is_sm100a():
+def test_library_is_sm90a():
     from bdbnn_b200 import build
     path = build.build()
     out = subprocess.run(["cuobjdump", "-lelf", path], capture_output=True, text=True).stdout
-    assert "sm_100a" in out, out[:400]
+    assert "sm_90a" in out, out[:400]
 
 
 def test_cpu_oracle_step_runs_and_learns():
@@ -264,8 +264,9 @@ def test_make_optimizer_cpu_is_plain_torch_and_fused_rejects_cpu():
 
 def test_wgrad_tiling_plans_are_sane_for_every_network_layer():
     """Host-only sweep of the wgrad planner (no GPU): every binary-conv geometry of the ResNet-18/34/20 shells,
-    both gradient operand widths — shared memory within the 227 KB CTA limit, one wave of CTAs, the
-    workspace large enough for the split the launch will use."""
+    both gradient operand widths — shared memory within the 227 KB CTA limit, at most three waves of CTAs on an H100
+    (132 SMs),
+    the accumulators within 128 registers per thread, the workspace large enough for the split the launch will use."""
     import ctypes
     from bdbnn_b200 import _lib
     from bdbnn_b200.functional import conv_shape
@@ -290,8 +291,8 @@ def test_wgrad_tiling_plans_are_sane_for_every_network_layer():
             ok, ksplit, ks_cap, mgroups, ntiles, smem, G, BN, UW, halo, k_stage, stages = list(out)
             assert ok == 1, (xs, ws, stride, halves)
             assert smem <= 227 * 1024 and stages >= 2 and k_stage % 16 == 0 and k_stage > 0
-            assert 1 <= ksplit <= ks_cap and ksplit * mgroups * ntiles <= 148           # one wave on a B200
-            assert UW in (16, 32, 64) and G * BN <= 512                                 # TMEM columns
+            assert 1 <= ksplit <= ks_cap and ksplit * mgroups * ntiles <= 3 * 132       # three waves on an H100
+            assert UW in (16, 32, 64) and G * BN <= 256 and halo == 0                   # accumulator registers
             assert need >= ksplit * ws[0] * ws[1] * ws[2] * ws[3] * 4, (xs, ws, halves, need, ksplit)
     # unsupported geometry is reported, not planned
     out = (ctypes.c_int32 * 12)()
@@ -300,8 +301,9 @@ def test_wgrad_tiling_plans_are_sane_for_every_network_layer():
 
 
 def test_conv_tiling_plans_are_sane_for_every_network_layer():
-    """Host-only sweep of the persistent forward / dgrad kernel's planner (no GPU): TMEM columns, shared memory
-    (dynamic + the kernel's static 6.5 KB of BN-statistics scratch in the forward) and ring depth."""
+    """Host-only sweep of the forward / dgrad kernel's planner (no GPU): one 128-row tile and one N tile of at most
+    128 columns (64 accumulator registers per thread) per CTA, a grid that covers every tile once, shared memory
+    (dynamic + the kernel's static BN-statistics scratch) and ring depth."""
     import ctypes
     from bdbnn_b200 import _lib
     from bdbnn_b200.functional import conv_shape
@@ -320,13 +322,15 @@ def test_conv_tiling_plans_are_sane_for_every_network_layer():
                     assert mode == 2 and cin % 128 != 0 or n == 2, (cin, cout, stride, mode)   # fp8 needs Cin % 128
                     continue
                 planned += 1
-                assert TS * BN * NB <= 512 and BN in (64, 128, 256) and NB in (1, 2)
-                assert stages >= 2 and 1 <= grid <= 148 and supers >= 1
-                static = 7 * 1024 if mode != 1 else 1024
+                assert TS == 1 and NB == 1 and halo == 0 and patch == 0 and BN in (64, 128)
+                assert stages >= 2 and supers >= 1 and grid == supers * n_tiles
+                assert stage_bytes % 1024 == 0 and smem >= stages * stage_bytes
+                # static: 8 consumer warps x 128 channels x (sum, sum of squares, max) floats + 2 x 8 ring barriers
+                static = 8 * 128 * 3 * 4 + 2 * 8 * 8
                 assert smem + static <= 227 * 1024, (cin, cout, stride, mode, smem)
                 assert BN * n_tiles == (cin if mode == 1 else cout)
     assert planned > 60
-    # 16/32-channel layers are served by the one-tile kernel: the probe says "not planned"
+    # 16/32-channel GEMMs take neither the int16 result nor the fused dgrad statistics: the probe says "not planned"
     out = (ctypes.c_int32 * 12)()
     sh = conv_shape((4, 16, 32, 32), (16, 16, 3, 3), 1, 1)
     assert L.bdbnn_debug_conv_plan(ctypes.byref(sh), 0, 1, out, 12) == 0 and out[0] == 0

@@ -1,5 +1,5 @@
 """CPU: pin the oracle against fixtures produced by the REFERENCE's own code
-(tests/golden/make_golden.py ran /root/reference/kurtosis.py and utils/KD_loss.py)."""
+(tests/golden/make_golden.py ran the reference's kurtosis.py and utils/KD_loss.py)."""
 import os
 
 import pytest
