@@ -59,6 +59,7 @@ SIGNATURES = {
     "bdbnn_wgrad_tc_workspace_bytes": (c_size_t, [_SH]),
     "bdbnn_debug_wgrad_plan": (c_int, [_SH, c_int, _P, c_int]),
     "bdbnn_debug_conv_plan": (c_int, [_SH, c_int, c_int, _P, c_int]),
+    "bdbnn_debug_tc_conv_ctas_per_sm": (c_int, [c_int, c_int, c_int, c_int, _P]),
     "bdbnn_binconv_wgrad_tc": (c_int, [_P, c_int, _P, _P, _P, _P, _P, _SH, _P, c_size_t, _P]),
     "bdbnn_kurtosis_multi_fwd": (c_int, [_P, _P, _P, c_int, _P, _P, _P, _P]),
     "bdbnn_kurtosis_multi_bwd": (c_int, [_P, _P, _P, c_int, _P, _P, _P, c_int, _P]),

@@ -34,6 +34,7 @@ struct TcConvParams {
   int32_t out_step, out_off_h, out_off_w, OHf, OWf;  // out pixel = (oh*out_step+off_h, ow*out_step+off_w) in OHf x OWf
   int32_t Nout, BN;          // GEMM N total / per CTA
   int32_t stages;
+  int32_t cm, cn;            // cluster: cm CTAs along M share the weight box, cn along N share the activation box
   int32_t row_bytes;         // KB * element size = swizzle span (32/64/128)
   const uint32_t* amax_bits; // FP16S: post-scale 2^-e (NULL otherwise)
   const float* add;          // dgrad: optional additive tensor
@@ -48,8 +49,12 @@ struct TcConvParams {
 };
 
 // KIND: 0 fp16, 1 bf16, 2 fp8 e4m3 operands; NW: wgmma N (16, 32, or 64 with BN/64 chunks)
+// Two CTAs per SM need <= 96 registers per thread: registers are allocated per warp inside each of the SM's four
+// 16K-register sub-partitions, and 2 x 9 warps put five warps on two of them.  The dgrad instances ask for that
+// bound (without it the NW = 64 ones took 102 registers and ran one CTA per SM); the forward ones fit at 96 without
+// it (0 = no minimum).  bdbnn_debug_tc_conv_ctas_per_sm reports the residency.
 template <int MODE, int KIND, int NW>
-__global__ void __launch_bounds__(kTcThreads)
+__global__ void __launch_bounds__(kTcThreads, MODE == 1 ? 2 : 0)
 tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const TcConvParams p) {
   constexpr int NCH = NW == 64 ? kMaxBN / 64 : 1;
@@ -70,11 +75,15 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int kb_total = p.n_kb * p.a_halves;
   const int n_iters = p.n_taps * kb_total;
   const bool do_stats = p.bn_sums != nullptr;
+  // cluster rank (x + y * cm); with cm * cn > 1 a ring slot is refilled only after the consumers of every CTA of the
+  // cluster released it, since any of them may multicast into it
+  const int cs = p.cm * p.cn;
+  const int rx = int(blockIdx.x) % p.cm, ry = int(blockIdx.y) % p.cn;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(smem_u32(&full_bar[s]), 1);
-      mbar_init(smem_u32(&empty_bar[s]), 2);      // one arrival per consumer warpgroup
+      mbar_init(smem_u32(&empty_bar[s]), 2 * cs);   // one arrival per consumer warpgroup of the cluster
     }
     fence_barrier_init();
   }
@@ -85,11 +94,17 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
   }
-  __syncthreads();
+  if (cs > 1) cluster_sync();   // peers' barriers are initialised before anyone multicasts or arrives on them
+  else __syncthreads();
 
   if (warp == kProducerWarp) {
     if (lane == 0) {
       const uint32_t tx = uint32_t(p.BNI * p.BH * p.BW + p.BN) * uint32_t(p.row_bytes);
+      // multicast groups: same M tile (column of the cluster) share A, same N tile (row) share B; the CTAs of a
+      // group take turns loading the shared box, one iteration each
+      uint16_t a_mask = 0, b_mask = 0;
+      for (int y = 0; y < p.cn; ++y) a_mask |= uint16_t(1u << (rx + y * p.cm));
+      for (int x = 0; x < p.cm; ++x) b_mask |= uint16_t(1u << (x + ry * p.cm));
       int it = 0;
       for (int ti = 0; ti < p.n_taps; ++ti) {
         const int dh = p.tap_dh[ti], dw = p.tap_dw[ti], tb = p.tap_b[ti];
@@ -101,8 +116,10 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           mbar_expect_tx(fb, tx);
           const uint32_t a_dst = tiles_base + stage * stage_bytes;
           const int kbb = kb >= p.n_kb ? kb - p.n_kb : kb;       // hi and lo halves share B
-          tma_load_4d(a_dst, &tmA, fb, kb * p.KB, dw, h0 * p.in_step + dh, n0);
-          tma_load_2d(a_dst + a_bytes, &tmB, fb, tb * p.Kc + kbb * p.KB, nn0);
+          if (p.cn == 1) tma_load_4d(a_dst, &tmA, fb, kb * p.KB, dw, h0 * p.in_step + dh, n0);
+          else if (it % p.cn == ry) tma_load_4d_mc(a_dst, &tmA, fb, kb * p.KB, dw, h0 * p.in_step + dh, n0, a_mask);
+          if (p.cm == 1) tma_load_2d(a_dst + a_bytes, &tmB, fb, tb * p.Kc + kbb * p.KB, nn0);
+          else if (it % p.cm == rx) tma_load_2d_mc(a_dst + a_bytes, &tmB, fb, tb * p.Kc + kbb * p.KB, nn0, b_mask);
         }
       }
     }
@@ -130,7 +147,12 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
       wgmma_commit();
       wgmma_wait<1>();
-      if (it > 0 && (threadIdx.x & 127) == 0) mbar_arrive(smem_u32(&empty_bar[(it - 1) % p.stages]));
+      if (it > 0 && (threadIdx.x & 127) == 0) {
+        const uint32_t eb = smem_u32(&empty_bar[(it - 1) % p.stages]);
+        if (cs == 1) mbar_arrive(eb);
+        else
+          for (int r = 0; r < cs; ++r) mbar_arrive_cluster(eb, uint32_t(r));
+      }
     }
     wgmma_wait<0>();
 #pragma unroll
@@ -154,6 +176,17 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
     for (int c = 0; c < NCH; ++c) {
       if (c >= nch) break;
+      // dgrad: `add` may alias `out`, so each pair's load of `add` waits for the previous pair's store.  Prefetching
+      // the chunk's `add` lines into L2 first turns that chain of HBM round trips into L2 hits (no registers held).
+      if (MODE == 1 && p.add != nullptr) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (!valid[h]) continue;
+          const float* row = p.add + pix[h] * p.Nout + nn0 + c * NW;
+#pragma unroll
+          for (int f = 0; f < NW; f += 32) asm volatile("prefetch.global.L2 [%0];" ::"l"(row + f));
+        }
+      }
 #pragma unroll
       for (int j = 0; j < NW / 8; ++j) {
         const int col = c * NW + 8 * j + 2 * (lane & 3);
@@ -233,6 +266,7 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       atomicMax(p.bn_ymax + nn0 + i, __float_as_uint(mx));
     }
   }
+  if (cs > 1) cluster_sync();   // no CTA exits while a peer may still multicast into it or arrive on its barriers
 }
 
 static bool chan_ok(int c) { return c == 16 || c == 32 || c == 64 || (c >= 128 && c % 128 == 0); }
@@ -253,6 +287,14 @@ static bool wide_gemm(const TcConvLaunch& L) {
   if (L.n_taps <= 0) return false;
   if (L.win ? (L.Kc != 32 || L.fmt < 0) : (L.Kc % 64 != 0)) return false;
   return L.Nout == 64 || L.Nout % 128 == 0;
+}
+
+// BDBNN_TC_CLUSTER=1: launch clusters that multicast the shared operand boxes.  Off by default: on an H100 the
+// ResNet-18 step's conv kernels ran 1.7-2x slower with them (DESIGN.md §7), every CTA of a cluster waiting for the
+// slowest one before a ring slot is refilled.
+static bool tc_cluster_enabled() {
+  const char* e = getenv("BDBNN_TC_CLUSTER");
+  return e && strcmp(e, "1") == 0;
 }
 
 // Tiling of one launch; returns false when the launch asks for something this kernel cannot give.
@@ -305,7 +347,31 @@ static bool plan_tc_conv(const TcConvLaunch& L, int mode, TcConvParams* pp, size
   p.stages = stages;
   *smem_out = size_t(stages) * stage_bytes + 1024;
   *tiles_out = p.tiles_h * ((L.NIMG + p.BNI - 1) / p.BNI);
+  // clusters of 2 neighbouring M tiles share the weight box, and of 2 N tiles (256 channels and up) the activation
+  // box; a grid side that does not divide keeps cluster size 1 there (the grid is never padded)
+  p.cm = p.cn = 1;
+  if (tc_cluster_enabled()) {
+    if (*tiles_out % 2 == 0) p.cm = 2;
+    if ((L.Nout / p.BN) % 2 == 0) p.cn = 2;
+  }
   return true;
+}
+
+template <typename K>
+static int launch_one(K kern, dim3 grid, size_t smem, cudaStream_t st, const CUtensorMap& tmA, const CUtensorMap& tmB,
+                      const TcConvParams& p) {
+  if (p.cm * p.cn == 1) {
+    kern<<<grid, kTcThreads, smem, st>>>(tmA, tmB, p);
+    return check_launch("tc_conv_kernel");
+  }
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid; cfg.blockDim = dim3(kTcThreads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = unsigned(p.cm); attr[0].val.clusterDim.y = unsigned(p.cn); attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr; cfg.numAttrs = 1;
+  BDBNN_CUDA(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, p));
+  return check_launch("tc_conv_kernel");
 }
 
 template <int MODE, int KIND>
@@ -314,15 +380,11 @@ static int launch_kind(const CUtensorMap& tmA, const CUtensorMap& tmB, const TcC
   auto kern = p.BN == 16 ? tc_conv_kernel<MODE, KIND, 16>
                          : (p.BN == 32 ? tc_conv_kernel<MODE, KIND, 32> : tc_conv_kernel<MODE, KIND, 64>);
   BDBNN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
-  if (p.bn_sums == nullptr) {
-    kern<<<grid, kTcThreads, smem, st>>>(tmA, tmB, p);
-    return check_launch("tc_conv_kernel");
-  }
+  if (p.bn_sums == nullptr) return launch_one(kern, grid, smem, st, tmA, tmB, p);
   TcConvParams q = p;
   int rc = det_sums_alloc(&q.stat_part, grid.x, 2 * p.Nout, st);
   if (rc) return rc;
-  kern<<<grid, kTcThreads, smem, st>>>(tmA, tmB, q);
-  rc = check_launch("tc_conv_kernel");
+  rc = launch_one(kern, grid, smem, st, tmA, tmB, q);
   if (rc) { cudaFreeAsync(q.stat_part, st); return rc; }
   return det_sums_finish(q.stat_part, grid.x, 2 * p.Nout, p.bn_sums, st);
 }
@@ -397,6 +459,7 @@ extern "C" int bdbnn_debug_trace(long long* device_buf) {
 // Host-only: the kernel's tiling for the forward (mode 0: 16-bit operands, 2: fp8) or the first dgrad phase
 // (mode 1) of a shape.  out[12] = {planned, halo, TS, NB, BN, n_tiles, supers, stages, dynamic smem, grid,
 // stage bytes, patch bytes}; halo = 0, TS = NB = 1 (one 128-row tile per CTA, no patch), supers = M tiles.
+// With n_out >= 14 also out[12..13] = cluster CTAs along M and along N (BDBNN_TC_CLUSTER applies).
 // planned = 0 when the GEMM is not eligible for the int16 result / fused dgrad statistics.  No CUDA call.
 extern "C" int bdbnn_debug_conv_plan(const bdbnn_conv_shape* s, int32_t mode, int32_t grad_halves, int32_t* out,
                                      int32_t n_out) {
@@ -404,7 +467,7 @@ extern "C" int bdbnn_debug_conv_plan(const bdbnn_conv_shape* s, int32_t mode, in
   if (rc) return rc;
   BDBNN_REQUIRE(out && n_out >= 12 && mode >= 0 && mode <= 2 && (grad_halves == 1 || grad_halves == 2),
                 "debug_conv_plan: bad arguments");
-  memset(out, 0, 12 * sizeof(int32_t));
+  memset(out, 0, size_t(n_out >= 14 ? 14 : 12) * sizeof(int32_t));
   if (!tc_shape_ok(s)) return BDBNN_OK;
   TcConvLaunch L;
   memset(&L, 0, sizeof(L));
@@ -443,9 +506,39 @@ extern "C" int bdbnn_debug_conv_plan(const bdbnn_conv_shape* s, int32_t mode, in
   size_t smem = 0;
   int tiles = 0;
   if (!plan_tc_conv(L, mode == 1 ? 1 : 0, &p, &smem, &tiles)) return BDBNN_OK;
-  const int32_t v[12] = {1, 0, 1, 1, p.BN, L.Nout / p.BN, tiles, p.stages, int32_t(smem), tiles * (L.Nout / p.BN),
-                         int32_t((uint32_t(kTileM + p.BN) * p.row_bytes + 1023u) & ~1023u), 0};
-  memcpy(out, v, sizeof(v));
+  const int32_t v[14] = {1, 0, 1, 1, p.BN, L.Nout / p.BN, tiles, p.stages, int32_t(smem), tiles * (L.Nout / p.BN),
+                         int32_t((uint32_t(kTileM + p.BN) * p.row_bytes + 1023u) & ~1023u), 0, p.cm, p.cn};
+  memcpy(out, v, size_t(n_out >= 14 ? 14 : 12) * sizeof(int32_t));
+  return BDBNN_OK;
+}
+
+// CTAs of one tc_conv_kernel instance that fit on an SM with `smem` bytes of dynamic shared memory (the dynamic smem
+// entry of bdbnn_debug_conv_plan).  mode 0 forward / 1 dgrad, fmt BDBNN_FMT_FP16 / BF16 or -1 (fp8, forward only),
+// bn = N tile (16, 32, 64 or 128).
+extern "C" int bdbnn_debug_tc_conv_ctas_per_sm(int32_t mode, int32_t fmt, int32_t bn, int32_t smem, int32_t* ctas) {
+  BDBNN_REQUIRE(ctas && (mode == 0 || mode == 1) && (bn == 16 || bn == 32 || bn == 64 || bn == 128) && smem >= 0 &&
+                    (fmt == BDBNN_FMT_FP16 || fmt == BDBNN_FMT_BF16 || (fmt == -1 && mode == 0)),
+                "debug_tc_conv_ctas_per_sm: bad arguments");
+  const void* kern;
+  if (fmt == -1)
+    kern = bn == 16 ? (const void*)tc_conv_kernel<0, 2, 16> : bn == 32 ? (const void*)tc_conv_kernel<0, 2, 32>
+                                                             : (const void*)tc_conv_kernel<0, 2, 64>;
+  else if (mode == 0 && fmt == BDBNN_FMT_FP16)
+    kern = bn == 16 ? (const void*)tc_conv_kernel<0, 0, 16> : bn == 32 ? (const void*)tc_conv_kernel<0, 0, 32>
+                                                             : (const void*)tc_conv_kernel<0, 0, 64>;
+  else if (mode == 0)
+    kern = bn == 16 ? (const void*)tc_conv_kernel<0, 1, 16> : bn == 32 ? (const void*)tc_conv_kernel<0, 1, 32>
+                                                             : (const void*)tc_conv_kernel<0, 1, 64>;
+  else if (fmt == BDBNN_FMT_FP16)
+    kern = bn == 16 ? (const void*)tc_conv_kernel<1, 0, 16> : bn == 32 ? (const void*)tc_conv_kernel<1, 0, 32>
+                                                             : (const void*)tc_conv_kernel<1, 0, 64>;
+  else
+    kern = bn == 16 ? (const void*)tc_conv_kernel<1, 1, 16> : bn == 32 ? (const void*)tc_conv_kernel<1, 1, 32>
+                                                             : (const void*)tc_conv_kernel<1, 1, 64>;
+  BDBNN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  int n = 0;
+  BDBNN_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, kTcThreads, size_t(smem)));
+  *ctas = n;
   return BDBNN_OK;
 }
 

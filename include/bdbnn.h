@@ -186,9 +186,16 @@ BDBNN_API size_t bdbnn_wgrad_tc_workspace_bytes(const bdbnn_conv_shape* s);
 /* Host-only: the forward/dgrad kernel's tiling for a shape (mode 0 = forward, 1 = first dgrad phase,
  * 2 = fp8 forward).  out[12] = {planned (0 = not eligible for the int16 result / fused dgrad statistics),
  * halo mode (0), M tiles per CTA (1), accumulator buffers (1), N tile, N tiles, M tiles, ring stages,
- * dynamic smem bytes, grid, stage bytes, patch bytes (0)}.  Makes no CUDA call. */
+ * dynamic smem bytes, grid, stage bytes, patch bytes (0)}; with n_out >= 14 also out[12], out[13] = thread-block
+ * cluster CTAs along M (sharing the weight box) and along N (sharing the activation box); 1 unless
+ * BDBNN_TC_CLUSTER=1, and 1 on a grid side that is odd.  Makes no CUDA call. */
 BDBNN_API int bdbnn_debug_conv_plan(const bdbnn_conv_shape* s, int32_t mode, int32_t grad_halves, int32_t* out,
                           int32_t n_out);
+/* CTAs of the forward (mode 0) / dgrad (mode 1) tensor-core kernel that fit on one SM of the current device, for
+ * operand format fmt (BDBNN_FMT_FP16 / BDBNN_FMT_BF16, -1 = fp8, forward only), N tile bn (16/32/64/128) and
+ * `smem` bytes of dynamic shared memory (bdbnn_debug_conv_plan out[8]), from the CUDA occupancy calculator.  Needs a
+ * CUDA device; sets that kernel's maximum dynamic shared memory attribute to `smem` (every launch sets it again). */
+BDBNN_API int bdbnn_debug_tc_conv_ctas_per_sm(int32_t mode, int32_t fmt, int32_t bn, int32_t smem, int32_t* ctas);
 /* Host-only: the tiling bdbnn_binconv_wgrad_tc would use, for tests.  out[12] = {supported, ksplit, ks_cap,
  * m_groups, n_tiles, dynamic smem bytes, M tiles per CTA, N tile, unit width, halo mode, K rows per stage,
  * ring stages}.  Makes no CUDA call. */
