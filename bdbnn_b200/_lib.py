@@ -76,6 +76,9 @@ SIGNATURES = {
     "bdbnn_bn_pool_bwd": (c_int, [_P] * 9 + [c_int] * 9 + [_P] * 9),
     "bdbnn_maxpool_fwd": (c_int, [_P, _P, _P] + [c_int] * 9 + [_P]),
     "bdbnn_maxpool_bwd": (c_int, [_P, _P, _P] + [c_int] * 9 + [_P]),
+    "bdbnn_bn_eval_fold": (c_int, [_P] * 5 + [c_int, ctypes.c_float, _P, _P, _P]),
+    "bdbnn_binconv_fwd_tc_eval": (c_int, [_P, _P, c_int] + [_P] * 6 + [_SH, _P]),
+    "bdbnn_stem_conv_fwd_eval": (c_int, [_P] * 5 + [c_int] * 3 + [_P]),
 }
 
 

@@ -390,9 +390,34 @@ int bn_stats_launch(const float* y, int64_t n_pix, int C, double* sums, uint32_t
                                  nullptr, st);
 }
 
+// Eval-mode BatchNorm folded into a per-channel affine map of the conv accumulator, in fp64 with every step rounded
+// on its own (nvcc would otherwise contract a*b+c into an FMA):  k = gamma / sqrt(rv + eps),
+// scale = float(alpha * k), shift = float(beta - rm * k).  oracle/eval_ref.py spells the same arithmetic.
+__global__ void bn_eval_fold_kernel(const float* __restrict__ alpha, const float* __restrict__ gamma,
+                                    const float* __restrict__ beta, const float* __restrict__ rm,
+                                    const float* __restrict__ rv, int C, double eps, float* __restrict__ scale,
+                                    float* __restrict__ shift) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  const double k = __ddiv_rn(double(gamma[c]), __dsqrt_rn(__dadd_rn(double(rv[c]), eps)));
+  const double a = alpha != nullptr ? double(alpha[c]) : 1.0;
+  scale[c] = __double2float_rn(__dmul_rn(a, k));
+  shift[c] = __double2float_rn(__dsub_rn(double(beta[c]), __dmul_rn(double(rm[c]), k)));
+}
+
 }  // namespace bdbnn
 
 using namespace bdbnn;
+
+extern "C" int bdbnn_bn_eval_fold(const float* alpha, const float* gamma, const float* beta, const float* running_mean,
+                                  const float* running_var, int32_t C, float eps, float* scale, float* shift,
+                                  void* stream) {
+  BDBNN_REQUIRE(C > 0, "bn_eval_fold: C must be positive");
+  BDBNN_REQUIRE(gamma && beta && running_mean && running_var && scale && shift, "bn_eval_fold: NULL pointer");
+  bn_eval_fold_kernel<<<(C + 127) / 128, 128, 0, cudaStream_t(stream)>>>(alpha, gamma, beta, running_mean, running_var,
+                                                                          C, double(eps), scale, shift);
+  return check_launch("bn_eval_fold_kernel");
+}
 
 static int bn_dims_ok(int64_t n_pix, int32_t C, bool pack) {
   BDBNN_REQUIRE(n_pix > 0 && C > 0 && (C & 3) == 0, "bn: C must be a positive multiple of 4");

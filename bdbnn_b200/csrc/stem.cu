@@ -172,6 +172,14 @@ extern "C" int bdbnn_stem_conv_fwd(const uint16_t* xw, const uint16_t* wf, const
   return launch_stem_fwd(xw, wf, alpha, y, g, bn_sums, bn_ymax, cudaStream_t(stream));
 }
 
+extern "C" int bdbnn_stem_conv_fwd_eval(const uint16_t* xw, const uint16_t* wf, const float* scale,
+                                        const float* shift, float* z, int32_t N, int32_t H, int32_t W, void* stream) {
+  StemGeom g;
+  BDBNN_REQUIRE(stem_geom(N, H, W, &g), "stem_conv_fwd_eval: geometry not supported");
+  BDBNN_REQUIRE(xw && wf && scale && shift && z, "stem_conv_fwd_eval: NULL pointer");
+  return launch_stem_eval(xw, wf, scale, shift, z, g, cudaStream_t(stream));
+}
+
 extern "C" int bdbnn_stem_conv_wgrad(const uint16_t* gys, const uint32_t* g_amax_bits, const uint16_t* xw,
                                      const uint32_t* x_amax_bits, float* gW, int32_t N, int32_t H, int32_t W,
                                      void* workspace, size_t workspace_bytes, void* stream) {

@@ -3,6 +3,8 @@
 //   tc_conv_kernel  : D[pix, n] = sum_{tap t} sum_{k} A[pix shifted by t, k] * B[n, t*Kc + k]
 //                     forward : A = sign(x)  (+-1 fp16/bf16/fp8, NHWC), B = sign(W) [Cout][T][Cin]; epilogue * alpha[n]
 //                     dgrad   : A = gy*gscale (bf16/fp16,  NHWC), B = sign(W)^T [Cin][T'][Cout]; epilogue * STE mask bit
+//                     eval    : the forward's operands; epilogue z = acc * scale[n] + shift[n] (+ residual), the
+//                               eval-mode BatchNorm folded into one affine map, and the +-1 copy of z
 //
 // Dataflow per CTA (one 128-row output tile, one N tile of BN <= 128 columns):
 //   warp 8 lane 0 : TMA producer. For every (tap, K-block) loads the activation box
@@ -37,8 +39,12 @@ struct TcConvParams {
   int32_t cm, cn;            // cluster: cm CTAs along M share the weight box, cn along N share the activation box
   int32_t row_bytes;         // KB * element size = swizzle span (32/64/128)
   const uint32_t* amax_bits; // FP16S: post-scale 2^-e (NULL otherwise)
-  const float* add;          // dgrad: optional additive tensor
-  const float* alpha;        // MODE 0: per-output-channel scale
+  const float* add;          // dgrad: optional additive tensor; eval: optional residual
+  const float* alpha;        // MODE 0: per-output-channel scale; MODE 2: folded BatchNorm scale
+  const float* shift;        // MODE 2: folded BatchNorm shift
+  uint16_t* zb;              // MODE 2: optional 16-bit +-1 copy of z (+1 = zb_one, -1 = zb_one | 0x8000)
+  uint8_t* zb8;              // MODE 2: optional fp8 e4m3 +-1 copy of z
+  uint32_t zb_one;           // MODE 2: 16-bit +1 (0x3C00 fp16, 0x3F80 bf16)
   const uint32_t* mask;      // MODE 1: STE mask words [pix][Nout/32 (ceil)]
   float* out;                // [pix][Nout] fp32
   int16_t* out_i16;          // MODE 0: the exact integer accumulator as int16 instead of out (y = alpha * int)
@@ -48,13 +54,14 @@ struct TcConvParams {
   const int16_t* st_y; const float* st_alpha; const float* st_mean; const float* st_invstd;   // MODE 1 statistics
 };
 
-// KIND: 0 fp16, 1 bf16, 2 fp8 e4m3 operands; NW: wgmma N (16, 32, or 64 with BN/64 chunks)
+// MODE: 0 forward, 1 dgrad, 2 eval forward; KIND: 0 fp16, 1 bf16, 2 fp8 e4m3 operands; NW: wgmma N (16, 32, or 64
+// with BN/64 chunks).
 // Two CTAs per SM need <= 96 registers per thread: registers are allocated per warp inside each of the SM's four
-// 16K-register sub-partitions, and 2 x 9 warps put five warps on two of them.  The dgrad instances ask for that
-// bound (without it the NW = 64 ones took 102 registers and ran one CTA per SM); the forward ones fit at 96 without
-// it (0 = no minimum).  bdbnn_debug_tc_conv_ctas_per_sm reports the residency.
+// 16K-register sub-partitions, and 2 x 9 warps put five warps on two of them.  The dgrad and eval instances ask for
+// that bound (without it the NW = 64 dgrad ones took 102 registers and ran one CTA per SM); the forward ones fit at
+// 96 without it (0 = no minimum).  bdbnn_debug_tc_conv_ctas_per_sm reports the residency.
 template <int MODE, int KIND, int NW>
-__global__ void __launch_bounds__(kTcThreads, MODE == 1 ? 2 : 0)
+__global__ void __launch_bounds__(kTcThreads, MODE == 0 ? 0 : 2)
 tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const TcConvParams p) {
   constexpr int NCH = NW == 64 ? kMaxBN / 64 : 1;
@@ -74,7 +81,7 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int nn0 = blockIdx.y * p.BN;
   const int kb_total = p.n_kb * p.a_halves;
   const int n_iters = p.n_taps * kb_total;
-  const bool do_stats = p.bn_sums != nullptr;
+  const bool do_stats = MODE != 2 && p.bn_sums != nullptr;
   // cluster rank (x + y * cm); with cm * cn > 1 a ring slot is refilled only after the consumers of every CTA of the
   // cluster released it, since any of them may multicast into it
   const int cs = p.cm * p.cn;
@@ -87,9 +94,10 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     }
     fence_barrier_init();
   }
-  for (int i = threadIdx.x; i < (kTcThreads / 32 - 1) * kMaxBN; i += blockDim.x) {
-    (&stat_sum[0][0])[i] = 0.f; (&stat_sq[0][0])[i] = 0.f; (&stat_max[0][0])[i] = 0.f;
-  }
+  if (MODE != 2)
+    for (int i = threadIdx.x; i < (kTcThreads / 32 - 1) * kMaxBN; i += blockDim.x) {
+      (&stat_sum[0][0])[i] = 0.f; (&stat_sq[0][0])[i] = 0.f; (&stat_max[0][0])[i] = 0.f;
+    }
   if (warp == kProducerWarp && lane == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
@@ -192,8 +200,9 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const int col = c * NW + 8 * j + 2 * (lane & 3);
         const int ch = nn0 + col;
         float a0 = 1.f, a1 = 1.f, sa0 = 0.f, sa1 = 0.f, sb0 = 0.f, sb1 = 0.f;
-        if (MODE == 0) {
+        if (MODE != 1) {
           a0 = __ldg(p.alpha + ch); a1 = __ldg(p.alpha + ch + 1);
+          if (MODE == 2) { sb0 = __ldg(p.shift + ch); sb1 = __ldg(p.shift + ch + 1); }
         } else if (do_stats) {               // yhat = y_int * alpha * invstd - mean * invstd of the producing unit
           const float is0 = __ldg(p.st_invstd + ch), is1 = __ldg(p.st_invstd + ch + 1);
           sa0 = __ldg(p.st_alpha + ch) * is0; sa1 = __ldg(p.st_alpha + ch + 1) * is1;
@@ -212,6 +221,22 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
               *reinterpret_cast<uint32_t*>(p.out_i16 + off) = (uint32_t(int(v0)) & 0xffffu) | (uint32_t(int(v1)) << 16);
             else
               *reinterpret_cast<float2*>(p.out + off) = make_float2(o0, o1);
+          } else if (MODE == 2) {
+            // two roundings per step, no FMA contraction: the CPU reference (oracle/eval_ref.py) matches bit for bit
+            o0 = __fadd_rn(__fmul_rn(v0, a0), sb0);
+            o1 = __fadd_rn(__fmul_rn(v1, a1), sb1);
+            if (p.add != nullptr) {          // the residual never aliases z (bdbnn_binconv_fwd_tc_eval rejects it)
+              const float2 r = __ldg(reinterpret_cast<const float2*>(p.add + off));
+              o0 = __fadd_rn(o0, r.x); o1 = __fadd_rn(o1, r.y);
+            }
+            *reinterpret_cast<float2*>(p.out + off) = make_float2(o0, o1);
+            // sign(v) = +1 iff v >= 0 (DESIGN.md §2): -0.0 -> +1, NaN -> -1
+            if (p.zb != nullptr)
+              *reinterpret_cast<uint32_t*>(p.zb + off) =
+                  (o0 >= 0.f ? p.zb_one : p.zb_one | 0x8000u) | ((o1 >= 0.f ? p.zb_one : p.zb_one | 0x8000u) << 16);
+            if (p.zb8 != nullptr)
+              *reinterpret_cast<uint16_t*>(p.zb8 + off) = uint16_t((o0 >= 0.f ? 0x38u : 0xB8u) |
+                                                                   ((o1 >= 0.f ? 0x38u : 0xB8u) << 8));
           } else {
             const uint32_t word = __ldg(p.mask + pix[h] * mask_words + (ch >> 5)) >> (ch & 31);
             o0 = (word & 1u) ? v0 * post : 0.0f;
@@ -334,6 +359,7 @@ static bool plan_tc_conv(const TcConvLaunch& L, int mode, TcConvParams* pp, size
   p.BN = pick_bn(L.Nout);
   if (L.fmt < 0 && p.BN < 64) return false;
   p.alpha = L.alpha; p.mask = L.mask; p.out = L.out; p.out_i16 = mode == 0 ? L.out_i16 : nullptr;
+  p.shift = L.shift; p.zb = L.zb; p.zb8 = L.zb8; p.zb_one = L.fmt == BDBNN_FMT_BF16 ? 0x3F80u : 0x3C00u;
   p.amax_bits = L.amax_bits; p.add = L.add;
   p.bn_sums = L.bn_sums; p.bn_ymax = L.bn_ymax;
   p.st_y = L.st_y; p.st_alpha = L.st_alpha; p.st_mean = L.st_mean; p.st_invstd = L.st_invstd;
@@ -414,8 +440,12 @@ static int launch_tc_conv(const TcConvLaunch& L, cudaStream_t st) {
   const bool stats_pass = MODE == 0 && L.bn_sums != nullptr && !wide_gemm(L) && L.out != nullptr;
   if (stats_pass) { p.bn_sums = nullptr; p.bn_ymax = nullptr; }
   if (L.fmt < 0) {
-    if (MODE != 0) { set_error("tc_conv: fp8 operands are forward only"); return BDBNN_ERR_UNSUPPORTED; }
-    return launch_kind<0, 2>(tmA, tmB, p, smem, grid, st);
+    if constexpr (MODE == 1) {
+      set_error("tc_conv: fp8 operands are forward only");
+      return BDBNN_ERR_UNSUPPORTED;
+    } else {
+      return launch_kind<MODE, 2>(tmA, tmB, p, smem, grid, st);
+    }
   }
   rc = L.fmt == BDBNN_FMT_BF16 ? launch_kind<MODE, 1>(tmA, tmB, p, smem, grid, st)
                                : launch_kind<MODE, 0>(tmA, tmB, p, smem, grid, st);
@@ -425,9 +455,9 @@ static int launch_tc_conv(const TcConvLaunch& L, cudaStream_t st) {
 
 // Stem conv forward (7x7 / stride 2 / pad 3 on 3 channels) as a 7-tap implicit GEMM over the packed
 // window view: tap r reads window row 2*oh + r, K = 32 values (8 pixels x 4 halves) per tap.
-int launch_stem_fwd(const uint16_t* xw, const uint16_t* wf, const float* alpha, float* y, const StemGeom& g,
-                    double* bn_sums, uint32_t* bn_ymax, cudaStream_t st) {
-  TcConvLaunch L;
+static void stem_launch(TcConvLaunch* Lp, const uint16_t* xw, const uint16_t* wf, const float* alpha, float* y,
+                        const StemGeom& g) {
+  TcConvLaunch& L = *Lp;
   memset(&L, 0, sizeof(L));
   L.A = xw; L.IH = g.HP; L.IW = g.Wo; L.Kc = kStemWin; L.a_halves = 1; L.in_step = 2;
   L.win = 1; L.win_stride = g.win_stride; L.win_row_stride = g.row_stride; L.win_img_stride = g.img_stride;
@@ -437,10 +467,25 @@ int launch_stem_fwd(const uint16_t* xw, const uint16_t* wf, const float* alpha, 
   L.n_taps = kStemTaps;
   L.out_step = 1; L.OHf = g.Ho; L.OWf = g.Wo;
   L.alpha = alpha; L.out = y; L.fmt = BDBNN_FMT_FP16;
+}
+
+int launch_stem_fwd(const uint16_t* xw, const uint16_t* wf, const float* alpha, float* y, const StemGeom& g,
+                    double* bn_sums, uint32_t* bn_ymax, cudaStream_t st) {
+  TcConvLaunch L;
+  stem_launch(&L, xw, wf, alpha, y, g);
   L.bn_sums = bn_sums; L.bn_ymax = bn_ymax;
   int rc = bn_stats_zero(bn_sums, bn_ymax, kStemCout, st);
   if (rc) return rc;
   return launch_tc_conv<0>(L, st);
+}
+
+// The same GEMM with the eval epilogue: z = acc * scale + shift (the folded eval-mode BatchNorm), no +-1 copy.
+int launch_stem_eval(const uint16_t* xw, const uint16_t* wf, const float* scale, const float* shift, float* z,
+                     const StemGeom& g, cudaStream_t st) {
+  TcConvLaunch L;
+  stem_launch(&L, xw, wf, scale, z, g);
+  L.shift = shift;
+  return launch_tc_conv<2>(L, st);
 }
 
 static long long* g_trace = nullptr;
@@ -456,16 +501,17 @@ extern "C" int bdbnn_debug_trace(long long* device_buf) {
   return BDBNN_OK;
 }
 
-// Host-only: the kernel's tiling for the forward (mode 0: 16-bit operands, 2: fp8) or the first dgrad phase
-// (mode 1) of a shape.  out[12] = {planned, halo, TS, NB, BN, n_tiles, supers, stages, dynamic smem, grid,
-// stage bytes, patch bytes}; halo = 0, TS = NB = 1 (one 128-row tile per CTA, no patch), supers = M tiles.
-// With n_out >= 14 also out[12..13] = cluster CTAs along M and along N (BDBNN_TC_CLUSTER applies).
-// planned = 0 when the GEMM is not eligible for the int16 result / fused dgrad statistics.  No CUDA call.
+// Host-only: the kernel's tiling for the forward (mode 0: 16-bit operands, 2: fp8), the first dgrad phase
+// (mode 1) or the eval forward (mode 3: 16-bit operands, 4: fp8) of a shape.  out[12] = {planned, halo, TS, NB, BN,
+// n_tiles, supers, stages, dynamic smem, grid, stage bytes, patch bytes}; halo = 0, TS = NB = 1 (one 128-row tile
+// per CTA, no patch), supers = M tiles.  With n_out >= 14 also out[12..13] = cluster CTAs along M and along N
+// (BDBNN_TC_CLUSTER applies).  planned = 0 when the GEMM is not eligible for the int16 result / fused dgrad
+// statistics (modes 0-2) or when the eval kernel cannot run the shape (modes 3-4).  No CUDA call.
 extern "C" int bdbnn_debug_conv_plan(const bdbnn_conv_shape* s, int32_t mode, int32_t grad_halves, int32_t* out,
                                      int32_t n_out) {
   int rc = validate_shape(s);
   if (rc) return rc;
-  BDBNN_REQUIRE(out && n_out >= 12 && mode >= 0 && mode <= 2 && (grad_halves == 1 || grad_halves == 2),
+  BDBNN_REQUIRE(out && n_out >= 12 && mode >= 0 && mode <= 4 && (grad_halves == 1 || grad_halves == 2),
                 "debug_conv_plan: bad arguments");
   memset(out, 0, size_t(n_out >= 14 ? 14 : 12) * sizeof(int32_t));
   if (!tc_shape_ok(s)) return BDBNN_OK;
@@ -498,14 +544,14 @@ extern "C" int bdbnn_debug_conv_plan(const bdbnn_conv_shape* s, int32_t mode, in
       }
     L.n_taps = T;
     L.out_step = 1; L.OHf = s->Ho; L.OWf = s->Wo;
-    L.fmt = mode == 2 ? -1 : BDBNN_FMT_FP16;
-    if (mode == 2 && s->Cin % 128 != 0) return BDBNN_OK;
+    L.fmt = (mode == 2 || mode == 4) ? -1 : BDBNN_FMT_FP16;
+    if (L.fmt == -1 && s->Cin % 128 != 0) return BDBNN_OK;
   }
-  if (L.n_taps == 0 || !wide_gemm(L)) return BDBNN_OK;
+  if (L.n_taps == 0 || (mode <= 2 && !wide_gemm(L))) return BDBNN_OK;
   TcConvParams p;
   size_t smem = 0;
   int tiles = 0;
-  if (!plan_tc_conv(L, mode == 1 ? 1 : 0, &p, &smem, &tiles)) return BDBNN_OK;
+  if (!plan_tc_conv(L, mode == 1 ? 1 : (mode <= 2 ? 0 : 2), &p, &smem, &tiles)) return BDBNN_OK;
   const int32_t v[14] = {1, 0, 1, 1, p.BN, L.Nout / p.BN, tiles, p.stages, int32_t(smem), tiles * (L.Nout / p.BN),
                          int32_t((uint32_t(kTileM + p.BN) * p.row_bytes + 1023u) & ~1023u), 0, p.cm, p.cn};
   memcpy(out, v, size_t(n_out >= 14 ? 14 : 12) * sizeof(int32_t));
@@ -513,14 +559,23 @@ extern "C" int bdbnn_debug_conv_plan(const bdbnn_conv_shape* s, int32_t mode, in
 }
 
 // CTAs of one tc_conv_kernel instance that fit on an SM with `smem` bytes of dynamic shared memory (the dynamic smem
-// entry of bdbnn_debug_conv_plan).  mode 0 forward / 1 dgrad, fmt BDBNN_FMT_FP16 / BF16 or -1 (fp8, forward only),
-// bn = N tile (16, 32, 64 or 128).
+// entry of bdbnn_debug_conv_plan).  mode 0 forward / 1 dgrad / 2 eval forward, fmt BDBNN_FMT_FP16 / BF16 or -1 (fp8,
+// forward and eval only), bn = N tile (16, 32, 64 or 128).
 extern "C" int bdbnn_debug_tc_conv_ctas_per_sm(int32_t mode, int32_t fmt, int32_t bn, int32_t smem, int32_t* ctas) {
-  BDBNN_REQUIRE(ctas && (mode == 0 || mode == 1) && (bn == 16 || bn == 32 || bn == 64 || bn == 128) && smem >= 0 &&
-                    (fmt == BDBNN_FMT_FP16 || fmt == BDBNN_FMT_BF16 || (fmt == -1 && mode == 0)),
+  BDBNN_REQUIRE(ctas && mode >= 0 && mode <= 2 && (bn == 16 || bn == 32 || bn == 64 || bn == 128) && smem >= 0 &&
+                    (fmt == BDBNN_FMT_FP16 || fmt == BDBNN_FMT_BF16 || (fmt == -1 && mode != 1)),
                 "debug_tc_conv_ctas_per_sm: bad arguments");
   const void* kern;
-  if (fmt == -1)
+  if (mode == 2 && fmt == -1)
+    kern = bn == 16 ? (const void*)tc_conv_kernel<2, 2, 16> : bn == 32 ? (const void*)tc_conv_kernel<2, 2, 32>
+                                                             : (const void*)tc_conv_kernel<2, 2, 64>;
+  else if (mode == 2 && fmt == BDBNN_FMT_FP16)
+    kern = bn == 16 ? (const void*)tc_conv_kernel<2, 0, 16> : bn == 32 ? (const void*)tc_conv_kernel<2, 0, 32>
+                                                             : (const void*)tc_conv_kernel<2, 0, 64>;
+  else if (mode == 2)
+    kern = bn == 16 ? (const void*)tc_conv_kernel<2, 1, 16> : bn == 32 ? (const void*)tc_conv_kernel<2, 1, 32>
+                                                             : (const void*)tc_conv_kernel<2, 1, 64>;
+  else if (fmt == -1)
     kern = bn == 16 ? (const void*)tc_conv_kernel<0, 2, 16> : bn == 32 ? (const void*)tc_conv_kernel<0, 2, 32>
                                                              : (const void*)tc_conv_kernel<0, 2, 64>;
   else if (mode == 0 && fmt == BDBNN_FMT_FP16)
@@ -558,6 +613,23 @@ extern "C" int bdbnn_tc_supported(const bdbnn_conv_shape* s) {
          (i16 ? BDBNN_TC_FWD_I16 : 0);
 }
 
+// The implicit GEMM of a forward conv: A = the +-1 activations (NHWC, fmt), B = the +-1 weights [Cout][T][Cin].
+static void fwd_launch(TcConvLaunch* Lp, const void* xb, const void* wf, int fmt, const bdbnn_conv_shape* s) {
+  TcConvLaunch& L = *Lp;
+  memset(&L, 0, sizeof(L));
+  L.A = static_cast<const uint16_t*>(xb); L.IH = s->H; L.IW = s->W; L.Kc = s->Cin; L.a_halves = 1; L.in_step = s->stride;
+  L.B = static_cast<const uint16_t*>(wf); L.b_taps = s->kh * s->kw; L.Nout = s->Cout;
+  L.NIMG = s->N; L.OH = s->Ho; L.OW = s->Wo;
+  for (int r = 0; r < s->kh; ++r)
+    for (int q = 0; q < s->kw; ++q) {
+      const int t = r * s->kw + q;
+      L.dh[t] = int8_t(r - s->pad); L.dw[t] = int8_t(q - s->pad); L.tb[t] = uint8_t(t);
+    }
+  L.n_taps = s->kh * s->kw;
+  L.out_step = 1; L.OHf = s->Ho; L.OWf = s->Wo;
+  L.fmt = fmt;
+}
+
 // Forward with the result stored as the exact integer accumulator (int16) — see include/bdbnn.h.
 extern "C" int bdbnn_binconv_fwd_tc_i16(const void* xb, const void* wf, int32_t fmt, const float* alpha,
                                         int16_t* y_int, const bdbnn_conv_shape* s, double* bn_sums,
@@ -571,18 +643,8 @@ extern "C" int bdbnn_binconv_fwd_tc_i16(const void* xb, const void* wf, int32_t 
     return BDBNN_ERR_UNSUPPORTED;
   }
   TcConvLaunch L;
-  memset(&L, 0, sizeof(L));
-  L.A = static_cast<const uint16_t*>(xb); L.IH = s->H; L.IW = s->W; L.Kc = s->Cin; L.a_halves = 1; L.in_step = s->stride;
-  L.B = static_cast<const uint16_t*>(wf); L.b_taps = s->kh * s->kw; L.Nout = s->Cout;
-  L.NIMG = s->N; L.OH = s->Ho; L.OW = s->Wo;
-  for (int r = 0; r < s->kh; ++r)
-    for (int q = 0; q < s->kw; ++q) {
-      const int t = r * s->kw + q;
-      L.dh[t] = int8_t(r - s->pad); L.dw[t] = int8_t(q - s->pad); L.tb[t] = uint8_t(t);
-    }
-  L.n_taps = s->kh * s->kw;
-  L.out_step = 1; L.OHf = s->Ho; L.OWf = s->Wo;
-  L.alpha = alpha; L.out = nullptr; L.out_i16 = y_int; L.fmt = fmt;
+  fwd_launch(&L, xb, wf, fmt, s);
+  L.alpha = alpha; L.out = nullptr; L.out_i16 = y_int;
   BDBNN_REQUIRE((bn_sums == nullptr) == (bn_ymax == nullptr), "binconv_fwd_tc_i16: bn_sums and bn_ymax go together");
   BDBNN_REQUIRE(bn_sums == nullptr || s->Cout <= 512, "binconv_fwd_tc_i16: statistics need Cout <= 512");
   L.bn_sums = bn_sums; L.bn_ymax = bn_ymax;
@@ -600,18 +662,8 @@ extern "C" int bdbnn_binconv_fwd_tc(const uint16_t* xb_bf16, const uint16_t* wf_
   BDBNN_REQUIRE(xb_bf16 && wf_bf16 && alpha && y, "binconv_fwd_tc: NULL pointer");
   if (!tc_shape_ok(s)) { set_error("binconv_fwd_tc: shape not supported by the tensor-core path"); return BDBNN_ERR_UNSUPPORTED; }
   TcConvLaunch L;
-  memset(&L, 0, sizeof(L));
-  L.A = xb_bf16; L.IH = s->H; L.IW = s->W; L.Kc = s->Cin; L.a_halves = 1; L.in_step = s->stride;
-  L.B = wf_bf16; L.b_taps = s->kh * s->kw; L.Nout = s->Cout;
-  L.NIMG = s->N; L.OH = s->Ho; L.OW = s->Wo;
-  for (int r = 0; r < s->kh; ++r)
-    for (int q = 0; q < s->kw; ++q) {
-      const int t = r * s->kw + q;
-      L.dh[t] = int8_t(r - s->pad); L.dw[t] = int8_t(q - s->pad); L.tb[t] = uint8_t(t);
-    }
-  L.n_taps = s->kh * s->kw;
-  L.out_step = 1; L.OHf = s->Ho; L.OWf = s->Wo;
-  L.alpha = alpha; L.out = y; L.fmt = fmt;
+  fwd_launch(&L, xb_bf16, wf_bf16, fmt, s);
+  L.alpha = alpha; L.out = y;
   BDBNN_REQUIRE((bn_sums == nullptr) == (bn_ymax == nullptr), "binconv_fwd_tc: bn_sums and bn_ymax go together");
   L.bn_sums = bn_sums; L.bn_ymax = bn_ymax;
   rc = bn_stats_zero(bn_sums, bn_ymax, s->Cout, cudaStream_t(stream));
@@ -630,25 +682,34 @@ extern "C" int bdbnn_binconv_fwd_tc8(const uint8_t* xb_fp8, const uint8_t* wf_fp
     return BDBNN_ERR_UNSUPPORTED;
   }
   TcConvLaunch L;
-  memset(&L, 0, sizeof(L));
-  L.A = reinterpret_cast<const uint16_t*>(xb_fp8); L.IH = s->H; L.IW = s->W; L.Kc = s->Cin; L.a_halves = 1;
-  L.in_step = s->stride;
-  L.B = reinterpret_cast<const uint16_t*>(wf_fp8); L.b_taps = s->kh * s->kw; L.Nout = s->Cout;
-  L.NIMG = s->N; L.OH = s->Ho; L.OW = s->Wo;
-  for (int r = 0; r < s->kh; ++r)
-    for (int q = 0; q < s->kw; ++q) {
-      const int t = r * s->kw + q;
-      L.dh[t] = int8_t(r - s->pad); L.dw[t] = int8_t(q - s->pad); L.tb[t] = uint8_t(t);
-    }
-  L.n_taps = s->kh * s->kw;
-  L.out_step = 1; L.OHf = s->Ho; L.OWf = s->Wo;
-  L.alpha = alpha; L.out = y; L.fmt = -1;
+  fwd_launch(&L, xb_fp8, wf_fp8, -1, s);
+  L.alpha = alpha; L.out = y;
   BDBNN_REQUIRE((bn_sums == nullptr) == (bn_ymax == nullptr), "binconv_fwd_tc8: bn_sums and bn_ymax go together");
   BDBNN_REQUIRE(bn_sums == nullptr || s->Cout <= 512, "binconv_fwd_tc8: statistics need Cout <= 512");
   L.bn_sums = bn_sums; L.bn_ymax = bn_ymax;
   rc = bn_stats_zero(bn_sums, bn_ymax, s->Cout, cudaStream_t(stream));
   if (rc) return rc;
   return launch_tc_conv<0>(L, cudaStream_t(stream));
+}
+
+// Eval-mode forward: z = alpha-folded BatchNorm of the conv (+ residual) and its +-1 copy — see include/bdbnn.h.
+extern "C" int bdbnn_binconv_fwd_tc_eval(const void* xb, const void* wf, int32_t fmt, const float* scale,
+                                         const float* shift, const float* residual, float* z, uint16_t* zb,
+                                         uint8_t* zb8, const bdbnn_conv_shape* s, void* stream) {
+  BDBNN_REQUIRE(fmt == BDBNN_FMT_FP16 || fmt == BDBNN_FMT_BF16 || fmt == -1, "binconv_fwd_tc_eval: bad operand format");
+  int rc = validate_shape(s);
+  if (rc) return rc;
+  BDBNN_REQUIRE(xb && wf && scale && shift && z, "binconv_fwd_tc_eval: NULL pointer");
+  BDBNN_REQUIRE(residual != z, "binconv_fwd_tc_eval: residual must not alias z");
+  BDBNN_REQUIRE(fmt != -1 || zb == nullptr, "binconv_fwd_tc_eval: the 16-bit copy needs 16-bit operands");
+  if (!tc_shape_ok(s) || (fmt == -1 && s->Cin % 128 != 0)) {
+    set_error("binconv_fwd_tc_eval: shape not supported by the tensor-core path");
+    return BDBNN_ERR_UNSUPPORTED;
+  }
+  TcConvLaunch L;
+  fwd_launch(&L, xb, wf, fmt, s);
+  L.alpha = scale; L.shift = shift; L.add = residual; L.out = z; L.zb = zb; L.zb8 = zb8;
+  return launch_tc_conv<2>(L, cudaStream_t(stream));
 }
 
 struct DgradStats {      // backward statistics of the BatchNorm unit that produced this conv's input (see tc_common.cuh)

@@ -123,6 +123,8 @@ def algorithmic_bytes(kernel, sh, gh=1):
         "fwd_xnor": n_in // 8 + n_w // 8 + 4 * n_out,         # read bits, write fp32 y
         "fwd_tc": 2 * n_in + 2 * n_w + 4 * n_out,             # read bf16 +-1, write fp32 y
         "fwd_tc8": n_in + n_w + 4 * n_out,                    # read fp8 +-1, write fp32 y
+        "fwd_tc_eval": 2 * n_in + 2 * n_w + 4 * n_out,        # read bf16 +-1, write fp32 z (+ residual, copy)
+        "fwd_tc8_eval": n_in + n_w + 4 * n_out,               # read fp8 +-1, write fp32 z (+ residual, copy)
         "dgrad": 4 * n_out + n_w // 8 + n_in // 8 + 4 * n_in,  # read gy, bits; write gx
         "wgrad": 4 * n_out + n_in // 8 + n_w // 8 + 4 * n_w,
         "grad_pack": 4 * n_out + 2 * gh * n_out,
@@ -1344,8 +1346,8 @@ def stem_conv_supported(x, weight, stride, padding):
     return bool(_lib.lib().bdbnn_stem_supported(x.shape[0], x.shape[2], x.shape[3]))
 
 
-def _stem_conv_fwd_impl(x, weight, want_stats=False):
-    """stem_pack -> stem_conv_fwd. Returns (y fp32 channels_last, xw, x_amax[, (sums, ymax) BN statistics of y])."""
+def _stem_pack_impl(x, weight):
+    """stem_pack. Returns (xw, x_amax, wf, alpha, timer key)."""
     L = _lib.lib()
     dev = x.device
     n, _, h, w = x.shape
@@ -1353,8 +1355,6 @@ def _stem_conv_fwd_impl(x, weight, want_stats=False):
     if not (xd.is_contiguous() or xd.is_contiguous(memory_format=torch.channels_last)):
         xd = xd.contiguous()
     wd = weight.detach().contiguous()
-    st = _stream()
-    ho, wo = (h - 1) // 2 + 1, (w - 1) // 2 + 1
     xw = torch.empty((int(L.bdbnn_stem_xw_bytes(n, h, w)) // 2,), dtype=torch.int16, device=dev)
     x_amax = torch.empty((1,), dtype=torch.int32, device=dev)
     wf = torch.empty((64, 7, 32), dtype=torch.int16, device=dev)
@@ -1362,7 +1362,18 @@ def _stem_conv_fwd_impl(x, weight, want_stats=False):
     key = f"stem_N{n}_{h}x{w}"
     with _timed("stem_pack", key, 4 * xd.numel() * 2 + xw.numel() * 2):
         _lib.check(L.bdbnn_stem_pack(_p(xd), n, h, w, xd.stride(0), xd.stride(1), xd.stride(2), xd.stride(3),
-                                     _p(wd), _p(xw), _p(x_amax), _p(wf), _p(alpha), st), "stem_pack")
+                                     _p(wd), _p(xw), _p(x_amax), _p(wf), _p(alpha), _stream()), "stem_pack")
+    return xw, x_amax, wf, alpha, key
+
+
+def _stem_conv_fwd_impl(x, weight, want_stats=False):
+    """stem_pack -> stem_conv_fwd. Returns (y fp32 channels_last, xw, x_amax[, (sums, ymax) BN statistics of y])."""
+    L = _lib.lib()
+    dev = x.device
+    n, _, h, w = x.shape
+    st = _stream()
+    ho, wo = (h - 1) // 2 + 1, (w - 1) // 2 + 1
+    xw, x_amax, wf, alpha, key = _stem_pack_impl(x, weight)
     y = torch.empty((n, 64, ho, wo), dtype=torch.float32, device=dev, memory_format=torch.channels_last)
     stats = None
     if want_stats and conv_stats_enabled():
@@ -1487,4 +1498,216 @@ def stem_bn_pool(y, gamma, beta, running_mean, running_var, momentum, eps, kerne
     if zs is not None:
         z._bdbnn_pack = (zs, zm, zb, grad_mode()[3], zb8)
         z._bdbnn_pack_version = z._version
+    return z
+
+
+# ---------------------------------------------------------------------------------------------------
+# Eval-mode forward (DESIGN.md §4g): BatchNorm with running statistics folded into the conv epilogue.
+# Plain functions, no autograd: the kernels have no backward, so grad mode must be off.
+# ---------------------------------------------------------------------------------------------------
+def _eval_only(what):
+    if torch.is_grad_enabled():
+        raise RuntimeError(f"bdbnn_b200.{what}: the eval-mode kernels have no backward; call under torch.no_grad() "
+                           "or torch.inference_mode()")
+
+
+def _on_x_device(fn):
+    """Device guard for the plain eval functions (see _on_device): launch on the device of the first argument."""
+    @functools.wraps(fn)
+    def guarded(x, *args, **kw):
+        if x.is_cuda and x.device.index != torch.cuda.current_device():
+            with torch.cuda.device(x.device):
+                return fn(x, *args, **kw)
+        return fn(x, *args, **kw)
+    return guarded
+
+
+def bn_eval_fold(gamma, beta, running_mean, running_var, eps, alpha=None):
+    """(scale, shift) float32 [C] with BN_eval(alpha * acc) = acc * scale + shift: in fp64, k = gamma/sqrt(rv + eps),
+    scale = alpha * k, shift = beta - rm * k, each rounded to fp32 once (include/bdbnn.h, bdbnn_bn_eval_fold)."""
+    L = _lib.lib()
+    c = gamma.numel()
+    vecs = [t.detach().contiguous() for t in (gamma, beta, running_mean, running_var)]
+    for t in vecs:
+        _require_cuda(t, "bn_eval_fold")
+        if t.numel() != c:
+            raise RuntimeError("bn_eval_fold: gamma, beta and the running statistics must have the same length")
+    if alpha is not None:
+        _require_cuda(alpha, "bn_eval_fold(alpha)")
+    _same_device(alpha, *vecs)
+    scale = torch.empty((c,), dtype=torch.float32, device=gamma.device)
+    shift = torch.empty((c,), dtype=torch.float32, device=gamma.device)
+    with _timed("bn_eval_fold", f"c{c}", (4 + 5) * 4 * c):
+        _lib.check(L.bdbnn_bn_eval_fold(_p(alpha), *[_p(t) for t in vecs], c, float(eps), _p(scale), _p(shift),
+                                        _stream()), "bn_eval_fold")
+    _lib.count(1)
+    return scale, shift
+
+
+def eval_unit_supported(x_shape, w_shape, stride, padding):
+    """The eval unit needs only the wgmma forward for the conv shape."""
+    sh = conv_shape(x_shape, w_shape, stride, padding)
+    return bool(int(_lib.lib().bdbnn_tc_supported(ctypes.byref(sh))) & 1)
+
+
+def eval_use8(cin, cout):
+    """fp8 operands for an eval unit: the fp8 forward exists (Cin % 128 == 0) and z's +-1 copy is fp8 too
+    (Cout % 128 == 0), since the eval kernel writes the 16-bit copy only from 16-bit operands."""
+    return fwd8_enabled() and cin % 128 == 0 and cout % 128 == 0
+
+
+@_on_x_device
+def conv_bn_add_eval(x, weight, gamma, beta, running_mean, running_var, eps, stride, padding, residual,
+                     shortcut=None):
+    """z = BN_eval(binconv2d(x, weight)) + residual in one kernel (bdbnn_binconv_fwd_tc_eval), under no_grad.
+    `shortcut` = (weight[Cout,Cin,1,1], gamma, beta, running_mean, running_var, eps, stride) computes the residual as
+    the real-valued 1x1 conv + BN_eval `downsample` branch of x.  The returned z carries `_bdbnn_eval_pack` =
+    (format, +-1 copy of z) for the next unit: fp8 bytes (format -1) when Cout % 128 == 0 and BDBNN_FWD8 is on, else
+    16-bit in the grad_mode() format.  x's own `_bdbnn_eval_pack` is used when it matches this conv's operand."""
+    _eval_only("conv_bn_add_eval")
+    _require_cuda(x, "conv_bn_add_eval(x)")
+    _require_cuda(weight, "conv_bn_add_eval(weight)")
+    _same_device(x, weight, gamma, beta, running_mean, running_var, residual)
+    if shortcut is not None:
+        if residual is not None:
+            raise RuntimeError("conv_bn_add_eval: pass either residual or shortcut")
+        residual = _shortcut_eval_impl(x, *shortcut)
+    L = _lib.lib()
+    sh = conv_shape(x.shape, weight.shape, stride, padding)
+    caps = int(L.bdbnn_tc_supported(ctypes.byref(sh)))
+    if not caps & 1:
+        raise RuntimeError("bdbnn_b200.conv_bn_add_eval: the wgmma forward does not support this shape")
+    dev = x.device
+    n, cin, h, wd = x.shape
+    cout, _, kh, kw = weight.shape
+    z_shape = (n, cout, sh.Ho, sh.Wo)
+    if residual is not None and tuple(residual.shape) != z_shape:
+        raise RuntimeError(f"conv_bn_add_eval: residual shape {tuple(residual.shape)} != output shape {z_shape}")
+    fmt = grad_mode()[3]
+    st = _stream()
+    key = _shape_key(sh)
+    pack = cout % 32 == 0
+    out8 = pack and cout % 128 == 0 and fwd8_enabled()
+    use8 = bool(caps & 8) and eval_use8(cin, cout)
+    want = -1 if use8 else fmt
+    pk = getattr(x, "_bdbnn_eval_pack", None)
+    if pk is not None and pk[0] == want and x._bdbnn_eval_pack_version == x._version:
+        xop = pk[1]
+    else:
+        cw = (cin + 31) // 32
+        xs = torch.empty((n, h, wd, cw), dtype=torch.int32, device=dev)
+        xm = torch.empty((n, h, wd, cw), dtype=torch.int32, device=dev)
+        xb = torch.empty((n, h, wd, cin), dtype=torch.int16, device=dev) if not use8 else None
+        with _timed("act_pack", key, algorithmic_bytes("act_pack" if use8 else "act_pack_tc", sh)):
+            _lib.check(L.bdbnn_act_pack(_p(_nhwc(x.detach())), n * h * wd, cin, _p(xs), _p(xm), _p(xb), fmt, st),
+                       "act_pack")
+        _lib.count(1)
+        xop = xb
+        if use8:
+            xop = torch.empty((n, h, wd, cin), dtype=torch.uint8, device=dev)
+            _lib.check(L.bdbnn_bits_to_fp8(_p(xs), n * h * wd, cin, _p(xop), st), "bits_to_fp8")
+            _lib.count(1)
+    pre = _PREPACKED.get(weight.data_ptr())
+    if pre is not None and pre[0] == weight._version and pre[1] == fmt and pre[2] == use8:
+        alpha, wop = pre[4], (pre[8] if use8 else pre[7])     # packed with every binary conv (prepack_weights)
+    else:
+        T, cw = kh * kw, (cin + 31) // 32
+        alpha = torch.empty((cout,), dtype=torch.float32, device=dev)
+        wsign = torch.empty((cout, T, cw), dtype=torch.int32, device=dev)
+        wmask = torch.empty(((cout * cin * T + 31) // 32,), dtype=torch.int32, device=dev)
+        wop = torch.empty((cout, T, cin), dtype=torch.uint8 if use8 else torch.int16, device=dev)
+        _lib.check(L.bdbnn_weight_pack(_p(weight.detach().contiguous()), cout, cin, kh, kw, _p(alpha), _p(wsign),
+                                       _p(wmask), None if use8 else _p(wop), None, _p(wop) if use8 else None, None,
+                                       None, fmt, st), "weight_pack")
+        _lib.count(2)
+    scale, shift = bn_eval_fold(gamma, beta, running_mean, running_var, eps, alpha)
+    rc = _nhwc(residual.detach()) if residual is not None else None
+    z = torch.empty(z_shape, dtype=torch.float32, device=dev, memory_format=torch.channels_last)
+    zb = torch.empty((n, sh.Ho, sh.Wo, cout), dtype=torch.int16, device=dev) if (pack and not out8) else None
+    zb8 = torch.empty((n, sh.Ho, sh.Wo, cout), dtype=torch.uint8, device=dev) if out8 else None
+    n_out = z.numel()
+    nbytes = (algorithmic_bytes("fwd_tc8_eval" if use8 else "fwd_tc_eval", sh) + (4 * n_out if rc is not None else 0)
+              + (2 * n_out if zb is not None else 0) + (n_out if zb8 is not None else 0))
+    with _timed("binconv_fwd_tc8_eval" if use8 else "binconv_fwd_tc_eval", key, nbytes):
+        _lib.check(L.bdbnn_binconv_fwd_tc_eval(_p(xop), _p(wop), want, _p(scale), _p(shift), _p(rc), _p(z), _p(zb),
+                                               _p(zb8), ctypes.byref(sh), st), "binconv_fwd_tc_eval")
+    _lib.count(1)
+    if pack and not z.is_inference():       # inference tensors have no version counter to guard the copy with
+        z._bdbnn_eval_pack = (-1, zb8) if out8 else (fmt, zb)
+        z._bdbnn_eval_pack_version = z._version
+    return z
+
+
+def shortcut_eval_supported(x, weight, stride):
+    """fp32 1x1 shortcut conv + BN_eval on the wgmma forward: CUDA fp32 x, [Cout,Cin,1,1] weight, Cin % 4 == 0, and
+    the forward available for the 1x1 GEMM over the samples."""
+    if not (x.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and weight.dim() == 4):
+        return False
+    cout, cin, kh, kw = weight.shape
+    if (kh, kw) != (1, 1) or cin != x.shape[1] or cin % 4:
+        return False
+    n, _, h, w = x.shape
+    ho, wo = (h - 1) // stride + 1, (w - 1) // stride + 1
+    return bool(int(_lib.lib().bdbnn_tc_supported(ctypes.byref(conv_shape((n, cin, ho, wo), weight.shape, 1, 0)))) & 1)
+
+
+@_on_x_device
+def _shortcut_eval_impl(x, weight, gamma, beta, running_mean, running_var, eps, stride):
+    """BN_eval(conv2d(x, weight[Cout,Cin,1,1], stride)): real_conv_pack -> fold(alpha) -> fwd_tc_eval over the packed
+    samples (fp16 operands, 1x1 stride 1), no residual and no +-1 copy."""
+    _eval_only("shortcut_eval")
+    _require_cuda(x, "shortcut_eval(x)")
+    L = _lib.lib()
+    dev = x.device
+    st = _stream()
+    n, cin, h, w = x.shape
+    cout = weight.shape[0]
+    ho, wo = (h - 1) // stride + 1, (w - 1) // stride + 1
+    sh1 = conv_shape((n, cin, ho, wo), weight.shape, 1, 0)
+    key = _shape_key(conv_shape(x.shape, weight.shape, stride, 0))
+    f32 = dict(dtype=torch.float32, device=dev)
+    xh = torch.empty((n, ho, wo, cin), dtype=torch.int16, device=dev)
+    amax2 = torch.empty((2,), dtype=torch.int32, device=dev)
+    wf = torch.empty((cout, cin), dtype=torch.int16, device=dev)
+    wt = torch.empty((cin, cout), dtype=torch.int16, device=dev)
+    alpha, gscale, inv_gscale = torch.empty((cout,), **f32), torch.empty((cout,), **f32), torch.empty((cout,), **f32)
+    with _timed("shortcut_pack", key, 4 * n * ho * wo * cin * 2 + 2 * n * ho * wo * cin):
+        _lib.check(L.bdbnn_real_conv_pack(_p(_nhwc(x.detach())), n, h, w, cin, stride, _p(weight.detach().contiguous()),
+                                          cout, _p(xh), _p(amax2), _p(wf), _p(wt), _p(alpha), _p(gscale),
+                                          _p(inv_gscale), st), "real_conv_pack")
+    _lib.count(4)       # x amax, x pack, W amax, W pack
+    scale, shift = bn_eval_fold(gamma, beta, running_mean, running_var, eps, alpha)
+    z = torch.empty((n, cout, ho, wo), memory_format=torch.channels_last, **f32)
+    with _timed("shortcut_fwd_tc_eval", key, 2 * xh.numel() + 2 * wf.numel() + 4 * z.numel()):
+        _lib.check(L.bdbnn_binconv_fwd_tc_eval(_p(xh), _p(wf), FMT_FP16, _p(scale), _p(shift), None, _p(z), None, None,
+                                               ctypes.byref(sh1), st), "binconv_fwd_tc_eval(shortcut)")
+    _lib.count(1)
+    return z
+
+
+@_on_x_device
+def stem_conv_bn_pool_eval(x, weight, gamma, beta, running_mean, running_var, eps, kernel_size, stride, padding):
+    """maxpool(BN_eval(stem_conv(x))) under no_grad: stem_pack -> fold(alpha) -> stem_conv_fwd_eval -> maxpool_fwd.
+    The BatchNorm is applied before the max (gamma may be negative), so the pool reads the folded result."""
+    _eval_only("stem_conv_bn_pool_eval")
+    _require_cuda(x, "stem_conv_bn_pool_eval(x)")
+    L = _lib.lib()
+    dev = x.device
+    st = _stream()
+    n, _, h, w = x.shape
+    ho, wo = (h - 1) // 2 + 1, (w - 1) // 2 + 1
+    k, s, p = int(kernel_size), int(stride), int(padding)
+    po, pw = (ho + 2 * p - k) // s + 1, (wo + 2 * p - k) // s + 1
+    xw, _x_amax, wf, alpha, key = _stem_pack_impl(x, weight)
+    scale, shift = bn_eval_fold(gamma, beta, running_mean, running_var, eps, alpha)
+    y = torch.empty((n, 64, ho, wo), dtype=torch.float32, device=dev, memory_format=torch.channels_last)
+    with _timed("stem_conv_fwd_eval", key, xw.numel() * 2 + 4 * y.numel()):
+        _lib.check(L.bdbnn_stem_conv_fwd_eval(_p(xw), _p(wf), _p(scale), _p(shift), _p(y), n, h, w, st),
+                   "stem_conv_fwd_eval")
+    _lib.count(4)       # x amax, x pack, W pack, conv
+    z = torch.empty((n, 64, po, pw), dtype=torch.float32, device=dev, memory_format=torch.channels_last)
+    idx = torch.empty((n, po, pw, 64), dtype=torch.uint8, device=dev)
+    with _timed("stem_maxpool_fwd", key, 4 * y.numel() + 5 * z.numel()):
+        _lib.check(L.bdbnn_maxpool_fwd(_p(y), _p(z), _p(idx), n, ho, wo, 64, k, s, p, po, pw, st), "maxpool_fwd")
+    _lib.count(1)
     return z

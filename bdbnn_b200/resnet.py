@@ -33,18 +33,60 @@ def _fused_unit(x, conv, bn, residual, shortcut=None):
     return z
 
 
+def _eval_mode(x, bn):
+    """Eval-mode forward without autograd on a CUDA fp32 tensor: the condition of every eval kernel path."""
+    return (x.is_cuda and x.dtype == torch.float32 and not bn.training and not torch.is_grad_enabled() and
+            F_.fuse_enabled())
+
+
+def _eval_unit(x, conv, bn, residual):
+    """BN_eval(conv(x)) + residual through the eval kernels when the pair qualifies, else None.  Applies under
+    no_grad / inference_mode only: with grad enabled the module chain keeps its autograd graph.  EDE changes only the
+    backward, so it does not exclude a unit."""
+    if not (_eval_mode(x, bn) and isinstance(conv, BinarizeConv2d) and isinstance(bn, nn.BatchNorm2d)):
+        return None
+    if not (bn.affine and bn.running_mean is not None and bn.running_var is not None) or conv.impl == "xnor":
+        return None
+    if not F_.eval_unit_supported(x.shape, conv.weight.shape, conv.stride[0], conv.padding[0]):
+        return None
+    return F_.conv_bn_add_eval(x, conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps,
+                               conv.stride[0], conv.padding[0], residual)
+
+
+def _eval_shortcut(x, ds):
+    """The `downsample` branch in eval mode: BN_eval(1x1 conv) on the wgmma forward when it qualifies, else ds(x)."""
+    if (isinstance(ds, nn.Sequential) and len(ds) == 2 and type(ds[0]) is nn.Conv2d and
+            isinstance(ds[1], nn.BatchNorm2d)):
+        conv, bn = ds[0], ds[1]
+        if (_eval_mode(x, bn) and bn.affine and bn.running_mean is not None and bn.running_var is not None and
+                conv.bias is None and conv.kernel_size == (1, 1) and conv.padding == (0, 0) and
+                conv.stride[0] == conv.stride[1] and conv.groups == 1 and
+                F_.shortcut_eval_supported(x, conv.weight, conv.stride[0])):
+            return F_._shortcut_eval_impl(x, conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps,
+                                          conv.stride[0])
+    return ds(x)
+
+
 def _prepack(model, x):
-    """Pack the weights of every binary conv that will run as a fused unit in this forward, in two launches
-    (functional.prepack_weights).  Returns True if functional._PREPACKED was filled (caller clears it)."""
-    if not (x.is_cuda and model.training and F_.fuse_enabled() and F_.prepack_enabled() and x.dtype == torch.float32):
+    """Pack the weights of every binary conv that will run as a fused (training) or eval unit in this forward, in
+    two launches (functional.prepack_weights).  Returns True if functional._PREPACKED was filled (caller clears it).
+    Packs are never kept across forwards: the fused optimizers update parameters in place without bumping
+    `_version`, so a cached pack could hold stale signs."""
+    if not (x.is_cuda and F_.fuse_enabled() and F_.prepack_enabled() and x.dtype == torch.float32):
+        return False
+    if not model.training and torch.is_grad_enabled():
         return False
     items = []
     for m in model.modules():
-        if isinstance(m, BinarizeConv2d) and m.impl != "xnor" and not m.ede_active and m.weight.is_cuda:
+        if (isinstance(m, BinarizeConv2d) and m.impl != "xnor" and m.weight.is_cuda and
+                not (model.training and m.ede_active)):
             cout, cin, kh, kw = m.weight.shape
             if (cin * kh * kw) % 32 == 0 and cin % 64 == 0 and cout % 32 == 0:
-                # the fp8 forward is used where the shape allows (same rule as _ConvBNAddUnit)
-                use8 = F_.fwd8_enabled() and cin % 128 == 0 and (cout == 64 or cout % 128 == 0)
+                # the fp8 forward is used where the shape allows (same rule as _ConvBNAddUnit / conv_bn_add_eval)
+                if model.training:
+                    use8 = F_.fwd8_enabled() and cin % 128 == 0 and (cout == 64 or cout % 128 == 0)
+                else:
+                    use8 = F_.eval_use8(cin, cout)
                 items.append((m.weight, use8))
     if not items:
         return False
@@ -93,14 +135,18 @@ class BasicBlock(nn.Module):
                 if out is not None:
                     self.downsample[1].num_batches_tracked.add_(1)
             if out is None:
-                residual = (F_.shortcut_conv_bn(x, *sc) if sc is not None else self.downsample(x))
+                residual = (F_.shortcut_conv_bn(x, *sc) if sc is not None else _eval_shortcut(x, self.downsample))
                 if sc is not None:
                     self.downsample[1].num_batches_tracked.add_(1)
+        if out is None:
+            out = _eval_unit(x, self.conv1, self.bn1, residual)
         if out is None:
             out = _fused_unit(x, self.conv1, self.bn1, residual)
         if out is None:
             out = self.bn1(self.conv1(x)) + residual
-        out2 = _fused_unit(out, self.conv2, self.bn2, out)
+        out2 = _eval_unit(out, self.conv2, self.bn2, out)
+        if out2 is None:
+            out2 = _fused_unit(out, self.conv2, self.bn2, out)
         if out2 is None:
             out2 = self.bn2(self.conv2(out)) + out
         return out2
@@ -138,6 +184,10 @@ class ResNetImageNet(nn.Module):
         c1, bn, mp = self.conv1, self.bn1, self.maxpool
         tc_stem = (type(c1) is nn.Conv2d and c1.bias is None and F_.stem_tc_enabled() and
                    F_.stem_conv_supported(x, c1.weight, c1.stride, c1.padding))   # BDBNN_STEM_TC=0 -> cuDNN
+        if (tc_stem and _eval_mode(x, bn) and isinstance(mp, MaxPool2dNHWC) and bn.affine and
+                bn.running_mean is not None and bn.running_var is not None):
+            return F_.stem_conv_bn_pool_eval(x, c1.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps,
+                                             mp.kernel_size, mp.stride, mp.padding)
         fuse = (x.is_cuda and bn.training and F_.fuse_enabled() and isinstance(mp, MaxPool2dNHWC) and bn.affine and
                 bn.track_running_stats and bn.momentum is not None and x.dtype == torch.float32 and
                 c1.out_channels % 4 == 0)
@@ -187,10 +237,14 @@ class BasicBlockCifar(nn.Module):
 
     def forward(self, x):
         residual = x if self.shortcut is None else self.shortcut(x)
-        out = _fused_unit(x, self.conv1, self.bn1, residual)
+        out = _eval_unit(x, self.conv1, self.bn1, residual)
+        if out is None:
+            out = _fused_unit(x, self.conv1, self.bn1, residual)
         if out is None:
             out = self.bn1(self.conv1(x)) + residual
-        out2 = _fused_unit(out, self.conv2, self.bn2, out)
+        out2 = _eval_unit(out, self.conv2, self.bn2, out)
+        if out2 is None:
+            out2 = _fused_unit(out, self.conv2, self.bn2, out)
         if out2 is None:
             out2 = self.bn2(self.conv2(out)) + out
         return out2

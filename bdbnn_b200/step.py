@@ -131,6 +131,39 @@ class FusedOps:
         return cross_entropy_topk(output, target, topk, meters)
 
 
+class EvalStep:
+    """One validation batch: the per-batch body of validate() (train.py:687-702) — the model in eval mode under
+    no_grad, criterion and top-1/top-5 accuracy accumulated into device meters; nothing is read back (the reference's
+    `.item()` calls are left to averages())."""
+
+    def __init__(self, model, ops=FusedOps):
+        self.model, self.ops = model, ops
+        self.meters = None          # device float64 {ce*N, acc1*N, acc5*N, N}
+
+    def __call__(self, images, target):
+        """Returns (output, loss, acc1, acc5) as device tensors."""
+        self.model.eval()                                                         # train.py:687
+        with torch.no_grad():                                                     # train.py:689
+            output = self.model(images)                                           # train.py:696
+            topk = (1, min(5, output.shape[1]))
+            if self.meters is None or self.meters.device != output.device:
+                self.meters = torch.zeros(4, dtype=torch.float64, device=output.device)
+            loss, (acc1, acc5) = self.ops.ce_acc(output, target, topk, self.meters)   # train.py:697-702
+        return output, loss, acc1, acc5
+
+    def averages(self):
+        """Running (loss, acc1, acc5) averages since construction / reset_meters() — one host read."""
+        if self.meters is None:
+            return None
+        m = self.meters.tolist()
+        n = max(m[3], 1.0)
+        return {"loss": m[0] / n, "acc1": m[1] / n, "acc5": m[2] / n, "samples": int(m[3])}
+
+    def reset_meters(self):
+        if self.meters is not None:
+            self.meters.zero_()
+
+
 class TrainStep:
     """One optimisation step. `grad_sync` (optional) is called between backward and optimizer.step()
     — the data-parallel gradient all-reduce (bdbnn_b200.ddp.GradAllReduce)."""

@@ -147,6 +147,32 @@ BDBNN_API int bdbnn_binconv_fwd_tc_i16(const void* xb, const void* wf, int32_t f
                              int16_t* y_int, const bdbnn_conv_shape* s, double* bn_sums, uint32_t* bn_ymax,
                              void* stream);
 
+/* ---- eval-mode forward: conv + BatchNorm(eval) + residual in one epilogue ------------------------------------
+ * Replaces the module chain model.eval() under torch.no_grad() runs per binary conv in validate()
+ * (train.py:677-714): act_pack, weight pack, conv, nn.BatchNorm2d(eval), residual add.
+ * bn_eval_fold : per channel, in fp64 with every step rounded separately (no FMA),
+ *                  k = gamma / sqrt(running_var + eps)    (eps: this fp32 value widened to double)
+ *                  scale[c] = float(alpha[c] * k),  shift[c] = float(beta - running_mean * k)
+ *                alpha may be NULL (= 1).  One launch, no scratch.
+ * binconv_fwd_tc_eval : the forward implicit GEMM of bdbnn_binconv_fwd_tc (same operands, tiling and
+ *                BDBNN_TC_CLUSTER behaviour) with, from the fp32 accumulator acc, rounding each step (no FMA):
+ *                  z = fp32(fp32(acc * scale[o]) + shift[o]);  z = fp32(z + residual)  if residual != NULL
+ *                z fp32 NHWC [N,Ho,Wo,Cout]; residual (may be NULL) has z's shape and must not alias it.
+ *                Optional +-1 copies of z for the next conv (sign(v) = +1 iff v >= 0: -0.0 -> +1, NaN -> -1):
+ *                zb  16-bit in format fmt (fp16 0x3C00/0xBC00, bf16 0x3F80/0xBF80), needs fmt >= 0;
+ *                zb8 fp8 e4m3 bytes (0x38 / 0xB8); both NHWC like z, NULL = not written.
+ *                fmt = BDBNN_FMT_FP16 / BDBNN_FMT_BF16 (16-bit operands) or -1 (fp8 operands, needs BDBNN_TC_FWD8).
+ *                Writes no statistics and allocates nothing.  Requires bdbnn_tc_supported(s) & BDBNN_TC_FWD.
+ *                The 1x1 `downsample` in eval: bdbnn_real_conv_pack, then this call as a 1x1 stride-1 conv over
+ *                xh (fmt FP16) with scale folded from the pack's alpha, no residual and no copies.
+ * stem_conv_fwd_eval : the stem GEMM of bdbnn_stem_conv_fwd with the same epilogue (no residual, no copies);
+ *                scale is folded from bdbnn_stem_pack's alpha.  The max-pool after it is bdbnn_maxpool_fwd. */
+BDBNN_API int bdbnn_bn_eval_fold(const float* alpha, const float* gamma, const float* beta, const float* running_mean,
+                       const float* running_var, int32_t C, float eps, float* scale, float* shift, void* stream);
+BDBNN_API int bdbnn_binconv_fwd_tc_eval(const void* xb, const void* wf, int32_t fmt, const float* scale,
+                              const float* shift, const float* residual, float* z, uint16_t* zb, uint8_t* zb8,
+                              const bdbnn_conv_shape* s, void* stream);
+
 /* ---- backward: data gradient -------------------------------------------------------------------
  * gx[n,h,w,c] = mask(n,h,w,c) * sum_{t,o} gy[n,ho,wo,o] * alpha[o] * sign(W[o,c,t])
  * Replaces cuDNN dgrad + the STE mask multiply that autograd runs under loss.backward()
@@ -184,15 +210,16 @@ BDBNN_API int bdbnn_binconv_dgrad_tc(const uint16_t* gys, int32_t grad_mode, con
                            const bdbnn_conv_shape* s, void* stream);
 BDBNN_API size_t bdbnn_wgrad_tc_workspace_bytes(const bdbnn_conv_shape* s);
 /* Host-only: the forward/dgrad kernel's tiling for a shape (mode 0 = forward, 1 = first dgrad phase,
- * 2 = fp8 forward).  out[12] = {planned (0 = not eligible for the int16 result / fused dgrad statistics),
+ * 2 = fp8 forward, 3 = eval forward, 4 = fp8 eval forward).  out[12] = {planned (modes 0-2: 0 = not eligible for the
+ * int16 result / fused dgrad statistics; modes 3-4: 0 = the eval kernel cannot run the shape),
  * halo mode (0), M tiles per CTA (1), accumulator buffers (1), N tile, N tiles, M tiles, ring stages,
  * dynamic smem bytes, grid, stage bytes, patch bytes (0)}; with n_out >= 14 also out[12], out[13] = thread-block
  * cluster CTAs along M (sharing the weight box) and along N (sharing the activation box); 1 unless
  * BDBNN_TC_CLUSTER=1, and 1 on a grid side that is odd.  Makes no CUDA call. */
 BDBNN_API int bdbnn_debug_conv_plan(const bdbnn_conv_shape* s, int32_t mode, int32_t grad_halves, int32_t* out,
                           int32_t n_out);
-/* CTAs of the forward (mode 0) / dgrad (mode 1) tensor-core kernel that fit on one SM of the current device, for
- * operand format fmt (BDBNN_FMT_FP16 / BDBNN_FMT_BF16, -1 = fp8, forward only), N tile bn (16/32/64/128) and
+/* CTAs of the forward (mode 0) / dgrad (mode 1) / eval forward (mode 2) tensor-core kernel that fit on one SM of the
+ * current device, for operand format fmt (BDBNN_FMT_FP16 / BDBNN_FMT_BF16, -1 = fp8, not dgrad), N tile bn (16/32/64/128) and
  * `smem` bytes of dynamic shared memory (bdbnn_debug_conv_plan out[8]), from the CUDA occupancy calculator.  Needs a
  * CUDA device; sets that kernel's maximum dynamic shared memory attribute to `smem` (every launch sets it again). */
 BDBNN_API int bdbnn_debug_tc_conv_ctas_per_sm(int32_t mode, int32_t fmt, int32_t bn, int32_t smem, int32_t* ctas);
@@ -345,6 +372,8 @@ BDBNN_API int bdbnn_stem_pack(const float* x, int32_t N, int32_t H, int32_t W, i
                     float* alpha, void* stream);
 BDBNN_API int bdbnn_stem_conv_fwd(const uint16_t* xw, const uint16_t* wf, const float* alpha, float* y, int32_t N,
                         int32_t H, int32_t W, double* bn_sums, uint32_t* bn_ymax, void* stream);
+BDBNN_API int bdbnn_stem_conv_fwd_eval(const uint16_t* xw, const uint16_t* wf, const float* scale, const float* shift,
+                             float* z, int32_t N, int32_t H, int32_t W, void* stream);
 BDBNN_API int bdbnn_stem_conv_wgrad(const uint16_t* gys, const uint32_t* g_amax_bits, const uint16_t* xw,
                           const uint32_t* x_amax_bits, float* gW, int32_t N, int32_t H, int32_t W,
                           void* workspace, size_t workspace_bytes, void* stream);
