@@ -6,15 +6,28 @@
 // contiguous one in NHWC memory, so a TMA box [pixels][64 channels] lands in shared memory exactly in
 // the canonical MN-major SWIZZLE_128B layout (8 pixel rows x 128 B per swizzle atom; SBO = 1024 B
 // between 8-row K groups; LBO = distance between MN chunks).
-// An M tile of 128 rows is two 64-channel "units" (tap, channel-chunk); unit u = tap * (Cin/64) + chunk.
-// Per K stage one TMA box per unit is loaded (plus the gys boxes); warpgroup 0 multiplies rows [0, 64) of
-// every M tile, warpgroup 1 rows [64, 128).
+// An M tile of 128 rows is two 64-channel "units" (tap, channel-chunk); warpgroup 0 multiplies rows [0, 64)
+// of every M tile, warpgroup 1 rows [64, 128).  The planner picks, per shape, whichever of two operand modes
+// moves fewer L2->shared-memory bytes:
+//
+// BOX mode: unit u = tap * (Cin/64) + chunk; per K stage one TMA box per unit is loaded (plus the gys boxes).
+//
+// PATCH mode (stride 1, one image per K stage): unit u = chunk * T + s * kh + r for tap (r, s), so the units of a
+// CTA share (chunk, filter column) pairs.  Per K stage ONE activation patch per distinct (chunk, s) pair of the CTA is
+// loaded: BH + kh - 1 input rows x Wo columns starting at (h0 - pad, s - pad), zero-filled outside the image — the
+// boxes of the kh taps of filter column s, stacked.  Tap (r, s) is that patch viewed from row r * Wo: a descriptor
+// whose start is a whole number of 128-byte rows into a 1024-byte-aligned SWIZZLE_128B tile reads the tile shifted by
+// that many rows, because the swizzle XOR is taken from absolute shared-memory address bits (as TMA's is).  The K
+// rows, the gys boxes, the K stages and the split are those of the box plan of the same shape, so both modes feed
+// every accumulator the same products in the same wgmma K steps and give bit-identical results.
 //
 // Each CTA owns up to G accumulators (G*BN <= 256: 128 fp32 registers per thread) that share the gys stage,
 // walks a contiguous range of K stages (split-K across CTAs) and writes its partial tiles to its own slice of
 // an fp32 workspace [ksplit][T*Cin][Cout] (plain stores, no atomics); the finalize kernel sums the
 // slices in a fixed order (run-to-run deterministic), applies 1/gscale[o], the FP16S 2^-e, the
 // |W|<=1 STE mask and the [t][c][o] -> OIHW transposition.
+#include <type_traits>
+
 #include "tc_common.cuh"
 
 namespace bdbnn {
@@ -24,12 +37,13 @@ constexpr int kMaxUnits = 16;      // units per CTA (G <= 4 M tiles of 2 units, 
 
 struct TcWgradParams {
   int32_t OW, OH, NIMG;          // gy pixel grid
+  int32_t patch;                 // 0: box mode, 1: patch mode (file comment)
   int32_t BW, BH, BNI, tiles_h;  // K stage = BNI x BH x BW output pixels
-  int32_t rows_a, rows_b;        // rows TMA writes per A box and per B box
+  int32_t rows_a, rows_b;        // rows TMA writes per A box (patch) and per B box
   int32_t k_stage;               // K rows consumed per stage (multiple of 16)
-  uint32_t a_box_bytes;          // smem footprint of one A box (1024-aligned)
+  uint32_t a_box_bytes;          // smem footprint of one A box or patch slot (1024-aligned)
   uint32_t b_box_bytes;
-  int32_t n_a_boxes;             // A boxes per stage
+  int32_t n_a_boxes;             // A boxes (patch slots) per stage: the most any M group loads
   int32_t n_kboxes, kboxes_per_cta;
   int32_t Cin, Cout, kh, kw, pad, stride;
   int32_t g_halves;              // 1: gys = bf16(g); 2: gys = [hi | lo] split, both accumulated
@@ -44,6 +58,16 @@ struct TcWgradParams {
   long long* trace;              // optional clock64 trace of CTA (0,0,0) (bdbnn_debug_trace)
 };
 
+// A boxes (box mode) or patches (patch mode) a CTA of M group `mg` loads per K stage.
+__host__ __device__ inline int wgrad_a_loads(const TcWgradParams& p, int mg) {
+  const int upt = kTileM / p.UW;
+  const int n_mtiles = (p.n_units + upt - 1) / upt;
+  const int g_cta = min(p.G, n_mtiles - mg * p.G);
+  if (!p.patch) return g_cta * upt;
+  const int u0 = mg * p.G * upt, u1 = min(u0 + g_cta * upt, p.n_units);
+  return (u1 - 1) / p.kh - u0 / p.kh + 1;                        // distinct (chunk, s) pairs: u / kh
+}
+
 #define BDBNN_WTR(r, ev)                                                                         \
   do {                                                                                           \
     if (p.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && tr_n < 1023) { \
@@ -53,17 +77,23 @@ struct TcWgradParams {
     }                                                                                            \
   } while (0)
 
-// NW: wgmma N (16 or 32 for the narrow N tiles, else 64 with BN/64 chunks).  Accumulator slot s = g * (BN/NW) + chunk.
-template <int KIND, int NW>
+// NW: wgmma N = the N tile BN (16, 32, 64, 128 or 256): one wgmma per M tile and K step reads the A operand once for
+// the whole N tile; the MN-major gys operand spans the tile's 64-channel boxes (LBO = box size).  Accumulator
+// slot g = M tile g of the CTA.
+// NS > 0: the plan's G slots, all issued unconditionally (a CTA of the last M group with fewer M tiles multiplies a
+// duplicate unit into the extra slots and does not store them), so the wgmma chain of a K step has no branch and
+// ptxas does not fence between its wgmmas.  NS = 0: up to 256 / NW slots, predicated on the CTA's count.
+template <int KIND, int NW, int NS>
 __global__ void __launch_bounds__(kTcThreads)
 tc_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmG,
                 const TcWgradParams p) {
-  constexpr int kSlots = 256 / NW;                               // 128 accumulator floats per thread
+  constexpr int kSlots = NS > 0 ? NS : 256 / NW;                 // at most 128 accumulator floats per thread
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[kMaxStages];
   __shared__ __align__(8) uint64_t empty_bar[kMaxStages];
-  __shared__ uint32_t unit_off[kMaxUnits];   // byte offset of unit i's operand box inside a stage
+  __shared__ uint32_t unit_off[kMaxUnits];   // byte offset of unit i's operand (box or patch view) inside a stage
   __shared__ int32_t unit_c[kMaxUnits], unit_dw[kMaxUnits], unit_dh[kMaxUnits];   // TMA coordinates of unit i
+  __shared__ int32_t unit_row[kMaxUnits];    // workspace row of unit i's first channel: t * Cin + chunk * UW
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t tiles_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -81,13 +111,23 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
   const int kb_begin = blockIdx.x * p.kboxes_per_cta;
   const int kb_end = min(kb_begin + p.kboxes_per_cta, p.n_kboxes);
 
-  if (threadIdx.x < g_cta * upt) {
+  const int q_first = p.patch ? mt0 * upt / p.kh : 0;             // first (chunk, s) pair of this CTA's patches
+  if (threadIdx.x < (NS > 0 ? p.G : g_cta) * upt) {
     int u = mt0 * upt + threadIdx.x;
-    if (u >= p.n_units) u = p.n_units - 1;                         // odd unit count: rows ignored
-    const int t = u / p.chunks_per_tap, j = u - t * p.chunks_per_tap;
-    unit_off[threadIdx.x] = threadIdx.x * p.a_box_bytes;
+    if (u >= p.n_units) u = p.n_units - 1;                         // beyond the last unit: rows ignored
     // the producer is ONE thread: everything per unit that needs a division is computed here, once
-    const int r = t / p.kw, sx = t - r * p.kw;
+    int j, r, sx;
+    if (p.patch) {
+      const int q = u / p.kh;                                      // (chunk, s) pair: q = chunk * kw + s
+      j = q / p.kw; sx = q - j * p.kw; r = u - q * p.kh;
+      unit_off[threadIdx.x] = uint32_t(q - q_first) * p.a_box_bytes + uint32_t(r * p.BW) * 128u;
+    } else {
+      const int t = u / p.chunks_per_tap;
+      j = u - t * p.chunks_per_tap; r = t / p.kw; sx = t - r * p.kw;
+      unit_off[threadIdx.x] = threadIdx.x * p.a_box_bytes;
+    }
+    const int t = r * p.kw + sx;
+    unit_row[threadIdx.x] = t * p.Cin + j * p.UW;
     unit_c[threadIdx.x] = j * 64;
     unit_dw[threadIdx.x] = sx - p.pad;
     unit_dh[threadIdx.x] = r - p.pad;
@@ -134,8 +174,8 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
 
   if (warp == kProducerWarp) {
     if (lane == 0) {
-      const int n_units_cta = g_cta * upt;
-      const uint32_t tx = uint32_t(n_units_cta) * uint32_t(p.rows_a) * a_row +
+      const int n_loads = wgrad_a_loads(p, blockIdx.y);
+      const uint32_t tx = uint32_t(n_loads) * uint32_t(p.rows_a) * a_row +
                           uint32_t(nb_boxes) * uint32_t(p.rows_b) * b_row;
       int tr_n = 0;
       int stage = 0;
@@ -149,9 +189,16 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
         mbar_expect_tx(fb, tx);
         const int n0 = tile_n * p.BNI, h0 = tile_h * p.BH;
         const uint32_t dst0 = tiles_base + stage * stage_bytes;
-        const int hs = h0 * p.stride;
-        for (int i = 0; i < n_units_cta; ++i)
-          tma_load_4d(dst0 + unit_off[i], &tmX, fb, unit_c[i], unit_dw[i], hs + unit_dh[i], n0);
+        if (p.patch) {
+          for (int i = 0, q = q_first; i < n_loads; ++i, ++q) {
+            const int j = q / p.kw;
+            tma_load_4d(dst0 + i * p.a_box_bytes, &tmX, fb, j * 64, q - j * p.kw - p.pad, h0 - p.pad, n0);
+          }
+        } else {
+          const int hs = h0 * p.stride;
+          for (int i = 0; i < n_loads; ++i)
+            tma_load_4d(dst0 + unit_off[i], &tmX, fb, unit_c[i], unit_dw[i], hs + unit_dh[i], n0);
+        }
         uint32_t bdst = dst0 + a_bytes;
         for (int hf = 0; hf < p.g_halves; ++hf)
           for (int jb = 0; jb < nb_chunks; ++jb, bdst += p.b_box_bytes)
@@ -162,8 +209,7 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
     }
   } else if (kb_end > kb_begin) {
     const int wg = warp >> 2, wq = warp & 3;
-    const int nch = p.BN / NW;                                     // wgmma chunks per M tile
-    const int n_slots = g_cta * nch;
+    const int n_slots = g_cta;
     const int u_wg = 64 / p.UW;                                    // units in this warpgroup's 64 rows
     float acc[kSlots][NW / 2];
 #pragma unroll
@@ -185,10 +231,9 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
           // 16 pixel rows per K step: 2 swizzle atoms of 8 rows
 #pragma unroll
           for (int s = 0; s < kSlots; ++s) {
-            if (s < n_slots) {
-              const int g = s / nch, c = s - g * nch;
-              const uint64_t ad = make_smem_desc(a0 + unit_off[g * upt + wg * u_wg] + uint32_t(k) * 16u * a_row, lbo_a, a_row);
-              const uint64_t bd = make_smem_desc(b0 + uint32_t(hf * nb_chunks + c) * p.b_box_bytes + uint32_t(k) * 16u * b_row,
+            if (NS > 0 || s < n_slots) {
+              const uint64_t ad = make_smem_desc(a0 + unit_off[s * upt + wg * u_wg] + uint32_t(k) * 16u * a_row, lbo_a, a_row);
+              const uint64_t bd = make_smem_desc(b0 + uint32_t(hf * nb_chunks) * p.b_box_bytes + uint32_t(k) * 16u * b_row,
                                                  p.b_box_bytes, b_row);
               wgmma_ss<NW, KIND, 1, 1>(acc[s], ad, bd);
             }
@@ -209,13 +254,12 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
 #pragma unroll
     for (int s = 0; s < kSlots; ++s) {
       if (s >= n_slots) break;
-      const int g = s / nch, c = s - g * nch;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int m = wg * 64 + wq * 16 + (lane >> 2) + 8 * h;
-        const int u = (mt0 + g) * upt + m / p.UW;
-        if (u >= p.n_units) continue;
-        float* wrow = slice + (int64_t(u) * p.UW + (m % p.UW)) * p.Cout + nn0 + c * NW + 2 * (lane & 3);   // row t*Cin + c
+        const int ul = s * upt + m / p.UW;
+        if ((mt0 * upt + ul) >= p.n_units) continue;
+        float* wrow = slice + (int64_t(unit_row[ul]) + (m % p.UW)) * p.Cout + nn0 + 2 * (lane & 3);   // row t*Cin + c
 #pragma unroll
         for (int j = 0; j < NW / 8; ++j)
           *reinterpret_cast<float2*>(wrow + 8 * j) = make_float2(acc[s][4 * j + 2 * h], acc[s][4 * j + 2 * h + 1]);
@@ -227,10 +271,19 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
 // Launch with the template arguments of the plan (operand format, wgmma N).
 static int launch_wgrad_kernel(const CUtensorMap& tmX, const CUtensorMap& tmG, const TcWgradParams& p, size_t smem,
                                dim3 grid, cudaStream_t st) {
-  const int nw = p.BN >= 64 ? 64 : p.BN;
-  auto pick = [&](auto k16, auto k32, auto k64) { return nw == 16 ? k16 : (nw == 32 ? k32 : k64); };
-  auto kern = p.fmt == BDBNN_FMT_BF16 ? pick(tc_wgrad_kernel<1, 16>, tc_wgrad_kernel<1, 32>, tc_wgrad_kernel<1, 64>)
-                                      : pick(tc_wgrad_kernel<0, 16>, tc_wgrad_kernel<0, 32>, tc_wgrad_kernel<0, 64>);
+  const int nw = p.BN, ns = nw >= 64 ? p.G : 0;
+  if (nw >= 64 && ns * nw > 256) { set_error("tc_wgrad_kernel: %d accumulators of %d columns", ns, nw); return BDBNN_ERR_UNSUPPORTED; }
+  using Kern = void (*)(CUtensorMap, CUtensorMap, TcWgradParams);
+  auto pick = [&](auto kind) -> Kern {
+    constexpr int K = decltype(kind)::value;
+    if (nw == 16) return tc_wgrad_kernel<K, 16, 0>;
+    if (nw == 32) return tc_wgrad_kernel<K, 32, 0>;
+    if (nw == 256) return tc_wgrad_kernel<K, 256, 1>;
+    if (nw == 128) return ns == 1 ? tc_wgrad_kernel<K, 128, 1> : tc_wgrad_kernel<K, 128, 2>;
+    return ns == 1 ? tc_wgrad_kernel<K, 64, 1> : ns == 2 ? tc_wgrad_kernel<K, 64, 2>
+                   : ns == 3 ? tc_wgrad_kernel<K, 64, 3> : tc_wgrad_kernel<K, 64, 4>;
+  };
+  Kern kern = p.fmt == BDBNN_FMT_BF16 ? pick(std::integral_constant<int, 1>()) : pick(std::integral_constant<int, 0>());
   BDBNN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
   kern<<<grid, kTcThreads, smem, st>>>(tmX, tmG, p);
   return check_launch("tc_wgrad_kernel");
@@ -272,12 +325,91 @@ struct WgradPlan {
   TcWgradParams p;
   int ksplit, ks_cap, mgroups, ntiles;
   size_t smem;
+  double l2_bytes;               // L2->shared-memory operand bytes of the launch (wgrad_l2_bytes)
   bool ok;
 };
 
+// Every (M group, N tile) column of CTAs loads each K stage once, whatever the split; TMA writes whole boxes.
+static double wgrad_l2_bytes(const WgradPlan& pl) {
+  const TcWgradParams& p = pl.p;
+  const double a_row = p.UW * 2, b_row = p.BN >= 64 ? 128 : p.BN * 2;
+  const int nb_boxes = (p.BN >= 64 ? p.BN / 64 : 1) * p.g_halves;
+  double per_stage = 0;
+  for (int mg = 0; mg < pl.mgroups; ++mg)
+    per_stage += wgrad_a_loads(p, mg) * p.rows_a * a_row + nb_boxes * p.rows_b * b_row;
+  return per_stage * pl.ntiles * p.n_kboxes;
+}
+
+// Shared-memory operand bytes the wgmmas of the launch read: per K step and warpgroup, each of the G accumulator
+// slots reads its 64-channel A unit and the N tile of gys (one wgmma of N = BN).
+static double wgrad_smem_read_bytes(const WgradPlan& pl) {
+  const TcWgradParams& p = pl.p;
+  const double per_step = 2.0 * p.G * (64 * 16 * 2 + p.BN * 16 * 2);
+  return per_step * (p.k_stage / 16) * p.g_halves * pl.mgroups * pl.ntiles * p.n_kboxes;
+}
+
+// Patch tilings are ranked by the L2->smem bytes plus 1/8 of the smem operand reads: with N = 64 wgmmas the gys
+// tile is read once per accumulator.  On an H100 80GB HBM3 (700 W) a patch tiling of the 14x14x256 layer with
+// BN = 128, G = 2 ran 0.51 ms per launch set against 0.65 ms with BN = 64, G = 4, although it moved 10 % more bytes
+// from L2 (and 30 % fewer from shared memory), while the 28x28x128 layer ran faster with BN = 64.
+static double wgrad_cost(const WgradPlan& pl) { return pl.l2_bytes + wgrad_smem_read_bytes(pl) / 8.0; }
+
 static WgradPlan plan_wgrad_small(const bdbnn_conv_shape* s, int halves);
 
+// Patch mode (file comment) on the K stages and split of `box`, or !ok where it does not apply.  Searches the N tile
+// and the M tiles per CTA for the lowest wgrad_cost, with a ring of at least 3 stages and no more CTA columns (M
+// groups x N tiles) than `box` has, so the launch stays within kWgradWaves waves.
+static WgradPlan plan_wgrad_patch(const bdbnn_conv_shape* s, int halves, const WgradPlan& box) {
+  WgradPlan best;
+  memset(&best, 0, sizeof(best));
+  const int T = s->kh * s->kw;
+  if (s->stride != 1 || T == 1 || box.p.UW != 64 || box.p.BNI != 1 || box.p.BH + s->kh - 1 > 256) return best;
+  const int chunks = s->Cin / 64, n_units = T * chunks, n_mtiles = (n_units + 1) / 2;
+  const uint32_t budget = 222u * 1024u;
+  for (int BN = 64; BN <= 256 && BN <= s->Cout; BN *= 2) {
+    if (s->Cout % BN) continue;
+    for (int G = 1; G * BN <= 256 && G <= n_mtiles; ++G) {
+      const int groups = (n_mtiles + G - 1) / G;
+      if ((n_mtiles + groups - 1) / groups != G) continue;       // balanced M groups only
+      if (groups * (s->Cout / BN) > box.mgroups * box.ntiles) continue;
+      WgradPlan pl = box;
+      TcWgradParams& p = pl.p;
+      p.patch = 1;
+      p.BN = BN; p.G = G;
+      p.rows_a = (p.BH + s->kh - 1) * p.BW;
+      // a view starts up to (kh-1)*Wo rows into its patch and reads k_stage rows
+      p.a_box_bytes = (uint32_t(p.k_stage + (s->kh - 1) * p.BW) * 128u + 1023u) & ~1023u;
+      p.b_box_bytes = uint32_t(p.k_stage) * 128u;
+      pl.mgroups = groups;
+      pl.ntiles = s->Cout / BN;
+      p.n_a_boxes = 0;
+      for (int mg = 0; mg < groups; ++mg) p.n_a_boxes = max(p.n_a_boxes, wgrad_a_loads(p, mg));
+      const size_t stage_bytes = size_t(p.n_a_boxes) * p.a_box_bytes + size_t(BN / 64 * halves) * p.b_box_bytes;
+      if (3 * stage_bytes > budget) continue;
+      int stages = int(budget / stage_bytes);
+      if (stages > kMaxStages) stages = kMaxStages;
+      if (stages > p.kboxes_per_cta) stages = p.kboxes_per_cta < 2 ? 2 : p.kboxes_per_cta;
+      p.stages = stages;
+      pl.smem = size_t(p.stages) * stage_bytes + 1024;
+      pl.l2_bytes = wgrad_l2_bytes(pl);
+      pl.ok = pl.smem <= 227u * 1024u;
+      if (pl.ok && (!best.ok || wgrad_cost(pl) < wgrad_cost(best))) best = pl;
+    }
+  }
+  return best;
+}
+
+static WgradPlan plan_wgrad_box(const bdbnn_conv_shape* s, int halves);
+
 static WgradPlan plan_wgrad(const bdbnn_conv_shape* s, int halves) {
+  const WgradPlan box = plan_wgrad_box(s, halves);
+  if (!box.ok || box.p.UW != 64) return box;
+  const WgradPlan patch = plan_wgrad_patch(s, halves, box);
+  return patch.ok && patch.l2_bytes < box.l2_bytes ? patch : box;
+}
+
+// Box mode: one [rows][64ch] box per unit (CIFAR widths: plan_wgrad_small).
+static WgradPlan plan_wgrad_box(const bdbnn_conv_shape* s, int halves) {
   WgradPlan pl;
   memset(&pl, 0, sizeof(pl));
   if (!s || (s->stride != 1 && s->stride != 2) || s->kh != s->kw || s->kh > 7 || s->pad > s->kh - 1) return pl;
@@ -355,6 +487,7 @@ static WgradPlan plan_wgrad(const bdbnn_conv_shape* s, int halves) {
   if (size_t(stages) * stage_bytes > budget) stages = 2;
   p.stages = stages;
   pl.smem = size_t(p.stages) * stage_bytes + 1024;
+  pl.l2_bytes = wgrad_l2_bytes(pl);
   pl.ok = pl.smem <= 227u * 1024u;
   return pl;
 }
@@ -417,6 +550,7 @@ static WgradPlan plan_wgrad_small(const bdbnn_conv_shape* s, int halves) {
   p.kboxes_per_cta = (p.n_kboxes + ks - 1) / ks;
   pl.ksplit = (p.n_kboxes + p.kboxes_per_cta - 1) / p.kboxes_per_cta;
   pl.smem = size_t(p.stages) * stage_bytes + 1024;
+  pl.l2_bytes = wgrad_l2_bytes(pl);
   pl.ok = p.stages >= 2 && pl.smem <= 227u * 1024u;
   return pl;
 }
@@ -510,6 +644,17 @@ extern "C" int bdbnn_debug_wgrad_plan(const bdbnn_conv_shape* s, int32_t grad_ha
   const int32_t v[12] = {pl.ok ? 1 : 0, pl.ksplit, pl.ks_cap, pl.mgroups, pl.ntiles, int32_t(pl.smem), pl.p.G, pl.p.BN,
                          pl.p.UW, 0, pl.p.k_stage, pl.p.stages};
   memcpy(out, v, sizeof(v));
+  if (n_out >= 16) {
+    out[12] = pl.p.patch;
+    out[13] = pl.p.patch ? pl.p.BW : 0;
+    out[14] = pl.p.patch ? pl.p.n_a_boxes : 0;
+    out[15] = int32_t((pl.l2_bytes + 1023.0) / 1024.0);
+  }
+  if (n_out >= 18) {
+    const WgradPlan box = plan_wgrad_box(s, grad_halves);
+    out[16] = int32_t((box.l2_bytes + 1023.0) / 1024.0);
+    out[17] = pl.p.kboxes_per_cta * pl.p.BNI * pl.p.BH * pl.p.OW;
+  }
   return BDBNN_OK;
 }
 
@@ -546,7 +691,10 @@ extern "C" int bdbnn_binconv_wgrad_tc(const uint16_t* gys_bf16, int32_t grad_mod
   pl.p.ws = static_cast<float*>(workspace);
   pl.p.trace = get_tc_trace();
   CUtensorMap tmX, tmG;
-  rc = make_act_map(&tmX, xb_bf16, s->N, s->H, s->W, s->Cin, pl.p.UW, pl.p.BW, pl.p.BH, pl.p.BNI, s->stride);
+  if (pl.p.patch)   // one patch: the kh boxes of a filter column, stacked
+    rc = make_act_map(&tmX, xb_bf16, s->N, s->H, s->W, s->Cin, 64, pl.p.BW, pl.p.BH + s->kh - 1, 1);
+  else
+    rc = make_act_map(&tmX, xb_bf16, s->N, s->H, s->W, s->Cin, pl.p.UW, pl.p.BW, pl.p.BH, pl.p.BNI, s->stride);
   if (rc) return rc;
   rc = make_act_map(&tmG, gys_bf16, s->N, s->Ho, s->Wo, s->Cout * grad_halves, pl.p.BN < 64 ? pl.p.BN : 64, pl.p.BW,
                     pl.p.BH, pl.p.BNI);

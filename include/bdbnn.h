@@ -224,8 +224,11 @@ BDBNN_API int bdbnn_debug_conv_plan(const bdbnn_conv_shape* s, int32_t mode, int
  * CUDA device; sets that kernel's maximum dynamic shared memory attribute to `smem` (every launch sets it again). */
 BDBNN_API int bdbnn_debug_tc_conv_ctas_per_sm(int32_t mode, int32_t fmt, int32_t bn, int32_t smem, int32_t* ctas);
 /* Host-only: the tiling bdbnn_binconv_wgrad_tc would use, for tests.  out[12] = {supported, ksplit, ks_cap,
- * m_groups, n_tiles, dynamic smem bytes, M tiles per CTA, N tile, unit width, halo mode, K rows per stage,
- * ring stages}.  Makes no CUDA call. */
+ * m_groups, n_tiles, dynamic smem bytes, M tiles per CTA, N tile, unit width, 0, K rows per stage,
+ * ring stages}.  With n_out >= 16 also out[12..15] = {operand mode (0 one box per tap, 1 one patch per channel
+ * chunk and filter column), patch width (0 in box mode), patches per stage (0 in box mode), L2->shared-memory operand
+ * KiB of the launch}; with n_out >= 18 also out[16] = the operand KiB of the box-mode plan of the same shape and
+ * out[17] = the longest fp32 accumulation chain of the launch in output pixels.  Makes no CUDA call. */
 BDBNN_API int bdbnn_debug_wgrad_plan(const bdbnn_conv_shape* s, int32_t grad_halves, int32_t* out, int32_t n_out);
 BDBNN_API int bdbnn_binconv_wgrad_tc(const uint16_t* gys, int32_t grad_mode, const uint32_t* amax_bits,
                            const uint16_t* xb, const uint32_t* wmask_bits, const float* inv_gscale,

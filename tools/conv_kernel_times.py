@@ -4,9 +4,11 @@
 
 Runs the step eagerly with functional.KernelTimer on for K steps after W warm-up steps and prints, per
 (family, shape key): ms per step, launches per step, TFLOP/s, compulsory HBM GB/s (functional.algorithmic_bytes),
-and the L2->shared-memory operand bytes the kernel's tiling implies (every CTA loads one activation box and one
-weight box per (tap, K block); a cluster of cm CTAs along M shares the weight box and of cn along N the activation
-box, as bdbnn_debug_conv_plan reports with BDBNN_TC_CLUSTER applied).  The card name, power limit and maximum SM
+and the L2->shared-memory operand bytes the kernel's tiling implies.  Forward / dgrad: every CTA loads one activation
+box and one weight box per (tap, K block); a cluster of cm CTAs along M shares the weight box and of cn along N the
+activation box, as bdbnn_debug_conv_plan reports with BDBNN_TC_CLUSTER applied.  Weight gradient: the bytes
+bdbnn_debug_wgrad_plan counts for the plan of the step's gradient mode (one box per tap, or one patch per channel
+chunk and filter column), with its operand mode, patch width and patches per stage.  The card name, power limit and maximum SM
 clock are read (read-only) from nvidia-smi.  Needs a CUDA device."""
 import argparse
 import ctypes
@@ -18,7 +20,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-FAMILIES = ("binconv_fwd_tc", "binconv_fwd_tc8", "binconv_dgrad_tc")
+FAMILIES = ("binconv_fwd_tc", "binconv_fwd_tc8", "binconv_dgrad_tc", "binconv_wgrad_tc")
 
 
 def parse_key(key):
@@ -35,6 +37,8 @@ def operand_bytes(L, fam, n, h, w, cin, cout, k, s):
     from bdbnn_b200.functional import conv_shape
     pad = k // 2
     sh = conv_shape((n, cin, h, w), (cout, cin, k, k), s, pad)
+    if fam == "binconv_wgrad_tc":
+        return wgrad_plan(L, sh)["l2_bytes"]
     mode = {"binconv_fwd_tc": 0, "binconv_fwd_tc8": 2, "binconv_dgrad_tc": 1}[fam]
     out = (ctypes.c_int32 * 14)()
     if L.bdbnn_debug_conv_plan(ctypes.byref(sh), mode, 1, out, 14) != 0 or not out[0]:
@@ -66,6 +70,15 @@ def operand_bytes(L, fam, n, h, w, cin, cout, k, s):
         iters = taps * n_kb
         total += ctas * iters * (bni * bh * ow * row / cn + bn * row / cm)
     return total
+
+
+def wgrad_plan(L, sh):
+    """Operand mode, patch width, patches per stage and L2->SMEM bytes of the wgrad launch in the step's mode."""
+    from bdbnn_b200.functional import grad_mode
+    out = (ctypes.c_int32 * 16)()
+    if L.bdbnn_debug_wgrad_plan(ctypes.byref(sh), grad_mode()[2], out, 16) != 0 or not out[0]:
+        return {"l2_bytes": None}
+    return {"mode": ("box", "patch")[out[12]], "PW": out[13], "patches": out[14], "l2_bytes": out[15] * 1024.0}
 
 
 def main():
@@ -111,11 +124,16 @@ def main():
         flop = 2.0 * n * ho * wo * cout * cin * k * k
         sec = d["ms"] / 1e3 / d["launches"]
         l2 = operand_bytes(L, fam, n, h, w, cin, cout, k, s)
-        rows.append({"family": fam, "key": key, "ms_per_step": round(d["ms"] / args.steps, 4),
-                     "launches_per_step": d["launches"] // args.steps, "tflops": round(flop / sec / 1e12, 1),
-                     "hbm_gbs": round(d["bytes"] / sec / 1e9, 1),
-                     "l2_smem_gb": round(l2 / 1e9, 3) if l2 is not None else None,
-                     "l2_smem_tbs": round(l2 / sec / 1e12, 2) if l2 is not None else None})
+        row = {"family": fam, "key": key, "ms_per_step": round(d["ms"] / args.steps, 4),
+               "launches_per_step": d["launches"] // args.steps, "tflops": round(flop / sec / 1e12, 1),
+               "hbm_gbs": round(d["bytes"] / sec / 1e9, 1),
+               "l2_smem_gb": round(l2 / 1e9, 3) if l2 is not None else None,
+               "l2_smem_tbs": round(l2 / sec / 1e12, 2) if l2 is not None else None}
+        if fam == "binconv_wgrad_tc":
+            from bdbnn_b200.functional import conv_shape
+            plan = wgrad_plan(L, conv_shape((n, cin, h, w), (cout, cin, k, k), s, k // 2))
+            row.update({key_: plan[key_] for key_ in ("mode", "PW", "patches") if key_ in plan})
+        rows.append(row)
     for r in sorted(rows, key=lambda r: (r["family"], -r["ms_per_step"])):
         print(json.dumps(r))
 
