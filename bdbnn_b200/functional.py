@@ -2,6 +2,7 @@
 
 PyTorch supplies device memory, streams and autograd bookkeeping only; every arithmetic step of the
 hot path is a kernel in libbdbnn_b200.so.  CUDA tensors are mandatory: CPU tensors raise."""
+import collections
 import ctypes
 import functools
 import os
@@ -173,6 +174,110 @@ def resolve_impl(impl, shape):
     return caps if (impl in ("auto", "tc") and (caps & 1)) else 0
 
 
+# act_pack of one activation: sign and mask bits [N,H,W,ceil(C/32)] int32, the 16-bit +-1 copy [N,H,W,C] in format
+# fmt, and its fp8 e4m3 copy (uint8); a copy that was not made is None
+_ActPack = collections.namedtuple("_ActPack", "sign mask xb fmt xb8")
+
+# bdbnn_weight_pack of one [Cout,Cin,kh,kw] weight; a buffer that was not requested is None (NULL to the kernel)
+_WeightPack = collections.namedtuple("_WeightPack", "alpha wsign wmask wf wf8 wt gscale inv_gscale")
+
+
+def _act_pack(x, sh, fmt, xb, xb8, have=None):
+    """act_pack of x (+ the 16-bit +-1 copy if `xb`), then bits_to_fp8 of its sign bits if `xb8`.
+    `have`: x's packs as its producer wrote them; then only a missing fp8 copy is made."""
+    L = _lib.lib()
+    n_pix = sh.N * sh.H * sh.W
+    st = _stream()
+    dev = x.device
+    if have is None:
+        cw = (sh.Cin + 31) // 32
+        have = _ActPack(torch.empty((sh.N, sh.H, sh.W, cw), dtype=torch.int32, device=dev),
+                        torch.empty((sh.N, sh.H, sh.W, cw), dtype=torch.int32, device=dev),
+                        torch.empty((sh.N, sh.H, sh.W, sh.Cin), dtype=torch.int16, device=dev) if xb else None,
+                        fmt, None)
+        with _timed("act_pack", _shape_key(sh), algorithmic_bytes("act_pack_tc" if xb else "act_pack", sh)):
+            _lib.check(L.bdbnn_act_pack(_p(_nhwc(x.detach())), n_pix, sh.Cin, _p(have.sign), _p(have.mask),
+                                        _p(have.xb), fmt, st), "act_pack")
+        _lib.count(1)
+    if xb8 and have.xb8 is None:
+        have = have._replace(xb8=torch.empty((sh.N, sh.H, sh.W, sh.Cin), dtype=torch.uint8, device=dev))
+        _lib.check(L.bdbnn_bits_to_fp8(_p(have.sign), n_pix, sh.Cin, _p(have.xb8), st), "bits_to_fp8")
+        _lib.count(1)
+    return have
+
+
+def _set_act_pack(z, pk):
+    """Attach z's packs for the next conv, stamped with z's version."""
+    z._bdbnn_pack = pk
+    z._bdbnn_pack_version = z._version
+
+
+def _get_act_pack(x, fmt):
+    """x's packs if they are in format fmt and describe x as it is (not modified in place since), else None."""
+    pk = getattr(x, "_bdbnn_pack", None)
+    if pk is not None and pk.fmt == fmt and getattr(x, "_bdbnn_pack_version", None) == x._version:
+        return pk
+    return None
+
+
+def _alloc_weight_pack(w_shape, dev, wf=False, wf8=False, grad=False):
+    """Buffers for bdbnn_weight_pack: alpha and the sign / mask bits always; the 16-bit (wf) and fp8 (wf8) forward
+    operands on request; with `grad` the transposed 16-bit operand and the gradient scales the backward reads."""
+    cout, cin, kh, kw = w_shape
+    T = kh * kw
+    f32 = dict(dtype=torch.float32, device=dev)
+    return _WeightPack(torch.empty((cout,), **f32),
+                       torch.empty((cout, T, (cin + 31) // 32), dtype=torch.int32, device=dev),
+                       torch.empty(((cout * cin * T + 31) // 32,), dtype=torch.int32, device=dev),
+                       torch.empty((cout, T, cin), dtype=torch.int16, device=dev) if wf else None,
+                       torch.empty((cout, T, cin), dtype=torch.uint8, device=dev) if wf8 else None,
+                       torch.empty((cin, T, cout), dtype=torch.int16, device=dev) if grad else None,
+                       torch.empty((cout,), **f32) if grad else None,
+                       torch.empty((cout,), **f32) if grad else None)
+
+
+def _weight_pack(weight, pk, fmt):
+    """bdbnn_weight_pack of `weight` into the buffers of pk (a _WeightPack)."""
+    cout, cin, kh, kw = weight.shape
+    _lib.check(_lib.lib().bdbnn_weight_pack(_p(weight.detach().contiguous()), cout, cin, kh, kw, _p(pk.alpha),
+                                            _p(pk.wsign), _p(pk.wmask), _p(pk.wf), _p(pk.wt), _p(pk.wf8),
+                                            _p(pk.gscale), _p(pk.inv_gscale), fmt, _stream()), "weight_pack")
+    _lib.count(2)
+
+
+def _wgrad_launch(launch, ws_bytes, w_shape, w_param, keep, family, key, nbytes):
+    """One weight-gradient GEMM: launch(gw pointer, workspace pointer, workspace bytes, stream) issues it.
+    Inside a wgrad_side scope (w_param given and eligible) it runs on the second stream into w_param's persistent
+    buffer and None is returned; otherwise it runs in line, timed, into a fresh gradient that is returned.
+    `keep`: the operands the kernel reads, referenced until the streams join (keep[0] gives the device)."""
+    dev = keep[0].device
+    sbuf = _WSIDE.target(w_param) if _WSIDE.active else None
+    gw = None
+    if sbuf is not None:
+        _WSIDE.keep.extend(t for t in keep if t is not None)
+        with torch.cuda.stream(_WSIDE.stream):
+            ws = torch.empty((max(ws_bytes, 4) // 4,), dtype=torch.float32, device=dev)
+            launch(_p(sbuf), _p(ws), ws_bytes, _stream())
+    else:
+        gw = torch.empty(w_shape, dtype=torch.float32, device=dev)
+        ws = torch.empty((max(ws_bytes, 4) // 4,), dtype=torch.float32, device=dev)
+        with _timed(family, key, nbytes):
+            launch(_p(gw), _p(ws), ws_bytes, _stream())
+    _lib.count(2)
+    return gw
+
+
+def _wgrad_tc(sh, gys, gcode, amax, xb, wmask, inv_gscale, w_shape, w_param, family, key, nbytes):
+    """bdbnn_binconv_wgrad_tc through _wgrad_launch."""
+    L = _lib.lib()
+    return _wgrad_launch(
+        lambda gw, ws, ws_bytes, st: _lib.check(L.bdbnn_binconv_wgrad_tc(
+            _p(gys), gcode, _p(amax), _p(xb), _p(wmask), _p(inv_gscale), gw, ctypes.byref(sh), ws, ws_bytes, st),
+            family),
+        int(L.bdbnn_wgrad_tc_workspace_bytes(ctypes.byref(sh))), w_shape, w_param,
+        (gys, amax, xb, wmask, inv_gscale), family, key, nbytes)
+
+
 class _BinConv2d(torch.autograd.Function):
     """y = alpha[o] * conv2d(sign(x), sign(W)) with STE backward (spec: DESIGN.md §2).
 
@@ -190,55 +295,29 @@ class _BinConv2d(torch.autograd.Function):
         sh = conv_shape(x.shape, weight.shape, stride, padding)
         use = resolve_impl(impl, sh)
         dev = x.device
-        xc = _nhwc(x.detach())
-        w = weight.detach().contiguous()
-        n, cin, h, wd = x.shape
-        cout, _, kh, kw = weight.shape
-        cw = (cin + 31) // 32
-        T = kh * kw
         st = _stream()
-        i32 = dict(dtype=torch.int32, device=dev)
-        sign_bits = torch.empty((n, h, wd, cw), **i32)
-        mask_bits = torch.empty((n, h, wd, cw), **i32)
         tc = bool(use & 1)
         gname, gcode, ghalves, fmt = grad_mode()
-        xb = torch.empty((n, h, wd, cin), dtype=torch.int16, device=dev) if tc else None
         key = _shape_key(sh)
-        with _timed("act_pack", key, algorithmic_bytes("act_pack_tc" if tc else "act_pack", sh)):
-            _lib.check(L.bdbnn_act_pack(_p(xc), n * h * wd, cin, _p(sign_bits), _p(mask_bits), _p(xb), fmt, st),
-                       "act_pack")
-        alpha = torch.empty((cout,), dtype=torch.float32, device=dev)
-        wsign = torch.empty((cout, T, cw), **i32)
-        wmask = torch.empty(((cout * cin * T + 31) // 32,), **i32)
-        wf = wt = gscale = inv_gscale = wf8 = xb8 = None
-        use8 = tc and bool(use & 8) and fwd8_enabled()
-        if use8:
-            wf8 = torch.empty((cout, T, cin), dtype=torch.uint8, device=dev)
-            xb8 = torch.empty((n, h, wd, cin), dtype=torch.uint8, device=dev)
-            _lib.check(L.bdbnn_bits_to_fp8(_p(sign_bits), n * h * wd, cin, _p(xb8), st), "bits_to_fp8")
-            _lib.count(1)
-        if tc:
-            wf = torch.empty((cout, T, cin), dtype=torch.int16, device=dev)
-            wt = torch.empty((cin, T, cout), dtype=torch.int16, device=dev)
-            gscale = torch.empty((cout,), dtype=torch.float32, device=dev)
-            inv_gscale = torch.empty((cout,), dtype=torch.float32, device=dev)
-        _lib.check(L.bdbnn_weight_pack(_p(w), cout, cin, kh, kw, _p(alpha), _p(wsign), _p(wmask),
-                                       _p(wf), _p(wt), _p(wf8), _p(gscale), _p(inv_gscale), fmt, st), "weight_pack")
-        y = torch.empty((n, cout, sh.Ho, sh.Wo), dtype=torch.float32, device=dev,
+        use8 = tc and bool(use & 8) and use_fwd8(sh.Cin, sh.Cout, eval_unit=False)
+        ap = _act_pack(x, sh, fmt, xb=tc, xb8=use8)
+        wp = _alloc_weight_pack(weight.shape, dev, wf=tc, wf8=use8, grad=tc)
+        _weight_pack(weight, wp, fmt)
+        y = torch.empty((sh.N, sh.Cout, sh.Ho, sh.Wo), dtype=torch.float32, device=dev,
                         memory_format=torch.channels_last)
         if use8:
             with _timed("binconv_fwd_tc8", key, algorithmic_bytes("fwd_tc8", sh)):
-                _lib.check(L.bdbnn_binconv_fwd_tc8(_p(xb8), _p(wf8), _p(alpha), _p(y), ctypes.byref(sh), None, None,
-                                                   st), "binconv_fwd_tc8")
+                _lib.check(L.bdbnn_binconv_fwd_tc8(_p(ap.xb8), _p(wp.wf8), _p(wp.alpha), _p(y), ctypes.byref(sh), None,
+                                                   None, st), "binconv_fwd_tc8")
         elif tc:
             with _timed("binconv_fwd_tc", key, algorithmic_bytes("fwd_tc", sh)):
-                _lib.check(L.bdbnn_binconv_fwd_tc(_p(xb), _p(wf), fmt, _p(alpha), _p(y), ctypes.byref(sh), None, None,
-                                                  st), "binconv_fwd_tc")
+                _lib.check(L.bdbnn_binconv_fwd_tc(_p(ap.xb), _p(wp.wf), fmt, _p(wp.alpha), _p(y), ctypes.byref(sh),
+                                                  None, None, st), "binconv_fwd_tc")
         else:
             with _timed("binconv_fwd_xnor", key, algorithmic_bytes("fwd_xnor", sh)):
-                _lib.check(L.bdbnn_binconv_fwd_xnor(_p(sign_bits), _p(wsign), _p(alpha), _p(y),
+                _lib.check(L.bdbnn_binconv_fwd_xnor(_p(ap.sign), _p(wp.wsign), _p(wp.alpha), _p(y),
                                                     ctypes.byref(sh), st), "binconv_fwd_xnor")
-        _lib.count(4)
+        _lib.count(1)
         ctx.sh = sh
         ctx.use = use
         ctx.gmode = (gname, gcode, ghalves)
@@ -246,6 +325,7 @@ class _BinConv2d(torch.autograd.Function):
         ctx.w_shape = tuple(weight.shape)
         ctx.w_param = weight if (weight.is_leaf and weight.requires_grad) else None
         ctx.ede = ede_k is not None
+        mask_bits, wmask = ap.mask, wp.wmask
         if ctx.ede:
             # EDE backward (train.py:409-415): soft-sign derivative needs the real values, and the
             # dgrad/wgrad kernels run with all-ones masks.
@@ -260,9 +340,10 @@ class _BinConv2d(torch.autograd.Function):
         else:
             ede_saved = ()
         if tc:
-            ctx.save_for_backward(sign_bits, mask_bits, wsign, wmask, alpha, xb, wt, gscale, inv_gscale, *ede_saved)
+            ctx.save_for_backward(ap.sign, mask_bits, wp.wsign, wmask, wp.alpha, ap.xb, wp.wt, wp.gscale,
+                                  wp.inv_gscale, *ede_saved)
         else:
-            ctx.save_for_backward(sign_bits, mask_bits, wsign, wmask, alpha, *ede_saved)
+            ctx.save_for_backward(ap.sign, mask_bits, wp.wsign, wmask, wp.alpha, *ede_saved)
         return y
 
     @staticmethod
@@ -297,45 +378,25 @@ class _BinConv2d(torch.autograd.Function):
                     _lib.check(L.bdbnn_binconv_dgrad_tc(_p(gys), gcode, _p(amax), _p(wt), _p(mask_bits), _p(None), _p(gx),
                                                         ctypes.byref(sh), st), "binconv_dgrad_tc")
                 _lib.count(_dgrad_launches(sh))
-            if need_w and not (ctx.use & 4):
-                # wgrad on CUDA cores from the saved sign bits (wgmma wgrad not available for this shape)
-                gw = torch.empty(ctx.w_shape, dtype=torch.float32, device=dev)
-                with _timed("binconv_wgrad_generic", key, algorithmic_bytes("wgrad", sh)):
-                    _lib.check(L.bdbnn_binconv_wgrad(_p(g), _p(sign_bits), _p(wmask), _p(gw),
-                                                     ctypes.byref(sh), st), "binconv_wgrad")
-                _lib.count(1)
-            elif need_w:
-                nbytes = int(L.bdbnn_wgrad_tc_workspace_bytes(ctypes.byref(sh)))
-                sbuf, sstream = (None, None) if ctx.ede else _side_launch(getattr(ctx, "w_param", None),
-                                                                          (gys, amax, xb, wmask, inv_gscale))
-                if sbuf is not None:      # wgrad_side scope: second stream, gw stays None
-                    with torch.cuda.stream(sstream):
-                        ws = torch.empty((max(nbytes, 4) // 4,), dtype=torch.float32, device=dev)
-                        _lib.check(L.bdbnn_binconv_wgrad_tc(_p(gys), gcode, _p(amax), _p(xb), _p(wmask), _p(inv_gscale),
-                                                            _p(sbuf), ctypes.byref(sh), _p(ws), nbytes, _stream()),
-                                   "binconv_wgrad_tc")
-                else:
-                    gw = torch.empty(ctx.w_shape, dtype=torch.float32, device=dev)
-                    ws = torch.empty((max(nbytes, 4) // 4,), dtype=torch.float32, device=dev)
-                    with _timed("binconv_wgrad_tc", key, algorithmic_bytes("wgrad_tc", sh, gh)):
-                        _lib.check(L.bdbnn_binconv_wgrad_tc(_p(gys), gcode, _p(amax), _p(xb), _p(wmask), _p(inv_gscale),
-                                                            _p(gw), ctypes.byref(sh), _p(ws), nbytes, st),
-                                   "binconv_wgrad_tc")
-                _lib.count(2)
-        else:
-            if need_x:
-                gx = torch.empty(ctx.x_shape, dtype=torch.float32, device=dev,
-                                 memory_format=torch.channels_last)
-                with _timed("binconv_dgrad_generic", key, algorithmic_bytes("dgrad", sh)):
-                    _lib.check(L.bdbnn_binconv_dgrad(_p(g), _p(wsign), _p(alpha), _p(mask_bits), _p(gx),
-                                                     ctypes.byref(sh), st), "binconv_dgrad")
-                _lib.count(1)
-            if need_w:
-                gw = torch.empty(ctx.w_shape, dtype=torch.float32, device=dev)
-                with _timed("binconv_wgrad_generic", key, algorithmic_bytes("wgrad", sh)):
-                    _lib.check(L.bdbnn_binconv_wgrad(_p(g), _p(sign_bits), _p(wmask), _p(gw),
-                                                     ctypes.byref(sh), st), "binconv_wgrad")
-                _lib.count(1)
+            if need_w and ctx.use & 4:
+                # EDE scales gw afterwards, so its wgrad stays in line (no w_param: never the second stream)
+                gw = _wgrad_tc(sh, gys, gcode, amax, xb, wmask, inv_gscale, ctx.w_shape,
+                               None if ctx.ede else ctx.w_param, "binconv_wgrad_tc", key,
+                               algorithmic_bytes("wgrad_tc", sh, gh))
+        elif need_x:
+            gx = torch.empty(ctx.x_shape, dtype=torch.float32, device=dev,
+                             memory_format=torch.channels_last)
+            with _timed("binconv_dgrad_generic", key, algorithmic_bytes("dgrad", sh)):
+                _lib.check(L.bdbnn_binconv_dgrad(_p(g), _p(wsign), _p(alpha), _p(mask_bits), _p(gx),
+                                                 ctypes.byref(sh), st), "binconv_dgrad")
+            _lib.count(1)
+        if need_w and not ctx.use & 4:
+            # wgrad on CUDA cores from the saved sign bits (no wgmma wgrad for this shape, or the xnor path)
+            gw = torch.empty(ctx.w_shape, dtype=torch.float32, device=dev)
+            with _timed("binconv_wgrad_generic", key, algorithmic_bytes("wgrad", sh)):
+                _lib.check(L.bdbnn_binconv_wgrad(_p(g), _p(sign_bits), _p(wmask), _p(gw),
+                                                 ctypes.byref(sh), st), "binconv_wgrad")
+            _lib.count(1)
         if ctx.ede:
             xv, wv, ek, et = saved[-4:]
             xv, wv = _nhwc(xv.detach()), wv.detach().contiguous()
@@ -600,6 +661,16 @@ def fwd8_enabled():
     return os.environ.get(_FWD8_ENV, "1") != "0"
 
 
+def use_fwd8(cin, cout, eval_unit):
+    """Whether a binary conv runs its forward on fp8 operands: BDBNN_FWD8 on and a shape the fp8 kernel takes
+    (Cin % 128 == 0, Cout 64 or a multiple of 128: bdbnn_tc_supported's BDBNN_TC_FWD8, which the units check too).
+    An eval unit also needs Cout % 128 == 0, since it writes the 16-bit +-1 copy of z only from 16-bit operands and
+    that copy is fp8 only for Cout % 128 == 0.  prepack_weights is given the same answer as the unit."""
+    if not fwd8_enabled() or cin % 128:
+        return False
+    return cout % 128 == 0 or (cout == 64 and not eval_unit)
+
+
 def conv_stats_enabled():
     return os.environ.get("BDBNN_CONV_STATS", "1") != "0"
 
@@ -628,8 +699,8 @@ def prepack_enabled():
 
 def prepack_weights(items):
     """items: list of (weight [Cout,Cin,kh,kw] CUDA fp32, use8) for the binary convs of one forward pass.
-    Returns {weight.data_ptr(): (version, fmt, use8, w, alpha, wsign, wmask, wf, wf8, wt, gscale, inv_gscale)} — the
-    tensors `_ConvBNAddUnit` would otherwise produce itself with one bdbnn_weight_pack call per layer."""
+    Returns {weight.data_ptr(): _Prepacked} — the operands (wf or wf8, wt and the gradient scales) `_ConvBNAddUnit`
+    would otherwise pack itself with one bdbnn_weight_pack call per layer."""
     if not items:
         return {}
     L = _lib.lib()
@@ -639,34 +710,40 @@ def prepack_weights(items):
     ws, packs = [], []
     for weight, use8 in items:
         _require_cuda(weight, "prepack_weights")
-        w = weight.detach().contiguous()
-        cout, cin, kh, kw = w.shape
-        T, cw = kh * kw, (cin + 31) // 32
-        if (cin * T) % 32:
+        _, cin, kh, kw = weight.shape
+        if (cin * kh * kw) % 32:
             raise RuntimeError("prepack_weights: Cin*kh*kw must be a multiple of 32")
-        i32 = dict(dtype=torch.int32, device=dev)
-        f32 = dict(dtype=torch.float32, device=dev)
-        alpha, gscale, inv_gscale = torch.empty((cout,), **f32), torch.empty((cout,), **f32), torch.empty((cout,), **f32)
-        wsign = torch.empty((cout, T, cw), **i32)
-        wmask = torch.empty(((cout * cin * T + 31) // 32,), **i32)
-        wf = torch.empty((cout, T, cin), dtype=torch.int16, device=dev) if not use8 else None
-        wf8 = torch.empty((cout, T, cin), dtype=torch.uint8, device=dev) if use8 else None
-        wt = torch.empty((cin, T, cout), dtype=torch.int16, device=dev)
-        ws.append(w)
-        packs.append((alpha, wsign, wmask, wf, wf8, wt, gscale, inv_gscale))
+        ws.append(weight.detach().contiguous())
+        packs.append(_alloc_weight_pack(weight.shape, dev, wf=not use8, wf8=use8, grad=True))
     P = ctypes.c_void_p * n
     I = ctypes.c_int32 * n
-    ptrs = lambda k: P(*[(p[k].data_ptr() if p[k] is not None else 0) for p in packs])
+
+    def ptrs(field):
+        return P(*[(t.data_ptr() if t is not None else 0) for t in (getattr(p, field) for p in packs)])
     _lib.check(L.bdbnn_weight_pack_multi(
         n, P(*[w.data_ptr() for w in ws]), I(*[w.shape[0] for w in ws]), I(*[w.shape[1] for w in ws]),
-        I(*[w.shape[2] * w.shape[3] for w in ws]), ptrs(0), ptrs(1), ptrs(2), ptrs(3), ptrs(5), ptrs(4), ptrs(6), ptrs(7),
-        fmt, _stream()), "weight_pack_multi")
+        I(*[w.shape[2] * w.shape[3] for w in ws]),
+        *map(ptrs, ("alpha", "wsign", "wmask", "wf", "wt", "wf8", "gscale", "inv_gscale")), fmt, _stream()),
+        "weight_pack_multi")
     _lib.count(2 * ((n + 31) // 32))
-    return {weight.data_ptr(): (weight._version, fmt, bool(use8), w) + pk
+    return {weight.data_ptr(): _Prepacked(weight._version, fmt, bool(use8), w, *pk)
             for (weight, use8), w, pk in zip(items, ws, packs)}
 
 
+# one prepack_weights entry: the guard (weight version, fmt, use8), the contiguous weight that was packed, then the
+# _WeightPack fields
+_Prepacked = collections.namedtuple("_Prepacked", ("version", "fmt", "use8", "w") + _WeightPack._fields)
+
 _PREPACKED = {}     # filled by the network shells for the duration of one forward pass (same thread)
+
+
+def _prepacked(weight, fmt, use8):
+    """The _WeightPack prepack_weights made for `weight` in this forward, or None if there is none for its current
+    version, fmt and operand width."""
+    pre = _PREPACKED.get(weight.data_ptr())
+    if pre is None or (pre.version, pre.fmt, pre.use8) != (weight._version, fmt, use8):
+        return None
+    return _WeightPack._make(getattr(pre, f) for f in _WeightPack._fields)
 
 
 def wgrad_side_enabled():
@@ -709,6 +786,14 @@ class _WgradSide:
 _WSIDE = _WgradSide()
 
 
+def _side_stream():
+    """The second stream of the current device, shared by the wgrad_side and forward_side scopes.
+    BDBNN_SIDE_PRIO: its CUDA priority (0 = lowest = default, -1 = above the default)."""
+    if _WSIDE.stream is None or _WSIDE.stream.device != torch.device("cuda", torch.cuda.current_device()):
+        _WSIDE.stream = torch.cuda.Stream(priority=int(os.environ.get("BDBNN_SIDE_PRIO", "0")))
+    return _WSIDE.stream
+
+
 class wgrad_side:
     """Scope (bdbnn_b200.step.TrainStep wraps `loss.backward()` in it) in which the weight gradients of the binary
     convs, the 1x1 shortcuts and the stem are computed on a SECOND stream: nothing in the backward chain consumes
@@ -730,9 +815,7 @@ class wgrad_side:
         if self.enable:
             if _WSIDE.active:
                 raise RuntimeError("wgrad_side scopes do not nest")
-            if _WSIDE.stream is None or _WSIDE.stream.device != torch.device("cuda", torch.cuda.current_device()):
-                # BDBNN_SIDE_PRIO: CUDA priority of the second stream (0 = lowest = default, -1 = above the default)
-                _WSIDE.stream = torch.cuda.Stream(priority=int(os.environ.get("BDBNN_SIDE_PRIO", "0")))
+            _side_stream()
             _WSIDE.used, _WSIDE.keep, _WSIDE.sink, _WSIDE.active = [], [], self.sink, True
         return self
 
@@ -764,12 +847,6 @@ class _FwdSide:
     def __init__(self):
         self.active = False
 
-    def stream(self):
-        dev = torch.device("cuda", torch.cuda.current_device())
-        if _WSIDE.stream is None or _WSIDE.stream.device != dev:
-            _WSIDE.stream = torch.cuda.Stream(priority=int(os.environ.get("BDBNN_SIDE_PRIO", "0")))
-        return _WSIDE.stream
-
 
 _FWD_SIDE = _FwdSide()
 
@@ -790,15 +867,6 @@ class forward_side:
     def __exit__(self, *exc):
         _FWD_SIDE.active = self.prev
         return False
-
-
-def _side_launch(param, keep):
-    """(gradient buffer, torch stream) for a wgrad on the side stream, or (None, None): run it in line."""
-    buf = _WSIDE.target(param) if _WSIDE.active else None
-    if buf is None:
-        return None, None
-    _WSIDE.keep.extend(t for t in keep if t is not None)
-    return buf, _WSIDE.stream
 
 
 def unit_supported(x_shape, w_shape, stride, padding):
@@ -828,7 +896,7 @@ class _ConvBNAddUnit(torch.autograd.Function):
                 # step scope (TrainStep): the shortcut branch depends only on x — run it on the second stream under the
                 # main conv; the streams join before bn_fwd reads the residual.  (Every side section starts by waiting
                 # for the main stream, which is what makes recycling of side-pool blocks safe.)
-                sc_join = _FWD_SIDE.stream()
+                sc_join = _side_stream()
                 sc_join.wait_stream(torch.cuda.current_stream())
                 with torch.cuda.stream(sc_join):
                     residual, sc_saved, ctx.sc_geom = _shortcut_fwd_impl(x, sc_weight, sc_gamma, sc_beta, sc_rm, sc_rv,
@@ -848,46 +916,22 @@ class _ConvBNAddUnit(torch.autograd.Function):
                 getattr(x, "_bdbnn_pack_version", None) == x._version and x.shape[1] <= 512):
             ctx.prod_bn = prod
         dev = x.device
-        n, cin, h, wd = x.shape
-        cout, _, kh, kw = weight.shape
-        cw, T = (cin + 31) // 32, kh * kw
+        n, cout = sh.N, sh.Cout
         st = _stream()
         gname, gcode, ghalves, fmt = grad_mode()
         key = _shape_key(sh)
         i32 = dict(dtype=torch.int32, device=dev)
         caps = int(L.bdbnn_tc_supported(ctypes.byref(sh)))
-        use8 = bool(caps & 8) and fwd8_enabled()
-        if xs is None:
-            xc = _nhwc(x.detach())
-            xs = torch.empty((n, h, wd, cw), **i32)
-            xm = torch.empty((n, h, wd, cw), **i32)
-            xb = torch.empty((n, h, wd, cin), dtype=torch.int16, device=dev)
-            with _timed("act_pack", key, algorithmic_bytes("act_pack_tc", sh)):
-                _lib.check(L.bdbnn_act_pack(_p(xc), n * h * wd, cin, _p(xs), _p(xm), _p(xb), fmt, st), "act_pack")
-            _lib.count(1)
-            xb8 = None
-        if use8 and xb8 is None:
-            xb8 = torch.empty((n, h, wd, cin), dtype=torch.uint8, device=dev)
-            _lib.check(L.bdbnn_bits_to_fp8(_p(xs), n * h * wd, cin, _p(xb8), st), "bits_to_fp8")
-            _lib.count(1)
-        pre = _PREPACKED.get(weight.data_ptr())
-        if pre is not None and pre[0] == weight._version and pre[1] == fmt and pre[2] == use8:
-            # packed with every other binary conv of the network at the start of this forward (prepack_weights)
-            w, alpha, wsign, wmask, wf, wf8, wt, gscale, inv_gscale = pre[3:]
-            n_wpack = 0
-        else:
-            w = weight.detach().contiguous()
-            alpha = torch.empty((cout,), dtype=torch.float32, device=dev)
-            wsign = torch.empty((cout, T, cw), **i32)
-            wmask = torch.empty(((cout * cin * T + 31) // 32,), **i32)
-            wf = torch.empty((cout, T, cin), dtype=torch.int16, device=dev) if not use8 else None
-            wf8 = torch.empty((cout, T, cin), dtype=torch.uint8, device=dev) if use8 else None
-            wt = torch.empty((cin, T, cout), dtype=torch.int16, device=dev)
-            gscale = torch.empty((cout,), dtype=torch.float32, device=dev)
-            inv_gscale = torch.empty((cout,), dtype=torch.float32, device=dev)
-            _lib.check(L.bdbnn_weight_pack(_p(w), cout, cin, kh, kw, _p(alpha), _p(wsign), _p(wmask), _p(wf), _p(wt),
-                                           _p(wf8), _p(gscale), _p(inv_gscale), fmt, st), "weight_pack")
-            n_wpack = 2
+        use8 = bool(caps & 8) and use_fwd8(sh.Cin, cout, eval_unit=False)
+        ap = _act_pack(x, sh, fmt, xb=True, xb8=use8,
+                       have=None if xs is None else _ActPack(xs, xm, xb, fmt, xb8))
+        xm, xb, xb8 = ap.mask, ap.xb, ap.xb8
+        # packed with every other binary conv of the network at the start of this forward (prepack_weights)
+        wp = _prepacked(weight, fmt, use8)
+        if wp is None:
+            wp = _alloc_weight_pack(weight.shape, dev, wf=not use8, wf8=use8, grad=True)
+            _weight_pack(weight, wp, fmt)
+        alpha = wp.alpha
         # BN batch statistics of y are accumulated by the conv kernel's epilogue (BDBNN_CONV_STATS=0: separate pass)
         sums = torch.empty((2 * cout,), dtype=torch.float64, device=dev)
         ymax = torch.empty((cout,), **i32)
@@ -898,7 +942,7 @@ class _ConvBNAddUnit(torch.autograd.Function):
             y = torch.empty((n, sh.Ho, sh.Wo, cout), dtype=torch.int16, device=dev)
             with _timed("binconv_fwd_tc8" if use8 else "binconv_fwd_tc", key,
                         algorithmic_bytes("fwd_tc8" if use8 else "fwd_tc", sh) - 2 * y.numel()):
-                _lib.check(L.bdbnn_binconv_fwd_tc_i16(_p(xb8) if use8 else _p(xb), _p(wf8) if use8 else _p(wf),
+                _lib.check(L.bdbnn_binconv_fwd_tc_i16(_p(xb8) if use8 else _p(xb), _p(wp.wf8) if use8 else _p(wp.wf),
                                                       -1 if use8 else fmt, _p(alpha), _p(y), ctypes.byref(sh), s_ptr,
                                                       m_ptr, st), "binconv_fwd_tc_i16")
         else:
@@ -906,13 +950,13 @@ class _ConvBNAddUnit(torch.autograd.Function):
                             memory_format=torch.channels_last)
             if use8:
                 with _timed("binconv_fwd_tc8", key, algorithmic_bytes("fwd_tc8", sh)):
-                    _lib.check(L.bdbnn_binconv_fwd_tc8(_p(xb8), _p(wf8), _p(alpha), _p(y), ctypes.byref(sh), s_ptr,
+                    _lib.check(L.bdbnn_binconv_fwd_tc8(_p(xb8), _p(wp.wf8), _p(alpha), _p(y), ctypes.byref(sh), s_ptr,
                                                        m_ptr, st), "binconv_fwd_tc8")
             else:
                 with _timed("binconv_fwd_tc", key, algorithmic_bytes("fwd_tc", sh)):
-                    _lib.check(L.bdbnn_binconv_fwd_tc(_p(xb), _p(wf), fmt, _p(alpha), _p(y), ctypes.byref(sh), s_ptr,
-                                                      m_ptr, st), "binconv_fwd_tc")
-        _lib.count(1 + n_wpack)
+                    _lib.check(L.bdbnn_binconv_fwd_tc(_p(xb), _p(wp.wf), fmt, _p(alpha), _p(y), ctypes.byref(sh),
+                                                      s_ptr, m_ptr, st), "binconv_fwd_tc")
+        _lib.count(1)
         n_pix = n * sh.Ho * sh.Wo
         if res_is_x:            # identity shortcut: the residual IS the conv input (one autograd edge)
             rc = _nhwc(x.detach())
@@ -951,8 +995,8 @@ class _ConvBNAddUnit(torch.autograd.Function):
         ctx.sc_w_param = sc_weight if (sc_weight is not None and sc_weight.is_leaf and sc_weight.requires_grad) else None
         ctx.has_res = residual is not None and sc_weight is None
         ctx.res_is_x = bool(res_is_x)
-        ctx.save_for_backward(y, mean, invstd, gamma.detach(), ymax, xm, xb, wt, wmask, gscale, inv_gscale, alpha,
-                              *sc_saved)
+        ctx.save_for_backward(y, mean, invstd, gamma.detach(), ymax, xm, xb, wp.wt, wp.wmask, wp.gscale, wp.inv_gscale,
+                              alpha, *sc_saved)
         _ConvBNAddUnit._last_bnctx = ctx.bnctx_out       # picked up by conv_bn_add right after apply() (same thread)
         if pack:
             if zb8 is not None:
@@ -1007,21 +1051,8 @@ class _ConvBNAddUnit(torch.autograd.Function):
         gx = gw = None
         # the weight gradient first: in a wgrad_side scope it forks off here and overlaps this unit's dgrad as well
         if ctx.needs_input_grad[1]:
-            nbytes = int(L.bdbnn_wgrad_tc_workspace_bytes(ctypes.byref(sh)))
-            sbuf, sstream = _side_launch(ctx.w_param, (gys, amax, xb, wmask, inv_gscale))
-            if sbuf is not None:          # wgrad_side scope: second stream, persistent gradient buffer, gw stays None
-                with torch.cuda.stream(sstream):
-                    ws = torch.empty((max(nbytes, 4) // 4,), dtype=torch.float32, device=dev)
-                    _lib.check(L.bdbnn_binconv_wgrad_tc(_p(gys), gcode, _p(amax), _p(xb), _p(wmask), _p(inv_gscale),
-                                                        _p(sbuf), ctypes.byref(sh), _p(ws), nbytes, _stream()),
-                               "binconv_wgrad_tc")
-            else:
-                gw = torch.empty(w_shape, dtype=torch.float32, device=dev)
-                ws = torch.empty((max(nbytes, 4) // 4,), dtype=torch.float32, device=dev)
-                with _timed("binconv_wgrad_tc", key, algorithmic_bytes("wgrad_tc", sh, gh)):
-                    _lib.check(L.bdbnn_binconv_wgrad_tc(_p(gys), gcode, _p(amax), _p(xb), _p(wmask), _p(inv_gscale),
-                                                        _p(gw), ctypes.byref(sh), _p(ws), nbytes, st), "binconv_wgrad_tc")
-            _lib.count(2)
+            gw = _wgrad_tc(sh, gys, gcode, amax, xb, wmask, inv_gscale, w_shape, ctx.w_param, "binconv_wgrad_tc", key,
+                           algorithmic_bytes("wgrad_tc", sh, gh))
         if ctx.needs_input_grad[0]:
             gx = torch.empty(x_shape, dtype=torch.float32, device=dev, memory_format=torch.channels_last)
             done = False
@@ -1067,15 +1098,11 @@ def conv_bn_add(x, weight, gamma, beta, residual, running_mean, running_var, mom
     """z = BN_train(binconv2d(x, weight)) + residual on the fused kernels.  `shortcut` = (weight[Cout,Cin,1,1],
     gamma, beta, running_mean, running_var, momentum, eps, stride) evaluates the real-valued 1x1 conv + BN
     `downsample` branch of x inside the same node and uses it as the residual.  The returned tensor carries
-    `_bdbnn_pack` = (sign bits, mask bits, +-1 copy, fmt) of z so that a following conv_bn_add skips its
+    `_bdbnn_pack` = (sign bits, mask bits, +-1 copy, fmt, fp8 copy) of z so that a following conv_bn_add skips its
     own activation pack; x's own `_bdbnn_pack` (if present and of the current format) is consumed."""
     fmt = grad_mode()[3]
-    pk = getattr(x, "_bdbnn_pack", None)
-    xs = xm = xb = xb8 = None
-    # the packs describe x as it was when its producer wrote it: ignore them if x was modified in place since
-    if pk is not None and pk[3] == fmt and getattr(x, "_bdbnn_pack_version", None) == x._version:
-        xs, xm, xb = pk[:3]
-        xb8 = pk[4] if len(pk) > 4 else None
+    pk = _get_act_pack(x, fmt)
+    xs, xm, xb, xb8 = (pk.sign, pk.mask, pk.xb, pk.xb8) if pk is not None else (None,) * 4
     res_is_x = residual is x and x.shape[1] == weight.shape[0] and int(stride) == 1
     if shortcut is not None:
         if residual is not None:
@@ -1087,8 +1114,7 @@ def conv_bn_add(x, weight, gamma, beta, residual, running_mean, running_var, mom
                                                   running_mean, running_var, momentum, eps, int(stride),
                                                   int(padding), xs, xm, xb, xb8, res_is_x)
     if zs is not None:
-        z._bdbnn_pack = (zs, zm, zb, fmt, zb8)
-        z._bdbnn_pack_version = z._version
+        _set_act_pack(z, _ActPack(zs, zm, zb, fmt, zb8))
         z._bdbnn_bnctx = _ConvBNAddUnit._last_bnctx      # (y_int, alpha, mean, invstd) of this unit, or None
     _ConvBNAddUnit._last_bnctx = None
     return z
@@ -1191,21 +1217,8 @@ def _shortcut_bwd_impl(gz, saved, geom, need_x, need_w, acc=None, w_param=None):
         _lib.count(_dgrad_launches(shs))
     if need_w:
         wones = torch.full(((cout * cin + 31) // 32,), -1, **i32)
-        nbytes = int(L.bdbnn_wgrad_tc_workspace_bytes(ctypes.byref(sh1)))
-        sbuf, sstream = _side_launch(w_param, (gys, amax, xh, wones, inv_gscale))
-        if sbuf is not None:              # wgrad_side scope: second stream, gw stays None
-            with torch.cuda.stream(sstream):
-                ws = torch.empty((max(nbytes, 4) // 4,), **f32)
-                _lib.check(L.bdbnn_binconv_wgrad_tc(_p(gys), 3, _p(amax), _p(xh), _p(wones), _p(inv_gscale), _p(sbuf),
-                                                    ctypes.byref(sh1), _p(ws), nbytes, _stream()),
-                           "binconv_wgrad_tc(shortcut)")
-        else:
-            gw = torch.empty(w_shape, **f32)
-            ws = torch.empty((max(nbytes, 4) // 4,), **f32)
-            with _timed("shortcut_wgrad_tc", key, 2 * gys.numel() + 2 * xh.numel()):
-                _lib.check(L.bdbnn_binconv_wgrad_tc(_p(gys), 3, _p(amax), _p(xh), _p(wones), _p(inv_gscale), _p(gw),
-                                                    ctypes.byref(sh1), _p(ws), nbytes, st), "binconv_wgrad_tc(shortcut)")
-        _lib.count(2)
+        gw = _wgrad_tc(sh1, gys, 3, amax, xh, wones, inv_gscale, w_shape, w_param, "shortcut_wgrad_tc", key,
+                       2 * gys.numel() + 2 * xh.numel())
     return gx, gw, dgamma, dbeta
 
 
@@ -1390,23 +1403,11 @@ def _stem_conv_fwd_impl(x, weight, want_stats=False):
 
 def _stem_wgrad_impl(gys, g_amax, xw, x_amax, n, h, w, w_param=None):
     L = _lib.lib()
-    dev = gys.device
-    nbytes = int(L.bdbnn_stem_wgrad_workspace_bytes(n, h, w))
-    sbuf, sstream = _side_launch(w_param, (gys, g_amax, xw, x_amax))
-    if sbuf is not None:                  # wgrad_side scope: second stream, the caller returns no gradient
-        with torch.cuda.stream(sstream):
-            ws = torch.empty((max(nbytes, 4) // 4,), dtype=torch.float32, device=dev)
-            _lib.check(L.bdbnn_stem_conv_wgrad(_p(gys), _p(g_amax), _p(xw), _p(x_amax), _p(sbuf), n, h, w,
-                                               _p(ws), nbytes, _stream()), "stem_conv_wgrad")
-        _lib.count(2)
-        return None
-    gw = torch.empty((64, 3, 7, 7), dtype=torch.float32, device=dev)
-    ws = torch.empty((max(nbytes, 4) // 4,), dtype=torch.float32, device=dev)
-    with _timed("stem_conv_wgrad", f"stem_N{n}_{h}x{w}", 2 * gys.numel() + xw.numel() * 2):
-        _lib.check(L.bdbnn_stem_conv_wgrad(_p(gys), _p(g_amax), _p(xw), _p(x_amax), _p(gw), n, h, w,
-                                           _p(ws), nbytes, _stream()), "stem_conv_wgrad")
-    _lib.count(2)
-    return gw
+    return _wgrad_launch(
+        lambda gw, ws, ws_bytes, st: _lib.check(L.bdbnn_stem_conv_wgrad(
+            _p(gys), _p(g_amax), _p(xw), _p(x_amax), gw, n, h, w, ws, ws_bytes, st), "stem_conv_wgrad"),
+        int(L.bdbnn_stem_wgrad_workspace_bytes(n, h, w)), (64, 3, 7, 7), w_param, (gys, g_amax, xw, x_amax),
+        "stem_conv_wgrad", f"stem_N{n}_{h}x{w}", 2 * gys.numel() + xw.numel() * 2)
 
 
 class _StemConv(torch.autograd.Function):
@@ -1479,8 +1480,7 @@ def stem_conv_bn_pool(x, weight, gamma, beta, running_mean, running_var, momentu
     z, zs, zm, zb, zb8 = _StemFused.apply(x, weight, gamma, beta, running_mean, running_var, momentum, eps,
                                           int(kernel_size), int(stride), int(padding))
     if zs is not None:
-        z._bdbnn_pack = (zs, zm, zb, grad_mode()[3], zb8)
-        z._bdbnn_pack_version = z._version
+        _set_act_pack(z, _ActPack(zs, zm, zb, grad_mode()[3], zb8))
     return z
 
 
@@ -1496,8 +1496,7 @@ def stem_bn_pool(y, gamma, beta, running_mean, running_var, momentum, eps, kerne
     z, zs, zm, zb, zb8 = _StemBNPool.apply(y, gamma, beta, running_mean, running_var, momentum, eps,
                                            int(kernel_size), int(stride), int(padding))
     if zs is not None:
-        z._bdbnn_pack = (zs, zm, zb, grad_mode()[3], zb8)
-        z._bdbnn_pack_version = z._version
+        _set_act_pack(z, _ActPack(zs, zm, zb, grad_mode()[3], zb8))
     return z
 
 
@@ -1550,12 +1549,6 @@ def eval_unit_supported(x_shape, w_shape, stride, padding):
     return bool(int(_lib.lib().bdbnn_tc_supported(ctypes.byref(sh))) & 1)
 
 
-def eval_use8(cin, cout):
-    """fp8 operands for an eval unit: the fp8 forward exists (Cin % 128 == 0) and z's +-1 copy is fp8 too
-    (Cout % 128 == 0), since the eval kernel writes the 16-bit copy only from 16-bit operands."""
-    return fwd8_enabled() and cin % 128 == 0 and cout % 128 == 0
-
-
 @_on_x_device
 def conv_bn_add_eval(x, weight, gamma, beta, running_mean, running_var, eps, stride, padding, residual,
                      shortcut=None):
@@ -1578,8 +1571,7 @@ def conv_bn_add_eval(x, weight, gamma, beta, running_mean, running_var, eps, str
     if not caps & 1:
         raise RuntimeError("bdbnn_b200.conv_bn_add_eval: the wgmma forward does not support this shape")
     dev = x.device
-    n, cin, h, wd = x.shape
-    cout, _, kh, kw = weight.shape
+    n, cout = sh.N, sh.Cout
     z_shape = (n, cout, sh.Ho, sh.Wo)
     if residual is not None and tuple(residual.shape) != z_shape:
         raise RuntimeError(f"conv_bn_add_eval: residual shape {tuple(residual.shape)} != output shape {z_shape}")
@@ -1588,38 +1580,20 @@ def conv_bn_add_eval(x, weight, gamma, beta, running_mean, running_var, eps, str
     key = _shape_key(sh)
     pack = cout % 32 == 0
     out8 = pack and cout % 128 == 0 and fwd8_enabled()
-    use8 = bool(caps & 8) and eval_use8(cin, cout)
+    use8 = bool(caps & 8) and use_fwd8(sh.Cin, cout, eval_unit=True)
     want = -1 if use8 else fmt
     pk = getattr(x, "_bdbnn_eval_pack", None)
     if pk is not None and pk[0] == want and x._bdbnn_eval_pack_version == x._version:
         xop = pk[1]
     else:
-        cw = (cin + 31) // 32
-        xs = torch.empty((n, h, wd, cw), dtype=torch.int32, device=dev)
-        xm = torch.empty((n, h, wd, cw), dtype=torch.int32, device=dev)
-        xb = torch.empty((n, h, wd, cin), dtype=torch.int16, device=dev) if not use8 else None
-        with _timed("act_pack", key, algorithmic_bytes("act_pack" if use8 else "act_pack_tc", sh)):
-            _lib.check(L.bdbnn_act_pack(_p(_nhwc(x.detach())), n * h * wd, cin, _p(xs), _p(xm), _p(xb), fmt, st),
-                       "act_pack")
-        _lib.count(1)
-        xop = xb
-        if use8:
-            xop = torch.empty((n, h, wd, cin), dtype=torch.uint8, device=dev)
-            _lib.check(L.bdbnn_bits_to_fp8(_p(xs), n * h * wd, cin, _p(xop), st), "bits_to_fp8")
-            _lib.count(1)
-    pre = _PREPACKED.get(weight.data_ptr())
-    if pre is not None and pre[0] == weight._version and pre[1] == fmt and pre[2] == use8:
-        alpha, wop = pre[4], (pre[8] if use8 else pre[7])     # packed with every binary conv (prepack_weights)
-    else:
-        T, cw = kh * kw, (cin + 31) // 32
-        alpha = torch.empty((cout,), dtype=torch.float32, device=dev)
-        wsign = torch.empty((cout, T, cw), dtype=torch.int32, device=dev)
-        wmask = torch.empty(((cout * cin * T + 31) // 32,), dtype=torch.int32, device=dev)
-        wop = torch.empty((cout, T, cin), dtype=torch.uint8 if use8 else torch.int16, device=dev)
-        _lib.check(L.bdbnn_weight_pack(_p(weight.detach().contiguous()), cout, cin, kh, kw, _p(alpha), _p(wsign),
-                                       _p(wmask), None if use8 else _p(wop), None, _p(wop) if use8 else None, None,
-                                       None, fmt, st), "weight_pack")
-        _lib.count(2)
+        ap = _act_pack(x, sh, fmt, xb=not use8, xb8=use8)
+        xop = ap.xb8 if use8 else ap.xb
+    # packed with every binary conv of the network at the start of this forward (prepack_weights)
+    wp = _prepacked(weight, fmt, use8)
+    if wp is None:
+        wp = _alloc_weight_pack(weight.shape, dev, wf=not use8, wf8=use8)
+        _weight_pack(weight, wp, fmt)
+    alpha, wop = wp.alpha, (wp.wf8 if use8 else wp.wf)
     scale, shift = bn_eval_fold(gamma, beta, running_mean, running_var, eps, alpha)
     rc = _nhwc(residual.detach()) if residual is not None else None
     z = torch.empty(z_shape, dtype=torch.float32, device=dev, memory_format=torch.channels_last)

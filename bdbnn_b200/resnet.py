@@ -82,12 +82,7 @@ def _prepack(model, x):
                 not (model.training and m.ede_active)):
             cout, cin, kh, kw = m.weight.shape
             if (cin * kh * kw) % 32 == 0 and cin % 64 == 0 and cout % 32 == 0:
-                # the fp8 forward is used where the shape allows (same rule as _ConvBNAddUnit / conv_bn_add_eval)
-                if model.training:
-                    use8 = F_.fwd8_enabled() and cin % 128 == 0 and (cout == 64 or cout % 128 == 0)
-                else:
-                    use8 = F_.eval_use8(cin, cout)
-                items.append((m.weight, use8))
+                items.append((m.weight, F_.use_fwd8(cin, cout, eval_unit=not model.training)))
     if not items:
         return False
     F_._PREPACKED.clear()

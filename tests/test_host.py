@@ -262,14 +262,17 @@ def test_make_optimizer_cpu_is_plain_torch_and_fused_rejects_cpu():
         FusedAdam([p]).step()
 
 
-def test_wgrad_tiling_plans_are_sane_for_every_network_layer():
+def test_wgrad_tiling_plans_are_sane_for_every_network_layer(monkeypatch):
     """Host-only sweep of the wgrad planner (no GPU): every binary-conv geometry of the ResNet-18/34/20 shells,
     both gradient operand widths — shared memory within the 227 KB CTA limit, at most three waves of CTAs on an H100
     (132 SMs),
-    the accumulators within 128 registers per thread, the workspace large enough for the split the launch will use."""
+    the accumulators within 128 registers per thread, the workspace large enough for the split the launch will use.
+    Also: the fp8 operand rule prepack_weights is given never asks for fp8 where the library has no fp8 forward,
+    so it agrees with the units, which apply the same rule under that capability bit."""
     import ctypes
     from bdbnn_b200 import _lib
-    from bdbnn_b200.functional import conv_shape
+    from bdbnn_b200.functional import conv_shape, use_fwd8
+    monkeypatch.setenv("BDBNN_FWD8", "1")
     L = _lib.lib()
     shapes = []
     for n in (1, 7, 256):
@@ -281,10 +284,17 @@ def test_wgrad_tiling_plans_are_sane_for_every_network_layer():
                    ((n, 16, 32, 32), (16, 16, 3, 3), 1), ((n, 16, 32, 32), (32, 16, 3, 3), 2),
                    ((n, 32, 16, 16), (32, 32, 3, 3), 1), ((n, 32, 16, 16), (64, 32, 3, 3), 2),
                    ((n, 64, 8, 8), (64, 64, 3, 3), 1)]
+    n_fp8 = 0
     for xs, ws, stride in shapes:
         pad = 1 if ws[2] == 3 else 0
         sh = conv_shape(xs, ws, stride, pad)
         need = int(L.bdbnn_wgrad_tc_workspace_bytes(ctypes.byref(sh)))
+        caps = int(L.bdbnn_tc_supported(ctypes.byref(sh)))
+        for eval_unit in (False, True):
+            prepacked = use_fwd8(ws[1], ws[0], eval_unit)
+            in_unit = bool(caps & 8) and use_fwd8(ws[1], ws[0], eval_unit)
+            assert prepacked == in_unit, (xs, ws, eval_unit)
+            n_fp8 += prepacked
         for halves in (1, 2):
             out = (ctypes.c_int32 * 12)()
             assert L.bdbnn_debug_wgrad_plan(ctypes.byref(sh), halves, out, 12) == 0
@@ -294,6 +304,7 @@ def test_wgrad_tiling_plans_are_sane_for_every_network_layer():
             assert 1 <= ksplit <= ks_cap and ksplit * mgroups * ntiles <= 3 * 132       # three waves on an H100
             assert UW in (16, 32, 64) and G * BN <= 256 and halo == 0                   # accumulator registers
             assert need >= ksplit * ws[0] * ws[1] * ws[2] * ws[3] * 4, (xs, ws, halves, need, ksplit)
+    assert n_fp8 > 0
     # unsupported geometry is reported, not planned
     out = (ctypes.c_int32 * 12)()
     sh = conv_shape((1, 40, 8, 8), (64, 40, 3, 3), 1, 1)
