@@ -79,6 +79,10 @@ SIGNATURES = {
     "bdbnn_bn_eval_fold": (c_int, [_P] * 5 + [c_int, ctypes.c_float, _P, _P, _P]),
     "bdbnn_binconv_fwd_tc_eval": (c_int, [_P, _P, c_int] + [_P] * 6 + [_SH, _P]),
     "bdbnn_stem_conv_fwd_eval": (c_int, [_P] * 5 + [c_int] * 3 + [_P]),
+    "bdbnn_stem_conv_fwd_eval_relu": (c_int, [_P] * 6 + [c_int] * 3 + [_P]),
+    "bdbnn_real_act_pack": (c_int, [_P, c_int64, c_int, _P, c_int, _P, _P]),
+    "bdbnn_real_weight_pack_multi": (c_int, [c_int] + [_P] * 8 + [_P]),
+    "bdbnn_real_conv_fwd_eval": (c_int, [_P] * 6 + [c_int, _P, _P, _SH, _P]),
 }
 
 

@@ -89,9 +89,144 @@ real_pack_w_kernel(const float* __restrict__ Wt, int Cout, int Cin, const uint32
   }
 }
 
+// k x k weights of many real-valued convs (the 3x3 convs of an fp32 ResNet teacher) in two launches: one scale per
+// tensor, wf[o][t][c] = fp16(W[o][c][t] * 2^ew) in the forward's [Cout][k*k][Cin] layout, alpha[o] = 2^-ew.  W is
+// read through its element strides, so a dense OIHW or channels_last weight needs no copy.
+constexpr int kRealPackMax = 48;          // keeps the table (kernel parameter) under 4 KB
+constexpr int kRealPackPerBlock = 4096;   // weights per block (256 threads x 16)
+struct RealWPackTable {
+  const float* W[kRealPackMax];
+  uint16_t* wf[kRealPackMax];
+  float* alpha[kRealPackMax];
+  int32_t Cout[kRealPackMax], Cin[kRealPackMax], T[kRealPackMax], KW[kRealPackMax];
+  int32_t sO[kRealPackMax], sC[kRealPackMax], sR[kRealPackMax], sS[kRealPackMax];   // element strides of W
+  int32_t blk0[kRealPackMax + 1];         // first block of tensor l (prefix sums of ceil(numel / kRealPackPerBlock))
+  int32_t n;
+};
+
+__device__ __forceinline__ int real_wpack_find(const RealWPackTable& tab, int b) {
+  int l = 0;
+  while (l + 1 < tab.n && b >= tab.blk0[l + 1]) ++l;
+  return l;
+}
+
+// amax[l] (pre-zeroed) = bits of max|W_l|, clamped to a finite value like the activation amax; W_l is dense (any
+// dimension order), so its numel elements are the first numel of its storage
+__global__ void __launch_bounds__(256)
+real_wamax_multi_kernel(const __grid_constant__ RealWPackTable tab, uint32_t* __restrict__ amax) {
+  const int l = real_wpack_find(tab, int(blockIdx.x));
+  const int n = tab.Cout[l] * tab.Cin[l] * tab.T[l];
+  const int base = (int(blockIdx.x) - tab.blk0[l]) * kRealPackPerBlock;
+  const int end = base + kRealPackPerBlock < n ? base + kRealPackPerBlock : n;
+  const float* W = tab.W[l];
+  float m = 0.f;
+  for (int i = base + threadIdx.x; i < end; i += blockDim.x) m = fmaxf(m, fabsf(__ldg(W + i)));
+  m = warp_max(m);
+  if (!(m < 3.0e38f)) m = 3.0e38f;
+  if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(amax + l, __float_as_uint(m));
+}
+
+// coalesced along the output (c fastest); an OIHW weight is read with stride k*k through L2, a channels_last one
+// in order
+__global__ void __launch_bounds__(256)
+real_wpack_multi_kernel(const __grid_constant__ RealWPackTable tab, const uint32_t* __restrict__ amax) {
+  const int l = real_wpack_find(tab, int(blockIdx.x));
+  const int Cin = tab.Cin[l], T = tab.T[l], KW = tab.KW[l], n = tab.Cout[l] * Cin * T;
+  const int sO = tab.sO[l], sC = tab.sC[l], sR = tab.sR[l], sS = tab.sS[l];
+  const int base = (int(blockIdx.x) - tab.blk0[l]) * kRealPackPerBlock;
+  const int end = base + kRealPackPerBlock < n ? base + kRealPackPerBlock : n;
+  const uint32_t a = __ldg(amax + l);
+  const float sw = amax_pow2_scale(a, false), isw = amax_pow2_scale(a, true);
+  const float* W = tab.W[l];
+  __half* wf = reinterpret_cast<__half*>(tab.wf[l]);
+  for (int j = base + threadIdx.x; j < end; j += blockDim.x) {
+    const int c = j % Cin, q = j / Cin;
+    const int t = q % T, o = q / T;
+    const int r = t / KW, sx = t - r * KW;
+    wf[j] = __float2half_rn(__ldg(W + int64_t(o) * sO + int64_t(c) * sC + int64_t(r) * sR + int64_t(sx) * sS) * sw);
+    if (c == 0 && t == 0) tab.alpha[l][o] = isw;
+  }
+}
+
 }  // namespace bdbnn
 
 using namespace bdbnn;
+
+extern "C" int bdbnn_real_act_pack(const float* x, int64_t n_pix, int32_t C, uint32_t* amax_bits, int32_t have_amax,
+                                   uint16_t* xh, void* stream) {
+  BDBNN_REQUIRE(n_pix > 0 && C > 0 && (C & 3) == 0, "real_act_pack: needs n_pix > 0 and C a positive multiple of 4");
+  BDBNN_REQUIRE(x && amax_bits && xh, "real_act_pack: NULL pointer");
+  cudaStream_t st = cudaStream_t(stream);
+  // the strided-sample kernels of bdbnn_real_conv_pack at stride 1 over n_pix 1x1 "images"
+  const int C4 = C / 4;
+  const int64_t total = n_pix * C4;
+  int64_t blocks = (total + 255) / 256;
+  const int64_t cap = int64_t(num_sms()) * 16;
+  if (blocks > cap) blocks = cap;
+  if (!have_amax) {
+    BDBNN_CUDA(cudaMemsetAsync(amax_bits, 0, sizeof(uint32_t), st));
+    real_amax_kernel<<<unsigned(blocks), 256, 0, st>>>(reinterpret_cast<const float4*>(x), 1, 1, C4, 1, 1, 1, total,
+                                                       amax_bits);
+    int rc = check_launch("real_amax_kernel");
+    if (rc) return rc;
+  }
+  real_pack_x_kernel<<<unsigned(blocks), 256, 0, st>>>(reinterpret_cast<const float4*>(x), 1, 1, C4, 1, 1, 1, total,
+                                                       amax_bits, reinterpret_cast<uint2*>(xh));
+  return check_launch("real_pack_x_kernel");
+}
+
+extern "C" int bdbnn_real_weight_pack_multi(int32_t count, const float* const* W_host, const int32_t* Cout_host,
+                                            const int32_t* Cin_host, const int32_t* kw_host,
+                                            const int64_t* strides_host, uint32_t* amax_bits,
+                                            uint16_t* const* wf_host, float* const* alpha_host, void* stream) {
+  BDBNN_REQUIRE(count >= 0, "real_weight_pack_multi: bad count");
+  BDBNN_REQUIRE(count == 0 || (W_host && Cout_host && Cin_host && kw_host && strides_host && amax_bits && wf_host &&
+                               alpha_host),
+                "real_weight_pack_multi: NULL table");
+  cudaStream_t st = cudaStream_t(stream);
+  if (count > 0) BDBNN_CUDA(cudaMemsetAsync(amax_bits, 0, size_t(count) * sizeof(uint32_t), st));
+  for (int off = 0; off < count; off += kRealPackMax) {
+    const int cnt = count - off < kRealPackMax ? count - off : kRealPackMax;
+    RealWPackTable tab;
+    memset(&tab, 0, sizeof(tab));
+    tab.n = cnt;
+    int64_t blocks = 0;
+    for (int i = 0; i < cnt; ++i) {
+      const int l = off + i;
+      const int k = kw_host[l];
+      const int64_t n = int64_t(Cout_host[l]) * Cin_host[l] * k * k;
+      const int64_t* st4 = strides_host + 4 * int64_t(l);
+      BDBNN_REQUIRE(W_host[l] && wf_host[l] && alpha_host[l], "real_weight_pack_multi: NULL pointer in tensor %d", l);
+      BDBNN_REQUIRE(Cout_host[l] > 0 && Cin_host[l] > 0 && k > 0 && n < (int64_t(1) << 30),
+                    "real_weight_pack_multi: bad dims in tensor %d", l);
+      // dense: the strides are a permutation of the contiguous strides of some dimension order
+      int64_t dims[4] = {Cout_host[l], Cin_host[l], k, k}, span = 1;
+      bool dense = true;
+      for (int d = 0; d < 4; ++d) {
+        BDBNN_REQUIRE(st4[d] >= 0 && st4[d] < (int64_t(1) << 30), "real_weight_pack_multi: bad strides in tensor %d", l);
+        span += (dims[d] - 1) * st4[d];
+      }
+      for (int d = 0; d < 4 && dense; ++d)
+        for (int e = d + 1; e < 4; ++e)
+          if (dims[d] > 1 && dims[e] > 1 && st4[d] == st4[e]) dense = false;
+      BDBNN_REQUIRE(dense && span == n, "real_weight_pack_multi: tensor %d is not dense", l);
+      tab.W[i] = W_host[l]; tab.wf[i] = wf_host[l]; tab.alpha[i] = alpha_host[l];
+      tab.Cout[i] = Cout_host[l]; tab.Cin[i] = Cin_host[l]; tab.T[i] = k * k; tab.KW[i] = k;
+      tab.sO[i] = int32_t(st4[0]); tab.sC[i] = int32_t(st4[1]); tab.sR[i] = int32_t(st4[2]); tab.sS[i] = int32_t(st4[3]);
+      tab.blk0[i] = int32_t(blocks);
+      blocks += (n + kRealPackPerBlock - 1) / kRealPackPerBlock;
+    }
+    BDBNN_REQUIRE(blocks < (int64_t(1) << 31), "real_weight_pack_multi: too many weights");
+    tab.blk0[cnt] = int32_t(blocks);
+    real_wamax_multi_kernel<<<unsigned(blocks), 256, 0, st>>>(tab, amax_bits + off);
+    int rc = check_launch("real_wamax_multi_kernel");
+    if (rc) return rc;
+    real_wpack_multi_kernel<<<unsigned(blocks), 256, 0, st>>>(tab, amax_bits + off);
+    rc = check_launch("real_wpack_multi_kernel");
+    if (rc) return rc;
+  }
+  return BDBNN_OK;
+}
 
 extern "C" int bdbnn_real_conv_pack(const float* x, int32_t N, int32_t H, int32_t W, int32_t Cin, int32_t stride,
                                     const float* weight, int32_t Cout, uint16_t* xh, uint32_t* x_amax_bits,

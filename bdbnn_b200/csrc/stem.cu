@@ -177,7 +177,16 @@ extern "C" int bdbnn_stem_conv_fwd_eval(const uint16_t* xw, const uint16_t* wf, 
   StemGeom g;
   BDBNN_REQUIRE(stem_geom(N, H, W, &g), "stem_conv_fwd_eval: geometry not supported");
   BDBNN_REQUIRE(xw && wf && scale && shift && z, "stem_conv_fwd_eval: NULL pointer");
-  return launch_stem_eval(xw, wf, scale, shift, z, g, cudaStream_t(stream));
+  return launch_stem_eval(xw, wf, scale, shift, z, g, 0, nullptr, cudaStream_t(stream));
+}
+
+extern "C" int bdbnn_stem_conv_fwd_eval_relu(const uint16_t* xw, const uint16_t* wf, const float* scale,
+                                             const float* shift, float* z, uint32_t* z_amax_bits, int32_t N,
+                                             int32_t H, int32_t W, void* stream) {
+  StemGeom g;
+  BDBNN_REQUIRE(stem_geom(N, H, W, &g), "stem_conv_fwd_eval_relu: geometry not supported");
+  BDBNN_REQUIRE(xw && wf && scale && shift && z, "stem_conv_fwd_eval_relu: NULL pointer");
+  return launch_stem_eval(xw, wf, scale, shift, z, g, 1, z_amax_bits, cudaStream_t(stream));
 }
 
 extern "C" int bdbnn_stem_conv_wgrad(const uint16_t* gys, const uint32_t* g_amax_bits, const uint16_t* xw,

@@ -359,11 +359,14 @@ struct TcConvLaunch {
   const float* alpha; const uint32_t* mask; float* out;
   int16_t* out_i16;              // forward, wide GEMMs only: write the integer accumulator as int16 instead of out
   int fmt;                       // operand format (BDBNN_FMT_*); -1 = fp8 e4m3 bytes (forward only)
-  const uint32_t* amax_bits;     // FP16S gradient: device word with max|A|; epilogue multiplies by 2^-e
+  const uint32_t* amax_bits;     // FP16S gradient / real-valued eval operand: device word with max|A|; the
+                                 // epilogue multiplies the accumulator by 2^-e
   const float* add;              // dgrad: optional tensor added to the result (shortcut gradient), or NULL;
                                  // eval: optional residual added to z
   // eval forward (MODE 2): z = acc * alpha + shift (+ add) written to `out`, optional +-1 copies of z
   const float* shift; uint16_t* zb; uint8_t* zb8;
+  int relu;                      // eval: z = relu(z) after the residual
+  uint32_t* z_amax;              // eval: optional bits of max|z| (zeroed by the caller)
   // forward only: per-output-channel BatchNorm statistics of the result, accumulated by the epilogue
   // (sum y, sum y^2 as doubles [2*Nout]; max|y| bits [Nout]); NULL = off.  Zeroed by the caller.
   double* bn_sums;
@@ -400,7 +403,7 @@ constexpr int kStemCout = 64, kStemTaps = 7, kStemWin = 32;
 int launch_stem_fwd(const uint16_t* xw, const uint16_t* wf, const float* alpha, float* y, const StemGeom& g,
                     double* bn_sums, uint32_t* bn_ymax, cudaStream_t st);
 int launch_stem_eval(const uint16_t* xw, const uint16_t* wf, const float* scale, const float* shift, float* z,
-                     const StemGeom& g, cudaStream_t st);
+                     const StemGeom& g, int relu, uint32_t* z_amax, cudaStream_t st);
 // zero the statistics buffers of a conv launch (no-op when off)
 inline int bn_stats_zero(double* sums, uint32_t* ymax, int C, cudaStream_t st) {
   if (!sums) return BDBNN_OK;

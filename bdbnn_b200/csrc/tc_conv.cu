@@ -38,10 +38,12 @@ struct TcConvParams {
   int32_t stages;
   int32_t cm, cn;            // cluster: cm CTAs along M share the weight box, cn along N share the activation box
   int32_t row_bytes;         // KB * element size = swizzle span (32/64/128)
-  const uint32_t* amax_bits; // FP16S: post-scale 2^-e (NULL otherwise)
+  const uint32_t* amax_bits; // MODE 1 FP16S / MODE 2 real operands: post-scale 2^-e of the A operand (NULL = 1)
   const float* add;          // dgrad: optional additive tensor; eval: optional residual
   const float* alpha;        // MODE 0: per-output-channel scale; MODE 2: folded BatchNorm scale
   const float* shift;        // MODE 2: folded BatchNorm shift
+  int32_t relu;              // MODE 2: z = relu(z) after the residual (NaN propagates, as torch.relu)
+  uint32_t* z_amax;          // MODE 2: optional bits of max|z| (pre-zeroed, integer atomicMax)
   uint16_t* zb;              // MODE 2: optional 16-bit +-1 copy of z (+1 = zb_one, -1 = zb_one | 0x8000)
   uint8_t* zb8;              // MODE 2: optional fp8 e4m3 +-1 copy of z
   uint32_t zb_one;           // MODE 2: 16-bit +1 (0x3C00 fp16, 0x3F80 bf16)
@@ -167,7 +169,8 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     for (int c = 0; c < NCH; ++c) wgmma_fence_regs(acc[c]);
 
     // ---- epilogue: this thread holds rows r and r + 8 (r = 64 wg + 16 wq + lane/4), column pairs 8j + 2(lane%4) ----
-    const float post = (MODE == 1 && p.amax_bits) ? amax_pow2_scale(__ldg(p.amax_bits), true) : 1.0f;
+    const float post = (MODE != 0 && p.amax_bits) ? amax_pow2_scale(__ldg(p.amax_bits), true) : 1.0f;
+    uint32_t zmax = 0u;                     // MODE 2: bits of this thread's max|z| (ordered as integers, NaN on top)
     const int mask_words = (p.Nout + 31) >> 5;
     int64_t pix[2];
     bool valid[2];
@@ -222,14 +225,20 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             else
               *reinterpret_cast<float2*>(p.out + off) = make_float2(o0, o1);
           } else if (MODE == 2) {
-            // two roundings per step, no FMA contraction: the CPU reference (oracle/eval_ref.py) matches bit for bit
-            o0 = __fadd_rn(__fmul_rn(v0, a0), sb0);
-            o1 = __fadd_rn(__fmul_rn(v1, a1), sb1);
+            // one rounding per step, no FMA contraction: the CPU reference (oracle/eval_ref.py) matches bit for bit.
+            // post = 2^-ex of real-valued operands (exact), 1 for the +-1 operands.
+            o0 = __fadd_rn(__fmul_rn(__fmul_rn(v0, post), a0), sb0);
+            o1 = __fadd_rn(__fmul_rn(__fmul_rn(v1, post), a1), sb1);
             if (p.add != nullptr) {          // the residual never aliases z (bdbnn_binconv_fwd_tc_eval rejects it)
               const float2 r = __ldg(reinterpret_cast<const float2*>(p.add + off));
               o0 = __fadd_rn(o0, r.x); o1 = __fadd_rn(o1, r.y);
             }
+            if (p.relu) {                    // torch.relu: NaN stays NaN (fmaxf alone would drop it)
+              o0 = o0 != o0 ? o0 : fmaxf(o0, 0.f);
+              o1 = o1 != o1 ? o1 : fmaxf(o1, 0.f);
+            }
             *reinterpret_cast<float2*>(p.out + off) = make_float2(o0, o1);
+            zmax = max(zmax, max(__float_as_uint(fabsf(o0)), __float_as_uint(fabsf(o1))));
             // sign(v) = +1 iff v >= 0 (DESIGN.md §2): -0.0 -> +1, NaN -> -1
             if (p.zb != nullptr)
               *reinterpret_cast<uint32_t*>(p.zb + off) =
@@ -274,6 +283,10 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           }
         }
       }
+    }
+    if (MODE == 2 && p.z_amax != nullptr) {   // max is order-free: the same bits every run
+      zmax = __reduce_max_sync(0xffffffffu, zmax);
+      if (lane == 0 && zmax != 0u) atomicMax(p.z_amax, zmax);
     }
   }
   if (do_stats) {
@@ -360,7 +373,7 @@ static bool plan_tc_conv(const TcConvLaunch& L, int mode, TcConvParams* pp, size
   if (L.fmt < 0 && p.BN < 64) return false;
   p.alpha = L.alpha; p.mask = L.mask; p.out = L.out; p.out_i16 = mode == 0 ? L.out_i16 : nullptr;
   p.shift = L.shift; p.zb = L.zb; p.zb8 = L.zb8; p.zb_one = L.fmt == BDBNN_FMT_BF16 ? 0x3F80u : 0x3C00u;
-  p.amax_bits = L.amax_bits; p.add = L.add;
+  p.amax_bits = L.amax_bits; p.add = L.add; p.relu = L.relu; p.z_amax = L.z_amax;
   p.bn_sums = L.bn_sums; p.bn_ymax = L.bn_ymax;
   p.st_y = L.st_y; p.st_alpha = L.st_alpha; p.st_mean = L.st_mean; p.st_invstd = L.st_invstd;
   const uint32_t stage_bytes = (uint32_t(kTileM + p.BN) * p.row_bytes + 1023u) & ~1023u;
@@ -479,12 +492,14 @@ int launch_stem_fwd(const uint16_t* xw, const uint16_t* wf, const float* alpha, 
   return launch_tc_conv<0>(L, st);
 }
 
-// The same GEMM with the eval epilogue: z = acc * scale + shift (the folded eval-mode BatchNorm), no +-1 copy.
+// The same GEMM with the eval epilogue: z = acc * scale + shift (the folded eval-mode BatchNorm), no +-1 copy;
+// optionally z = relu(z) and max|z| into z_amax (zeroed here).
 int launch_stem_eval(const uint16_t* xw, const uint16_t* wf, const float* scale, const float* shift, float* z,
-                     const StemGeom& g, cudaStream_t st) {
+                     const StemGeom& g, int relu, uint32_t* z_amax, cudaStream_t st) {
   TcConvLaunch L;
   stem_launch(&L, xw, wf, scale, z, g);
-  L.shift = shift;
+  L.shift = shift; L.relu = relu; L.z_amax = z_amax;
+  if (z_amax) BDBNN_CUDA(cudaMemsetAsync(z_amax, 0, sizeof(uint32_t), st));
   return launch_tc_conv<2>(L, st);
 }
 
@@ -710,6 +725,28 @@ extern "C" int bdbnn_binconv_fwd_tc_eval(const void* xb, const void* wf, int32_t
   fwd_launch(&L, xb, wf, fmt, s);
   L.alpha = scale; L.shift = shift; L.add = residual; L.out = z; L.zb = zb; L.zb8 = zb8;
   return launch_tc_conv<2>(L, cudaStream_t(stream));
+}
+
+// Eval-mode forward of a real-valued conv on fp16 operands (xh = fp16(x * 2^ex), wf = fp16(W * 2^ew)) — see
+// include/bdbnn.h.
+extern "C" int bdbnn_real_conv_fwd_eval(const uint16_t* xh, const uint32_t* x_amax_bits, const uint16_t* wf,
+                                        const float* scale, const float* shift, const float* residual, int32_t relu,
+                                        float* z, uint32_t* z_amax_bits, const bdbnn_conv_shape* s, void* stream) {
+  int rc = validate_shape(s);
+  if (rc) return rc;
+  BDBNN_REQUIRE(xh && x_amax_bits && wf && scale && shift && z, "real_conv_fwd_eval: NULL pointer");
+  BDBNN_REQUIRE(residual != z, "real_conv_fwd_eval: residual must not alias z");
+  if (!tc_shape_ok(s)) {
+    set_error("real_conv_fwd_eval: shape not supported by the tensor-core path");
+    return BDBNN_ERR_UNSUPPORTED;
+  }
+  cudaStream_t st = cudaStream_t(stream);
+  TcConvLaunch L;
+  fwd_launch(&L, xh, wf, BDBNN_FMT_FP16, s);
+  L.amax_bits = x_amax_bits;
+  L.alpha = scale; L.shift = shift; L.add = residual; L.out = z; L.relu = relu != 0; L.z_amax = z_amax_bits;
+  if (z_amax_bits) BDBNN_CUDA(cudaMemsetAsync(z_amax_bits, 0, sizeof(uint32_t), st));
+  return launch_tc_conv<2>(L, st);
 }
 
 struct DgradStats {      // backward statistics of the BatchNorm unit that produced this conv's input (see tc_common.cuh)

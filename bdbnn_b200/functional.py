@@ -1665,6 +1665,13 @@ def stem_conv_bn_pool_eval(x, weight, gamma, beta, running_mean, running_var, ep
     The BatchNorm is applied before the max (gamma may be negative), so the pool reads the folded result."""
     _eval_only("stem_conv_bn_pool_eval")
     _require_cuda(x, "stem_conv_bn_pool_eval(x)")
+    return _stem_eval_impl(x, weight, gamma, beta, running_mean, running_var, eps, kernel_size, stride, padding,
+                           relu=False)[0]
+
+
+def _stem_eval_impl(x, weight, gamma, beta, running_mean, running_var, eps, kernel_size, stride, padding, relu):
+    """stem_pack -> fold(alpha) -> stem_conv_fwd_eval (relu: stem_conv_fwd_eval_relu, which also writes max|z|) ->
+    maxpool_fwd.  Returns (z, z_amax or None)."""
     L = _lib.lib()
     dev = x.device
     st = _stream()
@@ -1675,13 +1682,119 @@ def stem_conv_bn_pool_eval(x, weight, gamma, beta, running_mean, running_var, ep
     xw, _x_amax, wf, alpha, key = _stem_pack_impl(x, weight)
     scale, shift = bn_eval_fold(gamma, beta, running_mean, running_var, eps, alpha)
     y = torch.empty((n, 64, ho, wo), dtype=torch.float32, device=dev, memory_format=torch.channels_last)
-    with _timed("stem_conv_fwd_eval", key, xw.numel() * 2 + 4 * y.numel()):
-        _lib.check(L.bdbnn_stem_conv_fwd_eval(_p(xw), _p(wf), _p(scale), _p(shift), _p(y), n, h, w, st),
-                   "stem_conv_fwd_eval")
+    z_amax = None
+    if relu:
+        z_amax = torch.empty((1,), dtype=torch.int32, device=dev)
+        with _timed("stem_conv_fwd_eval_relu", key, xw.numel() * 2 + 4 * y.numel()):
+            _lib.check(L.bdbnn_stem_conv_fwd_eval_relu(_p(xw), _p(wf), _p(scale), _p(shift), _p(y), _p(z_amax), n, h,
+                                                       w, st), "stem_conv_fwd_eval_relu")
+    else:
+        with _timed("stem_conv_fwd_eval", key, xw.numel() * 2 + 4 * y.numel()):
+            _lib.check(L.bdbnn_stem_conv_fwd_eval(_p(xw), _p(wf), _p(scale), _p(shift), _p(y), n, h, w, st),
+                       "stem_conv_fwd_eval")
     _lib.count(4)       # x amax, x pack, W pack, conv
     z = torch.empty((n, 64, po, pw), dtype=torch.float32, device=dev, memory_format=torch.channels_last)
     idx = torch.empty((n, po, pw, 64), dtype=torch.uint8, device=dev)
     with _timed("stem_maxpool_fwd", key, 4 * y.numel() + 5 * z.numel()):
         _lib.check(L.bdbnn_maxpool_fwd(_p(y), _p(z), _p(idx), n, ho, wo, 64, k, s, p, po, pw, st), "maxpool_fwd")
     _lib.count(1)
-    return z
+    return z, z_amax
+
+
+# ---------------------------------------------------------------------------------------------------
+# Eval-mode forward of real-valued convs (DESIGN.md §4h): the frozen fp32 teacher of the KD step.  fp16 operands
+# with power-of-two scales (TF32-class), BatchNorm folded into the epilogue, residual and ReLU there too; each conv
+# also returns max|z| as a device word so that the next conv packs its input in one pass.
+# ---------------------------------------------------------------------------------------------------
+def _dense(w):
+    """w itself when it is dense in some dimension order (contiguous or channels_last), else a contiguous copy."""
+    if w.is_contiguous() or w.is_contiguous(memory_format=torch.channels_last):
+        return w
+    return w.contiguous()
+
+
+def real_weight_pack(weights):
+    """fp16 operands of real-valued k x k conv weights, all in two launches (bdbnn_real_weight_pack_multi): one
+    power-of-two scale per tensor.  Contiguous and channels_last weights are read in place, through their strides.
+    Returns [(wf [Cout][k*k][Cin] int16, alpha[Cout] = 2^-ew)] in input order, on the weights' device."""
+    L = _lib.lib()
+    if not weights:
+        return []
+    ws = [_dense(w.detach()) for w in weights]
+    for w in ws:
+        _require_cuda(w, "real_weight_pack")
+        if w.dim() != 4 or w.shape[2] != w.shape[3]:
+            raise RuntimeError(f"bdbnn_b200.real_weight_pack: expected [Cout,Cin,k,k] weights, got {tuple(w.shape)}")
+    _same_device(*ws)
+    dev = ws[0].device
+    with torch.cuda.device(dev):            # launch on the weights' device, whichever device is current
+        wf = [torch.empty((w.shape[0], w.shape[2] * w.shape[3], w.shape[1]), dtype=torch.int16, device=dev)
+              for w in ws]
+        alpha = [torch.empty((w.shape[0],), dtype=torch.float32, device=dev) for w in ws]
+        amax = torch.empty((len(ws),), dtype=torch.int32, device=dev)
+        n = len(ws)
+        ints = lambda vals: (ctypes.c_int32 * n)(*vals)
+        strides = (ctypes.c_int64 * (4 * n))(*[st for w in ws for st in w.stride()])
+        n_w = sum(w.numel() for w in ws)
+        with _timed("real_weight_pack", f"n{n}", 4 * n_w * 2 + 2 * n_w):    # amax read, pack read, fp16 write
+            _lib.check(L.bdbnn_real_weight_pack_multi(
+                n, _ptr_array(ws), ints([w.shape[0] for w in ws]), ints([w.shape[1] for w in ws]),
+                ints([w.shape[3] for w in ws]), strides, _p(amax), _ptr_array(wf), _ptr_array(alpha), _stream()),
+                "real_weight_pack_multi")
+    _lib.count(2 * ((n + 47) // 48))
+    return list(zip(wf, alpha))
+
+
+@_on_x_device
+def real_conv_bn_eval(x, x_amax, wpack, gamma, beta, running_mean, running_var, eps, stride, padding, residual=None,
+                      relu=True):
+    """z = relu(BN_eval(conv2d(x, W)) + residual) of a real-valued conv under no_grad, with wpack = (wf, alpha) of
+    real_weight_pack(W): real_act_pack -> fold(alpha) -> real_conv_fwd_eval.  x fp32 CUDA (channels_last avoids a
+    copy); x_amax = the device word of max|x| a previous call returned (None: computed here, one more pass over x).
+    Returns (z fp32 channels_last, z_amax int32[1] = bits of max|z|)."""
+    _eval_only("real_conv_bn_eval")
+    _require_cuda(x, "real_conv_bn_eval(x)")
+    wf, alpha = wpack
+    _same_device(x, wf, gamma, beta, running_mean, running_var, residual)
+    L = _lib.lib()
+    n, cin, h, w = x.shape
+    cout, taps, cin_w = wf.shape
+    k = int(round(taps ** 0.5))
+    sh = conv_shape(x.shape, (cout, cin_w, k, k), stride, padding)
+    if not int(L.bdbnn_tc_supported(ctypes.byref(sh))) & 1:
+        raise RuntimeError("bdbnn_b200.real_conv_bn_eval: the wgmma forward does not support this shape")
+    z_shape = (n, cout, sh.Ho, sh.Wo)
+    if residual is not None and tuple(residual.shape) != z_shape:
+        raise RuntimeError(f"real_conv_bn_eval: residual shape {tuple(residual.shape)} != output shape {z_shape}")
+    dev = x.device
+    st = _stream()
+    key = _shape_key(sh)
+    xc = _nhwc(x.detach())
+    xh = torch.empty((n, h, w, cin), dtype=torch.int16, device=dev)
+    have = x_amax is not None
+    amax = x_amax if have else torch.empty((1,), dtype=torch.int32, device=dev)
+    n_in = xc.numel()
+    with _timed("real_act_pack", key, 4 * n_in + 2 * n_in):
+        _lib.check(L.bdbnn_real_act_pack(_p(xc), n * h * w, cin, _p(amax), int(have), _p(xh), st), "real_act_pack")
+    _lib.count(1 if have else 2)
+    scale, shift = bn_eval_fold(gamma, beta, running_mean, running_var, eps, alpha)
+    rc = _nhwc(residual.detach()) if residual is not None else None
+    z = torch.empty(z_shape, dtype=torch.float32, device=dev, memory_format=torch.channels_last)
+    z_amax = torch.empty((1,), dtype=torch.int32, device=dev)
+    n_out = z.numel()
+    with _timed("real_conv_fwd_eval", key, algorithmic_bytes("fwd_tc_eval", sh) + (4 * n_out if rc is not None else 0)):
+        _lib.check(L.bdbnn_real_conv_fwd_eval(_p(xh), _p(amax), _p(wf), _p(scale), _p(shift), _p(rc), int(bool(relu)),
+                                              _p(z), _p(z_amax), ctypes.byref(sh), st), "real_conv_fwd_eval")
+    _lib.count(1)
+    return z, z_amax
+
+
+@_on_x_device
+def stem_conv_bn_relu_pool_eval(x, weight, gamma, beta, running_mean, running_var, eps, kernel_size, stride, padding):
+    """maxpool(relu(BN_eval(stem_conv(x)))) under no_grad, the ReLU in the conv epilogue.  Returns (z fp32
+    channels_last, z_amax int32[1] = bits of max|z|): every stem output lies in some pool window, so the pooled
+    maximum is the stem's."""
+    _eval_only("stem_conv_bn_relu_pool_eval")
+    _require_cuda(x, "stem_conv_bn_relu_pool_eval(x)")
+    return _stem_eval_impl(x, weight, gamma, beta, running_mean, running_var, eps, kernel_size, stride, padding,
+                           relu=True)

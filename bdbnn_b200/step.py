@@ -24,6 +24,7 @@ import torch.nn.functional as F
 
 from . import losses as _losses
 from .modules import HardBinaryConv, HardBinaryConv_cifar, HardBinaryConv_react
+from .teacher import FrozenResNetTeacher
 
 IMAGENET_DIFFKURT = [1.8, 1.4, 1.4, 1.4, 1.4, 1.2, 1.4, 1.2, 1.2, 1.4,
                      1.4, 1.4, 1.2, 1.2, 1.2, 1.2, 1.4, 1, 1]                      # train.py:467-470
@@ -242,6 +243,9 @@ class TrainStep:
             from .functional import _timed
             if t_stream is not None:
                 torch.cuda.current_stream().wait_stream(t_stream)
+            elif isinstance(self.teacher, FrozenResNetTeacher):
+                with torch.no_grad():                                             # its kernels time themselves
+                    output_teacher = self.teacher(images)                         # train.py:603
             else:
                 with torch.no_grad(), _timed("teacher_forward(cuDNN fp32)", "teacher", 0):
                     output_teacher = self.teacher(images)                         # train.py:603

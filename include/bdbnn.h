@@ -377,6 +377,12 @@ BDBNN_API int bdbnn_stem_conv_fwd(const uint16_t* xw, const uint16_t* wf, const 
                         int32_t H, int32_t W, double* bn_sums, uint32_t* bn_ymax, void* stream);
 BDBNN_API int bdbnn_stem_conv_fwd_eval(const uint16_t* xw, const uint16_t* wf, const float* scale, const float* shift,
                              float* z, int32_t N, int32_t H, int32_t W, void* stream);
+/* stem_conv_fwd_eval followed by z = relu(z) in the same epilogue (torch.relu: NaN propagates), for an fp32 teacher
+ * whose stem is conv1 -> bn1 -> relu -> maxpool.  z_amax_bits (one word, may be NULL) receives the bits of max|z|,
+ * zeroed here; the max-pool after it keeps that maximum, so the first block's activation pack can take it. */
+BDBNN_API int bdbnn_stem_conv_fwd_eval_relu(const uint16_t* xw, const uint16_t* wf, const float* scale,
+                                  const float* shift, float* z, uint32_t* z_amax_bits, int32_t N, int32_t H,
+                                  int32_t W, void* stream);
 BDBNN_API int bdbnn_stem_conv_wgrad(const uint16_t* gys, const uint32_t* g_amax_bits, const uint16_t* xw,
                           const uint32_t* x_amax_bits, float* gW, int32_t N, int32_t H, int32_t W,
                           void* workspace, size_t workspace_bytes, void* stream);
@@ -436,6 +442,38 @@ BDBNN_API int bdbnn_optim_sgd_multi_graph(float* const* params_host, const float
 BDBNN_API int bdbnn_real_conv_pack(const float* x, int32_t N, int32_t H, int32_t W, int32_t Cin, int32_t stride,
                          const float* weight, int32_t Cout, uint16_t* xh, uint32_t* x_amax_bits, uint16_t* wf,
                          uint16_t* wt, float* alpha, float* gscale, float* inv_gscale, void* stream);
+
+/* ---- eval-mode forward of real-valued k x k convs (the frozen fp32 teacher of the KD step) --------------------
+ * Operands as for the stem and the shortcut: fp16 after power-of-two scales (amax_pow2_scale of common.cuh:
+ * max * 2^e in [2^13, 2^14)), fp32 accumulation — TF32-class, the format cuDNN gives the reference by default.
+ *   real_act_pack          : xh[p][c] = fp16(x[p][c] * 2^ex), x dense fp32 NHWC [n_pix][C], C % 4 == 0.  ex from
+ *                            amax_bits (one word): computed here (bits of max|x|, non-finite clamped to 3e38) when
+ *                            have_amax == 0, else read as given (e.g. the z_amax_bits of the conv that wrote x).
+ *                            One launch with the amax given, two without.
+ *   real_weight_pack_multi : for `count` fp32 weights W_l [Cout][Cin][k][k] (host tables: Cout, Cin, k = kw_host[l],
+ *                            and strides_host[4l..4l+3] = W_l's element strides along Cout, Cin, kh, kw; W_l must be
+ *                            dense in some dimension order, e.g. contiguous or channels_last), one scale per tensor:
+ *                            wf_l[o][t][c] = fp16(W_l[o][c][t] * 2^ew_l) (the forward's [Cout][k*k][Cin] layout),
+ *                            alpha_l[o] = 2^-ew_l for every o; amax_bits = device scratch of `count` words (bits of
+ *                            max|W_l|, zeroed here).  Two launches per 48 tensors.
+ *   real_conv_fwd_eval     : the forward implicit GEMM of bdbnn_binconv_fwd_tc over xh / wf (fp16), with, rounding
+ *                            every step (no FMA):
+ *                              z = fp32(fp32(fp32(acc * 2^-ex) * scale[o]) + shift[o])   (2^-ex from x_amax_bits)
+ *                              z = fp32(z + residual)  if residual != NULL (z's shape, must not alias it)
+ *                              z = relu(z)             if relu != 0 (torch.relu: NaN propagates)
+ *                            (scale, shift) = bdbnn_bn_eval_fold with the weight's alpha.  z fp32 NHWC; z_amax_bits
+ *                            (one word, may be NULL; zeroed here) receives the bits of max|z| (integer atomicMax
+ *                            of |z|'s bits: run-to-run identical, NaN above every number).  Requires
+ *                            bdbnn_tc_supported(s) & BDBNN_TC_FWD.  One launch. */
+BDBNN_API int bdbnn_real_act_pack(const float* x, int64_t n_pix, int32_t C, uint32_t* amax_bits, int32_t have_amax,
+                        uint16_t* xh, void* stream);
+BDBNN_API int bdbnn_real_weight_pack_multi(int32_t count, const float* const* W_host, const int32_t* Cout_host,
+                                 const int32_t* Cin_host, const int32_t* kw_host, const int64_t* strides_host,
+                                 uint32_t* amax_bits,
+                                 uint16_t* const* wf_host, float* const* alpha_host, void* stream);
+BDBNN_API int bdbnn_real_conv_fwd_eval(const uint16_t* xh, const uint32_t* x_amax_bits, const uint16_t* wf,
+                             const float* scale, const float* shift, const float* residual, int32_t relu, float* z,
+                             uint32_t* z_amax_bits, const bdbnn_conv_shape* s, void* stream);
 
 #ifdef __cplusplus
 }

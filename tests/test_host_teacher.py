@@ -1,0 +1,130 @@
+"""Host: the FrozenResNetTeacher wrapper keeps the wrapped torchvision model's module tree, names and parameters, and
+off the kernel path (here: a CPU input) is the model's own forward, bit for bit."""
+import copy
+
+import pytest
+import torch
+import torch.nn as nn
+
+torchvision = pytest.importorskip("torchvision")
+
+
+def _teacher(arch, seed=0):
+    torch.manual_seed(seed)
+    m = getattr(torchvision.models, arch)()
+    g = torch.Generator().manual_seed(seed + 1)
+    for mod in m.modules():                  # non-trivial BatchNorm buffers and affine parameters
+        if isinstance(mod, nn.BatchNorm2d):
+            c = mod.num_features
+            mod.weight.data = torch.randn(c, generator=g)
+            mod.bias.data = torch.randn(c, generator=g) * 0.2
+            mod.running_mean.copy_(torch.randn(c, generator=g) * 0.2)
+            mod.running_var.copy_(torch.rand(c, generator=g) + 0.5)
+    return m.eval()
+
+
+@pytest.mark.parametrize("arch", ["resnet18", "resnet34"])
+def test_wrapper_keeps_names_and_parameter_objects(arch):
+    from bdbnn_b200 import FrozenResNetTeacher
+    m = _teacher(arch)
+    t = FrozenResNetTeacher(m)
+    assert t.wrapped is m
+    assert [n for n, _ in t.named_modules()] == [n for n, _ in m.named_modules()]
+    assert [n for n, _ in t.named_parameters()] == [n for n, _ in m.named_parameters()]
+    assert list(t.state_dict().keys()) == list(m.state_dict().keys())
+    for (_, a), (_, b) in zip(t.named_parameters(), m.named_parameters()):
+        assert a is b
+    for (na, a), (nb, b) in zip(t.named_modules(), m.named_modules()):
+        if na:
+            assert a is b
+
+
+def test_matched_weight_pairs_unchanged_by_the_wrapper():
+    from bdbnn_b200 import FrozenResNetTeacher
+    from bdbnn_b200.losses import matched_weight_pairs
+    from bdbnn_b200.resnet import resnet18
+    stud = resnet18()
+    m = _teacher("resnet18")
+    bare = [(n, s, t) for n, s, t in matched_weight_pairs(stud, m)]
+    wrapped = [(n, s, t) for n, s, t in matched_weight_pairs(stud, FrozenResNetTeacher(m))]
+    assert [n for n, _, _ in wrapped] == [n for n, _, _ in bare] and len(bare) > 0
+    assert all(a[1] is b[1] and a[2] is b[2] for a, b in zip(wrapped, bare))
+
+
+@pytest.mark.parametrize("arch", ["resnet18", "resnet34"])
+def test_cpu_forward_is_the_models(arch):
+    from bdbnn_b200 import FrozenResNetTeacher
+    m = _teacher(arch)
+    t = FrozenResNetTeacher(m)
+    x = torch.randn(2, 3, 64, 64, generator=torch.Generator().manual_seed(3))
+    assert not t.kernel_path(x)
+    with torch.no_grad():
+        assert torch.equal(t(x), m(x))
+    t.train()
+    assert m.training and all(mod.training for mod in m.modules())
+    y_t = t(x)
+    y_m = m(x)
+    assert torch.equal(y_t, y_m)
+    t.eval()
+    assert not m.training and not any(mod.training for mod in m.modules())
+
+
+def test_unsupported_structures_raise_type_error():
+    from bdbnn_b200 import FrozenResNetTeacher
+    with pytest.raises(TypeError):
+        FrozenResNetTeacher(torchvision.models.resnet50())
+    with pytest.raises(TypeError):
+        FrozenResNetTeacher(nn.DataParallel(torchvision.models.resnet18()))
+    m = torchvision.models.resnet18()
+    m.layer2[0].conv1 = nn.Conv2d(64, 128, 5, 2, 2, bias=False)
+    with pytest.raises(TypeError):
+        FrozenResNetTeacher(m)
+
+
+def test_wrapping_the_module_of_a_data_parallel_keeps_its_names():
+    """train.py wraps the teacher in nn.DataParallel (train.py:258); the wrapper goes inside it."""
+    from bdbnn_b200 import FrozenResNetTeacher
+    m = _teacher("resnet18")
+    dp = nn.DataParallel(m)
+    keys = list(dp.state_dict().keys())
+    names = [n for n, _ in dp.named_modules()]
+    dp.module = FrozenResNetTeacher(dp.module)
+    assert list(dp.state_dict().keys()) == keys and [n for n, _ in dp.named_modules()] == names
+    x = torch.randn(1, 3, 64, 64)
+    with torch.no_grad():
+        assert torch.equal(dp(x), m(x))
+
+
+def test_load_state_dict_round_trips():
+    from bdbnn_b200 import FrozenResNetTeacher
+    a, b = _teacher("resnet18", 0), _teacher("resnet18", 7)
+    t = FrozenResNetTeacher(a)
+    sd_b = copy.deepcopy(b.state_dict())
+    t.load_state_dict(sd_b)
+    for k, v in a.state_dict().items():
+        assert torch.equal(v, sd_b[k]), k
+    for k, v in t.state_dict().items():
+        assert torch.equal(v, sd_b[k]), k
+    x = torch.randn(1, 3, 64, 64)
+    with torch.no_grad():
+        assert torch.equal(t(x), b(x))
+
+
+def test_launch_formula():
+    from bdbnn_b200.teacher import launches_per_forward
+    assert launches_per_forward(torchvision.models.resnet18()) == 2 + 6 + 3 * 16 + 6 * 3
+    assert launches_per_forward(torchvision.models.resnet34()) == 2 + 6 + 3 * 32 + 6 * 3
+
+
+def test_pool_arguments_are_normalised_or_rejected():
+    """Square tuple arguments of the stem max-pool are read as ints; a non-square pool keeps the model's forward."""
+    from bdbnn_b200 import FrozenResNetTeacher
+    m = _teacher("resnet18")
+    m.maxpool = nn.MaxPool2d((3, 3), (2, 2), (1, 1))
+    assert FrozenResNetTeacher(m)._pool_args() == (3, 2, 1)
+    m.maxpool = nn.MaxPool2d((3, 2), 2, 1)
+    t = FrozenResNetTeacher(m)
+    assert t._pool_args() is None
+    x = torch.randn(1, 3, 64, 64)
+    with torch.no_grad():
+        assert torch.equal(t(x), m(x))

@@ -1,0 +1,196 @@
+"""Throughput of the KD step's frozen fp32 teacher (train.py:250-277, run at train.py:603): this repository's kernel
+teacher (bdbnn_b200.FrozenResNetTeacher) against the torchvision model on cuDNN.
+
+    python tools/teacher_throughput.py [--models resnet18,resnet34] [--batch 256] [--iters 20] [--warmup 5]
+                                       [--rounds 3] [--steps 50] [--step-warmup 10] [--no-step]
+
+224x224 channels_last images, random weights and BatchNorm statistics.  Teacher forward arms, alternated round by
+round, each warmed up first, images/s from CUDA events over --iters forwards:
+
+    kernel_eager     FrozenResNetTeacher, launched eagerly
+    kernel_graphed   the same forward captured once as a CUDA graph and replayed
+    cudnn_default    the torchvision model with TF32 allowed and cudnn.benchmark off (bench.py's timed path)
+    cudnn_benchmark  the same with cudnn.benchmark = True (train.py:368)
+
+The two kernel arms run in this process.  Each cuDNN arm runs in a process of its own, started afresh every round:
+PyTorch caches the cuDNN plan of a conv shape whatever `benchmark` was when it was chosen, so in one process the arm
+that ran first would serve its plans to the other and the benchmark arm would not autotune.
+
+Then one eager kernel-teacher forward under functional.KernelTimer (per-family times), and the full KD step:
+GraphedTrainStep(TrainStep(resnet18 student, kurtosis + KD config, teacher=...)) with the kernel teacher and with
+the torchvision teacher (cudnn.benchmark off throughout this process), alternated, --step-warmup steps then --steps
+timed steps per round.  The card name, power limit and maximum SM clock are read (read-only) from nvidia-smi.
+Needs a CUDA device."""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+
+def _graphed(torch, fn, warmup):
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s):
+        for _ in range(warmup):
+            fn()
+    torch.cuda.current_stream().wait_stream(s)
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        fn()
+    return g.replay
+
+
+def _timed_loop(torch, fn, iters):
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(iters):
+        fn()
+    e1.record()
+    e1.synchronize()
+    return e0.elapsed_time(e1) / 1e3
+
+
+def _teacher(torch, name, dev):
+    import torch.nn as nn
+    import torchvision
+    torch.manual_seed(1)
+    m = getattr(torchvision.models, name)()
+    g = torch.Generator().manual_seed(2)
+    for mod in m.modules():
+        if isinstance(mod, nn.BatchNorm2d):
+            c = mod.num_features
+            mod.weight.data = torch.rand(c, generator=g) + 0.5
+            mod.bias.data = torch.randn(c, generator=g) * 0.1
+            mod.running_mean.copy_(torch.randn(c, generator=g) * 0.1)
+            mod.running_var.copy_(torch.rand(c, generator=g) + 0.5)
+    for p in m.parameters():
+        p.requires_grad = False
+    return m.to(dev).to(memory_format=torch.channels_last).eval()
+
+
+def _images(torch, batch, dev):
+    x = torch.randn(batch, 3, 224, 224, generator=torch.Generator().manual_seed(0))
+    return x.to(dev).contiguous(memory_format=torch.channels_last)
+
+
+def cudnn_arm(torch, name, mode, args, dev):
+    """One round of a cuDNN arm, in a fresh process: warm-up (autotuning when mode == "benchmark"), then --iters
+    timed forwards.  Prints one JSON line."""
+    torch.backends.cudnn.allow_tf32 = True
+    torch.backends.cudnn.benchmark = mode == "benchmark"
+    tv = _teacher(torch, name, dev)
+    x = _images(torch, args.batch, dev)
+    with torch.no_grad():
+        for _ in range(args.warmup):
+            tv(x)
+        torch.cuda.synchronize()
+        rate = args.batch * args.iters / _timed_loop(torch, lambda: tv(x), args.iters)
+    print(json.dumps({"img_per_s": round(rate, 1)}), flush=True)
+
+
+def _cudnn_round(name, mode, args):
+    cmd = [sys.executable, os.path.abspath(__file__), "--cudnn-arm", mode, "--models", name, "--batch", str(args.batch),
+           "--iters", str(args.iters), "--warmup", str(args.warmup)]
+    r = subprocess.run(cmd, capture_output=True, text=True, check=True)
+    return json.loads(r.stdout.strip().splitlines()[-1])["img_per_s"]
+
+
+def forward_arms(torch, name, args, dev):
+    from bdbnn_b200 import FrozenResNetTeacher
+    from bdbnn_b200.functional import KernelTimer
+    kt = FrozenResNetTeacher(_teacher(torch, name, dev))
+    x = _images(torch, args.batch, dev)
+    with torch.no_grad():
+        assert kt.kernel_path(x)
+        arms = {"kernel_eager": lambda: kt(x), "kernel_graphed": _graphed(torch, lambda: kt(x), args.warmup)}
+        for fn in arms.values():
+            for _ in range(args.warmup):
+                fn()
+        torch.cuda.synchronize()
+        rates = {a: [] for a in list(arms) + ["cudnn_default", "cudnn_benchmark"]}
+        for _ in range(args.rounds):
+            for arm, fn in arms.items():
+                rates[arm].append(round(args.batch * args.iters / _timed_loop(torch, fn, args.iters), 1))
+            for mode in ("default", "benchmark"):
+                rates["cudnn_" + mode].append(_cudnn_round(name, mode, args))
+        print(json.dumps({"teacher": name, "img_per_s": rates}), flush=True)
+        KernelTimer.start()
+        kt(x)
+        kern = KernelTimer.stop()
+    fams = {}
+    for (fam, _key), d in kern.items():
+        f = fams.setdefault(fam, {"ms": 0.0, "launches": 0})
+        f["ms"] += d["ms"]
+        f["launches"] += d["launches"]
+    total = sum(f["ms"] for f in fams.values())
+    for fam, f in sorted(fams.items(), key=lambda kv: -kv[1]["ms"]):
+        print(json.dumps({"teacher": name, "family": fam, "ms": round(f["ms"], 4), "launches": f["launches"]}))
+    print(json.dumps({"teacher": name, "kernel_timer_total_ms": round(total, 4)}), flush=True)
+
+
+def kd_step_arms(torch, name, args, dev):
+    from bdbnn_b200 import FrozenResNetTeacher
+    from bdbnn_b200.resnet import resnet18
+    from bdbnn_b200.step import GraphedTrainStep, StepConfig, TrainStep, make_optimizer
+    torch.backends.cudnn.benchmark = False
+    tv = _teacher(torch, name, dev)
+    cfg = StepConfig(w_kurtosis=True, teacher_student=True, alpha=0.9, beta=200.0, w_lambda_ce=1.0)
+    g = torch.Generator().manual_seed(0)
+    x = torch.randn(args.batch, 3, 224, 224, generator=g).to(dev).contiguous(memory_format=torch.channels_last)
+    y = torch.randint(0, 1000, (args.batch,), generator=g).to(dev)
+    steps = {}
+    for arm, teacher in (("kernel_teacher", FrozenResNetTeacher(tv)), ("cudnn_teacher", tv)):
+        torch.manual_seed(0)
+        model = resnet18().to(dev)
+        steps[arm] = GraphedTrainStep(TrainStep(model, make_optimizer(model), cfg, teacher=teacher))
+    for st in steps.values():
+        for _ in range(args.step_warmup):
+            st(x, y)
+    torch.cuda.synchronize()
+    rates = {a: [] for a in steps}
+    for _ in range(args.rounds):
+        for arm, st in steps.items():
+            rates[arm].append(round(args.batch * args.steps / _timed_loop(torch, lambda: st(x, y), args.steps), 1))
+    print(json.dumps({"kd_step": f"resnet18 student, {name} teacher", "img_per_s": rates}), flush=True)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--models", default="resnet18,resnet34")
+    ap.add_argument("--batch", type=int, default=256)
+    ap.add_argument("--iters", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--steps", type=int, default=50)
+    ap.add_argument("--step-warmup", type=int, default=10)
+    ap.add_argument("--no-step", action="store_true")
+    ap.add_argument("--cudnn-arm", choices=("default", "benchmark"), default=None, help=argparse.SUPPRESS)
+    args = ap.parse_args()
+    import torch
+    if not torch.cuda.is_available():
+        raise SystemExit("teacher_throughput: no CUDA device")
+    if args.cudnn_arm:
+        cudnn_arm(torch, args.models, args.cudnn_arm, args, torch.device("cuda", 0))
+        return
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True)
+    print(json.dumps({"gpu": q.stdout.strip().splitlines()[0] if q.returncode == 0 else None,
+                      "batch": args.batch, "iters": args.iters, "rounds": args.rounds}), flush=True)
+    dev = torch.device("cuda", 0)
+    torch.backends.cudnn.allow_tf32 = True
+    torch.backends.cudnn.benchmark = False
+    for name in args.models.split(","):
+        forward_arms(torch, name, args, dev)
+        torch.cuda.empty_cache()
+    if not args.no_step:
+        for name in args.models.split(","):
+            kd_step_arms(torch, name, args, dev)
+            torch.cuda.empty_cache()
+
+
+if __name__ == "__main__":
+    main()
