@@ -83,6 +83,16 @@ SIGNATURES = {
     "bdbnn_real_act_pack": (c_int, [_P, c_int64, c_int, _P, c_int, _P, _P]),
     "bdbnn_real_weight_pack_multi": (c_int, [c_int] + [_P] * 8 + [_P]),
     "bdbnn_real_conv_fwd_eval": (c_int, [_P] * 6 + [c_int, _P, _P, _SH, _P]),
+    "bdbnn_bn_fwd_pad_shortcut": (c_int, [_P, _P] + [c_int] * 5 + [_P, _P, c_int, ctypes.c_float, ctypes.c_float] +
+                                  [_P] * 12 + [c_int, c_int, _P]),
+    "bdbnn_bn_fwd_i16_pad_shortcut": (c_int, [_P, _P, _P] + [c_int] * 5 + [_P, _P, c_int, ctypes.c_float,
+                                                                          ctypes.c_float] + [_P] * 12 + [c_int, _P]),
+    "bdbnn_pad_shortcut_bwd": (c_int, [_P, _P] + [c_int] * 6 + [_P]),
+    "bdbnn_cifar_stem_fwd": (c_int, [_P, c_int, c_int, c_int, c_int64, c_int64, c_int64, c_int64, _P, c_int, _P, _P, _P,
+                                     _P]),
+    "bdbnn_cifar_stem_wgrad_workspace_bytes": (c_size_t, [c_int] * 4),
+    "bdbnn_cifar_stem_wgrad": (c_int, [_P, c_int, c_int, c_int, c_int64, c_int64, c_int64, c_int64, _P, _P, c_int, _P,
+                                       _P, c_size_t, _P]),
 }
 
 

@@ -222,23 +222,34 @@ __global__ void bn_finalize_kernel(const double* __restrict__ sums, int64_t n_pi
   }
 }
 
+// Option-A (parameter-free) shortcut read in place as the residual: r[n,i,j,c] = x[n,2i,2j,c-pad] for
+// pad <= c < pad+Cin, else 0; x fp32 NHWC [N,H,W,Cin], z [N,Ho,Wo,C] with Ho = ceil(H/2), Wo = ceil(W/2).
+struct PadResidual {
+  const float4* x;
+  int H, W, Ho, Wo, Cin4, pad4;
+};
+
 // z = y*a + b (+ residual); optionally the sign / STE-mask bits and the +-1 16-bit copy of z.
-template <bool PACK, bool I16 = false, int U = 4>
+// SUB: the residual is the option-A shortcut of `sub.x` (res is unused).  P16: C == 16, one sign / mask word per
+// pixel from 4 lanes (bits 16-31 zero, as bdbnn_act_pack writes them) instead of one per 32 channels from 8 lanes.
+template <bool PACK, bool I16 = false, int U = 4, bool SUB = false, bool P16 = false>
 __global__ void __launch_bounds__(kBnThreads)
 bn_apply_add_pack_kernel(const void* __restrict__ y, const float4* __restrict__ res,
                          const float* __restrict__ a, const float* __restrict__ b, int64_t n4, int C4,
                          float4* __restrict__ z, uint32_t* __restrict__ sign_bits,
                          uint32_t* __restrict__ mask_bits, uint2* __restrict__ xb4, uint32_t* __restrict__ xb8,
-                         uint32_t one16) {
+                         uint32_t one16, const PadResidual sub = PadResidual{}) {
+  constexpr int GL = P16 ? 4 : 8;                                 // lanes (float4 groups) per bit word
   const int lane = threadIdx.x & 31;
-  const uint32_t group_mask = 0xffu << (lane & 24);
-  const int sh = (lane & 7) * 4;
+  const uint32_t group_mask = (P16 ? 0xfu : 0xffu) << (lane & (32 - GL));
+  const int sh = (lane & (GL - 1)) * 4;
   const uint32_t pos = one16, neg = one16 | 0x8000u;
   const int64_t nthreads = int64_t(gridDim.x) * blockDim.x;       // multiple of C4 (host guarantees)
   int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
   const int c4 = int(i % C4);                                     // constant per thread
   const float4 av = *reinterpret_cast<const float4*>(a + c4 * 4);
   const float4 bv = *reinterpret_cast<const float4*>(b + c4 * 4);
+  const bool sub_on = SUB && c4 >= sub.pad4 && c4 < sub.pad4 + sub.Cin4;   // constant per thread too
   auto emit = [&](int64_t i, const float4 v, const float4 r) {
     float4 o = make_float4(fmaf(v.x, av.x, bv.x), fmaf(v.y, av.y, bv.y), fmaf(v.z, av.z, bv.z),
                            fmaf(v.w, av.w, bv.w));
@@ -252,9 +263,9 @@ bn_apply_add_pack_kernel(const void* __restrict__ y, const float4* __restrict__ 
                      m3 = fabsf(o.w) <= 1.0f;
       const uint32_t sw = __reduce_or_sync(group_mask, (s0 | (s1 << 1) | (s2 << 2) | (s3 << 3)) << sh);
       const uint32_t mw = __reduce_or_sync(group_mask, (m0 | (m1 << 1) | (m2 << 2) | (m3 << 3)) << sh);
-      if ((lane & 7) == 0) {
-        sign_bits[i >> 3] = sw;
-        mask_bits[i >> 3] = mw;
+      if ((lane & (GL - 1)) == 0) {
+        sign_bits[i / GL] = sw;
+        mask_bits[i / GL] = mw;
       }
       uint2 q;
       q.x = (s0 ? pos : neg) | ((s1 ? pos : neg) << 16);
@@ -265,6 +276,18 @@ bn_apply_add_pack_kernel(const void* __restrict__ y, const float4* __restrict__ 
     }
   };
   const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
+  auto load_r = [&](int64_t e) {
+    if (SUB) {
+      if (!sub_on) return zero4;
+      int64_t q = e / C4;
+      const int j = int(q % sub.Wo);
+      q /= sub.Wo;
+      const int hi = int(q % sub.Ho);
+      const int64_t n = q / sub.Ho;
+      return __ldg(sub.x + ((n * sub.H + 2 * hi) * int64_t(sub.W) + 2 * j) * sub.Cin4 + (c4 - sub.pad4));
+    }
+    return res != nullptr ? __ldcs(res + e) : zero4;
+  };
   // two elements per thread and iteration: all four loads are issued before the first dependent instruction
   // (whole 8-lane pack groups take the same branch: n4 and nthreads are multiples of 8)
   for (; i + (U - 1) * nthreads < n4; i += U * nthreads) {
@@ -272,11 +295,11 @@ bn_apply_add_pack_kernel(const void* __restrict__ y, const float4* __restrict__ 
 #pragma unroll
     for (int u = 0; u < U; ++u) v[u] = load_y4<I16>(y, i + u * nthreads);       // I16: `a` already carries alpha
 #pragma unroll
-    for (int u = 0; u < U; ++u) r[u] = res != nullptr ? __ldcs(res + i + u * nthreads) : zero4;
+    for (int u = 0; u < U; ++u) r[u] = load_r(i + u * nthreads);
 #pragma unroll
     for (int u = 0; u < U; ++u) emit(i + u * nthreads, v[u], r[u]);
   }
-  for (; i < n4; i += nthreads) emit(i, load_y4<I16>(y, i), res != nullptr ? __ldcs(res + i) : zero4);
+  for (; i < n4; i += nthreads) emit(i, load_y4<I16>(y, i), load_r(i));
 }
 
 // [C] math of the backward.  consts[c] = {m1, m2*invstd, mean, a*gscale}; gy*gscale = (gz - m1 -
@@ -430,11 +453,15 @@ static int bn_fwd_impl(const void* y, const float* alpha_i16, const float* resid
                        const float* beta, int64_t n_pix, int32_t C, float eps, float momentum, float* running_mean,
                        float* running_var, double* sums_ws, uint32_t* ymax_bits, float* mean, float* invstd,
                        float* ab_ws, float* z, uint32_t* sign_bits, uint32_t* mask_bits, uint16_t* xb,
-                       uint8_t* xb_fp8, int32_t fmt, int32_t stats_ready, void* stream) {
+                       uint8_t* xb_fp8, int32_t fmt, int32_t stats_ready, void* stream,
+                       const PadResidual* sub = nullptr) {
   const bool pack = sign_bits != nullptr;
   const bool i16 = alpha_i16 != nullptr;
+  // 16-channel packs (one word per pixel): the CIFAR stem's BatchNorm, fp32 y only
+  const bool p16 = pack && C == 16;
   BDBNN_REQUIRE(!i16 || stats_ready, "bn_fwd_i16: the statistics must come from the conv epilogue (stats_ready = 1)");
-  int rc = bn_dims_ok(n_pix, C, pack);
+  BDBNN_REQUIRE(!(p16 && (i16 || sub)), "bn_fwd: 16-channel packs only without int16 y and option-A residual");
+  int rc = bn_dims_ok(n_pix, C, pack && !p16);
   if (rc) return rc;
   BDBNN_REQUIRE(y && gamma && beta && sums_ws && ymax_bits && mean && invstd && ab_ws && z, "bn_fwd: NULL pointer");
   BDBNN_REQUIRE(!pack || (mask_bits && xb), "bn_fwd: packing needs sign_bits, mask_bits and xb");
@@ -457,7 +484,28 @@ static int bn_fwd_impl(const void* y, const float* alpha_i16, const float* resid
   const int grid = bn_grid(n4, C4);
   const float4* r4 = reinterpret_cast<const float4*>(residual);
   float4* z4 = reinterpret_cast<float4*>(z);
-  if (pack) {
+  if (sub != nullptr) {
+    const uint32_t one16 = fmt == BDBNN_FMT_FP16 ? 0x3C00u : 0x3F80u;
+    uint2* xb2 = reinterpret_cast<uint2*>(xb);
+    uint32_t* xb8 = reinterpret_cast<uint32_t*>(xb_fp8);
+    if (pack && i16)
+      bn_apply_add_pack_kernel<true, true, 4, true><<<grid, kBnThreads, 0, st>>>(y, nullptr, a, b, n4, C4, z4, sign_bits,
+                                                                                mask_bits, xb2, xb8, one16, *sub);
+    else if (pack)
+      bn_apply_add_pack_kernel<true, false, 4, true><<<grid, kBnThreads, 0, st>>>(y, nullptr, a, b, n4, C4, z4, sign_bits,
+                                                                                 mask_bits, xb2, xb8, one16, *sub);
+    else if (i16)
+      bn_apply_add_pack_kernel<false, true, 4, true><<<grid, kBnThreads, 0, st>>>(y, nullptr, a, b, n4, C4, z4, nullptr,
+                                                                                 nullptr, nullptr, nullptr, 0u, *sub);
+    else
+      bn_apply_add_pack_kernel<false, false, 4, true><<<grid, kBnThreads, 0, st>>>(y, nullptr, a, b, n4, C4, z4, nullptr,
+                                                                                  nullptr, nullptr, nullptr, 0u, *sub);
+  } else if (p16) {
+    const uint32_t one16 = fmt == BDBNN_FMT_FP16 ? 0x3C00u : 0x3F80u;
+    bn_apply_add_pack_kernel<true, false, 4, false, true><<<grid, kBnThreads, 0, st>>>(
+        y, r4, a, b, n4, C4, z4, sign_bits, mask_bits, reinterpret_cast<uint2*>(xb),
+        reinterpret_cast<uint32_t*>(xb_fp8), one16);
+  } else if (pack) {
     const uint32_t one16 = fmt == BDBNN_FMT_FP16 ? 0x3C00u : 0x3F80u;
     uint2* xb2 = reinterpret_cast<uint2*>(xb);
     uint32_t* xb8 = reinterpret_cast<uint32_t*>(xb_fp8);
@@ -500,6 +548,50 @@ extern "C" int bdbnn_bn_fwd_i16(const int16_t* y_int, const float* alpha, const 
   BDBNN_REQUIRE(alpha != nullptr, "bn_fwd_i16: NULL alpha");
   return bn_fwd_impl(y_int, alpha, residual, gamma, beta, n_pix, C, eps, momentum, running_mean, running_var, sums_ws,
                      ymax_bits, mean, invstd, ab_ws, z, sign_bits, mask_bits, xb, xb_fp8, fmt, 1, stream);
+}
+
+// Geometry of the option-A residual of bdbnn_bn_fwd_pad_shortcut / _i16_pad_shortcut; n_pix of z.
+static int pad_residual(const float* x, int32_t N, int32_t H, int32_t W, int32_t Cin, int32_t pad, int32_t C,
+                        PadResidual* r, int64_t* n_pix) {
+  BDBNN_REQUIRE(x != nullptr, "bn_fwd_pad_shortcut: NULL x");
+  BDBNN_REQUIRE(N > 0 && H > 0 && W > 0 && Cin > 0, "bn_fwd_pad_shortcut: non-positive dims");
+  BDBNN_REQUIRE(Cin % 4 == 0 && pad >= 0 && pad % 4 == 0 && pad + Cin <= C,
+                "bn_fwd_pad_shortcut: needs Cin and pad multiples of 4 and pad + Cin <= C");
+  BDBNN_REQUIRE((uintptr_t(x) & 15) == 0, "bn_fwd_pad_shortcut: x must be 16-byte aligned");
+  r->x = reinterpret_cast<const float4*>(x);
+  r->H = H; r->W = W; r->Ho = (H + 1) / 2; r->Wo = (W + 1) / 2; r->Cin4 = Cin / 4; r->pad4 = pad / 4;
+  *n_pix = int64_t(N) * r->Ho * r->Wo;
+  return BDBNN_OK;
+}
+
+extern "C" int bdbnn_bn_fwd_pad_shortcut(const float* y, const float* x, int32_t N, int32_t H, int32_t W, int32_t Cin,
+                                         int32_t pad, const float* gamma, const float* beta, int32_t C, float eps,
+                                         float momentum, float* running_mean, float* running_var, double* sums_ws,
+                                         uint32_t* ymax_bits, float* mean, float* invstd, float* ab_ws, float* z,
+                                         uint32_t* sign_bits, uint32_t* mask_bits, uint16_t* xb, uint8_t* xb_fp8,
+                                         int32_t fmt, int32_t stats_ready, void* stream) {
+  PadResidual r;
+  int64_t n_pix = 0;
+  int rc = pad_residual(x, N, H, W, Cin, pad, C, &r, &n_pix);
+  if (rc) return rc;
+  return bn_fwd_impl(y, nullptr, nullptr, gamma, beta, n_pix, C, eps, momentum, running_mean, running_var, sums_ws,
+                     ymax_bits, mean, invstd, ab_ws, z, sign_bits, mask_bits, xb, xb_fp8, fmt, stats_ready, stream, &r);
+}
+
+extern "C" int bdbnn_bn_fwd_i16_pad_shortcut(const int16_t* y_int, const float* alpha, const float* x, int32_t N,
+                                             int32_t H, int32_t W, int32_t Cin, int32_t pad, const float* gamma,
+                                             const float* beta, int32_t C, float eps, float momentum,
+                                             float* running_mean, float* running_var, double* sums_ws,
+                                             uint32_t* ymax_bits, float* mean, float* invstd, float* ab_ws, float* z,
+                                             uint32_t* sign_bits, uint32_t* mask_bits, uint16_t* xb, uint8_t* xb_fp8,
+                                             int32_t fmt, void* stream) {
+  BDBNN_REQUIRE(alpha != nullptr, "bn_fwd_i16_pad_shortcut: NULL alpha");
+  PadResidual r;
+  int64_t n_pix = 0;
+  int rc = pad_residual(x, N, H, W, Cin, pad, C, &r, &n_pix);
+  if (rc) return rc;
+  return bn_fwd_impl(y_int, alpha, nullptr, gamma, beta, n_pix, C, eps, momentum, running_mean, running_var, sums_ws,
+                     ymax_bits, mean, invstd, ab_ws, z, sign_bits, mask_bits, xb, xb_fp8, fmt, 1, stream, &r);
 }
 
 static int bn_bwd_pack_impl(const float* gz, const void* y, const float* alpha_i16, const float* mean,

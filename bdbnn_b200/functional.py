@@ -883,9 +883,12 @@ class _ConvBNAddUnit(torch.autograd.Function):
     @_on_device
     def forward(ctx, x, weight, gamma, beta, residual, running_mean, running_var, momentum, eps, stride,
                 padding, xs, xm, xb, xb8, res_is_x, sc_weight=None, sc_gamma=None, sc_beta=None, sc_rm=None,
-                sc_rv=None, sc_momentum=None, sc_eps=None, sc_stride=None):
+                sc_rv=None, sc_momentum=None, sc_eps=None, sc_stride=None, sc_pad=None):
         _require_cuda(x, "conv_bn_add(x)")
         _same_device(x, weight, gamma, beta, residual, running_mean, running_var, sc_weight)
+        # sc_pad: the option-A shortcut (x[:, :, ::2, ::2] zero-padded by sc_pad channels on each side) is read in
+        # place by bn_fwd as the residual, and its gradient is added in place to this conv's (see backward)
+        ctx.sc_pad = sc_pad
         # optional real-valued 1x1 shortcut branch evaluated inside this node: its output is the residual,
         # and its input gradient is added in place to this conv's (see backward)
         ctx.n_sc = 0
@@ -974,9 +977,26 @@ class _ConvBNAddUnit(torch.autograd.Function):
         ybytes = 2 if i16 else 4
         if sc_join is not None:
             torch.cuda.current_stream().wait_stream(sc_join)
-        with _timed("bn_fwd", key, ((0 if in_conv else 4) + ybytes + 8 + (2.25 if pack else 0) +
-                                    (1 if zb8 is not None else 0)) * n_pix * cout):
-            if i16:
+        # residual bytes: a dense residual is read whole; the option-A one only over its Cin real channels
+        res_bytes = 4 * n_pix * (x.shape[1] if sc_pad is not None else cout)
+        with _timed("bn_fwd", key, ((0 if in_conv else 4) + ybytes + 4 + (2.25 if pack else 0) +
+                                    (1 if zb8 is not None else 0)) * n_pix * cout + res_bytes):
+            if sc_pad is not None:
+                xc = _nhwc(x.detach())
+                _, cin, h, w = x.shape
+                if i16:
+                    _lib.check(L.bdbnn_bn_fwd_i16_pad_shortcut(
+                        _p(y), _p(alpha), _p(xc), n, h, w, cin, int(sc_pad), _p(gamma.detach()), _p(beta.detach()),
+                        cout, float(eps), float(momentum), _p(running_mean), _p(running_var), _p(sums), _p(ymax),
+                        _p(mean), _p(invstd), _p(ab), _p(z), _p(zs), _p(zm), _p(zb), _p(zb8), fmt, st),
+                        "bn_fwd_i16_pad_shortcut")
+                else:
+                    _lib.check(L.bdbnn_bn_fwd_pad_shortcut(
+                        _p(y), _p(xc), n, h, w, cin, int(sc_pad), _p(gamma.detach()), _p(beta.detach()), cout,
+                        float(eps), float(momentum), _p(running_mean), _p(running_var), _p(sums), _p(ymax), _p(mean),
+                        _p(invstd), _p(ab), _p(z), _p(zs), _p(zm), _p(zb), _p(zb8), fmt, 1 if in_conv else 0, st),
+                        "bn_fwd_pad_shortcut")
+            elif i16:
                 _lib.check(L.bdbnn_bn_fwd_i16(_p(y), _p(alpha), _p(rc), _p(gamma.detach()), _p(beta.detach()), n_pix,
                                               cout, float(eps), float(momentum), _p(running_mean), _p(running_var),
                                               _p(sums), _p(ymax), _p(mean), _p(invstd), _p(ab), _p(z), _p(zs), _p(zm),
@@ -1010,7 +1030,7 @@ class _ConvBNAddUnit(torch.autograd.Function):
     @_on_device
     def backward(ctx, gz, _g1, _g2, _g3, _g4):
         if gz is None:
-            return (None,) * 24
+            return (None,) * 25
         L = _lib.lib()
         sh = ctx.sh
         st = _stream()
@@ -1078,6 +1098,13 @@ class _ConvBNAddUnit(torch.autograd.Function):
                                                         _p(g) if ctx.res_is_x else _p(None), _p(gx),
                                                         ctypes.byref(sh), st), "binconv_dgrad_tc")
                 _lib.count(_dgrad_launches(sh))
+            if ctx.sc_pad is not None:
+                # option-A shortcut: its gradient gz[:, pad:pad+Cin] lands on the even positions, added in place
+                n_sub = sh.N * sh.Ho * sh.Wo * sh.Cin
+                with _timed("pad_shortcut_bwd", key, 12 * n_sub):
+                    _lib.check(L.bdbnn_pad_shortcut_bwd(_p(g), _p(gx), sh.N, sh.H, sh.W, sh.Cin, cout, int(ctx.sc_pad),
+                                                        st), "pad_shortcut_bwd")
+                _lib.count(1)
         gres = gz if (ctx.has_res and ctx.needs_input_grad[4]) else None
         sc_gw = sc_dg = sc_db = None
         if ctx.n_sc:
@@ -1090,21 +1117,44 @@ class _ConvBNAddUnit(torch.autograd.Function):
             sc_db = sc_db if ctx.needs_input_grad[18] else None
         return (gx, gw, dgamma if ctx.needs_input_grad[2] else None, dbeta if ctx.needs_input_grad[3] else None,
                 gres, None, None, None, None, None, None, None, None, None, None, None,
-                sc_gw, sc_dg, sc_db, None, None, None, None, None)
+                sc_gw, sc_dg, sc_db, None, None, None, None, None, None)
+
+
+PadShortcut = collections.namedtuple("PadShortcut", "pad")
+PadShortcut.__doc__ = """The CIFAR ResNets' parameter-free option-A shortcut, F.pad(x[:, :, ::2, ::2]) with `pad` zero
+channels on each side, as a conv_bn_add `shortcut`."""
+
+
+def pad_shortcut_supported(x_shape, w_shape, stride, pad):
+    """Option-A shortcut inside the fused unit: stride 2, Cout = Cin + 2*pad, Cin and pad multiples of 4 (the BN
+    apply kernel reads the shortcut in float4 channel groups)."""
+    cin, cout = x_shape[1], w_shape[0]
+    return int(stride) == 2 and pad >= 0 and pad % 4 == 0 and cin % 4 == 0 and cout == cin + 2 * pad
 
 
 def conv_bn_add(x, weight, gamma, beta, residual, running_mean, running_var, momentum, eps, stride, padding,
                 shortcut=None):
     """z = BN_train(binconv2d(x, weight)) + residual on the fused kernels.  `shortcut` = (weight[Cout,Cin,1,1],
     gamma, beta, running_mean, running_var, momentum, eps, stride) evaluates the real-valued 1x1 conv + BN
-    `downsample` branch of x inside the same node and uses it as the residual.  The returned tensor carries
+    `downsample` branch of x inside the same node and uses it as the residual; `shortcut` = PadShortcut(pad) uses
+    the option-A shortcut of x, read in place by the BatchNorm apply, its gradient added in place to this conv's
+    input gradient (no padded tensor in either direction).  The returned tensor carries
     `_bdbnn_pack` = (sign bits, mask bits, +-1 copy, fmt, fp8 copy) of z so that a following conv_bn_add skips its
     own activation pack; x's own `_bdbnn_pack` (if present and of the current format) is consumed."""
     fmt = grad_mode()[3]
     pk = _get_act_pack(x, fmt)
     xs, xm, xb, xb8 = (pk.sign, pk.mask, pk.xb, pk.xb8) if pk is not None else (None,) * 4
     res_is_x = residual is x and x.shape[1] == weight.shape[0] and int(stride) == 1
-    if shortcut is not None:
+    if isinstance(shortcut, PadShortcut):
+        if residual is not None:
+            raise RuntimeError("conv_bn_add: pass either residual or shortcut")
+        if not pad_shortcut_supported(x.shape, weight.shape, stride, shortcut.pad):
+            raise RuntimeError(f"conv_bn_add: option-A shortcut with pad {shortcut.pad} does not fit input "
+                               f"{tuple(x.shape)}, weight {tuple(weight.shape)}, stride {stride}")
+        z, zs, zm, zb, zb8 = _ConvBNAddUnit.apply(x, weight, gamma, beta, None, running_mean, running_var, momentum,
+                                                  eps, int(stride), int(padding), xs, xm, xb, xb8, False,
+                                                  *([None] * 8), int(shortcut.pad))
+    elif shortcut is not None:
         if residual is not None:
             raise RuntimeError("conv_bn_add: pass either residual or shortcut")
         z, zs, zm, zb, zb8 = _ConvBNAddUnit.apply(x, weight, gamma, beta, None, running_mean, running_var, momentum,
@@ -1495,6 +1545,129 @@ def stem_bn_pool(y, gamma, beta, running_mean, running_var, momentum, eps, kerne
     """maxpool(BN_train(y)); the result carries `_bdbnn_pack` for the first binary conv."""
     z, zs, zm, zb, zb8 = _StemBNPool.apply(y, gamma, beta, running_mean, running_var, momentum, eps,
                                            int(kernel_size), int(stride), int(padding))
+    if zs is not None:
+        _set_act_pack(z, _ActPack(zs, zm, zb, grad_mode()[3], zb8))
+    return z
+
+
+# ---------------------------------------------------------------------------------------------------
+# CIFAR stem (DESIGN.md §4i): fp32 3x3 / stride-1 / pad-1 conv on 3 channels + BatchNorm(train), one node
+# ---------------------------------------------------------------------------------------------------
+def cifar_stem_supported(x_shape, w_shape, stride, padding):
+    """The CIFAR stem kernels' geometry: x [N,3,H,W], weight [Cout,3,3,3] with Cout in {16, 32, 48, 64}, stride 1,
+    pad 1 (stride / padding as the (h, w) pairs nn.Conv2d keeps)."""
+    if len(x_shape) != 4 or x_shape[1] != 3 or min(x_shape) < 1 or len(w_shape) != 4:
+        return False
+    cout = w_shape[0]
+    return (tuple(w_shape[1:]) == (3, 3, 3) and cout % 16 == 0 and 16 <= cout <= 64 and
+            tuple(stride) == (1, 1) and tuple(padding) == (1, 1))
+
+
+def _dense_images(x):
+    xd = x.detach()
+    if not (xd.is_contiguous() or xd.is_contiguous(memory_format=torch.channels_last)):
+        xd = xd.contiguous()
+    return xd
+
+
+class _CifarStem(torch.autograd.Function):
+    """z = BN_train(conv3x3(x, W)) for the CIFAR stem (csrc/cifar_stem.cu, csrc/bn.cu).
+    forward : cifar_stem_fwd (fp32 direct conv + BN statistics) -> bn_fwd (z + the first binary conv's packs)
+    backward: bn_bwd_pack (dgamma, dbeta, fp16 x 2^e gradient operand) -> cifar_stem_wgrad ; no input gradient.
+    Saved for backward: the images, y and the BN constants."""
+
+    @staticmethod
+    @_on_device
+    def forward(ctx, x, weight, gamma, beta, running_mean, running_var, momentum, eps):
+        _require_cuda(x, "cifar_stem_conv_bn(x)")
+        _require_cuda(weight, "cifar_stem_conv_bn(weight)")
+        _same_device(x, weight, gamma, beta, running_mean, running_var)
+        if not cifar_stem_supported(x.shape, weight.shape, (1, 1), (1, 1)):
+            raise RuntimeError(f"bdbnn_b200.cifar_stem_conv_bn: unsupported input {tuple(x.shape)} / weight "
+                               f"{tuple(weight.shape)}")
+        ctx.set_materialize_grads(False)
+        L = _lib.lib()
+        dev = x.device
+        st = _stream()
+        xd = _dense_images(x)
+        n, _, h, w = xd.shape
+        cout = weight.shape[0]
+        n_pix = n * h * w
+        key = f"cifar_stem_N{n}_{h}x{w}_c{cout}"
+        f32 = dict(dtype=torch.float32, device=dev)
+        y = torch.empty((n, cout, h, w), memory_format=torch.channels_last, **f32)
+        sums = torch.empty((2 * cout,), dtype=torch.float64, device=dev)
+        ymax = torch.empty((cout,), dtype=torch.int32, device=dev)
+        with _timed("cifar_stem_fwd", key, 4 * xd.numel() + 4 * y.numel()):
+            _lib.check(L.bdbnn_cifar_stem_fwd(_p(xd), n, h, w, *xd.stride(), _p(weight.detach().contiguous()), cout,
+                                              _p(y), _p(sums), _p(ymax), st), "cifar_stem_fwd")
+        _lib.count(2)       # conv, statistics sum
+        fmt = grad_mode()[3]
+        pack = cout % 32 == 0 or cout == 16
+        i32 = dict(dtype=torch.int32, device=dev)
+        cw = (cout + 31) // 32
+        zs = torch.empty((n, h, w, cw), **i32) if pack else None
+        zm = torch.empty((n, h, w, cw), **i32) if pack else None
+        zb = torch.empty((n, h, w, cout), dtype=torch.int16, device=dev) if pack else None
+        zb8 = torch.empty((n, h, w, cout), dtype=torch.uint8, device=dev) if (pack and cout % 32 == 0 and
+                                                                                fwd8_enabled()) else None
+        z = torch.empty_like(y)
+        mean, invstd, ab = torch.empty((cout,), **f32), torch.empty((cout,), **f32), torch.empty((2 * cout,), **f32)
+        with _timed("cifar_stem_bn_fwd", key, (8 + (2.25 if pack else 0) + (1 if zb8 is not None else 0)) * y.numel()):
+            _lib.check(L.bdbnn_bn_fwd(_p(y), None, _p(gamma.detach()), _p(beta.detach()), n_pix, cout, float(eps),
+                                      float(momentum), _p(running_mean), _p(running_var), _p(sums), _p(ymax),
+                                      _p(mean), _p(invstd), _p(ab), _p(z), _p(zs), _p(zm), _p(zb), _p(zb8), fmt, 1,
+                                      st), "bn_fwd(cifar stem)")
+        _lib.count(2)       # finalize, apply
+        ctx.geom = (n, h, w, cout)
+        ctx.w_param = weight if (weight.is_leaf and weight.requires_grad) else None
+        ctx.save_for_backward(xd, y, mean, invstd, gamma.detach(), ymax)
+        nd = [t for t in (zs, zm, zb, zb8) if t is not None]
+        if nd:
+            ctx.mark_non_differentiable(*nd)
+        return z, zs, zm, zb, zb8
+
+    @staticmethod
+    @_on_device
+    def backward(ctx, gz, *_unused):
+        if gz is None or not (ctx.needs_input_grad[1] or ctx.needs_input_grad[2] or ctx.needs_input_grad[3]):
+            return (None,) * 8
+        L = _lib.lib()
+        xd, y, mean, invstd, gamma, ymax = ctx.saved_tensors
+        n, h, w, cout = ctx.geom
+        n_pix = n * h * w
+        dev = gz.device
+        st = _stream()
+        key = f"cifar_stem_N{n}_{h}x{w}_c{cout}"
+        g = _nhwc(gz)
+        i32 = dict(dtype=torch.int32, device=dev)
+        f32 = dict(dtype=torch.float32, device=dev)
+        sums = torch.empty((2 * cout,), dtype=torch.float64, device=dev)
+        gmax, amax = torch.empty((cout,), **i32), torch.empty((1,), **i32)
+        consts, dgamma, dbeta = torch.empty((4 * cout,), **f32), torch.empty((cout,), **f32), torch.empty((cout,), **f32)
+        ones = torch.ones((cout,), **f32)
+        gys = torch.empty((n, h, w, cout), dtype=torch.int16, device=dev)
+        with _timed("cifar_stem_bn_bwd", key, 18 * n_pix * cout):
+            _lib.check(L.bdbnn_bn_bwd_pack(_p(g), _p(y), _p(mean), _p(invstd), _p(gamma), _p(ones), _p(ymax), n_pix,
+                                           cout, 3, _p(sums), _p(gmax), _p(consts), _p(dgamma), _p(dbeta), _p(amax),
+                                           _p(gys), st), "bn_bwd_pack(cifar stem)")
+        _lib.count(3)
+        gw = None
+        if ctx.needs_input_grad[1]:
+            gw = _wgrad_launch(
+                lambda gwp, ws, ws_bytes, s: _lib.check(L.bdbnn_cifar_stem_wgrad(
+                    _p(xd), n, h, w, *xd.stride(), _p(gys), _p(amax), cout, gwp, ws, ws_bytes, s), "cifar_stem_wgrad"),
+                int(L.bdbnn_cifar_stem_wgrad_workspace_bytes(n, h, w, cout)), (cout, 3, 3, 3), ctx.w_param,
+                (xd, gys, amax), "cifar_stem_wgrad", key, 4 * xd.numel() + 2 * gys.numel())
+        return (None, gw, dgamma if ctx.needs_input_grad[2] else None, dbeta if ctx.needs_input_grad[3] else None,
+                None, None, None, None)
+
+
+def cifar_stem_conv_bn(x, weight, gamma, beta, running_mean, running_var, momentum, eps):
+    """BN_train(conv2d(x, weight, stride 1, pad 1)) of the CIFAR stem (see cifar_stem_supported) as one node: fp32
+    conv, BatchNorm with its running-statistics update (the caller adds 1 to num_batches_tracked), TF32-class weight
+    gradient, no input gradient.  The result carries `_bdbnn_pack` for the first binary conv."""
+    z, zs, zm, zb, zb8 = _CifarStem.apply(x, weight, gamma, beta, running_mean, running_var, momentum, eps)
     if zs is not None:
         _set_act_pack(z, _ActPack(zs, zm, zb, grad_mode()[3], zb8))
     return z

@@ -231,18 +231,47 @@ class BasicBlockCifar(nn.Module):
         self.shortcut = _PadShortcut(planes) if (stride != 1 or inplanes != planes) else None
 
     def forward(self, x):
-        residual = x if self.shortcut is None else self.shortcut(x)
-        out = _eval_unit(x, self.conv1, self.bn1, residual)
+        out = None
+        if self.shortcut is not None and F_.shortcut_tc_enabled():
+            # conv1 + bn1 + the option-A shortcut as ONE node: bn_fwd reads the shortcut in place as the residual,
+            # and its gradient is added in place to conv1's input gradient (BDBNN_SHORTCUT_TC=0: _PadShortcut)
+            sc = F_.PadShortcut(self.shortcut.pad)
+            if F_.pad_shortcut_supported(x.shape, self.conv1.weight.shape, self.conv1.stride[0], sc.pad):
+                out = _fused_unit(x, self.conv1, self.bn1, None, shortcut=sc)
         if out is None:
-            out = _fused_unit(x, self.conv1, self.bn1, residual)
-        if out is None:
-            out = self.bn1(self.conv1(x)) + residual
+            out = self._conv1_unit(x)
         out2 = _eval_unit(out, self.conv2, self.bn2, out)
         if out2 is None:
             out2 = _fused_unit(out, self.conv2, self.bn2, out)
         if out2 is None:
             out2 = self.bn2(self.conv2(out)) + out
         return out2
+
+    def _conv1_unit(self, x):
+        residual = x if self.shortcut is None else self.shortcut(x)
+        out = _eval_unit(x, self.conv1, self.bn1, residual)
+        if out is None:
+            out = _fused_unit(x, self.conv1, self.bn1, residual)
+        if out is None:
+            out = self.bn1(self.conv1(x)) + residual
+        return out
+
+
+def _cifar_stem_qualifies(x, c1, bn):
+    """Whether the CIFAR stem conv1 + bn1 runs as functional.cifar_stem_conv_bn: training mode on a CUDA fp32 batch
+    of 3-channel images that does not require grad, a bias-free 3x3 / stride-1 / pad-1 nn.Conv2d, an affine
+    BatchNorm2d that tracks running statistics, and neither BDBNN_STEM_TC=0 nor BDBNN_FUSE_BN=0."""
+    if not (type(c1) is nn.Conv2d and isinstance(bn, nn.BatchNorm2d) and bn.training and F_.fuse_enabled() and
+            F_.stem_tc_enabled()):
+        return False
+    if not (x.is_cuda and x.dtype == torch.float32 and c1.weight.dtype == torch.float32 and
+            not (x.requires_grad and torch.is_grad_enabled())):
+        return False
+    if c1.bias is not None or c1.groups != 1 or c1.dilation != (1, 1) or c1.padding_mode != "zeros":
+        return False
+    if not (bn.affine and bn.track_running_stats and bn.momentum is not None and bn.num_features == c1.out_channels):
+        return False
+    return F_.cifar_stem_supported(tuple(x.shape), tuple(c1.weight.shape), c1.stride, c1.padding)
 
 
 class ResNetCifar(nn.Module):
@@ -269,13 +298,21 @@ class ResNetCifar(nn.Module):
     def forward(self, x):
         packed = _prepack(self, x)
         try:
-            # fp32 stem on cuDNN: TF32 off, or cuDNN may pick a TF32 algorithm for some batch sizes (on the H100 at
-            # batch 8 but not 16), and the binary layers behind it amplify that 1e-3 difference into different signs
-            cudnn = torch.backends.cudnn
-            with cudnn.flags(enabled=cudnn.enabled, benchmark=cudnn.benchmark, deterministic=cudnn.deterministic,
-                             allow_tf32=False):
-                x = self.conv1(x)
-            x = self.bn1(x)
+            c1, bn = self.conv1, self.bn1
+            if _cifar_stem_qualifies(x, c1, bn):
+                # fp32 direct conv + BatchNorm(train) on this repository's kernels, handing layer1.0.conv1 its packs
+                x = F_.cifar_stem_conv_bn(x, c1.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var,
+                                          bn.momentum, bn.eps)
+                bn.num_batches_tracked.add_(1)
+            else:
+                # fp32 stem on cuDNN: TF32 off, or cuDNN may pick a TF32 algorithm for some batch sizes (on the H100 at
+                # batch 8 but not 16), and the binary layers behind it amplify that 1e-3 difference into different
+                # signs
+                cudnn = torch.backends.cudnn
+                with cudnn.flags(enabled=cudnn.enabled, benchmark=cudnn.benchmark, deterministic=cudnn.deterministic,
+                                 allow_tf32=False):
+                    x = c1(x)
+                x = bn(x)
             x = self.layer3(self.layer2(self.layer1(x)))
         finally:
             if packed:

@@ -322,6 +322,53 @@ BDBNN_API int bdbnn_binconv_dgrad_tc_stats(const uint16_t* gys_bf16, int32_t gra
                                  const float* prod_mean, const float* prod_invstd, double* prod_sums,
                                  uint32_t* prod_gmax, void* stream);
 
+/* bdbnn_bn_fwd with C == 16 and sign_bits != NULL writes ONE sign / mask word per pixel (bits 0-15; bits 16-31
+ * are 0, as bdbnn_act_pack writes them for 16 channels): the packs of the CIFAR stem's BatchNorm output for the
+ * first 16-channel binary conv.  (fp32 y only; not with bdbnn_bn_fwd_i16.)
+ *
+ * Option-A shortcut of the CIFAR ResNets (stride-2 subsample + zero channel padding) as the residual, read in place:
+ * bn_fwd_pad_shortcut / bn_fwd_i16_pad_shortcut = bdbnn_bn_fwd / bdbnn_bn_fwd_i16 with
+ *   residual[n,i,j,c] = x[n,2i,2j,c-pad] for pad <= c < pad+Cin, else 0
+ * x fp32 NHWC [N,H,W,Cin] (16-byte aligned); z [N,Ho,Wo,C] with Ho = ceil(H/2), Wo = ceil(W/2), n_pix = N*Ho*Wo.
+ * Needs Cin % 4 == 0, pad % 4 == 0, pad + Cin <= C.  Results equal bn_fwd with that residual materialised.
+ * pad_shortcut_bwd: the shortcut's gradient added in place to the block input's, gx fp32 NHWC [N,H,W,Cin]:
+ *   gx[n,2i,2j,c] += gz[n,i,j,c+pad]   (gz fp32 NHWC [N,Ho,Wo,Cout]; same conditions, Cout % 4 == 0). */
+BDBNN_API int bdbnn_bn_fwd_pad_shortcut(const float* y, const float* x, int32_t N, int32_t H, int32_t W, int32_t Cin,
+                              int32_t pad, const float* gamma, const float* beta, int32_t C, float eps,
+                              float momentum, float* running_mean, float* running_var, double* sums_ws,
+                              uint32_t* ymax_bits, float* mean, float* invstd, float* ab_ws, float* z,
+                              uint32_t* sign_bits, uint32_t* mask_bits, uint16_t* xb, uint8_t* xb_fp8, int32_t fmt,
+                              int32_t stats_ready, void* stream);
+BDBNN_API int bdbnn_bn_fwd_i16_pad_shortcut(const int16_t* y_int, const float* alpha, const float* x, int32_t N,
+                                  int32_t H, int32_t W, int32_t Cin, int32_t pad, const float* gamma,
+                                  const float* beta, int32_t C, float eps, float momentum, float* running_mean,
+                                  float* running_var, double* sums_ws, uint32_t* ymax_bits, float* mean,
+                                  float* invstd, float* ab_ws, float* z, uint32_t* sign_bits, uint32_t* mask_bits,
+                                  uint16_t* xb, uint8_t* xb_fp8, int32_t fmt, void* stream);
+BDBNN_API int bdbnn_pad_shortcut_bwd(const float* gz, float* gx, int32_t N, int32_t H, int32_t W, int32_t Cin,
+                           int32_t Cout, int32_t pad, void* stream);
+
+/* ---- CIFAR stem: 3x3 / stride 1 / pad 1, 3 -> Cout channels (Cout in {16, 32, 48, 64}), fp32, CUDA cores ------
+ * Replaces the fp32 nn.Conv2d `conv1` of the CIFAR ResNets (models/cifar10; model(images), train.py:492 and its
+ * weight gradient under loss.backward(), train.py:528), which the reference runs on cuDNN.
+ *   cifar_stem_fwd   : y fp32 NHWC [N,H,W,Cout] = conv(x, W): one fp32 FMA per tap, taps in the order (c, r, s), no
+ *                      reduced-precision operands.  x [N,3,H,W] through element strides (NCHW or channels_last),
+ *                      weight contiguous [Cout][3][3][3]; y 16-byte aligned.  bn_sums / bn_ymax (both or neither):
+ *                      the BatchNorm statistics of y as bdbnn_binconv_fwd_tc writes them (for bdbnn_bn_fwd with
+ *                      stats_ready = 1), from per-block partials summed in a fixed order; zeroed here.
+ *   cifar_stem_wgrad : gW fp32 [Cout][3][3][3] (overwritten) = 2^-e * sum_pix x_tap(pix) * gys[pix][o], gys =
+ *                      fp16(gy * 2^e) [N,H,W,Cout] with e from g_amax_bits (bdbnn_bn_bwd_pack, FP16S, gscale = 1):
+ *                      TF32-class.  fp32 sums per block, block partials (in the workspace, of
+ *                      bdbnn_cifar_stem_wgrad_workspace_bytes) added in block order by a finalize kernel.
+ * Two launches (+ the statistics' fixed-order sum) forward, two backward; no input gradient. */
+BDBNN_API int bdbnn_cifar_stem_fwd(const float* x, int32_t N, int32_t H, int32_t W, int64_t sN, int64_t sC,
+                         int64_t sH, int64_t sW, const float* weight, int32_t Cout, float* y, double* bn_sums,
+                         uint32_t* bn_ymax, void* stream);
+BDBNN_API size_t bdbnn_cifar_stem_wgrad_workspace_bytes(int32_t N, int32_t H, int32_t W, int32_t Cout);
+BDBNN_API int bdbnn_cifar_stem_wgrad(const float* x, int32_t N, int32_t H, int32_t W, int64_t sN, int64_t sC,
+                           int64_t sH, int64_t sW, const uint16_t* gys, const uint32_t* g_amax_bits, int32_t Cout,
+                           float* gW, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- stem: BatchNorm(train) + MaxPool fused (the BN output is never written) -----------------------
  * bn_pool_fwd: y fp32 NHWC [N,H,W,C] (stem conv output) -> z = maxpool_k,s,p(gamma*(y-mean)*invstd+beta)
  *              [N,Ho,Wo,C], idx = winning tap per output element (1 byte), y_sel = y at the winner;
