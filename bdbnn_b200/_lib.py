@@ -90,6 +90,11 @@ SIGNATURES = {
     "bdbnn_pad_shortcut_bwd": (c_int, [_P, _P] + [c_int] * 6 + [_P]),
     "bdbnn_cifar_stem_fwd": (c_int, [_P, c_int, c_int, c_int, c_int64, c_int64, c_int64, c_int64, _P, c_int, _P, _P, _P,
                                      _P]),
+    "bdbnn_cifar_stem_fwd_eval": (c_int, [_P, c_int, c_int, c_int, c_int64, c_int64, c_int64, c_int64, _P, c_int] +
+                                  [_P] * 5),
+    "bdbnn_binconv_fwd_tc_eval_pad_shortcut": (c_int, [_P, _P, c_int, _P, _P, _P] + [c_int] * 4 + [_P, _P, _P, _SH,
+                                                                                                 _P]),
+    "bdbnn_real_conv_fwd_eval_pad_shortcut": (c_int, [_P] * 6 + [c_int] * 5 + [_P, _P, _SH, _P]),
     "bdbnn_cifar_stem_wgrad_workspace_bytes": (c_size_t, [c_int] * 4),
     "bdbnn_cifar_stem_wgrad": (c_int, [_P, c_int, c_int, c_int, c_int64, c_int64, c_int64, c_int64, _P, _P, c_int, _P,
                                        _P, c_size_t, _P]),

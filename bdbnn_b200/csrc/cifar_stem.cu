@@ -39,10 +39,14 @@ __device__ __forceinline__ void cifar_stem_taps(const float* __restrict__ x, int
 // One thread per output pixel, kCsGroup output channels per block row (blockIdx.y).  If part != NULL, the block's
 // per-channel sum y and sum y^2 (warp butterflies in fp32, then the warps in order in fp64) go to its row of part
 // ([gridDim.x][2*Cout]) and max|y| to ymax (integer atomicMax of the bits: order-free).
+// EVAL: the eval-mode BatchNorm folded into the epilogue instead, y = fp32(fp32(acc * scale[o]) + shift[o]) (no FMA
+// contraction, as tc_conv_kernel's eval epilogue), and the bits of max|y| over all channels into ymax[0].
+template <bool EVAL>
 __global__ void __launch_bounds__(kCsThreads)
 cifar_stem_fwd_kernel(const float* __restrict__ x, int N, int H, int W, int64_t sN, int64_t sC, int64_t sH,
                       int64_t sW, const float* __restrict__ wt, int Cout, float* __restrict__ y,
-                      double* __restrict__ part, uint32_t* __restrict__ ymax) {
+                      double* __restrict__ part, uint32_t* __restrict__ ymax, const float* __restrict__ scale,
+                      const float* __restrict__ shift) {
   __shared__ float ws[kCsGroup][kCsTaps];
   __shared__ float red_s[kCsThreads / 32][kCsGroup], red_q[kCsThreads / 32][kCsGroup];
   __shared__ float red_m[kCsThreads / 32][kCsGroup];
@@ -66,10 +70,24 @@ cifar_stem_fwd_kernel(const float* __restrict__ x, int N, int H, int W, int64_t 
     for (int t = 0; t < kCsTaps; ++t)
 #pragma unroll
       for (int o = 0; o < kCsGroup; ++o) acc[o] = fmaf(v[t], ws[o][t], acc[o]);
+    if (EVAL) {
+#pragma unroll
+      for (int o = 0; o < kCsGroup; ++o)
+        acc[o] = __fadd_rn(__fmul_rn(acc[o], __ldg(scale + o0 + o)), __ldg(shift + o0 + o));
+    }
     float4* dst = reinterpret_cast<float4*>(y + p * Cout + o0);
 #pragma unroll
     for (int k = 0; k < kCsGroup / 4; ++k)
       dst[k] = make_float4(acc[4 * k], acc[4 * k + 1], acc[4 * k + 2], acc[4 * k + 3]);
+  }
+  if (EVAL) {   // max|z| as integer bits (NaN above every number): order-free, the same bits every run
+    uint32_t m = 0u;
+    if (valid)
+#pragma unroll
+      for (int o = 0; o < kCsGroup; ++o) m = max(m, __float_as_uint(fabsf(acc[o])));
+    m = __reduce_max_sync(0xffffffffu, m);
+    if ((threadIdx.x & 31) == 0 && m != 0u) atomicMax(ymax, m);
+    return;
   }
   if (part == nullptr) return;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -214,11 +232,28 @@ extern "C" int bdbnn_cifar_stem_fwd(const float* x, int32_t N, int32_t H, int32_
     int rc = det_sums_alloc(&part, grid.x, 2 * Cout, st);
     if (rc) return rc;
   }
-  cifar_stem_fwd_kernel<<<grid, kCsThreads, 0, st>>>(x, N, H, W, sN, sC, sH, sW, weight, Cout, y, part, bn_ymax);
+  cifar_stem_fwd_kernel<false><<<grid, kCsThreads, 0, st>>>(x, N, H, W, sN, sC, sH, sW, weight, Cout, y, part,
+                                                            bn_ymax, nullptr, nullptr);
   int rc = check_launch("cifar_stem_fwd_kernel");
   if (part == nullptr) return rc;
   if (rc) { cudaFreeAsync(part, st); return rc; }
   return det_sums_finish(part, grid.x, 2 * Cout, bn_sums, st);
+}
+
+extern "C" int bdbnn_cifar_stem_fwd_eval(const float* x, int32_t N, int32_t H, int32_t W, int64_t sN, int64_t sC,
+                                         int64_t sH, int64_t sW, const float* weight, int32_t Cout, const float* scale,
+                                         const float* shift, float* z, uint32_t* z_amax_bits, void* stream) {
+  BDBNN_REQUIRE(N > 0 && H > 0 && W > 0, "cifar_stem_fwd_eval: non-positive dims");
+  BDBNN_REQUIRE(cifar_stem_cout_ok(Cout), "cifar_stem_fwd_eval: Cout must be 16, 32, 48 or 64");
+  BDBNN_REQUIRE(x && weight && scale && shift && z && z_amax_bits, "cifar_stem_fwd_eval: NULL pointer");
+  BDBNN_REQUIRE((uintptr_t(z) & 15) == 0, "cifar_stem_fwd_eval: z must be 16-byte aligned");
+  cudaStream_t st = cudaStream_t(stream);
+  const int64_t n_pix = int64_t(N) * H * W;
+  const dim3 grid(unsigned((n_pix + kCsThreads - 1) / kCsThreads), unsigned(Cout / kCsGroup));
+  BDBNN_CUDA(cudaMemsetAsync(z_amax_bits, 0, sizeof(uint32_t), st));
+  cifar_stem_fwd_kernel<true><<<grid, kCsThreads, 0, st>>>(x, N, H, W, sN, sC, sH, sW, weight, Cout, z, nullptr,
+                                                           z_amax_bits, scale, shift);
+  return check_launch("cifar_stem_fwd_eval_kernel");
 }
 
 extern "C" size_t bdbnn_cifar_stem_wgrad_workspace_bytes(int32_t N, int32_t H, int32_t W, int32_t Cout) {

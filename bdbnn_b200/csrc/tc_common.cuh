@@ -363,6 +363,9 @@ struct TcConvLaunch {
                                  // epilogue multiplies the accumulator by 2^-e
   const float* add;              // dgrad: optional tensor added to the result (shortcut gradient), or NULL;
                                  // eval: optional residual added to z
+  // eval, 16-bit operands: pad_res = 1 reads the residual as the option-A shortcut add[n][2*oh][2*ow][c - res_coff]
+  // of an NHWC [.][res_H][res_W][res_C] tensor, +0.0 outside the channel band (tc_conv_kernel's PADRES instances)
+  int pad_res, res_H, res_W, res_C, res_coff;
   // eval forward (MODE 2): z = acc * alpha + shift (+ add) written to `out`, optional +-1 copies of z
   const float* shift; uint16_t* zb; uint8_t* zb8;
   int relu;                      // eval: z = relu(z) after the residual

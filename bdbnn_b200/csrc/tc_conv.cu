@@ -54,6 +54,9 @@ struct TcConvParams {
   double* stat_part;         // this launch's per-CTA statistics rows [gridDim.x][2*Nout] (det_sums_finish adds them)
   uint32_t* bn_ymax;
   const int16_t* st_y; const float* st_alpha; const float* st_mean; const float* st_invstd;   // MODE 1 statistics
+  // PADRES instances: output pixel (n, oh, ow), channel ch reads the residual add[n][2*oh][2*ow][ch - res_coff] of an
+  // NHWC [.][res_H][res_W][res_C] tensor inside the band res_coff <= ch < res_coff + res_C, +0.0 outside it
+  int32_t res_H, res_W, res_C, res_coff;
 };
 
 // MODE: 0 forward, 1 dgrad, 2 eval forward; KIND: 0 fp16, 1 bf16, 2 fp8 e4m3 operands; NW: wgmma N (16, 32, or 64
@@ -62,7 +65,9 @@ struct TcConvParams {
 // 16K-register sub-partitions, and 2 x 9 warps put five warps on two of them.  The dgrad and eval instances ask for
 // that bound (without it the NW = 64 dgrad ones took 102 registers and ran one CTA per SM); the forward ones fit at
 // 96 without it (0 = no minimum).  bdbnn_debug_tc_conv_ctas_per_sm reports the residency.
-template <int MODE, int KIND, int NW>
+// PADRES (MODE 2, 16-bit operands only): the residual is the CIFAR option-A shortcut read in place (res_* fields),
+// an instance of its own so that the dense-residual instances keep their code.
+template <int MODE, int KIND, int NW, bool PADRES = false>
 __global__ void __launch_bounds__(kTcThreads, MODE == 0 ? 0 : 2)
 tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const TcConvParams p) {
@@ -172,7 +177,7 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const float post = (MODE != 0 && p.amax_bits) ? amax_pow2_scale(__ldg(p.amax_bits), true) : 1.0f;
     uint32_t zmax = 0u;                     // MODE 2: bits of this thread's max|z| (ordered as integers, NaN on top)
     const int mask_words = (p.Nout + 31) >> 5;
-    int64_t pix[2];
+    int64_t pix[2], rpix[2];                // rpix: PADRES residual pixel
     bool valid[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -183,6 +188,7 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       const int oh = (h0 + hi) * p.out_step + p.out_off_h, ow = wi * p.out_step + p.out_off_w;
       valid[h] = (ni < p.BNI) && (h0 + hi < p.OH) && (n0 + ni < p.NIMG) && oh < p.OHf && ow < p.OWf;
       pix[h] = (int64_t(n0 + ni) * p.OHf + oh) * p.OWf + ow;
+      if (PADRES) rpix[h] = (int64_t(n0 + ni) * p.res_H + 2 * oh) * p.res_W + 2 * ow;
     }
 #pragma unroll
     for (int c = 0; c < NCH; ++c) {
@@ -229,7 +235,15 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             // post = 2^-ex of real-valued operands (exact), 1 for the +-1 operands.
             o0 = __fadd_rn(__fmul_rn(__fmul_rn(v0, post), a0), sb0);
             o1 = __fadd_rn(__fmul_rn(__fmul_rn(v1, post), a1), sb1);
-            if (p.add != nullptr) {          // the residual never aliases z (bdbnn_binconv_fwd_tc_eval rejects it)
+            if (PADRES) {
+              // outside the channel band the residual is +0.0 and is still added: -0.0 + 0.0 = +0.0, as the
+              // materialised zero-padded tensor gives (ch and the band edges are even, so a pair is in or out)
+              float2 r = make_float2(0.f, 0.f);
+              const int rc = ch - p.res_coff;
+              if (unsigned(rc) < unsigned(p.res_C))
+                r = __ldg(reinterpret_cast<const float2*>(p.add + rpix[h] * p.res_C + rc));
+              o0 = __fadd_rn(o0, r.x); o1 = __fadd_rn(o1, r.y);
+            } else if (p.add != nullptr) {   // the residual never aliases z (the entry points reject it)
               const float2 r = __ldg(reinterpret_cast<const float2*>(p.add + off));
               o0 = __fadd_rn(o0, r.x); o1 = __fadd_rn(o1, r.y);
             }
@@ -374,6 +388,10 @@ static bool plan_tc_conv(const TcConvLaunch& L, int mode, TcConvParams* pp, size
   p.alpha = L.alpha; p.mask = L.mask; p.out = L.out; p.out_i16 = mode == 0 ? L.out_i16 : nullptr;
   p.shift = L.shift; p.zb = L.zb; p.zb8 = L.zb8; p.zb_one = L.fmt == BDBNN_FMT_BF16 ? 0x3F80u : 0x3C00u;
   p.amax_bits = L.amax_bits; p.add = L.add; p.relu = L.relu; p.z_amax = L.z_amax;
+  if (L.pad_res) {
+    if (mode != 2 || L.fmt < 0 || !L.add) return false;
+    p.res_H = L.res_H; p.res_W = L.res_W; p.res_C = L.res_C; p.res_coff = L.res_coff;
+  }
   p.bn_sums = L.bn_sums; p.bn_ymax = L.bn_ymax;
   p.st_y = L.st_y; p.st_alpha = L.st_alpha; p.st_mean = L.st_mean; p.st_invstd = L.st_invstd;
   const uint32_t stage_bytes = (uint32_t(kTileM + p.BN) * p.row_bytes + 1023u) & ~1023u;
@@ -413,11 +431,11 @@ static int launch_one(K kern, dim3 grid, size_t smem, cudaStream_t st, const CUt
   return check_launch("tc_conv_kernel");
 }
 
-template <int MODE, int KIND>
+template <int MODE, int KIND, bool PADRES = false>
 static int launch_kind(const CUtensorMap& tmA, const CUtensorMap& tmB, const TcConvParams& p, size_t smem, dim3 grid,
                        cudaStream_t st) {
-  auto kern = p.BN == 16 ? tc_conv_kernel<MODE, KIND, 16>
-                         : (p.BN == 32 ? tc_conv_kernel<MODE, KIND, 32> : tc_conv_kernel<MODE, KIND, 64>);
+  auto kern = p.BN == 16 ? tc_conv_kernel<MODE, KIND, 16, PADRES>
+                         : (p.BN == 32 ? tc_conv_kernel<MODE, KIND, 32, PADRES> : tc_conv_kernel<MODE, KIND, 64, PADRES>);
   BDBNN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
   if (p.bn_sums == nullptr) return launch_one(kern, grid, smem, st, tmA, tmB, p);
   TcConvParams q = p;
@@ -459,6 +477,11 @@ static int launch_tc_conv(const TcConvLaunch& L, cudaStream_t st) {
     } else {
       return launch_kind<MODE, 2>(tmA, tmB, p, smem, grid, st);
     }
+  }
+  if constexpr (MODE == 2) {
+    if (L.pad_res)
+      return L.fmt == BDBNN_FMT_BF16 ? launch_kind<2, 1, true>(tmA, tmB, p, smem, grid, st)
+                                     : launch_kind<2, 0, true>(tmA, tmB, p, smem, grid, st);
   }
   rc = L.fmt == BDBNN_FMT_BF16 ? launch_kind<MODE, 1>(tmA, tmB, p, smem, grid, st)
                                : launch_kind<MODE, 0>(tmA, tmB, p, smem, grid, st);
@@ -574,14 +597,20 @@ extern "C" int bdbnn_debug_conv_plan(const bdbnn_conv_shape* s, int32_t mode, in
 }
 
 // CTAs of one tc_conv_kernel instance that fit on an SM with `smem` bytes of dynamic shared memory (the dynamic smem
-// entry of bdbnn_debug_conv_plan).  mode 0 forward / 1 dgrad / 2 eval forward, fmt BDBNN_FMT_FP16 / BF16 or -1 (fp8,
-// forward and eval only), bn = N tile (16, 32, 64 or 128).
+// entry of bdbnn_debug_conv_plan).  mode 0 forward / 1 dgrad / 2 eval forward / 3 eval forward with the option-A
+// residual, fmt BDBNN_FMT_FP16 / BF16 or -1 (fp8, forward and dense eval only), bn = N tile (16, 32, 64 or 128).
 extern "C" int bdbnn_debug_tc_conv_ctas_per_sm(int32_t mode, int32_t fmt, int32_t bn, int32_t smem, int32_t* ctas) {
-  BDBNN_REQUIRE(ctas && mode >= 0 && mode <= 2 && (bn == 16 || bn == 32 || bn == 64 || bn == 128) && smem >= 0 &&
-                    (fmt == BDBNN_FMT_FP16 || fmt == BDBNN_FMT_BF16 || (fmt == -1 && mode != 1)),
+  BDBNN_REQUIRE(ctas && mode >= 0 && mode <= 3 && (bn == 16 || bn == 32 || bn == 64 || bn == 128) && smem >= 0 &&
+                    (fmt == BDBNN_FMT_FP16 || fmt == BDBNN_FMT_BF16 || (fmt == -1 && (mode == 0 || mode == 2))),
                 "debug_tc_conv_ctas_per_sm: bad arguments");
   const void* kern;
-  if (mode == 2 && fmt == -1)
+  if (mode == 3 && fmt == BDBNN_FMT_FP16)
+    kern = bn == 16 ? (const void*)tc_conv_kernel<2, 0, 16, true> : bn == 32 ? (const void*)tc_conv_kernel<2, 0, 32, true>
+                                                                   : (const void*)tc_conv_kernel<2, 0, 64, true>;
+  else if (mode == 3)
+    kern = bn == 16 ? (const void*)tc_conv_kernel<2, 1, 16, true> : bn == 32 ? (const void*)tc_conv_kernel<2, 1, 32, true>
+                                                                   : (const void*)tc_conv_kernel<2, 1, 64, true>;
+  else if (mode == 2 && fmt == -1)
     kern = bn == 16 ? (const void*)tc_conv_kernel<2, 2, 16> : bn == 32 ? (const void*)tc_conv_kernel<2, 2, 32>
                                                              : (const void*)tc_conv_kernel<2, 2, 64>;
   else if (mode == 2 && fmt == BDBNN_FMT_FP16)
@@ -745,6 +774,68 @@ extern "C" int bdbnn_real_conv_fwd_eval(const uint16_t* xh, const uint32_t* x_am
   fwd_launch(&L, xh, wf, BDBNN_FMT_FP16, s);
   L.amax_bits = x_amax_bits;
   L.alpha = scale; L.shift = shift; L.add = residual; L.out = z; L.relu = relu != 0; L.z_amax = z_amax_bits;
+  if (z_amax_bits) BDBNN_CUDA(cudaMemsetAsync(z_amax_bits, 0, sizeof(uint32_t), st));
+  return launch_tc_conv<2>(L, st);
+}
+
+// The option-A shortcut of a stride-2 conv as the eval epilogue's residual, read in place from x_res (NHWC fp32
+// [N][H_res][W_res][C_res]): r[n,i,j,c] = x_res[n,2i,2j,c-pad] for pad <= c < pad + C_res, else +0.0.
+static int pad_residual(TcConvLaunch* L, const float* x_res, int32_t H_res, int32_t W_res, int32_t C_res, int32_t pad,
+                        const float* z, const bdbnn_conv_shape* s) {
+  BDBNN_REQUIRE(x_res != nullptr, "pad_shortcut: NULL x_res");
+  BDBNN_REQUIRE(x_res != z, "pad_shortcut: x_res must not alias z");
+  BDBNN_REQUIRE((uintptr_t(x_res) & 15) == 0, "pad_shortcut: x_res must be 16-byte aligned");
+  BDBNN_REQUIRE(H_res > 0 && W_res > 0 && C_res > 0 && pad >= 0, "pad_shortcut: non-positive x_res dims or pad < 0");
+  BDBNN_REQUIRE(C_res % 4 == 0 && pad % 4 == 0, "pad_shortcut: C_res and pad must be multiples of 4");
+  BDBNN_REQUIRE(s->Cout == C_res + 2 * pad, "pad_shortcut: Cout %d != C_res + 2 * pad = %d", s->Cout, C_res + 2 * pad);
+  BDBNN_REQUIRE(s->stride == 2 && s->Ho == (H_res + 1) / 2 && s->Wo == (W_res + 1) / 2,
+                "pad_shortcut: needs a stride-2 conv with Ho = ceil(H_res / 2), Wo = ceil(W_res / 2)");
+  L->add = x_res;
+  L->pad_res = 1; L->res_H = H_res; L->res_W = W_res; L->res_C = C_res; L->res_coff = pad;
+  return BDBNN_OK;
+}
+
+extern "C" int bdbnn_binconv_fwd_tc_eval_pad_shortcut(const void* xb, const void* wf, int32_t fmt, const float* scale,
+                                                      const float* shift, const float* x_res, int32_t H_res,
+                                                      int32_t W_res, int32_t C_res, int32_t pad, float* z,
+                                                      uint16_t* zb, uint8_t* zb8, const bdbnn_conv_shape* s,
+                                                      void* stream) {
+  BDBNN_REQUIRE(fmt == BDBNN_FMT_FP16 || fmt == BDBNN_FMT_BF16,
+                "binconv_fwd_tc_eval_pad_shortcut: needs 16-bit operands (BDBNN_FMT_FP16 / BF16)");
+  int rc = validate_shape(s);
+  if (rc) return rc;
+  BDBNN_REQUIRE(xb && wf && scale && shift && z, "binconv_fwd_tc_eval_pad_shortcut: NULL pointer");
+  TcConvLaunch L;
+  fwd_launch(&L, xb, wf, fmt, s);
+  rc = pad_residual(&L, x_res, H_res, W_res, C_res, pad, z, s);
+  if (rc) return rc;
+  if (!tc_shape_ok(s)) {
+    set_error("binconv_fwd_tc_eval_pad_shortcut: shape not supported by the tensor-core path");
+    return BDBNN_ERR_UNSUPPORTED;
+  }
+  L.alpha = scale; L.shift = shift; L.out = z; L.zb = zb; L.zb8 = zb8;
+  return launch_tc_conv<2>(L, cudaStream_t(stream));
+}
+
+extern "C" int bdbnn_real_conv_fwd_eval_pad_shortcut(const uint16_t* xh, const uint32_t* x_amax_bits,
+                                                     const uint16_t* wf, const float* scale, const float* shift,
+                                                     const float* x_res, int32_t H_res, int32_t W_res, int32_t C_res,
+                                                     int32_t pad, int32_t relu, float* z, uint32_t* z_amax_bits,
+                                                     const bdbnn_conv_shape* s, void* stream) {
+  int rc = validate_shape(s);
+  if (rc) return rc;
+  BDBNN_REQUIRE(xh && x_amax_bits && wf && scale && shift && z, "real_conv_fwd_eval_pad_shortcut: NULL pointer");
+  TcConvLaunch L;
+  fwd_launch(&L, xh, wf, BDBNN_FMT_FP16, s);
+  rc = pad_residual(&L, x_res, H_res, W_res, C_res, pad, z, s);
+  if (rc) return rc;
+  if (!tc_shape_ok(s)) {
+    set_error("real_conv_fwd_eval_pad_shortcut: shape not supported by the tensor-core path");
+    return BDBNN_ERR_UNSUPPORTED;
+  }
+  cudaStream_t st = cudaStream_t(stream);
+  L.amax_bits = x_amax_bits;
+  L.alpha = scale; L.shift = shift; L.out = z; L.relu = relu != 0; L.z_amax = z_amax_bits;
   if (z_amax_bits) BDBNN_CUDA(cudaMemsetAsync(z_amax_bits, 0, sizeof(uint32_t), st));
   return launch_tc_conv<2>(L, st);
 }

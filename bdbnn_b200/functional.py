@@ -1727,14 +1727,20 @@ def conv_bn_add_eval(x, weight, gamma, beta, running_mean, running_var, eps, str
                      shortcut=None):
     """z = BN_eval(binconv2d(x, weight)) + residual in one kernel (bdbnn_binconv_fwd_tc_eval), under no_grad.
     `shortcut` = (weight[Cout,Cin,1,1], gamma, beta, running_mean, running_var, eps, stride) computes the residual as
-    the real-valued 1x1 conv + BN_eval `downsample` branch of x.  The returned z carries `_bdbnn_eval_pack` =
-    (format, +-1 copy of z) for the next unit: fp8 bytes (format -1) when Cout % 128 == 0 and BDBNN_FWD8 is on, else
-    16-bit in the grad_mode() format.  x's own `_bdbnn_eval_pack` is used when it matches this conv's operand."""
+    the real-valued 1x1 conv + BN_eval `downsample` branch of x; `shortcut` = PadShortcut(pad) takes the option-A
+    shortcut of x as the residual, read in place by the epilogue (binconv_fwd_tc_eval_pad_shortcut, 16-bit operands),
+    bit-identical to passing F.pad(x[:, :, ::2, ::2], (0, 0, 0, 0, pad, pad)) as `residual`.  The returned z carries
+    `_bdbnn_eval_pack` = (format, +-1 copy of z) for the next unit: fp8 bytes (format -1) when Cout % 128 == 0 and
+    BDBNN_FWD8 is on, else 16-bit in the grad_mode() format.  x's own `_bdbnn_eval_pack` is used when it matches this
+    conv's operand."""
     _eval_only("conv_bn_add_eval")
     _require_cuda(x, "conv_bn_add_eval(x)")
     _require_cuda(weight, "conv_bn_add_eval(weight)")
     _same_device(x, weight, gamma, beta, running_mean, running_var, residual)
-    if shortcut is not None:
+    pad_sc = isinstance(shortcut, PadShortcut)
+    if pad_sc:
+        _check_pad_shortcut("conv_bn_add_eval", x, weight.shape, stride, residual, shortcut)
+    elif shortcut is not None:
         if residual is not None:
             raise RuntimeError("conv_bn_add_eval: pass either residual or shortcut")
         residual = _shortcut_eval_impl(x, *shortcut)
@@ -1754,6 +1760,9 @@ def conv_bn_add_eval(x, weight, gamma, beta, running_mean, running_var, eps, str
     pack = cout % 32 == 0
     out8 = pack and cout % 128 == 0 and fwd8_enabled()
     use8 = bool(caps & 8) and use_fwd8(sh.Cin, cout, eval_unit=True)
+    if pad_sc and use8:
+        raise RuntimeError("bdbnn_b200.conv_bn_add_eval: the option-A shortcut needs 16-bit operands (fp8 forward "
+                           f"chosen for {sh.Cin} input channels)")
     want = -1 if use8 else fmt
     pk = getattr(x, "_bdbnn_eval_pack", None)
     if pk is not None and pk[0] == want and x._bdbnn_eval_pack_version == x._version:
@@ -1773,11 +1782,20 @@ def conv_bn_add_eval(x, weight, gamma, beta, running_mean, running_var, eps, str
     zb = torch.empty((n, sh.Ho, sh.Wo, cout), dtype=torch.int16, device=dev) if (pack and not out8) else None
     zb8 = torch.empty((n, sh.Ho, sh.Wo, cout), dtype=torch.uint8, device=dev) if out8 else None
     n_out = z.numel()
-    nbytes = (algorithmic_bytes("fwd_tc8_eval" if use8 else "fwd_tc_eval", sh) + (4 * n_out if rc is not None else 0)
-              + (2 * n_out if zb is not None else 0) + (n_out if zb8 is not None else 0))
-    with _timed("binconv_fwd_tc8_eval" if use8 else "binconv_fwd_tc_eval", key, nbytes):
-        _lib.check(L.bdbnn_binconv_fwd_tc_eval(_p(xop), _p(wop), want, _p(scale), _p(shift), _p(rc), _p(z), _p(zb),
-                                               _p(zb8), ctypes.byref(sh), st), "binconv_fwd_tc_eval")
+    copies = (2 * n_out if zb is not None else 0) + (n_out if zb8 is not None else 0)
+    if pad_sc:
+        xr = _nhwc(x.detach())
+        nbytes = algorithmic_bytes("fwd_tc_eval", sh) + _pad_res_bytes(sh) + copies
+        with _timed("binconv_fwd_tc_eval_pad_shortcut", key, nbytes):
+            _lib.check(L.bdbnn_binconv_fwd_tc_eval_pad_shortcut(
+                _p(xop), _p(wop), want, _p(scale), _p(shift), _p(xr), sh.H, sh.W, sh.Cin, int(shortcut.pad), _p(z),
+                _p(zb), _p(zb8), ctypes.byref(sh), st), "binconv_fwd_tc_eval_pad_shortcut")
+    else:
+        nbytes = (algorithmic_bytes("fwd_tc8_eval" if use8 else "fwd_tc_eval", sh) +
+                  (4 * n_out if rc is not None else 0) + copies)
+        with _timed("binconv_fwd_tc8_eval" if use8 else "binconv_fwd_tc_eval", key, nbytes):
+            _lib.check(L.bdbnn_binconv_fwd_tc_eval(_p(xop), _p(wop), want, _p(scale), _p(shift), _p(rc), _p(z),
+                                                   _p(zb), _p(zb8), ctypes.byref(sh), st), "binconv_fwd_tc_eval")
     _lib.count(1)
     if pack and not z.is_inference():       # inference tensors have no version counter to guard the copy with
         z._bdbnn_eval_pack = (-1, zb8) if out8 else (fmt, zb)
@@ -1920,10 +1938,13 @@ def real_weight_pack(weights):
 
 @_on_x_device
 def real_conv_bn_eval(x, x_amax, wpack, gamma, beta, running_mean, running_var, eps, stride, padding, residual=None,
-                      relu=True):
+                      relu=True, shortcut=None):
     """z = relu(BN_eval(conv2d(x, W)) + residual) of a real-valued conv under no_grad, with wpack = (wf, alpha) of
     real_weight_pack(W): real_act_pack -> fold(alpha) -> real_conv_fwd_eval.  x fp32 CUDA (channels_last avoids a
     copy); x_amax = the device word of max|x| a previous call returned (None: computed here, one more pass over x).
+    `shortcut` = PadShortcut(pad) takes the option-A shortcut of x, F.pad(x[:, :, ::2, ::2]) with `pad` zero
+    channels on each side, as the residual: the epilogue reads x in place (real_conv_fwd_eval_pad_shortcut), no
+    padded tensor is written, and z is bit-identical to passing that tensor as `residual`.
     Returns (z fp32 channels_last, z_amax int32[1] = bits of max|z|)."""
     _eval_only("real_conv_bn_eval")
     _require_cuda(x, "real_conv_bn_eval(x)")
@@ -1936,6 +1957,8 @@ def real_conv_bn_eval(x, x_amax, wpack, gamma, beta, running_mean, running_var, 
     sh = conv_shape(x.shape, (cout, cin_w, k, k), stride, padding)
     if not int(L.bdbnn_tc_supported(ctypes.byref(sh))) & 1:
         raise RuntimeError("bdbnn_b200.real_conv_bn_eval: the wgmma forward does not support this shape")
+    if shortcut is not None:
+        _check_pad_shortcut("real_conv_bn_eval", x, (cout, cin_w, k, k), stride, residual, shortcut)
     z_shape = (n, cout, sh.Ho, sh.Wo)
     if residual is not None and tuple(residual.shape) != z_shape:
         raise RuntimeError(f"real_conv_bn_eval: residual shape {tuple(residual.shape)} != output shape {z_shape}")
@@ -1955,9 +1978,59 @@ def real_conv_bn_eval(x, x_amax, wpack, gamma, beta, running_mean, running_var, 
     z = torch.empty(z_shape, dtype=torch.float32, device=dev, memory_format=torch.channels_last)
     z_amax = torch.empty((1,), dtype=torch.int32, device=dev)
     n_out = z.numel()
-    with _timed("real_conv_fwd_eval", key, algorithmic_bytes("fwd_tc_eval", sh) + (4 * n_out if rc is not None else 0)):
-        _lib.check(L.bdbnn_real_conv_fwd_eval(_p(xh), _p(amax), _p(wf), _p(scale), _p(shift), _p(rc), int(bool(relu)),
-                                              _p(z), _p(z_amax), ctypes.byref(sh), st), "real_conv_fwd_eval")
+    if shortcut is not None:
+        with _timed("real_conv_fwd_eval_pad_shortcut", key, algorithmic_bytes("fwd_tc_eval", sh) + _pad_res_bytes(sh)):
+            _lib.check(L.bdbnn_real_conv_fwd_eval_pad_shortcut(
+                _p(xh), _p(amax), _p(wf), _p(scale), _p(shift), _p(xc), h, w, cin, int(shortcut.pad), int(bool(relu)),
+                _p(z), _p(z_amax), ctypes.byref(sh), st), "real_conv_fwd_eval_pad_shortcut")
+    else:
+        with _timed("real_conv_fwd_eval", key,
+                    algorithmic_bytes("fwd_tc_eval", sh) + (4 * n_out if rc is not None else 0)):
+            _lib.check(L.bdbnn_real_conv_fwd_eval(_p(xh), _p(amax), _p(wf), _p(scale), _p(shift), _p(rc),
+                                                  int(bool(relu)), _p(z), _p(z_amax), ctypes.byref(sh), st),
+                       "real_conv_fwd_eval")
+    _lib.count(1)
+    return z, z_amax
+
+
+def _check_pad_shortcut(what, x, w_shape, stride, residual, shortcut):
+    if not isinstance(shortcut, PadShortcut):
+        raise TypeError(f"bdbnn_b200.{what}: shortcut must be a PadShortcut, got {type(shortcut).__name__}")
+    if residual is not None:
+        raise RuntimeError(f"bdbnn_b200.{what}: pass either residual or shortcut")
+    if not pad_shortcut_supported(x.shape, w_shape, stride, shortcut.pad):
+        raise RuntimeError(f"bdbnn_b200.{what}: option-A shortcut with pad {shortcut.pad} does not fit input "
+                           f"{tuple(x.shape)}, weight {tuple(w_shape)}, stride {stride}")
+
+
+def _pad_res_bytes(sh):
+    """Algorithmic bytes of the option-A residual: the sampled pixels' Cin channels, read once (fp32)."""
+    return 4 * sh.N * sh.Ho * sh.Wo * sh.Cin
+
+
+@_on_x_device
+def cifar_stem_conv_bn_eval(x, weight, gamma, beta, running_mean, running_var, eps):
+    """BN_eval(conv2d(x, weight, stride 1, pad 1)) of the CIFAR stem under no_grad: fold (alpha = 1) ->
+    cifar_stem_fwd_eval, the fp32 direct conv of cifar_stem_conv_bn with the folded BatchNorm in its epilogue.
+    Returns (z fp32 channels_last [N,Cout,H,W], z_amax int32[1] = bits of max|z|)."""
+    _eval_only("cifar_stem_conv_bn_eval")
+    _require_cuda(x, "cifar_stem_conv_bn_eval(x)")
+    _require_cuda(weight, "cifar_stem_conv_bn_eval(weight)")
+    _same_device(x, weight, gamma, beta, running_mean, running_var)
+    if not cifar_stem_supported(x.shape, weight.shape, (1, 1), (1, 1)):
+        raise RuntimeError(f"bdbnn_b200.cifar_stem_conv_bn_eval: unsupported input {tuple(x.shape)} / weight "
+                           f"{tuple(weight.shape)}")
+    L = _lib.lib()
+    xd = _dense_images(x)
+    n, _, h, w = xd.shape
+    cout = weight.shape[0]
+    scale, shift = bn_eval_fold(gamma, beta, running_mean, running_var, eps)
+    z = torch.empty((n, cout, h, w), dtype=torch.float32, device=x.device, memory_format=torch.channels_last)
+    z_amax = torch.empty((1,), dtype=torch.int32, device=x.device)
+    with _timed("cifar_stem_fwd_eval", f"cifar_stem_N{n}_{h}x{w}_c{cout}", 4 * xd.numel() + 4 * z.numel()):
+        _lib.check(L.bdbnn_cifar_stem_fwd_eval(_p(xd), n, h, w, *xd.stride(), _p(weight.detach().contiguous()), cout,
+                                               _p(scale), _p(shift), _p(z), _p(z_amax), _stream()),
+                   "cifar_stem_fwd_eval")
     _lib.count(1)
     return z, z_amax
 

@@ -39,18 +39,21 @@ def _eval_mode(x, bn):
             F_.fuse_enabled())
 
 
-def _eval_unit(x, conv, bn, residual):
+def _eval_unit(x, conv, bn, residual, shortcut=None):
     """BN_eval(conv(x)) + residual through the eval kernels when the pair qualifies, else None.  Applies under
     no_grad / inference_mode only: with grad enabled the module chain keeps its autograd graph.  EDE changes only the
-    backward, so it does not exclude a unit."""
+    backward, so it does not exclude a unit.  `shortcut` = functional.PadShortcut: the option-A shortcut of x, read
+    in place, is the residual (the caller checked pad_shortcut_supported)."""
     if not (_eval_mode(x, bn) and isinstance(conv, BinarizeConv2d) and isinstance(bn, nn.BatchNorm2d)):
         return None
     if not (bn.affine and bn.running_mean is not None and bn.running_var is not None) or conv.impl == "xnor":
         return None
     if not F_.eval_unit_supported(x.shape, conv.weight.shape, conv.stride[0], conv.padding[0]):
         return None
+    if shortcut is not None and F_.use_fwd8(x.shape[1], conv.weight.shape[0], eval_unit=True):
+        return None                       # the in-place option-A read has 16-bit operands only
     return F_.conv_bn_add_eval(x, conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps,
-                               conv.stride[0], conv.padding[0], residual)
+                               conv.stride[0], conv.padding[0], residual, shortcut=shortcut)
 
 
 def _eval_shortcut(x, ds):
@@ -233,11 +236,14 @@ class BasicBlockCifar(nn.Module):
     def forward(self, x):
         out = None
         if self.shortcut is not None and F_.shortcut_tc_enabled():
-            # conv1 + bn1 + the option-A shortcut as ONE node: bn_fwd reads the shortcut in place as the residual,
-            # and its gradient is added in place to conv1's input gradient (BDBNN_SHORTCUT_TC=0: _PadShortcut)
+            # conv1 + bn1 + the option-A shortcut as ONE node: bn_fwd (training) or the eval epilogue reads the
+            # shortcut in place as the residual, and in training its gradient is added in place to conv1's input
+            # gradient (BDBNN_SHORTCUT_TC=0: _PadShortcut)
             sc = F_.PadShortcut(self.shortcut.pad)
             if F_.pad_shortcut_supported(x.shape, self.conv1.weight.shape, self.conv1.stride[0], sc.pad):
-                out = _fused_unit(x, self.conv1, self.bn1, None, shortcut=sc)
+                out = _eval_unit(x, self.conv1, self.bn1, None, shortcut=sc)
+                if out is None:
+                    out = _fused_unit(x, self.conv1, self.bn1, None, shortcut=sc)
         if out is None:
             out = self._conv1_unit(x)
         out2 = _eval_unit(out, self.conv2, self.bn2, out)

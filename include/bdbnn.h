@@ -218,8 +218,9 @@ BDBNN_API size_t bdbnn_wgrad_tc_workspace_bytes(const bdbnn_conv_shape* s);
  * BDBNN_TC_CLUSTER=1, and 1 on a grid side that is odd.  Makes no CUDA call. */
 BDBNN_API int bdbnn_debug_conv_plan(const bdbnn_conv_shape* s, int32_t mode, int32_t grad_halves, int32_t* out,
                           int32_t n_out);
-/* CTAs of the forward (mode 0) / dgrad (mode 1) / eval forward (mode 2) tensor-core kernel that fit on one SM of the
- * current device, for operand format fmt (BDBNN_FMT_FP16 / BDBNN_FMT_BF16, -1 = fp8, not dgrad), N tile bn (16/32/64/128) and
+/* CTAs of the forward (mode 0) / dgrad (mode 1) / eval forward (mode 2) / eval forward with the option-A residual of
+ * the *_pad_shortcut entry points (mode 3) tensor-core kernel that fit on one SM of the current device, for operand
+ * format fmt (BDBNN_FMT_FP16 / BDBNN_FMT_BF16, -1 = fp8: modes 0 and 2 only), N tile bn (16/32/64/128) and
  * `smem` bytes of dynamic shared memory (bdbnn_debug_conv_plan out[8]), from the CUDA occupancy calculator.  Needs a
  * CUDA device; sets that kernel's maximum dynamic shared memory attribute to `smem` (every launch sets it again). */
 BDBNN_API int bdbnn_debug_tc_conv_ctas_per_sm(int32_t mode, int32_t fmt, int32_t bn, int32_t smem, int32_t* ctas);
@@ -360,10 +361,18 @@ BDBNN_API int bdbnn_pad_shortcut_bwd(const float* gz, float* gx, int32_t N, int3
  *                      fp16(gy * 2^e) [N,H,W,Cout] with e from g_amax_bits (bdbnn_bn_bwd_pack, FP16S, gscale = 1):
  *                      TF32-class.  fp32 sums per block, block partials (in the workspace, of
  *                      bdbnn_cifar_stem_wgrad_workspace_bytes) added in block order by a finalize kernel.
- * Two launches (+ the statistics' fixed-order sum) forward, two backward; no input gradient. */
+ * Two launches (+ the statistics' fixed-order sum) forward, two backward; no input gradient.
+ *   cifar_stem_fwd_eval : the same conv (same taps, same FMA order, same strides rules) with BatchNorm(eval) in the
+ *                      epilogue, each step rounded (no FMA): z = fp32(fp32(y * scale[o]) + shift[o]), (scale,
+ *                      shift) = bdbnn_bn_eval_fold with alpha = NULL.  z fp32 NHWC [N,H,W,Cout], 16-byte aligned;
+ *                      z_amax_bits (one word, zeroed here) receives the bits of max|z| (integer atomicMax).  One
+ *                      launch; replaces the eval-mode conv1 + bn1 of an fp32 CIFAR ResNet (the KD teacher). */
 BDBNN_API int bdbnn_cifar_stem_fwd(const float* x, int32_t N, int32_t H, int32_t W, int64_t sN, int64_t sC,
                          int64_t sH, int64_t sW, const float* weight, int32_t Cout, float* y, double* bn_sums,
                          uint32_t* bn_ymax, void* stream);
+BDBNN_API int bdbnn_cifar_stem_fwd_eval(const float* x, int32_t N, int32_t H, int32_t W, int64_t sN, int64_t sC,
+                              int64_t sH, int64_t sW, const float* weight, int32_t Cout, const float* scale,
+                              const float* shift, float* z, uint32_t* z_amax_bits, void* stream);
 BDBNN_API size_t bdbnn_cifar_stem_wgrad_workspace_bytes(int32_t N, int32_t H, int32_t W, int32_t Cout);
 BDBNN_API int bdbnn_cifar_stem_wgrad(const float* x, int32_t N, int32_t H, int32_t W, int64_t sN, int64_t sC,
                            int64_t sH, int64_t sW, const uint16_t* gys, const uint32_t* g_amax_bits, int32_t Cout,
@@ -521,6 +530,24 @@ BDBNN_API int bdbnn_real_weight_pack_multi(int32_t count, const float* const* W_
 BDBNN_API int bdbnn_real_conv_fwd_eval(const uint16_t* xh, const uint32_t* x_amax_bits, const uint16_t* wf,
                              const float* scale, const float* shift, const float* residual, int32_t relu, float* z,
                              uint32_t* z_amax_bits, const bdbnn_conv_shape* s, void* stream);
+
+/* ---- eval forward with the CIFAR option-A shortcut as the residual, read in place ------------------------------
+ * Replaces F.pad(x[:, :, ::2, ::2], (0, 0, 0, 0, pad, pad)) (models/cifar10's LambdaLayer, the `shortcut` of a
+ * stride-2 BasicBlock) and the residual add after it.  The same launches as bdbnn_binconv_fwd_tc_eval and
+ * bdbnn_real_conv_fwd_eval, with `residual` replaced by
+ *   r[n,i,j,c] = x_res[n, 2i, 2j, c - pad]   for pad <= c < pad + C_res,   +0.0 otherwise
+ * x_res fp32 NHWC [N][H_res][W_res][C_res], 16-byte aligned, not aliasing z.  Outside the band +0.0 is still added,
+ * so z is bit-identical to passing the materialised zero-padded tensor as `residual` (-0.0 + 0.0 = +0.0).  Needs a
+ * stride-2 conv with Ho = ceil(H_res / 2), Wo = ceil(W_res / 2), Cout == C_res + 2 * pad, and C_res, pad multiples
+ * of 4.  binconv_fwd_tc_eval_pad_shortcut takes 16-bit operands only (the fp8 forward starts at 128 channels). */
+BDBNN_API int bdbnn_binconv_fwd_tc_eval_pad_shortcut(const void* xb, const void* wf, int32_t fmt, const float* scale,
+                                           const float* shift, const float* x_res, int32_t H_res, int32_t W_res,
+                                           int32_t C_res, int32_t pad, float* z, uint16_t* zb, uint8_t* zb8,
+                                           const bdbnn_conv_shape* s, void* stream);
+BDBNN_API int bdbnn_real_conv_fwd_eval_pad_shortcut(const uint16_t* xh, const uint32_t* x_amax_bits, const uint16_t* wf,
+                                          const float* scale, const float* shift, const float* x_res, int32_t H_res,
+                                          int32_t W_res, int32_t C_res, int32_t pad, int32_t relu, float* z,
+                                          uint32_t* z_amax_bits, const bdbnn_conv_shape* s, void* stream);
 
 #ifdef __cplusplus
 }

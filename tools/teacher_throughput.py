@@ -1,15 +1,17 @@
 """Throughput of the KD step's frozen fp32 teacher (train.py:250-277, run at train.py:603): this repository's kernel
-teacher (bdbnn_b200.FrozenResNetTeacher) against the torchvision model on cuDNN.
+teacher (bdbnn_b200.FrozenResNetTeacher) against the unwrapped model on cuDNN.
 
-    python tools/teacher_throughput.py [--models resnet18,resnet34] [--batch 256] [--iters 20] [--warmup 5]
+    python tools/teacher_throughput.py [--models resnet18,resnet34,resnet20] [--batch N] [--iters 20] [--warmup 5]
                                        [--rounds 3] [--steps 50] [--step-warmup 10] [--no-step]
 
-224x224 channels_last images, random weights and BatchNorm statistics.  Teacher forward arms, alternated round by
+resnet18 / resnet34: the torchvision models on 224x224 images, batch 256 by default.  resnet20: the fp32 CIFAR
+ResNet-20 (bdbnn_b200.resnet.ResNetCifar(3) with bias-free nn.Conv2d convs) on 32x32 images, batch 128 by default.
+channels_last images, random weights and BatchNorm statistics.  Teacher forward arms, alternated round by
 round, each warmed up first, images/s from CUDA events over --iters forwards:
 
     kernel_eager     FrozenResNetTeacher, launched eagerly
     kernel_graphed   the same forward captured once as a CUDA graph and replayed
-    cudnn_default    the torchvision model with TF32 allowed and cudnn.benchmark off (bench.py's timed path)
+    cudnn_default    the unwrapped model with TF32 allowed and cudnn.benchmark off (bench.py's timed path)
     cudnn_benchmark  the same with cudnn.benchmark = True (train.py:368)
 
 The two kernel arms run in this process.  Each cuDNN arm runs in a process of its own, started afresh every round:
@@ -17,8 +19,9 @@ PyTorch caches the cuDNN plan of a conv shape whatever `benchmark` was when it w
 that ran first would serve its plans to the other and the benchmark arm would not autotune.
 
 Then one eager kernel-teacher forward under functional.KernelTimer (per-family times), and the full KD step:
-GraphedTrainStep(TrainStep(resnet18 student, kurtosis + KD config, teacher=...)) with the kernel teacher and with
-the torchvision teacher (cudnn.benchmark off throughout this process), alternated, --step-warmup steps then --steps
+GraphedTrainStep(TrainStep(student, kurtosis + KD config, teacher=...)) with the kernel teacher and with the
+unwrapped teacher (cudnn.benchmark off throughout this process; the student is the binary resnet18, or resnet20 for
+the CIFAR teacher), alternated, --step-warmup steps then --steps
 timed steps per round.  The card name, power limit and maximum SM clock are read (read-only) from nvidia-smi.
 Needs a CUDA device."""
 import argparse
@@ -54,11 +57,26 @@ def _timed_loop(torch, fn, iters):
     return e0.elapsed_time(e1) / 1e3
 
 
+CIFAR = ("resnet20",)
+
+
+def _hw(name):
+    return 32 if name in CIFAR else 224
+
+
+def _batch(args, name):
+    return args.batch if args.batch is not None else (128 if name in CIFAR else 256)
+
+
 def _teacher(torch, name, dev):
     import torch.nn as nn
-    import torchvision
     torch.manual_seed(1)
-    m = getattr(torchvision.models, name)()
+    if name in CIFAR:
+        from bdbnn_b200.resnet import ResNetCifar
+        m = ResNetCifar(3, conv_cls=lambda i, o, k, s, p: nn.Conv2d(i, o, k, s, p, bias=False))
+    else:
+        import torchvision
+        m = getattr(torchvision.models, name)()
     g = torch.Generator().manual_seed(2)
     for mod in m.modules():
         if isinstance(mod, nn.BatchNorm2d):
@@ -72,8 +90,8 @@ def _teacher(torch, name, dev):
     return m.to(dev).to(memory_format=torch.channels_last).eval()
 
 
-def _images(torch, batch, dev):
-    x = torch.randn(batch, 3, 224, 224, generator=torch.Generator().manual_seed(0))
+def _images(torch, name, batch, dev):
+    x = torch.randn(batch, 3, _hw(name), _hw(name), generator=torch.Generator().manual_seed(0))
     return x.to(dev).contiguous(memory_format=torch.channels_last)
 
 
@@ -83,17 +101,19 @@ def cudnn_arm(torch, name, mode, args, dev):
     torch.backends.cudnn.allow_tf32 = True
     torch.backends.cudnn.benchmark = mode == "benchmark"
     tv = _teacher(torch, name, dev)
-    x = _images(torch, args.batch, dev)
+    batch = _batch(args, name)
+    x = _images(torch, name, batch, dev)
     with torch.no_grad():
         for _ in range(args.warmup):
             tv(x)
         torch.cuda.synchronize()
-        rate = args.batch * args.iters / _timed_loop(torch, lambda: tv(x), args.iters)
+        rate = batch * args.iters / _timed_loop(torch, lambda: tv(x), args.iters)
     print(json.dumps({"img_per_s": round(rate, 1)}), flush=True)
 
 
 def _cudnn_round(name, mode, args):
-    cmd = [sys.executable, os.path.abspath(__file__), "--cudnn-arm", mode, "--models", name, "--batch", str(args.batch),
+    cmd = [sys.executable, os.path.abspath(__file__), "--cudnn-arm", mode, "--models", name, "--batch",
+           str(_batch(args, name)),
            "--iters", str(args.iters), "--warmup", str(args.warmup)]
     r = subprocess.run(cmd, capture_output=True, text=True, check=True)
     return json.loads(r.stdout.strip().splitlines()[-1])["img_per_s"]
@@ -103,7 +123,8 @@ def forward_arms(torch, name, args, dev):
     from bdbnn_b200 import FrozenResNetTeacher
     from bdbnn_b200.functional import KernelTimer
     kt = FrozenResNetTeacher(_teacher(torch, name, dev))
-    x = _images(torch, args.batch, dev)
+    batch = _batch(args, name)
+    x = _images(torch, name, batch, dev)
     with torch.no_grad():
         assert kt.kernel_path(x)
         arms = {"kernel_eager": lambda: kt(x), "kernel_graphed": _graphed(torch, lambda: kt(x), args.warmup)}
@@ -114,10 +135,10 @@ def forward_arms(torch, name, args, dev):
         rates = {a: [] for a in list(arms) + ["cudnn_default", "cudnn_benchmark"]}
         for _ in range(args.rounds):
             for arm, fn in arms.items():
-                rates[arm].append(round(args.batch * args.iters / _timed_loop(torch, fn, args.iters), 1))
+                rates[arm].append(round(batch * args.iters / _timed_loop(torch, fn, args.iters), 1))
             for mode in ("default", "benchmark"):
                 rates["cudnn_" + mode].append(_cudnn_round(name, mode, args))
-        print(json.dumps({"teacher": name, "img_per_s": rates}), flush=True)
+        print(json.dumps({"teacher": name, "batch": batch, "img_per_s": rates}), flush=True)
         KernelTimer.start()
         kt(x)
         kern = KernelTimer.stop()
@@ -134,18 +155,20 @@ def forward_arms(torch, name, args, dev):
 
 def kd_step_arms(torch, name, args, dev):
     from bdbnn_b200 import FrozenResNetTeacher
-    from bdbnn_b200.resnet import resnet18
+    from bdbnn_b200.resnet import resnet18, resnet20
     from bdbnn_b200.step import GraphedTrainStep, StepConfig, TrainStep, make_optimizer
     torch.backends.cudnn.benchmark = False
     tv = _teacher(torch, name, dev)
     cfg = StepConfig(w_kurtosis=True, teacher_student=True, alpha=0.9, beta=200.0, w_lambda_ce=1.0)
     g = torch.Generator().manual_seed(0)
-    x = torch.randn(args.batch, 3, 224, 224, generator=g).to(dev).contiguous(memory_format=torch.channels_last)
-    y = torch.randint(0, 1000, (args.batch,), generator=g).to(dev)
+    batch, hw = _batch(args, name), _hw(name)
+    student, classes = (resnet20, 10) if name in CIFAR else (resnet18, 1000)
+    x = torch.randn(batch, 3, hw, hw, generator=g).to(dev).contiguous(memory_format=torch.channels_last)
+    y = torch.randint(0, classes, (batch,), generator=g).to(dev)
     steps = {}
     for arm, teacher in (("kernel_teacher", FrozenResNetTeacher(tv)), ("cudnn_teacher", tv)):
         torch.manual_seed(0)
-        model = resnet18().to(dev)
+        model = student().to(dev)
         steps[arm] = GraphedTrainStep(TrainStep(model, make_optimizer(model), cfg, teacher=teacher))
     for st in steps.values():
         for _ in range(args.step_warmup):
@@ -154,14 +177,15 @@ def kd_step_arms(torch, name, args, dev):
     rates = {a: [] for a in steps}
     for _ in range(args.rounds):
         for arm, st in steps.items():
-            rates[arm].append(round(args.batch * args.steps / _timed_loop(torch, lambda: st(x, y), args.steps), 1))
-    print(json.dumps({"kd_step": f"resnet18 student, {name} teacher", "img_per_s": rates}), flush=True)
+            rates[arm].append(round(batch * args.steps / _timed_loop(torch, lambda: st(x, y), args.steps), 1))
+    print(json.dumps({"kd_step": f"{student.__name__} student, {name} teacher", "batch": batch, "img_per_s": rates}),
+          flush=True)
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--models", default="resnet18,resnet34")
-    ap.add_argument("--batch", type=int, default=256)
+    ap.add_argument("--batch", type=int, default=None, help="default: 256 (resnet18/34), 128 (resnet20)")
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--rounds", type=int, default=3)
@@ -179,7 +203,7 @@ def main():
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                        capture_output=True, text=True)
     print(json.dumps({"gpu": q.stdout.strip().splitlines()[0] if q.returncode == 0 else None,
-                      "batch": args.batch, "iters": args.iters, "rounds": args.rounds}), flush=True)
+                      "iters": args.iters, "rounds": args.rounds}), flush=True)
     dev = torch.device("cuda", 0)
     torch.backends.cudnn.allow_tf32 = True
     torch.backends.cudnn.benchmark = False
