@@ -280,6 +280,23 @@ def _cifar_stem_qualifies(x, c1, bn):
     return F_.cifar_stem_supported(tuple(x.shape), tuple(c1.weight.shape), c1.stride, c1.padding)
 
 
+def _cifar_stem(x, c1, bn):
+    """conv1 + bn1 of a CIFAR shell: functional.cifar_stem_conv_bn when _cifar_stem_qualifies, else cuDNN + bn."""
+    if _cifar_stem_qualifies(x, c1, bn):
+        # fp32 direct conv + BatchNorm(train) on this repository's kernels, handing layer1.0.conv1 its packs
+        z = F_.cifar_stem_conv_bn(x, c1.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.momentum,
+                                  bn.eps)
+        bn.num_batches_tracked.add_(1)
+        return z
+    # fp32 stem on cuDNN: TF32 off, or cuDNN may pick a TF32 algorithm for some batch sizes (on the H100 at batch 8 but
+    # not 16), and the binary layers behind it amplify that 1e-3 difference into different signs
+    cudnn = torch.backends.cudnn
+    with cudnn.flags(enabled=cudnn.enabled, benchmark=cudnn.benchmark, deterministic=cudnn.deterministic,
+                     allow_tf32=False):
+        y = c1(x)
+    return bn(y)
+
+
 class ResNetCifar(nn.Module):
     """ResNet-20-style CIFAR net: fp32 3x3 stem + 3 stages x n blocks (18 binary convs for n=3)."""
 
@@ -304,22 +321,39 @@ class ResNetCifar(nn.Module):
     def forward(self, x):
         packed = _prepack(self, x)
         try:
-            c1, bn = self.conv1, self.bn1
-            if _cifar_stem_qualifies(x, c1, bn):
-                # fp32 direct conv + BatchNorm(train) on this repository's kernels, handing layer1.0.conv1 its packs
-                x = F_.cifar_stem_conv_bn(x, c1.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var,
-                                          bn.momentum, bn.eps)
-                bn.num_batches_tracked.add_(1)
-            else:
-                # fp32 stem on cuDNN: TF32 off, or cuDNN may pick a TF32 algorithm for some batch sizes (on the H100 at
-                # batch 8 but not 16), and the binary layers behind it amplify that 1e-3 difference into different
-                # signs
-                cudnn = torch.backends.cudnn
-                with cudnn.flags(enabled=cudnn.enabled, benchmark=cudnn.benchmark, deterministic=cudnn.deterministic,
-                                 allow_tf32=False):
-                    x = c1(x)
-                x = bn(x)
+            x = _cifar_stem(x, self.conv1, self.bn1)
             x = self.layer3(self.layer2(self.layer1(x)))
+        finally:
+            if packed:
+                F_._PREPACKED.clear()
+        return self.fc(torch.flatten(self.avgpool(x), 1))
+
+
+class ResNetCifar18(nn.Module):
+    """ResNet-18 for 32x32 inputs (DESIGN.md §4k): the fp32 3x3 / stride-1 CIFAR stem with 64 outputs and no max-pool,
+    then the ImageNet ResNet-18's four stages of Bi-Real BasicBlocks (64/128/256/512 channels at 32/16/8/4 pixels) with
+    fp32 1x1 conv + BN `downsample` shortcuts at layer2.0, layer3.0 and layer4.0: 16 binary 3x3 convs and 19 hookable
+    convs after the stem, as the reference's CIFAR --diffkurt list (train.py:472-475) indexes them."""
+
+    def __init__(self, num_classes=10, conv_cls=HardBinaryConv_cifar):
+        super().__init__()
+        self.inplanes = 64
+        self.conv1 = nn.Conv2d(3, 64, kernel_size=3, stride=1, padding=1, bias=False)
+        self.bn1 = nn.BatchNorm2d(64)
+        self.layer1 = self._make_layer(64, 2, 1, conv_cls)
+        self.layer2 = self._make_layer(128, 2, 2, conv_cls)
+        self.layer3 = self._make_layer(256, 2, 2, conv_cls)
+        self.layer4 = self._make_layer(512, 2, 2, conv_cls)
+        self.avgpool = nn.AdaptiveAvgPool2d(1)
+        self.fc = nn.Linear(512, num_classes)
+
+    _make_layer = ResNetImageNet._make_layer
+
+    def forward(self, x):
+        packed = _prepack(self, x)
+        try:
+            x = _cifar_stem(x, self.conv1, self.bn1)
+            x = self.layer4(self.layer3(self.layer2(self.layer1(x))))
         finally:
             if packed:
                 F_._PREPACKED.clear()
@@ -336,3 +370,7 @@ def resnet34(pretrained=False, conv_cls=HardBinaryConv, **kw):
 
 def resnet20(conv_cls=HardBinaryConv_cifar, **kw):
     return ResNetCifar(3, conv_cls=conv_cls, **kw)
+
+
+def resnet18_cifar(num_classes=10, conv_cls=HardBinaryConv_cifar):
+    return ResNetCifar18(num_classes=num_classes, conv_cls=conv_cls)

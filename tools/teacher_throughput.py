@@ -1,11 +1,12 @@
 """Throughput of the KD step's frozen fp32 teacher (train.py:250-277, run at train.py:603): this repository's kernel
 teacher (bdbnn_b200.FrozenResNetTeacher) against the unwrapped model on cuDNN.
 
-    python tools/teacher_throughput.py [--models resnet18,resnet34,resnet20] [--batch N] [--iters 20] [--warmup 5]
-                                       [--rounds 3] [--steps 50] [--step-warmup 10] [--no-step]
+    python tools/teacher_throughput.py [--models resnet18,resnet34,resnet20,resnet18_cifar] [--batch N] [--iters 20]
+                                       [--warmup 5] [--rounds 3] [--steps 50] [--step-warmup 10] [--no-step]
 
 resnet18 / resnet34: the torchvision models on 224x224 images, batch 256 by default.  resnet20: the fp32 CIFAR
-ResNet-20 (bdbnn_b200.resnet.ResNetCifar(3) with bias-free nn.Conv2d convs) on 32x32 images, batch 128 by default.
+ResNet-20 (bdbnn_b200.resnet.ResNetCifar(3) with bias-free nn.Conv2d convs) on 32x32 images, batch 128 by default;
+resnet18_cifar: the fp32 CIFAR ResNet-18 (bdbnn_b200.resnet.resnet18_cifar(conv_cls=<bias-free nn.Conv2d>)), the same.
 channels_last images, random weights and BatchNorm statistics.  Teacher forward arms, alternated round by
 round, each warmed up first, images/s from CUDA events over --iters forwards:
 
@@ -20,8 +21,8 @@ that ran first would serve its plans to the other and the benchmark arm would no
 
 Then one eager kernel-teacher forward under functional.KernelTimer (per-family times), and the full KD step:
 GraphedTrainStep(TrainStep(student, kurtosis + KD config, teacher=...)) with the kernel teacher and with the
-unwrapped teacher (cudnn.benchmark off throughout this process; the student is the binary resnet18, or resnet20 for
-the CIFAR teacher), alternated, --step-warmup steps then --steps
+unwrapped teacher (cudnn.benchmark off throughout this process; the student is the binary resnet18, or the binary
+CIFAR net of the teacher's shape for a CIFAR teacher), alternated, --step-warmup steps then --steps
 timed steps per round.  The card name, power limit and maximum SM clock are read (read-only) from nvidia-smi.
 Needs a CUDA device."""
 import argparse
@@ -57,7 +58,7 @@ def _timed_loop(torch, fn, iters):
     return e0.elapsed_time(e1) / 1e3
 
 
-CIFAR = ("resnet20",)
+CIFAR = ("resnet20", "resnet18_cifar")
 
 
 def _hw(name):
@@ -71,9 +72,13 @@ def _batch(args, name):
 def _teacher(torch, name, dev):
     import torch.nn as nn
     torch.manual_seed(1)
-    if name in CIFAR:
+    fp32_conv = lambda i, o, k, s, p: nn.Conv2d(i, o, k, s, p, bias=False)
+    if name == "resnet18_cifar":
+        from bdbnn_b200.resnet import resnet18_cifar
+        m = resnet18_cifar(conv_cls=fp32_conv)
+    elif name in CIFAR:
         from bdbnn_b200.resnet import ResNetCifar
-        m = ResNetCifar(3, conv_cls=lambda i, o, k, s, p: nn.Conv2d(i, o, k, s, p, bias=False))
+        m = ResNetCifar(3, conv_cls=fp32_conv)
     else:
         import torchvision
         m = getattr(torchvision.models, name)()
@@ -155,14 +160,14 @@ def forward_arms(torch, name, args, dev):
 
 def kd_step_arms(torch, name, args, dev):
     from bdbnn_b200 import FrozenResNetTeacher
-    from bdbnn_b200.resnet import resnet18, resnet20
+    from bdbnn_b200.resnet import resnet18, resnet18_cifar, resnet20
     from bdbnn_b200.step import GraphedTrainStep, StepConfig, TrainStep, make_optimizer
     torch.backends.cudnn.benchmark = False
     tv = _teacher(torch, name, dev)
     cfg = StepConfig(w_kurtosis=True, teacher_student=True, alpha=0.9, beta=200.0, w_lambda_ce=1.0)
     g = torch.Generator().manual_seed(0)
     batch, hw = _batch(args, name), _hw(name)
-    student, classes = (resnet20, 10) if name in CIFAR else (resnet18, 1000)
+    student, classes = {"resnet20": (resnet20, 10), "resnet18_cifar": (resnet18_cifar, 10)}.get(name, (resnet18, 1000))
     x = torch.randn(batch, 3, hw, hw, generator=g).to(dev).contiguous(memory_format=torch.channels_last)
     y = torch.randint(0, classes, (batch,), generator=g).to(dev)
     steps = {}
