@@ -98,6 +98,8 @@ SIGNATURES = {
     "bdbnn_cifar_stem_wgrad_workspace_bytes": (c_size_t, [c_int] * 4),
     "bdbnn_cifar_stem_wgrad": (c_int, [_P, c_int, c_int, c_int, c_int64, c_int64, c_int64, c_int64, _P, _P, c_int, _P,
                                        _P, c_size_t, _P]),
+    "bdbnn_cifar_batch": (c_int, [_P, _P, c_int64, ctypes.c_uint64, ctypes.c_uint32, c_int64, c_int, c_int, _P, _P, _P,
+                                  c_int64, c_int64, c_int64, c_int64, _P, _P]),
 }
 
 

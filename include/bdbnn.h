@@ -549,6 +549,22 @@ BDBNN_API int bdbnn_real_conv_fwd_eval_pad_shortcut(const uint16_t* xh, const ui
                                           int32_t W_res, int32_t C_res, int32_t pad, int32_t relu, float* z,
                                           uint32_t* z_amax_bits, const bdbnn_conv_shape* s, void* stream);
 
+/* ---- CIFAR input batch from the device-resident dataset --------------------------------------------------------
+ * Replaces the CIFAR DataLoaders of loader.py:7-50 (torchvision RandomCrop(32, padding=4), RandomHorizontalFlip,
+ * ToTensor, Normalize in CPU workers, then the H2D copy of train.py:488-491).  images uint8 [n][32][32][3] (HWC per
+ * image, 16-byte aligned), labels int64 [n].  Output element (b, c, i, j), with idx = perm(seed, epoch, pos0 + b):
+ *   (dy, dx, flip) = draw(seed, epoch, idx) if augment, else (4, 4, 0);
+ *   u = pixel (i + dy - 4, (flip ? 31 - j : j) + dx - 4) of image idx, channel c, or 0 outside the image;
+ *   out = fp32((fp32(u / 255) - mean[c]) / std[c]), every step rounded to nearest (to_tensor, then normalize);
+ * written through the element strides (sN, sC, sH, sW) (NCHW or channels_last); target[b] = labels[idx].
+ * perm is a keyed Feistel bijection of [0, n) and draw a Philox-4x32-10 draw keyed by the dataset index (DESIGN.md
+ * §4l; oracle/cifar_data_ref.py restates both).  mean_host / std_host: 3 floats each, HOST memory.  Needs
+ * 1 <= n < 2^31 and 0 <= pos0, pos0 + B <= n.  One launch, B blocks; nothing read back. */
+BDBNN_API int bdbnn_cifar_batch(const uint8_t* images, const int64_t* labels, int64_t n, uint64_t seed,
+                                uint32_t epoch, int64_t pos0, int32_t B, int32_t augment, const float* mean_host,
+                                const float* std_host, float* out, int64_t sN, int64_t sC, int64_t sH, int64_t sW,
+                                int64_t* target, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
