@@ -100,6 +100,7 @@ SIGNATURES = {
                                        _P, c_size_t, _P]),
     "bdbnn_cifar_batch": (c_int, [_P, _P, c_int64, ctypes.c_uint64, ctypes.c_uint32, c_int64, c_int, c_int, _P, _P, _P,
                                   c_int64, c_int64, c_int64, c_int64, _P, _P]),
+    "bdbnn_imagenet_batch": (c_int, [_P, _P, c_int, _P, _P, _P, c_int64, c_int64, c_int64, c_int64, _P, _P]),
 }
 
 

@@ -1,4 +1,6 @@
-"""CIFAR-10 / CIFAR-100 training and validation batches fed from device memory (csrc/cifar_data.cu).
+"""CIFAR-10 / CIFAR-100 training and validation batches fed from device memory (csrc/cifar_data.cu), and ImageNet
+batches decoded from an ImageFolder and resized-cropped on the device (csrc/imagenet_data.cu, ImageNetDeviceLoader
+and dataloader_imagenet below; DESIGN.md §4m).
 
 The reference's CIFAR loaders (loader.py:7-50) run torchvision's RandomCrop(32, padding=4), RandomHorizontalFlip,
 ToTensor and Normalize per image in 4 (CIFAR-100: 16) CPU worker processes and copy every batch to the device
@@ -32,9 +34,13 @@ dataset each epoch; here each rank reads 1 / world_size of it.  Without drop_las
 by one (the last global batches go to the lower ranks); with drop_last every rank has n // (batch_size *
 world_size) full batches, which a data-parallel step needs."""
 import ctypes
+import io
+import math
 import os
 import pickle
 import sys
+import threading
+from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import torch
@@ -227,3 +233,450 @@ def dataloader_cifar100(split='train', batch_size=128, root=None):
     """loader.py:31-50 on the device (CIFAR-100 fine labels, normalised with the CIFAR-10 statistics as the reference
     does).  Returns a CifarDeviceLoader."""
     return _dataloader("cifar100", split, batch_size, root)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# ImageNet (csrc/imagenet_data.cu, DESIGN.md §4m)
+# ---------------------------------------------------------------------------------------------------------------------
+IMAGENET_MEAN = (0.485, 0.456, 0.406)            # loader.py:53-54
+IMAGENET_STD = (0.229, 0.224, 0.225)
+IMAGENET_OUT = 224                               # RandomResizedCrop(224), CenterCrop(224)
+IMAGENET_EVAL_SHORT = 256                        # Resize(256)
+IMAGENET_MAX_SIDE = 8192                         # larger decoded images are rejected by the kernel
+_RRC_SCALE = (0.08, 1.0)
+_RRC_RATIO = (3.0 / 4.0, 4.0 / 3.0)
+_M32 = np.uint64(0xFFFFFFFF)
+
+# bdbnn_imagenet_desc (include/bdbnn.h)
+_DESC = np.dtype([("src", "<u8"), ("sC", "<i8"), ("sH", "<i8"), ("sW", "<i8"), ("H", "<i4"), ("W", "<i4"),
+                  ("x0", "<i4"), ("y0", "<i4"), ("w", "<i4"), ("h", "<i4"), ("RH", "<i4"), ("RW", "<i4"),
+                  ("oy0", "<i4"), ("ox0", "<i4"), ("flip", "<i4"), ("reserved", "<i4"), ("label", "<i8")])
+assert _DESC.itemsize == 88
+
+
+def _philox(seed, c0, c1, c2, c3):
+    """Philox-4x32-10 of csrc/cifar_data.cu, vectorised: four uint64 arrays holding the 32-bit output words."""
+    c = list(np.broadcast_arrays(*[np.asarray(v, dtype=np.uint64) & _M32 for v in (c0, c1, c2, c3)]))
+    seed = int(seed)
+    k0, k1 = seed & 0xFFFFFFFF, seed >> 32
+    m0, m1, s32 = np.uint64(0xD2511F53), np.uint64(0xCD9E8D57), np.uint64(32)
+    for _ in range(10):
+        p0, p1 = m0 * c[0], m1 * c[2]
+        c = [(p1 >> s32) ^ c[1] ^ np.uint64(k0), p1 & _M32, (p0 >> s32) ^ c[3] ^ np.uint64(k1), p0 & _M32]
+        k0, k1 = (k0 + 0x9E3779B9) & 0xFFFFFFFF, (k1 + 0xBB67AE85) & 0xFFFFFFFF
+    return c
+
+
+def epoch_permutation(seed, epoch, pos, n):
+    """Dataset indices (int64) of epoch positions pos (< n): the keyed Feistel bijection of csrc/cifar_data.cu
+    (DESIGN.md §4l), cycle-walked into [0, n), vectorised over pos."""
+    a, b = _philox(seed, epoch, 0, 1, 0), _philox(seed, epoch, 0, 1, 1)
+    keys = [np.uint64(int(w)) for w in a + b]
+    m = max(int(n) - 1, 0).bit_length()
+    x = np.array(pos, dtype=np.uint64, ndmin=1)
+    todo = np.ones(x.shape, dtype=bool)
+    while todo.any():
+        y = x[todo]
+        wl, wr = m - m // 2, m // 2
+        for k in keys:
+            L, R = y >> np.uint64(wr), y & np.uint64((1 << wr) - 1)
+            h = ((R ^ k) * np.uint64(0x85EBCA6B)) & _M32
+            h ^= h >> np.uint64(13)
+            h = (h * np.uint64(0xC2B2AE35)) & _M32
+            h ^= h >> np.uint64(16)
+            y = (R << np.uint64(wl)) | ((L ^ h) & np.uint64((1 << wl) - 1))
+            wl, wr = wr, wl
+        x[todo] = y
+        todo = x >= np.uint64(n)
+    return x.astype(np.int64)
+
+
+def random_resized_crop_params(seed, epoch, idx, H, W):
+    """(i, j, h, w, flip) int64 arrays for dataset indices idx of images H x W (arrays of equal shape):
+    torchvision's RandomResizedCrop.get_params (scale (0.08, 1), ratio (3/4, 4/3), 10 attempts, then the central
+    fallback) in float64 with Python's math, and RandomHorizontalFlip, on the repository's stream: attempt a of image
+    idx takes Philox(seed, (epoch, idx, 2, a)) = (w0, w1, w2, w3):
+        target = H W (0.08 + 0.92 w0 2^-32), ratio = exp(log(3/4) + (log(4/3) - log(3/4)) w1 2^-32),
+        w = round(sqrt(target ratio)), h = round(sqrt(target / ratio)), i = (w2 (H - h + 1)) >> 32,
+        j = (w3 (W - w + 1)) >> 32,
+    flip = Philox(seed, (epoch, idx, 3, 0)).w0 >> 31."""
+    idx = np.array(idx, dtype=np.uint64, ndmin=1)
+    H, W = np.broadcast_to(np.asarray(H, np.int64), idx.shape), np.broadcast_to(np.asarray(W, np.int64), idx.shape)
+    words = [_philox(seed, epoch, idx, 2, a) for a in range(10)]
+    flip = (_philox(seed, epoch, idx, 3, 0)[0] >> np.uint64(31)).astype(np.int64)
+    lr0, lr1 = math.log(_RRC_RATIO[0]), math.log(_RRC_RATIO[1])
+    s0, ds = _RRC_SCALE[0], _RRC_SCALE[1] - _RRC_SCALE[0]
+    out = np.zeros((idx.size, 4), np.int64)
+    for k in range(idx.size):
+        Hk, Wk = int(H[k]), int(W[k])
+        area = Hk * Wk
+        for a in range(10):
+            w0, w1, w2, w3 = (int(v[k]) for v in words[a])
+            target = area * (s0 + ds * (w0 * 2.0 ** -32))
+            ratio = math.exp(lr0 + (lr1 - lr0) * (w1 * 2.0 ** -32))
+            w = int(round(math.sqrt(target * ratio)))
+            h = int(round(math.sqrt(target / ratio)))
+            if 0 < w <= Wk and 0 < h <= Hk:
+                out[k] = ((w2 * (Hk - h + 1)) >> 32, (w3 * (Wk - w + 1)) >> 32, h, w)
+                break
+        else:
+            in_ratio = Wk / Hk
+            if in_ratio < _RRC_RATIO[0]:
+                w, h = Wk, int(round(Wk / _RRC_RATIO[0]))
+            elif in_ratio > _RRC_RATIO[1]:
+                h, w = Hk, int(round(Hk * _RRC_RATIO[1]))
+            else:
+                w, h = Wk, Hk
+            out[k] = ((Hk - h) // 2, (Wk - w) // 2, h, w)
+    return out[:, 0], out[:, 1], out[:, 2], out[:, 3], flip
+
+
+def eval_resize_geometry(H, W):
+    """(RH, RW, oy0, ox0) of an H x W image: torchvision's Resize(256) size (short side 256, long side
+    int(256 * long / short)) and CenterCrop(224)'s window origin int(round((R - 224) / 2.0)), half to even."""
+    short, long = (W, H) if W <= H else (H, W)
+    new_short, new_long = IMAGENET_EVAL_SHORT, int(IMAGENET_EVAL_SHORT * long / short)
+    RW, RH = (new_short, new_long) if W <= H else (new_long, new_short)
+    return RH, RW, int(round((RH - IMAGENET_OUT) / 2.0)), int(round((RW - IMAGENET_OUT) / 2.0))
+
+
+def index_image_folder(root):
+    """(samples [(path, class index)], class_to_idx) of an ImageFolder root: torchvision.datasets.ImageFolder's
+    indexing (sorted class directories, its extensions, its sample order)."""
+    from torchvision.datasets.folder import IMG_EXTENSIONS, find_classes, make_dataset
+    if not os.path.isdir(root):
+        raise FileNotFoundError(f"index_image_folder: {root} is not a directory")
+    classes, class_to_idx = find_classes(root)
+    return make_dataset(root, class_to_idx, IMG_EXTENSIONS), class_to_idx
+
+
+def _jpeg_components(data):
+    """Colour components of a baseline / progressive / lossless JPEG (the Nf of its SOF header), 0 if `data` is not a
+    JPEG or has no frame header."""
+    if len(data) < 4 or data[0] != 0xFF or data[1] != 0xD8:
+        return 0
+    p = 2
+    while p + 4 <= len(data):
+        if data[p] != 0xFF:
+            return 0
+        m = data[p + 1]
+        if m == 0xFF:
+            p += 1
+            continue
+        if m in (0x01,) or 0xD0 <= m <= 0xD7:
+            p += 2
+            continue
+        seg = (data[p + 2] << 8) | data[p + 3]
+        if 0xC0 <= m <= 0xCF and m not in (0xC4, 0xC8, 0xCC):
+            return data[p + 9] if p + 9 < len(data) else 0
+        if m == 0xDA:
+            return 0
+        p += 2 + seg
+    return 0
+
+
+def _pil_decode(data):
+    """uint8 HWC [H, W, 3] of an image file through PIL (Image.open(f).convert('RGB'), as ImageFolder's loader)."""
+    from PIL import Image
+    with Image.open(io.BytesIO(data)) as im:
+        return np.array(im.convert("RGB"))
+
+
+def _read(path):
+    with open(path, "rb") as fh:
+        return fh.read()
+
+
+class ImageNetBatchKernel:
+    """bdbnn_imagenet_batch with its descriptor buffers: two pinned host tables and two device tables, used in turn;
+    before a table is rewritten the host waits on the event recorded after the launch that last read it."""
+
+    def __init__(self, device, mean=IMAGENET_MEAN, std=IMAGENET_STD):
+        self.device = torch.device(device)
+        self._mean = (ctypes.c_float * 3)(*mean)
+        self._std = (ctypes.c_float * 3)(*std)
+        self._slots = [None, None]               # (pinned host bytes, device bytes, event)
+        self._turn = 0
+
+    def _slot(self, B):
+        k = self._turn
+        self._turn ^= 1
+        s = self._slots[k]
+        if s is not None:
+            s[2].synchronize()
+        if s is None or s[0].numel() < B * _DESC.itemsize:
+            s = (torch.empty(B * _DESC.itemsize, dtype=torch.uint8, pin_memory=True),
+                 torch.empty(B * _DESC.itemsize, dtype=torch.uint8, device=self.device), torch.cuda.Event())
+            self._slots[k] = s
+        return s
+
+    def __call__(self, sources, geometry, labels, images, target):
+        """One descriptor copy and one launch on the current stream; returns (images, target).
+        sources: B pairs (uint8 tensor on the device, hwc): [3, H, W] when hwc is False, [H, W, 3] when True, any
+        strides; geometry: int [B, 9] rows (y0, x0, h, w, RH, RW, oy0, ox0, flip) as bdbnn_imagenet_desc; labels: B
+        integers; images fp32 [B, 3, 224, 224] (NCHW or channels_last) and target int64 [B] on the device.  The
+        sources must stay alive until the launch has run."""
+        B = len(sources)
+        geometry = np.asarray(geometry, dtype=np.int64).reshape(B, 9)
+        host, dev, ev = self._slot(B)
+        d = host[:B * _DESC.itemsize].numpy().view(_DESC)
+        for k, (src, hwc) in enumerate(sources):
+            if src.dtype != torch.uint8 or src.device != self.device or src.dim() != 3:
+                raise ValueError(f"ImageNetBatchKernel: source {k} must be a uint8 3-d tensor on {self.device}")
+            if hwc:
+                (Hk, Wk, C), (sH, sW, sC) = src.shape, src.stride()
+            else:
+                (C, Hk, Wk), (sC, sH, sW) = src.shape, src.stride()
+            if C != 3:
+                raise ValueError(f"ImageNetBatchKernel: source {k} has {C} channels, need 3")
+            d[k] = (src.data_ptr(), sC, sH, sW, Hk, Wk, geometry[k, 1], geometry[k, 0], geometry[k, 3],
+                    geometry[k, 2], geometry[k, 4], geometry[k, 5], geometry[k, 6], geometry[k, 7], geometry[k, 8], 0,
+                    int(labels[k]))
+        _check_imagenet_outputs(images, target, B, self.device)
+        with torch.cuda.device(self.device):
+            st = torch.cuda.current_stream()
+            _lib.check(_lib.lib().bdbnn_imagenet_batch(
+                ctypes.c_void_p(host.data_ptr()), ctypes.c_void_p(dev.data_ptr()), B, self._mean, self._std,
+                ctypes.c_void_p(images.data_ptr()), *images.stride(), ctypes.c_void_p(target.data_ptr()),
+                ctypes.c_void_p(st.cuda_stream)), "imagenet_batch")
+            ev.record(st)
+        _lib.count(1)
+        return images, target
+
+
+def _check_imagenet_outputs(images, target, b, device):
+    if not (torch.is_tensor(images) and torch.is_tensor(target)):
+        raise ValueError("ImageNet batch: images and target must be tensors")
+    if images.device != device or target.device != device:
+        raise ValueError(f"ImageNet batch: buffers on {images.device} / {target.device}, loader on {device}")
+    if images.dtype != torch.float32 or target.dtype != torch.int64:
+        raise ValueError(f"ImageNet batch: need float32 images and int64 target, got {images.dtype} / {target.dtype}")
+    if tuple(images.shape) != (b, 3, IMAGENET_OUT, IMAGENET_OUT) or tuple(target.shape) != (b,):
+        raise ValueError(f"ImageNet batch: this batch needs images [{b},3,224,224] and target [{b}], got "
+                         f"{tuple(images.shape)} / {tuple(target.shape)}")
+    if not (images.is_contiguous() or images.is_contiguous(memory_format=torch.channels_last)) or \
+            not target.is_contiguous():
+        raise ValueError("ImageNet batch: images must be NCHW- or channels_last-contiguous, target contiguous")
+
+
+class ImageNetDeviceLoader:
+    """An epoch-by-epoch iterable of device batches (images fp32 NCHW [B,3,224,224], target int64 [B]) over an
+    ImageFolder tree, with the transforms of loader.py:52-85: train = RandomResizedCrop(224) + RandomHorizontalFlip,
+    otherwise Resize(256) + CenterCrop(224); then ToTensor + Normalize.  Files are read in a thread pool and decoded
+    per batch; the resize, crop, flip and normalisation of the whole batch is one launch of bdbnn_imagenet_batch.
+
+    root: the class-folder directory (indexed as torchvision.datasets.ImageFolder indexes it).  decode='cpu' (the
+    default) decodes with libjpeg-turbo (torchvision.io.decode_jpeg on the host) in `workers` threads and copies the
+    batch to the device through pinned memory; decode='cuda' decodes JPEGs with nvjpeg (torchvision.io.decode_jpeg on
+    the device, one batched call per batch).  'cpu' is the default because it measured faster: on an H100 host with
+    16 CPUs nvjpeg's batched decode fed the ResNet-18 step at about 450 img/s against about 740 for 'cpu' (DESIGN.md
+    §4m).  Files that are not 1- or 3-component JPEGs (CMYK JPEGs, PNGs under a .JPEG name) and files
+    the decoder rejects are decoded with PIL (Image.open(f).convert('RGB'), ImageFolder's loader), one at a time.
+    With decode='cpu' every batch is bit-identical to torchvision's PIL transform chain for the same crop parameters.
+
+    The training split is shuffled by the epoch permutation of §4l and sharded as CifarDeviceLoader (shard_spans);
+    the validation split is read in order, as the reference's (shuffle=train_flag).  Crop and flip are pure functions
+    of (seed, epoch, dataset index), random_resized_crop_params.  seed=None draws one from torch's default CPU
+    generator.  The next batch is read and decoded in a background thread while the current one is used; `fill`
+    orders its launch after that decode with an event, without a host synchronisation on the device's work."""
+
+    def __init__(self, root, batch_size, train, seed=None, drop_last=False, rank=0, world_size=1, device=None, *,
+                 decode="cpu", workers=16, mean=IMAGENET_MEAN, std=IMAGENET_STD):
+        if decode not in ("cuda", "cpu"):
+            raise ValueError(f"ImageNetDeviceLoader: decode must be 'cuda' or 'cpu', got {decode!r}")
+        if int(batch_size) < 1 or int(world_size) < 1 or not 0 <= int(rank) < int(world_size) or int(workers) < 1:
+            raise ValueError(f"ImageNetDeviceLoader: need batch_size >= 1, workers >= 1 and 0 <= rank < world_size, "
+                             f"got {batch_size}, {workers}, {rank}, {world_size}")
+        if seed is None:
+            seed = int(torch.randint(0, 2 ** 62, (), dtype=torch.int64))
+        if not 0 <= int(seed) < 2 ** 64:
+            raise ValueError(f"ImageNetDeviceLoader: seed must be in [0, 2^64), got {seed}")
+        device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        if device.type != "cuda":
+            raise ValueError(f"ImageNetDeviceLoader: the batch kernel needs a CUDA device, got {device}")
+        if device.index is None:
+            device = torch.device("cuda", torch.cuda.current_device())
+        self.samples, self.class_to_idx = index_image_folder(root)
+        self.n = len(self.samples)
+        if not 1 <= self.n < 2 ** 31:
+            raise ValueError(f"ImageNetDeviceLoader: need 1 <= n < 2^31 images under {root}, found {self.n}")
+        self.batch_size, self.train, self.seed, self.drop_last = int(batch_size), bool(train), int(seed), bool(drop_last)
+        self.rank, self.world_size, self.device, self.decode = int(rank), int(world_size), device, decode
+        self.labels = np.array([c for _, c in self.samples], dtype=np.int64)
+        self.spans = shard_spans(self.n, self.batch_size, self.rank, self.world_size, self.drop_last)
+        self.kernel = ImageNetBatchKernel(device, mean, std)
+        self._pool = ThreadPoolExecutor(int(workers))
+        self._ahead = ThreadPoolExecutor(1)
+        self._pending = None                     # ((epoch, batch index), future of _prepare)
+        self._stream = torch.cuda.Stream(device)
+        self._staging = [None, None]             # decode='cpu': pinned buffers used in turn, with their copy events
+        self._turn = 0
+        self._lock = threading.Lock()
+        self._next_epoch = 0
+
+    def __len__(self):
+        return len(self.spans)
+
+    def set_epoch(self, epoch):
+        self._next_epoch = int(epoch)
+
+    def batch_positions(self, batch_index):
+        """(first epoch position, size) of this rank's batch `batch_index`."""
+        if not 0 <= batch_index < len(self.spans):
+            raise IndexError(f"ImageNetDeviceLoader: batch {batch_index} outside [0, {len(self.spans)})")
+        return self.spans[batch_index]
+
+    def indices(self, epoch, batch_index):
+        """Dataset indices of this rank's batch `batch_index` of epoch `epoch`."""
+        pos0, b = self.batch_positions(batch_index)
+        pos = np.arange(pos0, pos0 + b)
+        return epoch_permutation(self.seed, epoch, pos, self.n) if self.train else pos
+
+    def geometry(self, epoch, idx, sizes):
+        """int [B, 9] rows (y0, x0, h, w, RH, RW, oy0, ox0, flip) of dataset indices idx with decoded sizes [(H, W)]."""
+        H = np.array([s[0] for s in sizes], np.int64)
+        W = np.array([s[1] for s in sizes], np.int64)
+        g = np.zeros((len(idx), 9), np.int64)
+        if self.train:
+            i, j, h, w, flip = random_resized_crop_params(self.seed, epoch, idx, H, W)
+            g[:, 0], g[:, 1], g[:, 2], g[:, 3], g[:, 4], g[:, 5], g[:, 8] = i, j, h, w, IMAGENET_OUT, IMAGENET_OUT, flip
+        else:
+            g[:, 2], g[:, 3] = H, W
+            for k in range(len(idx)):
+                g[k, 4:8] = eval_resize_geometry(int(H[k]), int(W[k]))
+        return g
+
+    # -- decode ------------------------------------------------------------------------------------------------------
+    def _host_decode(self, data):
+        """uint8 (tensor, hwc) of one file on the host: decode_jpeg for 1- and 3-component JPEGs, else PIL."""
+        from torchvision.io import ImageReadMode, decode_jpeg
+        if _jpeg_components(data) in (1, 3):
+            try:
+                return decode_jpeg(torch.frombuffer(bytearray(data), dtype=torch.uint8), mode=ImageReadMode.RGB), False
+            except RuntimeError:
+                pass
+        return torch.from_numpy(np.ascontiguousarray(_pil_decode(data))), True
+
+    def _decode_cuda(self, blobs):
+        """[(device tensor, hwc)] of the batch's files, on self._stream: one batched nvjpeg call for the 1- and
+        3-component JPEGs (per file if the batched call fails), PIL + an H2D copy for the rest."""
+        from torchvision.io import ImageReadMode, decode_jpeg
+        out = [None] * len(blobs)
+        jpeg = [k for k, d in enumerate(blobs) if _jpeg_components(d) in (1, 3)]
+        tensors = [torch.frombuffer(bytearray(blobs[k]), dtype=torch.uint8) for k in jpeg]
+        if tensors:
+            try:
+                for k, t in zip(jpeg, decode_jpeg(tensors, mode=ImageReadMode.RGB, device=self.device)):
+                    out[k] = (t, False)
+            except RuntimeError:
+                for k, t in zip(jpeg, tensors):
+                    try:
+                        out[k] = (decode_jpeg(t, mode=ImageReadMode.RGB, device=self.device), False)
+                    except RuntimeError:
+                        pass
+        for k in range(len(blobs)):
+            if out[k] is None:
+                a = torch.from_numpy(np.ascontiguousarray(_pil_decode(blobs[k]))).pin_memory()
+                out[k] = (a.to(self.device, non_blocking=True), True)
+        return out
+
+    def _decode_cpu(self, blobs):
+        """[(device tensor, hwc)] of the batch's files: host decode in the pool, one pinned staging buffer, one H2D
+        copy on self._stream."""
+        dec = list(self._pool.map(self._host_decode, blobs))
+        sizes = [t.numel() for t, _ in dec]
+        offs = np.concatenate([[0], np.cumsum(sizes)])
+        total = int(offs[-1])
+        k = self._turn
+        self._turn ^= 1
+        st = self._staging[k]
+        if st is not None:
+            st[1].synchronize()                  # the copy that last read this buffer has run
+        if st is None or st[0].numel() < total:
+            st = (torch.empty(int(total * 1.25) + 4096, dtype=torch.uint8, pin_memory=True), torch.cuda.Event())
+            self._staging[k] = st
+        pinned = st[0]
+
+        def put(a):
+            t, o = a
+            pinned[o:o + t.numel()].copy_(t.reshape(-1))
+        list(self._pool.map(put, zip([t for t, _ in dec], offs[:-1].tolist())))
+        buf = torch.empty(total, dtype=torch.uint8, device=self.device)
+        buf.copy_(pinned[:total], non_blocking=True)
+        st[1].record(self._stream)
+        return [(buf[int(offs[i]):int(offs[i + 1])].view(t.shape), hwc) for i, (t, hwc) in enumerate(dec)]
+
+    def _prepare(self, epoch, batch_index):
+        """Read and decode one batch on self._stream: (dataset indices, [(device tensor, hwc)], event)."""
+        idx = self.indices(epoch, batch_index)
+        blobs = list(self._pool.map(_read, [self.samples[int(k)][0] for k in idx]))
+        with self._lock, torch.cuda.device(self.device), torch.cuda.stream(self._stream):
+            srcs = self._decode_cuda(blobs) if self.decode == "cuda" else self._decode_cpu(blobs)
+            ev = torch.cuda.Event()
+            ev.record(self._stream)
+        return idx, srcs, ev
+
+    def _next_of(self, epoch, batch_index):
+        return (epoch, batch_index + 1) if batch_index + 1 < len(self) else (epoch + 1, 0)
+
+    def fill(self, epoch, batch_index, images, target):
+        """Write this rank's batch `batch_index` of epoch `epoch` into the caller's buffers (fp32 [b,3,224,224], NCHW
+        or channels_last, and int64 [b], on the loader's device) with one launch on the current stream, ordered after
+        the batch's decode by an event; returns (images, target).  Starts reading and decoding the next batch."""
+        if not 0 <= int(epoch) < 2 ** 32:
+            raise ValueError(f"ImageNetDeviceLoader.fill: epoch must be in [0, 2^32), got {epoch}")
+        epoch, batch_index = int(epoch), int(batch_index)
+        b = self.batch_positions(batch_index)[1]
+        _check_imagenet_outputs(images, target, b, self.device)
+        if self._pending is not None and self._pending[0] == (epoch, batch_index):
+            idx, srcs, ev = self._pending[1].result()
+        else:
+            if self._pending is not None:
+                self._pending[1].result()
+            idx, srcs, ev = self._prepare(epoch, batch_index)
+        self._pending = None
+        nxt = self._next_of(epoch, batch_index)
+        if nxt[0] < 2 ** 32:
+            self._pending = (nxt, self._ahead.submit(self._prepare, *nxt))
+        sizes = [(t.shape[0], t.shape[1]) if hwc else (t.shape[1], t.shape[2]) for t, hwc in srcs]
+        geo = self.geometry(epoch, idx, sizes)
+        with torch.cuda.device(self.device):
+            st = torch.cuda.current_stream()
+            st.wait_event(ev)
+            for t, _ in srcs:
+                t.record_stream(st)
+            self.kernel(srcs, geo, self.labels[idx], images, target)
+        return images, target
+
+    def __iter__(self):
+        epoch = self._next_epoch
+        self._next_epoch += 1
+        return self._epoch(epoch)
+
+    def _epoch(self, epoch):
+        for i in range(len(self)):
+            b = self.batch_positions(i)[1]
+            yield self.fill(epoch, i, torch.empty((b, 3, IMAGENET_OUT, IMAGENET_OUT), device=self.device),
+                            torch.empty((b,), dtype=torch.int64, device=self.device))
+
+    def close(self):
+        """Finish the pending read-ahead and stop the threads."""
+        if self._pending is not None:
+            self._pending[1].result()
+            self._pending = None
+        self._ahead.shutdown()
+        self._pool.shutdown()
+
+
+def dataloader_imagenet(split='train', batch_size=128, data_path='./', distributed=False, **kwargs):
+    """loader.py:52-85 on the device: ImageFolder data_path/train (RandomResizedCrop(224) + RandomHorizontalFlip,
+    shuffled) or data_path/val (Resize(256) + CenterCrop(224), in order), normalised with loader.py's constants.
+    distributed=True shards the training split over torch.distributed's ranks (the validation split is read whole by
+    every rank, as the reference's, which has no sampler there).  Keyword arguments go to ImageNetDeviceLoader."""
+    train = split == 'train'
+    rank, world = 0, 1
+    if distributed and train:
+        import torch.distributed as dist
+        rank, world = dist.get_rank(), dist.get_world_size()
+    return ImageNetDeviceLoader(os.path.join(data_path, 'train' if train else 'val'), batch_size, train, rank=rank,
+                                world_size=world, **kwargs)

@@ -565,6 +565,40 @@ BDBNN_API int bdbnn_cifar_batch(const uint8_t* images, const int64_t* labels, in
                                 const float* std_host, float* out, int64_t sN, int64_t sC, int64_t sH, int64_t sW,
                                 int64_t* target, void* stream);
 
+/* ---- ImageNet input batch from decoded uint8 images (csrc/imagenet_data.cu) ---------------------------------------
+ * Replaces the per-image PIL transforms of loader.py:52-85 (RandomResizedCrop(224) + RandomHorizontalFlip, or
+ * Resize(256) + CenterCrop(224); then ToTensor, Normalize) for images already decoded to uint8 RGB on the device.
+ * One descriptor per image (88 bytes):
+ *   src            : device pointer to the decoded image; pixel (c, y, x) at src[c * sC + y * sH + x * sW] (uint8
+ *                    element strides: CHW planar and HWC both work); H x W, each side in [1, 8192]
+ *   x0, y0, w, h   : crop box inside the source
+ *   RH, RW         : size the box is resized to, in [224, 2^22] per side
+ *   oy0, ox0       : origin of the 224 x 224 output window inside the resized image
+ *   flip           : 1 mirrors the output columns (after the resize, as torchvision's hflip)
+ *   label          : written to target[b]
+ * Training: box = the crop, resized = 224 x 224, window (0, 0).  Evaluation: box = the whole image, resized =
+ * Resize(256)'s size, window = CenterCrop(224)'s offsets.  Output element (b, c, i, j) = fp32((fp32(u / 255) -
+ * mean[c]) / std[c]), each step rounded, u = pixel (oy0 + i, ox0 + (flip ? 223 - j : j)) of Pillow's antialiased
+ * bilinear resize (uint8, 22-bit fixed point, horizontal pass then vertical; DESIGN.md §4m,
+ * oracle/imagenet_data_ref.py) of the box to RH x RW; written through the element strides (sN, sC, sH, sW).
+ * desc_host: B descriptors in HOST memory (pinned, so that the copy is asynchronous: keep them unchanged until work
+ * queued on `stream` after this call has run); desc_dev: device memory for B descriptors, 8-byte aligned.  Every
+ * descriptor is validated on the host.  mean_host / std_host: 3 floats each, HOST memory.  One H2D copy and one
+ * launch on `stream`; nothing read back. */
+typedef struct bdbnn_imagenet_desc {
+  const uint8_t* src;
+  int64_t sC, sH, sW;
+  int32_t H, W;
+  int32_t x0, y0, w, h;
+  int32_t RH, RW;
+  int32_t oy0, ox0;
+  int32_t flip, reserved;
+  int64_t label;
+} bdbnn_imagenet_desc;
+BDBNN_API int bdbnn_imagenet_batch(const bdbnn_imagenet_desc* desc_host, bdbnn_imagenet_desc* desc_dev, int32_t B,
+                                   const float* mean_host, const float* std_host, float* out, int64_t sN,
+                                   int64_t sC, int64_t sH, int64_t sW, int64_t* target, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,0 +1,281 @@
+"""Throughput of the graphed ImageNet ResNet-18 CE step (batch 256, bench.py's workload) when it is fed real JPEG
+batches from disk, four ways:
+
+    a  the reference pipeline (loader.py:52-85, train.py:488-491): torchvision ImageFolder with RandomResizedCrop(224),
+       RandomHorizontalFlip, ToTensor, Normalize on PIL images in a 16-worker DataLoader with pin_memory, .cuda()
+    b  ImageNetDeviceLoader(decode='cuda').fill into the step's static input buffers (nvjpeg decode)
+    c  ImageNetDeviceLoader(decode='cpu', workers=16).fill (libjpeg-turbo decode in 16 host threads)
+    d  one batch resident in device memory, never rewritten
+
+    python tools/imagenet_input_throughput.py [--rounds 3] [--steps 70] [--warmup 20] [--images 23040]
+
+The data is a synthetic ImageFolder written to a temporary directory (removed at the end): --images JPEGs (quality 90,
+textured so that a 500 x 375 file is about 100 KB) in 100 classes, sized like ImageNet's 500 x 375 / 375 x 500 /
+500 x 333 with one image in 200 of 2 000-4 000 px.  Every file is read once before timing, so the timed passes read
+from the page cache (warm files).  Every arm runs in a process of its own, started afresh every round, the arms
+alternated (a, b, c, d per round); each process captures the step, runs --warmup steps and times --steps steps with a
+host clock between two device synchronisations.  Then, once: each loader alone (img/s, no step), the batch kernel alone
+(CUDA events around 200 launches on one decoded batch of 256) and one evaluation pass (Resize(256) + CenterCrop(224)
+through ImageNetDeviceLoader (decode="cpu") into the eval-mode forward).  The card name, power limit and maximum SM
+clock are read (read-only) from nvidia-smi.  Needs a CUDA device."""
+import argparse
+import json
+import os
+import shutil
+import subprocess
+import sys
+import tempfile
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+BATCH, CLASSES = 256, 100
+
+
+def _write_one(args):
+    path, seed = args
+    import numpy as np
+    from PIL import Image
+    rng = np.random.default_rng(seed)
+    if seed % 200 == 7:
+        H, W = (int(v) for v in rng.integers(2000, 4001, 2))
+    else:
+        H, W = [(375, 500), (500, 375), (333, 500)][seed % 3]
+    x = np.arange(W, dtype=np.float32)[None, :, None] / (4 + rng.random(3, dtype=np.float32) * 30)
+    y = np.arange(H, dtype=np.float32)[:, None, None] / (4 + rng.random(3, dtype=np.float32) * 30)
+    img = 127 + 90 * np.sin(x + y) + rng.integers(-24, 25, (H, W, 3), dtype=np.int16)
+    Image.fromarray(np.clip(img, 0, 255).astype(np.uint8)).save(path, "JPEG", quality=90)
+    return os.path.getsize(path)
+
+
+def write_folder(root, n):
+    from multiprocessing import Pool
+    jobs = []
+    for k in range(n):
+        d = os.path.join(root, "train", f"n{k % CLASSES:08d}")
+        os.makedirs(d, exist_ok=True)
+        jobs.append((os.path.join(d, f"img_{k:06d}.JPEG"), k))
+    with Pool(min(32, os.cpu_count() or 1)) as p:
+        sizes = p.map(_write_one, jobs, chunksize=64)
+    return sum(sizes) / len(sizes)
+
+
+def _warm(root):
+    for dirpath, _, files in os.walk(root):
+        for f in files:
+            with open(os.path.join(dirpath, f), "rb") as fh:
+                fh.read()
+
+
+def _step(torch):
+    from bdbnn_b200.resnet import resnet18
+    from bdbnn_b200.step import GraphedTrainStep, StepConfig, TrainStep, make_optimizer
+    torch.backends.cudnn.benchmark = False
+    torch.manual_seed(0)
+    model = resnet18().cuda()
+    return GraphedTrainStep(TrainStep(model, make_optimizer(model, "imagenet"), StepConfig()))
+
+
+def _reference_loader(torch, root):
+    import torchvision.datasets as datasets
+    import torchvision.transforms as T
+    from bdbnn_b200.data import IMAGENET_MEAN, IMAGENET_STD
+    ds = datasets.ImageFolder(os.path.join(root, "train"), T.Compose([
+        T.RandomResizedCrop(224), T.RandomHorizontalFlip(), T.ToTensor(), T.Normalize(IMAGENET_MEAN, IMAGENET_STD)]))
+    return torch.utils.data.DataLoader(ds, batch_size=BATCH, shuffle=True, num_workers=16, pin_memory=True,
+                                       drop_last=True)
+
+
+def _feeder(torch, args):
+    """next() -> (images, target) on the device for arm a, b or c; for b / c the step's static buffers once known."""
+    from bdbnn_b200.data import ImageNetDeviceLoader
+    if args.arm == "a":
+        it = iter(_reference_loader(torch, args.root))
+
+        def nxt(gstep):
+            x, y = next(it)
+            return (x.cuda(non_blocking=True).contiguous(memory_format=torch.channels_last),
+                    y.cuda(non_blocking=True))
+        return nxt
+    loader = ImageNetDeviceLoader(os.path.join(args.root, "train"), BATCH, True, seed=0, drop_last=True,
+                                  decode="cuda" if args.arm == "b" else "cpu", workers=16)
+    state = {"epoch": 0, "i": 0}
+
+    def nxt(gstep):
+        if state["i"] == len(loader):
+            state["epoch"], state["i"] = state["epoch"] + 1, 0
+        if gstep is None or gstep.static_images is None:
+            x = torch.empty(BATCH, 3, 224, 224, device="cuda").contiguous(memory_format=torch.channels_last)
+            y = torch.empty(BATCH, dtype=torch.int64, device="cuda")
+        else:
+            x, y = gstep.static_images, gstep.static_target
+        out = loader.fill(state["epoch"], state["i"], x, y)
+        state["i"] += 1
+        return out
+    return nxt
+
+
+def arm(torch, args):
+    gstep = _step(torch)
+    if args.arm == "d":
+        g = torch.Generator().manual_seed(0)
+        gstep(torch.randn(BATCH, 3, 224, 224, generator=g).cuda().contiguous(memory_format=torch.channels_last),
+              torch.randint(0, CLASSES, (BATCH,), generator=g).cuda())
+
+        def run(steps):
+            for _ in range(steps):
+                gstep(gstep.static_images, gstep.static_target)
+    else:
+        nxt = _feeder(torch, args)
+
+        def run(steps):
+            for _ in range(steps):
+                gstep(*nxt(gstep))
+    run(args.warmup)
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    run(args.steps)
+    torch.cuda.synchronize()
+    s = time.perf_counter() - t0
+    print(json.dumps({"arm": args.arm, "s": round(s, 4), "img_per_s": round(args.steps * BATCH / s, 1)}), flush=True)
+
+
+def loaders_alone(torch, args):
+    """img/s of each loader with nothing else on the device: 5 warm-up batches, then 30 timed."""
+    res = {}
+    for which in "abc":
+        args.arm = which
+        nxt = _feeder(torch, args)
+        for _ in range(5):
+            nxt(None)
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        for _ in range(30):
+            nxt(None)
+        torch.cuda.synchronize()
+        res[which] = round(30 * BATCH / (time.perf_counter() - t0), 1)
+    print(json.dumps({"loader_alone_img_per_s": res}), flush=True)
+
+
+def kernel_time(torch, args):
+    """The batch kernel alone on one nvjpeg-decoded training batch of 256: CUDA events around 200 launches."""
+    import numpy as np
+    from bdbnn_b200.data import ImageNetBatchKernel, ImageNetDeviceLoader
+    loader = ImageNetDeviceLoader(os.path.join(args.root, "train"), BATCH, True, seed=0, drop_last=True, decode="cuda")
+    idx, srcs, ev = loader._prepare(0, 0)
+    torch.cuda.current_stream().wait_event(ev)
+    sizes = [(t.shape[1], t.shape[2]) if not hwc else (t.shape[0], t.shape[1]) for t, hwc in srcs]
+    geo = loader.geometry(0, idx, sizes)
+    kern = ImageNetBatchKernel(torch.device("cuda", torch.cuda.current_device()))
+    x = torch.empty(BATCH, 3, 224, 224, device="cuda").contiguous(memory_format=torch.channels_last)
+    y = torch.empty(BATCH, dtype=torch.int64, device="cuda")
+    for _ in range(20):
+        kern(srcs, geo, loader.labels[idx], x, y)
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(200):
+        kern(srcs, geo, loader.labels[idx], x, y)
+    e1.record()
+    e1.synchronize()
+    src_bytes = int(sum(t.numel() for t, _ in srcs))
+    print(json.dumps({"kernel_us_per_batch": round(e0.elapsed_time(e1) * 1e3 / 200, 1),
+                      "decoded_MB_per_batch": round(src_bytes / 1e6, 1),
+                      "out_MB_per_batch": round(BATCH * 3 * 224 * 224 * 4 / 1e6, 1),
+                      "mean_px": round(float(np.mean([h * w for h, w in sizes])), 0)}), flush=True)
+    loader.close()
+
+
+def eval_pass(torch, args):
+    """One pass of Resize(256) + CenterCrop(224) batches (decode="cpu") through the eval-mode forward, against the
+    same number of forwards on a resident batch."""
+    from bdbnn_b200.data import ImageNetDeviceLoader
+    from bdbnn_b200.resnet import resnet18
+    torch.manual_seed(0)
+    model = resnet18().cuda().eval()
+    loader = ImageNetDeviceLoader(os.path.join(args.root, "train"), BATCH, False, drop_last=True)
+    n = min(len(loader), 40)
+    x = torch.empty(BATCH, 3, 224, 224, device="cuda").contiguous(memory_format=torch.channels_last)
+    y = torch.empty(BATCH, dtype=torch.int64, device="cuda")
+    with torch.no_grad():
+        for i in range(3):
+            model(loader.fill(0, i, x, y)[0])
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        for i in range(n):
+            model(loader.fill(0, i, x, y)[0])
+        torch.cuda.synchronize()
+        fed = n * BATCH / (time.perf_counter() - t0)
+        t0 = time.perf_counter()
+        for i in range(n):
+            model(x)
+        torch.cuda.synchronize()
+        resident = n * BATCH / (time.perf_counter() - t0)
+    print(json.dumps({"eval_img_per_s": {"loader_cpu": round(fed, 1), "resident": round(resident, 1),
+                                         "batches": n}}), flush=True)
+    loader.close()
+
+
+def _run(args, which):
+    cmd = [sys.executable, os.path.abspath(__file__), "--arm", which, "--root", args.root, "--steps", str(args.steps),
+           "--warmup", str(args.warmup)]
+    r = subprocess.run(cmd, capture_output=True, text=True)
+    if r.returncode != 0:
+        raise SystemExit(f"imagenet_input_throughput: arm {which} failed:\n{r.stderr[-3000:]}")
+    return json.loads(r.stdout.strip().splitlines()[-1])
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--steps", type=int, default=70)
+    ap.add_argument("--warmup", type=int, default=20)
+    ap.add_argument("--images", type=int, default=90 * BATCH)
+    ap.add_argument("--arm", choices=("a", "b", "c", "d", "extras"), help=argparse.SUPPRESS)
+    ap.add_argument("--root", help=argparse.SUPPRESS)
+    args = ap.parse_args()
+    import torch
+    if not torch.cuda.is_available():
+        raise SystemExit("imagenet_input_throughput: no CUDA device")
+    if args.arm == "extras":
+        loaders_alone(torch, args)
+        kernel_time(torch, args)
+        eval_pass(torch, args)
+        return
+    if args.arm:
+        arm(torch, args)
+        return
+    if (args.warmup + args.steps) * BATCH > args.images:
+        raise SystemExit("imagenet_input_throughput: --images must cover --warmup + --steps batches (one epoch)")
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True)
+    tmp = tempfile.mkdtemp(prefix="imagenet_input_")
+    try:
+        t0 = time.perf_counter()
+        mean_bytes = write_folder(tmp, args.images)
+        _warm(tmp)
+        args.root = tmp
+        print(json.dumps({"gpu": q.stdout.strip().splitlines()[0] if q.returncode == 0 else None, "batch": BATCH,
+                          "images": args.images, "mean_file_KB": round(mean_bytes / 1e3, 1), "steps": args.steps,
+                          "warmup": args.warmup, "rounds": args.rounds, "host_cpus": os.cpu_count(),
+                          "write_s": round(time.perf_counter() - t0, 1), "page_cache": "warm"}), flush=True)
+        res = {a: [] for a in "abcd"}
+        for _ in range(args.rounds):
+            for a in "abcd":
+                r = _run(args, a)
+                print(json.dumps(r), flush=True)
+                res[a].append(r["img_per_s"])
+        med = {a: sorted(v)[len(v) // 2] for a, v in res.items()}
+        print(json.dumps({"img_per_s": res, "b_over_d_median": round(med["b"] / med["d"], 4),
+                          "c_over_d_median": round(med["c"] / med["d"], 4),
+                          "b_over_a_median": round(med["b"] / med["a"], 3),
+                          "c_over_a_median": round(med["c"] / med["a"], 3)}), flush=True)
+        cmd = [sys.executable, os.path.abspath(__file__), "--arm", "extras", "--root", tmp]
+        r = subprocess.run(cmd, capture_output=True, text=True)
+        print(r.stdout.strip() if r.returncode == 0 else f"extras failed:\n{r.stderr[-3000:]}", flush=True)
+    finally:
+        shutil.rmtree(tmp, ignore_errors=True)
+
+
+if __name__ == "__main__":
+    main()
