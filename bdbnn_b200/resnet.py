@@ -8,6 +8,8 @@ non-linearity other than the sign inside the conv.
 
 The builders take `conv_cls` so the CPU oracle (oracle/models_ref.py) can instantiate the same
 topology around its pure-PyTorch conv."""
+import contextlib
+
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
@@ -56,14 +58,37 @@ def _eval_unit(x, conv, bn, residual, shortcut=None):
                                conv.stride[0], conv.padding[0], residual, shortcut=shortcut)
 
 
+def _unit(x, conv, bn, residual, shortcut=None):
+    """BN(conv(x)) + residual: the eval unit, else the fused training unit, else the module chain.  With `shortcut` =
+    functional.PadShortcut the residual is the option-A shortcut of x read in place (the caller checked
+    pad_shortcut_supported), which only the units can do: None when neither takes the pair."""
+    out = _eval_unit(x, conv, bn, residual, shortcut)
+    if out is None:
+        out = _fused_unit(x, conv, bn, residual, shortcut)
+    if out is None and shortcut is None:
+        out = bn(conv(x)) + residual
+    return out
+
+
+def _downsample_pair(ds):
+    """(conv, bn) of a `downsample` branch the 1x1 shortcut kernels take, Sequential(bias-free 1x1 nn.Conv2d,
+    BatchNorm2d) with a square stride, no padding and one group, else None."""
+    if not (isinstance(ds, nn.Sequential) and len(ds) == 2 and type(ds[0]) is nn.Conv2d and
+            isinstance(ds[1], nn.BatchNorm2d)):
+        return None
+    conv, bn = ds[0], ds[1]
+    if not (conv.bias is None and conv.kernel_size == (1, 1) and conv.padding == (0, 0) and
+            conv.stride[0] == conv.stride[1] and conv.groups == 1):
+        return None
+    return conv, bn
+
+
 def _eval_shortcut(x, ds):
     """The `downsample` branch in eval mode: BN_eval(1x1 conv) on the wgmma forward when it qualifies, else ds(x)."""
-    if (isinstance(ds, nn.Sequential) and len(ds) == 2 and type(ds[0]) is nn.Conv2d and
-            isinstance(ds[1], nn.BatchNorm2d)):
-        conv, bn = ds[0], ds[1]
+    pair = _downsample_pair(ds)
+    if pair is not None:
+        conv, bn = pair
         if (_eval_mode(x, bn) and bn.affine and bn.running_mean is not None and bn.running_var is not None and
-                conv.bias is None and conv.kernel_size == (1, 1) and conv.padding == (0, 0) and
-                conv.stride[0] == conv.stride[1] and conv.groups == 1 and
                 F_.shortcut_eval_supported(x, conv.weight, conv.stride[0])):
             return F_._shortcut_eval_impl(x, conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps,
                                           conv.stride[0])
@@ -93,16 +118,27 @@ def _prepack(model, x):
     return True
 
 
+@contextlib.contextmanager
+def _prepacked_weights(model, x):
+    """The stem and the layers of a shell's forward run inside this: _prepack before them, and functional._PREPACKED
+    cleared after them, on an exception too, when this forward filled it."""
+    packed = _prepack(model, x)
+    try:
+        yield
+    finally:
+        if packed:
+            F_._PREPACKED.clear()
+
+
 def _shortcut_args(x, ds):
-    """Arguments for the tcgen05 `downsample` path — Sequential(fp32 1x1 Conv2d, BatchNorm2d) in training
-    mode on a supported geometry — or None."""
-    if not (isinstance(ds, nn.Sequential) and len(ds) == 2 and type(ds[0]) is nn.Conv2d and
-            isinstance(ds[1], nn.BatchNorm2d)):
+    """Arguments for the wgmma `downsample` path — a _downsample_pair in training mode on a supported geometry — or
+    None."""
+    pair = _downsample_pair(ds)
+    if pair is None:
         return None
-    conv, bn = ds[0], ds[1]
+    conv, bn = pair
     if not (x.is_cuda and bn.training and bn.affine and bn.track_running_stats and bn.momentum is not None and
-            conv.bias is None and conv.kernel_size == (1, 1) and conv.padding == (0, 0) and
-            conv.stride[0] == conv.stride[1] and conv.groups == 1 and F_.fuse_enabled() and F_.shortcut_tc_enabled()):
+            F_.fuse_enabled() and F_.shortcut_tc_enabled()):
         return None
     if not F_.shortcut_supported(x, conv.weight, conv.stride[0]):
         return None
@@ -128,26 +164,16 @@ class BasicBlock(nn.Module):
             # conv1 + bn1 + the real-valued 1x1 shortcut (conv + bn) as ONE node when everything qualifies:
             # the shortcut's input gradient is then added in place to conv1's (no zero fill, no add kernel)
             sc = _shortcut_args(x, self.downsample)
-            if sc is not None:
+            if sc is None:
+                residual = _eval_shortcut(x, self.downsample)
+            else:
                 out = _fused_unit(x, self.conv1, self.bn1, None, shortcut=sc)
-                if out is not None:
-                    self.downsample[1].num_batches_tracked.add_(1)
-            if out is None:
-                residual = (F_.shortcut_conv_bn(x, *sc) if sc is not None else _eval_shortcut(x, self.downsample))
-                if sc is not None:
-                    self.downsample[1].num_batches_tracked.add_(1)
+                if out is None:
+                    residual = F_.shortcut_conv_bn(x, *sc)
+                self.downsample[1].num_batches_tracked.add_(1)
         if out is None:
-            out = _eval_unit(x, self.conv1, self.bn1, residual)
-        if out is None:
-            out = _fused_unit(x, self.conv1, self.bn1, residual)
-        if out is None:
-            out = self.bn1(self.conv1(x)) + residual
-        out2 = _eval_unit(out, self.conv2, self.bn2, out)
-        if out2 is None:
-            out2 = _fused_unit(out, self.conv2, self.bn2, out)
-        if out2 is None:
-            out2 = self.bn2(self.conv2(out)) + out
-        return out2
+            out = _unit(x, self.conv1, self.bn1, residual)
+        return _unit(out, self.conv2, self.bn2, out)
 
 
 class ResNetImageNet(nn.Module):
@@ -203,13 +229,9 @@ class ResNetImageNet(nn.Module):
         return mp(bn(y))
 
     def forward(self, x):
-        packed = _prepack(self, x)
-        try:
+        with _prepacked_weights(self, x):
             x = self._stem(x)
             x = self.layer4(self.layer3(self.layer2(self.layer1(x))))
-        finally:
-            if packed:
-                F_._PREPACKED.clear()
         return self.fc(torch.flatten(self.avgpool(x), 1))
 
 
@@ -241,26 +263,10 @@ class BasicBlockCifar(nn.Module):
             # gradient (BDBNN_SHORTCUT_TC=0: _PadShortcut)
             sc = F_.PadShortcut(self.shortcut.pad)
             if F_.pad_shortcut_supported(x.shape, self.conv1.weight.shape, self.conv1.stride[0], sc.pad):
-                out = _eval_unit(x, self.conv1, self.bn1, None, shortcut=sc)
-                if out is None:
-                    out = _fused_unit(x, self.conv1, self.bn1, None, shortcut=sc)
+                out = _unit(x, self.conv1, self.bn1, None, shortcut=sc)
         if out is None:
-            out = self._conv1_unit(x)
-        out2 = _eval_unit(out, self.conv2, self.bn2, out)
-        if out2 is None:
-            out2 = _fused_unit(out, self.conv2, self.bn2, out)
-        if out2 is None:
-            out2 = self.bn2(self.conv2(out)) + out
-        return out2
-
-    def _conv1_unit(self, x):
-        residual = x if self.shortcut is None else self.shortcut(x)
-        out = _eval_unit(x, self.conv1, self.bn1, residual)
-        if out is None:
-            out = _fused_unit(x, self.conv1, self.bn1, residual)
-        if out is None:
-            out = self.bn1(self.conv1(x)) + residual
-        return out
+            out = _unit(x, self.conv1, self.bn1, x if self.shortcut is None else self.shortcut(x))
+        return _unit(out, self.conv2, self.bn2, out)
 
 
 def _cifar_stem_qualifies(x, c1, bn):
@@ -319,13 +325,9 @@ class ResNetCifar(nn.Module):
         return nn.Sequential(*layers)
 
     def forward(self, x):
-        packed = _prepack(self, x)
-        try:
+        with _prepacked_weights(self, x):
             x = _cifar_stem(x, self.conv1, self.bn1)
             x = self.layer3(self.layer2(self.layer1(x)))
-        finally:
-            if packed:
-                F_._PREPACKED.clear()
         return self.fc(torch.flatten(self.avgpool(x), 1))
 
 
@@ -350,13 +352,9 @@ class ResNetCifar18(nn.Module):
     _make_layer = ResNetImageNet._make_layer
 
     def forward(self, x):
-        packed = _prepack(self, x)
-        try:
+        with _prepacked_weights(self, x):
             x = _cifar_stem(x, self.conv1, self.bn1)
             x = self.layer4(self.layer3(self.layer2(self.layer1(x))))
-        finally:
-            if packed:
-                F_._PREPACKED.clear()
         return self.fc(torch.flatten(self.avgpool(x), 1))
 
 

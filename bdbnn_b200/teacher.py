@@ -16,12 +16,51 @@ CUDA-core launch and its option-A shortcuts are read in place by conv1's epilogu
 ResNet-18 has the same stem and no ReLU; each of its 1x1 `downsample` branches runs on the shortcut eval GEMM and is
 conv1's residual (DESIGN.md §4k).  Anything else returns the wrapped model's own forward."""
 import ctypes
+from typing import NamedTuple
 
 import torch
 import torch.nn as nn
 
 from . import _lib
 from . import functional as F_
+from .resnet import BasicBlock, BasicBlockCifar, ResNetCifar, ResNetCifar18, _PadShortcut
+
+
+class _Family(NamedTuple):
+    """What the structure check, the geometry walk, the kernel forward and the launch count know of a network."""
+    children: tuple     # names of the model's children, in order
+    block: type         # of every residual block
+    pooled_stem: bool   # 7x7 / stride-2 conv + BatchNorm + ReLU + max-pool (stem_conv_bn_relu_pool_eval, 6 launches);
+    #                     else the 3x3 CIFAR stem conv + BatchNorm (cifar_stem_conv_bn_eval, 2 launches)
+    relu: bool          # a ReLU follows each conv + BatchNorm (+ residual); else there is none anywhere
+    shortcut: str       # the block attribute that is None or the shortcut of a block that changes shape: "downsample",
+    #                     a 1x1 conv + BatchNorm on the shortcut eval GEMM (6 launches), or "shortcut", the option-A
+    #                     _PadShortcut that conv1's epilogue reads in place (no launch)
+    bireal: bool        # out = bn1(conv1(x)) + shortcut(x); out2 = bn2(conv2(out)) + out (Bi-Real: one shortcut per
+    #                     conv); else out = bn1(conv1(x)); out2 = bn2(conv2(out)) + shortcut(x)
+
+
+_LAYERS = ("layer1", "layer2", "layer3", "layer4")
+_CIFAR = _Family(("conv1", "bn1") + _LAYERS[:3] + ("avgpool", "fc"), BasicBlockCifar, False, False, "shortcut", True)
+_CIFAR18 = _Family(("conv1", "bn1") + _LAYERS + ("avgpool", "fc"), BasicBlock, False, False, "downsample", True)
+
+
+def _family(model):
+    """The _Family of `model` by its exact type: a subclass or a wrapper (nn.DataParallel) is refused."""
+    if type(model) is ResNetCifar:
+        return _CIFAR
+    if type(model) is ResNetCifar18:
+        return _CIFAR18
+    from torchvision.models import resnet as tv
+    if type(model) is not tv.ResNet:
+        raise TypeError(f"FrozenResNetTeacher wraps a torchvision ResNet with BasicBlocks (resnet18/34) or an fp32 "
+                        f"bdbnn_b200.resnet.ResNetCifar / ResNetCifar18, got {type(model).__name__}")
+    return _Family(("conv1", "bn1", "relu", "maxpool") + _LAYERS + ("avgpool", "fc"), tv.BasicBlock, True, True,
+                   "downsample", False)
+
+
+def _bn_args(bn):
+    return bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps
 
 
 def _check_bn(bn, where):
@@ -34,170 +73,94 @@ def _check_conv(conv, where, k, bias=False):
         raise TypeError(f"FrozenResNetTeacher: {where} must be nn.Conv2d, got {type(conv).__name__}")
     if (conv.kernel_size != (k, k) or conv.groups != 1 or conv.dilation != (1, 1) or (conv.bias is not None) != bias
             or conv.padding_mode != "zeros" or conv.stride[0] != conv.stride[1] or conv.padding[0] != conv.padding[1]):
-        raise TypeError(f"FrozenResNetTeacher: {where} is not a {k}x{k} conv of a torchvision BasicBlock ResNet")
+        raise TypeError(f"FrozenResNetTeacher: {where} is not a {k}x{k} conv of a BasicBlock ResNet")
 
 
-def _cifar_blocks(model):
-    """[(name, block)] of layer1..layer3 after checking that `model` (a ResNetCifar) has nn.Conv2d convs throughout:
-    the fp32 CIFAR teacher.  A ResNetCifar with binary convs is a student, whose eval forward has its own units."""
-    from .resnet import BasicBlockCifar, _PadShortcut
-    names = [n for n, _ in model.named_children()]
-    if names != ["conv1", "bn1", "layer1", "layer2", "layer3", "avgpool", "fc"]:
-        raise TypeError(f"FrozenResNetTeacher: unexpected children {names}")
-    if list(model.named_parameters(recurse=False)) or list(model.named_buffers(recurse=False)):
-        raise TypeError("FrozenResNetTeacher: the model itself must hold no parameters or buffers")
-    _check_stem_cifar(model)
-    if type(model.avgpool) is not nn.AdaptiveAvgPool2d or type(model.fc) is not nn.Linear:
-        raise TypeError("FrozenResNetTeacher: the head must be nn.AdaptiveAvgPool2d and nn.Linear")
-    out = []
-    for li in range(1, 4):
-        layer = getattr(model, f"layer{li}")
-        if type(layer) is not nn.Sequential:
-            raise TypeError(f"FrozenResNetTeacher: layer{li} must be nn.Sequential")
-        for bi, blk in layer.named_children():
-            where = f"layer{li}.{bi}"
-            if type(blk) is not BasicBlockCifar:
-                raise TypeError(f"FrozenResNetTeacher: {where} is a {type(blk).__name__}; only BasicBlockCifar is "
-                                "supported")
-            _check_conv(blk.conv1, where + ".conv1", 3)
-            _check_conv(blk.conv2, where + ".conv2", 3)
-            if blk.conv2.stride != (1, 1) or blk.conv1.padding != (1, 1) or blk.conv2.padding != (1, 1):
-                raise TypeError(f"FrozenResNetTeacher: {where} convs are not the BasicBlockCifar's")
-            _check_bn(blk.bn1, where + ".bn1")
-            _check_bn(blk.bn2, where + ".bn2")
-            sc = blk.shortcut
-            cin, cout = blk.conv1.in_channels, blk.conv1.out_channels
-            if sc is None:
-                if blk.conv1.stride != (1, 1) or cin != cout:
-                    raise TypeError(f"FrozenResNetTeacher: {where} changes shape but has no shortcut")
-            elif type(sc) is not _PadShortcut or not F_.pad_shortcut_supported(
-                    (1, cin, 1, 1), tuple(blk.conv1.weight.shape), blk.conv1.stride[0], sc.pad):
-                raise TypeError(f"FrozenResNetTeacher: {where}.shortcut must be the option-A _PadShortcut of a "
-                                "stride-2 conv1 with Cout = Cin + 2 * pad (multiples of 4)")
-            out.append((where, blk))
-    return out
-
-
-def _check_stem_cifar(model):
+def _check_stem(model, fam):
     c1 = model.conv1
-    _check_conv(c1, "conv1", 3)
-    if c1.in_channels != 3 or not F_.cifar_stem_supported((1, 3, 1, 1), tuple(c1.weight.shape), c1.stride,
-                                                          c1.padding):
-        raise TypeError("FrozenResNetTeacher: conv1 must be the 3x3 / stride-1 / pad-1 CIFAR stem on 3 channels with "
-                        "16, 32, 48 or 64 outputs")
-    _check_bn(model.bn1, "bn1")
+    if fam.pooled_stem:
+        _check_conv(c1, "conv1", 7)
+        if c1.stride != (2, 2) or c1.padding != (3, 3) or c1.in_channels != 3:
+            raise TypeError("FrozenResNetTeacher: conv1 must be the 7x7 / stride-2 / pad-3 stem on 3 channels")
+        _check_bn(model.bn1, "bn1")
+        mp = model.maxpool
+        if type(model.relu) is not nn.ReLU or type(mp) is not nn.MaxPool2d or mp.ceil_mode or mp.dilation != 1 \
+                or mp.return_indices:
+            raise TypeError("FrozenResNetTeacher: the stem must end in nn.ReLU and nn.MaxPool2d")
+    else:
+        _check_conv(c1, "conv1", 3)
+        if c1.in_channels != 3 or not F_.cifar_stem_supported((1, 3, 1, 1), tuple(c1.weight.shape), c1.stride,
+                                                              c1.padding):
+            raise TypeError("FrozenResNetTeacher: conv1 must be the 3x3 / stride-1 / pad-1 CIFAR stem on 3 channels "
+                            "with 16, 32, 48 or 64 outputs")
+        _check_bn(model.bn1, "bn1")
+        if fam is _CIFAR18 and c1.out_channels != 64:
+            raise TypeError("FrozenResNetTeacher: the CIFAR ResNet-18 stem must have 64 outputs")
 
 
-def _cifar18_blocks(model):
-    """[(name, block)] of layer1..layer4 after checking that `model` (a ResNetCifar18) has nn.Conv2d convs throughout:
-    the fp32 CIFAR ResNet-18 teacher.  Its blocks are Bi-Real BasicBlocks (no ReLU), each `downsample` the
-    Sequential(bias-free 1x1 nn.Conv2d, nn.BatchNorm2d) of a block that changes shape.  A ResNetCifar18 with binary
-    convs is a student, whose eval forward has its own units."""
-    from .resnet import BasicBlock
+def _check_shortcut(blk, where, fam):
+    sc = getattr(blk, fam.shortcut)
+    conv1 = blk.conv1
+    cin, cout = conv1.in_channels, conv1.out_channels
+    # whether the shortcut fits conv1's shape change is asked of this package's blocks, not of a torchvision block
+    own = fam is _CIFAR or fam is _CIFAR18
+    if sc is None:
+        if own and (conv1.stride != (1, 1) or cin != cout):
+            raise TypeError(f"FrozenResNetTeacher: {where} changes shape but has no {fam.shortcut}")
+    elif fam.shortcut == "shortcut":
+        if type(sc) is not _PadShortcut or not F_.pad_shortcut_supported((1, cin, 1, 1), tuple(conv1.weight.shape),
+                                                                         conv1.stride[0], sc.pad):
+            raise TypeError(f"FrozenResNetTeacher: {where}.shortcut must be the option-A _PadShortcut of a stride-2 "
+                            "conv1 with Cout = Cin + 2 * pad (multiples of 4)")
+    else:
+        if type(sc) is not nn.Sequential or len(sc) != 2:
+            raise TypeError(f"FrozenResNetTeacher: {where}.downsample must be Sequential(1x1 Conv2d, BatchNorm2d)")
+        _check_conv(sc[0], where + ".downsample.0", 1)
+        if sc[0].padding != (0, 0):
+            raise TypeError(f"FrozenResNetTeacher: {where}.downsample.0 must have no padding")
+        if own and (sc[0].stride != conv1.stride or sc[0].in_channels != cin or sc[0].out_channels != cout):
+            raise TypeError(f"FrozenResNetTeacher: {where}.downsample.0 must map conv1's input to its output shape")
+        _check_bn(sc[1], where + ".downsample.1")
+
+
+def _blocks(model):
+    """(family, [(name, block)] of the residual blocks) after checking that `model` is a torchvision BasicBlock
+    ResNet, or a ResNetCifar or ResNetCifar18 with nn.Conv2d convs throughout: the fp32 teachers.  A CIFAR shell with
+    binary convs is a student, whose eval forward has its own units."""
+    fam = _family(model)
     names = [n for n, _ in model.named_children()]
-    if names != ["conv1", "bn1", "layer1", "layer2", "layer3", "layer4", "avgpool", "fc"]:
+    if names != list(fam.children):
         raise TypeError(f"FrozenResNetTeacher: unexpected children {names}")
     if list(model.named_parameters(recurse=False)) or list(model.named_buffers(recurse=False)):
         raise TypeError("FrozenResNetTeacher: the model itself must hold no parameters or buffers")
-    _check_stem_cifar(model)
-    if model.conv1.out_channels != 64:
-        raise TypeError("FrozenResNetTeacher: the CIFAR ResNet-18 stem must have 64 outputs")
+    _check_stem(model, fam)
     if type(model.avgpool) is not nn.AdaptiveAvgPool2d or type(model.fc) is not nn.Linear:
         raise TypeError("FrozenResNetTeacher: the head must be nn.AdaptiveAvgPool2d and nn.Linear")
     out = []
-    for li in range(1, 5):
-        layer = getattr(model, f"layer{li}")
+    for lname in (n for n in fam.children if n in _LAYERS):
+        layer = getattr(model, lname)
         if type(layer) is not nn.Sequential:
-            raise TypeError(f"FrozenResNetTeacher: layer{li} must be nn.Sequential")
+            raise TypeError(f"FrozenResNetTeacher: {lname} must be nn.Sequential")
         for bi, blk in layer.named_children():
-            where = f"layer{li}.{bi}"
-            if type(blk) is not BasicBlock:
-                raise TypeError(f"FrozenResNetTeacher: {where} is a {type(blk).__name__}; only the Bi-Real "
-                                "bdbnn_b200.resnet.BasicBlock is supported")
-            if [n for n, _ in blk.named_children()] != ["conv1", "bn1", "conv2", "bn2"] + (
+            where = f"{lname}.{bi}"
+            if type(blk) is not fam.block:
+                raise TypeError(f"FrozenResNetTeacher: {where} is a {type(blk).__name__}; only "
+                                f"{fam.block.__module__}.{fam.block.__name__} is supported")
+            # the Bi-Real BasicBlock has no other child (a `relu`, say, would never run on the kernel path)
+            if fam is _CIFAR18 and [n for n, _ in blk.named_children()] != ["conv1", "bn1", "conv2", "bn2"] + (
                     ["downsample"] if blk.downsample is not None else []):
                 raise TypeError(f"FrozenResNetTeacher: {where} has unexpected children")
             _check_conv(blk.conv1, where + ".conv1", 3)
             _check_conv(blk.conv2, where + ".conv2", 3)
             if blk.conv2.stride != (1, 1) or blk.conv1.padding != (1, 1) or blk.conv2.padding != (1, 1):
-                raise TypeError(f"FrozenResNetTeacher: {where} convs are not the BasicBlock's")
+                raise TypeError(f"FrozenResNetTeacher: {where} convs are not the {fam.block.__name__}'s")
             _check_bn(blk.bn1, where + ".bn1")
             _check_bn(blk.bn2, where + ".bn2")
-            ds = blk.downsample
-            cin, cout = blk.conv1.in_channels, blk.conv1.out_channels
-            if ds is None:
-                if blk.conv1.stride != (1, 1) or cin != cout:
-                    raise TypeError(f"FrozenResNetTeacher: {where} changes shape but has no downsample")
-            else:
-                if type(ds) is not nn.Sequential or len(ds) != 2:
-                    raise TypeError(f"FrozenResNetTeacher: {where}.downsample must be Sequential(1x1 Conv2d, "
-                                    "BatchNorm2d)")
-                _check_conv(ds[0], where + ".downsample.0", 1)
-                if ds[0].padding != (0, 0) or ds[0].stride != blk.conv1.stride or ds[0].in_channels != cin or \
-                        ds[0].out_channels != cout:
-                    raise TypeError(f"FrozenResNetTeacher: {where}.downsample.0 must map conv1's input to its output "
-                                    "shape with no padding")
-                _check_bn(ds[1], where + ".downsample.1")
-            out.append((where, blk))
-    return out
-
-
-def _blocks(model):
-    """[(name, block)] of the residual blocks after checking that `model` is a torchvision BasicBlock ResNet, an
-    fp32 ResNetCifar (_cifar_blocks) or an fp32 ResNetCifar18 (_cifar18_blocks)."""
-    from .resnet import ResNetCifar, ResNetCifar18
-    if type(model) is ResNetCifar:
-        return _cifar_blocks(model)
-    if type(model) is ResNetCifar18:
-        return _cifar18_blocks(model)
-    from torchvision.models.resnet import BasicBlock, ResNet
-    if type(model) is not ResNet:
-        raise TypeError(f"FrozenResNetTeacher wraps a torchvision ResNet with BasicBlocks (resnet18/34) or an fp32 "
-                        f"bdbnn_b200.resnet.ResNetCifar, got {type(model).__name__}")
-    names = [n for n, _ in model.named_children()]
-    if names != ["conv1", "bn1", "relu", "maxpool", "layer1", "layer2", "layer3", "layer4", "avgpool", "fc"]:
-        raise TypeError(f"FrozenResNetTeacher: unexpected children {names}")
-    if list(model.named_parameters(recurse=False)) or list(model.named_buffers(recurse=False)):
-        raise TypeError("FrozenResNetTeacher: the model itself must hold no parameters or buffers")
-    _check_conv(model.conv1, "conv1", 7)
-    if model.conv1.stride != (2, 2) or model.conv1.padding != (3, 3) or model.conv1.in_channels != 3:
-        raise TypeError("FrozenResNetTeacher: conv1 must be the 7x7 / stride-2 / pad-3 stem on 3 channels")
-    _check_bn(model.bn1, "bn1")
-    mp = model.maxpool
-    if type(model.relu) is not nn.ReLU or type(mp) is not nn.MaxPool2d or mp.ceil_mode or mp.dilation != 1 \
-            or mp.return_indices:
-        raise TypeError("FrozenResNetTeacher: the stem must end in nn.ReLU and nn.MaxPool2d")
-    if type(model.avgpool) is not nn.AdaptiveAvgPool2d or type(model.fc) is not nn.Linear:
-        raise TypeError("FrozenResNetTeacher: the head must be nn.AdaptiveAvgPool2d and nn.Linear")
-    out = []
-    for li in range(1, 5):
-        layer = getattr(model, f"layer{li}")
-        if type(layer) is not nn.Sequential:
-            raise TypeError(f"FrozenResNetTeacher: layer{li} must be nn.Sequential")
-        for bi, blk in layer.named_children():
-            where = f"layer{li}.{bi}"
-            if type(blk) is not BasicBlock:
-                raise TypeError(f"FrozenResNetTeacher: {where} is a {type(blk).__name__}; only torchvision BasicBlock "
-                                "is supported")
-            _check_conv(blk.conv1, where + ".conv1", 3)
-            _check_conv(blk.conv2, where + ".conv2", 3)
-            if blk.conv2.stride != (1, 1) or blk.conv1.padding != (1, 1) or blk.conv2.padding != (1, 1):
-                raise TypeError(f"FrozenResNetTeacher: {where} convs are not the BasicBlock's")
-            _check_bn(blk.bn1, where + ".bn1")
-            _check_bn(blk.bn2, where + ".bn2")
-            if type(blk.relu) is not nn.ReLU:
+            if fam.relu and type(blk.relu) is not nn.ReLU:
                 raise TypeError(f"FrozenResNetTeacher: {where}.relu must be nn.ReLU")
-            ds = blk.downsample
-            if ds is not None:
-                if type(ds) is not nn.Sequential or len(ds) != 2:
-                    raise TypeError(f"FrozenResNetTeacher: {where}.downsample must be Sequential(1x1 Conv2d, "
-                                    "BatchNorm2d)")
-                _check_conv(ds[0], where + ".downsample.0", 1)
-                if ds[0].padding != (0, 0):
-                    raise TypeError(f"FrozenResNetTeacher: {where}.downsample.0 must have no padding")
-                _check_bn(ds[1], where + ".downsample.1")
+            _check_shortcut(blk, where, fam)
             out.append((where, blk))
-    return out
+    return fam, out
 
 
 class FrozenResNetTeacher(nn.Module):
@@ -208,10 +171,8 @@ class FrozenResNetTeacher(nn.Module):
 
     def __init__(self, model):
         super().__init__()
-        blocks = _blocks(model)
-        from .resnet import ResNetCifar, ResNetCifar18
-        self.__dict__["_cifar"] = type(model) is ResNetCifar
-        self.__dict__["_cifar18"] = type(model) is ResNetCifar18
+        family, blocks = _blocks(model)
+        self.__dict__["_family"] = family
         self.__dict__["_wrapped"] = model      # not a submodule: no "_wrapped." prefix in the names
         for name, child in model.named_children():
             self.add_module(name, child)
@@ -222,8 +183,16 @@ class FrozenResNetTeacher(nn.Module):
 
     @property
     def wrapped(self):
-        """The torchvision model this teacher runs."""
+        """The model this teacher runs."""
         return self._wrapped
+
+    @property
+    def _cifar(self):
+        return self._family is _CIFAR
+
+    @property
+    def _cifar18(self):
+        return self._family is _CIFAR18
 
     def train(self, mode=True):
         super().train(mode)
@@ -247,31 +216,31 @@ class FrozenResNetTeacher(nn.Module):
         return tuple(out)
 
     def _geometry_supported(self, x):
-        """Every conv of the network has the wgmma forward at this input size (host-only checks, cached)."""
-        if self._cifar or self._cifar18:
-            return self._cifar_geometry_supported(x)
-        pool = self._pool_args()
+        """The stem, every 3x3 conv and every shortcut of the network have their kernel at this input size (host-only
+        checks, cached).  The max-pool's arguments are part of the key: they are read at every forward, so a
+        `maxpool` assigned after wrapping is seen."""
+        pool = self._pool_args() if self._family.pooled_stem else ()
         if pool is None:
             return False
         key = (x.device, tuple(x.shape), pool)
         ok = self._geom_ok.get(key)
-        if ok is not None:
-            return ok
-        n, _, h, w = x.shape
-        ok = F_.stem_conv_supported(x, self.conv1.weight, self.conv1.stride, self.conv1.padding)
-        k, s, p = pool
-        ho, wo = (h - 1) // 2 + 1, (w - 1) // 2 + 1
-        ok = ok and self._basic_blocks_supported((n, 64, (ho + 2 * p - k) // s + 1, (wo + 2 * p - k) // s + 1))
-        self._geom_ok[key] = ok
+        if ok is None:
+            ok = self._geom_ok[key] = self._walk_geometry(x, pool)
         return ok
 
-    def _basic_blocks_supported(self, shape):
-        """Every 3x3 conv and every `downsample` GEMM of the BasicBlocks has the wgmma forward for an input of
-        `shape` to the first block."""
+    def _walk_geometry(self, x, pool):
+        fam, c1 = self._family, self.conv1
+        n, _, h, w = x.shape
+        if fam.pooled_stem:
+            ok = F_.stem_conv_supported(x, c1.weight, c1.stride, c1.padding)
+            k, s, p = pool
+            ho, wo = (h - 1) // 2 + 1, (w - 1) // 2 + 1
+            shape = (n, 64, (ho + 2 * p - k) // s + 1, (wo + 2 * p - k) // s + 1)
+        else:
+            ok = F_.cifar_stem_supported(tuple(x.shape), tuple(c1.weight.shape), c1.stride, c1.padding)
+            shape = (n, c1.out_channels, h, w)
         L = _lib.lib()
         fwd_ok = lambda sh: sh.Cin % 4 == 0 and bool(int(L.bdbnn_tc_supported(ctypes.byref(sh))) & 1)
-        n = shape[0]
-        ok = True
         for blk in self._blocks:
             if not ok:
                 break
@@ -280,40 +249,15 @@ class FrozenResNetTeacher(nn.Module):
                 sh = F_.conv_shape(shape, conv.weight.shape, conv.stride[0], conv.padding[0])
                 ok = ok and fwd_ok(sh)
                 shape = (n, sh.Cout, sh.Ho, sh.Wo)
-            if blk.downsample is not None:       # the 1x1 GEMM over the strided samples (shortcut_eval_supported)
-                ds = blk.downsample[0]
-                sd = ds.stride[0]
+            sc = getattr(blk, fam.shortcut)
+            if sc is None:
+                continue
+            if fam.shortcut == "shortcut":       # the option-A residual of conv1, read in place
+                ok = ok and F_.pad_shortcut_supported(x_shape, blk.conv1.weight.shape, blk.conv1.stride[0], sc.pad)
+            else:                                # the 1x1 GEMM over the strided samples (shortcut_eval_supported)
+                sd = sc[0].stride[0]
                 sampled = (n, x_shape[1], (x_shape[2] - 1) // sd + 1, (x_shape[3] - 1) // sd + 1)
-                ok = ok and fwd_ok(F_.conv_shape(sampled, ds.weight.shape, 1, 0))
-        return ok
-
-    def _cifar_geometry_supported(self, x):
-        key = (x.device, tuple(x.shape))
-        ok = self._geom_ok.get(key)
-        if ok is not None:
-            return ok
-        if self._cifar18:
-            c1 = self.conv1
-            ok = (F_.cifar_stem_supported(tuple(x.shape), tuple(c1.weight.shape), c1.stride, c1.padding) and
-                  self._basic_blocks_supported((x.shape[0], c1.out_channels, x.shape[2], x.shape[3])))
-            self._geom_ok[key] = ok
-            return ok
-        L = _lib.lib()
-        fwd_ok = lambda sh: sh.Cin % 4 == 0 and bool(int(L.bdbnn_tc_supported(ctypes.byref(sh))) & 1)
-        c1 = self.conv1
-        ok = F_.cifar_stem_supported(tuple(x.shape), tuple(c1.weight.shape), c1.stride, c1.padding)
-        n, _, h, w = x.shape
-        shape = (n, c1.out_channels, h, w)
-        for blk in self._blocks:
-            if not ok:
-                break
-            if blk.shortcut is not None:     # the option-A residual of conv1, read in place
-                ok = F_.pad_shortcut_supported(shape, blk.conv1.weight.shape, blk.conv1.stride[0], blk.shortcut.pad)
-            for conv in (blk.conv1, blk.conv2):
-                sh = F_.conv_shape(shape, conv.weight.shape, conv.stride[0], conv.padding[0])
-                ok = ok and fwd_ok(sh)
-                shape = (n, sh.Cout, sh.Ho, sh.Wo)
-        self._geom_ok[key] = ok
+                ok = ok and fwd_ok(F_.conv_shape(sampled, sc[0].weight.shape, 1, 0))
         return ok
 
     def kernel_path(self, x):
@@ -340,62 +284,26 @@ class FrozenResNetTeacher(nn.Module):
             return self._kernel_forward(x)
 
     def _kernel_forward(self, x):
-        if self._cifar:
-            return self._cifar_kernel_forward(x)
-        if self._cifar18:
-            return self._cifar18_kernel_forward(x)
-        bn = self.bn1
-        z, z_amax = F_.stem_conv_bn_relu_pool_eval(x, self.conv1.weight, bn.weight, bn.bias, bn.running_mean,
-                                                   bn.running_var, bn.eps, *self._pool_args())
+        fam = self._family
+        if fam.pooled_stem:
+            z, z_amax = F_.stem_conv_bn_relu_pool_eval(x, self.conv1.weight, *_bn_args(self.bn1), *self._pool_args())
+        else:
+            z, z_amax = F_.cifar_stem_conv_bn_eval(x, self.conv1.weight, *_bn_args(self.bn1))
         # packed at every forward, never cached: a load_state_dict or an in-place update is always seen
         packs = F_.real_weight_pack([c.weight for c in self._convs])
         for i, blk in enumerate(self._blocks):
-            identity = z
-            if blk.downsample is not None:
-                ds, dbn = blk.downsample
-                identity = F_._shortcut_eval_impl(z, ds.weight, dbn.weight, dbn.bias, dbn.running_mean,
-                                                  dbn.running_var, dbn.eps, ds.stride[0])
-            b1, b2 = blk.bn1, blk.bn2
-            y, y_amax = F_.real_conv_bn_eval(z, z_amax, packs[2 * i], b1.weight, b1.bias, b1.running_mean,
-                                             b1.running_var, b1.eps, blk.conv1.stride[0], blk.conv1.padding[0])
-            z, z_amax = F_.real_conv_bn_eval(y, y_amax, packs[2 * i + 1], b2.weight, b2.bias, b2.running_mean,
-                                             b2.running_var, b2.eps, 1, 1, residual=identity)
-        return self.fc(torch.flatten(self.avgpool(z), 1))
-
-    def _cifar_kernel_forward(self, x):
-        # BasicBlockCifar: out = bn1(conv1(x)) + shortcut(x); out2 = bn2(conv2(out)) + out; no ReLU anywhere
-        bn = self.bn1
-        z, z_amax = F_.cifar_stem_conv_bn_eval(x, self.conv1.weight, bn.weight, bn.bias, bn.running_mean,
-                                               bn.running_var, bn.eps)
-        packs = F_.real_weight_pack([c.weight for c in self._convs])
-        for i, blk in enumerate(self._blocks):
-            b1, b2 = blk.bn1, blk.bn2
-            res = dict(residual=z) if blk.shortcut is None else dict(shortcut=F_.PadShortcut(blk.shortcut.pad))
-            y, y_amax = F_.real_conv_bn_eval(z, z_amax, packs[2 * i], b1.weight, b1.bias, b1.running_mean,
-                                             b1.running_var, b1.eps, blk.conv1.stride[0], blk.conv1.padding[0],
-                                             relu=False, **res)
-            z, z_amax = F_.real_conv_bn_eval(y, y_amax, packs[2 * i + 1], b2.weight, b2.bias, b2.running_mean,
-                                             b2.running_var, b2.eps, 1, 1, residual=y, relu=False)
-        return self.fc(torch.flatten(self.avgpool(z), 1))
-
-    def _cifar18_kernel_forward(self, x):
-        # Bi-Real BasicBlock: out = bn1(conv1(x)) + downsample(x) (or x); out2 = bn2(conv2(out)) + out; no ReLU
-        bn = self.bn1
-        z, z_amax = F_.cifar_stem_conv_bn_eval(x, self.conv1.weight, bn.weight, bn.bias, bn.running_mean,
-                                               bn.running_var, bn.eps)
-        packs = F_.real_weight_pack([c.weight for c in self._convs])
-        for i, blk in enumerate(self._blocks):
-            identity = z
-            if blk.downsample is not None:
-                ds, dbn = blk.downsample
-                identity = F_._shortcut_eval_impl(z, ds.weight, dbn.weight, dbn.bias, dbn.running_mean,
-                                                  dbn.running_var, dbn.eps, ds.stride[0])
-            b1, b2 = blk.bn1, blk.bn2
-            y, y_amax = F_.real_conv_bn_eval(z, z_amax, packs[2 * i], b1.weight, b1.bias, b1.running_mean,
-                                             b1.running_var, b1.eps, blk.conv1.stride[0], blk.conv1.padding[0],
-                                             residual=identity, relu=False)
-            z, z_amax = F_.real_conv_bn_eval(y, y_amax, packs[2 * i + 1], b2.weight, b2.bias, b2.running_mean,
-                                             b2.running_var, b2.eps, 1, 1, residual=y, relu=False)
+            sc = getattr(blk, fam.shortcut)
+            if sc is None:
+                res = dict(residual=z)
+            elif fam.shortcut == "shortcut":
+                res = dict(shortcut=F_.PadShortcut(sc.pad))
+            else:
+                res = dict(residual=F_._shortcut_eval_impl(z, sc[0].weight, *_bn_args(sc[1]), sc[0].stride[0]))
+            # the shortcut is conv1's residual and conv1's output is conv2's on a Bi-Real block, else it is conv2's
+            y, y_amax = F_.real_conv_bn_eval(z, z_amax, packs[2 * i], *_bn_args(blk.bn1), blk.conv1.stride[0],
+                                             blk.conv1.padding[0], relu=fam.relu, **(res if fam.bireal else {}))
+            z, z_amax = F_.real_conv_bn_eval(y, y_amax, packs[2 * i + 1], *_bn_args(blk.bn2), 1, 1, relu=fam.relu,
+                                             **(dict(residual=y) if fam.bireal else res))
         return self.fc(torch.flatten(self.avgpool(z), 1))
 
 
@@ -407,12 +315,8 @@ def launches_per_forward(model):
       CIFAR ResNet (DESIGN.md §4j): 2 for the stem (fold, conv); the option-A shortcuts launch nothing;
       CIFAR ResNet-18 (DESIGN.md §4k): 2 for the stem (fold, conv) and 6 per `downsample`."""
     m = model.wrapped if isinstance(model, FrozenResNetTeacher) else model
-    cifar = [b for b in m.modules() if type(b).__name__ == "BasicBlockCifar"]
-    if cifar:
-        n3 = 2 * len(cifar)
-        return 2 * ((n3 + 47) // 48) + 2 + 3 * n3
-    blocks = [b for b in m.modules() if type(b).__name__ == "BasicBlock"]
+    fam = _family(m)
+    blocks = [b for b in m.modules() if type(b) is fam.block]
     n3 = 2 * len(blocks)
-    n_ds = sum(1 for b in blocks if b.downsample is not None)
-    stem = 2 if type(m).__name__ == "ResNetCifar18" else 6
-    return 2 * ((n3 + 47) // 48) + stem + 3 * n3 + 6 * n_ds
+    n_ds = sum(1 for b in blocks if b.downsample is not None) if fam.shortcut == "downsample" else 0
+    return 2 * ((n3 + 47) // 48) + (6 if fam.pooled_stem else 2) + 3 * n3 + 6 * n_ds

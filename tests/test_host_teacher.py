@@ -75,10 +75,48 @@ def test_unsupported_structures_raise_type_error():
         FrozenResNetTeacher(torchvision.models.resnet50())
     with pytest.raises(TypeError):
         FrozenResNetTeacher(nn.DataParallel(torchvision.models.resnet18()))
-    m = torchvision.models.resnet18()
-    m.layer2[0].conv1 = nn.Conv2d(64, 128, 5, 2, 2, bias=False)
+
+    class Sub(torchvision.models.ResNet):
+        pass
     with pytest.raises(TypeError):
+        FrozenResNetTeacher(Sub(torchvision.models.resnet.BasicBlock, [2, 2, 2, 2]))
+
+    def ds(*extra, padding=0):
+        return nn.Sequential(nn.Conv2d(64, 128, 1, 2, padding, bias=False), nn.BatchNorm2d(128), *extra)
+    edits = [lambda m: setattr(m.layer2[0], "conv1", nn.Conv2d(64, 128, 5, 2, 2, bias=False)),     # a 5x5 conv
+             lambda m: setattr(m, "relu", nn.ReLU6()),
+             lambda m: setattr(m, "relu", nn.Identity()),
+             lambda m: setattr(m.layer3[1], "relu", nn.ReLU6()),
+             lambda m: setattr(m.layer1[0], "relu", nn.Identity()),
+             lambda m: setattr(m, "maxpool", nn.MaxPool2d(3, 2, 1, ceil_mode=True)),
+             lambda m: setattr(m.layer2[0], "downsample", ds(nn.Identity())),                       # of length 3
+             lambda m: setattr(m.layer2[0], "downsample", ds(padding=1)),
+             lambda m: setattr(m.layer4[1], "bn1", nn.SyncBatchNorm(512)),
+             lambda m: setattr(m.layer2[0].downsample, "1", nn.SyncBatchNorm(128)),
+             lambda m: setattr(m, "conv1", nn.Conv2d(3, 64, 7, 2, 3, bias=True)),
+             lambda m: delattr(m, "avgpool"),                                                       # a missing child
+             lambda m: m.register_parameter("scale", nn.Parameter(torch.ones(1))),
+             lambda m: m.register_buffer("steps", torch.zeros(1))]
+    for i, edit in enumerate(edits):
+        m = torchvision.models.resnet18()
         FrozenResNetTeacher(m)
+        edit(m)
+        with pytest.raises(TypeError):
+            FrozenResNetTeacher(m)
+            pytest.fail(f"edit {i} was accepted")
+
+
+def test_a_torchvision_downsample_is_not_compared_with_conv1():
+    """The wrapper asks that a torchvision `downsample` is Sequential(bias-free unpadded 1x1 nn.Conv2d, BatchNorm2d);
+    unlike for this package's own BasicBlock, not that it maps conv1's input to conv1's output shape, nor that a
+    block without one keeps its shape."""
+    from bdbnn_b200 import FrozenResNetTeacher
+    m = torchvision.models.resnet18()
+    m.layer2[0].downsample[0] = nn.Conv2d(64, 128, 1, 1, bias=False)         # stride 1 beside a stride-2 conv1
+    assert len(FrozenResNetTeacher(m)._blocks) == 8
+    m = torchvision.models.resnet18()
+    m.layer3[0].downsample = None
+    assert len(FrozenResNetTeacher(m)._blocks) == 8
 
 
 def test_wrapping_the_module_of_a_data_parallel_keeps_its_names():
@@ -111,9 +149,11 @@ def test_load_state_dict_round_trips():
 
 
 def test_launch_formula():
+    from bdbnn_b200 import FrozenResNetTeacher
     from bdbnn_b200.teacher import launches_per_forward
     assert launches_per_forward(torchvision.models.resnet18()) == 2 + 6 + 3 * 16 + 6 * 3
     assert launches_per_forward(torchvision.models.resnet34()) == 2 + 6 + 3 * 32 + 6 * 3
+    assert launches_per_forward(FrozenResNetTeacher(torchvision.models.resnet18())) == 2 + 6 + 3 * 16 + 6 * 3
 
 
 def test_pool_arguments_are_normalised_or_rejected():
