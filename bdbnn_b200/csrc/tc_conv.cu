@@ -11,8 +11,11 @@
 //                   [BNI images][BH rows][BW=OW cols][KB channels] at coordinates shifted by the tap —
 //                   TMA zero-fills out-of-image coordinates, which IS the conv's zero padding — and the
 //                   matching [BN x KB] weight box, into a `stages`-deep ring of swizzled K-major tiles.
-//   warpgroups 0/1: wgmma (fp32 accumulate in registers) for tile rows [0, 64) / [64, 128), one wgmma group in
-//                   flight: a ring slot is released once the group after it was issued and the one reading it retired.
+//   warpgroups 0/1: wgmma (fp32 accumulate in registers) for tile rows [0, 64) / [64, 128): per ring slot one wgmma
+//                   as wide as the N tile for every 32 bytes of the K rows, an unbroken chain (the kernel is
+//                   instantiated per N width, so the A tile is read from shared memory once per K step).  One wgmma
+//                   group in flight: a ring slot is released once the group after it was issued and the one reading
+//                   it retired.
 //                   Then the epilogue from the same registers: alpha or STE mask, optional int16 result, additive
 //                   tensor, and the per-channel BatchNorm statistics of the result (forward: sum y, sum y^2,
 //                   max|y|; dgrad: the backward sums of the BatchNorm unit that produced the conv input).
@@ -59,11 +62,22 @@ struct TcConvParams {
   int32_t res_H, res_W, res_C, res_coff;
 };
 
-// MODE: 0 forward, 1 dgrad, 2 eval forward; KIND: 0 fp16, 1 bf16, 2 fp8 e4m3 operands; NW: wgmma N (16, 32, or 64
-// with BN/64 chunks).
+// One K block of a ring slot: KS wgmmas back to back, each over 32 bytes of every row (row_bytes = 32 * KS).  KS and
+// the N width are compile-time, so nothing stands between the wgmmas of a group: ptxas keeps the accumulator in place
+// and issues them as one uninterrupted chain.
+template <int NW, int KIND, int KS>
+__device__ __forceinline__ void wgmma_k_block(float (&acc)[NW / 2], uint32_t a_src, uint32_t b_src) {
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < KS; ++k)
+    wgmma_ss<NW, KIND>(acc, make_kmajor_desc(a_src + k * 32, 32 * KS), make_kmajor_desc(b_src + k * 32, 32 * KS));
+}
+
+// MODE: 0 forward, 1 dgrad, 2 eval forward; KIND: 0 fp16, 1 bf16, 2 fp8 e4m3 operands; NW: the N tile (BN = 16, 32,
+// 64 or 128), one wgmma wide.
 // Two CTAs per SM need <= 96 registers per thread: registers are allocated per warp inside each of the SM's four
 // 16K-register sub-partitions, and 2 x 9 warps put five warps on two of them.  The dgrad and eval instances ask for
-// that bound (without it the NW = 64 dgrad ones took 102 registers and ran one CTA per SM); the forward ones fit at
+// that bound (without it the 128-column dgrad ones took 102 registers and ran one CTA per SM); the forward ones fit at
 // 96 without it (0 = no minimum).  bdbnn_debug_tc_conv_ctas_per_sm reports the residency.
 // PADRES (MODE 2, 16-bit operands only): the residual is the CIFAR option-A shortcut read in place (res_* fields),
 // an instance of its own so that the dense-residual instances keep their code.
@@ -71,7 +85,6 @@ template <int MODE, int KIND, int NW, bool PADRES = false>
 __global__ void __launch_bounds__(kTcThreads, MODE == 0 ? 0 : 2)
 tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const TcConvParams p) {
-  constexpr int NCH = NW == 64 ? kMaxBN / 64 : 1;
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[kMaxStages];
   __shared__ __align__(8) uint64_t empty_bar[kMaxStages];
@@ -140,26 +153,17 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     }
   } else {
     const int wg = warp >> 2, wq = warp & 3;
-    const int nch = p.BN / NW;
-    float acc[NCH][NW / 2];
+    float acc[NW / 2];
 #pragma unroll
-    for (int c = 0; c < NCH; ++c)
-#pragma unroll
-      for (int i = 0; i < NW / 2; ++i) acc[c][i] = 0.f;
-    const int k_steps = p.row_bytes / 32;          // one wgmma consumes 32 bytes of every row
+    for (int i = 0; i < NW / 2; ++i) acc[i] = 0.f;
     for (int it = 0; it < n_iters; ++it) {
       const int stage = it % p.stages;
       mbar_wait(smem_u32(&full_bar[stage]), uint32_t(it / p.stages) & 1u);
       const uint32_t a_src = tiles_base + stage * stage_bytes + uint32_t(wg * 64 * p.row_bytes);
       const uint32_t b_src = tiles_base + stage * stage_bytes + a_bytes;
-      wgmma_fence();
-      for (int k = 0; k < k_steps; ++k) {
-        const uint64_t ad = make_kmajor_desc(a_src + k * 32, p.row_bytes);
-#pragma unroll
-        for (int c = 0; c < NCH; ++c)
-          if (c < nch)
-            wgmma_ss<NW, KIND>(acc[c], ad, make_kmajor_desc(b_src + uint32_t(c * NW * p.row_bytes) + k * 32, p.row_bytes));
-      }
+      if (p.row_bytes == 128) wgmma_k_block<NW, KIND, 4>(acc, a_src, b_src);
+      else if (p.row_bytes == 64) wgmma_k_block<NW, KIND, 2>(acc, a_src, b_src);
+      else wgmma_k_block<NW, KIND, 1>(acc, a_src, b_src);
       wgmma_commit();
       wgmma_wait<1>();
       if (it > 0 && (threadIdx.x & 127) == 0) {
@@ -170,14 +174,14 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
     }
     wgmma_wait<0>();
-#pragma unroll
-    for (int c = 0; c < NCH; ++c) wgmma_fence_regs(acc[c]);
+    wgmma_fence_regs(acc);
 
     // ---- epilogue: this thread holds rows r and r + 8 (r = 64 wg + 16 wq + lane/4), column pairs 8j + 2(lane%4) ----
     const float post = (MODE != 0 && p.amax_bits) ? amax_pow2_scale(__ldg(p.amax_bits), true) : 1.0f;
     uint32_t zmax = 0u;                     // MODE 2: bits of this thread's max|z| (ordered as integers, NaN on top)
     const int mask_words = (p.Nout + 31) >> 5;
-    int64_t pix[2], rpix[2];                // rpix: PADRES residual pixel
+    int64_t pix[2];
+    int32_t rpix[2];                        // PADRES residual pixel (32 bits, plan_tc_conv checks: keeps 96 registers)
     bool valid[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -188,113 +192,110 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       const int oh = (h0 + hi) * p.out_step + p.out_off_h, ow = wi * p.out_step + p.out_off_w;
       valid[h] = (ni < p.BNI) && (h0 + hi < p.OH) && (n0 + ni < p.NIMG) && oh < p.OHf && ow < p.OWf;
       pix[h] = (int64_t(n0 + ni) * p.OHf + oh) * p.OWf + ow;
-      if (PADRES) rpix[h] = (int64_t(n0 + ni) * p.res_H + 2 * oh) * p.res_W + 2 * ow;
+      if (PADRES) rpix[h] = ((n0 + ni) * p.res_H + 2 * oh) * p.res_W + 2 * ow;
     }
 #pragma unroll
-    for (int c = 0; c < NCH; ++c) {
-      if (c >= nch) break;
+    for (int j = 0; j < NW / 8; ++j) {
       // dgrad: `add` may alias `out`, so each pair's load of `add` waits for the previous pair's store.  Prefetching
-      // the chunk's `add` lines into L2 first turns that chain of HBM round trips into L2 hits (no registers held).
-      if (MODE == 1 && p.add != nullptr) {
+      // the next 64 columns' `add` lines into L2 first turns that chain of HBM round trips into L2 hits (no
+      // registers held).
+      if (MODE == 1 && j % 8 == 0 && p.add != nullptr) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           if (!valid[h]) continue;
-          const float* row = p.add + pix[h] * p.Nout + nn0 + c * NW;
+          const float* row = p.add + pix[h] * p.Nout + nn0 + 8 * j;
 #pragma unroll
-          for (int f = 0; f < NW; f += 32) asm volatile("prefetch.global.L2 [%0];" ::"l"(row + f));
+          for (int f = 0; f < (NW < 64 ? NW : 64); f += 32) asm volatile("prefetch.global.L2 [%0];" ::"l"(row + f));
         }
       }
+      const int col = 8 * j + 2 * (lane & 3);
+      const int ch = nn0 + col;
+      float a0 = 1.f, a1 = 1.f, sa0 = 0.f, sa1 = 0.f, sb0 = 0.f, sb1 = 0.f;
+      if (MODE != 1) {
+        a0 = __ldg(p.alpha + ch); a1 = __ldg(p.alpha + ch + 1);
+        if (MODE == 2) { sb0 = __ldg(p.shift + ch); sb1 = __ldg(p.shift + ch + 1); }
+      } else if (do_stats) {               // yhat = y_int * alpha * invstd - mean * invstd of the producing unit
+        const float is0 = __ldg(p.st_invstd + ch), is1 = __ldg(p.st_invstd + ch + 1);
+        sa0 = __ldg(p.st_alpha + ch) * is0; sa1 = __ldg(p.st_alpha + ch + 1) * is1;
+        sb0 = __ldg(p.st_mean + ch) * is0; sb1 = __ldg(p.st_mean + ch + 1) * is1;
+      }
+      float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f, m0 = 0.f, m1 = 0.f;
 #pragma unroll
-      for (int j = 0; j < NW / 8; ++j) {
-        const int col = c * NW + 8 * j + 2 * (lane & 3);
-        const int ch = nn0 + col;
-        float a0 = 1.f, a1 = 1.f, sa0 = 0.f, sa1 = 0.f, sb0 = 0.f, sb1 = 0.f;
-        if (MODE != 1) {
-          a0 = __ldg(p.alpha + ch); a1 = __ldg(p.alpha + ch + 1);
-          if (MODE == 2) { sb0 = __ldg(p.shift + ch); sb1 = __ldg(p.shift + ch + 1); }
-        } else if (do_stats) {               // yhat = y_int * alpha * invstd - mean * invstd of the producing unit
-          const float is0 = __ldg(p.st_invstd + ch), is1 = __ldg(p.st_invstd + ch + 1);
-          sa0 = __ldg(p.st_alpha + ch) * is0; sa1 = __ldg(p.st_alpha + ch + 1) * is1;
-          sb0 = __ldg(p.st_mean + ch) * is0; sb1 = __ldg(p.st_mean + ch + 1) * is1;
-        }
-        float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f, m0 = 0.f, m1 = 0.f;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          if (!valid[h]) continue;
-          const float v0 = acc[c][4 * j + 2 * h], v1 = acc[c][4 * j + 2 * h + 1];
-          const int64_t off = pix[h] * p.Nout + ch;
-          float o0, o1;
-          if (MODE == 0) {
-            o0 = v0 * a0; o1 = v1 * a1;
-            if (p.out_i16 != nullptr)        // exact: |v| <= taps * Kc <= 32767
-              *reinterpret_cast<uint32_t*>(p.out_i16 + off) = (uint32_t(int(v0)) & 0xffffu) | (uint32_t(int(v1)) << 16);
-            else
-              *reinterpret_cast<float2*>(p.out + off) = make_float2(o0, o1);
-          } else if (MODE == 2) {
-            // one rounding per step, no FMA contraction: the CPU reference (oracle/eval_ref.py) matches bit for bit.
-            // post = 2^-ex of real-valued operands (exact), 1 for the +-1 operands.
-            o0 = __fadd_rn(__fmul_rn(__fmul_rn(v0, post), a0), sb0);
-            o1 = __fadd_rn(__fmul_rn(__fmul_rn(v1, post), a1), sb1);
-            if (PADRES) {
-              // outside the channel band the residual is +0.0 and is still added: -0.0 + 0.0 = +0.0, as the
-              // materialised zero-padded tensor gives (ch and the band edges are even, so a pair is in or out)
-              float2 r = make_float2(0.f, 0.f);
-              const int rc = ch - p.res_coff;
-              if (unsigned(rc) < unsigned(p.res_C))
-                r = __ldg(reinterpret_cast<const float2*>(p.add + rpix[h] * p.res_C + rc));
-              o0 = __fadd_rn(o0, r.x); o1 = __fadd_rn(o1, r.y);
-            } else if (p.add != nullptr) {   // the residual never aliases z (the entry points reject it)
-              const float2 r = __ldg(reinterpret_cast<const float2*>(p.add + off));
-              o0 = __fadd_rn(o0, r.x); o1 = __fadd_rn(o1, r.y);
-            }
-            if (p.relu) {                    // torch.relu: NaN stays NaN (fmaxf alone would drop it)
-              o0 = o0 != o0 ? o0 : fmaxf(o0, 0.f);
-              o1 = o1 != o1 ? o1 : fmaxf(o1, 0.f);
-            }
+      for (int h = 0; h < 2; ++h) {
+        if (!valid[h]) continue;
+        const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+        const int64_t off = pix[h] * p.Nout + ch;
+        float o0, o1;
+        if (MODE == 0) {
+          o0 = v0 * a0; o1 = v1 * a1;
+          if (p.out_i16 != nullptr)        // exact: |v| <= taps * Kc <= 32767
+            *reinterpret_cast<uint32_t*>(p.out_i16 + off) = (uint32_t(int(v0)) & 0xffffu) | (uint32_t(int(v1)) << 16);
+          else
             *reinterpret_cast<float2*>(p.out + off) = make_float2(o0, o1);
-            zmax = max(zmax, max(__float_as_uint(fabsf(o0)), __float_as_uint(fabsf(o1))));
-            // sign(v) = +1 iff v >= 0 (DESIGN.md §2): -0.0 -> +1, NaN -> -1
-            if (p.zb != nullptr)
-              *reinterpret_cast<uint32_t*>(p.zb + off) =
-                  (o0 >= 0.f ? p.zb_one : p.zb_one | 0x8000u) | ((o1 >= 0.f ? p.zb_one : p.zb_one | 0x8000u) << 16);
-            if (p.zb8 != nullptr)
-              *reinterpret_cast<uint16_t*>(p.zb8 + off) = uint16_t((o0 >= 0.f ? 0x38u : 0xB8u) |
-                                                                   ((o1 >= 0.f ? 0x38u : 0xB8u) << 8));
-          } else {
-            const uint32_t word = __ldg(p.mask + pix[h] * mask_words + (ch >> 5)) >> (ch & 31);
-            o0 = (word & 1u) ? v0 * post : 0.0f;
-            o1 = (word & 2u) ? v1 * post : 0.0f;
-            if (p.add != nullptr) {          // plain load: add may alias out
-              const float2 ad = *reinterpret_cast<const float2*>(p.add + off);
-              o0 += ad.x; o1 += ad.y;
-            }
-            *reinterpret_cast<float2*>(p.out + off) = make_float2(o0, o1);
+        } else if (MODE == 2) {
+          // one rounding per step, no FMA contraction: the CPU reference (oracle/eval_ref.py) matches bit for bit.
+          // post = 2^-ex of real-valued operands (exact), 1 for the +-1 operands.
+          o0 = __fadd_rn(__fmul_rn(__fmul_rn(v0, post), a0), sb0);
+          o1 = __fadd_rn(__fmul_rn(__fmul_rn(v1, post), a1), sb1);
+          if (PADRES) {
+            // outside the channel band the residual is +0.0 and is still added: -0.0 + 0.0 = +0.0, as the
+            // materialised zero-padded tensor gives (ch and the band edges are even, so a pair is in or out)
+            float2 r = make_float2(0.f, 0.f);
+            const int rc = ch - p.res_coff;
+            if (unsigned(rc) < unsigned(p.res_C))
+              r = __ldg(reinterpret_cast<const float2*>(p.add + int64_t(rpix[h]) * p.res_C + rc));
+            o0 = __fadd_rn(o0, r.x); o1 = __fadd_rn(o1, r.y);
+          } else if (p.add != nullptr) {   // the residual never aliases z (the entry points reject it)
+            const float2 r = __ldg(reinterpret_cast<const float2*>(p.add + off));
+            o0 = __fadd_rn(o0, r.x); o1 = __fadd_rn(o1, r.y);
           }
-          if (do_stats) {
-            s0 += o0; s1 += o1;
-            if (MODE == 1) {
-              const uint32_t yr = __ldg(reinterpret_cast<const uint32_t*>(p.st_y + off));
-              q0 += o0 * fmaf(float(int16_t(yr & 0xffffu)), sa0, -sb0);
-              q1 += o1 * fmaf(float(int16_t(yr >> 16)), sa1, -sb1);
-            } else {
-              q0 += o0 * o0; q1 += o1 * o1;
-            }
-            m0 = fmaxf(m0, fabsf(o0)); m1 = fmaxf(m1, fabsf(o1));
+          if (p.relu) {                    // torch.relu: NaN stays NaN (fmaxf alone would drop it)
+            o0 = o0 != o0 ? o0 : fmaxf(o0, 0.f);
+            o1 = o1 != o1 ? o1 : fmaxf(o1, 0.f);
           }
+          *reinterpret_cast<float2*>(p.out + off) = make_float2(o0, o1);
+          zmax = max(zmax, max(__float_as_uint(fabsf(o0)), __float_as_uint(fabsf(o1))));
+          // sign(v) = +1 iff v >= 0 (DESIGN.md §2): -0.0 -> +1, NaN -> -1
+          if (p.zb != nullptr)
+            *reinterpret_cast<uint32_t*>(p.zb + off) =
+                (o0 >= 0.f ? p.zb_one : p.zb_one | 0x8000u) | ((o1 >= 0.f ? p.zb_one : p.zb_one | 0x8000u) << 16);
+          if (p.zb8 != nullptr)
+            *reinterpret_cast<uint16_t*>(p.zb8 + off) = uint16_t((o0 >= 0.f ? 0x38u : 0xB8u) |
+                                                                 ((o1 >= 0.f ? 0x38u : 0xB8u) << 8));
+        } else {
+          const uint32_t word = __ldg(p.mask + pix[h] * mask_words + (ch >> 5)) >> (ch & 31);
+          o0 = (word & 1u) ? v0 * post : 0.0f;
+          o1 = (word & 2u) ? v1 * post : 0.0f;
+          if (p.add != nullptr) {          // plain load: add may alias out
+            const float2 ad = *reinterpret_cast<const float2*>(p.add + off);
+            o0 += ad.x; o1 += ad.y;
+          }
+          *reinterpret_cast<float2*>(p.out + off) = make_float2(o0, o1);
         }
         if (do_stats) {
-          // lanes with the same lane % 4 hold the same two channels for different rows
+          s0 += o0; s1 += o1;
+          if (MODE == 1) {
+            const uint32_t yr = __ldg(reinterpret_cast<const uint32_t*>(p.st_y + off));
+            q0 += o0 * fmaf(float(int16_t(yr & 0xffffu)), sa0, -sb0);
+            q1 += o1 * fmaf(float(int16_t(yr >> 16)), sa1, -sb1);
+          } else {
+            q0 += o0 * o0; q1 += o1 * o1;
+          }
+          m0 = fmaxf(m0, fabsf(o0)); m1 = fmaxf(m1, fabsf(o1));
+        }
+      }
+      if (do_stats) {
+        // lanes with the same lane % 4 hold the same two channels for different rows
 #pragma unroll
-          for (int d = 4; d <= 16; d <<= 1) {
-            s0 += __shfl_xor_sync(0xffffffffu, s0, d); s1 += __shfl_xor_sync(0xffffffffu, s1, d);
-            q0 += __shfl_xor_sync(0xffffffffu, q0, d); q1 += __shfl_xor_sync(0xffffffffu, q1, d);
-            m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, d)); m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, d));
-          }
-          if (lane < 4) {            // each warp owns distinct rows: one writer per (warp, channel)
-            stat_sum[warp][col] = s0; stat_sum[warp][col + 1] = s1;
-            stat_sq[warp][col] = q0; stat_sq[warp][col + 1] = q1;
-            stat_max[warp][col] = m0; stat_max[warp][col + 1] = m1;
-          }
+        for (int d = 4; d <= 16; d <<= 1) {
+          s0 += __shfl_xor_sync(0xffffffffu, s0, d); s1 += __shfl_xor_sync(0xffffffffu, s1, d);
+          q0 += __shfl_xor_sync(0xffffffffu, q0, d); q1 += __shfl_xor_sync(0xffffffffu, q1, d);
+          m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, d)); m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, d));
+        }
+        if (lane < 4) {            // each warp owns distinct rows: one writer per (warp, channel)
+          stat_sum[warp][col] = s0; stat_sum[warp][col + 1] = s1;
+          stat_sq[warp][col] = q0; stat_sq[warp][col + 1] = q1;
+          stat_max[warp][col] = m0; stat_max[warp][col + 1] = m1;
         }
       }
     }
@@ -390,6 +391,7 @@ static bool plan_tc_conv(const TcConvLaunch& L, int mode, TcConvParams* pp, size
   p.amax_bits = L.amax_bits; p.add = L.add; p.relu = L.relu; p.z_amax = L.z_amax;
   if (L.pad_res) {
     if (mode != 2 || L.fmt < 0 || !L.add) return false;
+    if (int64_t(L.NIMG) * L.res_H * L.res_W > INT32_MAX) return false;   // rpix is 32 bits
     p.res_H = L.res_H; p.res_W = L.res_W; p.res_C = L.res_C; p.res_coff = L.res_coff;
   }
   p.bn_sums = L.bn_sums; p.bn_ymax = L.bn_ymax;
@@ -431,11 +433,20 @@ static int launch_one(K kern, dim3 grid, size_t smem, cudaStream_t st, const CUt
   return check_launch("tc_conv_kernel");
 }
 
+// The instance for an N tile of bn columns (16, 32, 64 or 128).
+using TcConvKernel = decltype(&tc_conv_kernel<0, 0, 16, false>);
+template <int MODE, int KIND, bool PADRES = false>
+static TcConvKernel kernel_for(int bn) {
+  return bn == 16   ? tc_conv_kernel<MODE, KIND, 16, PADRES>
+         : bn == 32 ? tc_conv_kernel<MODE, KIND, 32, PADRES>
+         : bn == 64 ? tc_conv_kernel<MODE, KIND, 64, PADRES>
+                    : tc_conv_kernel<MODE, KIND, 128, PADRES>;
+}
+
 template <int MODE, int KIND, bool PADRES = false>
 static int launch_kind(const CUtensorMap& tmA, const CUtensorMap& tmB, const TcConvParams& p, size_t smem, dim3 grid,
                        cudaStream_t st) {
-  auto kern = p.BN == 16 ? tc_conv_kernel<MODE, KIND, 16, PADRES>
-                         : (p.BN == 32 ? tc_conv_kernel<MODE, KIND, 32, PADRES> : tc_conv_kernel<MODE, KIND, 64, PADRES>);
+  const TcConvKernel kern = kernel_for<MODE, KIND, PADRES>(p.BN);
   BDBNN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
   if (p.bn_sums == nullptr) return launch_one(kern, grid, smem, st, tmA, tmB, p);
   TcConvParams q = p;
@@ -603,37 +614,12 @@ extern "C" int bdbnn_debug_tc_conv_ctas_per_sm(int32_t mode, int32_t fmt, int32_
   BDBNN_REQUIRE(ctas && mode >= 0 && mode <= 3 && (bn == 16 || bn == 32 || bn == 64 || bn == 128) && smem >= 0 &&
                     (fmt == BDBNN_FMT_FP16 || fmt == BDBNN_FMT_BF16 || (fmt == -1 && (mode == 0 || mode == 2))),
                 "debug_tc_conv_ctas_per_sm: bad arguments");
-  const void* kern;
-  if (mode == 3 && fmt == BDBNN_FMT_FP16)
-    kern = bn == 16 ? (const void*)tc_conv_kernel<2, 0, 16, true> : bn == 32 ? (const void*)tc_conv_kernel<2, 0, 32, true>
-                                                                   : (const void*)tc_conv_kernel<2, 0, 64, true>;
-  else if (mode == 3)
-    kern = bn == 16 ? (const void*)tc_conv_kernel<2, 1, 16, true> : bn == 32 ? (const void*)tc_conv_kernel<2, 1, 32, true>
-                                                                   : (const void*)tc_conv_kernel<2, 1, 64, true>;
-  else if (mode == 2 && fmt == -1)
-    kern = bn == 16 ? (const void*)tc_conv_kernel<2, 2, 16> : bn == 32 ? (const void*)tc_conv_kernel<2, 2, 32>
-                                                             : (const void*)tc_conv_kernel<2, 2, 64>;
-  else if (mode == 2 && fmt == BDBNN_FMT_FP16)
-    kern = bn == 16 ? (const void*)tc_conv_kernel<2, 0, 16> : bn == 32 ? (const void*)tc_conv_kernel<2, 0, 32>
-                                                             : (const void*)tc_conv_kernel<2, 0, 64>;
-  else if (mode == 2)
-    kern = bn == 16 ? (const void*)tc_conv_kernel<2, 1, 16> : bn == 32 ? (const void*)tc_conv_kernel<2, 1, 32>
-                                                             : (const void*)tc_conv_kernel<2, 1, 64>;
-  else if (fmt == -1)
-    kern = bn == 16 ? (const void*)tc_conv_kernel<0, 2, 16> : bn == 32 ? (const void*)tc_conv_kernel<0, 2, 32>
-                                                             : (const void*)tc_conv_kernel<0, 2, 64>;
-  else if (mode == 0 && fmt == BDBNN_FMT_FP16)
-    kern = bn == 16 ? (const void*)tc_conv_kernel<0, 0, 16> : bn == 32 ? (const void*)tc_conv_kernel<0, 0, 32>
-                                                             : (const void*)tc_conv_kernel<0, 0, 64>;
-  else if (mode == 0)
-    kern = bn == 16 ? (const void*)tc_conv_kernel<0, 1, 16> : bn == 32 ? (const void*)tc_conv_kernel<0, 1, 32>
-                                                             : (const void*)tc_conv_kernel<0, 1, 64>;
-  else if (fmt == BDBNN_FMT_FP16)
-    kern = bn == 16 ? (const void*)tc_conv_kernel<1, 0, 16> : bn == 32 ? (const void*)tc_conv_kernel<1, 0, 32>
-                                                             : (const void*)tc_conv_kernel<1, 0, 64>;
-  else
-    kern = bn == 16 ? (const void*)tc_conv_kernel<1, 1, 16> : bn == 32 ? (const void*)tc_conv_kernel<1, 1, 32>
-                                                             : (const void*)tc_conv_kernel<1, 1, 64>;
+  const int kind = fmt == -1 ? 2 : (fmt == BDBNN_FMT_BF16 ? 1 : 0);
+  TcConvKernel kern;
+  if (mode == 3) kern = kind == 0 ? kernel_for<2, 0, true>(bn) : kernel_for<2, 1, true>(bn);
+  else if (mode == 2) kern = kind == 2 ? kernel_for<2, 2>(bn) : kind == 0 ? kernel_for<2, 0>(bn) : kernel_for<2, 1>(bn);
+  else if (mode == 0) kern = kind == 2 ? kernel_for<0, 2>(bn) : kind == 0 ? kernel_for<0, 0>(bn) : kernel_for<0, 1>(bn);
+  else kern = kind == 0 ? kernel_for<1, 0>(bn) : kernel_for<1, 1>(bn);
   BDBNN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   int n = 0;
   BDBNN_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, kTcThreads, size_t(smem)));
