@@ -95,9 +95,17 @@ SIGNATURES = {
     "bdbnn_binconv_fwd_tc_eval_pad_shortcut": (c_int, [_P, _P, c_int, _P, _P, _P] + [c_int] * 4 + [_P, _P, _P, _SH,
                                                                                                  _P]),
     "bdbnn_real_conv_fwd_eval_pad_shortcut": (c_int, [_P] * 6 + [c_int] * 5 + [_P, _P, _SH, _P]),
+    "bdbnn_cifar_stem_fwd_eval_hardtanh": (c_int, [_P, c_int, c_int, c_int, c_int64, c_int64, c_int64, c_int64, _P,
+                                                   c_int] + [_P] * 5),
     "bdbnn_cifar_stem_wgrad_workspace_bytes": (c_size_t, [c_int] * 4),
     "bdbnn_cifar_stem_wgrad": (c_int, [_P, c_int, c_int, c_int, c_int64, c_int64, c_int64, c_int64, _P, _P, c_int, _P,
                                        _P, c_size_t, _P]),
+    "bdbnn_bn_fwd_hardtanh": (c_int, [_P] * 4 + [c_int64, c_int, ctypes.c_float, ctypes.c_float] + [_P] * 12 +
+                              [c_int, c_int, _P]),
+    "bdbnn_bn_bwd_pack_hardtanh": (c_int, [_P] * 9 + [c_int64, c_int, c_int] + [_P] * 8),
+    "bdbnn_pool2_i16": (c_int, [_P, _P] + [c_int] * 4 + [_P] * 5),
+    "bdbnn_pool2_bn_bwd_pack": (c_int, [_P] * 10 + [c_int] * 5 + [_P] * 8),
+    "bdbnn_pool2_bn_eval_hardtanh": (c_int, [_P] * 3 + [c_int] * 4 + [_P] * 3 + [c_int, _P]),
     "bdbnn_cifar_batch": (c_int, [_P, _P, c_int64, ctypes.c_uint64, ctypes.c_uint32, c_int64, c_int, c_int, _P, _P, _P,
                                   c_int64, c_int64, c_int64, c_int64, _P, _P]),
     "bdbnn_imagenet_batch": (c_int, [_P, _P, c_int, _P, _P, _P, c_int64, c_int64, c_int64, c_int64, _P, _P]),

@@ -50,11 +50,55 @@ __device__ __forceinline__ float4 load_y4(const void* __restrict__ y, int64_t i)
 // Per-channel (sum a, sum b, max c) over pixels; thread = one float4 channel group, strided over pixels.
 // Each block adds its threads' partials of a channel in thread order and writes them to its row of `part`
 // ([gridDim.x][2C], summed in block order by det_sums_finish): the sums are the same in every run.
-template <bool BWD, bool I16 = false>
+// The block tail shared with pool2_i16_kernel: thread partials (sa, sb) of channel group c4 and max bits mx go to the
+// block's row of `part` (threads added in thread order) and to maxbits.  shs: [2][blockDim] float4, then [C] uint32
+// zeroed by the caller before its first __syncthreads.
+__device__ __forceinline__ void block_partials(float4* shs, uint32_t* shm, int C4, int c4, float4 sa, float4 sb,
+                                               float4 mx, double* __restrict__ part, uint32_t* __restrict__ maxbits) {
+  const int C = C4 * 4;
+  const int c = c4 * 4;
+  shs[threadIdx.x] = sa;
+  shs[blockDim.x + threadIdx.x] = sb;
+  atomicMax(&shm[c + 0], __float_as_uint(mx.x)); atomicMax(&shm[c + 1], __float_as_uint(mx.y));
+  atomicMax(&shm[c + 2], __float_as_uint(mx.z)); atomicMax(&shm[c + 3], __float_as_uint(mx.w));
+  __syncthreads();
+  const int first = int((int64_t(blockIdx.x) * blockDim.x) % C4);     // channel group of thread 0
+  double* row = part + int64_t(blockIdx.x) * 2 * C;
+  for (int g = threadIdx.x; g < C4; g += blockDim.x) {
+    float4 a = make_float4(0, 0, 0, 0), b = a;
+    for (int t = (g - first + C4) % C4; t < int(blockDim.x); t += C4) {
+      const float4 u = shs[t], v = shs[blockDim.x + t];
+      a.x += u.x; a.y += u.y; a.z += u.z; a.w += u.w;
+      b.x += v.x; b.y += v.y; b.z += v.z; b.w += v.w;
+    }
+    row[4 * g + 0] = a.x; row[4 * g + 1] = a.y; row[4 * g + 2] = a.z; row[4 * g + 3] = a.w;
+    row[C + 4 * g + 0] = b.x; row[C + 4 * g + 1] = b.y; row[C + 4 * g + 2] = b.z; row[C + 4 * g + 3] = b.w;
+  }
+  for (int i = threadIdx.x; i < C; i += blockDim.x) atomicMax(maxbits + i, shm[i]);
+}
+
+// Hardtanh's gradient mask on the pre-activation u = fmaf(y, a, b) of the forward (the same fp32 operation, so the
+// same u): gz passes where -1 < u < 1, strictly, and not at NaN (DESIGN.md §4n).
+__device__ __forceinline__ float4 htanh_mask(float4 g, const float4 v, const float4 a, const float4 b) {
+  const float ux = fmaf(v.x, a.x, b.x), uy = fmaf(v.y, a.y, b.y), uz = fmaf(v.z, a.z, b.z), uw = fmaf(v.w, a.w, b.w);
+  g.x = (ux > -1.0f && ux < 1.0f) ? g.x : 0.0f;
+  g.y = (uy > -1.0f && uy < 1.0f) ? g.y : 0.0f;
+  g.z = (uz > -1.0f && uz < 1.0f) ? g.z : 0.0f;
+  g.w = (uw > -1.0f && uw < 1.0f) ? g.w : 0.0f;
+  return g;
+}
+
+// torch.nn.Hardtanh: clamp to [-1, 1], NaN stays NaN
+__device__ __forceinline__ float htanh(float u) { return u != u ? u : fminf(fmaxf(u, -1.0f), 1.0f); }
+
+// HT (backward only): gz is first multiplied by Hardtanh's mask on u = fmaf(y, ab[c], ab[C + c]) (ab: the forward's
+// bn_finalize output, alpha folded in for I16).
+template <bool BWD, bool I16 = false, bool HT = false>
 __global__ void __launch_bounds__(kBnThreads)
 bn_reduce_kernel(const float4* __restrict__ p0, const void* __restrict__ p1, const float* __restrict__ mean,
                  const float* __restrict__ invstd, int64_t n_pix, int C4, double* __restrict__ part,
-                 uint32_t* __restrict__ maxbits, const float* __restrict__ alpha = nullptr) {
+                 uint32_t* __restrict__ maxbits, const float* __restrict__ alpha = nullptr,
+                 const float* __restrict__ ab = nullptr) {
   extern __shared__ float4 shs[];             // [2][blockDim] per-thread partials, then [C] max bits
   const int C = C4 * 4;
   uint32_t* shm = reinterpret_cast<uint32_t*>(shs + 2 * blockDim.x);   // non-negative floats order like uints
@@ -75,12 +119,18 @@ bn_reduce_kernel(const float4* __restrict__ p0, const void* __restrict__ p1, con
       is = make_float4(al.x * is.x, al.y * is.y, al.z * is.z, al.w * is.w);           // alpha*invstd
     }
   }
+  float4 ha = make_float4(0, 0, 0, 0), hb = ha;
+  if (HT) {
+    ha = *reinterpret_cast<const float4*>(ab + c4 * 4);
+    hb = *reinterpret_cast<const float4*>(ab + C + c4 * 4);
+  }
   float4 sa = make_float4(0, 0, 0, 0), sb = sa, mx = sa;
 #pragma unroll 8
   for (int64_t p = gtid / C4; p < n_pix; p += p_step) {
-    const float4 u = __ldcs(p0 + p * C4 + c4);
+    float4 u = __ldcs(p0 + p * C4 + c4);
     if (BWD) {   // u = gz, v = y:  a = gz, b = gz * yhat, c = |gz|
       const float4 v = load_y4<I16>(p1, p * C4 + c4);
+      if (HT) u = htanh_mask(u, v, ha, hb);
       sa.x += u.x; sa.y += u.y; sa.z += u.z; sa.w += u.w;
       if (I16) {
         sb.x += u.x * fmaf(v.x, is.x, -mu.x); sb.y += u.y * fmaf(v.y, is.y, -mu.y);
@@ -96,25 +146,7 @@ bn_reduce_kernel(const float4* __restrict__ p0, const void* __restrict__ p1, con
     mx.x = fmaxf(mx.x, fabsf(u.x)); mx.y = fmaxf(mx.y, fabsf(u.y));
     mx.z = fmaxf(mx.z, fabsf(u.z)); mx.w = fmaxf(mx.w, fabsf(u.w));
   }
-  const int c = c4 * 4;
-  shs[threadIdx.x] = sa;
-  shs[blockDim.x + threadIdx.x] = sb;
-  atomicMax(&shm[c + 0], __float_as_uint(mx.x)); atomicMax(&shm[c + 1], __float_as_uint(mx.y));
-  atomicMax(&shm[c + 2], __float_as_uint(mx.z)); atomicMax(&shm[c + 3], __float_as_uint(mx.w));
-  __syncthreads();
-  const int first = int((int64_t(blockIdx.x) * blockDim.x) % C4);     // channel group of thread 0
-  double* row = part + int64_t(blockIdx.x) * 2 * C;
-  for (int g = threadIdx.x; g < C4; g += blockDim.x) {
-    float4 a = make_float4(0, 0, 0, 0), b = a;
-    for (int t = (g - first + C4) % C4; t < int(blockDim.x); t += C4) {
-      const float4 u = shs[t], v = shs[blockDim.x + t];
-      a.x += u.x; a.y += u.y; a.z += u.z; a.w += u.w;
-      b.x += v.x; b.y += v.y; b.z += v.z; b.w += v.w;
-    }
-    row[4 * g + 0] = a.x; row[4 * g + 1] = a.y; row[4 * g + 2] = a.z; row[4 * g + 3] = a.w;
-    row[C + 4 * g + 0] = b.x; row[C + 4 * g + 1] = b.y; row[C + 4 * g + 2] = b.z; row[C + 4 * g + 3] = b.w;
-  }
-  for (int i = threadIdx.x; i < C; i += blockDim.x) atomicMax(maxbits + i, shm[i]);
+  block_partials(shs, shm, C4, c4, sa, sb, mx, part, maxbits);
 }
 
 // ---- run-to-run deterministic sums across blocks ----------------------------------------------------
@@ -180,15 +212,16 @@ int det_sums_finish(double* part, int64_t nparts, int width, double* sums, cudaS
 }
 
 // bn_reduce_kernel over `grid` blocks with its partials summed into sums[2C] (pre-zeroed or accumulated)
-template <bool BWD, bool I16 = false>
+template <bool BWD, bool I16 = false, bool HT = false>
 static int bn_reduce_launch(int grid, const float4* p0, const void* p1, const float* mean, const float* invstd,
                             int64_t n_pix, int C4, double* sums, uint32_t* maxbits, const float* alpha,
-                            cudaStream_t st) {
+                            cudaStream_t st, const float* ab = nullptr) {
   double* part = nullptr;
   int rc = det_sums_alloc(&part, grid, 8 * C4, st);
   if (rc) return rc;
-  bn_reduce_kernel<BWD, I16><<<grid, kBnThreads, 2 * kBnThreads * sizeof(float4) + size_t(4 * C4) * sizeof(uint32_t),
-                               st>>>(p0, p1, mean, invstd, n_pix, C4, part, maxbits, alpha);
+  bn_reduce_kernel<BWD, I16, HT><<<grid, kBnThreads, 2 * kBnThreads * sizeof(float4) +
+                                   size_t(4 * C4) * sizeof(uint32_t), st>>>(p0, p1, mean, invstd, n_pix, C4, part,
+                                                                            maxbits, alpha, ab);
   rc = check_launch(BWD ? "bn_reduce_kernel<bwd>" : "bn_reduce_kernel<fwd>");
   if (rc) { cudaFreeAsync(part, st); return rc; }
   return det_sums_finish(part, grid, 8 * C4, sums, st);
@@ -232,7 +265,9 @@ struct PadResidual {
 // z = y*a + b (+ residual); optionally the sign / STE-mask bits and the +-1 16-bit copy of z.
 // SUB: the residual is the option-A shortcut of `sub.x` (res is unused).  P16: C == 16, one sign / mask word per
 // pixel from 4 lanes (bits 16-31 zero, as bdbnn_act_pack writes them) instead of one per 32 channels from 8 lanes.
-template <bool PACK, bool I16 = false, int U = 4, bool SUB = false, bool P16 = false>
+// HT: z = hardtanh(u) for u = y*a + b, and the mask bits are Hardtanh's strict -1 < u < 1 (the product of its
+// gradient and the next conv's STE indicator, which is 1 on hardtanh's range except at NaN).
+template <bool PACK, bool I16 = false, int U = 4, bool SUB = false, bool P16 = false, bool HT = false>
 __global__ void __launch_bounds__(kBnThreads)
 bn_apply_add_pack_kernel(const void* __restrict__ y, const float4* __restrict__ res,
                          const float* __restrict__ a, const float* __restrict__ b, int64_t n4, int C4,
@@ -254,13 +289,17 @@ bn_apply_add_pack_kernel(const void* __restrict__ y, const float4* __restrict__ 
     float4 o = make_float4(fmaf(v.x, av.x, bv.x), fmaf(v.y, av.y, bv.y), fmaf(v.z, av.z, bv.z),
                            fmaf(v.w, av.w, bv.w));
     o.x += r.x; o.y += r.y; o.z += r.z; o.w += r.w;
+    if (HT) { o.x = htanh(o.x); o.y = htanh(o.y); o.z = htanh(o.z); o.w = htanh(o.w); }
     // z (4 B/element, re-read only after the next conv has run) is stored evict-first so that the next conv's
     // operands written below (xb / xb8, 1-2 B/element) have a chance to stay in the 126 MB L2
     __stcs(z + i, o);
     if (PACK) {
       const uint32_t s0 = o.x >= 0.0f, s1 = o.y >= 0.0f, s2 = o.z >= 0.0f, s3 = o.w >= 0.0f;
-      const uint32_t m0 = fabsf(o.x) <= 1.0f, m1 = fabsf(o.y) <= 1.0f, m2 = fabsf(o.z) <= 1.0f,
-                     m3 = fabsf(o.w) <= 1.0f;
+      // HT: o is clamped, and clamp(u) lies strictly inside (-1, 1) exactly when u does
+      const uint32_t m0 = HT ? (o.x > -1.0f && o.x < 1.0f) : fabsf(o.x) <= 1.0f,
+                     m1 = HT ? (o.y > -1.0f && o.y < 1.0f) : fabsf(o.y) <= 1.0f,
+                     m2 = HT ? (o.z > -1.0f && o.z < 1.0f) : fabsf(o.z) <= 1.0f,
+                     m3 = HT ? (o.w > -1.0f && o.w < 1.0f) : fabsf(o.w) <= 1.0f;
       const uint32_t sw = __reduce_or_sync(group_mask, (s0 | (s1 << 1) | (s2 << 2) | (s3 << 3)) << sh);
       const uint32_t mw = __reduce_or_sync(group_mask, (m0 | (m1 << 1) | (m2 << 2) | (m3 << 3)) << sh);
       if ((lane & (GL - 1)) == 0) {
@@ -345,11 +384,12 @@ __global__ void bn_bwd_bound_kernel(const double* __restrict__ sums, const uint3
   }
 }
 
-// gys = 16-bit operand of the conv backward, straight from gz and y.
-template <int MODE, bool I16 = false, int U = 4>
+// gys = 16-bit operand of the conv backward, straight from gz and y.  HT: gz times Hardtanh's mask (bn_reduce_kernel).
+template <int MODE, bool I16 = false, int U = 4, bool HT = false>
 __global__ void __launch_bounds__(kBnThreads)
 bn_bwd_pack_kernel(const float4* __restrict__ gz, const void* __restrict__ y, const float4* __restrict__ consts,
-                   const uint32_t* __restrict__ amax_bits, int64_t n4, int C4, uint16_t* __restrict__ out) {
+                   const uint32_t* __restrict__ amax_bits, int64_t n4, int C4, uint16_t* __restrict__ out,
+                   const float* __restrict__ ab = nullptr) {
   constexpr int HALVES = MODE == 2 ? 2 : 1;
   const int64_t nthreads = int64_t(gridDim.x) * blockDim.x;       // multiple of C4
   int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -357,9 +397,15 @@ bn_bwd_pack_kernel(const float4* __restrict__ gz, const void* __restrict__ y, co
   const float up = MODE == 3 ? amax_pow2_scale(*amax_bits, false) : 1.0f;
   const float4 k0 = consts[c4 * 4 + 0], k1 = consts[c4 * 4 + 1], k2 = consts[c4 * 4 + 2], k3 = consts[c4 * 4 + 3];
   const int C = C4 * 4;
+  float4 ha = make_float4(0, 0, 0, 0), hb = ha;
+  if (HT) {
+    ha = *reinterpret_cast<const float4*>(ab + c4 * 4);
+    hb = *reinterpret_cast<const float4*>(ab + C + c4 * 4);
+  }
   int64_t pix = i / C4;
   const int64_t pix_step = nthreads / C4;
-  auto emit = [&](int64_t pix, const float4 g, const float4 v) {
+  auto emit = [&](int64_t pix, float4 g, const float4 v) {
+    if (HT) g = htanh_mask(g, v, ha, hb);
     const float a0 = (g.x - k0.x - (v.x - k0.z) * k0.y) * k0.w * up;
     const float a1 = (g.y - k1.x - (v.y - k1.z) * k1.y) * k1.w * up;
     const float a2 = (g.z - k2.x - (v.z - k2.z) * k2.y) * k2.w * up;
@@ -392,6 +438,160 @@ bn_bwd_pack_kernel(const float4* __restrict__ gz, const void* __restrict__ y, co
     for (int u = 0; u < U; ++u) emit(pix + u * pix_step, g[u], v[u]);
   }
   for (; i < n4; i += nthreads, pix += pix_step) emit(pix, __ldcs(gz + i), load_y4<I16>(y, i));
+}
+
+// Hardtanh units after a 2x2 / stride-2 max-pool (DESIGN.md §4n), int16 conv results y_int [N][H][W][C] (H, W even):
+//   pool2_i16_kernel      : p = 2x2 max of y_int (exact: alpha >= 0 and fp32 rounding are monotone), the winner's tap
+//                           (dy*2 + dx, first maximum in scan order, one byte per channel), and the BatchNorm batch
+//                           statistics of alpha*p (partials per block, summed in block order) with max|alpha*p|
+//   pool2_bwd_pack_kernel : the BatchNorm backward on the pooled tensor (gz times Hardtanh's mask) written as the conv
+//                           backward's 16-bit operand at the conv-output resolution: the value at the winner, 0 elsewhere
+//   pool2_eval_kernel     : z = hardtanh(fp32(fp32(max * scale) + shift)) from the folded eval BatchNorm, + the +-1 copy
+__device__ __forceinline__ int4 pool2_quad(const int16_t* __restrict__ y, int64_t off) {
+  const uint2 r = __ldcs(reinterpret_cast<const uint2*>(y + off));
+  return make_int4(int16_t(r.x & 0xffffu), int16_t(r.x >> 16), int16_t(r.y & 0xffffu), int16_t(r.y >> 16));
+}
+
+// max over the window at (n, 2ho, 2wo), channels 4*c4..4*c4+3; tap bytes in *win (strict > keeps the first maximum)
+__device__ __forceinline__ int4 pool2_max(const int16_t* __restrict__ y, int64_t n, int ho, int wo, int H, int W,
+                                          int C, int c4, uint32_t* win) {
+  int4 m = make_int4(0, 0, 0, 0);
+  uint32_t tx = 0, ty = 0, tz = 0, tw = 0;
+#pragma unroll
+  for (int t = 0; t < 4; ++t) {
+    const int64_t off = ((n * H + 2 * ho + (t >> 1)) * W + 2 * wo + (t & 1)) * C + 4 * c4;
+    const int4 v = pool2_quad(y, off);
+    if (t == 0 || v.x > m.x) { m.x = v.x; tx = t; }
+    if (t == 0 || v.y > m.y) { m.y = v.y; ty = t; }
+    if (t == 0 || v.z > m.z) { m.z = v.z; tz = t; }
+    if (t == 0 || v.w > m.w) { m.w = v.w; tw = t; }
+  }
+  *win = tx | (ty << 8) | (tz << 16) | (tw << 24);
+  return m;
+}
+
+// thread = one channel group, strided over pooled pixels as bn_reduce_kernel (grid * blockDim a multiple of C4)
+__global__ void __launch_bounds__(kBnThreads)
+pool2_i16_kernel(const int16_t* __restrict__ y, const float* __restrict__ alpha, int H, int W, int C4, int64_t n_pool,
+                 int16_t* __restrict__ p, uint32_t* __restrict__ idx, double* __restrict__ part,
+                 uint32_t* __restrict__ maxbits) {
+  extern __shared__ float4 shs[];
+  const int C = C4 * 4;
+  uint32_t* shm = reinterpret_cast<uint32_t*>(shs + 2 * blockDim.x);
+  for (int i = threadIdx.x; i < C; i += blockDim.x) shm[i] = 0u;
+  __syncthreads();
+  const int Ho = H / 2, Wo = W / 2;
+  const int64_t gtid = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  const int64_t nthreads = int64_t(gridDim.x) * blockDim.x;
+  const int c4 = int(gtid % C4);
+  const int64_t p_step = nthreads / C4;
+  const float4 al = *reinterpret_cast<const float4*>(alpha + c4 * 4);
+  float4 sa = make_float4(0, 0, 0, 0), sb = sa, mx = sa;
+  for (int64_t q = gtid / C4; q < n_pool; q += p_step) {
+    const int wo = int(q % Wo);
+    const int64_t r = q / Wo;
+    const int ho = int(r % Ho);
+    uint32_t win;
+    const int4 m = pool2_max(y, r / Ho, ho, wo, H, W, C, c4, &win);
+    const int64_t o = q * C4 + c4;
+    *reinterpret_cast<uint2*>(p + 4 * o) = make_uint2((uint32_t(m.x) & 0xffffu) | (uint32_t(m.y) << 16),
+                                                      (uint32_t(m.z) & 0xffffu) | (uint32_t(m.w) << 16));
+    idx[o] = win;
+    // alpha * p is the conv's fp32 output at the winner (one fp32 multiply, as the conv epilogue)
+    const float4 v = make_float4(float(m.x) * al.x, float(m.y) * al.y, float(m.z) * al.z, float(m.w) * al.w);
+    sa.x += v.x; sa.y += v.y; sa.z += v.z; sa.w += v.w;
+    sb.x += v.x * v.x; sb.y += v.y * v.y; sb.z += v.z * v.z; sb.w += v.w * v.w;
+    mx.x = fmaxf(mx.x, fabsf(v.x)); mx.y = fmaxf(mx.y, fabsf(v.y));
+    mx.z = fmaxf(mx.z, fabsf(v.z)); mx.w = fmaxf(mx.w, fabsf(v.w));
+  }
+  block_partials(shs, shm, C4, c4, sa, sb, mx, part, maxbits);
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(kBnThreads)
+pool2_bwd_pack_kernel(const float4* __restrict__ gz, const int16_t* __restrict__ p, const uint32_t* __restrict__ idx,
+                      const float4* __restrict__ consts, const float* __restrict__ ab,
+                      const uint32_t* __restrict__ amax_bits, int H, int W, int C4, int64_t n4,
+                      uint16_t* __restrict__ out) {
+  constexpr int HALVES = MODE == 2 ? 2 : 1;
+  const int64_t nthreads = int64_t(gridDim.x) * blockDim.x;       // multiple of C4
+  int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  const int c4 = int(i % C4);
+  const int C = C4 * 4, Ho = H / 2, Wo = W / 2;
+  const float up = MODE == 3 ? amax_pow2_scale(*amax_bits, false) : 1.0f;
+  const float4 k0 = consts[c4 * 4 + 0], k1 = consts[c4 * 4 + 1], k2 = consts[c4 * 4 + 2], k3 = consts[c4 * 4 + 3];
+  const float4 ha = *reinterpret_cast<const float4*>(ab + c4 * 4);
+  const float4 hb = *reinterpret_cast<const float4*>(ab + C + c4 * 4);
+  for (; i < n4; i += nthreads) {
+    const float4 v = load_y4<true>(p, i);
+    const float4 g = htanh_mask(__ldcs(gz + i), v, ha, hb);
+    const uint32_t win = __ldcs(idx + i);
+    const float a0 = (g.x - k0.x - (v.x - k0.z) * k0.y) * k0.w * up;
+    const float a1 = (g.y - k1.x - (v.y - k1.z) * k1.y) * k1.w * up;
+    const float a2 = (g.z - k2.x - (v.z - k2.z) * k2.y) * k2.w * up;
+    const float a3 = (g.w - k3.x - (v.w - k3.z) * k3.y) * k3.w * up;
+    const int64_t q = i / C4;
+    const int wo = int(q % Wo);
+    const int64_t r = q / Wo;
+    const int ho = int(r % Ho);
+    const int64_t n = r / Ho;
+#pragma unroll
+    for (int t = 0; t < 4; ++t) {
+      const float b0 = (win & 0xffu) == uint32_t(t) ? a0 : 0.0f;
+      const float b1 = ((win >> 8) & 0xffu) == uint32_t(t) ? a1 : 0.0f;
+      const float b2 = ((win >> 16) & 0xffu) == uint32_t(t) ? a2 : 0.0f;
+      const float b3 = (win >> 24) == uint32_t(t) ? a3 : 0.0f;
+      const int64_t pix = (n * H + 2 * ho + (t >> 1)) * W + 2 * wo + (t & 1);
+      uint16_t* dst = out + pix * (int64_t(HALVES) * C) + c4 * 4;
+      uint2 o;
+      if (MODE == 3) {
+        o.x = bn_pack_f16x2(b0, b1);
+        o.y = bn_pack_f16x2(b2, b3);
+      } else {
+        o.x = bn_pack_bf16x2(b0, b1);
+        o.y = bn_pack_bf16x2(b2, b3);
+      }
+      *reinterpret_cast<uint2*>(dst) = o;
+      if (MODE == 2) {
+        uint2 l;
+        l.x = bn_pack_bf16x2(b0 - bn_bf16_round(b0), b1 - bn_bf16_round(b1));
+        l.y = bn_pack_bf16x2(b2 - bn_bf16_round(b2), b3 - bn_bf16_round(b3));
+        *reinterpret_cast<uint2*>(dst + C) = l;
+      }
+    }
+  }
+}
+
+__global__ void __launch_bounds__(kBnThreads)
+pool2_eval_kernel(const int16_t* __restrict__ y, const float* __restrict__ scale, const float* __restrict__ shift,
+                  int H, int W, int C4, int64_t n4, float4* __restrict__ z, uint2* __restrict__ zb,
+                  uint32_t* __restrict__ zb8, uint32_t one16) {
+  const int64_t nthreads = int64_t(gridDim.x) * blockDim.x;       // multiple of C4
+  int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  const int c4 = int(i % C4);
+  const int Ho = H / 2, Wo = W / 2;
+  const float4 sc = *reinterpret_cast<const float4*>(scale + c4 * 4);
+  const float4 sf = *reinterpret_cast<const float4*>(shift + c4 * 4);
+  const uint32_t pos = one16, neg = one16 | 0x8000u;
+  for (; i < n4; i += nthreads) {
+    const int64_t q = i / C4;
+    const int wo = int(q % Wo);
+    const int64_t r = q / Wo;
+    uint32_t win;
+    const int4 m = pool2_max(y, r / Ho, int(r % Ho), wo, H, W, C4 * 4, c4, &win);
+    // one rounding per step, no FMA contraction (the eval epilogue of tc_conv_kernel)
+    float4 o;
+    o.x = htanh(__fadd_rn(__fmul_rn(float(m.x), sc.x), sf.x));
+    o.y = htanh(__fadd_rn(__fmul_rn(float(m.y), sc.y), sf.y));
+    o.z = htanh(__fadd_rn(__fmul_rn(float(m.z), sc.z), sf.z));
+    o.w = htanh(__fadd_rn(__fmul_rn(float(m.w), sc.w), sf.w));
+    z[i] = o;
+    const bool s0 = o.x >= 0.0f, s1 = o.y >= 0.0f, s2 = o.z >= 0.0f, s3 = o.w >= 0.0f;
+    if (zb != nullptr)
+      zb[i] = make_uint2((s0 ? pos : neg) | ((s1 ? pos : neg) << 16), (s2 ? pos : neg) | ((s3 ? pos : neg) << 16));
+    if (zb8 != nullptr)
+      zb8[i] = 0x38383838u | ((s0 ? 0u : 0x80u) | (s1 ? 0u : 0x8000u) | (s2 ? 0u : 0x800000u) | (s3 ? 0u : 0x80000000u));
+  }
 }
 
 static int bn_grid(int64_t work, int C4, int per_sm = 8) {
@@ -454,13 +654,14 @@ static int bn_fwd_impl(const void* y, const float* alpha_i16, const float* resid
                        float* running_var, double* sums_ws, uint32_t* ymax_bits, float* mean, float* invstd,
                        float* ab_ws, float* z, uint32_t* sign_bits, uint32_t* mask_bits, uint16_t* xb,
                        uint8_t* xb_fp8, int32_t fmt, int32_t stats_ready, void* stream,
-                       const PadResidual* sub = nullptr) {
+                       const PadResidual* sub = nullptr, bool ht = false) {
   const bool pack = sign_bits != nullptr;
   const bool i16 = alpha_i16 != nullptr;
   // 16-channel packs (one word per pixel): the CIFAR stem's BatchNorm, fp32 y only
   const bool p16 = pack && C == 16;
   BDBNN_REQUIRE(!i16 || stats_ready, "bn_fwd_i16: the statistics must come from the conv epilogue (stats_ready = 1)");
   BDBNN_REQUIRE(!(p16 && (i16 || sub)), "bn_fwd: 16-channel packs only without int16 y and option-A residual");
+  BDBNN_REQUIRE(!ht || (pack && !p16 && !sub && !residual), "bn_fwd_hardtanh: needs the packs, C %% 32 == 0 and no residual");
   int rc = bn_dims_ok(n_pix, C, pack && !p16);
   if (rc) return rc;
   BDBNN_REQUIRE(y && gamma && beta && sums_ws && ymax_bits && mean && invstd && ab_ws && z, "bn_fwd: NULL pointer");
@@ -505,6 +706,16 @@ static int bn_fwd_impl(const void* y, const float* alpha_i16, const float* resid
     bn_apply_add_pack_kernel<true, false, 4, false, true><<<grid, kBnThreads, 0, st>>>(
         y, r4, a, b, n4, C4, z4, sign_bits, mask_bits, reinterpret_cast<uint2*>(xb),
         reinterpret_cast<uint32_t*>(xb_fp8), one16);
+  } else if (ht) {
+    const uint32_t one16 = fmt == BDBNN_FMT_FP16 ? 0x3C00u : 0x3F80u;
+    uint2* xb2 = reinterpret_cast<uint2*>(xb);
+    uint32_t* xb8 = reinterpret_cast<uint32_t*>(xb_fp8);
+    if (i16)
+      bn_apply_add_pack_kernel<true, true, 4, false, false, true><<<grid, kBnThreads, 0, st>>>(
+          y, nullptr, a, b, n4, C4, z4, sign_bits, mask_bits, xb2, xb8, one16);
+    else
+      bn_apply_add_pack_kernel<true, false, 4, false, false, true><<<grid, kBnThreads, 0, st>>>(
+          y, nullptr, a, b, n4, C4, z4, sign_bits, mask_bits, xb2, xb8, one16);
   } else if (pack) {
     const uint32_t one16 = fmt == BDBNN_FMT_FP16 ? 0x3C00u : 0x3F80u;
     uint2* xb2 = reinterpret_cast<uint2*>(xb);
@@ -538,6 +749,17 @@ extern "C" int bdbnn_bn_fwd(const float* y, const float* residual, const float* 
                             uint16_t* xb, uint8_t* xb_fp8, int32_t fmt, int32_t stats_ready, void* stream) {
   return bn_fwd_impl(y, nullptr, residual, gamma, beta, n_pix, C, eps, momentum, running_mean, running_var, sums_ws,
                      ymax_bits, mean, invstd, ab_ws, z, sign_bits, mask_bits, xb, xb_fp8, fmt, stats_ready, stream);
+}
+
+extern "C" int bdbnn_bn_fwd_hardtanh(const void* y, const float* alpha, const float* gamma, const float* beta,
+                                     int64_t n_pix, int32_t C, float eps, float momentum, float* running_mean,
+                                     float* running_var, double* sums_ws, uint32_t* ymax_bits, float* mean,
+                                     float* invstd, float* ab_ws, float* z, uint32_t* sign_bits, uint32_t* mask_bits,
+                                     uint16_t* xb, uint8_t* xb_fp8, int32_t fmt, int32_t stats_ready, void* stream) {
+  BDBNN_REQUIRE(sign_bits != nullptr, "bn_fwd_hardtanh: NULL sign_bits");
+  return bn_fwd_impl(y, alpha, nullptr, gamma, beta, n_pix, C, eps, momentum, running_mean, running_var, sums_ws,
+                     ymax_bits, mean, invstd, ab_ws, z, sign_bits, mask_bits, xb, xb_fp8, fmt, stats_ready, stream,
+                     nullptr, true);
 }
 
 extern "C" int bdbnn_bn_fwd_i16(const int16_t* y_int, const float* alpha, const float* residual, const float* gamma,
@@ -598,8 +820,10 @@ static int bn_bwd_pack_impl(const float* gz, const void* y, const float* alpha_i
                             const float* invstd, const float* gamma, const float* gscale, const uint32_t* ymax_bits,
                             int64_t n_pix, int32_t C, int32_t grad_mode, double* sums_ws, uint32_t* gmax_bits,
                             float* consts_ws, float* dgamma, float* dbeta, uint32_t* amax_bits, uint16_t* gys,
-                            int stats_ready, void* stream) {
+                            int stats_ready, void* stream, const float* ab_ht = nullptr) {
   const bool i16 = alpha_i16 != nullptr;
+  const bool ht = ab_ht != nullptr;
+  BDBNN_REQUIRE(!(ht && stats_ready), "bn_bwd_pack_hardtanh: the sums are of the masked gradient (stats_ready = 0)");
   int rc = bn_dims_ok(n_pix, C, false);
   if (rc) return rc;
   BDBNN_REQUIRE(gz && y && mean && invstd && gamma && gscale && ymax_bits && sums_ws && gmax_bits && consts_ws &&
@@ -612,12 +836,17 @@ static int bn_bwd_pack_impl(const float* gz, const void* y, const float* alpha_i
     BDBNN_CUDA(cudaMemsetAsync(sums_ws, 0, size_t(2 * C) * sizeof(double), st));
     BDBNN_CUDA(cudaMemsetAsync(gmax_bits, 0, size_t(C) * sizeof(uint32_t), st));
     const int rgrid = bn_grid(n_pix * C4 / 8, C4, n_pix * C4 > (int64_t(16) << 20) ? 8 : 3);
-    if (i16)
-      rc = bn_reduce_launch<true, true>(rgrid, reinterpret_cast<const float4*>(gz), y, mean, invstd, n_pix, C4, sums_ws,
-                                        gmax_bits, alpha_i16, st);
+    const float4* g4 = reinterpret_cast<const float4*>(gz);
+    if (i16 && ht)
+      rc = bn_reduce_launch<true, true, true>(rgrid, g4, y, mean, invstd, n_pix, C4, sums_ws, gmax_bits, alpha_i16, st,
+                                              ab_ht);
+    else if (ht)
+      rc = bn_reduce_launch<true, false, true>(rgrid, g4, y, mean, invstd, n_pix, C4, sums_ws, gmax_bits, nullptr, st,
+                                               ab_ht);
+    else if (i16)
+      rc = bn_reduce_launch<true, true>(rgrid, g4, y, mean, invstd, n_pix, C4, sums_ws, gmax_bits, alpha_i16, st);
     else
-      rc = bn_reduce_launch<true, false>(rgrid, reinterpret_cast<const float4*>(gz), y, mean, invstd, n_pix, C4,
-                                         sums_ws, gmax_bits, nullptr, st);
+      rc = bn_reduce_launch<true, false>(rgrid, g4, y, mean, invstd, n_pix, C4, sums_ws, gmax_bits, nullptr, st);
     if (rc) return rc;
   }
   bn_bwd_bound_kernel<<<1, 256, 0, st>>>(sums_ws, gmax_bits, ymax_bits, n_pix, C, mean, invstd, gamma, gscale,
@@ -632,7 +861,20 @@ static int bn_bwd_pack_impl(const float* gz, const void* y, const float* alpha_i
   const int grid = bn_grid(n4, C4, bwd_per_sm);
   const float4* g4 = reinterpret_cast<const float4*>(gz);
   const float4* k4 = reinterpret_cast<const float4*>(consts_ws);
-  if (i16) {
+  if (ht) {
+    if (i16 && grad_mode == BDBNN_GRAD_FP16S)
+      bn_bwd_pack_kernel<3, true, 4, true><<<grid, kBnThreads, 0, st>>>(g4, y, k4, amax_bits, n4, C4, gys, ab_ht);
+    else if (i16 && grad_mode == BDBNN_GRAD_BF16X2)
+      bn_bwd_pack_kernel<2, true, 4, true><<<grid, kBnThreads, 0, st>>>(g4, y, k4, amax_bits, n4, C4, gys, ab_ht);
+    else if (i16)
+      bn_bwd_pack_kernel<1, true, 4, true><<<grid, kBnThreads, 0, st>>>(g4, y, k4, amax_bits, n4, C4, gys, ab_ht);
+    else if (grad_mode == BDBNN_GRAD_FP16S)
+      bn_bwd_pack_kernel<3, false, 4, true><<<grid, kBnThreads, 0, st>>>(g4, y, k4, amax_bits, n4, C4, gys, ab_ht);
+    else if (grad_mode == BDBNN_GRAD_BF16X2)
+      bn_bwd_pack_kernel<2, false, 4, true><<<grid, kBnThreads, 0, st>>>(g4, y, k4, amax_bits, n4, C4, gys, ab_ht);
+    else
+      bn_bwd_pack_kernel<1, false, 4, true><<<grid, kBnThreads, 0, st>>>(g4, y, k4, amax_bits, n4, C4, gys, ab_ht);
+  } else if (i16) {
     if (grad_mode == BDBNN_GRAD_FP16S)
       bn_bwd_pack_kernel<3, true><<<grid, kBnThreads, 0, st>>>(g4, y, k4, amax_bits, n4, C4, gys);
     else if (grad_mode == BDBNN_GRAD_BF16X2)
@@ -657,6 +899,102 @@ extern "C" int bdbnn_bn_bwd_pack(const float* gz, const float* y, const float* m
                                  uint32_t* amax_bits, uint16_t* gys, void* stream) {
   return bn_bwd_pack_impl(gz, y, nullptr, mean, invstd, gamma, gscale, ymax_bits, n_pix, C, grad_mode, sums_ws,
                           gmax_bits, consts_ws, dgamma, dbeta, amax_bits, gys, 0, stream);
+}
+
+extern "C" int bdbnn_bn_bwd_pack_hardtanh(const float* gz, const void* y, const float* alpha, const float* ab,
+                                          const float* mean, const float* invstd, const float* gamma,
+                                          const float* gscale, const uint32_t* ymax_bits, int64_t n_pix, int32_t C,
+                                          int32_t grad_mode, double* sums_ws, uint32_t* gmax_bits, float* consts_ws,
+                                          float* dgamma, float* dbeta, uint32_t* amax_bits, uint16_t* gys,
+                                          void* stream) {
+  BDBNN_REQUIRE(ab != nullptr, "bn_bwd_pack_hardtanh: NULL ab");
+  return bn_bwd_pack_impl(gz, y, alpha, mean, invstd, gamma, gscale, ymax_bits, n_pix, C, grad_mode, sums_ws,
+                          gmax_bits, consts_ws, dgamma, dbeta, amax_bits, gys, 0, stream, ab);
+}
+
+// ---- 2x2 max-pool units (pool2_* kernels) ----------------------------------------------------------------------------
+static int pool2_dims_ok(const char* what, int32_t N, int32_t H, int32_t W, int32_t C) {
+  BDBNN_REQUIRE(N > 0 && H > 0 && W > 0, "%s: non-positive dims", what);
+  BDBNN_REQUIRE(H % 2 == 0 && W % 2 == 0, "%s: H and W must be even", what);
+  BDBNN_REQUIRE(C > 0 && C % 32 == 0 && C <= 4096, "%s: C must be a positive multiple of 32, <= 4096", what);
+  return BDBNN_OK;
+}
+
+extern "C" int bdbnn_pool2_i16(const int16_t* y_int, const float* alpha, int32_t N, int32_t H, int32_t W, int32_t C,
+                               int16_t* p_int, uint8_t* idx, double* sums, uint32_t* ymax_bits, void* stream) {
+  int rc = pool2_dims_ok("pool2_i16", N, H, W, C);
+  if (rc) return rc;
+  BDBNN_REQUIRE(y_int && alpha && p_int && idx && sums && ymax_bits, "pool2_i16: NULL pointer");
+  cudaStream_t st = cudaStream_t(stream);
+  const int C4 = C / 4;
+  const int64_t n_pool = int64_t(N) * (H / 2) * (W / 2);
+  BDBNN_CUDA(cudaMemsetAsync(sums, 0, size_t(2 * C) * sizeof(double), st));
+  BDBNN_CUDA(cudaMemsetAsync(ymax_bits, 0, size_t(C) * sizeof(uint32_t), st));
+  const int grid = bn_grid(n_pool * C4 / 2, C4);
+  double* part = nullptr;
+  rc = det_sums_alloc(&part, grid, 2 * C, st);
+  if (rc) return rc;
+  pool2_i16_kernel<<<grid, kBnThreads, 2 * kBnThreads * sizeof(float4) + size_t(C) * sizeof(uint32_t), st>>>(
+      y_int, alpha, H, W, C4, n_pool, p_int, reinterpret_cast<uint32_t*>(idx), part, ymax_bits);
+  rc = check_launch("pool2_i16_kernel");
+  if (rc) { cudaFreeAsync(part, st); return rc; }
+  return det_sums_finish(part, grid, 2 * C, sums, st);
+}
+
+extern "C" int bdbnn_pool2_bn_bwd_pack(const float* gz, const int16_t* p_int, const uint8_t* idx, const float* alpha,
+                                       const float* ab, const float* mean, const float* invstd, const float* gamma,
+                                       const float* gscale, const uint32_t* ymax_bits, int32_t N, int32_t H, int32_t W,
+                                       int32_t C, int32_t grad_mode, double* sums_ws, uint32_t* gmax_bits,
+                                       float* consts_ws, float* dgamma, float* dbeta, uint32_t* amax_bits,
+                                       uint16_t* gys, void* stream) {
+  int rc = pool2_dims_ok("pool2_bn_bwd_pack", N, H, W, C);
+  if (rc) return rc;
+  BDBNN_REQUIRE(gz && p_int && idx && alpha && ab && mean && invstd && gamma && gscale && ymax_bits && sums_ws &&
+                    gmax_bits && consts_ws && dgamma && dbeta && amax_bits && gys,
+                "pool2_bn_bwd_pack: NULL pointer");
+  BDBNN_REQUIRE(grad_mode >= BDBNN_GRAD_BF16 && grad_mode <= BDBNN_GRAD_FP16S, "pool2_bn_bwd_pack: bad grad_mode");
+  cudaStream_t st = cudaStream_t(stream);
+  const int C4 = C / 4;
+  const int64_t n_pool = int64_t(N) * (H / 2) * (W / 2);
+  BDBNN_CUDA(cudaMemsetAsync(sums_ws, 0, size_t(2 * C) * sizeof(double), st));
+  BDBNN_CUDA(cudaMemsetAsync(gmax_bits, 0, size_t(C) * sizeof(uint32_t), st));
+  // BatchNorm's backward over the pooled tensor (it normalised the pooled values); each conv-output position takes at
+  // most one pooled gradient, so the FP16S bound needs no multiplier
+  rc = bn_reduce_launch<true, true, true>(bn_grid(n_pool * C4 / 8, C4, 3), reinterpret_cast<const float4*>(gz), p_int,
+                                          mean, invstd, n_pool, C4, sums_ws, gmax_bits, alpha, st, ab);
+  if (rc) return rc;
+  bn_bwd_bound_kernel<<<1, 256, 0, st>>>(sums_ws, gmax_bits, ymax_bits, n_pool, C, mean, invstd, gamma, gscale,
+                                         reinterpret_cast<float4*>(consts_ws), dgamma, dbeta, amax_bits, 1.0f, alpha);
+  rc = check_launch("bn_bwd_bound_kernel");
+  if (rc) return rc;
+  const int64_t n4 = n_pool * C4;
+  const int grid = bn_grid(n4, C4);
+  const float4* g4 = reinterpret_cast<const float4*>(gz);
+  const float4* k4 = reinterpret_cast<const float4*>(consts_ws);
+  const uint32_t* w4 = reinterpret_cast<const uint32_t*>(idx);
+  if (grad_mode == BDBNN_GRAD_FP16S)
+    pool2_bwd_pack_kernel<3><<<grid, kBnThreads, 0, st>>>(g4, p_int, w4, k4, ab, amax_bits, H, W, C4, n4, gys);
+  else if (grad_mode == BDBNN_GRAD_BF16X2)
+    pool2_bwd_pack_kernel<2><<<grid, kBnThreads, 0, st>>>(g4, p_int, w4, k4, ab, amax_bits, H, W, C4, n4, gys);
+  else
+    pool2_bwd_pack_kernel<1><<<grid, kBnThreads, 0, st>>>(g4, p_int, w4, k4, ab, amax_bits, H, W, C4, n4, gys);
+  return check_launch("pool2_bwd_pack_kernel");
+}
+
+extern "C" int bdbnn_pool2_bn_eval_hardtanh(const int16_t* y_int, const float* scale, const float* shift, int32_t N,
+                                            int32_t H, int32_t W, int32_t C, float* z, uint16_t* zb, uint8_t* zb8,
+                                            int32_t fmt, void* stream) {
+  int rc = pool2_dims_ok("pool2_bn_eval_hardtanh", N, H, W, C);
+  if (rc) return rc;
+  BDBNN_REQUIRE(y_int && scale && shift && z, "pool2_bn_eval_hardtanh: NULL pointer");
+  cudaStream_t st = cudaStream_t(stream);
+  const int C4 = C / 4;
+  const int64_t n4 = int64_t(N) * (H / 2) * (W / 2) * C4;
+  pool2_eval_kernel<<<bn_grid(n4, C4), kBnThreads, 0, st>>>(y_int, scale, shift, H, W, C4, n4,
+                                                           reinterpret_cast<float4*>(z), reinterpret_cast<uint2*>(zb),
+                                                           reinterpret_cast<uint32_t*>(zb8),
+                                                           fmt == BDBNN_FMT_FP16 ? 0x3C00u : 0x3F80u);
+  return check_launch("pool2_eval_kernel");
 }
 
 extern "C" int bdbnn_bn_bwd_pack_i16(const float* gz, const int16_t* y_int, const float* alpha, const float* mean,

@@ -17,9 +17,9 @@ namespace bdbnn {
 constexpr int kCsThreads = 256;
 constexpr int kCsTaps = 27;           // 3 input channels x 3 x 3, tap t = c*9 + r*3 + s (OIHW order)
 constexpr int kCsGroup = 16;          // output channels per forward block (blockIdx.y)
-constexpr int kCsMaxCout = 64;
+constexpr int kCsMaxCout = 64;        // the ResNet stems: 16, 32, 48, 64; VGG-Small's 128 has instances of its own
 constexpr int kCsChunk = 128;         // pixels per shared-memory stage of the weight gradient
-constexpr int kCsOutPerThread = kCsMaxCout * kCsTaps / kCsThreads + 1;
+constexpr int kCsWideCout = 128;
 
 // The 27 taps of output pixel (n, h, w), zero outside the image; x addressed through element strides.
 __device__ __forceinline__ void cifar_stem_taps(const float* __restrict__ x, int n, int h, int w, int H, int W,
@@ -41,7 +41,8 @@ __device__ __forceinline__ void cifar_stem_taps(const float* __restrict__ x, int
 // ([gridDim.x][2*Cout]) and max|y| to ymax (integer atomicMax of the bits: order-free).
 // EVAL: the eval-mode BatchNorm folded into the epilogue instead, y = fp32(fp32(acc * scale[o]) + shift[o]) (no FMA
 // contraction, as tc_conv_kernel's eval epilogue), and the bits of max|y| over all channels into ymax[0].
-template <bool EVAL>
+// HT (with EVAL): z = hardtanh(BN_eval(conv)), torch.nn.Hardtanh (NaN stays NaN) — the VGG-Small stem.
+template <bool EVAL, bool HT = false>
 __global__ void __launch_bounds__(kCsThreads)
 cifar_stem_fwd_kernel(const float* __restrict__ x, int N, int H, int W, int64_t sN, int64_t sC, int64_t sH,
                       int64_t sW, const float* __restrict__ wt, int Cout, float* __restrict__ y,
@@ -74,6 +75,10 @@ cifar_stem_fwd_kernel(const float* __restrict__ x, int N, int H, int W, int64_t 
 #pragma unroll
       for (int o = 0; o < kCsGroup; ++o)
         acc[o] = __fadd_rn(__fmul_rn(acc[o], __ldg(scale + o0 + o)), __ldg(shift + o0 + o));
+      if (HT) {
+#pragma unroll
+        for (int o = 0; o < kCsGroup; ++o) acc[o] = acc[o] != acc[o] ? acc[o] : fminf(fmaxf(acc[o], -1.0f), 1.0f);
+      }
     }
     float4* dst = reinterpret_cast<float4*>(y + p * Cout + o0);
 #pragma unroll
@@ -119,14 +124,17 @@ static int cifar_stem_wgrad_grid(int64_t n_pix) {
   return int(blocks < 1 ? 1 : blocks);
 }
 
-// Block b stages pixel chunks b, b + gridDim.x, ... (x taps [27][chunk], gradient [chunk][Cout] as floats) and every
+// Block b stages pixel chunks b, b + gridDim.x, ... (x taps [27][chunk] as floats, gradient [chunk][Cout] as GT: float
+// for the ResNet stems, the fp16 values themselves for 128 channels, which keeps them under 48 KB) and every
 // thread adds, in pixel order, the terms of the outputs idx = tid + k*256 (o = idx % Cout, t = idx / Cout) in fp32.
 // The block's sums go to its row of part ([gridDim.x][Cout*27], index o*27 + t = OIHW).
+template <int MAXC, typename GT>
 __global__ void __launch_bounds__(kCsThreads)
 cifar_stem_wgrad_kernel(const float* __restrict__ x, int N, int H, int W, int64_t sN, int64_t sC, int64_t sH,
                         int64_t sW, const __half* __restrict__ gys, int Cout, double* __restrict__ part) {
+  constexpr int kCsOutPerThread = MAXC * kCsTaps / kCsThreads + 1;
   __shared__ float xs[kCsTaps][kCsChunk + 1];
-  __shared__ float gs[kCsChunk][kCsMaxCout];
+  __shared__ GT gs[kCsChunk][MAXC];
   const int64_t n_pix = int64_t(N) * H * W;
   const int64_t n_chunks = (n_pix + kCsChunk - 1) / kCsChunk;
   const int n_out = Cout * kCsTaps;
@@ -154,7 +162,7 @@ cifar_stem_wgrad_kernel(const float* __restrict__ x, int N, int H, int W, int64_
     }
     for (int i = threadIdx.x; i < kCsChunk * Cout; i += blockDim.x) {
       const int j = i / Cout, o = i - j * Cout;
-      gs[j][o] = j < np ? __half2float(gys[(p0 + j) * Cout + o]) : 0.0f;
+      gs[j][o] = j < np ? GT(gys[(p0 + j) * Cout + o]) : GT(0.0f);
     }
     __syncthreads();
 #pragma unroll
@@ -163,7 +171,7 @@ cifar_stem_wgrad_kernel(const float* __restrict__ x, int N, int H, int W, int64_
       if (idx >= n_out) break;
       const int o = idx % Cout, t = idx / Cout;
       float a = acc[k];
-      for (int j = 0; j < np; ++j) a = fmaf(xs[t][j], gs[j][o], a);
+      for (int j = 0; j < np; ++j) a = fmaf(xs[t][j], float(gs[j][o]), a);
       acc[k] = a;
     }
   }
@@ -208,7 +216,9 @@ pad_shortcut_bwd_kernel(const float4* __restrict__ gz, float4* __restrict__ gx, 
   }
 }
 
-static bool cifar_stem_cout_ok(int Cout) { return Cout >= kCsGroup && Cout <= kCsMaxCout && Cout % kCsGroup == 0; }
+static bool cifar_stem_cout_ok(int Cout) {
+  return Cout % kCsGroup == 0 && ((Cout >= kCsGroup && Cout <= kCsMaxCout) || Cout == kCsWideCout);
+}
 
 }  // namespace bdbnn
 
@@ -218,7 +228,7 @@ extern "C" int bdbnn_cifar_stem_fwd(const float* x, int32_t N, int32_t H, int32_
                                     int64_t sH, int64_t sW, const float* weight, int32_t Cout, float* y,
                                     double* bn_sums, uint32_t* bn_ymax, void* stream) {
   BDBNN_REQUIRE(N > 0 && H > 0 && W > 0, "cifar_stem_fwd: non-positive dims");
-  BDBNN_REQUIRE(cifar_stem_cout_ok(Cout), "cifar_stem_fwd: Cout must be 16, 32, 48 or 64");
+  BDBNN_REQUIRE(cifar_stem_cout_ok(Cout), "cifar_stem_fwd: Cout must be 16, 32, 48, 64 or 128");
   BDBNN_REQUIRE(x && weight && y, "cifar_stem_fwd: NULL pointer");
   BDBNN_REQUIRE((bn_sums == nullptr) == (bn_ymax == nullptr), "cifar_stem_fwd: bn_sums and bn_ymax go together");
   BDBNN_REQUIRE((uintptr_t(y) & 15) == 0, "cifar_stem_fwd: y must be 16-byte aligned");
@@ -240,20 +250,36 @@ extern "C" int bdbnn_cifar_stem_fwd(const float* x, int32_t N, int32_t H, int32_
   return det_sums_finish(part, grid.x, 2 * Cout, bn_sums, st);
 }
 
-extern "C" int bdbnn_cifar_stem_fwd_eval(const float* x, int32_t N, int32_t H, int32_t W, int64_t sN, int64_t sC,
-                                         int64_t sH, int64_t sW, const float* weight, int32_t Cout, const float* scale,
-                                         const float* shift, float* z, uint32_t* z_amax_bits, void* stream) {
-  BDBNN_REQUIRE(N > 0 && H > 0 && W > 0, "cifar_stem_fwd_eval: non-positive dims");
-  BDBNN_REQUIRE(cifar_stem_cout_ok(Cout), "cifar_stem_fwd_eval: Cout must be 16, 32, 48 or 64");
+template <bool HT>
+static int cifar_stem_eval_launch(const float* x, int32_t N, int32_t H, int32_t W, int64_t sN, int64_t sC, int64_t sH,
+                                  int64_t sW, const float* weight, int32_t Cout, const float* scale, const float* shift,
+                                  float* z, uint32_t* z_amax_bits, void* stream) {
   BDBNN_REQUIRE(x && weight && scale && shift && z && z_amax_bits, "cifar_stem_fwd_eval: NULL pointer");
   BDBNN_REQUIRE((uintptr_t(z) & 15) == 0, "cifar_stem_fwd_eval: z must be 16-byte aligned");
   cudaStream_t st = cudaStream_t(stream);
   const int64_t n_pix = int64_t(N) * H * W;
   const dim3 grid(unsigned((n_pix + kCsThreads - 1) / kCsThreads), unsigned(Cout / kCsGroup));
   BDBNN_CUDA(cudaMemsetAsync(z_amax_bits, 0, sizeof(uint32_t), st));
-  cifar_stem_fwd_kernel<true><<<grid, kCsThreads, 0, st>>>(x, N, H, W, sN, sC, sH, sW, weight, Cout, z, nullptr,
-                                                           z_amax_bits, scale, shift);
+  cifar_stem_fwd_kernel<true, HT><<<grid, kCsThreads, 0, st>>>(x, N, H, W, sN, sC, sH, sW, weight, Cout, z, nullptr,
+                                                               z_amax_bits, scale, shift);
   return check_launch("cifar_stem_fwd_eval_kernel");
+}
+
+extern "C" int bdbnn_cifar_stem_fwd_eval(const float* x, int32_t N, int32_t H, int32_t W, int64_t sN, int64_t sC,
+                                         int64_t sH, int64_t sW, const float* weight, int32_t Cout, const float* scale,
+                                         const float* shift, float* z, uint32_t* z_amax_bits, void* stream) {
+  BDBNN_REQUIRE(N > 0 && H > 0 && W > 0, "cifar_stem_fwd_eval: non-positive dims");
+  BDBNN_REQUIRE(cifar_stem_cout_ok(Cout) && Cout <= kCsMaxCout, "cifar_stem_fwd_eval: Cout must be 16, 32, 48 or 64");
+  return cifar_stem_eval_launch<false>(x, N, H, W, sN, sC, sH, sW, weight, Cout, scale, shift, z, z_amax_bits, stream);
+}
+
+extern "C" int bdbnn_cifar_stem_fwd_eval_hardtanh(const float* x, int32_t N, int32_t H, int32_t W, int64_t sN,
+                                                  int64_t sC, int64_t sH, int64_t sW, const float* weight, int32_t Cout,
+                                                  const float* scale, const float* shift, float* z,
+                                                  uint32_t* z_amax_bits, void* stream) {
+  BDBNN_REQUIRE(N > 0 && H > 0 && W > 0, "cifar_stem_fwd_eval_hardtanh: non-positive dims");
+  BDBNN_REQUIRE(cifar_stem_cout_ok(Cout), "cifar_stem_fwd_eval_hardtanh: Cout must be 16, 32, 48, 64 or 128");
+  return cifar_stem_eval_launch<true>(x, N, H, W, sN, sC, sH, sW, weight, Cout, scale, shift, z, z_amax_bits, stream);
 }
 
 extern "C" size_t bdbnn_cifar_stem_wgrad_workspace_bytes(int32_t N, int32_t H, int32_t W, int32_t Cout) {
@@ -265,15 +291,19 @@ extern "C" int bdbnn_cifar_stem_wgrad(const float* x, int32_t N, int32_t H, int3
                                       int64_t sH, int64_t sW, const uint16_t* gys, const uint32_t* g_amax_bits,
                                       int32_t Cout, float* gW, void* workspace, size_t workspace_bytes, void* stream) {
   BDBNN_REQUIRE(N > 0 && H > 0 && W > 0, "cifar_stem_wgrad: non-positive dims");
-  BDBNN_REQUIRE(cifar_stem_cout_ok(Cout), "cifar_stem_wgrad: Cout must be 16, 32, 48 or 64");
+  BDBNN_REQUIRE(cifar_stem_cout_ok(Cout), "cifar_stem_wgrad: Cout must be 16, 32, 48, 64 or 128");
   BDBNN_REQUIRE(x && gys && g_amax_bits && gW && workspace, "cifar_stem_wgrad: NULL pointer");
   BDBNN_REQUIRE(workspace_bytes >= bdbnn_cifar_stem_wgrad_workspace_bytes(N, H, W, Cout),
                 "cifar_stem_wgrad: workspace too small (needs bdbnn_cifar_stem_wgrad_workspace_bytes)");
   cudaStream_t st = cudaStream_t(stream);
   const int grid = cifar_stem_wgrad_grid(int64_t(N) * H * W);
   double* part = static_cast<double*>(workspace);
-  cifar_stem_wgrad_kernel<<<grid, kCsThreads, 0, st>>>(x, N, H, W, sN, sC, sH, sW, reinterpret_cast<const __half*>(gys),
-                                                       Cout, part);
+  const __half* gh = reinterpret_cast<const __half*>(gys);
+  if (Cout <= kCsMaxCout)
+    cifar_stem_wgrad_kernel<kCsMaxCout, float><<<grid, kCsThreads, 0, st>>>(x, N, H, W, sN, sC, sH, sW, gh, Cout, part);
+  else
+    cifar_stem_wgrad_kernel<kCsWideCout, __half><<<grid, kCsThreads, 0, st>>>(x, N, H, W, sN, sC, sH, sW, gh, Cout,
+                                                                              part);
   int rc = check_launch("cifar_stem_wgrad_kernel");
   if (rc) return rc;
   const int n_out = Cout * kCsTaps;

@@ -883,8 +883,9 @@ class _ConvBNAddUnit(torch.autograd.Function):
     @_on_device
     def forward(ctx, x, weight, gamma, beta, residual, running_mean, running_var, momentum, eps, stride,
                 padding, xs, xm, xb, xb8, res_is_x, sc_weight=None, sc_gamma=None, sc_beta=None, sc_rm=None,
-                sc_rv=None, sc_momentum=None, sc_eps=None, sc_stride=None, sc_pad=None):
+                sc_rv=None, sc_momentum=None, sc_eps=None, sc_stride=None, sc_pad=None, hardtanh=False):
         _require_cuda(x, "conv_bn_add(x)")
+        ctx.hardtanh = bool(hardtanh)
         _same_device(x, weight, gamma, beta, residual, running_mean, running_var, sc_weight)
         # sc_pad: the option-A shortcut (x[:, :, ::2, ::2] zero-padded by sc_pad channels on each side) is read in
         # place by bn_fwd as the residual, and its gradient is added in place to this conv's (see backward)
@@ -981,7 +982,12 @@ class _ConvBNAddUnit(torch.autograd.Function):
         res_bytes = 4 * n_pix * (x.shape[1] if sc_pad is not None else cout)
         with _timed("bn_fwd", key, ((0 if in_conv else 4) + ybytes + 4 + (2.25 if pack else 0) +
                                     (1 if zb8 is not None else 0)) * n_pix * cout + res_bytes):
-            if sc_pad is not None:
+            if ctx.hardtanh:
+                _lib.check(L.bdbnn_bn_fwd_hardtanh(
+                    _p(y), _p(alpha) if i16 else None, _p(gamma.detach()), _p(beta.detach()), n_pix, cout, float(eps),
+                    float(momentum), _p(running_mean), _p(running_var), _p(sums), _p(ymax), _p(mean), _p(invstd),
+                    _p(ab), _p(z), _p(zs), _p(zm), _p(zb), _p(zb8), fmt, 1 if in_conv else 0, st), "bn_fwd_hardtanh")
+            elif sc_pad is not None:
                 xc = _nhwc(x.detach())
                 _, cin, h, w = x.shape
                 if i16:
@@ -1008,15 +1014,17 @@ class _ConvBNAddUnit(torch.autograd.Function):
                                           1 if in_conv else 0, st), "bn_fwd")
         _lib.count(2 if in_conv else 3)
         ctx.y_i16 = i16
-        ctx.bnctx_out = (y, alpha, mean, invstd) if i16 else None
+        # a consumer's dgrad epilogue may accumulate this unit's backward sums only where gz needs no Hardtanh mask
+        ctx.bnctx_out = (y, alpha, mean, invstd) if (i16 and not ctx.hardtanh) else None
         ctx.sh, ctx.gmode = sh, (gname, gcode, ghalves)
         ctx.shapes = (tuple(x.shape), tuple(weight.shape))
         ctx.w_param = weight if (weight.is_leaf and weight.requires_grad) else None
         ctx.sc_w_param = sc_weight if (sc_weight is not None and sc_weight.is_leaf and sc_weight.requires_grad) else None
         ctx.has_res = residual is not None and sc_weight is None
         ctx.res_is_x = bool(res_is_x)
+        # ab (the BatchNorm's per-channel a, b) lets the Hardtanh backward recompute its mask exactly
         ctx.save_for_backward(y, mean, invstd, gamma.detach(), ymax, xm, xb, wp.wt, wp.wmask, wp.gscale, wp.inv_gscale,
-                              alpha, *sc_saved)
+                              alpha, *sc_saved, *((ab,) if ctx.hardtanh else ()))
         _ConvBNAddUnit._last_bnctx = ctx.bnctx_out       # picked up by conv_bn_add right after apply() (same thread)
         if pack:
             if zb8 is not None:
@@ -1030,7 +1038,7 @@ class _ConvBNAddUnit(torch.autograd.Function):
     @_on_device
     def backward(ctx, gz, _g1, _g2, _g3, _g4):
         if gz is None:
-            return (None,) * 25
+            return (None,) * 26
         L = _lib.lib()
         sh = ctx.sh
         st = _stream()
@@ -1057,7 +1065,12 @@ class _ConvBNAddUnit(torch.autograd.Function):
         if ctx.y_i16 and stt is not None and stt[2].data_ptr() == y.data_ptr() and stt[3] == gz._version:
             sums, gmax, ready = stt[0], stt[1], 1
         with _timed("bn_bwd_pack", key, ((0 if ready else 4 + ybytes) + 4 + ybytes + 2 * gh) * n_pix * cout):
-            if ctx.y_i16:
+            if ctx.hardtanh:
+                _lib.check(L.bdbnn_bn_bwd_pack_hardtanh(
+                    _p(g), _p(y), _p(alpha) if ctx.y_i16 else None, _p(ctx.saved_tensors[12]), _p(mean), _p(invstd),
+                    _p(gamma), _p(gscale), _p(ymax), n_pix, cout, gcode, _p(sums), _p(gmax), _p(consts), _p(dgamma),
+                    _p(dbeta), _p(amax), _p(gys), st), "bn_bwd_pack_hardtanh")
+            elif ctx.y_i16:
                 _lib.check(L.bdbnn_bn_bwd_pack_i16(_p(g), _p(y), _p(alpha), _p(mean), _p(invstd), _p(gamma), _p(gscale),
                                                    _p(ymax), n_pix, cout, gcode, _p(sums), _p(gmax), _p(consts),
                                                    _p(dgamma), _p(dbeta), _p(amax), _p(gys), ready, st),
@@ -1117,7 +1130,7 @@ class _ConvBNAddUnit(torch.autograd.Function):
             sc_db = sc_db if ctx.needs_input_grad[18] else None
         return (gx, gw, dgamma if ctx.needs_input_grad[2] else None, dbeta if ctx.needs_input_grad[3] else None,
                 gres, None, None, None, None, None, None, None, None, None, None, None,
-                sc_gw, sc_dg, sc_db, None, None, None, None, None, None)
+                sc_gw, sc_dg, sc_db, None, None, None, None, None, None, None)
 
 
 PadShortcut = collections.namedtuple("PadShortcut", "pad")
@@ -1133,19 +1146,27 @@ def pad_shortcut_supported(x_shape, w_shape, stride, pad):
 
 
 def conv_bn_add(x, weight, gamma, beta, residual, running_mean, running_var, momentum, eps, stride, padding,
-                shortcut=None):
+                shortcut=None, hardtanh=False):
     """z = BN_train(binconv2d(x, weight)) + residual on the fused kernels.  `shortcut` = (weight[Cout,Cin,1,1],
     gamma, beta, running_mean, running_var, momentum, eps, stride) evaluates the real-valued 1x1 conv + BN
     `downsample` branch of x inside the same node and uses it as the residual; `shortcut` = PadShortcut(pad) uses
     the option-A shortcut of x, read in place by the BatchNorm apply, its gradient added in place to this conv's
     input gradient (no padded tensor in either direction).  The returned tensor carries
     `_bdbnn_pack` = (sign bits, mask bits, +-1 copy, fmt, fp8 copy) of z so that a following conv_bn_add skips its
-    own activation pack; x's own `_bdbnn_pack` (if present and of the current format) is consumed."""
+    own activation pack; x's own `_bdbnn_pack` (if present and of the current format) is consumed.
+    `hardtanh`: z = hardtanh(BN_train(binconv2d(x, weight))) without residual (the VGG-Small units, DESIGN.md §4n);
+    the mask bits of z's pack are Hardtanh's strict -1 < u < 1 and the backward applies that mask to gz."""
     fmt = grad_mode()[3]
     pk = _get_act_pack(x, fmt)
     xs, xm, xb, xb8 = (pk.sign, pk.mask, pk.xb, pk.xb8) if pk is not None else (None,) * 4
     res_is_x = residual is x and x.shape[1] == weight.shape[0] and int(stride) == 1
-    if isinstance(shortcut, PadShortcut):
+    if hardtanh:
+        if residual is not None or shortcut is not None or weight.shape[0] % 32:
+            raise RuntimeError("conv_bn_add: hardtanh needs Cout % 32 == 0 and neither residual nor shortcut")
+        z, zs, zm, zb, zb8 = _ConvBNAddUnit.apply(x, weight, gamma, beta, None, running_mean, running_var, momentum,
+                                                  eps, int(stride), int(padding), xs, xm, xb, xb8, False,
+                                                  *([None] * 9), True)
+    elif isinstance(shortcut, PadShortcut):
         if residual is not None:
             raise RuntimeError("conv_bn_add: pass either residual or shortcut")
         if not pad_shortcut_supported(x.shape, weight.shape, stride, shortcut.pad):
@@ -1553,14 +1574,15 @@ def stem_bn_pool(y, gamma, beta, running_mean, running_var, momentum, eps, kerne
 # ---------------------------------------------------------------------------------------------------
 # CIFAR stem (DESIGN.md §4i): fp32 3x3 / stride-1 / pad-1 conv on 3 channels + BatchNorm(train), one node
 # ---------------------------------------------------------------------------------------------------
-def cifar_stem_supported(x_shape, w_shape, stride, padding):
+def cifar_stem_supported(x_shape, w_shape, stride, padding, hardtanh=False):
     """The CIFAR stem kernels' geometry: x [N,3,H,W], weight [Cout,3,3,3] with Cout in {16, 32, 48, 64}, stride 1,
-    pad 1 (stride / padding as the (h, w) pairs nn.Conv2d keeps)."""
+    pad 1 (stride / padding as the (h, w) pairs nn.Conv2d keeps).  With `hardtanh` (the VGG-Small stem, DESIGN.md §4n)
+    Cout is 128."""
     if len(x_shape) != 4 or x_shape[1] != 3 or min(x_shape) < 1 or len(w_shape) != 4:
         return False
     cout = w_shape[0]
-    return (tuple(w_shape[1:]) == (3, 3, 3) and cout % 16 == 0 and 16 <= cout <= 64 and
-            tuple(stride) == (1, 1) and tuple(padding) == (1, 1))
+    width_ok = cout == 128 if hardtanh else (cout % 16 == 0 and 16 <= cout <= 64)
+    return tuple(w_shape[1:]) == (3, 3, 3) and width_ok and tuple(stride) == (1, 1) and tuple(padding) == (1, 1)
 
 
 def _dense_images(x):
@@ -1578,11 +1600,12 @@ class _CifarStem(torch.autograd.Function):
 
     @staticmethod
     @_on_device
-    def forward(ctx, x, weight, gamma, beta, running_mean, running_var, momentum, eps):
+    def forward(ctx, x, weight, gamma, beta, running_mean, running_var, momentum, eps, hardtanh=False):
         _require_cuda(x, "cifar_stem_conv_bn(x)")
         _require_cuda(weight, "cifar_stem_conv_bn(weight)")
         _same_device(x, weight, gamma, beta, running_mean, running_var)
-        if not cifar_stem_supported(x.shape, weight.shape, (1, 1), (1, 1)):
+        ctx.hardtanh = bool(hardtanh)
+        if not cifar_stem_supported(x.shape, weight.shape, (1, 1), (1, 1), ctx.hardtanh):
             raise RuntimeError(f"bdbnn_b200.cifar_stem_conv_bn: unsupported input {tuple(x.shape)} / weight "
                                f"{tuple(weight.shape)}")
         ctx.set_materialize_grads(False)
@@ -1614,14 +1637,20 @@ class _CifarStem(torch.autograd.Function):
         z = torch.empty_like(y)
         mean, invstd, ab = torch.empty((cout,), **f32), torch.empty((cout,), **f32), torch.empty((2 * cout,), **f32)
         with _timed("cifar_stem_bn_fwd", key, (8 + (2.25 if pack else 0) + (1 if zb8 is not None else 0)) * y.numel()):
-            _lib.check(L.bdbnn_bn_fwd(_p(y), None, _p(gamma.detach()), _p(beta.detach()), n_pix, cout, float(eps),
-                                      float(momentum), _p(running_mean), _p(running_var), _p(sums), _p(ymax),
-                                      _p(mean), _p(invstd), _p(ab), _p(z), _p(zs), _p(zm), _p(zb), _p(zb8), fmt, 1,
-                                      st), "bn_fwd(cifar stem)")
+            if ctx.hardtanh:
+                _lib.check(L.bdbnn_bn_fwd_hardtanh(_p(y), None, _p(gamma.detach()), _p(beta.detach()), n_pix, cout,
+                                                   float(eps), float(momentum), _p(running_mean), _p(running_var),
+                                                   _p(sums), _p(ymax), _p(mean), _p(invstd), _p(ab), _p(z), _p(zs),
+                                                   _p(zm), _p(zb), _p(zb8), fmt, 1, st), "bn_fwd_hardtanh(cifar stem)")
+            else:
+                _lib.check(L.bdbnn_bn_fwd(_p(y), None, _p(gamma.detach()), _p(beta.detach()), n_pix, cout, float(eps),
+                                          float(momentum), _p(running_mean), _p(running_var), _p(sums), _p(ymax),
+                                          _p(mean), _p(invstd), _p(ab), _p(z), _p(zs), _p(zm), _p(zb), _p(zb8), fmt, 1,
+                                          st), "bn_fwd(cifar stem)")
         _lib.count(2)       # finalize, apply
         ctx.geom = (n, h, w, cout)
         ctx.w_param = weight if (weight.is_leaf and weight.requires_grad) else None
-        ctx.save_for_backward(xd, y, mean, invstd, gamma.detach(), ymax)
+        ctx.save_for_backward(xd, y, mean, invstd, gamma.detach(), ymax, *((ab,) if ctx.hardtanh else ()))
         nd = [t for t in (zs, zm, zb, zb8) if t is not None]
         if nd:
             ctx.mark_non_differentiable(*nd)
@@ -1631,9 +1660,9 @@ class _CifarStem(torch.autograd.Function):
     @_on_device
     def backward(ctx, gz, *_unused):
         if gz is None or not (ctx.needs_input_grad[1] or ctx.needs_input_grad[2] or ctx.needs_input_grad[3]):
-            return (None,) * 8
+            return (None,) * 9
         L = _lib.lib()
-        xd, y, mean, invstd, gamma, ymax = ctx.saved_tensors
+        xd, y, mean, invstd, gamma, ymax = ctx.saved_tensors[:6]
         n, h, w, cout = ctx.geom
         n_pix = n * h * w
         dev = gz.device
@@ -1648,9 +1677,15 @@ class _CifarStem(torch.autograd.Function):
         ones = torch.ones((cout,), **f32)
         gys = torch.empty((n, h, w, cout), dtype=torch.int16, device=dev)
         with _timed("cifar_stem_bn_bwd", key, 18 * n_pix * cout):
-            _lib.check(L.bdbnn_bn_bwd_pack(_p(g), _p(y), _p(mean), _p(invstd), _p(gamma), _p(ones), _p(ymax), n_pix,
-                                           cout, 3, _p(sums), _p(gmax), _p(consts), _p(dgamma), _p(dbeta), _p(amax),
-                                           _p(gys), st), "bn_bwd_pack(cifar stem)")
+            if ctx.hardtanh:
+                _lib.check(L.bdbnn_bn_bwd_pack_hardtanh(_p(g), _p(y), None, _p(ctx.saved_tensors[6]), _p(mean),
+                                                        _p(invstd), _p(gamma), _p(ones), _p(ymax), n_pix, cout, 3,
+                                                        _p(sums), _p(gmax), _p(consts), _p(dgamma), _p(dbeta), _p(amax),
+                                                        _p(gys), st), "bn_bwd_pack_hardtanh(cifar stem)")
+            else:
+                _lib.check(L.bdbnn_bn_bwd_pack(_p(g), _p(y), _p(mean), _p(invstd), _p(gamma), _p(ones), _p(ymax),
+                                               n_pix, cout, 3, _p(sums), _p(gmax), _p(consts), _p(dgamma), _p(dbeta),
+                                               _p(amax), _p(gys), st), "bn_bwd_pack(cifar stem)")
         _lib.count(3)
         gw = None
         if ctx.needs_input_grad[1]:
@@ -1660,14 +1695,16 @@ class _CifarStem(torch.autograd.Function):
                 int(L.bdbnn_cifar_stem_wgrad_workspace_bytes(n, h, w, cout)), (cout, 3, 3, 3), ctx.w_param,
                 (xd, gys, amax), "cifar_stem_wgrad", key, 4 * xd.numel() + 2 * gys.numel())
         return (None, gw, dgamma if ctx.needs_input_grad[2] else None, dbeta if ctx.needs_input_grad[3] else None,
-                None, None, None, None)
+                None, None, None, None, None)
 
 
-def cifar_stem_conv_bn(x, weight, gamma, beta, running_mean, running_var, momentum, eps):
+def cifar_stem_conv_bn(x, weight, gamma, beta, running_mean, running_var, momentum, eps, hardtanh=False):
     """BN_train(conv2d(x, weight, stride 1, pad 1)) of the CIFAR stem (see cifar_stem_supported) as one node: fp32
     conv, BatchNorm with its running-statistics update (the caller adds 1 to num_batches_tracked), TF32-class weight
-    gradient, no input gradient.  The result carries `_bdbnn_pack` for the first binary conv."""
-    z, zs, zm, zb, zb8 = _CifarStem.apply(x, weight, gamma, beta, running_mean, running_var, momentum, eps)
+    gradient, no input gradient.  The result carries `_bdbnn_pack` for the first binary conv.  `hardtanh`: the result
+    is hardtanh(BN_train(...)) with Hardtanh's strict mask in the pack (conv_bn_add(hardtanh=True))."""
+    z, zs, zm, zb, zb8 = _CifarStem.apply(x, weight, gamma, beta, running_mean, running_var, momentum, eps,
+                                          bool(hardtanh))
     if zs is not None:
         _set_act_pack(z, _ActPack(zs, zm, zb, grad_mode()[3], zb8))
     return z
@@ -2009,15 +2046,17 @@ def _pad_res_bytes(sh):
 
 
 @_on_x_device
-def cifar_stem_conv_bn_eval(x, weight, gamma, beta, running_mean, running_var, eps):
+def cifar_stem_conv_bn_eval(x, weight, gamma, beta, running_mean, running_var, eps, hardtanh=False):
     """BN_eval(conv2d(x, weight, stride 1, pad 1)) of the CIFAR stem under no_grad: fold (alpha = 1) ->
     cifar_stem_fwd_eval, the fp32 direct conv of cifar_stem_conv_bn with the folded BatchNorm in its epilogue.
-    Returns (z fp32 channels_last [N,Cout,H,W], z_amax int32[1] = bits of max|z|)."""
+    Returns (z fp32 channels_last [N,Cout,H,W], z_amax int32[1] = bits of max|z|).  `hardtanh`: z =
+    hardtanh(BN_eval(...)) in the same epilogue (cifar_stem_fwd_eval_hardtanh), with the widths of
+    cifar_stem_supported(hardtanh=True)."""
     _eval_only("cifar_stem_conv_bn_eval")
     _require_cuda(x, "cifar_stem_conv_bn_eval(x)")
     _require_cuda(weight, "cifar_stem_conv_bn_eval(weight)")
     _same_device(x, weight, gamma, beta, running_mean, running_var)
-    if not cifar_stem_supported(x.shape, weight.shape, (1, 1), (1, 1)):
+    if not cifar_stem_supported(x.shape, weight.shape, (1, 1), (1, 1), hardtanh):
         raise RuntimeError(f"bdbnn_b200.cifar_stem_conv_bn_eval: unsupported input {tuple(x.shape)} / weight "
                            f"{tuple(weight.shape)}")
     L = _lib.lib()
@@ -2028,9 +2067,9 @@ def cifar_stem_conv_bn_eval(x, weight, gamma, beta, running_mean, running_var, e
     z = torch.empty((n, cout, h, w), dtype=torch.float32, device=x.device, memory_format=torch.channels_last)
     z_amax = torch.empty((1,), dtype=torch.int32, device=x.device)
     with _timed("cifar_stem_fwd_eval", f"cifar_stem_N{n}_{h}x{w}_c{cout}", 4 * xd.numel() + 4 * z.numel()):
-        _lib.check(L.bdbnn_cifar_stem_fwd_eval(_p(xd), n, h, w, *xd.stride(), _p(weight.detach().contiguous()), cout,
-                                               _p(scale), _p(shift), _p(z), _p(z_amax), _stream()),
-                   "cifar_stem_fwd_eval")
+        fn = L.bdbnn_cifar_stem_fwd_eval_hardtanh if hardtanh else L.bdbnn_cifar_stem_fwd_eval
+        _lib.check(fn(_p(xd), n, h, w, *xd.stride(), _p(weight.detach().contiguous()), cout, _p(scale), _p(shift),
+                      _p(z), _p(z_amax), _stream()), "cifar_stem_fwd_eval")
     _lib.count(1)
     return z, z_amax
 
@@ -2044,3 +2083,189 @@ def stem_conv_bn_relu_pool_eval(x, weight, gamma, beta, running_mean, running_va
     _require_cuda(x, "stem_conv_bn_relu_pool_eval(x)")
     return _stem_eval_impl(x, weight, gamma, beta, running_mean, running_var, eps, kernel_size, stride, padding,
                            relu=True)
+
+
+# ---------------------------------------------------------------------------------------------------
+# VGG-Small units (DESIGN.md §4n): binary conv -> 2x2 max-pool -> BatchNorm -> Hardtanh as one node
+# ---------------------------------------------------------------------------------------------------
+def pool_unit_supported(x_shape, w_shape, stride, padding):
+    """conv_pool_bn's geometry: all three wgmma kernels and the int16 result for the conv, an even conv output and
+    Cout % 32 == 0 (the pooled packs)."""
+    sh = conv_shape(x_shape, w_shape, stride, padding)
+    caps = int(_lib.lib().bdbnn_tc_supported(ctypes.byref(sh)))
+    return caps & 23 == 23 and sh.Ho % 2 == 0 and sh.Wo % 2 == 0 and sh.Cout % 32 == 0
+
+
+class _ConvPoolBNUnit(torch.autograd.Function):
+    """z = hardtanh(BN_train(maxpool2x2(binconv2d(x, weight)))).
+    forward : [act_pack(x)] -> fwd_tc_i16 (no statistics) -> pool2_i16 (p, winner, statistics of alpha*p) ->
+              bn_fwd_hardtanh(p) (z + the next conv's packs)
+    backward: pool2_bn_bwd_pack (BN + Hardtanh backward on the pooled tensor, gys at the winners) -> wgrad_tc, dgrad_tc.
+    Saved for backward: the pooled int16 p, the winner bytes, x's mask bits and +-1 copy, the weight operands."""
+
+    @staticmethod
+    @_on_device
+    def forward(ctx, x, weight, gamma, beta, running_mean, running_var, momentum, eps, padding, xs, xm, xb, xb8):
+        _require_cuda(x, "conv_pool_bn(x)")
+        _same_device(x, weight, gamma, beta, running_mean, running_var)
+        if not pool_unit_supported(x.shape, weight.shape, 1, padding):
+            raise RuntimeError(f"bdbnn_b200.conv_pool_bn: unsupported input {tuple(x.shape)} / weight "
+                               f"{tuple(weight.shape)}")
+        ctx.set_materialize_grads(False)
+        L = _lib.lib()
+        sh = conv_shape(x.shape, weight.shape, 1, padding)
+        dev = x.device
+        n, cout, ho, wo = sh.N, sh.Cout, sh.Ho // 2, sh.Wo // 2
+        st = _stream()
+        gname, gcode, ghalves, fmt = grad_mode()
+        key = _shape_key(sh)
+        i32 = dict(dtype=torch.int32, device=dev)
+        f32 = dict(dtype=torch.float32, device=dev)
+        use8 = bool(int(L.bdbnn_tc_supported(ctypes.byref(sh))) & 8) and use_fwd8(sh.Cin, cout, eval_unit=False)
+        ap = _act_pack(x, sh, fmt, xb=True, xb8=use8, have=None if xs is None else _ActPack(xs, xm, xb, fmt, xb8))
+        wp = _prepacked(weight, fmt, use8)
+        if wp is None:
+            wp = _alloc_weight_pack(weight.shape, dev, wf=not use8, wf8=use8, grad=True)
+            _weight_pack(weight, wp, fmt)
+        y = torch.empty((n, sh.Ho, sh.Wo, cout), dtype=torch.int16, device=dev)
+        with _timed("binconv_fwd_tc8" if use8 else "binconv_fwd_tc", key,
+                    algorithmic_bytes("fwd_tc8" if use8 else "fwd_tc", sh) - 2 * y.numel()):
+            _lib.check(L.bdbnn_binconv_fwd_tc_i16(_p(ap.xb8) if use8 else _p(ap.xb), _p(wp.wf8) if use8 else _p(wp.wf),
+                                                  -1 if use8 else fmt, _p(wp.alpha), _p(y), ctypes.byref(sh), None,
+                                                  None, st), "binconv_fwd_tc_i16")
+        _lib.count(1)
+        p = torch.empty((n, ho, wo, cout), dtype=torch.int16, device=dev)
+        idx = torch.empty((n, ho, wo, cout), dtype=torch.uint8, device=dev)
+        sums = torch.empty((2 * cout,), dtype=torch.float64, device=dev)
+        ymax = torch.empty((cout,), **i32)
+        with _timed("pool2_i16", key, 2 * y.numel() + 3 * p.numel()):
+            _lib.check(L.bdbnn_pool2_i16(_p(y), _p(wp.alpha), n, sh.Ho, sh.Wo, cout, _p(p), _p(idx), _p(sums),
+                                         _p(ymax), st), "pool2_i16")
+        _lib.count(2)       # pool, statistics sum
+        n_pool = n * ho * wo
+        z = torch.empty((n, cout, ho, wo), memory_format=torch.channels_last, **f32)
+        mean, invstd, ab = torch.empty((cout,), **f32), torch.empty((cout,), **f32), torch.empty((2 * cout,), **f32)
+        zs = torch.empty((n, ho, wo, cout // 32), **i32)
+        zm = torch.empty((n, ho, wo, cout // 32), **i32)
+        zb = torch.empty((n, ho, wo, cout), dtype=torch.int16, device=dev)
+        zb8 = torch.empty((n, ho, wo, cout), dtype=torch.uint8, device=dev) if fwd8_enabled() else None
+        with _timed("bn_fwd", key, (2 + 4 + 2.25 + (1 if zb8 is not None else 0)) * n_pool * cout):
+            _lib.check(L.bdbnn_bn_fwd_hardtanh(
+                _p(p), _p(wp.alpha), _p(gamma.detach()), _p(beta.detach()), n_pool, cout, float(eps), float(momentum),
+                _p(running_mean), _p(running_var), _p(sums), _p(ymax), _p(mean), _p(invstd), _p(ab), _p(z), _p(zs),
+                _p(zm), _p(zb), _p(zb8), fmt, 1, st), "bn_fwd_hardtanh")
+        _lib.count(2)
+        ctx.sh, ctx.gmode = sh, (gname, gcode, ghalves)
+        ctx.shapes = (tuple(x.shape), tuple(weight.shape))
+        ctx.w_param = weight if (weight.is_leaf and weight.requires_grad) else None
+        ctx.save_for_backward(p, idx, wp.alpha, ab, mean, invstd, gamma.detach(), ymax, ap.mask, ap.xb, wp.wt, wp.wmask,
+                              wp.gscale, wp.inv_gscale)
+        nd = [t for t in (zs, zm, zb, zb8) if t is not None]
+        ctx.mark_non_differentiable(*nd)
+        return z, zs, zm, zb, zb8
+
+    @staticmethod
+    @_on_device
+    def backward(ctx, gz, *_unused):
+        if gz is None:
+            return (None,) * 13
+        L = _lib.lib()
+        sh = ctx.sh
+        st = _stream()
+        dev = gz.device
+        p, idx, alpha, ab, mean, invstd, gamma, ymax, xm, xb, wt, wmask, gscale, inv_gscale = ctx.saved_tensors
+        gname, gcode, gh = ctx.gmode
+        key = _shape_key(sh)
+        cout = sh.Cout
+        i32 = dict(dtype=torch.int32, device=dev)
+        f32 = dict(dtype=torch.float32, device=dev)
+        sums = torch.empty((2 * cout,), dtype=torch.float64, device=dev)
+        gmax, amax = torch.empty((cout,), **i32), torch.empty((1,), **i32)
+        consts, dgamma, dbeta = torch.empty((4 * cout,), **f32), torch.empty((cout,), **f32), torch.empty((cout,), **f32)
+        gys = torch.empty((sh.N, sh.Ho, sh.Wo, gh * cout), dtype=torch.int16, device=dev)
+        n_pool = p.numel()
+        with _timed("pool2_bn_bwd_pack", key, 2 * (4 + 2 + 1) * n_pool + 2 * gys.numel()):
+            _lib.check(L.bdbnn_pool2_bn_bwd_pack(_p(_nhwc(gz)), _p(p), _p(idx), _p(alpha), _p(ab), _p(mean), _p(invstd),
+                                                 _p(gamma), _p(gscale), _p(ymax), sh.N, sh.Ho, sh.Wo, cout, gcode,
+                                                 _p(sums), _p(gmax), _p(consts), _p(dgamma), _p(dbeta), _p(amax),
+                                                 _p(gys), st), "pool2_bn_bwd_pack")
+        _lib.count(3)
+        x_shape, w_shape = ctx.shapes
+        gx = gw = None
+        if ctx.needs_input_grad[1]:
+            gw = _wgrad_tc(sh, gys, gcode, amax, xb, wmask, inv_gscale, w_shape, ctx.w_param, "binconv_wgrad_tc", key,
+                           algorithmic_bytes("wgrad_tc", sh, gh))
+        if ctx.needs_input_grad[0]:
+            gx = torch.empty(x_shape, dtype=torch.float32, device=dev, memory_format=torch.channels_last)
+            with _timed("binconv_dgrad_tc", key, algorithmic_bytes("dgrad_tc", sh, gh)):
+                _lib.check(L.bdbnn_binconv_dgrad_tc(_p(gys), gcode, _p(amax), _p(wt), _p(xm), _p(None), _p(gx),
+                                                    ctypes.byref(sh), st), "binconv_dgrad_tc")
+            _lib.count(_dgrad_launches(sh))
+        return (gx, gw, dgamma if ctx.needs_input_grad[2] else None, dbeta if ctx.needs_input_grad[3] else None,
+                None, None, None, None, None, None, None, None, None)
+
+
+def conv_pool_bn(x, weight, gamma, beta, running_mean, running_var, momentum, eps, padding=1):
+    """z = hardtanh(BN_train(max_pool2d(binconv2d(x, weight, stride 1), 2, 2))) as one node (see pool_unit_supported):
+    the pooled VGG-Small unit.  The winner of each window is the first maximum in scan order, as torch.nn.MaxPool2d's;
+    BatchNorm updates its running statistics (the caller adds 1 to num_batches_tracked).  Like conv_bn_add, x's
+    `_bdbnn_pack` is consumed and the result carries its own, with Hardtanh's strict mask."""
+    fmt = grad_mode()[3]
+    pk = _get_act_pack(x, fmt)
+    xs, xm, xb, xb8 = (pk.sign, pk.mask, pk.xb, pk.xb8) if pk is not None else (None,) * 4
+    z, zs, zm, zb, zb8 = _ConvPoolBNUnit.apply(x, weight, gamma, beta, running_mean, running_var, momentum, eps,
+                                               int(padding), xs, xm, xb, xb8)
+    _set_act_pack(z, _ActPack(zs, zm, zb, fmt, zb8))
+    return z
+
+
+@_on_x_device
+def conv_pool_bn_eval(x, weight, gamma, beta, running_mean, running_var, eps, padding=1):
+    """hardtanh(BN_eval(max_pool2d(binconv2d(x, weight), 2, 2))) under no_grad: the int16 forward, then one kernel for
+    the 2x2 integer max, the folded BatchNorm z = fp32(fp32(max * scale) + shift) (bn_eval_fold with alpha, each step
+    rounded once), Hardtanh and the +-1 copy of z for the next unit (`_bdbnn_eval_pack`, as conv_bn_add_eval)."""
+    _eval_only("conv_pool_bn_eval")
+    _require_cuda(x, "conv_pool_bn_eval(x)")
+    _require_cuda(weight, "conv_pool_bn_eval(weight)")
+    _same_device(x, weight, gamma, beta, running_mean, running_var)
+    if not pool_unit_supported(x.shape, weight.shape, 1, padding):
+        raise RuntimeError(f"bdbnn_b200.conv_pool_bn_eval: unsupported input {tuple(x.shape)} / weight "
+                           f"{tuple(weight.shape)}")
+    L = _lib.lib()
+    sh = conv_shape(x.shape, weight.shape, 1, padding)
+    dev = x.device
+    n, cout, ho, wo = sh.N, sh.Cout, sh.Ho // 2, sh.Wo // 2
+    fmt = grad_mode()[3]
+    st = _stream()
+    key = _shape_key(sh)
+    use8 = bool(int(L.bdbnn_tc_supported(ctypes.byref(sh))) & 8) and use_fwd8(sh.Cin, cout, eval_unit=True)
+    want = -1 if use8 else fmt
+    pk = getattr(x, "_bdbnn_eval_pack", None)
+    if pk is not None and pk[0] == want and x._bdbnn_eval_pack_version == x._version:
+        xop = pk[1]
+    else:
+        ap = _act_pack(x, sh, fmt, xb=not use8, xb8=use8)
+        xop = ap.xb8 if use8 else ap.xb
+    wp = _prepacked(weight, fmt, use8)
+    if wp is None:
+        wp = _alloc_weight_pack(weight.shape, dev, wf=not use8, wf8=use8)
+        _weight_pack(weight, wp, fmt)
+    y = torch.empty((n, sh.Ho, sh.Wo, cout), dtype=torch.int16, device=dev)
+    with _timed("binconv_fwd_tc8" if use8 else "binconv_fwd_tc", key,
+                algorithmic_bytes("fwd_tc8" if use8 else "fwd_tc", sh) - 2 * y.numel()):
+        _lib.check(L.bdbnn_binconv_fwd_tc_i16(_p(xop), _p(wp.wf8) if use8 else _p(wp.wf), want, _p(wp.alpha), _p(y),
+                                              ctypes.byref(sh), None, None, st), "binconv_fwd_tc_i16")
+    _lib.count(1)
+    scale, shift = bn_eval_fold(gamma, beta, running_mean, running_var, eps, wp.alpha)
+    out8 = cout % 128 == 0 and fwd8_enabled()
+    z = torch.empty((n, cout, ho, wo), dtype=torch.float32, device=dev, memory_format=torch.channels_last)
+    zb = None if out8 else torch.empty((n, ho, wo, cout), dtype=torch.int16, device=dev)
+    zb8 = torch.empty((n, ho, wo, cout), dtype=torch.uint8, device=dev) if out8 else None
+    with _timed("pool2_bn_eval_hardtanh", key, 2 * y.numel() + (4 + (1 if out8 else 2)) * z.numel()):
+        _lib.check(L.bdbnn_pool2_bn_eval_hardtanh(_p(y), _p(scale), _p(shift), n, sh.Ho, sh.Wo, cout, _p(z), _p(zb),
+                                                  _p(zb8), fmt, st), "pool2_bn_eval_hardtanh")
+    _lib.count(1)
+    if not z.is_inference():
+        z._bdbnn_eval_pack = (-1, zb8) if out8 else (fmt, zb)
+        z._bdbnn_eval_pack_version = z._version
+    return z

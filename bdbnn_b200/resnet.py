@@ -269,10 +269,11 @@ class BasicBlockCifar(nn.Module):
         return _unit(out, self.conv2, self.bn2, out)
 
 
-def _cifar_stem_qualifies(x, c1, bn):
+def _cifar_stem_qualifies(x, c1, bn, hardtanh=False):
     """Whether the CIFAR stem conv1 + bn1 runs as functional.cifar_stem_conv_bn: training mode on a CUDA fp32 batch
     of 3-channel images that does not require grad, a bias-free 3x3 / stride-1 / pad-1 nn.Conv2d, an affine
-    BatchNorm2d that tracks running statistics, and neither BDBNN_STEM_TC=0 nor BDBNN_FUSE_BN=0."""
+    BatchNorm2d that tracks running statistics, and neither BDBNN_STEM_TC=0 nor BDBNN_FUSE_BN=0.  `hardtanh`: the
+    geometry of the VGG-Small stem (functional.cifar_stem_supported)."""
     if not (type(c1) is nn.Conv2d and isinstance(bn, nn.BatchNorm2d) and bn.training and F_.fuse_enabled() and
             F_.stem_tc_enabled()):
         return False
@@ -283,7 +284,7 @@ def _cifar_stem_qualifies(x, c1, bn):
         return False
     if not (bn.affine and bn.track_running_stats and bn.momentum is not None and bn.num_features == c1.out_channels):
         return False
-    return F_.cifar_stem_supported(tuple(x.shape), tuple(c1.weight.shape), c1.stride, c1.padding)
+    return F_.cifar_stem_supported(tuple(x.shape), tuple(c1.weight.shape), c1.stride, c1.padding, hardtanh)
 
 
 def _cifar_stem(x, c1, bn):

@@ -349,7 +349,45 @@ BDBNN_API int bdbnn_bn_fwd_i16_pad_shortcut(const int16_t* y_int, const float* a
 BDBNN_API int bdbnn_pad_shortcut_bwd(const float* gz, float* gx, int32_t N, int32_t H, int32_t W, int32_t Cin,
                            int32_t Cout, int32_t pad, void* stream);
 
-/* ---- CIFAR stem: 3x3 / stride 1 / pad 1, 3 -> Cout channels (Cout in {16, 32, 48, 64}), fp32, CUDA cores ------
+/* ---- Hardtanh and 2x2 max-pool units of the CIFAR VGG-Small (DESIGN.md §4n) -----------------------------------------
+ * bn_fwd_hardtanh : bdbnn_bn_fwd without residual, then z = hardtanh(u) for the BatchNorm output u (torch.nn.Hardtanh:
+ *          clamp to [-1, 1], NaN stays NaN).  y is int16 (y = alpha[c] * y_int, statistics ready: stats_ready must be 1)
+ *          when alpha != NULL, else fp32.  The packs (needed: sign_bits, mask_bits, xb; C % 32 == 0) are sign(u) and
+ *          mask = (-1 < u < 1), strictly and 0 at NaN: Hardtanh's gradient times the next conv's STE indicator.
+ * bn_bwd_pack_hardtanh : bdbnn_bn_bwd_pack(_i16) of gz * mask, the mask recomputed from y and the forward's ab_ws
+ *          (`ab`, float[2C]); the sums are always computed here.
+ * pool2_i16 : p_int int16 NHWC [N,H/2,W/2,C] = 2x2 / stride-2 max of y_int [N,H,W,C] (H, W even, C % 32 == 0), idx
+ *          uint8 [N,H/2,W/2,C] = the winner's tap dy*2 + dx (first maximum in scan order, as torch.nn.MaxPool2d), and
+ *          the BatchNorm statistics of alpha*p into sums double[2C] / ymax_bits u32[C] (zeroed here; per-block
+ *          partials summed in a fixed order) for bn_fwd_hardtanh(p_int, alpha, n_pix = N*H/2*W/2, stats_ready = 1).
+ * pool2_bn_bwd_pack : the BatchNorm + Hardtanh backward of that unit over the pooled tensor (gz fp32 NHWC
+ *          [N,H/2,W/2,C]), written as gys at the conv-output resolution [N,H,W,(2)C]: the packed value at the winner,
+ *          0 elsewhere (the max-pool backward).  Scratch and outputs as bdbnn_bn_bwd_pack.
+ * pool2_bn_eval_hardtanh : z fp32 NHWC [N,H/2,W/2,C] = hardtanh(fp32(fp32(m * scale[c]) + shift[c])) for m the 2x2
+ *          max of y_int, scale / shift from bdbnn_bn_eval_fold with alpha; optionally the +-1 copy of z, 16-bit in
+ *          format fmt (zb) and / or e4m3 (zb8). */
+BDBNN_API int bdbnn_bn_fwd_hardtanh(const void* y, const float* alpha, const float* gamma, const float* beta,
+                          int64_t n_pix, int32_t C, float eps, float momentum, float* running_mean,
+                          float* running_var, double* sums_ws, uint32_t* ymax_bits, float* mean, float* invstd,
+                          float* ab_ws, float* z, uint32_t* sign_bits, uint32_t* mask_bits, uint16_t* xb,
+                          uint8_t* xb_fp8, int32_t fmt, int32_t stats_ready, void* stream);
+BDBNN_API int bdbnn_bn_bwd_pack_hardtanh(const float* gz, const void* y, const float* alpha, const float* ab,
+                               const float* mean, const float* invstd, const float* gamma, const float* gscale,
+                               const uint32_t* ymax_bits, int64_t n_pix, int32_t C, int32_t grad_mode,
+                               double* sums_ws, uint32_t* gmax_bits, float* consts_ws, float* dgamma, float* dbeta,
+                               uint32_t* amax_bits, uint16_t* gys, void* stream);
+BDBNN_API int bdbnn_pool2_i16(const int16_t* y_int, const float* alpha, int32_t N, int32_t H, int32_t W, int32_t C,
+                    int16_t* p_int, uint8_t* idx, double* sums, uint32_t* ymax_bits, void* stream);
+BDBNN_API int bdbnn_pool2_bn_bwd_pack(const float* gz, const int16_t* p_int, const uint8_t* idx, const float* alpha,
+                            const float* ab, const float* mean, const float* invstd, const float* gamma,
+                            const float* gscale, const uint32_t* ymax_bits, int32_t N, int32_t H, int32_t W, int32_t C,
+                            int32_t grad_mode, double* sums_ws, uint32_t* gmax_bits, float* consts_ws, float* dgamma,
+                            float* dbeta, uint32_t* amax_bits, uint16_t* gys, void* stream);
+BDBNN_API int bdbnn_pool2_bn_eval_hardtanh(const int16_t* y_int, const float* scale, const float* shift, int32_t N,
+                                 int32_t H, int32_t W, int32_t C, float* z, uint16_t* zb, uint8_t* zb8, int32_t fmt,
+                                 void* stream);
+
+/* ---- CIFAR stem: 3x3 / stride 1 / pad 1, 3 -> Cout channels (Cout in {16, 32, 48, 64, 128}), fp32, CUDA cores -
  * Replaces the fp32 nn.Conv2d `conv1` of the CIFAR ResNets (models/cifar10; model(images), train.py:492 and its
  * weight gradient under loss.backward(), train.py:528), which the reference runs on cuDNN.
  *   cifar_stem_fwd   : y fp32 NHWC [N,H,W,Cout] = conv(x, W): one fp32 FMA per tap, taps in the order (c, r, s), no
@@ -373,6 +411,12 @@ BDBNN_API int bdbnn_cifar_stem_fwd(const float* x, int32_t N, int32_t H, int32_t
 BDBNN_API int bdbnn_cifar_stem_fwd_eval(const float* x, int32_t N, int32_t H, int32_t W, int64_t sN, int64_t sC,
                               int64_t sH, int64_t sW, const float* weight, int32_t Cout, const float* scale,
                               const float* shift, float* z, uint32_t* z_amax_bits, void* stream);
+/* cifar_stem_fwd_eval_hardtanh: the same with z = hardtanh(BN_eval(conv)) (torch.nn.Hardtanh, NaN stays NaN) and Cout
+ * in {16, 32, 48, 64, 128}: the eval stem of VGG-Small (DESIGN.md §4n); z_amax_bits is max|z| after the clamp. */
+BDBNN_API int bdbnn_cifar_stem_fwd_eval_hardtanh(const float* x, int32_t N, int32_t H, int32_t W, int64_t sN,
+                                       int64_t sC, int64_t sH, int64_t sW, const float* weight, int32_t Cout,
+                                       const float* scale, const float* shift, float* z, uint32_t* z_amax_bits,
+                                       void* stream);
 BDBNN_API size_t bdbnn_cifar_stem_wgrad_workspace_bytes(int32_t N, int32_t H, int32_t W, int32_t Cout);
 BDBNN_API int bdbnn_cifar_stem_wgrad(const float* x, int32_t N, int32_t H, int32_t W, int64_t sN, int64_t sC,
                            int64_t sH, int64_t sW, const uint16_t* gys, const uint32_t* g_amax_bits, int32_t Cout,
