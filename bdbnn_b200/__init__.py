@@ -4,9 +4,9 @@ from .modules import BinarizeConv2d, HardBinaryConv, HardBinaryConv_react, HardB
 from .losses import (KurtosisWeight, DistributionLoss, DistributionLoss_layer,
                      kurtosis_regularization, matched_weight_pairs)
 from .functional import binconv2d, kurtosis_multi, kd_logits_loss, kd_layer_loss
-from .teacher import FrozenResNetTeacher
+from .teacher import FrozenResNetTeacher, FrozenVGGTeacher
 
 __all__ = ["BinarizeConv2d", "HardBinaryConv", "HardBinaryConv_react", "HardBinaryConv_cifar",
            "KurtosisWeight", "DistributionLoss", "DistributionLoss_layer", "kurtosis_regularization",
            "matched_weight_pairs", "binconv2d", "kurtosis_multi", "kd_logits_loss", "kd_layer_loss",
-           "FrozenResNetTeacher"]
+           "FrozenResNetTeacher", "FrozenVGGTeacher"]

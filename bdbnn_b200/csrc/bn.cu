@@ -447,6 +447,7 @@ bn_bwd_pack_kernel(const float4* __restrict__ gz, const void* __restrict__ y, co
 //   pool2_bwd_pack_kernel : the BatchNorm backward on the pooled tensor (gz times Hardtanh's mask) written as the conv
 //                           backward's 16-bit operand at the conv-output resolution: the value at the winner, 0 elsewhere
 //   pool2_eval_kernel     : z = hardtanh(fp32(fp32(max * scale) + shift)) from the folded eval BatchNorm, + the +-1 copy
+//   real_pool2_eval_kernel: the same on the fp32 output of a real-valued conv (the fp32 VGG-Small teacher), + max|z|
 __device__ __forceinline__ int4 pool2_quad(const int16_t* __restrict__ y, int64_t off) {
   const uint2 r = __ldcs(reinterpret_cast<const uint2*>(y + off));
   return make_int4(int16_t(r.x & 0xffffu), int16_t(r.x >> 16), int16_t(r.y & 0xffffu), int16_t(r.y >> 16));
@@ -562,6 +563,26 @@ pool2_bwd_pack_kernel(const float4* __restrict__ gz, const int16_t* __restrict__
   }
 }
 
+// fp32 y: the max of the window as F.max_pool2d takes it (scan order, `v > m || v is NaN`): NaN if the window holds
+// one, and of equal values (+0.0 / -0.0) the first
+__device__ __forceinline__ float pool2_fmax(float m, float v) { return (v > m || v != v) ? v : m; }
+
+__device__ __forceinline__ float4 pool2_max_f32(const float* __restrict__ y, int64_t n, int ho, int wo, int H, int W,
+                                                int C, int c4) {
+  float4 m;
+#pragma unroll
+  for (int t = 0; t < 4; ++t) {
+    const int64_t off = ((n * H + 2 * ho + (t >> 1)) * W + 2 * wo + (t & 1)) * C + 4 * c4;
+    const float4 v = __ldcs(reinterpret_cast<const float4*>(y + off));
+    if (t == 0) {
+      m = v;
+    } else {
+      m.x = pool2_fmax(m.x, v.x); m.y = pool2_fmax(m.y, v.y); m.z = pool2_fmax(m.z, v.z); m.w = pool2_fmax(m.w, v.w);
+    }
+  }
+  return m;
+}
+
 __global__ void __launch_bounds__(kBnThreads)
 pool2_eval_kernel(const int16_t* __restrict__ y, const float* __restrict__ scale, const float* __restrict__ shift,
                   int H, int W, int C4, int64_t n4, float4* __restrict__ z, uint2* __restrict__ zb,
@@ -592,6 +613,36 @@ pool2_eval_kernel(const int16_t* __restrict__ y, const float* __restrict__ scale
     if (zb8 != nullptr)
       zb8[i] = 0x38383838u | ((s0 ? 0u : 0x80u) | (s1 ? 0u : 0x8000u) | (s2 ? 0u : 0x800000u) | (s3 ? 0u : 0x80000000u));
   }
+}
+
+// pool2_eval_kernel on an fp32 conv output (a kernel of its own, so that the int16 one keeps its code): no +-1 copy,
+// the bits of max|z| into z_amax instead (integer atomicMax, NaN on top: run-to-run identical)
+__global__ void __launch_bounds__(kBnThreads)
+real_pool2_eval_kernel(const float* __restrict__ y, const float* __restrict__ scale, const float* __restrict__ shift,
+                       int H, int W, int C4, int64_t n4, float4* __restrict__ z, uint32_t* __restrict__ z_amax) {
+  const int64_t nthreads = int64_t(gridDim.x) * blockDim.x;       // multiple of C4
+  int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  const int c4 = int(i % C4);
+  const int Ho = H / 2, Wo = W / 2;
+  const float4 sc = *reinterpret_cast<const float4*>(scale + c4 * 4);
+  const float4 sf = *reinterpret_cast<const float4*>(shift + c4 * 4);
+  uint32_t zmax = 0u;
+  for (; i < n4; i += nthreads) {
+    const int64_t q = i / C4;
+    const int wo = int(q % Wo);
+    const int64_t r = q / Wo;
+    const float4 m = pool2_max_f32(y, r / Ho, int(r % Ho), wo, H, W, C4 * 4, c4);
+    float4 o;
+    o.x = htanh(__fadd_rn(__fmul_rn(m.x, sc.x), sf.x));
+    o.y = htanh(__fadd_rn(__fmul_rn(m.y, sc.y), sf.y));
+    o.z = htanh(__fadd_rn(__fmul_rn(m.z, sc.z), sf.z));
+    o.w = htanh(__fadd_rn(__fmul_rn(m.w, sc.w), sf.w));
+    z[i] = o;
+    zmax = max(zmax, max(max(__float_as_uint(fabsf(o.x)), __float_as_uint(fabsf(o.y))),
+                         max(__float_as_uint(fabsf(o.z)), __float_as_uint(fabsf(o.w)))));
+  }
+  zmax = __reduce_max_sync(0xffffffffu, zmax);      // every lane of the (whole) warp gets here
+  if ((threadIdx.x & 31) == 0 && zmax != 0u) atomicMax(z_amax, zmax);
 }
 
 static int bn_grid(int64_t work, int C4, int per_sm = 8) {
@@ -995,6 +1046,21 @@ extern "C" int bdbnn_pool2_bn_eval_hardtanh(const int16_t* y_int, const float* s
                                                            reinterpret_cast<uint32_t*>(zb8),
                                                            fmt == BDBNN_FMT_FP16 ? 0x3C00u : 0x3F80u);
   return check_launch("pool2_eval_kernel");
+}
+
+extern "C" int bdbnn_real_pool2_bn_eval_hardtanh(const float* y, const float* scale, const float* shift, int32_t N,
+                                                 int32_t H, int32_t W, int32_t C, float* z, uint32_t* z_amax_bits,
+                                                 void* stream) {
+  int rc = pool2_dims_ok("real_pool2_bn_eval_hardtanh", N, H, W, C);
+  if (rc) return rc;
+  BDBNN_REQUIRE(y && scale && shift && z && z_amax_bits, "real_pool2_bn_eval_hardtanh: NULL pointer");
+  cudaStream_t st = cudaStream_t(stream);
+  const int C4 = C / 4;
+  const int64_t n4 = int64_t(N) * (H / 2) * (W / 2) * C4;
+  BDBNN_CUDA(cudaMemsetAsync(z_amax_bits, 0, sizeof(uint32_t), st));
+  real_pool2_eval_kernel<<<bn_grid(n4, C4), kBnThreads, 0, st>>>(y, scale, shift, H, W, C4, n4,
+                                                                 reinterpret_cast<float4*>(z), z_amax_bits);
+  return check_launch("real_pool2_eval_kernel");
 }
 
 extern "C" int bdbnn_bn_bwd_pack_i16(const float* gz, const int16_t* y_int, const float* alpha, const float* mean,

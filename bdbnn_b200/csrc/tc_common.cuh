@@ -378,6 +378,7 @@ struct TcConvLaunch {
   // eval forward (MODE 2): z = acc * alpha + shift (+ add) written to `out`, optional +-1 copies of z
   const float* shift; uint16_t* zb; uint8_t* zb8;
   int relu;                      // eval: z = relu(z) after the residual
+  int hardtanh;                  // eval, fp16 operands, no option-A residual: z = clamp(z, -1, 1) instead of relu
   uint32_t* z_amax;              // eval: optional bits of max|z| (zeroed by the caller)
   // forward only: per-output-channel BatchNorm statistics of the result, accumulated by the epilogue
   // (sum y, sum y^2 as doubles [2*Nout]; max|y| bits [Nout]); NULL = off.  Zeroed by the caller.

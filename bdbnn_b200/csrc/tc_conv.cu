@@ -81,7 +81,9 @@ __device__ __forceinline__ void wgmma_k_block(float (&acc)[NW / 2], uint32_t a_s
 // 96 without it (0 = no minimum).  bdbnn_debug_tc_conv_ctas_per_sm reports the residency.
 // PADRES (MODE 2, 16-bit operands only): the residual is the CIFAR option-A shortcut read in place (res_* fields),
 // an instance of its own so that the dense-residual instances keep their code.
-template <int MODE, int KIND, int NW, bool PADRES = false>
+// HARDTANH (MODE 2, fp16 operands, no PADRES): z = hardtanh(z) where relu would apply (p.relu is not read), the
+// VGG-Small teacher's unpooled convs; instances of their own for the same reason.
+template <int MODE, int KIND, int NW, bool PADRES = false, bool HARDTANH = false>
 __global__ void __launch_bounds__(kTcThreads, MODE == 0 ? 0 : 2)
 tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const TcConvParams p) {
@@ -249,7 +251,10 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             const float2 r = __ldg(reinterpret_cast<const float2*>(p.add + off));
             o0 = __fadd_rn(o0, r.x); o1 = __fadd_rn(o1, r.y);
           }
-          if (p.relu) {                    // torch.relu: NaN stays NaN (fmaxf alone would drop it)
+          if (HARDTANH) {                  // torch.nn.Hardtanh: NaN stays NaN, -0.0 stays -0.0
+            o0 = o0 < -1.f ? -1.f : (o0 > 1.f ? 1.f : o0);
+            o1 = o1 < -1.f ? -1.f : (o1 > 1.f ? 1.f : o1);
+          } else if (p.relu) {             // torch.relu: NaN stays NaN (fmaxf alone would drop it)
             o0 = o0 != o0 ? o0 : fmaxf(o0, 0.f);
             o1 = o1 != o1 ? o1 : fmaxf(o1, 0.f);
           }
@@ -435,18 +440,18 @@ static int launch_one(K kern, dim3 grid, size_t smem, cudaStream_t st, const CUt
 
 // The instance for an N tile of bn columns (16, 32, 64 or 128).
 using TcConvKernel = decltype(&tc_conv_kernel<0, 0, 16, false>);
-template <int MODE, int KIND, bool PADRES = false>
+template <int MODE, int KIND, bool PADRES = false, bool HARDTANH = false>
 static TcConvKernel kernel_for(int bn) {
-  return bn == 16   ? tc_conv_kernel<MODE, KIND, 16, PADRES>
-         : bn == 32 ? tc_conv_kernel<MODE, KIND, 32, PADRES>
-         : bn == 64 ? tc_conv_kernel<MODE, KIND, 64, PADRES>
-                    : tc_conv_kernel<MODE, KIND, 128, PADRES>;
+  return bn == 16   ? tc_conv_kernel<MODE, KIND, 16, PADRES, HARDTANH>
+         : bn == 32 ? tc_conv_kernel<MODE, KIND, 32, PADRES, HARDTANH>
+         : bn == 64 ? tc_conv_kernel<MODE, KIND, 64, PADRES, HARDTANH>
+                    : tc_conv_kernel<MODE, KIND, 128, PADRES, HARDTANH>;
 }
 
-template <int MODE, int KIND, bool PADRES = false>
+template <int MODE, int KIND, bool PADRES = false, bool HARDTANH = false>
 static int launch_kind(const CUtensorMap& tmA, const CUtensorMap& tmB, const TcConvParams& p, size_t smem, dim3 grid,
                        cudaStream_t st) {
-  const TcConvKernel kern = kernel_for<MODE, KIND, PADRES>(p.BN);
+  const TcConvKernel kern = kernel_for<MODE, KIND, PADRES, HARDTANH>(p.BN);
   BDBNN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
   if (p.bn_sums == nullptr) return launch_one(kern, grid, smem, st, tmA, tmB, p);
   TcConvParams q = p;
@@ -490,6 +495,13 @@ static int launch_tc_conv(const TcConvLaunch& L, cudaStream_t st) {
     }
   }
   if constexpr (MODE == 2) {
+    if (L.hardtanh) {
+      if (L.pad_res || L.fmt != BDBNN_FMT_FP16) {
+        set_error("tc_conv: the Hardtanh epilogue takes fp16 operands without the option-A residual");
+        return BDBNN_ERR_UNSUPPORTED;
+      }
+      return launch_kind<2, 0, false, true>(tmA, tmB, p, smem, grid, st);
+    }
     if (L.pad_res)
       return L.fmt == BDBNN_FMT_BF16 ? launch_kind<2, 1, true>(tmA, tmB, p, smem, grid, st)
                                      : launch_kind<2, 0, true>(tmA, tmB, p, smem, grid, st);
@@ -609,14 +621,18 @@ extern "C" int bdbnn_debug_conv_plan(const bdbnn_conv_shape* s, int32_t mode, in
 
 // CTAs of one tc_conv_kernel instance that fit on an SM with `smem` bytes of dynamic shared memory (the dynamic smem
 // entry of bdbnn_debug_conv_plan).  mode 0 forward / 1 dgrad / 2 eval forward / 3 eval forward with the option-A
-// residual, fmt BDBNN_FMT_FP16 / BF16 or -1 (fp8, forward and dense eval only), bn = N tile (16, 32, 64 or 128).
+// residual / 5 eval forward with the Hardtanh epilogue (4 is not a mode), fmt BDBNN_FMT_FP16 / BF16 or -1 (fp8,
+// forward and dense eval only; mode 5 takes fp16 only), bn = N tile (16, 32, 64 or 128).
 extern "C" int bdbnn_debug_tc_conv_ctas_per_sm(int32_t mode, int32_t fmt, int32_t bn, int32_t smem, int32_t* ctas) {
-  BDBNN_REQUIRE(ctas && mode >= 0 && mode <= 3 && (bn == 16 || bn == 32 || bn == 64 || bn == 128) && smem >= 0 &&
-                    (fmt == BDBNN_FMT_FP16 || fmt == BDBNN_FMT_BF16 || (fmt == -1 && (mode == 0 || mode == 2))),
+  BDBNN_REQUIRE(ctas && ((mode >= 0 && mode <= 3) || mode == 5) && (bn == 16 || bn == 32 || bn == 64 || bn == 128) &&
+                    smem >= 0 &&
+                    (fmt == BDBNN_FMT_FP16 || fmt == BDBNN_FMT_BF16 || (fmt == -1 && (mode == 0 || mode == 2))) &&
+                    (mode != 5 || fmt == BDBNN_FMT_FP16),
                 "debug_tc_conv_ctas_per_sm: bad arguments");
   const int kind = fmt == -1 ? 2 : (fmt == BDBNN_FMT_BF16 ? 1 : 0);
   TcConvKernel kern;
-  if (mode == 3) kern = kind == 0 ? kernel_for<2, 0, true>(bn) : kernel_for<2, 1, true>(bn);
+  if (mode == 5) kern = kernel_for<2, 0, false, true>(bn);
+  else if (mode == 3) kern = kind == 0 ? kernel_for<2, 0, true>(bn) : kernel_for<2, 1, true>(bn);
   else if (mode == 2) kern = kind == 2 ? kernel_for<2, 2>(bn) : kind == 0 ? kernel_for<2, 0>(bn) : kernel_for<2, 1>(bn);
   else if (mode == 0) kern = kind == 2 ? kernel_for<0, 2>(bn) : kind == 0 ? kernel_for<0, 0>(bn) : kernel_for<0, 1>(bn);
   else kern = kind == 0 ? kernel_for<1, 0>(bn) : kernel_for<1, 1>(bn);
@@ -745,11 +761,13 @@ extern "C" int bdbnn_binconv_fwd_tc_eval(const void* xb, const void* wf, int32_t
 // Eval-mode forward of a real-valued conv on fp16 operands (xh = fp16(x * 2^ex), wf = fp16(W * 2^ew)) — see
 // include/bdbnn.h.
 extern "C" int bdbnn_real_conv_fwd_eval(const uint16_t* xh, const uint32_t* x_amax_bits, const uint16_t* wf,
-                                        const float* scale, const float* shift, const float* residual, int32_t relu,
+                                        const float* scale, const float* shift, const float* residual, int32_t act,
                                         float* z, uint32_t* z_amax_bits, const bdbnn_conv_shape* s, void* stream) {
   int rc = validate_shape(s);
   if (rc) return rc;
   BDBNN_REQUIRE(xh && x_amax_bits && wf && scale && shift && z, "real_conv_fwd_eval: NULL pointer");
+  BDBNN_REQUIRE(act >= BDBNN_ACT_NONE && act <= BDBNN_ACT_HARDTANH,
+                "real_conv_fwd_eval: act must be 0 (none), 1 (ReLU) or 2 (Hardtanh), got %d", act);
   BDBNN_REQUIRE(residual != z, "real_conv_fwd_eval: residual must not alias z");
   if (!tc_shape_ok(s)) {
     set_error("real_conv_fwd_eval: shape not supported by the tensor-core path");
@@ -759,7 +777,8 @@ extern "C" int bdbnn_real_conv_fwd_eval(const uint16_t* xh, const uint32_t* x_am
   TcConvLaunch L;
   fwd_launch(&L, xh, wf, BDBNN_FMT_FP16, s);
   L.amax_bits = x_amax_bits;
-  L.alpha = scale; L.shift = shift; L.add = residual; L.out = z; L.relu = relu != 0; L.z_amax = z_amax_bits;
+  L.alpha = scale; L.shift = shift; L.add = residual; L.out = z; L.z_amax = z_amax_bits;
+  L.relu = act == BDBNN_ACT_RELU; L.hardtanh = act == BDBNN_ACT_HARDTANH;
   if (z_amax_bits) BDBNN_CUDA(cudaMemsetAsync(z_amax_bits, 0, sizeof(uint32_t), st));
   return launch_tc_conv<2>(L, st);
 }

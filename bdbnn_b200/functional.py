@@ -16,6 +16,7 @@ _IMPL_ENV = "BDBNN_IMPL"          # auto | xnor | tc
 _GRAD_ENV = "BDBNN_GRAD_MODE"     # fp16s (default) | bf16x2 | bf16  — rounding of gy*gscale (include/bdbnn.h)
 GRAD_MODES = {"bf16": 1, "bf16x2": 2, "fp16s": 3}
 FMT_FP16, FMT_BF16 = 0, 1
+ACT_NONE, ACT_RELU, ACT_HARDTANH = 0, 1, 2     # activation codes of bdbnn_real_conv_fwd_eval (include/bdbnn.h)
 
 
 def grad_mode():
@@ -1975,15 +1976,21 @@ def real_weight_pack(weights):
 
 @_on_x_device
 def real_conv_bn_eval(x, x_amax, wpack, gamma, beta, running_mean, running_var, eps, stride, padding, residual=None,
-                      relu=True, shortcut=None):
+                      relu=True, shortcut=None, hardtanh=False):
     """z = relu(BN_eval(conv2d(x, W)) + residual) of a real-valued conv under no_grad, with wpack = (wf, alpha) of
     real_weight_pack(W): real_act_pack -> fold(alpha) -> real_conv_fwd_eval.  x fp32 CUDA (channels_last avoids a
     copy); x_amax = the device word of max|x| a previous call returned (None: computed here, one more pass over x).
     `shortcut` = PadShortcut(pad) takes the option-A shortcut of x, F.pad(x[:, :, ::2, ::2]) with `pad` zero
     channels on each side, as the residual: the epilogue reads x in place (real_conv_fwd_eval_pad_shortcut), no
     padded tensor is written, and z is bit-identical to passing that tensor as `residual`.
+    `hardtanh` (with relu=False, without `shortcut`): z = hardtanh(BN_eval(conv2d(x, W)) + residual) in the same
+    epilogue, torch.nn.Hardtanh() bit for bit.
     Returns (z fp32 channels_last, z_amax int32[1] = bits of max|z|)."""
     _eval_only("real_conv_bn_eval")
+    if hardtanh and relu:
+        raise ValueError("bdbnn_b200.real_conv_bn_eval: pass relu=False with hardtanh=True")
+    if hardtanh and shortcut is not None:
+        raise ValueError("bdbnn_b200.real_conv_bn_eval: the Hardtanh epilogue takes no option-A shortcut")
     _require_cuda(x, "real_conv_bn_eval(x)")
     wf, alpha = wpack
     _same_device(x, wf, gamma, beta, running_mean, running_var, residual)
@@ -2023,9 +2030,61 @@ def real_conv_bn_eval(x, x_amax, wpack, gamma, beta, running_mean, running_var, 
     else:
         with _timed("real_conv_fwd_eval", key,
                     algorithmic_bytes("fwd_tc_eval", sh) + (4 * n_out if rc is not None else 0)):
-            _lib.check(L.bdbnn_real_conv_fwd_eval(_p(xh), _p(amax), _p(wf), _p(scale), _p(shift), _p(rc),
-                                                  int(bool(relu)), _p(z), _p(z_amax), ctypes.byref(sh), st),
-                       "real_conv_fwd_eval")
+            act = ACT_HARDTANH if hardtanh else (ACT_RELU if relu else ACT_NONE)
+            _lib.check(L.bdbnn_real_conv_fwd_eval(_p(xh), _p(amax), _p(wf), _p(scale), _p(shift), _p(rc), act, _p(z),
+                                                  _p(z_amax), ctypes.byref(sh), st), "real_conv_fwd_eval")
+    _lib.count(1)
+    return z, z_amax
+
+
+@_on_x_device
+def real_conv_pool_bn_eval(x, x_amax, wpack, gamma, beta, running_mean, running_var, eps, padding=1):
+    """z = hardtanh(BN_eval(max_pool2d(conv2d(x, W, stride 1), 2, 2))) of a real-valued conv under no_grad, the pooled
+    unit of the fp32 VGG-Small teacher: real_act_pack -> real_conv_fwd_eval with scale = alpha, shift = 0 and no
+    activation, so that y = fp32(fp32(acc * 2^-ex) * alpha) is the conv output (alpha a power of two: exact) -> fold
+    (alpha = 1) -> real_pool2_bn_eval_hardtanh: z = hardtanh(fp32(fp32(max * scale) + shift)) for max the window's
+    maximum of y, as F.max_pool2d takes it (NaN wins).  The BatchNorm follows the max, as in the model (gamma may be
+    negative).  wpack, x_amax as real_conv_bn_eval.  Returns (z fp32 channels_last [N,Cout,H/2,W/2], z_amax int32[1] =
+    bits of max|z|)."""
+    _eval_only("real_conv_pool_bn_eval")
+    _require_cuda(x, "real_conv_pool_bn_eval(x)")
+    wf, alpha = wpack
+    _same_device(x, wf, gamma, beta, running_mean, running_var)
+    L = _lib.lib()
+    n, cin, h, w = x.shape
+    cout, taps, cin_w = wf.shape
+    k = int(round(taps ** 0.5))
+    sh = conv_shape(x.shape, (cout, cin_w, k, k), 1, padding)
+    if not int(L.bdbnn_tc_supported(ctypes.byref(sh))) & 1:
+        raise RuntimeError("bdbnn_b200.real_conv_pool_bn_eval: the wgmma forward does not support this shape")
+    if sh.Ho % 2 or sh.Wo % 2 or cout % 32:
+        raise RuntimeError(f"bdbnn_b200.real_conv_pool_bn_eval: the 2x2 pool needs an even conv output and Cout % 32 "
+                           f"== 0, got {sh.Ho}x{sh.Wo}, Cout {cout}")
+    dev = x.device
+    st = _stream()
+    key = _shape_key(sh)
+    xc = _nhwc(x.detach())
+    xh = torch.empty((n, h, w, cin), dtype=torch.int16, device=dev)
+    have = x_amax is not None
+    amax = x_amax if have else torch.empty((1,), dtype=torch.int32, device=dev)
+    n_in = xc.numel()
+    with _timed("real_act_pack", key, 4 * n_in + 2 * n_in):
+        _lib.check(L.bdbnn_real_act_pack(_p(xc), n * h * w, cin, _p(amax), int(have), _p(xh), st), "real_act_pack")
+    _lib.count(1 if have else 2)
+    y = torch.empty((n, sh.Ho, sh.Wo, cout), dtype=torch.float32, device=dev)
+    # -0.0 is the identity of fp32 addition (+0.0 would turn a -0.0 conv output into +0.0 and move a pool's tie)
+    no_shift = torch.full((cout,), -0.0, dtype=torch.float32, device=dev)
+    with _timed("real_conv_fwd_eval", key, algorithmic_bytes("fwd_tc_eval", sh)):
+        _lib.check(L.bdbnn_real_conv_fwd_eval(_p(xh), _p(amax), _p(wf), _p(alpha), _p(no_shift), None, ACT_NONE, _p(y),
+                                              None, ctypes.byref(sh), st), "real_conv_fwd_eval")
+    _lib.count(1)
+    scale, shift = bn_eval_fold(gamma, beta, running_mean, running_var, eps)
+    z = torch.empty((n, cout, sh.Ho // 2, sh.Wo // 2), dtype=torch.float32, device=dev,
+                    memory_format=torch.channels_last)
+    z_amax = torch.empty((1,), dtype=torch.int32, device=dev)
+    with _timed("real_pool2_bn_eval_hardtanh", key, 4 * y.numel() + 4 * z.numel()):
+        _lib.check(L.bdbnn_real_pool2_bn_eval_hardtanh(_p(y), _p(scale), _p(shift), n, sh.Ho, sh.Wo, cout, _p(z),
+                                                       _p(z_amax), st), "real_pool2_bn_eval_hardtanh")
     _lib.count(1)
     return z, z_amax
 

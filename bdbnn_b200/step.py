@@ -24,7 +24,7 @@ import torch.nn.functional as F
 
 from . import losses as _losses
 from .modules import HardBinaryConv, HardBinaryConv_cifar, HardBinaryConv_react
-from .teacher import FrozenResNetTeacher
+from .teacher import _FrozenTeacher
 
 IMAGENET_DIFFKURT = [1.8, 1.4, 1.4, 1.4, 1.4, 1.2, 1.4, 1.2, 1.2, 1.4,
                      1.4, 1.4, 1.2, 1.2, 1.2, 1.2, 1.4, 1, 1]                      # train.py:467-470
@@ -243,7 +243,7 @@ class TrainStep:
             from .functional import _timed
             if t_stream is not None:
                 torch.cuda.current_stream().wait_stream(t_stream)
-            elif isinstance(self.teacher, FrozenResNetTeacher):
+            elif isinstance(self.teacher, _FrozenTeacher):
                 with torch.no_grad():                                             # its kernels time themselves
                     output_teacher = self.teacher(images)                         # train.py:603
             else:

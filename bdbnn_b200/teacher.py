@@ -3,8 +3,10 @@
     teacher = FrozenResNetTeacher(torchvision.models.resnet18())      # or resnet34
     teacher = FrozenResNetTeacher(resnet.ResNetCifar(3, conv_cls=nn.Conv2d))   # the CIFAR KD step's ResNet-20
     teacher = FrozenResNetTeacher(resnet.resnet18_cifar(conv_cls=nn.Conv2d))   # ... and its ResNet-18 (the default)
+    teacher = FrozenVGGTeacher(vgg.vgg_small(conv_cls=lambda i, o, k, s, p: nn.Conv2d(i, o, k, s, p, bias=False)))
 
-wraps a torchvision BasicBlock ResNet, or an fp32 CIFAR ResNet of bdbnn_b200.resnet, without copying it: the wrapper's children ARE the model's children, so
+wraps a torchvision BasicBlock ResNet, an fp32 CIFAR ResNet of bdbnn_b200.resnet, or the fp32 VGG-Small of
+bdbnn_b200.vgg, without copying it: the wrapper's children ARE the model's children, so
 `named_modules()`, `named_parameters()` and `state_dict()` have exactly the model's names (DistributionLoss_layer pairs
 teacher and student convs by name), the parameters are the same objects, and `.cuda()`, `.to()`, `.eval()` and
 `load_state_dict` act on the model.
@@ -14,7 +16,9 @@ In eval mode on a CUDA fp32 input, with no autograd graph to record, the forward
 §4h); avgpool and fc stay in torch.  The CIFAR ResNet has no ReLU; its stem conv + BatchNorm runs as one fp32
 CUDA-core launch and its option-A shortcuts are read in place by conv1's epilogue (DESIGN.md §4j).  The CIFAR
 ResNet-18 has the same stem and no ReLU; each of its 1x1 `downsample` branches runs on the shortcut eval GEMM and is
-conv1's residual (DESIGN.md §4k).  Anything else returns the wrapped model's own forward."""
+conv1's residual (DESIGN.md §4k).  VGG-Small's Hardtanh is in the epilogue of its stem and of its unpooled convs; its
+pooled convs write their fp32 output and one more kernel takes the 2x2 max, BatchNorm and Hardtanh (DESIGN.md §4o).
+Anything else returns the wrapped model's own forward."""
 import ctypes
 from typing import NamedTuple
 
@@ -24,6 +28,7 @@ import torch.nn as nn
 from . import _lib
 from . import functional as F_
 from .resnet import BasicBlock, BasicBlockCifar, ResNetCifar, ResNetCifar18, _PadShortcut
+from .vgg import VGGSmall
 
 
 class _Family(NamedTuple):
@@ -63,17 +68,17 @@ def _bn_args(bn):
     return bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps
 
 
-def _check_bn(bn, where):
+def _check_bn(bn, where, who="FrozenResNetTeacher"):
     if type(bn) is not nn.BatchNorm2d:
-        raise TypeError(f"FrozenResNetTeacher: {where} must be nn.BatchNorm2d, got {type(bn).__name__}")
+        raise TypeError(f"{who}: {where} must be nn.BatchNorm2d, got {type(bn).__name__}")
 
 
-def _check_conv(conv, where, k, bias=False):
+def _check_conv(conv, where, k, bias=False, who="FrozenResNetTeacher", net="a BasicBlock ResNet"):
     if type(conv) is not nn.Conv2d:
-        raise TypeError(f"FrozenResNetTeacher: {where} must be nn.Conv2d, got {type(conv).__name__}")
+        raise TypeError(f"{who}: {where} must be nn.Conv2d, got {type(conv).__name__}")
     if (conv.kernel_size != (k, k) or conv.groups != 1 or conv.dilation != (1, 1) or (conv.bias is not None) != bias
             or conv.padding_mode != "zeros" or conv.stride[0] != conv.stride[1] or conv.padding[0] != conv.padding[1]):
-        raise TypeError(f"FrozenResNetTeacher: {where} is not a {k}x{k} conv of a BasicBlock ResNet")
+        raise TypeError(f"{who}: {where} is not a {k}x{k} conv of {net}")
 
 
 def _check_stem(model, fam):
@@ -163,21 +168,17 @@ def _blocks(model):
     return fam, out
 
 
-class FrozenResNetTeacher(nn.Module):
-    """A torchvision resnet18 / resnet34 teacher, or an fp32 CIFAR ResNet (ResNetCifar with nn.Conv2d convs, any
-    depth and class count, or ResNetCifar18 with nn.Conv2d convs, any class count), whose eval forward runs on the
-    real-valued eval kernels.  Raises TypeError for any other structure (Bottleneck, binary convs, nn.DataParallel,
-    custom blocks)."""
+class _FrozenTeacher(nn.Module):
+    """What the frozen teachers share: the wrapped model's children adopted as this module's own (same names, same
+    parameter objects), `wrapped` and `train`, the conditions of the kernel path that do not depend on the network,
+    and the device guard of the forward.  A subclass checks the structure before calling __init__ and supplies
+    _geometry_supported(x) (host-only, cached) and _kernel_forward(x)."""
 
     def __init__(self, model):
         super().__init__()
-        family, blocks = _blocks(model)
-        self.__dict__["_family"] = family
         self.__dict__["_wrapped"] = model      # not a submodule: no "_wrapped." prefix in the names
         for name, child in model.named_children():
             self.add_module(name, child)
-        self.__dict__["_blocks"] = [blk for _, blk in blocks]
-        self.__dict__["_convs"] = [c for blk in self._blocks for c in (blk.conv1, blk.conv2)]
         self.__dict__["_geom_ok"] = {}
         self.training = model.training
 
@@ -185,6 +186,50 @@ class FrozenResNetTeacher(nn.Module):
     def wrapped(self):
         """The model this teacher runs."""
         return self._wrapped
+
+    def train(self, mode=True):
+        super().train(mode)
+        self._wrapped.training = mode
+        return self
+
+    def _bns(self):
+        return [m for m in self.modules() if isinstance(m, nn.BatchNorm2d)]
+
+    def kernel_path(self, x):
+        """True when forward(x) runs on the eval kernels (see the module docstring)."""
+        if not (torch.is_tensor(x) and x.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and x.shape[1] == 3):
+            return False
+        if self.training:
+            return False
+        for bn in self._bns():
+            if bn.training or not bn.affine or not bn.track_running_stats or bn.running_mean is None:
+                return False
+        if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters())):
+            return False
+        if any(p.device != x.device or p.dtype != torch.float32 for p in self.parameters()):
+            return False
+        return self._geometry_supported(x)
+
+    def forward(self, x):
+        if not self.kernel_path(x):
+            return self._wrapped(x)
+        # every launch, the weight pack and the torch head included, goes to x's device, whichever device is current
+        with torch.no_grad(), torch.cuda.device(x.device):
+            return self._kernel_forward(x)
+
+
+class FrozenResNetTeacher(_FrozenTeacher):
+    """A torchvision resnet18 / resnet34 teacher, or an fp32 CIFAR ResNet (ResNetCifar with nn.Conv2d convs, any
+    depth and class count, or ResNetCifar18 with nn.Conv2d convs, any class count), whose eval forward runs on the
+    real-valued eval kernels.  Raises TypeError for any other structure (Bottleneck, binary convs, nn.DataParallel,
+    custom blocks)."""
+
+    def __init__(self, model):
+        family, blocks = _blocks(model)
+        super().__init__(model)
+        self.__dict__["_family"] = family
+        self.__dict__["_blocks"] = [blk for _, blk in blocks]
+        self.__dict__["_convs"] = [c for blk in self._blocks for c in (blk.conv1, blk.conv2)]
 
     @property
     def _cifar(self):
@@ -194,15 +239,7 @@ class FrozenResNetTeacher(nn.Module):
     def _cifar18(self):
         return self._family is _CIFAR18
 
-    def train(self, mode=True):
-        super().train(mode)
-        self._wrapped.training = mode
-        return self
-
     # ---- path selection ----------------------------------------------------------------------------------------
-    def _bns(self):
-        return [m for m in self.modules() if isinstance(m, nn.BatchNorm2d)]
-
     def _pool_args(self):
         """(kernel_size, stride, padding) of the stem max-pool as ints, or None when one of them is not square."""
         mp = self.maxpool
@@ -260,29 +297,7 @@ class FrozenResNetTeacher(nn.Module):
                 ok = ok and fwd_ok(F_.conv_shape(sampled, sc[0].weight.shape, 1, 0))
         return ok
 
-    def kernel_path(self, x):
-        """True when forward(x) runs on the eval kernels (see the module docstring)."""
-        if not (torch.is_tensor(x) and x.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and x.shape[1] == 3):
-            return False
-        if self.training:
-            return False
-        for bn in self._bns():
-            if bn.training or not bn.affine or not bn.track_running_stats or bn.running_mean is None:
-                return False
-        if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters())):
-            return False
-        if any(p.device != x.device or p.dtype != torch.float32 for p in self.parameters()):
-            return False
-        return self._geometry_supported(x)
-
     # ---- forward -----------------------------------------------------------------------------------------------
-    def forward(self, x):
-        if not self.kernel_path(x):
-            return self._wrapped(x)
-        # every launch, the weight pack and the torch head included, goes to x's device, whichever device is current
-        with torch.no_grad(), torch.cuda.device(x.device):
-            return self._kernel_forward(x)
-
     def _kernel_forward(self, x):
         fam = self._family
         if fam.pooled_stem:
@@ -307,14 +322,110 @@ class FrozenResNetTeacher(nn.Module):
         return self.fc(torch.flatten(self.avgpool(z), 1))
 
 
+_VGG_CHILDREN = ("conv0", "bn0", "conv1", "pooling", "bn1", "conv2", "bn2", "conv3", "bn3", "conv4", "bn4", "conv5",
+                 "bn5", "nonlinear", "fc")
+_VGG_POOLED = (True, False, True, False, True)     # a 2x2 max-pool follows conv1, conv3, conv5
+
+
+def _check_vgg(model):
+    """Raise TypeError unless `model` is a VGGSmall whose six convs are bias-free 3x3 / stride-1 / pad-1 nn.Conv2d: the
+    fp32 teacher.  The binary VGG-Small is a student, whose eval forward has its own units."""
+    who = "FrozenVGGTeacher"
+    if type(model) is not VGGSmall:
+        raise TypeError(f"{who} wraps a bdbnn_b200.vgg.VGGSmall with nn.Conv2d convs, got {type(model).__name__}")
+    names = [n for n, _ in model.named_children()]
+    if names != list(_VGG_CHILDREN):
+        raise TypeError(f"{who}: unexpected children {names}")
+    if list(model.named_parameters(recurse=False)) or list(model.named_buffers(recurse=False)):
+        raise TypeError(f"{who}: the model itself must hold no parameters or buffers")
+    cin = 3
+    for i in range(6):
+        conv = getattr(model, f"conv{i}")
+        _check_conv(conv, f"conv{i}", 3, who=who, net="VGG-Small")
+        if conv.stride != (1, 1) or conv.padding != (1, 1) or conv.in_channels != cin:
+            raise TypeError(f"{who}: conv{i} must be a stride-1 / pad-1 conv on {cin} channels")
+        cin = conv.out_channels
+        _check_bn(getattr(model, f"bn{i}"), f"bn{i}", who=who)
+    c0 = model.conv0
+    if c0.out_channels != 128 or not F_.cifar_stem_supported((1, 3, 1, 1), tuple(c0.weight.shape), c0.stride,
+                                                             c0.padding, True):
+        raise TypeError(f"{who}: conv0 must be the 3x3 / stride-1 / pad-1 stem from 3 to 128 channels")
+    if type(model.fc) is not nn.Linear:
+        raise TypeError(f"{who}: fc must be nn.Linear")
+
+
+class FrozenVGGTeacher(_FrozenTeacher):
+    """The fp32 CIFAR VGG-Small teacher (bdbnn_b200.vgg.VGGSmall with bias-free nn.Conv2d convs, any class count),
+    whose eval forward runs on the real-valued eval kernels (DESIGN.md §4o):
+
+        z = hardtanh(BN_eval(conv0(x)))                   cifar_stem_conv_bn_eval(hardtanh=True)
+        z = hardtanh(BN_eval(maxpool2x2(conv(z))))        conv1, conv3, conv5: real_conv_pool_bn_eval
+        z = hardtanh(BN_eval(conv(z)))                    conv2, conv4: real_conv_bn_eval(hardtanh=True)
+        logits = fc(flatten(z))                           torch, NCHW flattening as VGGSmall.forward
+
+    while `nonlinear` and `pooling` are nn.Hardtanh(-1, 1) and nn.MaxPool2d(2, 2) (read at every forward); else, and
+    on anything FrozenResNetTeacher would not run, the wrapped model's own forward.  Raises TypeError for any other
+    structure (binary convs, biased convs, extra children, nn.DataParallel, subclasses, other BatchNorms)."""
+
+    def __init__(self, model):
+        _check_vgg(model)
+        super().__init__(model)
+
+    def _geometry_supported(self, x):
+        """The stem and every conv have their kernel at this input size, and every pooled map is even (host-only
+        checks, cached per (device, shape)); the two shared modules are read at every forward."""
+        if not (VGGSmall._modules_standard(self) and self._wrapped._modules_standard()):
+            return False
+        key = (x.device, tuple(x.shape))
+        ok = self._geom_ok.get(key)
+        if ok is None:
+            ok = self._geom_ok[key] = self._walk_geometry(x)
+        return ok
+
+    def _walk_geometry(self, x):
+        n, _, h, w = x.shape
+        c0 = self.conv0
+        ok = F_.cifar_stem_supported(tuple(x.shape), tuple(c0.weight.shape), c0.stride, c0.padding, True)
+        shape = (n, c0.out_channels, h, w)
+        L = _lib.lib()
+        for i, pooled in enumerate(_VGG_POOLED):
+            if not ok:
+                break
+            sh = F_.conv_shape(shape, getattr(self, f"conv{i + 1}").weight.shape, 1, 1)
+            ok = sh.Cin % 4 == 0 and bool(int(L.bdbnn_tc_supported(ctypes.byref(sh))) & 1)
+            if pooled:
+                ok = ok and sh.Ho % 2 == 0 and sh.Wo % 2 == 0 and sh.Cout % 32 == 0
+                shape = (n, sh.Cout, sh.Ho // 2, sh.Wo // 2)
+            else:
+                shape = (n, sh.Cout, sh.Ho, sh.Wo)
+        return ok
+
+    def _kernel_forward(self, x):
+        z, z_amax = F_.cifar_stem_conv_bn_eval(x, self.conv0.weight, *_bn_args(self.bn0), hardtanh=True)
+        convs = [getattr(self, f"conv{i}") for i in range(1, 6)]
+        # packed at every forward, never cached: a load_state_dict or an in-place update is always seen
+        packs = F_.real_weight_pack([c.weight for c in convs])
+        for i, pooled in enumerate(_VGG_POOLED):
+            bn = _bn_args(getattr(self, f"bn{i + 1}"))
+            if pooled:
+                z, z_amax = F_.real_conv_pool_bn_eval(z, z_amax, packs[i], *bn)
+            else:
+                z, z_amax = F_.real_conv_bn_eval(z, z_amax, packs[i], *bn, 1, 1, relu=False, hardtanh=True)
+        return self.fc(torch.flatten(z, 1))
+
+
 def launches_per_forward(model):
     """C-ABI kernel launches of one kernel-path forward: 2 weight-pack launches per 48 3x3 convs and 3 per 3x3 conv
     (activation pack with the amax given, fold, conv), plus
       torchvision ResNet (DESIGN.md §4h): 6 for the stem (x amax, x pack, W pack, fold, conv, max-pool) and 6 per
         `downsample` (x amax, x pack, W amax, W pack, fold, conv);
       CIFAR ResNet (DESIGN.md §4j): 2 for the stem (fold, conv); the option-A shortcuts launch nothing;
-      CIFAR ResNet-18 (DESIGN.md §4k): 2 for the stem (fold, conv) and 6 per `downsample`."""
-    m = model.wrapped if isinstance(model, FrozenResNetTeacher) else model
+      CIFAR ResNet-18 (DESIGN.md §4k): 2 for the stem (fold, conv) and 6 per `downsample`;
+      VGG-Small (DESIGN.md §4o): 2 for the stem (fold, conv) and 1 more per pooled conv (its pool)."""
+    m = model.wrapped if isinstance(model, _FrozenTeacher) else model
+    if type(m) is VGGSmall:
+        _check_vgg(m)
+        return 2 + 2 + sum(4 if pooled else 3 for pooled in _VGG_POOLED)
     fam = _family(m)
     blocks = [b for b in m.modules() if type(b) is fam.block]
     n3 = 2 * len(blocks)

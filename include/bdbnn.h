@@ -219,8 +219,9 @@ BDBNN_API size_t bdbnn_wgrad_tc_workspace_bytes(const bdbnn_conv_shape* s);
 BDBNN_API int bdbnn_debug_conv_plan(const bdbnn_conv_shape* s, int32_t mode, int32_t grad_halves, int32_t* out,
                           int32_t n_out);
 /* CTAs of the forward (mode 0) / dgrad (mode 1) / eval forward (mode 2) / eval forward with the option-A residual of
- * the *_pad_shortcut entry points (mode 3) tensor-core kernel that fit on one SM of the current device, for operand
- * format fmt (BDBNN_FMT_FP16 / BDBNN_FMT_BF16, -1 = fp8: modes 0 and 2 only), N tile bn (16/32/64/128) and
+ * the *_pad_shortcut entry points (mode 3) / eval forward with the Hardtanh epilogue of bdbnn_real_conv_fwd_eval
+ * (mode 5, BDBNN_FMT_FP16 only; 4 is not a mode) tensor-core kernel that fit on one SM of the current device, for
+ * operand format fmt (BDBNN_FMT_FP16 / BDBNN_FMT_BF16, -1 = fp8: modes 0 and 2 only), N tile bn (16/32/64/128) and
  * `smem` bytes of dynamic shared memory (bdbnn_debug_conv_plan out[8]), from the CUDA occupancy calculator.  Needs a
  * CUDA device; sets that kernel's maximum dynamic shared memory attribute to `smem` (every launch sets it again). */
 BDBNN_API int bdbnn_debug_tc_conv_ctas_per_sm(int32_t mode, int32_t fmt, int32_t bn, int32_t smem, int32_t* ctas);
@@ -365,7 +366,12 @@ BDBNN_API int bdbnn_pad_shortcut_bwd(const float* gz, float* gx, int32_t N, int3
  *          0 elsewhere (the max-pool backward).  Scratch and outputs as bdbnn_bn_bwd_pack.
  * pool2_bn_eval_hardtanh : z fp32 NHWC [N,H/2,W/2,C] = hardtanh(fp32(fp32(m * scale[c]) + shift[c])) for m the 2x2
  *          max of y_int, scale / shift from bdbnn_bn_eval_fold with alpha; optionally the +-1 copy of z, 16-bit in
- *          format fmt (zb) and / or e4m3 (zb8). */
+ *          format fmt (zb) and / or e4m3 (zb8).
+ * real_pool2_bn_eval_hardtanh : the same unit after a real-valued conv (the fp32 VGG-Small teacher): y fp32 NHWC
+ *          [N,H,W,C] (H, W even, C % 32 == 0), z fp32 NHWC [N,H/2,W/2,C] = hardtanh(fp32(fp32(m * scale[c]) +
+ *          shift[c])) for m the 2x2 max of y (NaN if the window holds one, as F.max_pool2d), no +-1 copy;
+ *          z_amax_bits (one word, zeroed here) receives the bits of max|z| (integer atomicMax, as
+ *          bdbnn_real_conv_fwd_eval), for the next conv's bdbnn_real_act_pack. */
 BDBNN_API int bdbnn_bn_fwd_hardtanh(const void* y, const float* alpha, const float* gamma, const float* beta,
                           int64_t n_pix, int32_t C, float eps, float momentum, float* running_mean,
                           float* running_var, double* sums_ws, uint32_t* ymax_bits, float* mean, float* invstd,
@@ -386,6 +392,9 @@ BDBNN_API int bdbnn_pool2_bn_bwd_pack(const float* gz, const int16_t* p_int, con
 BDBNN_API int bdbnn_pool2_bn_eval_hardtanh(const int16_t* y_int, const float* scale, const float* shift, int32_t N,
                                  int32_t H, int32_t W, int32_t C, float* z, uint16_t* zb, uint8_t* zb8, int32_t fmt,
                                  void* stream);
+BDBNN_API int bdbnn_real_pool2_bn_eval_hardtanh(const float* y, const float* scale, const float* shift, int32_t N,
+                                      int32_t H, int32_t W, int32_t C, float* z, uint32_t* z_amax_bits,
+                                      void* stream);
 
 /* ---- CIFAR stem: 3x3 / stride 1 / pad 1, 3 -> Cout channels (Cout in {16, 32, 48, 64, 128}), fp32, CUDA cores -
  * Replaces the fp32 nn.Conv2d `conv1` of the CIFAR ResNets (models/cifar10; model(images), train.py:492 and its
@@ -560,11 +569,19 @@ BDBNN_API int bdbnn_real_conv_pack(const float* x, int32_t N, int32_t H, int32_t
  *                            every step (no FMA):
  *                              z = fp32(fp32(fp32(acc * 2^-ex) * scale[o]) + shift[o])   (2^-ex from x_amax_bits)
  *                              z = fp32(z + residual)  if residual != NULL (z's shape, must not alias it)
- *                              z = relu(z)             if relu != 0 (torch.relu: NaN propagates)
+ *                              then the activation code `act`:
+ *                                BDBNN_ACT_NONE     (0) z as it is
+ *                                BDBNN_ACT_RELU     (1) z = relu(z)             (torch.relu: NaN propagates)
+ *                                BDBNN_ACT_HARDTANH (2) z = clamp(z, -1, 1)     (torch.nn.Hardtanh(): NaN stays NaN,
+ *                                                                                -0.0 stays -0.0)
+ *                              any other value is rejected (BDBNN_ERR_INVALID_ARG)
  *                            (scale, shift) = bdbnn_bn_eval_fold with the weight's alpha.  z fp32 NHWC; z_amax_bits
  *                            (one word, may be NULL; zeroed here) receives the bits of max|z| (integer atomicMax
  *                            of |z|'s bits: run-to-run identical, NaN above every number).  Requires
  *                            bdbnn_tc_supported(s) & BDBNN_TC_FWD.  One launch. */
+#define BDBNN_ACT_NONE 0
+#define BDBNN_ACT_RELU 1
+#define BDBNN_ACT_HARDTANH 2
 BDBNN_API int bdbnn_real_act_pack(const float* x, int64_t n_pix, int32_t C, uint32_t* amax_bits, int32_t have_amax,
                         uint16_t* xh, void* stream);
 BDBNN_API int bdbnn_real_weight_pack_multi(int32_t count, const float* const* W_host, const int32_t* Cout_host,
@@ -572,7 +589,7 @@ BDBNN_API int bdbnn_real_weight_pack_multi(int32_t count, const float* const* W_
                                  uint32_t* amax_bits,
                                  uint16_t* const* wf_host, float* const* alpha_host, void* stream);
 BDBNN_API int bdbnn_real_conv_fwd_eval(const uint16_t* xh, const uint32_t* x_amax_bits, const uint16_t* wf,
-                             const float* scale, const float* shift, const float* residual, int32_t relu, float* z,
+                             const float* scale, const float* shift, const float* residual, int32_t act, float* z,
                              uint32_t* z_amax_bits, const bdbnn_conv_shape* s, void* stream);
 
 /* ---- eval forward with the CIFAR option-A shortcut as the residual, read in place ------------------------------

@@ -1,16 +1,18 @@
 """Throughput of the KD step's frozen fp32 teacher (train.py:250-277, run at train.py:603): this repository's kernel
-teacher (bdbnn_b200.FrozenResNetTeacher) against the unwrapped model on cuDNN.
+teacher (bdbnn_b200.FrozenResNetTeacher / FrozenVGGTeacher) against the unwrapped model on cuDNN.
 
-    python tools/teacher_throughput.py [--models resnet18,resnet34,resnet20,resnet18_cifar] [--batch N] [--iters 20]
+    python tools/teacher_throughput.py [--models resnet18,resnet34,resnet20,resnet18_cifar,vgg_small] [--batch N]
+                                       [--iters 20]
                                        [--warmup 5] [--rounds 3] [--steps 50] [--step-warmup 10] [--no-step]
 
 resnet18 / resnet34: the torchvision models on 224x224 images, batch 256 by default.  resnet20: the fp32 CIFAR
 ResNet-20 (bdbnn_b200.resnet.ResNetCifar(3) with bias-free nn.Conv2d convs) on 32x32 images, batch 128 by default;
-resnet18_cifar: the fp32 CIFAR ResNet-18 (bdbnn_b200.resnet.resnet18_cifar(conv_cls=<bias-free nn.Conv2d>)), the same.
+resnet18_cifar: the fp32 CIFAR ResNet-18 (bdbnn_b200.resnet.resnet18_cifar(conv_cls=<bias-free nn.Conv2d>)), the same;
+vgg_small: the fp32 CIFAR VGG-Small (bdbnn_b200.vgg.vgg_small(conv_cls=<bias-free nn.Conv2d>)), the same.
 channels_last images, random weights and BatchNorm statistics.  Teacher forward arms, alternated round by
 round, each warmed up first, images/s from CUDA events over --iters forwards:
 
-    kernel_eager     FrozenResNetTeacher, launched eagerly
+    kernel_eager     FrozenResNetTeacher / FrozenVGGTeacher, launched eagerly
     kernel_graphed   the same forward captured once as a CUDA graph and replayed
     cudnn_default    the unwrapped model with TF32 allowed and cudnn.benchmark off (bench.py's timed path)
     cudnn_benchmark  the same with cudnn.benchmark = True (train.py:368)
@@ -22,7 +24,7 @@ that ran first would serve its plans to the other and the benchmark arm would no
 Then one eager kernel-teacher forward under functional.KernelTimer (per-family times), and the full KD step:
 GraphedTrainStep(TrainStep(student, kurtosis + KD config, teacher=...)) with the kernel teacher and with the
 unwrapped teacher (cudnn.benchmark off throughout this process; the student is the binary resnet18, or the binary
-CIFAR net of the teacher's shape for a CIFAR teacher), alternated, --step-warmup steps then --steps
+CIFAR net of the teacher's shape for a CIFAR teacher, the binary vgg_small for vgg_small), alternated, --step-warmup steps then --steps
 timed steps per round.  The card name, power limit and maximum SM clock are read (read-only) from nvidia-smi.
 Needs a CUDA device."""
 import argparse
@@ -58,7 +60,7 @@ def _timed_loop(torch, fn, iters):
     return e0.elapsed_time(e1) / 1e3
 
 
-CIFAR = ("resnet20", "resnet18_cifar")
+CIFAR = ("resnet20", "resnet18_cifar", "vgg_small")
 
 
 def _hw(name):
@@ -76,6 +78,9 @@ def _teacher(torch, name, dev):
     if name == "resnet18_cifar":
         from bdbnn_b200.resnet import resnet18_cifar
         m = resnet18_cifar(conv_cls=fp32_conv)
+    elif name == "vgg_small":
+        from bdbnn_b200.vgg import vgg_small
+        m = vgg_small(conv_cls=fp32_conv)
     elif name in CIFAR:
         from bdbnn_b200.resnet import ResNetCifar
         m = ResNetCifar(3, conv_cls=fp32_conv)
@@ -124,10 +129,14 @@ def _cudnn_round(name, mode, args):
     return json.loads(r.stdout.strip().splitlines()[-1])["img_per_s"]
 
 
+def _wrap(name, model):
+    from bdbnn_b200 import FrozenResNetTeacher, FrozenVGGTeacher
+    return (FrozenVGGTeacher if name == "vgg_small" else FrozenResNetTeacher)(model)
+
+
 def forward_arms(torch, name, args, dev):
-    from bdbnn_b200 import FrozenResNetTeacher
     from bdbnn_b200.functional import KernelTimer
-    kt = FrozenResNetTeacher(_teacher(torch, name, dev))
+    kt = _wrap(name, _teacher(torch, name, dev))
     batch = _batch(args, name)
     x = _images(torch, name, batch, dev)
     with torch.no_grad():
@@ -159,19 +168,20 @@ def forward_arms(torch, name, args, dev):
 
 
 def kd_step_arms(torch, name, args, dev):
-    from bdbnn_b200 import FrozenResNetTeacher
     from bdbnn_b200.resnet import resnet18, resnet18_cifar, resnet20
     from bdbnn_b200.step import GraphedTrainStep, StepConfig, TrainStep, make_optimizer
+    from bdbnn_b200.vgg import vgg_small
     torch.backends.cudnn.benchmark = False
     tv = _teacher(torch, name, dev)
     cfg = StepConfig(w_kurtosis=True, teacher_student=True, alpha=0.9, beta=200.0, w_lambda_ce=1.0)
     g = torch.Generator().manual_seed(0)
     batch, hw = _batch(args, name), _hw(name)
-    student, classes = {"resnet20": (resnet20, 10), "resnet18_cifar": (resnet18_cifar, 10)}.get(name, (resnet18, 1000))
+    student, classes = {"resnet20": (resnet20, 10), "resnet18_cifar": (resnet18_cifar, 10),
+                        "vgg_small": (vgg_small, 10)}.get(name, (resnet18, 1000))
     x = torch.randn(batch, 3, hw, hw, generator=g).to(dev).contiguous(memory_format=torch.channels_last)
     y = torch.randint(0, classes, (batch,), generator=g).to(dev)
     steps = {}
-    for arm, teacher in (("kernel_teacher", FrozenResNetTeacher(tv)), ("cudnn_teacher", tv)):
+    for arm, teacher in (("kernel_teacher", _wrap(name, tv)), ("cudnn_teacher", tv)):
         torch.manual_seed(0)
         model = student().to(dev)
         steps[arm] = GraphedTrainStep(TrainStep(model, make_optimizer(model), cfg, teacher=teacher))
@@ -190,7 +200,7 @@ def kd_step_arms(torch, name, args, dev):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--models", default="resnet18,resnet34")
-    ap.add_argument("--batch", type=int, default=None, help="default: 256 (resnet18/34), 128 (resnet20)")
+    ap.add_argument("--batch", type=int, default=None, help="default: 256 (resnet18/34), 128 (the CIFAR nets)")
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--rounds", type=int, default=3)
