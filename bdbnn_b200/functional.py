@@ -221,6 +221,22 @@ def _get_act_pack(x, fmt):
     return None
 
 
+def _set_eval_pack(z, fmt, zb):
+    """Attach the eval units' +-1 copy of z (format fmt, -1 = fp8 bytes) for the next unit, stamped with z's version.
+    Inference tensors have no version counter to guard the copy with, so they get none."""
+    if not z.is_inference():
+        z._bdbnn_eval_pack = (fmt, zb)
+        z._bdbnn_eval_pack_version = z._version
+
+
+def _get_eval_pack(x, fmt):
+    """x's eval +-1 copy if it is in format fmt and describes x as it is (not modified in place since), else None."""
+    pk = getattr(x, "_bdbnn_eval_pack", None)
+    if pk is not None and pk[0] == fmt and x._bdbnn_eval_pack_version == x._version:
+        return pk[1]
+    return None
+
+
 def _alloc_weight_pack(w_shape, dev, wf=False, wf8=False, grad=False):
     """Buffers for bdbnn_weight_pack: alpha and the sign / mask bits always; the 16-bit (wf) and fp8 (wf8) forward
     operands on request; with `grad` the transposed 16-bit operand and the gradient scales the backward reads."""
@@ -279,6 +295,51 @@ def _wgrad_tc(sh, gys, gcode, amax, xb, wmask, inv_gscale, w_shape, w_param, fam
         (gys, amax, xb, wmask, inv_gscale), family, key, nbytes)
 
 
+def _dgrad_tc(sh, gys, gcode, amax, wt, mask, add, gx, family, nbytes):
+    """bdbnn_binconv_dgrad_tc into gx, timed; `add` (or None) is summed into the result in the epilogue."""
+    with _timed(family, _shape_key(sh), nbytes):
+        _lib.check(_lib.lib().bdbnn_binconv_dgrad_tc(_p(gys), gcode, _p(amax), _p(wt), _p(mask), _p(add), _p(gx),
+                                                     ctypes.byref(sh), _stream()), family)
+    _lib.count(_dgrad_launches(sh))
+
+
+# the BatchNorm backward's outputs: its sums and per-channel max|g|, the constants of its apply pass, dgamma, dbeta,
+# and the conv backward's 16-bit gradient operand gys with its amax word
+_BNGrads = collections.namedtuple("_BNGrads", "sums gmax consts dgamma dbeta amax gys")
+
+
+def _bn_grads(cout, out_shape, gh, dev):
+    """Buffers of one BatchNorm backward over cout channels; gys is [*out_shape, gh * cout] (gh bf16 halves)."""
+    f32 = dict(dtype=torch.float32, device=dev)
+    return _BNGrads(torch.empty((2 * cout,), dtype=torch.float64, device=dev),
+                    torch.empty((cout,), dtype=torch.int32, device=dev),
+                    torch.empty((4 * cout,), **f32), torch.empty((cout,), **f32), torch.empty((cout,), **f32),
+                    torch.empty((1,), dtype=torch.int32, device=dev),
+                    torch.empty((*out_shape, gh * cout), dtype=torch.int16, device=dev))
+
+
+def _fwd_tc(sh, use8, x, wp, fmt, y, stats=None):
+    """One forward launch of the binary conv on the wgmma kernels, into y: an int16 y (the exact accumulator,
+    y = alpha * y_int) through binconv_fwd_tc_i16, an fp32 y through binconv_fwd_tc8 or binconv_fwd_tc.
+    x: the activation operand, or an _ActPack to take it from; use8: fp8 operands (wp.wf8), else 16-bit ones in
+    format fmt (wp.wf); stats: (sums, ymax) for the BatchNorm statistics in the epilogue, or None."""
+    L = _lib.lib()
+    if isinstance(x, _ActPack):
+        x = x.xb8 if use8 else x.xb
+    kind = "fwd_tc8" if use8 else "fwd_tc"
+    i16 = y.dtype == torch.int16
+    ops = (_p(x), _p(wp.wf8 if use8 else wp.wf))
+    tail = (_p(wp.alpha), _p(y), ctypes.byref(sh), *(map(_p, stats) if stats else (None, None)), _stream())
+    with _timed("binconv_" + kind, _shape_key(sh), algorithmic_bytes(kind, sh) - (2 * y.numel() if i16 else 0)):
+        if i16:
+            _lib.check(L.bdbnn_binconv_fwd_tc_i16(*ops, -1 if use8 else fmt, *tail), "binconv_fwd_tc_i16")
+        elif use8:
+            _lib.check(L.bdbnn_binconv_fwd_tc8(*ops, *tail), "binconv_fwd_tc8")
+        else:
+            _lib.check(L.bdbnn_binconv_fwd_tc(*ops, fmt, *tail), "binconv_fwd_tc")
+    _lib.count(1)
+
+
 class _BinConv2d(torch.autograd.Function):
     """y = alpha[o] * conv2d(sign(x), sign(W)) with STE backward (spec: DESIGN.md §2).
 
@@ -306,19 +367,13 @@ class _BinConv2d(torch.autograd.Function):
         _weight_pack(weight, wp, fmt)
         y = torch.empty((sh.N, sh.Cout, sh.Ho, sh.Wo), dtype=torch.float32, device=dev,
                         memory_format=torch.channels_last)
-        if use8:
-            with _timed("binconv_fwd_tc8", key, algorithmic_bytes("fwd_tc8", sh)):
-                _lib.check(L.bdbnn_binconv_fwd_tc8(_p(ap.xb8), _p(wp.wf8), _p(wp.alpha), _p(y), ctypes.byref(sh), None,
-                                                   None, st), "binconv_fwd_tc8")
-        elif tc:
-            with _timed("binconv_fwd_tc", key, algorithmic_bytes("fwd_tc", sh)):
-                _lib.check(L.bdbnn_binconv_fwd_tc(_p(ap.xb), _p(wp.wf), fmt, _p(wp.alpha), _p(y), ctypes.byref(sh),
-                                                  None, None, st), "binconv_fwd_tc")
+        if tc:
+            _fwd_tc(sh, use8, ap, wp, fmt, y)
         else:
             with _timed("binconv_fwd_xnor", key, algorithmic_bytes("fwd_xnor", sh)):
                 _lib.check(L.bdbnn_binconv_fwd_xnor(_p(ap.sign), _p(wp.wsign), _p(wp.alpha), _p(y),
                                                     ctypes.byref(sh), st), "binconv_fwd_xnor")
-        _lib.count(1)
+            _lib.count(1)
         ctx.sh = sh
         ctx.use = use
         ctx.gmode = (gname, gcode, ghalves)
@@ -375,10 +430,8 @@ class _BinConv2d(torch.autograd.Function):
             if need_x:
                 gx = torch.empty(ctx.x_shape, dtype=torch.float32, device=dev,
                                  memory_format=torch.channels_last)
-                with _timed("binconv_dgrad_tc", key, algorithmic_bytes("dgrad_tc", sh, gh)):
-                    _lib.check(L.bdbnn_binconv_dgrad_tc(_p(gys), gcode, _p(amax), _p(wt), _p(mask_bits), _p(None), _p(gx),
-                                                        ctypes.byref(sh), st), "binconv_dgrad_tc")
-                _lib.count(_dgrad_launches(sh))
+                _dgrad_tc(sh, gys, gcode, amax, wt, mask_bits, None, gx, "binconv_dgrad_tc",
+                          algorithmic_bytes("dgrad_tc", sh, gh))
             if need_w and ctx.use & 4:
                 # EDE scales gw afterwards, so its wgrad stays in line (no w_param: never the second stream)
                 gw = _wgrad_tc(sh, gys, gcode, amax, xb, wmask, inv_gscale, ctx.w_shape,
@@ -747,6 +800,28 @@ def _prepacked(weight, fmt, use8):
     return _WeightPack._make(getattr(pre, f) for f in _WeightPack._fields)
 
 
+def _unit_operands(x, weight, sh, caps, train):
+    """(use8, activation, _WeightPack) of a fused unit's binary conv, caps = bdbnn_tc_supported(sh).
+    train: the activation is x's _ActPack with the 16-bit copy (the backward reads it and the mask bits), completed
+    from the packs its producer attached when they are current; the weight pack has the gradient operands.
+    eval: the activation is the one operand the forward reads, x's `_bdbnn_eval_pack` when it matches.
+    The weights come from prepack_weights when it packed them for this forward."""
+    fmt = grad_mode()[3]
+    use8 = bool(caps & 8) and use_fwd8(sh.Cin, sh.Cout, eval_unit=not train)
+    if train:
+        act = _act_pack(x, sh, fmt, xb=True, xb8=use8, have=_get_act_pack(x, fmt))
+    else:
+        act = _get_eval_pack(x, -1 if use8 else fmt)
+        if act is None:
+            ap = _act_pack(x, sh, fmt, xb=not use8, xb8=use8)
+            act = ap.xb8 if use8 else ap.xb
+    wp = _prepacked(weight, fmt, use8)
+    if wp is None:
+        wp = _alloc_weight_pack(weight.shape, x.device, wf=not use8, wf8=use8, grad=train)
+        _weight_pack(weight, wp, fmt)
+    return use8, act, wp
+
+
 def wgrad_side_enabled():
     """BDBNN_WGRAD_SIDE (default 1): inside TrainStep's backward the weight-gradient GEMMs run on a second stream."""
     return os.environ.get("BDBNN_WGRAD_SIDE", "1") != "0"
@@ -877,14 +952,15 @@ def unit_supported(x_shape, w_shape, stride, padding):
 
 
 class _ConvBNAddUnit(torch.autograd.Function):
-    """forward : [act_pack(x) unless packs are handed in] -> weight_pack -> fwd_tc -> bn_fwd(+residual, +pack of z)
-    backward: bn_bwd_pack(gz, y) -> dgrad_tc, wgrad_tc ; residual grad = gz."""
+    """forward : [act_pack(x) unless x carries its producer's packs] -> weight_pack -> fwd_tc -> bn_fwd(+residual,
+              +pack of z)
+    backward: bn_bwd_pack(gz, y) -> wgrad_tc, dgrad_tc ; residual grad = gz."""
 
     @staticmethod
     @_on_device
     def forward(ctx, x, weight, gamma, beta, residual, running_mean, running_var, momentum, eps, stride,
-                padding, xs, xm, xb, xb8, res_is_x, sc_weight=None, sc_gamma=None, sc_beta=None, sc_rm=None,
-                sc_rv=None, sc_momentum=None, sc_eps=None, sc_stride=None, sc_pad=None, hardtanh=False):
+                padding, res_is_x, sc_weight=None, sc_gamma=None, sc_beta=None, sc_rm=None, sc_rv=None,
+                sc_momentum=None, sc_eps=None, sc_stride=None, sc_pad=None, hardtanh=False):
         _require_cuda(x, "conv_bn_add(x)")
         ctx.hardtanh = bool(hardtanh)
         _same_device(x, weight, gamma, beta, residual, running_mean, running_var, sc_weight)
@@ -927,41 +1003,19 @@ class _ConvBNAddUnit(torch.autograd.Function):
         key = _shape_key(sh)
         i32 = dict(dtype=torch.int32, device=dev)
         caps = int(L.bdbnn_tc_supported(ctypes.byref(sh)))
-        use8 = bool(caps & 8) and use_fwd8(sh.Cin, cout, eval_unit=False)
-        ap = _act_pack(x, sh, fmt, xb=True, xb8=use8,
-                       have=None if xs is None else _ActPack(xs, xm, xb, fmt, xb8))
-        xm, xb, xb8 = ap.mask, ap.xb, ap.xb8
-        # packed with every other binary conv of the network at the start of this forward (prepack_weights)
-        wp = _prepacked(weight, fmt, use8)
-        if wp is None:
-            wp = _alloc_weight_pack(weight.shape, dev, wf=not use8, wf8=use8, grad=True)
-            _weight_pack(weight, wp, fmt)
+        use8, ap, wp = _unit_operands(x, weight, sh, caps, train=True)
         alpha = wp.alpha
         # BN batch statistics of y are accumulated by the conv kernel's epilogue (BDBNN_CONV_STATS=0: separate pass)
         sums = torch.empty((2 * cout,), dtype=torch.float64, device=dev)
         ymax = torch.empty((cout,), **i32)
         in_conv = conv_stats_enabled() and cout <= 512
-        s_ptr, m_ptr = (_p(sums), _p(ymax)) if in_conv else (None, None)
         i16 = bool(caps & 16) and in_conv and y_i16_enabled()
         if i16:     # y kept as the exact integer accumulator, int16 NHWC (y = alpha * y_int)
             y = torch.empty((n, sh.Ho, sh.Wo, cout), dtype=torch.int16, device=dev)
-            with _timed("binconv_fwd_tc8" if use8 else "binconv_fwd_tc", key,
-                        algorithmic_bytes("fwd_tc8" if use8 else "fwd_tc", sh) - 2 * y.numel()):
-                _lib.check(L.bdbnn_binconv_fwd_tc_i16(_p(xb8) if use8 else _p(xb), _p(wp.wf8) if use8 else _p(wp.wf),
-                                                      -1 if use8 else fmt, _p(alpha), _p(y), ctypes.byref(sh), s_ptr,
-                                                      m_ptr, st), "binconv_fwd_tc_i16")
         else:
             y = torch.empty((n, cout, sh.Ho, sh.Wo), dtype=torch.float32, device=dev,
                             memory_format=torch.channels_last)
-            if use8:
-                with _timed("binconv_fwd_tc8", key, algorithmic_bytes("fwd_tc8", sh)):
-                    _lib.check(L.bdbnn_binconv_fwd_tc8(_p(xb8), _p(wp.wf8), _p(alpha), _p(y), ctypes.byref(sh), s_ptr,
-                                                       m_ptr, st), "binconv_fwd_tc8")
-            else:
-                with _timed("binconv_fwd_tc", key, algorithmic_bytes("fwd_tc", sh)):
-                    _lib.check(L.bdbnn_binconv_fwd_tc(_p(xb), _p(wp.wf), fmt, _p(alpha), _p(y), ctypes.byref(sh),
-                                                      s_ptr, m_ptr, st), "binconv_fwd_tc")
-        _lib.count(1)
+        _fwd_tc(sh, use8, ap, wp, fmt, y, (sums, ymax) if in_conv else None)
         n_pix = n * sh.Ho * sh.Wo
         if res_is_x:            # identity shortcut: the residual IS the conv input (one autograd edge)
             rc = _nhwc(x.detach())
@@ -981,38 +1035,29 @@ class _ConvBNAddUnit(torch.autograd.Function):
             torch.cuda.current_stream().wait_stream(sc_join)
         # residual bytes: a dense residual is read whole; the option-A one only over its Cin real channels
         res_bytes = 4 * n_pix * (x.shape[1] if sc_pad is not None else cout)
+        # the arguments every BatchNorm apply variant takes: gamma, beta, then (after the geometry) the running
+        # statistics, the statistics of y, the outputs and the operand format
+        gb = (_p(gamma.detach()), _p(beta.detach()))
+        bn = (float(eps), float(momentum), _p(running_mean), _p(running_var), _p(sums), _p(ymax), _p(mean), _p(invstd),
+              _p(ab), _p(z), _p(zs), _p(zm), _p(zb), _p(zb8), fmt)
         with _timed("bn_fwd", key, ((0 if in_conv else 4) + ybytes + 4 + (2.25 if pack else 0) +
                                     (1 if zb8 is not None else 0)) * n_pix * cout + res_bytes):
             if ctx.hardtanh:
-                _lib.check(L.bdbnn_bn_fwd_hardtanh(
-                    _p(y), _p(alpha) if i16 else None, _p(gamma.detach()), _p(beta.detach()), n_pix, cout, float(eps),
-                    float(momentum), _p(running_mean), _p(running_var), _p(sums), _p(ymax), _p(mean), _p(invstd),
-                    _p(ab), _p(z), _p(zs), _p(zm), _p(zb), _p(zb8), fmt, 1 if in_conv else 0, st), "bn_fwd_hardtanh")
+                _lib.check(L.bdbnn_bn_fwd_hardtanh(_p(y), _p(alpha) if i16 else None, *gb, n_pix, cout, *bn,
+                                                   1 if in_conv else 0, st), "bn_fwd_hardtanh")
             elif sc_pad is not None:
                 xc = _nhwc(x.detach())
                 _, cin, h, w = x.shape
                 if i16:
-                    _lib.check(L.bdbnn_bn_fwd_i16_pad_shortcut(
-                        _p(y), _p(alpha), _p(xc), n, h, w, cin, int(sc_pad), _p(gamma.detach()), _p(beta.detach()),
-                        cout, float(eps), float(momentum), _p(running_mean), _p(running_var), _p(sums), _p(ymax),
-                        _p(mean), _p(invstd), _p(ab), _p(z), _p(zs), _p(zm), _p(zb), _p(zb8), fmt, st),
-                        "bn_fwd_i16_pad_shortcut")
+                    _lib.check(L.bdbnn_bn_fwd_i16_pad_shortcut(_p(y), _p(alpha), _p(xc), n, h, w, cin, int(sc_pad), *gb,
+                                                               cout, *bn, st), "bn_fwd_i16_pad_shortcut")
                 else:
-                    _lib.check(L.bdbnn_bn_fwd_pad_shortcut(
-                        _p(y), _p(xc), n, h, w, cin, int(sc_pad), _p(gamma.detach()), _p(beta.detach()), cout,
-                        float(eps), float(momentum), _p(running_mean), _p(running_var), _p(sums), _p(ymax), _p(mean),
-                        _p(invstd), _p(ab), _p(z), _p(zs), _p(zm), _p(zb), _p(zb8), fmt, 1 if in_conv else 0, st),
-                        "bn_fwd_pad_shortcut")
+                    _lib.check(L.bdbnn_bn_fwd_pad_shortcut(_p(y), _p(xc), n, h, w, cin, int(sc_pad), *gb, cout, *bn,
+                                                           1 if in_conv else 0, st), "bn_fwd_pad_shortcut")
             elif i16:
-                _lib.check(L.bdbnn_bn_fwd_i16(_p(y), _p(alpha), _p(rc), _p(gamma.detach()), _p(beta.detach()), n_pix,
-                                              cout, float(eps), float(momentum), _p(running_mean), _p(running_var),
-                                              _p(sums), _p(ymax), _p(mean), _p(invstd), _p(ab), _p(z), _p(zs), _p(zm),
-                                              _p(zb), _p(zb8), fmt, st), "bn_fwd_i16")
+                _lib.check(L.bdbnn_bn_fwd_i16(_p(y), _p(alpha), _p(rc), *gb, n_pix, cout, *bn, st), "bn_fwd_i16")
             else:
-                _lib.check(L.bdbnn_bn_fwd(_p(y), _p(rc), _p(gamma.detach()), _p(beta.detach()), n_pix, cout, float(eps),
-                                          float(momentum), _p(running_mean), _p(running_var), _p(sums), _p(ymax),
-                                          _p(mean), _p(invstd), _p(ab), _p(z), _p(zs), _p(zm), _p(zb), _p(zb8), fmt,
-                                          1 if in_conv else 0, st), "bn_fwd")
+                _lib.check(L.bdbnn_bn_fwd(_p(y), _p(rc), *gb, n_pix, cout, *bn, 1 if in_conv else 0, st), "bn_fwd")
         _lib.count(2 if in_conv else 3)
         ctx.y_i16 = i16
         # a consumer's dgrad epilogue may accumulate this unit's backward sums only where gz needs no Hardtanh mask
@@ -1024,8 +1069,8 @@ class _ConvBNAddUnit(torch.autograd.Function):
         ctx.has_res = residual is not None and sc_weight is None
         ctx.res_is_x = bool(res_is_x)
         # ab (the BatchNorm's per-channel a, b) lets the Hardtanh backward recompute its mask exactly
-        ctx.save_for_backward(y, mean, invstd, gamma.detach(), ymax, xm, xb, wp.wt, wp.wmask, wp.gscale, wp.inv_gscale,
-                              alpha, *sc_saved, *((ab,) if ctx.hardtanh else ()))
+        ctx.save_for_backward(y, mean, invstd, gamma.detach(), ymax, ap.mask, ap.xb, wp.wt, wp.wmask, wp.gscale,
+                              wp.inv_gscale, alpha, *sc_saved, *((ab,) if ctx.hardtanh else ()))
         _ConvBNAddUnit._last_bnctx = ctx.bnctx_out       # picked up by conv_bn_add right after apply() (same thread)
         if pack:
             if zb8 is not None:
@@ -1039,7 +1084,7 @@ class _ConvBNAddUnit(torch.autograd.Function):
     @_on_device
     def backward(ctx, gz, _g1, _g2, _g3, _g4):
         if gz is None:
-            return (None,) * 26
+            return (None,) * 22
         L = _lib.lib()
         sh = ctx.sh
         st = _stream()
@@ -1050,14 +1095,7 @@ class _ConvBNAddUnit(torch.autograd.Function):
         g = _nhwc(gz)
         cout = sh.Cout
         n_pix = sh.N * sh.Ho * sh.Wo
-        i32 = dict(dtype=torch.int32, device=dev)
-        sums = torch.empty((2 * cout,), dtype=torch.float64, device=dev)
-        gmax = torch.empty((cout,), **i32)
-        consts = torch.empty((4 * cout,), dtype=torch.float32, device=dev)
-        dgamma = torch.empty((cout,), dtype=torch.float32, device=dev)
-        dbeta = torch.empty((cout,), dtype=torch.float32, device=dev)
-        amax = torch.empty((1,), **i32)
-        gys = torch.empty((sh.N, sh.Ho, sh.Wo, gh * cout), dtype=torch.int16, device=dev)
+        sums, gmax, consts, dgamma, dbeta, amax, gys = _bn_grads(cout, (sh.N, sh.Ho, sh.Wo), gh, dev)
         ybytes = 2 if ctx.y_i16 else 4
         # backward sums already accumulated by the dgrad kernel that produced gz?  (attached to the gradient tensor
         # by the next unit's backward; identity of y guards against a foreign tensor)
@@ -1065,21 +1103,19 @@ class _ConvBNAddUnit(torch.autograd.Function):
         stt = getattr(gz, "_bdbnn_bwdstats", None)
         if ctx.y_i16 and stt is not None and stt[2].data_ptr() == y.data_ptr() and stt[3] == gz._version:
             sums, gmax, ready = stt[0], stt[1], 1
+        # the arguments after the geometry that every BatchNorm backward variant takes
+        out = (gcode, _p(sums), _p(gmax), _p(consts), _p(dgamma), _p(dbeta), _p(amax), _p(gys))
         with _timed("bn_bwd_pack", key, ((0 if ready else 4 + ybytes) + 4 + ybytes + 2 * gh) * n_pix * cout):
             if ctx.hardtanh:
                 _lib.check(L.bdbnn_bn_bwd_pack_hardtanh(
                     _p(g), _p(y), _p(alpha) if ctx.y_i16 else None, _p(ctx.saved_tensors[12]), _p(mean), _p(invstd),
-                    _p(gamma), _p(gscale), _p(ymax), n_pix, cout, gcode, _p(sums), _p(gmax), _p(consts), _p(dgamma),
-                    _p(dbeta), _p(amax), _p(gys), st), "bn_bwd_pack_hardtanh")
+                    _p(gamma), _p(gscale), _p(ymax), n_pix, cout, *out, st), "bn_bwd_pack_hardtanh")
             elif ctx.y_i16:
                 _lib.check(L.bdbnn_bn_bwd_pack_i16(_p(g), _p(y), _p(alpha), _p(mean), _p(invstd), _p(gamma), _p(gscale),
-                                                   _p(ymax), n_pix, cout, gcode, _p(sums), _p(gmax), _p(consts),
-                                                   _p(dgamma), _p(dbeta), _p(amax), _p(gys), ready, st),
-                           "bn_bwd_pack_i16")
+                                                   _p(ymax), n_pix, cout, *out, ready, st), "bn_bwd_pack_i16")
             else:
                 _lib.check(L.bdbnn_bn_bwd_pack(_p(g), _p(y), _p(mean), _p(invstd), _p(gamma), _p(gscale), _p(ymax),
-                                               n_pix, cout, gcode, _p(sums), _p(gmax), _p(consts), _p(dgamma),
-                                               _p(dbeta), _p(amax), _p(gys), st), "bn_bwd_pack")
+                                               n_pix, cout, *out, st), "bn_bwd_pack")
         _lib.count(2 if ready else 3)
         x_shape, w_shape = ctx.shapes
         gx = gw = None
@@ -1094,7 +1130,7 @@ class _ConvBNAddUnit(torch.autograd.Function):
                 # gx = dgrad + gz is the producing unit's gz: accumulate ITS BatchNorm backward sums in this epilogue
                 py, palpha, pmean, pinvstd = ctx.prod_bn
                 psums = torch.empty((2 * sh.Cin,), dtype=torch.float64, device=dev)
-                pgmax = torch.empty((sh.Cin,), **i32)
+                pgmax = torch.empty((sh.Cin,), dtype=torch.int32, device=dev)
                 with _timed("binconv_dgrad_tc", key, algorithmic_bytes("dgrad_tc", sh, gh) + 2 * gx.numel()):
                     rc = L.bdbnn_binconv_dgrad_tc_stats(_p(gys), gcode, _p(amax), _p(wt), _p(xm), _p(g), _p(gx),
                                                         ctypes.byref(sh), _p(py), _p(palpha), _p(pmean), _p(pinvstd),
@@ -1106,12 +1142,9 @@ class _ConvBNAddUnit(torch.autograd.Function):
                 elif rc != -3:           # BDBNN_ERR_UNSUPPORTED: plain dgrad below
                     _lib.check(rc, "binconv_dgrad_tc_stats")
             if not done:
-                with _timed("binconv_dgrad_tc", key, algorithmic_bytes("dgrad_tc", sh, gh)):
-                    # identity shortcut: d/dx = dgrad + gz, summed in the dgrad epilogue (no separate add kernel)
-                    _lib.check(L.bdbnn_binconv_dgrad_tc(_p(gys), gcode, _p(amax), _p(wt), _p(xm),
-                                                        _p(g) if ctx.res_is_x else _p(None), _p(gx),
-                                                        ctypes.byref(sh), st), "binconv_dgrad_tc")
-                _lib.count(_dgrad_launches(sh))
+                # identity shortcut: d/dx = dgrad + gz, summed in the dgrad epilogue (no separate add kernel)
+                _dgrad_tc(sh, gys, gcode, amax, wt, xm, g if ctx.res_is_x else None, gx, "binconv_dgrad_tc",
+                          algorithmic_bytes("dgrad_tc", sh, gh))
             if ctx.sc_pad is not None:
                 # option-A shortcut: its gradient gz[:, pad:pad+Cin] lands on the even positions, added in place
                 n_sub = sh.N * sh.Ho * sh.Wo * sh.Cin
@@ -1124,13 +1157,13 @@ class _ConvBNAddUnit(torch.autograd.Function):
         if ctx.n_sc:
             # shortcut branch: residual gradient = gz; its dgrad accumulates into gx in place
             sgx, sc_gw, sc_dg, sc_db = _shortcut_bwd_impl(gz, ctx.saved_tensors[12:], ctx.sc_geom,
-                                                          ctx.needs_input_grad[0], ctx.needs_input_grad[16], acc=gx,
+                                                          ctx.needs_input_grad[0], ctx.needs_input_grad[12], acc=gx,
                                                           w_param=ctx.sc_w_param)
             gx = sgx if sgx is not None else gx
-            sc_dg = sc_dg if ctx.needs_input_grad[17] else None
-            sc_db = sc_db if ctx.needs_input_grad[18] else None
+            sc_dg = sc_dg if ctx.needs_input_grad[13] else None
+            sc_db = sc_db if ctx.needs_input_grad[14] else None
         return (gx, gw, dgamma if ctx.needs_input_grad[2] else None, dbeta if ctx.needs_input_grad[3] else None,
-                gres, None, None, None, None, None, None, None, None, None, None, None,
+                gres, None, None, None, None, None, None, None,
                 sc_gw, sc_dg, sc_db, None, None, None, None, None, None, None)
 
 
@@ -1157,36 +1190,26 @@ def conv_bn_add(x, weight, gamma, beta, residual, running_mean, running_var, mom
     own activation pack; x's own `_bdbnn_pack` (if present and of the current format) is consumed.
     `hardtanh`: z = hardtanh(BN_train(binconv2d(x, weight))) without residual (the VGG-Small units, DESIGN.md §4n);
     the mask bits of z's pack are Hardtanh's strict -1 < u < 1 and the backward applies that mask to gz."""
-    fmt = grad_mode()[3]
-    pk = _get_act_pack(x, fmt)
-    xs, xm, xb, xb8 = (pk.sign, pk.mask, pk.xb, pk.xb8) if pk is not None else (None,) * 4
     res_is_x = residual is x and x.shape[1] == weight.shape[0] and int(stride) == 1
+    sc, sc_pad = (None,) * 8, None       # the 1x1 shortcut's arguments, the option-A shortcut's pad
     if hardtanh:
         if residual is not None or shortcut is not None or weight.shape[0] % 32:
             raise RuntimeError("conv_bn_add: hardtanh needs Cout % 32 == 0 and neither residual nor shortcut")
-        z, zs, zm, zb, zb8 = _ConvBNAddUnit.apply(x, weight, gamma, beta, None, running_mean, running_var, momentum,
-                                                  eps, int(stride), int(padding), xs, xm, xb, xb8, False,
-                                                  *([None] * 9), True)
-    elif isinstance(shortcut, PadShortcut):
-        if residual is not None:
-            raise RuntimeError("conv_bn_add: pass either residual or shortcut")
-        if not pad_shortcut_supported(x.shape, weight.shape, stride, shortcut.pad):
-            raise RuntimeError(f"conv_bn_add: option-A shortcut with pad {shortcut.pad} does not fit input "
-                               f"{tuple(x.shape)}, weight {tuple(weight.shape)}, stride {stride}")
-        z, zs, zm, zb, zb8 = _ConvBNAddUnit.apply(x, weight, gamma, beta, None, running_mean, running_var, momentum,
-                                                  eps, int(stride), int(padding), xs, xm, xb, xb8, False,
-                                                  *([None] * 8), int(shortcut.pad))
     elif shortcut is not None:
         if residual is not None:
             raise RuntimeError("conv_bn_add: pass either residual or shortcut")
-        z, zs, zm, zb, zb8 = _ConvBNAddUnit.apply(x, weight, gamma, beta, None, running_mean, running_var, momentum,
-                                                  eps, int(stride), int(padding), xs, xm, xb, xb8, False, *shortcut)
-    else:
-        z, zs, zm, zb, zb8 = _ConvBNAddUnit.apply(x, weight, gamma, beta, None if res_is_x else residual,
-                                                  running_mean, running_var, momentum, eps, int(stride),
-                                                  int(padding), xs, xm, xb, xb8, res_is_x)
+        if not isinstance(shortcut, PadShortcut):
+            sc = tuple(shortcut)
+        elif pad_shortcut_supported(x.shape, weight.shape, stride, shortcut.pad):
+            sc_pad = int(shortcut.pad)
+        else:
+            raise RuntimeError(f"conv_bn_add: option-A shortcut with pad {shortcut.pad} does not fit input "
+                               f"{tuple(x.shape)}, weight {tuple(weight.shape)}, stride {stride}")
+    z, zs, zm, zb, zb8 = _ConvBNAddUnit.apply(x, weight, gamma, beta, None if res_is_x else residual, running_mean,
+                                              running_var, momentum, eps, int(stride), int(padding), res_is_x, *sc,
+                                              sc_pad, bool(hardtanh))
     if zs is not None:
-        _set_act_pack(z, _ActPack(zs, zm, zb, fmt, zb8))
+        _set_act_pack(z, _ActPack(zs, zm, zb, grad_mode()[3], zb8))
         z._bdbnn_bnctx = _ConvBNAddUnit._last_bnctx      # (y_int, alpha, mean, invstd) of this unit, or None
     _ConvBNAddUnit._last_bnctx = None
     return z
@@ -1269,11 +1292,7 @@ def _shortcut_bwd_impl(gz, saved, geom, need_x, need_w, acc=None, w_param=None):
     key = _shape_key(shs)
     g = _nhwc(gz)
     i32 = dict(dtype=torch.int32, device=dev)
-    f32 = dict(dtype=torch.float32, device=dev)
-    sums = torch.empty((2 * cout,), dtype=torch.float64, device=dev)
-    gmax, amax = torch.empty((cout,), **i32), torch.empty((1,), **i32)
-    consts, dgamma, dbeta = torch.empty((4 * cout,), **f32), torch.empty((cout,), **f32), torch.empty((cout,), **f32)
-    gys = torch.empty((sh1.N, sh1.Ho, sh1.Wo, cout), dtype=torch.int16, device=dev)
+    sums, gmax, consts, dgamma, dbeta, amax, gys = _bn_grads(cout, (sh1.N, sh1.Ho, sh1.Wo), 1, dev)
     with _timed("shortcut_bn_bwd", key, 18 * n_pix * cout):
         _lib.check(L.bdbnn_bn_bwd_pack(_p(g), _p(y), _p(mean), _p(invstd), _p(gamma), _p(gscale), _p(ymax), n_pix,
                                        cout, 3, _p(sums), _p(gmax), _p(consts), _p(dgamma), _p(dbeta), _p(amax),
@@ -1282,11 +1301,10 @@ def _shortcut_bwd_impl(gz, saved, geom, need_x, need_w, acc=None, w_param=None):
     gx = gw = None
     if need_x:
         ones = torch.full((x_shape[0], x_shape[2], x_shape[3], (cin + 31) // 32), -1, **i32)
-        gx = acc if acc is not None else torch.empty(x_shape, memory_format=torch.channels_last, **f32)
-        with _timed("shortcut_dgrad_tc", key, 2 * gys.numel() + (4 * gx.numel() if acc is None else 8 * n_pix * cin)):
-            _lib.check(L.bdbnn_binconv_dgrad_tc(_p(gys), 3, _p(amax), _p(wt), _p(ones), _p(acc), _p(gx),
-                                                ctypes.byref(shs), st), "binconv_dgrad_tc(shortcut)")
-        _lib.count(_dgrad_launches(shs))
+        gx = acc if acc is not None else torch.empty(x_shape, dtype=torch.float32, device=dev,
+                                                     memory_format=torch.channels_last)
+        _dgrad_tc(shs, gys, 3, amax, wt, ones, acc, gx, "shortcut_dgrad_tc",
+                  2 * gys.numel() + (4 * gx.numel() if acc is None else 8 * n_pix * cin))
     if need_w:
         wones = torch.full(((cout * cin + 31) // 32,), -1, **i32)
         gw = _wgrad_tc(sh1, gys, 3, amax, xh, wones, inv_gscale, w_shape, w_param, "shortcut_wgrad_tc", key,
@@ -1670,23 +1688,17 @@ class _CifarStem(torch.autograd.Function):
         st = _stream()
         key = f"cifar_stem_N{n}_{h}x{w}_c{cout}"
         g = _nhwc(gz)
-        i32 = dict(dtype=torch.int32, device=dev)
-        f32 = dict(dtype=torch.float32, device=dev)
-        sums = torch.empty((2 * cout,), dtype=torch.float64, device=dev)
-        gmax, amax = torch.empty((cout,), **i32), torch.empty((1,), **i32)
-        consts, dgamma, dbeta = torch.empty((4 * cout,), **f32), torch.empty((cout,), **f32), torch.empty((cout,), **f32)
-        ones = torch.ones((cout,), **f32)
-        gys = torch.empty((n, h, w, cout), dtype=torch.int16, device=dev)
+        sums, gmax, consts, dgamma, dbeta, amax, gys = _bn_grads(cout, (n, h, w), 1, dev)
+        ones = torch.ones((cout,), dtype=torch.float32, device=dev)
+        out = (3, _p(sums), _p(gmax), _p(consts), _p(dgamma), _p(dbeta), _p(amax), _p(gys), st)
         with _timed("cifar_stem_bn_bwd", key, 18 * n_pix * cout):
             if ctx.hardtanh:
                 _lib.check(L.bdbnn_bn_bwd_pack_hardtanh(_p(g), _p(y), None, _p(ctx.saved_tensors[6]), _p(mean),
-                                                        _p(invstd), _p(gamma), _p(ones), _p(ymax), n_pix, cout, 3,
-                                                        _p(sums), _p(gmax), _p(consts), _p(dgamma), _p(dbeta), _p(amax),
-                                                        _p(gys), st), "bn_bwd_pack_hardtanh(cifar stem)")
+                                                        _p(invstd), _p(gamma), _p(ones), _p(ymax), n_pix, cout, *out),
+                           "bn_bwd_pack_hardtanh(cifar stem)")
             else:
                 _lib.check(L.bdbnn_bn_bwd_pack(_p(g), _p(y), _p(mean), _p(invstd), _p(gamma), _p(ones), _p(ymax),
-                                               n_pix, cout, 3, _p(sums), _p(gmax), _p(consts), _p(dgamma), _p(dbeta),
-                                               _p(amax), _p(gys), st), "bn_bwd_pack(cifar stem)")
+                                               n_pix, cout, *out), "bn_bwd_pack(cifar stem)")
         _lib.count(3)
         gw = None
         if ctx.needs_input_grad[1]:
@@ -1797,22 +1809,11 @@ def conv_bn_add_eval(x, weight, gamma, beta, running_mean, running_var, eps, str
     key = _shape_key(sh)
     pack = cout % 32 == 0
     out8 = pack and cout % 128 == 0 and fwd8_enabled()
-    use8 = bool(caps & 8) and use_fwd8(sh.Cin, cout, eval_unit=True)
+    use8, xop, wp = _unit_operands(x, weight, sh, caps, train=False)
     if pad_sc and use8:
         raise RuntimeError("bdbnn_b200.conv_bn_add_eval: the option-A shortcut needs 16-bit operands (fp8 forward "
                            f"chosen for {sh.Cin} input channels)")
     want = -1 if use8 else fmt
-    pk = getattr(x, "_bdbnn_eval_pack", None)
-    if pk is not None and pk[0] == want and x._bdbnn_eval_pack_version == x._version:
-        xop = pk[1]
-    else:
-        ap = _act_pack(x, sh, fmt, xb=not use8, xb8=use8)
-        xop = ap.xb8 if use8 else ap.xb
-    # packed with every binary conv of the network at the start of this forward (prepack_weights)
-    wp = _prepacked(weight, fmt, use8)
-    if wp is None:
-        wp = _alloc_weight_pack(weight.shape, dev, wf=not use8, wf8=use8)
-        _weight_pack(weight, wp, fmt)
     alpha, wop = wp.alpha, (wp.wf8 if use8 else wp.wf)
     scale, shift = bn_eval_fold(gamma, beta, running_mean, running_var, eps, alpha)
     rc = _nhwc(residual.detach()) if residual is not None else None
@@ -1835,9 +1836,8 @@ def conv_bn_add_eval(x, weight, gamma, beta, running_mean, running_var, eps, str
             _lib.check(L.bdbnn_binconv_fwd_tc_eval(_p(xop), _p(wop), want, _p(scale), _p(shift), _p(rc), _p(z),
                                                    _p(zb), _p(zb8), ctypes.byref(sh), st), "binconv_fwd_tc_eval")
     _lib.count(1)
-    if pack and not z.is_inference():       # inference tensors have no version counter to guard the copy with
-        z._bdbnn_eval_pack = (-1, zb8) if out8 else (fmt, zb)
-        z._bdbnn_eval_pack_version = z._version
+    if pack:
+        _set_eval_pack(z, *((-1, zb8) if out8 else (fmt, zb)))
     return z
 
 
@@ -1974,6 +1974,21 @@ def real_weight_pack(weights):
     return list(zip(wf, alpha))
 
 
+def _real_act_pack(x, x_amax, sh):
+    """real_act_pack of x for the conv sh.  x_amax: the device word of max|x| a previous call returned (None: computed
+    here, one more pass over x).  Returns (x NHWC, its fp16 operand, the amax word the operand was scaled by)."""
+    xc = _nhwc(x.detach())
+    xh = torch.empty((sh.N, sh.H, sh.W, sh.Cin), dtype=torch.int16, device=x.device)
+    have = x_amax is not None
+    amax = x_amax if have else torch.empty((1,), dtype=torch.int32, device=x.device)
+    n_in = xc.numel()
+    with _timed("real_act_pack", _shape_key(sh), 4 * n_in + 2 * n_in):
+        _lib.check(_lib.lib().bdbnn_real_act_pack(_p(xc), sh.N * sh.H * sh.W, sh.Cin, _p(amax), int(have), _p(xh),
+                                                  _stream()), "real_act_pack")
+    _lib.count(1 if have else 2)
+    return xc, xh, amax
+
+
 @_on_x_device
 def real_conv_bn_eval(x, x_amax, wpack, gamma, beta, running_mean, running_var, eps, stride, padding, residual=None,
                       relu=True, shortcut=None, hardtanh=False):
@@ -2009,14 +2024,7 @@ def real_conv_bn_eval(x, x_amax, wpack, gamma, beta, running_mean, running_var, 
     dev = x.device
     st = _stream()
     key = _shape_key(sh)
-    xc = _nhwc(x.detach())
-    xh = torch.empty((n, h, w, cin), dtype=torch.int16, device=dev)
-    have = x_amax is not None
-    amax = x_amax if have else torch.empty((1,), dtype=torch.int32, device=dev)
-    n_in = xc.numel()
-    with _timed("real_act_pack", key, 4 * n_in + 2 * n_in):
-        _lib.check(L.bdbnn_real_act_pack(_p(xc), n * h * w, cin, _p(amax), int(have), _p(xh), st), "real_act_pack")
-    _lib.count(1 if have else 2)
+    xc, xh, amax = _real_act_pack(x, x_amax, sh)
     scale, shift = bn_eval_fold(gamma, beta, running_mean, running_var, eps, alpha)
     rc = _nhwc(residual.detach()) if residual is not None else None
     z = torch.empty(z_shape, dtype=torch.float32, device=dev, memory_format=torch.channels_last)
@@ -2051,7 +2059,7 @@ def real_conv_pool_bn_eval(x, x_amax, wpack, gamma, beta, running_mean, running_
     wf, alpha = wpack
     _same_device(x, wf, gamma, beta, running_mean, running_var)
     L = _lib.lib()
-    n, cin, h, w = x.shape
+    n = x.shape[0]
     cout, taps, cin_w = wf.shape
     k = int(round(taps ** 0.5))
     sh = conv_shape(x.shape, (cout, cin_w, k, k), 1, padding)
@@ -2063,14 +2071,7 @@ def real_conv_pool_bn_eval(x, x_amax, wpack, gamma, beta, running_mean, running_
     dev = x.device
     st = _stream()
     key = _shape_key(sh)
-    xc = _nhwc(x.detach())
-    xh = torch.empty((n, h, w, cin), dtype=torch.int16, device=dev)
-    have = x_amax is not None
-    amax = x_amax if have else torch.empty((1,), dtype=torch.int32, device=dev)
-    n_in = xc.numel()
-    with _timed("real_act_pack", key, 4 * n_in + 2 * n_in):
-        _lib.check(L.bdbnn_real_act_pack(_p(xc), n * h * w, cin, _p(amax), int(have), _p(xh), st), "real_act_pack")
-    _lib.count(1 if have else 2)
+    _, xh, amax = _real_act_pack(x, x_amax, sh)
     y = torch.empty((n, sh.Ho, sh.Wo, cout), dtype=torch.float32, device=dev)
     # -0.0 is the identity of fp32 addition (+0.0 would turn a -0.0 conv output into +0.0 and move a pool's tie)
     no_shift = torch.full((cout,), -0.0, dtype=torch.float32, device=dev)
@@ -2157,14 +2158,14 @@ def pool_unit_supported(x_shape, w_shape, stride, padding):
 
 class _ConvPoolBNUnit(torch.autograd.Function):
     """z = hardtanh(BN_train(maxpool2x2(binconv2d(x, weight)))).
-    forward : [act_pack(x)] -> fwd_tc_i16 (no statistics) -> pool2_i16 (p, winner, statistics of alpha*p) ->
-              bn_fwd_hardtanh(p) (z + the next conv's packs)
+    forward : [act_pack(x) unless x carries its producer's packs] -> fwd_tc_i16 (no statistics) -> pool2_i16 (p,
+              winner, statistics of alpha*p) -> bn_fwd_hardtanh(p) (z + the next conv's packs)
     backward: pool2_bn_bwd_pack (BN + Hardtanh backward on the pooled tensor, gys at the winners) -> wgrad_tc, dgrad_tc.
     Saved for backward: the pooled int16 p, the winner bytes, x's mask bits and +-1 copy, the weight operands."""
 
     @staticmethod
     @_on_device
-    def forward(ctx, x, weight, gamma, beta, running_mean, running_var, momentum, eps, padding, xs, xm, xb, xb8):
+    def forward(ctx, x, weight, gamma, beta, running_mean, running_var, momentum, eps, padding):
         _require_cuda(x, "conv_pool_bn(x)")
         _same_device(x, weight, gamma, beta, running_mean, running_var)
         if not pool_unit_supported(x.shape, weight.shape, 1, padding):
@@ -2180,19 +2181,9 @@ class _ConvPoolBNUnit(torch.autograd.Function):
         key = _shape_key(sh)
         i32 = dict(dtype=torch.int32, device=dev)
         f32 = dict(dtype=torch.float32, device=dev)
-        use8 = bool(int(L.bdbnn_tc_supported(ctypes.byref(sh))) & 8) and use_fwd8(sh.Cin, cout, eval_unit=False)
-        ap = _act_pack(x, sh, fmt, xb=True, xb8=use8, have=None if xs is None else _ActPack(xs, xm, xb, fmt, xb8))
-        wp = _prepacked(weight, fmt, use8)
-        if wp is None:
-            wp = _alloc_weight_pack(weight.shape, dev, wf=not use8, wf8=use8, grad=True)
-            _weight_pack(weight, wp, fmt)
+        use8, ap, wp = _unit_operands(x, weight, sh, int(L.bdbnn_tc_supported(ctypes.byref(sh))), train=True)
         y = torch.empty((n, sh.Ho, sh.Wo, cout), dtype=torch.int16, device=dev)
-        with _timed("binconv_fwd_tc8" if use8 else "binconv_fwd_tc", key,
-                    algorithmic_bytes("fwd_tc8" if use8 else "fwd_tc", sh) - 2 * y.numel()):
-            _lib.check(L.bdbnn_binconv_fwd_tc_i16(_p(ap.xb8) if use8 else _p(ap.xb), _p(wp.wf8) if use8 else _p(wp.wf),
-                                                  -1 if use8 else fmt, _p(wp.alpha), _p(y), ctypes.byref(sh), None,
-                                                  None, st), "binconv_fwd_tc_i16")
-        _lib.count(1)
+        _fwd_tc(sh, use8, ap, wp, fmt, y)
         p = torch.empty((n, ho, wo, cout), dtype=torch.int16, device=dev)
         idx = torch.empty((n, ho, wo, cout), dtype=torch.uint8, device=dev)
         sums = torch.empty((2 * cout,), dtype=torch.float64, device=dev)
@@ -2227,27 +2218,21 @@ class _ConvPoolBNUnit(torch.autograd.Function):
     @_on_device
     def backward(ctx, gz, *_unused):
         if gz is None:
-            return (None,) * 13
+            return (None,) * 9
         L = _lib.lib()
         sh = ctx.sh
-        st = _stream()
         dev = gz.device
         p, idx, alpha, ab, mean, invstd, gamma, ymax, xm, xb, wt, wmask, gscale, inv_gscale = ctx.saved_tensors
         gname, gcode, gh = ctx.gmode
         key = _shape_key(sh)
         cout = sh.Cout
-        i32 = dict(dtype=torch.int32, device=dev)
-        f32 = dict(dtype=torch.float32, device=dev)
-        sums = torch.empty((2 * cout,), dtype=torch.float64, device=dev)
-        gmax, amax = torch.empty((cout,), **i32), torch.empty((1,), **i32)
-        consts, dgamma, dbeta = torch.empty((4 * cout,), **f32), torch.empty((cout,), **f32), torch.empty((cout,), **f32)
-        gys = torch.empty((sh.N, sh.Ho, sh.Wo, gh * cout), dtype=torch.int16, device=dev)
+        sums, gmax, consts, dgamma, dbeta, amax, gys = _bn_grads(cout, (sh.N, sh.Ho, sh.Wo), gh, dev)
         n_pool = p.numel()
         with _timed("pool2_bn_bwd_pack", key, 2 * (4 + 2 + 1) * n_pool + 2 * gys.numel()):
             _lib.check(L.bdbnn_pool2_bn_bwd_pack(_p(_nhwc(gz)), _p(p), _p(idx), _p(alpha), _p(ab), _p(mean), _p(invstd),
                                                  _p(gamma), _p(gscale), _p(ymax), sh.N, sh.Ho, sh.Wo, cout, gcode,
                                                  _p(sums), _p(gmax), _p(consts), _p(dgamma), _p(dbeta), _p(amax),
-                                                 _p(gys), st), "pool2_bn_bwd_pack")
+                                                 _p(gys), _stream()), "pool2_bn_bwd_pack")
         _lib.count(3)
         x_shape, w_shape = ctx.shapes
         gx = gw = None
@@ -2256,12 +2241,10 @@ class _ConvPoolBNUnit(torch.autograd.Function):
                            algorithmic_bytes("wgrad_tc", sh, gh))
         if ctx.needs_input_grad[0]:
             gx = torch.empty(x_shape, dtype=torch.float32, device=dev, memory_format=torch.channels_last)
-            with _timed("binconv_dgrad_tc", key, algorithmic_bytes("dgrad_tc", sh, gh)):
-                _lib.check(L.bdbnn_binconv_dgrad_tc(_p(gys), gcode, _p(amax), _p(wt), _p(xm), _p(None), _p(gx),
-                                                    ctypes.byref(sh), st), "binconv_dgrad_tc")
-            _lib.count(_dgrad_launches(sh))
+            _dgrad_tc(sh, gys, gcode, amax, wt, xm, None, gx, "binconv_dgrad_tc",
+                      algorithmic_bytes("dgrad_tc", sh, gh))
         return (gx, gw, dgamma if ctx.needs_input_grad[2] else None, dbeta if ctx.needs_input_grad[3] else None,
-                None, None, None, None, None, None, None, None, None)
+                None, None, None, None, None)
 
 
 def conv_pool_bn(x, weight, gamma, beta, running_mean, running_var, momentum, eps, padding=1):
@@ -2269,12 +2252,9 @@ def conv_pool_bn(x, weight, gamma, beta, running_mean, running_var, momentum, ep
     the pooled VGG-Small unit.  The winner of each window is the first maximum in scan order, as torch.nn.MaxPool2d's;
     BatchNorm updates its running statistics (the caller adds 1 to num_batches_tracked).  Like conv_bn_add, x's
     `_bdbnn_pack` is consumed and the result carries its own, with Hardtanh's strict mask."""
-    fmt = grad_mode()[3]
-    pk = _get_act_pack(x, fmt)
-    xs, xm, xb, xb8 = (pk.sign, pk.mask, pk.xb, pk.xb8) if pk is not None else (None,) * 4
     z, zs, zm, zb, zb8 = _ConvPoolBNUnit.apply(x, weight, gamma, beta, running_mean, running_var, momentum, eps,
-                                               int(padding), xs, xm, xb, xb8)
-    _set_act_pack(z, _ActPack(zs, zm, zb, fmt, zb8))
+                                               int(padding))
+    _set_act_pack(z, _ActPack(zs, zm, zb, grad_mode()[3], zb8))
     return z
 
 
@@ -2297,24 +2277,9 @@ def conv_pool_bn_eval(x, weight, gamma, beta, running_mean, running_var, eps, pa
     fmt = grad_mode()[3]
     st = _stream()
     key = _shape_key(sh)
-    use8 = bool(int(L.bdbnn_tc_supported(ctypes.byref(sh))) & 8) and use_fwd8(sh.Cin, cout, eval_unit=True)
-    want = -1 if use8 else fmt
-    pk = getattr(x, "_bdbnn_eval_pack", None)
-    if pk is not None and pk[0] == want and x._bdbnn_eval_pack_version == x._version:
-        xop = pk[1]
-    else:
-        ap = _act_pack(x, sh, fmt, xb=not use8, xb8=use8)
-        xop = ap.xb8 if use8 else ap.xb
-    wp = _prepacked(weight, fmt, use8)
-    if wp is None:
-        wp = _alloc_weight_pack(weight.shape, dev, wf=not use8, wf8=use8)
-        _weight_pack(weight, wp, fmt)
+    use8, xop, wp = _unit_operands(x, weight, sh, int(L.bdbnn_tc_supported(ctypes.byref(sh))), train=False)
     y = torch.empty((n, sh.Ho, sh.Wo, cout), dtype=torch.int16, device=dev)
-    with _timed("binconv_fwd_tc8" if use8 else "binconv_fwd_tc", key,
-                algorithmic_bytes("fwd_tc8" if use8 else "fwd_tc", sh) - 2 * y.numel()):
-        _lib.check(L.bdbnn_binconv_fwd_tc_i16(_p(xop), _p(wp.wf8) if use8 else _p(wp.wf), want, _p(wp.alpha), _p(y),
-                                              ctypes.byref(sh), None, None, st), "binconv_fwd_tc_i16")
-    _lib.count(1)
+    _fwd_tc(sh, use8, xop, wp, fmt, y)
     scale, shift = bn_eval_fold(gamma, beta, running_mean, running_var, eps, wp.alpha)
     out8 = cout % 128 == 0 and fwd8_enabled()
     z = torch.empty((n, cout, ho, wo), dtype=torch.float32, device=dev, memory_format=torch.channels_last)
@@ -2324,7 +2289,5 @@ def conv_pool_bn_eval(x, weight, gamma, beta, running_mean, running_var, eps, pa
         _lib.check(L.bdbnn_pool2_bn_eval_hardtanh(_p(y), _p(scale), _p(shift), n, sh.Ho, sh.Wo, cout, _p(z), _p(zb),
                                                   _p(zb8), fmt, st), "pool2_bn_eval_hardtanh")
     _lib.count(1)
-    if not z.is_inference():
-        z._bdbnn_eval_pack = (-1, zb8) if out8 else (fmt, zb)
-        z._bdbnn_eval_pack_version = z._version
+    _set_eval_pack(z, *((-1, zb8) if out8 else (fmt, zb)))
     return z
