@@ -110,6 +110,13 @@ SIGNATURES = {
     "bdbnn_cifar_batch": (c_int, [_P, _P, c_int64, ctypes.c_uint64, ctypes.c_uint32, c_int64, c_int, c_int, _P, _P, _P,
                                   c_int64, c_int64, c_int64, c_int64, _P, _P]),
     "bdbnn_imagenet_batch": (c_int, [_P, _P, c_int, _P, _P, _P, c_int64, c_int64, c_int64, c_int64, _P, _P]),
+    "bdbnn_jpeg_parse": (c_int, [ctypes.c_char_p, c_int64, _P, _P, c_int64, _P, c_int]),
+    "bdbnn_jpeg_subseq_bits": (c_int, []),
+    "bdbnn_debug_jpeg_subseq_bits": (c_int, [c_int]),
+    "bdbnn_jpeg_workspace_bytes": (c_size_t, [c_int64, c_int64]),
+    "bdbnn_jpeg_check_batch": (c_int, [_P, c_int, _P, c_int, c_int64, c_int64, c_size_t]),
+    "bdbnn_jpeg_decode_batch": (c_int, [_P, _P, c_int, _P, _P, c_int, _P, _P, c_int64, _P, c_size_t, _P, c_int64, _P,
+                                        _P, _P, _P]),
 }
 
 

@@ -375,6 +375,95 @@ def _jpeg_components(data):
     return 0
 
 
+# bdbnn_jpeg_desc / bdbnn_jpeg_seg (include/bdbnn.h): the fields the host reads and sets, then the tables
+_JDESC = np.dtype([("H", "<i4"), ("W", "<i4"), ("ncomp", "<i4"), ("hmax", "<i4"), ("vmax", "<i4"), ("mcux", "<i4"),
+                   ("mcuy", "<i4"), ("bpm", "<i4"), ("restart", "<i4"), ("nseg", "<i4"), ("data_bytes", "<i4"),
+                   ("reserved", "<i4"), ("data_off", "<i8"), ("coef_off", "<i8"), ("rgb_off", "<i8"),
+                   ("blk_comp", "u1", 8), ("comp_dc", "u1", 4), ("comp_ac", "u1", 4), ("qt", "<u2", (3, 64)),
+                   ("huff", "V5680")])
+assert _JDESC.itemsize == 6152
+_JSEG = np.dtype([("off", "<i8"), ("img", "<i4"), ("nbytes", "<i4"), ("mcu0", "<i4"), ("nmcu", "<i4"),
+                  ("sub0", "<i4"), ("nsub", "<i4")])
+assert _JSEG.itemsize == 32
+
+
+def jpeg_parse(data):
+    """bdbnn_jpeg_parse of one file: (descriptor record, unstuffed entropy-coded bytes, [segment start offsets]), or
+    None when the device decoder does not take the file."""
+    desc = np.zeros(1, _JDESC)
+    out = np.empty(len(data) + 16, np.uint8)
+    seg = np.empty(len(data) // 3 + 2, np.uint32)
+    rc = _lib.lib().bdbnn_jpeg_parse(bytes(data), len(data), desc.ctypes.data, out.ctypes.data, out.size,
+                                     seg.ctypes.data, seg.size)
+    if rc == -3:                                 # BDBNN_ERR_UNSUPPORTED
+        return None
+    _lib.check(rc, "jpeg_parse")
+    return desc[0], out[:int(desc["data_bytes"][0])].tobytes(), seg[:int(desc["nseg"][0])].tolist()
+
+
+def jpeg_segment_table(descs, rel_off, subseq_bits):
+    """bdbnn_jpeg_seg rows of a batch: descs (_JDESC, data_off set), rel_off[i] the segment start offsets of image i
+    (relative to its data).  Segment k of image i holds MCUs [k R, min((k + 1) R, total)), R the restart interval
+    (total without one), and max(1, ceil(8 bytes / subseq_bits)) subsequences."""
+    nseg = descs["nseg"].astype(np.int64)
+    n = int(nseg.sum())
+    img = np.repeat(np.arange(len(descs)), nseg)
+    first = np.concatenate([[0], np.cumsum(nseg)[:-1]]).astype(np.int64)
+    local = np.arange(n) - first[img]
+    rel = np.concatenate(rel_off).astype(np.int64) if n else np.zeros(0, np.int64)
+    end = np.empty(n, np.int64)
+    end[:-1] = rel[1:]
+    end[first + nseg - 1] = descs["data_bytes"]
+    total = descs["mcux"].astype(np.int64) * descs["mcuy"]
+    R = np.where(descs["restart"] > 0, descs["restart"], total)
+    segs = np.zeros(n, _JSEG)
+    segs["off"] = descs["data_off"][img] + rel
+    segs["img"] = img
+    segs["nbytes"] = end - rel
+    segs["mcu0"] = local * R[img]
+    segs["nmcu"] = np.minimum(R[img], total[img] - local * R[img])
+    nsub = np.maximum(1, (8 * (end - rel) + subseq_bits - 1) // subseq_bits)
+    segs["nsub"] = nsub
+    segs["sub0"] = np.concatenate([[0], np.cumsum(nsub)[:-1]])
+    return segs
+
+
+def jpeg_batch_layout(descs):
+    """Set coef_off and rgb_off of a batch's descriptors (images back to back); returns (blocks, pixels)."""
+    blocks = descs["mcux"].astype(np.int64) * descs["mcuy"] * descs["bpm"]
+    pix = descs["H"].astype(np.int64) * descs["W"]
+    descs["coef_off"] = np.concatenate([[0], np.cumsum(blocks)[:-1]])
+    descs["rgb_off"] = 3 * np.concatenate([[0], np.cumsum(pix)[:-1]])
+    return int(blocks.sum()), int(pix.sum())
+
+
+def jpeg_decode_batch(descs, segs, staging, device, stream):
+    """bdbnn_jpeg_decode_batch on `stream`: descs (_JDESC, every offset set), segs (_JSEG), staging the uint8 host
+    tensor (pinned) holding the images' unstuffed data.  Returns (rgb uint8 device tensor, pinned int32 status per
+    image, pinned int32 [1] synchronisation rounds, workspace tensor); all are ready, and staging may be rewritten,
+    once `stream` has run the queued work."""
+    lib = _lib.lib()
+    n_blocks, n_pix = int((descs["mcux"].astype(np.int64) * descs["mcuy"] * descs["bpm"]).sum()), \
+        int((descs["H"].astype(np.int64) * descs["W"]).sum())
+    n_sub = int(segs["nsub"].astype(np.int64).sum())
+    data_bytes = int(staging.numel())
+    with torch.cuda.device(device), torch.cuda.stream(stream):
+        data_dev = torch.empty(max(data_bytes, 1), dtype=torch.uint8, device=device)
+        desc_dev = torch.empty(descs.nbytes, dtype=torch.uint8, device=device)
+        seg_dev = torch.empty(segs.nbytes, dtype=torch.uint8, device=device)
+        work = torch.empty(lib.bdbnn_jpeg_workspace_bytes(n_blocks, n_sub), dtype=torch.uint8, device=device)
+        rgb = torch.empty(3 * n_pix, dtype=torch.uint8, device=device)
+        status_dev = torch.empty(len(descs), dtype=torch.int32, device=device)
+        status = torch.empty(len(descs) + 1, dtype=torch.int32, pin_memory=True)
+        _lib.check(lib.bdbnn_jpeg_decode_batch(
+            descs.ctypes.data, desc_dev.data_ptr(), len(descs), segs.ctypes.data, seg_dev.data_ptr(), len(segs),
+            staging.data_ptr(), data_dev.data_ptr(), data_bytes, work.data_ptr(), work.numel(), rgb.data_ptr(),
+            rgb.numel(), status_dev.data_ptr(), status.data_ptr(), status.data_ptr() + 4 * len(descs),
+            ctypes.c_void_p(stream.cuda_stream)), "jpeg_decode_batch")
+    _lib.count(6)
+    return rgb, status[:len(descs)], status[len(descs):], work
+
+
 def _pil_decode(data):
     """uint8 HWC [H, W, 3] of an image file through PIL (Image.open(f).convert('RGB'), as ImageFolder's loader)."""
     from PIL import Image
@@ -473,6 +562,12 @@ class ImageNetDeviceLoader:
     §4m).  Files that are not 1- or 3-component JPEGs (CMYK JPEGs, PNGs under a .JPEG name) and files
     the decoder rejects are decoded with PIL (Image.open(f).convert('RGB'), ImageFolder's loader), one at a time.
     With decode='cpu' every batch is bit-identical to torchvision's PIL transform chain for the same crop parameters.
+    decode='kernel' decodes baseline JPEGs on the device with this repository's kernels (csrc/jpeg_decode.cu): the
+    pool threads only parse headers and copy the unstuffed entropy-coded data into pinned memory, and the Huffman
+    decode, IDCT, upsampling and colour conversion of the batch run on the loader's stream, with libjpeg-turbo's
+    integer arithmetic, so the batches are bit-identical to decode='cpu' (and to the PIL chain).  Files the device
+    decoder does not take (progressive, CMYK, PNG, other sampling, ...; include/bdbnn.h) or flags while decoding
+    (corrupt data) are decoded as in decode='cpu', one at a time; decode_stats counts them.
 
     The training split is shuffled by the epoch permutation of §4l and sharded as CifarDeviceLoader (shard_spans);
     the validation split is read in order, as the reference's (shuffle=train_flag).  Crop and flip are pure functions
@@ -482,8 +577,8 @@ class ImageNetDeviceLoader:
 
     def __init__(self, root, batch_size, train, seed=None, drop_last=False, rank=0, world_size=1, device=None, *,
                  decode="cpu", workers=16, mean=IMAGENET_MEAN, std=IMAGENET_STD):
-        if decode not in ("cuda", "cpu"):
-            raise ValueError(f"ImageNetDeviceLoader: decode must be 'cuda' or 'cpu', got {decode!r}")
+        if decode not in ("cuda", "cpu", "kernel"):
+            raise ValueError(f"ImageNetDeviceLoader: decode must be 'cpu', 'cuda' or 'kernel', got {decode!r}")
         if int(batch_size) < 1 or int(world_size) < 1 or not 0 <= int(rank) < int(world_size) or int(workers) < 1:
             raise ValueError(f"ImageNetDeviceLoader: need batch_size >= 1, workers >= 1 and 0 <= rank < world_size, "
                              f"got {batch_size}, {workers}, {rank}, {world_size}")
@@ -510,6 +605,10 @@ class ImageNetDeviceLoader:
         self._pending = None                     # ((epoch, batch index), future of _prepare)
         self._stream = torch.cuda.Stream(device)
         self._staging = [None, None]             # decode='cpu': pinned buffers used in turn, with their copy events
+        self._jstage = None                      # decode='kernel': pinned buffer of the unstuffed data
+        # decode='kernel': files decoded on the device, parse rejections, device flags, most synchronisation rounds
+        # of a block
+        self.decode_stats = {"device": 0, "rejected": 0, "flagged": 0, "rounds": 0}
         self._turn = 0
         self._lock = threading.Lock()
         self._next_epoch = 0
@@ -606,12 +705,64 @@ class ImageNetDeviceLoader:
         st[1].record(self._stream)
         return [(buf[int(offs[i]):int(offs[i + 1])].view(t.shape), hwc) for i, (t, hwc) in enumerate(dec)]
 
+    def _decode_kernel(self, blobs):
+        """[(device tensor, hwc)] of the batch's files: header parse and unstuffing in the pool, one
+        bdbnn_jpeg_decode_batch on self._stream, then a wait for its status words (this runs in the read-ahead
+        thread) and _host_decode for the files the parse rejected or the device flagged."""
+        lib = _lib.lib()
+        B = len(blobs)
+        size = np.array([len(b) for b in blobs], np.int64)
+        data_off = np.concatenate([[0], np.cumsum((size + 16) // 16 * 16)])
+        seg_cap = size // 3 + 2
+        seg_base = np.concatenate([[0], np.cumsum(seg_cap)])
+        # the previous call waited for its decode, so nothing reads this buffer any more
+        if self._jstage is None or self._jstage.numel() < data_off[-1]:
+            self._jstage = torch.empty(int(data_off[-1] * 1.25) + 4096, dtype=torch.uint8, pin_memory=True)
+        stage = self._jstage
+        descs = np.zeros(B, _JDESC)
+        seg_off = np.empty(int(seg_base[-1]), np.uint32)
+
+        def parse(k):
+            return lib.bdbnn_jpeg_parse(blobs[k], len(blobs[k]), descs.ctypes.data + k * _JDESC.itemsize,
+                                        stage.data_ptr() + int(data_off[k]), int(size[k]),
+                                        seg_off.ctypes.data + 4 * int(seg_base[k]), int(seg_cap[k]))
+        rc = list(self._pool.map(parse, range(B)))
+        for k in range(B):
+            if rc[k] not in (0, -3):             # -3: BDBNN_ERR_UNSUPPORTED, the host decodes the file
+                _lib.check(rc[k], "jpeg_parse")
+        acc = [k for k in range(B) if rc[k] == 0]
+        out = [None] * B
+        if acc:
+            a = descs[acc]
+            a["data_off"] = data_off[acc]
+            jpeg_batch_layout(a)
+            segs = jpeg_segment_table(a, [seg_off[seg_base[k]:seg_base[k] + descs["nseg"][k]] for k in acc],
+                                      lib.bdbnn_jpeg_subseq_bits())
+            rgb, status, rounds, _ = jpeg_decode_batch(a, segs, stage[:int(data_off[-1])], self.device, self._stream)
+            done = torch.cuda.Event()
+            done.record(self._stream)
+            done.synchronize()
+            st = status.numpy()
+            for j, k in enumerate(acc):
+                if st[j] == 0:
+                    H, W, o = int(a["H"][j]), int(a["W"][j]), int(a["rgb_off"][j])
+                    out[k] = (rgb[o:o + H * W * 3].view(H, W, 3), True)
+            self.decode_stats["flagged"] += int((st != 0).sum())
+            self.decode_stats["device"] += int((st == 0).sum())
+            self.decode_stats["rounds"] = max(self.decode_stats["rounds"], int(rounds[0]))
+        self.decode_stats["rejected"] += B - len(acc)
+        rest = [k for k in range(B) if out[k] is None]
+        for k, (t, hwc) in zip(rest, self._pool.map(self._host_decode, [blobs[k] for k in rest])):
+            out[k] = (t.pin_memory().to(self.device, non_blocking=True), hwc)
+        return out
+
     def _prepare(self, epoch, batch_index):
         """Read and decode one batch on self._stream: (dataset indices, [(device tensor, hwc)], event)."""
         idx = self.indices(epoch, batch_index)
         blobs = list(self._pool.map(_read, [self.samples[int(k)][0] for k in idx]))
         with self._lock, torch.cuda.device(self.device), torch.cuda.stream(self._stream):
-            srcs = self._decode_cuda(blobs) if self.decode == "cuda" else self._decode_cpu(blobs)
+            srcs = {"cuda": self._decode_cuda, "cpu": self._decode_cpu, "kernel": self._decode_kernel}[self.decode](
+                blobs)
             ev = torch.cuda.Event()
             ev.record(self._stream)
         return idx, srcs, ev

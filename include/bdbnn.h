@@ -660,6 +660,93 @@ BDBNN_API int bdbnn_imagenet_batch(const bdbnn_imagenet_desc* desc_host, bdbnn_i
                                    const float* mean_host, const float* std_host, float* out, int64_t sN,
                                    int64_t sC, int64_t sH, int64_t sW, int64_t* target, void* stream);
 
+/* ---- Baseline JPEG decode on the device (csrc/jpeg_decode.cu) -----------------------------------------------------
+ * Replaces libjpeg-turbo's decode (torchvision.io.decode_jpeg on the host, mode RGB) of the files it takes, with the
+ * same pixels: jpeg_idct_islow, fancy upsampling, ycc_rgb_convert (DESIGN.md §4m, oracle/jpeg_ref.py).  Taken:
+ * SOF0, or SOF1 with 8-bit samples; Huffman; one scan with every component in frame order; 1 component, or 3 that
+ * libjpeg treats as YCbCr (a JFIF marker, an Adobe marker with transform 1, or ids 1, 2, 3 without an Adobe marker);
+ * luma sampling 1x1, 2x1 or 2x2 with chroma 1x1; any restart interval; sides in [1, 8192].
+ *
+ * bdbnn_jpeg_parse (host only, thread-safe, allocates nothing): reads file_host's markers up to SOS, fills *desc_host
+ * and writes the entropy-coded data, with stuffed 0x00 bytes dropped and split at the RST markers, to data_host[0,
+ * desc->data_bytes); segment k starts at data_host[seg_off_host[k]], k < desc->nseg.  Returns 0, or
+ * BDBNN_ERR_UNSUPPORTED for a file it does not take (progressive, arithmetic, lossless, 12-bit, CMYK / RGB, other
+ * sampling, several scans, DNL, an RST out of sequence, any marker but RSTn / EOI inside the scan, a missing EOI, a
+ * header anomaly, or data_cap / seg_cap too small: data_cap >= file_bytes and seg_cap >= file_bytes / 3 + 2
+ * suffice), BDBNN_ERR_INVALID_ARG for NULL pointers or negative sizes.  The caller sets data_off, coef_off and
+ * rgb_off. */
+typedef struct bdbnn_jpeg_huff {
+  uint16_t lut[512];    /* 9-bit lookahead: (code length << 8) | symbol, 0 for longer (or invalid) codes */
+  int32_t maxcode[18];  /* largest code of each length (index = length), -1 if none */
+  int32_t valoff[17];   /* a length-l code's symbol is vals[code + valoff[l]] */
+  uint8_t vals[256];
+} bdbnn_jpeg_huff;
+typedef struct bdbnn_jpeg_desc {
+  int32_t H, W;
+  int32_t ncomp;        /* 1 or 3 */
+  int32_t hmax, vmax;   /* luma sampling factors (1, 1 for one component) */
+  int32_t mcux, mcuy;   /* MCU grid */
+  int32_t bpm;          /* blocks per MCU */
+  int32_t restart;      /* restart interval in MCUs, 0 = none */
+  int32_t nseg;         /* entropy-coded segments */
+  int32_t data_bytes;   /* unstuffed bytes */
+  int32_t reserved;
+  int64_t data_off;     /* caller: offset of this image's data in data_dev */
+  int64_t coef_off;     /* caller: first block of this image (sum of the earlier images' mcux * mcuy * bpm) */
+  int64_t rgb_off;      /* caller: offset of this image's H x W x 3 output in rgb (3 x the earlier images' pixels) */
+  uint8_t blk_comp[8];  /* component of each block of the MCU */
+  uint8_t comp_dc[4], comp_ac[4];       /* Huffman table of each component: dc[] / ac[] index */
+  uint16_t qt[3][64];   /* quantisation table of each component, natural order */
+  bdbnn_jpeg_huff dc[2], ac[2];
+} bdbnn_jpeg_desc;
+BDBNN_API int bdbnn_jpeg_parse(const uint8_t* file_host, int64_t file_bytes, bdbnn_jpeg_desc* desc_host,
+                               uint8_t* data_host, int64_t data_cap, uint32_t* seg_off_host, int32_t seg_cap);
+
+/* One entropy-coded segment of a batch: bytes [off, off + nbytes) of data_dev, MCUs [mcu0, mcu0 + nmcu) of image img,
+ * cut into nsub = max(1, ceil(8 nbytes / S)) subsequences of S = bdbnn_jpeg_subseq_bits() bits, the first being
+ * sub0 = the earlier segments' nsub summed.  Segments are listed image by image, in order. */
+typedef struct bdbnn_jpeg_seg {
+  int64_t off;
+  int32_t img, nbytes;
+  int32_t mcu0, nmcu;
+  int32_t sub0, nsub;
+} bdbnn_jpeg_seg;
+/* Status bits of an image (any one sends it to the host decoder) */
+#define BDBNN_JPEG_PAST_END 1     /* a needed bit past the end of a segment */
+#define BDBNN_JPEG_BAD_CODE 2     /* an invalid Huffman code */
+#define BDBNN_JPEG_K_OVERFLOW 4   /* a coefficient or zero run past index 63 */
+#define BDBNN_JPEG_DC_RANGE 8     /* a DC value outside int16 */
+#define BDBNN_JPEG_PADDING 16     /* more than 7 bits left after a segment's last MCU */
+#define BDBNN_JPEG_IDCT_RANGE 32  /* IDCT inputs or intermediates outside the range where libjpeg-turbo's SIMD and
+                                     C paths agree (dequantised or pass-1 values outside int16, pass-2 outside
+                                     [-512, 511]) */
+/* Subsequence length S in bits (1024, or the bdbnn_debug_jpeg_subseq_bits override). */
+BDBNN_API int bdbnn_jpeg_subseq_bits(void);
+/* Tests only: sets S to bits in [8, 2^20], 0 restores the default.  Process-wide. */
+BDBNN_API int bdbnn_debug_jpeg_subseq_bits(int32_t bits);
+/* Device workspace for a batch of n_blocks blocks (sum of mcux * mcuy * bpm) and n_sub subsequences.  The
+ * workspace begins with the int16 coefficients [n_blocks][64] (natural order, blocks in MCU order, DC after
+ * prediction), valid after bdbnn_jpeg_decode_batch. */
+BDBNN_API size_t bdbnn_jpeg_workspace_bytes(int64_t n_blocks, int64_t n_sub);
+/* Host only: the validation bdbnn_jpeg_decode_batch runs before it touches any device pointer, of n_img
+ * descriptors and n_seg segments (offsets, MCU coverage, subsequence counts at the current S) against data_bytes,
+ * rgb_bytes and work_bytes.  0 or BDBNN_ERR_INVALID_ARG. */
+BDBNN_API int bdbnn_jpeg_check_batch(const bdbnn_jpeg_desc* desc_host, int32_t n_img, const bdbnn_jpeg_seg* seg_host,
+                                     int32_t n_seg, int64_t data_bytes, int64_t rgb_bytes, size_t work_bytes);
+/* Decodes n_img images into rgb (uint8 HWC, image i at rgb + desc[i].rgb_off).  desc_host, seg_host and data_host
+ * (data_bytes bytes) are copied to desc_dev, seg_dev and data_dev (pass pinned host memory for asynchronous
+ * copies); every descriptor and segment is validated on the host first.  work: 256-byte aligned, work_bytes >=
+ * bdbnn_jpeg_workspace_bytes.  status_dev / status_host: n_img int32 each; status_host (pinned) receives each
+ * image's BDBNN_JPEG_* bits by a copy queued last on `stream`; rounds_host (pinned, may be NULL) likewise receives
+ * the most barrier rounds one block of the synchronisation phase took.  Everything is queued on `stream`; nothing
+ * waits on the host.  Keep the host buffers unchanged, and read rgb, status_host and rounds_host, once work queued
+ * on `stream` after this call has run. */
+BDBNN_API int bdbnn_jpeg_decode_batch(const bdbnn_jpeg_desc* desc_host, bdbnn_jpeg_desc* desc_dev, int32_t n_img,
+                                      const bdbnn_jpeg_seg* seg_host, bdbnn_jpeg_seg* seg_dev, int32_t n_seg,
+                                      const uint8_t* data_host, uint8_t* data_dev, int64_t data_bytes, void* work,
+                                      size_t work_bytes, uint8_t* rgb, int64_t rgb_bytes, int32_t* status_dev,
+                                      int32_t* status_host, int32_t* rounds_host, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,11 +1,13 @@
 """Throughput of the graphed ImageNet ResNet-18 CE step (batch 256, bench.py's workload) when it is fed real JPEG
-batches from disk, four ways:
+batches from disk, five ways:
 
     a  the reference pipeline (loader.py:52-85, train.py:488-491): torchvision ImageFolder with RandomResizedCrop(224),
        RandomHorizontalFlip, ToTensor, Normalize on PIL images in a 16-worker DataLoader with pin_memory, .cuda()
     b  ImageNetDeviceLoader(decode='cuda').fill into the step's static input buffers (nvjpeg decode)
     c  ImageNetDeviceLoader(decode='cpu', workers=16).fill (libjpeg-turbo decode in 16 host threads)
     d  one batch resident in device memory, never rewritten
+    e  ImageNetDeviceLoader(decode='kernel', workers=16).fill (header parse in 16 host threads, Huffman decode, IDCT,
+       upsampling and colour conversion on the device, csrc/jpeg_decode.cu)
 
     python tools/imagenet_input_throughput.py [--rounds 3] [--steps 70] [--warmup 20] [--images 23040]
 
@@ -13,10 +15,12 @@ The data is a synthetic ImageFolder written to a temporary directory (removed at
 textured so that a 500 x 375 file is about 100 KB) in 100 classes, sized like ImageNet's 500 x 375 / 375 x 500 /
 500 x 333 with one image in 200 of 2 000-4 000 px.  Every file is read once before timing, so the timed passes read
 from the page cache (warm files).  Every arm runs in a process of its own, started afresh every round, the arms
-alternated (a, b, c, d per round); each process captures the step, runs --warmup steps and times --steps steps with a
-host clock between two device synchronisations.  Then, once: each loader alone (img/s, no step), the batch kernel alone
-(CUDA events around 200 launches on one decoded batch of 256) and one evaluation pass (Resize(256) + CenterCrop(224)
-through ImageNetDeviceLoader (decode="cpu") into the eval-mode forward).  The card name, power limit and maximum SM
+alternated (a, b, c, d, e per round); each process captures the step, runs --warmup steps and times --steps steps with
+a host clock between two device synchronisations, and the step's own device time with CUDA events around each replay.  Then, once: each loader alone (img/s, no step; for e the share of
+files sent to the host decoder and the synchronisation launches), the batch kernel alone (CUDA events around 200
+launches on one decoded batch of 256), the device JPEG decode of one batch of 256 by kernel (torch.profiler, CUDA
+activities) and one evaluation pass (Resize(256) + CenterCrop(224) through ImageNetDeviceLoader with decode="cpu" and
+decode="kernel" into the eval-mode forward).  The card name, power limit and maximum SM
 clock are read (read-only) from nvidia-smi.  Needs a CUDA device."""
 import argparse
 import json
@@ -99,7 +103,7 @@ def _feeder(torch, args):
                     y.cuda(non_blocking=True))
         return nxt
     loader = ImageNetDeviceLoader(os.path.join(args.root, "train"), BATCH, True, seed=0, drop_last=True,
-                                  decode="cuda" if args.arm == "b" else "cpu", workers=16)
+                                  decode={"b": "cuda", "c": "cpu", "e": "kernel"}[args.arm], workers=16)
     state = {"epoch": 0, "i": 0}
 
     def nxt(gstep):
@@ -113,11 +117,22 @@ def _feeder(torch, args):
         out = loader.fill(state["epoch"], state["i"], x, y)
         state["i"] += 1
         return out
+    nxt.loader = loader
     return nxt
 
 
 def arm(torch, args):
     gstep = _step(torch)
+    events = []
+
+    def timed(x, y):
+        # the step's own device time (CUDA events on the step's stream around the graph replay), so that arm e shows
+        # the step time while the JPEG decode runs beside it on the loader's stream
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        gstep(x, y)
+        e1.record()
+        events.append((e0, e1))
     if args.arm == "d":
         g = torch.Generator().manual_seed(0)
         gstep(torch.randn(BATCH, 3, 224, 224, generator=g).cuda().contiguous(memory_format=torch.channels_last),
@@ -125,26 +140,29 @@ def arm(torch, args):
 
         def run(steps):
             for _ in range(steps):
-                gstep(gstep.static_images, gstep.static_target)
+                timed(gstep.static_images, gstep.static_target)
     else:
         nxt = _feeder(torch, args)
 
         def run(steps):
             for _ in range(steps):
-                gstep(*nxt(gstep))
+                timed(*nxt(gstep))
     run(args.warmup)
     torch.cuda.synchronize()
+    events.clear()
     t0 = time.perf_counter()
     run(args.steps)
     torch.cuda.synchronize()
     s = time.perf_counter() - t0
-    print(json.dumps({"arm": args.arm, "s": round(s, 4), "img_per_s": round(args.steps * BATCH / s, 1)}), flush=True)
+    step_ms = sum(a.elapsed_time(b) for a, b in events) / len(events)
+    print(json.dumps({"arm": args.arm, "s": round(s, 4), "img_per_s": round(args.steps * BATCH / s, 1),
+                      "step_device_ms": round(step_ms, 3)}), flush=True)
 
 
 def loaders_alone(torch, args):
     """img/s of each loader with nothing else on the device: 5 warm-up batches, then 30 timed."""
     res = {}
-    for which in "abc":
+    for which in "abce":
         args.arm = which
         nxt = _feeder(torch, args)
         for _ in range(5):
@@ -155,7 +173,63 @@ def loaders_alone(torch, args):
             nxt(None)
         torch.cuda.synchronize()
         res[which] = round(30 * BATCH / (time.perf_counter() - t0), 1)
+        if which == "e":
+            st = dict(nxt.loader.decode_stats)
+            files = st["device"] + st["rejected"] + st["flagged"]
+            st["host_share"] = round((st["rejected"] + st["flagged"]) / files, 4)
+            print(json.dumps({"kernel_decode_stats": st}), flush=True)
     print(json.dumps({"loader_alone_img_per_s": res}), flush=True)
+
+
+def decode_phases(torch, args):
+    """The device JPEG decode of one training batch of 256 (bdbnn_jpeg_decode_batch) by kernel: torch.profiler with
+    CUDA activities over 5 decodes after 2 warm-up decodes; plus the host's wall time per decode call (parse excluded)
+    and the whole _decode_kernel (parse, decode, wait) per batch."""
+    import numpy as np
+    from torch.profiler import ProfilerActivity, profile
+    from bdbnn_b200 import _lib
+    from bdbnn_b200 import data as D
+    loader = D.ImageNetDeviceLoader(os.path.join(args.root, "train"), BATCH, True, seed=0, drop_last=True,
+                                    decode="kernel", workers=16)
+    idx = loader.indices(0, 0)
+    blobs = [D._read(loader.samples[int(k)][0]) for k in idx]
+    parsed = [D.jpeg_parse(b) for b in blobs]
+    acc = [p for p in parsed if p is not None]
+    descs = np.concatenate([p[0][None] for p in acc])
+    descs["data_off"] = np.concatenate([[0], np.cumsum([len(p[1]) for p in acc])[:-1]])
+    staging = torch.from_numpy(np.frombuffer(b"".join(p[1] for p in acc), np.uint8).copy()).pin_memory()
+    D.jpeg_batch_layout(descs)
+    segs = D.jpeg_segment_table(descs, [np.array(p[2]) for p in acc], _lib.lib().bdbnn_jpeg_subseq_bits())
+    dev, st = torch.device("cuda", torch.cuda.current_device()), torch.cuda.current_stream()
+    for _ in range(2):
+        D.jpeg_decode_batch(descs, segs, staging, dev, st)
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    for _ in range(5):
+        _, status, rounds, _ = D.jpeg_decode_batch(descs, segs, staging, dev, st)
+        torch.cuda.synchronize()
+        rounds = int(rounds[0])
+    call_ms = (time.perf_counter() - t0) * 1e3 / 5
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(5):
+            D.jpeg_decode_batch(descs, segs, staging, dev, st)
+        torch.cuda.synchronize()
+    us = {}
+    for e in prof.key_averages():
+        name = e.key.split("(")[0].split("<")[0].replace("bdbnn::", "").replace("void ", "")
+        if name.startswith("jpeg_") or "Memcpy" in name or "Memset" in name:
+            us[name] = round(getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0)) / 5, 1)
+    t0 = time.perf_counter()
+    for _ in range(5):
+        with torch.cuda.stream(loader._stream):
+            loader._decode_kernel(blobs)
+    whole_ms = (time.perf_counter() - t0) * 1e3 / 5
+    print(json.dumps({"kernel_decode_batch": {
+        "files_on_device": len(acc), "entropy_MB": round(staging.numel() / 1e6, 2),
+        "subsequences": int(segs["nsub"].sum()), "max_block_rounds": rounds, "flagged": int((status.numpy() != 0).sum()),
+        "us_per_batch_by_kernel": us, "decode_call_ms": round(call_ms, 2),
+        "parse_decode_wait_ms": round(whole_ms, 2)}}), flush=True)
+    loader.close()
 
 
 def kernel_time(torch, args):
@@ -186,14 +260,14 @@ def kernel_time(torch, args):
     loader.close()
 
 
-def eval_pass(torch, args):
-    """One pass of Resize(256) + CenterCrop(224) batches (decode="cpu") through the eval-mode forward, against the
-    same number of forwards on a resident batch."""
+def eval_pass(torch, args, decode):
+    """One pass of Resize(256) + CenterCrop(224) batches through the eval-mode forward, against the same number of
+    forwards on a resident batch."""
     from bdbnn_b200.data import ImageNetDeviceLoader
     from bdbnn_b200.resnet import resnet18
     torch.manual_seed(0)
     model = resnet18().cuda().eval()
-    loader = ImageNetDeviceLoader(os.path.join(args.root, "train"), BATCH, False, drop_last=True)
+    loader = ImageNetDeviceLoader(os.path.join(args.root, "train"), BATCH, False, drop_last=True, decode=decode)
     n = min(len(loader), 40)
     x = torch.empty(BATCH, 3, 224, 224, device="cuda").contiguous(memory_format=torch.channels_last)
     y = torch.empty(BATCH, dtype=torch.int64, device="cuda")
@@ -211,7 +285,7 @@ def eval_pass(torch, args):
             model(x)
         torch.cuda.synchronize()
         resident = n * BATCH / (time.perf_counter() - t0)
-    print(json.dumps({"eval_img_per_s": {"loader_cpu": round(fed, 1), "resident": round(resident, 1),
+    print(json.dumps({"eval_img_per_s": {f"loader_{decode}": round(fed, 1), "resident": round(resident, 1),
                                          "batches": n}}), flush=True)
     loader.close()
 
@@ -227,11 +301,11 @@ def _run(args, which):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--rounds", type=int, default=3, help="0 runs only the once-only measurements")
     ap.add_argument("--steps", type=int, default=70)
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--images", type=int, default=90 * BATCH)
-    ap.add_argument("--arm", choices=("a", "b", "c", "d", "extras"), help=argparse.SUPPRESS)
+    ap.add_argument("--arm", choices=("a", "b", "c", "d", "e", "extras"), help=argparse.SUPPRESS)
     ap.add_argument("--root", help=argparse.SUPPRESS)
     args = ap.parse_args()
     import torch
@@ -240,12 +314,14 @@ def main():
     if args.arm == "extras":
         loaders_alone(torch, args)
         kernel_time(torch, args)
-        eval_pass(torch, args)
+        decode_phases(torch, args)
+        eval_pass(torch, args, "cpu")
+        eval_pass(torch, args, "kernel")
         return
     if args.arm:
         arm(torch, args)
         return
-    if (args.warmup + args.steps) * BATCH > args.images:
+    if args.rounds and (args.warmup + args.steps) * BATCH > args.images:
         raise SystemExit("imagenet_input_throughput: --images must cover --warmup + --steps batches (one epoch)")
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                        capture_output=True, text=True)
@@ -259,20 +335,23 @@ def main():
                           "images": args.images, "mean_file_KB": round(mean_bytes / 1e3, 1), "steps": args.steps,
                           "warmup": args.warmup, "rounds": args.rounds, "host_cpus": os.cpu_count(),
                           "write_s": round(time.perf_counter() - t0, 1), "page_cache": "warm"}), flush=True)
-        res = {a: [] for a in "abcd"}
+        res = {a: [] for a in "abcde"}
         for _ in range(args.rounds):
-            for a in "abcd":
+            for a in "abcde":
                 r = _run(args, a)
                 print(json.dumps(r), flush=True)
                 res[a].append(r["img_per_s"])
-        med = {a: sorted(v)[len(v) // 2] for a, v in res.items()}
-        print(json.dumps({"img_per_s": res, "b_over_d_median": round(med["b"] / med["d"], 4),
-                          "c_over_d_median": round(med["c"] / med["d"], 4),
-                          "b_over_a_median": round(med["b"] / med["a"], 3),
-                          "c_over_a_median": round(med["c"] / med["a"], 3)}), flush=True)
+        med = {a: sorted(v)[len(v) // 2] for a, v in res.items() if v}
+        if len(med) == 5:
+            print(json.dumps({"img_per_s": res, "b_over_d_median": round(med["b"] / med["d"], 4),
+                              "c_over_d_median": round(med["c"] / med["d"], 4),
+                              "b_over_a_median": round(med["b"] / med["a"], 3),
+                              "c_over_a_median": round(med["c"] / med["a"], 3),
+                              "e_over_d_median": round(med["e"] / med["d"], 4),
+                              "e_over_c_median": round(med["e"] / med["c"], 3)}), flush=True)
         cmd = [sys.executable, os.path.abspath(__file__), "--arm", "extras", "--root", tmp]
-        r = subprocess.run(cmd, capture_output=True, text=True)
-        print(r.stdout.strip() if r.returncode == 0 else f"extras failed:\n{r.stderr[-3000:]}", flush=True)
+        if subprocess.run(cmd).returncode != 0:                 # its results stream to stdout as they come
+            print("extras failed", flush=True)
     finally:
         shutil.rmtree(tmp, ignore_errors=True)
 
