@@ -82,6 +82,7 @@ SIGNATURES = {
     "bdbnn_stem_conv_fwd_eval_relu": (c_int, [_P] * 6 + [c_int] * 3 + [_P]),
     "bdbnn_real_act_pack": (c_int, [_P, c_int64, c_int, _P, c_int, _P, _P]),
     "bdbnn_real_weight_pack_multi": (c_int, [c_int] + [_P] * 8 + [_P]),
+    "bdbnn_real_weight_pack_multi_grad": (c_int, [c_int] + [_P] * 11 + [_P]),
     "bdbnn_real_conv_fwd_eval": (c_int, [_P] * 6 + [c_int, _P, _P, _SH, _P]),
     "bdbnn_bn_fwd_pad_shortcut": (c_int, [_P, _P] + [c_int] * 5 + [_P, _P, c_int, ctypes.c_float, ctypes.c_float] +
                                   [_P] * 12 + [c_int, c_int, _P]),

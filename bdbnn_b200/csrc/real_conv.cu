@@ -148,6 +148,54 @@ real_wpack_multi_kernel(const __grid_constant__ RealWPackTable tab, const uint32
   }
 }
 
+// The dgrad operands of the same convs (the W32/A1 convs of DESIGN.md §4p): wt[c][k*k-1-t][o] = wf[o][t][c] and, per
+// output channel, gscale = 2^-ew, inv_gscale = 2^ew.  A third launch rather than a store in real_wpack_multi_kernel:
+// wt runs along o, wf along c, so one of the two would be written in scattered 2-byte stores; here each block moves a
+// 32 x 32 (o, c) tile of one tap through shared memory, reading wf and writing wt in whole rows.  Copying wf's fp16
+// bits (not rounding W again) makes wt exactly wf transposed and flipped.  grid = sum of the tensors' tiles,
+// block = (32, 8).
+struct RealWtTable {
+  const uint16_t* wf[kRealPackMax];
+  uint16_t* wt[kRealPackMax];
+  float* gscale[kRealPackMax];
+  float* inv_gscale[kRealPackMax];
+  int32_t Cout[kRealPackMax], Cin[kRealPackMax], T[kRealPackMax];
+  int32_t tile0[kRealPackMax + 1];        // first tile of tensor l (prefix sums of T * ceil(Cout/32) * ceil(Cin/32))
+  int32_t n;
+};
+
+__global__ void __launch_bounds__(256)
+real_wt_multi_kernel(const __grid_constant__ RealWtTable tab, const uint32_t* __restrict__ amax) {
+  __shared__ uint16_t tile[32][33];
+  const int b = int(blockIdx.x);
+  int l = 0;
+  while (l + 1 < tab.n && b >= tab.tile0[l + 1]) ++l;
+  const int Cout = tab.Cout[l], Cin = tab.Cin[l], T = tab.T[l];
+  const int tc = (Cin + 31) / 32, to = (Cout + 31) / 32;
+  const int q = b - tab.tile0[l];
+  const int t = q / (to * tc), r = q - t * (to * tc);
+  const int o0 = (r / tc) * 32, c0 = (r % tc) * 32;
+  const uint16_t* wf = tab.wf[l];
+  for (int i = threadIdx.y; i < 32; i += 8) {
+    const int o = o0 + i, c = c0 + threadIdx.x;
+    if (o < Cout && c < Cin) tile[i][threadIdx.x] = wf[(int64_t(o) * T + t) * Cin + c];
+  }
+  __syncthreads();
+  uint16_t* wt = tab.wt[l];
+  for (int i = threadIdx.y; i < 32; i += 8) {
+    const int c = c0 + i, o = o0 + threadIdx.x;
+    if (c < Cin && o < Cout) wt[(int64_t(c) * T + (T - 1 - t)) * Cout + o] = tile[threadIdx.x][i];
+  }
+  if (q == 0) {
+    const uint32_t a = __ldg(amax + l);
+    const float sw = amax_pow2_scale(a, false), isw = amax_pow2_scale(a, true);
+    for (int o = threadIdx.y * 32 + threadIdx.x; o < Cout; o += 256) {
+      tab.gscale[l][o] = isw;
+      tab.inv_gscale[l][o] = sw;
+    }
+  }
+}
+
 }  // namespace bdbnn
 
 using namespace bdbnn;
@@ -175,57 +223,105 @@ extern "C" int bdbnn_real_act_pack(const float* x, int64_t n_pix, int32_t C, uin
   return check_launch("real_pack_x_kernel");
 }
 
-extern "C" int bdbnn_real_weight_pack_multi(int32_t count, const float* const* W_host, const int32_t* Cout_host,
-                                            const int32_t* Cin_host, const int32_t* kw_host,
-                                            const int64_t* strides_host, uint32_t* amax_bits,
-                                            uint16_t* const* wf_host, float* const* alpha_host, void* stream) {
+// One host body for both entry points: the gradient outputs (wt, gscale, inv_gscale) come as a group, all NULL or
+// all given.  NULL: the two launches and their results are those of the forward-only pack.
+static int real_weight_pack_multi(int32_t count, const float* const* W_host, const int32_t* Cout_host,
+                                  const int32_t* Cin_host, const int32_t* kw_host, const int64_t* strides_host,
+                                  uint32_t* amax_bits, uint16_t* const* wf_host, float* const* alpha_host,
+                                  uint16_t* const* wt_host, float* const* gscale_host, float* const* inv_gscale_host,
+                                  void* stream) {
   BDBNN_REQUIRE(count >= 0, "real_weight_pack_multi: bad count");
   BDBNN_REQUIRE(count == 0 || (W_host && Cout_host && Cin_host && kw_host && strides_host && amax_bits && wf_host &&
                                alpha_host),
                 "real_weight_pack_multi: NULL table");
+  const bool grad = wt_host != nullptr;
+  BDBNN_REQUIRE((gscale_host != nullptr) == grad && (inv_gscale_host != nullptr) == grad,
+                "real_weight_pack_multi: wt, gscale and inv_gscale are given together or not at all");
+  // every tensor is checked before the first launch
+  for (int l = 0; l < count; ++l) {
+    const int k = kw_host[l];
+    const int64_t n = int64_t(Cout_host[l]) * Cin_host[l] * k * k;
+    const int64_t* st4 = strides_host + 4 * int64_t(l);
+    BDBNN_REQUIRE(W_host[l] && wf_host[l] && alpha_host[l], "real_weight_pack_multi: NULL pointer in tensor %d", l);
+    BDBNN_REQUIRE(!grad || (wt_host[l] && gscale_host[l] && inv_gscale_host[l]),
+                  "real_weight_pack_multi: NULL gradient output in tensor %d", l);
+    BDBNN_REQUIRE(Cout_host[l] > 0 && Cin_host[l] > 0 && k > 0 && n < (int64_t(1) << 30),
+                  "real_weight_pack_multi: bad dims in tensor %d", l);
+    // dense: the strides are a permutation of the contiguous strides of some dimension order
+    int64_t dims[4] = {Cout_host[l], Cin_host[l], k, k}, span = 1;
+    bool dense = true;
+    for (int d = 0; d < 4; ++d) {
+      BDBNN_REQUIRE(st4[d] >= 0 && st4[d] < (int64_t(1) << 30), "real_weight_pack_multi: bad strides in tensor %d", l);
+      span += (dims[d] - 1) * st4[d];
+    }
+    for (int d = 0; d < 4 && dense; ++d)
+      for (int e = d + 1; e < 4; ++e)
+        if (dims[d] > 1 && dims[e] > 1 && st4[d] == st4[e]) dense = false;
+    BDBNN_REQUIRE(dense && span == n, "real_weight_pack_multi: tensor %d is not dense", l);
+  }
   cudaStream_t st = cudaStream_t(stream);
   if (count > 0) BDBNN_CUDA(cudaMemsetAsync(amax_bits, 0, size_t(count) * sizeof(uint32_t), st));
   for (int off = 0; off < count; off += kRealPackMax) {
     const int cnt = count - off < kRealPackMax ? count - off : kRealPackMax;
     RealWPackTable tab;
     memset(&tab, 0, sizeof(tab));
+    RealWtTable gtab;
+    memset(&gtab, 0, sizeof(gtab));
     tab.n = cnt;
-    int64_t blocks = 0;
+    gtab.n = cnt;
+    int64_t blocks = 0, tiles = 0;
     for (int i = 0; i < cnt; ++i) {
       const int l = off + i;
       const int k = kw_host[l];
       const int64_t n = int64_t(Cout_host[l]) * Cin_host[l] * k * k;
       const int64_t* st4 = strides_host + 4 * int64_t(l);
-      BDBNN_REQUIRE(W_host[l] && wf_host[l] && alpha_host[l], "real_weight_pack_multi: NULL pointer in tensor %d", l);
-      BDBNN_REQUIRE(Cout_host[l] > 0 && Cin_host[l] > 0 && k > 0 && n < (int64_t(1) << 30),
-                    "real_weight_pack_multi: bad dims in tensor %d", l);
-      // dense: the strides are a permutation of the contiguous strides of some dimension order
-      int64_t dims[4] = {Cout_host[l], Cin_host[l], k, k}, span = 1;
-      bool dense = true;
-      for (int d = 0; d < 4; ++d) {
-        BDBNN_REQUIRE(st4[d] >= 0 && st4[d] < (int64_t(1) << 30), "real_weight_pack_multi: bad strides in tensor %d", l);
-        span += (dims[d] - 1) * st4[d];
-      }
-      for (int d = 0; d < 4 && dense; ++d)
-        for (int e = d + 1; e < 4; ++e)
-          if (dims[d] > 1 && dims[e] > 1 && st4[d] == st4[e]) dense = false;
-      BDBNN_REQUIRE(dense && span == n, "real_weight_pack_multi: tensor %d is not dense", l);
       tab.W[i] = W_host[l]; tab.wf[i] = wf_host[l]; tab.alpha[i] = alpha_host[l];
       tab.Cout[i] = Cout_host[l]; tab.Cin[i] = Cin_host[l]; tab.T[i] = k * k; tab.KW[i] = k;
       tab.sO[i] = int32_t(st4[0]); tab.sC[i] = int32_t(st4[1]); tab.sR[i] = int32_t(st4[2]); tab.sS[i] = int32_t(st4[3]);
       tab.blk0[i] = int32_t(blocks);
       blocks += (n + kRealPackPerBlock - 1) / kRealPackPerBlock;
+      if (grad) {
+        gtab.wf[i] = wf_host[l]; gtab.wt[i] = wt_host[l];
+        gtab.gscale[i] = gscale_host[l]; gtab.inv_gscale[i] = inv_gscale_host[l];
+        gtab.Cout[i] = Cout_host[l]; gtab.Cin[i] = Cin_host[l]; gtab.T[i] = k * k;
+        gtab.tile0[i] = int32_t(tiles);
+        tiles += int64_t(k) * k * ((Cout_host[l] + 31) / 32) * ((Cin_host[l] + 31) / 32);
+      }
     }
     BDBNN_REQUIRE(blocks < (int64_t(1) << 31), "real_weight_pack_multi: too many weights");
     tab.blk0[cnt] = int32_t(blocks);
+    gtab.tile0[cnt] = int32_t(tiles);
     real_wamax_multi_kernel<<<unsigned(blocks), 256, 0, st>>>(tab, amax_bits + off);
     int rc = check_launch("real_wamax_multi_kernel");
     if (rc) return rc;
     real_wpack_multi_kernel<<<unsigned(blocks), 256, 0, st>>>(tab, amax_bits + off);
     rc = check_launch("real_wpack_multi_kernel");
     if (rc) return rc;
+    if (grad) {
+      real_wt_multi_kernel<<<unsigned(tiles), dim3(32, 8), 0, st>>>(gtab, amax_bits + off);
+      rc = check_launch("real_wt_multi_kernel");
+      if (rc) return rc;
+    }
   }
   return BDBNN_OK;
+}
+
+extern "C" int bdbnn_real_weight_pack_multi(int32_t count, const float* const* W_host, const int32_t* Cout_host,
+                                            const int32_t* Cin_host, const int32_t* kw_host,
+                                            const int64_t* strides_host, uint32_t* amax_bits,
+                                            uint16_t* const* wf_host, float* const* alpha_host, void* stream) {
+  return real_weight_pack_multi(count, W_host, Cout_host, Cin_host, kw_host, strides_host, amax_bits, wf_host,
+                                alpha_host, nullptr, nullptr, nullptr, stream);
+}
+
+extern "C" int bdbnn_real_weight_pack_multi_grad(int32_t count, const float* const* W_host, const int32_t* Cout_host,
+                                                 const int32_t* Cin_host, const int32_t* kw_host,
+                                                 const int64_t* strides_host, uint32_t* amax_bits,
+                                                 uint16_t* const* wf_host, float* const* alpha_host,
+                                                 uint16_t* const* wt_host, float* const* gscale_host,
+                                                 float* const* inv_gscale_host, void* stream) {
+  return real_weight_pack_multi(count, W_host, Cout_host, Cin_host, kw_host, strides_host, amax_bits, wf_host,
+                                alpha_host, wt_host, gscale_host, inv_gscale_host, stream);
 }
 
 extern "C" int bdbnn_real_conv_pack(const float* x, int32_t N, int32_t H, int32_t W, int32_t Cin, int32_t stride,

@@ -473,6 +473,64 @@ def binconv2d(x, weight, stride=1, padding=1, impl=None, ede=None):
     return _BinConv2d.apply(x, weight, int(stride), int(padding), impl)
 
 
+class _BinActConv2d(torch.autograd.Function):
+    """y = conv2d(sign(x), W) with a real-valued W and the hard-tanh STE on x (DESIGN.md §4p).
+
+    forward : act_pack (sign + mask bits, fp16 +-1 copy) -> real_weight_grad_pack -> binconv_fwd_tc (fp32 y)
+    backward: grad_pack(gy, gscale) -> dgrad_tc (B = wt, x's mask fused), wgrad_tc (all-ones weight mask)"""
+
+    @staticmethod
+    @_on_device
+    def forward(ctx, x, weight, stride, padding):
+        _require_cuda(x, "binact_conv2d(x)")
+        _require_cuda(weight, "binact_conv2d(weight)")
+        _same_device(x, weight)
+        _require_fp16s("binact_conv2d")
+        sh = conv_shape(x.shape, weight.shape, stride, padding)
+        if (int(_lib.lib().bdbnn_tc_supported(ctypes.byref(sh))) & 7) != 7:
+            raise RuntimeError(f"bdbnn_b200.binact_conv2d: the wgmma kernels do not support {_shape_key(sh)}")
+        ap = _act_pack(x, sh, FMT_FP16, xb=True, xb8=False)
+        wp, = real_weight_grad_pack([weight])
+        y = torch.empty((sh.N, sh.Cout, sh.Ho, sh.Wo), dtype=torch.float32, device=x.device,
+                        memory_format=torch.channels_last)
+        _fwd_tc(sh, False, ap, wp, FMT_FP16, y)
+        ctx.sh = sh
+        ctx.x_shape, ctx.w_shape = tuple(x.shape), tuple(weight.shape)
+        ctx.w_param = weight if (weight.is_leaf and weight.requires_grad) else None
+        ctx.save_for_backward(ap.mask, ap.xb, wp.wt, wp.wmask, wp.gscale, wp.inv_gscale)
+        return y
+
+    @staticmethod
+    @_on_device
+    def backward(ctx, gy):
+        sh = ctx.sh
+        dev = gy.device
+        mask, xb, wt, wmask, gscale, inv_gscale = ctx.saved_tensors
+        key = _shape_key(sh)
+        gys = torch.empty((sh.N, sh.Ho, sh.Wo, sh.Cout), dtype=torch.int16, device=dev)
+        amax = torch.empty((1,), dtype=torch.int32, device=dev)
+        with _timed("grad_pack", key, algorithmic_bytes("grad_pack_amax", sh)):
+            _lib.check(_lib.lib().bdbnn_grad_pack(_p(_nhwc(gy)), _p(gscale), sh.N * sh.Ho * sh.Wo, sh.Cout, 3, _p(amax),
+                                                  _p(gys), _stream()), "grad_pack")
+        _lib.count(2)
+        gx = gw = None
+        if ctx.needs_input_grad[0]:
+            gx = torch.empty(ctx.x_shape, dtype=torch.float32, device=dev, memory_format=torch.channels_last)
+            _dgrad_tc(sh, gys, 3, amax, wt, mask, None, gx, "binact_dgrad_tc", algorithmic_bytes("dgrad_tc", sh))
+        if ctx.needs_input_grad[1]:
+            gw = _wgrad_tc(sh, gys, 3, amax, xb, wmask, inv_gscale, ctx.w_shape, ctx.w_param, "binact_wgrad_tc", key,
+                           algorithmic_bytes("wgrad_tc", sh))
+        return gx, gw, None, None
+
+
+def binact_conv2d(x, weight, stride=1, padding=1):
+    """W32/A1 conv2d: conv2d(sign(x), W) with a real-valued fp32 weight and the hard-tanh STE on x (the first step
+    of the two-step ImageNet recipe, DESIGN.md §4p).  x [N,Cin,H,W] fp32 CUDA (NHWC is copy-free), weight
+    [Cout,Cin,kh,kw] fp32.  Returns [N,Cout,Ho,Wo] fp32 (channels_last strides).  Needs BDBNN_GRAD_MODE=fp16s and
+    a shape all three wgmma kernels take; anything else raises."""
+    return _BinActConv2d.apply(x, weight, int(stride), int(padding))
+
+
 def _ptr_array(tensors):
     return (ctypes.c_void_p * len(tensors))(*[t.data_ptr() for t in tensors])
 
@@ -800,14 +858,17 @@ def _prepacked(weight, fmt, use8):
     return _WeightPack._make(getattr(pre, f) for f in _WeightPack._fields)
 
 
-def _unit_operands(x, weight, sh, caps, train):
+def _unit_operands(x, weight, sh, caps, train, real=False):
     """(use8, activation, _WeightPack) of a fused unit's binary conv, caps = bdbnn_tc_supported(sh).
     train: the activation is x's _ActPack with the 16-bit copy (the backward reads it and the mask bits), completed
     from the packs its producer attached when they are current; the weight pack has the gradient operands.
     eval: the activation is the one operand the forward reads, x's `_bdbnn_eval_pack` when it matches.
-    The weights come from prepack_weights when it packed them for this forward."""
+    The weights come from prepack_weights (real_prepack_weights) when it packed them for this forward.
+    real: W32/A1 conv (DESIGN.md §4p): fp16 real weights from real_weight_grad_pack, never fp8."""
+    if real:
+        _require_fp16s("the W32/A1 conv unit")
     fmt = grad_mode()[3]
-    use8 = bool(caps & 8) and use_fwd8(sh.Cin, sh.Cout, eval_unit=not train)
+    use8 = not real and bool(caps & 8) and use_fwd8(sh.Cin, sh.Cout, eval_unit=not train)
     if train:
         act = _act_pack(x, sh, fmt, xb=True, xb8=use8, have=_get_act_pack(x, fmt))
     else:
@@ -816,7 +877,9 @@ def _unit_operands(x, weight, sh, caps, train):
             ap = _act_pack(x, sh, fmt, xb=not use8, xb8=use8)
             act = ap.xb8 if use8 else ap.xb
     wp = _prepacked(weight, fmt, use8)
-    if wp is None:
+    if wp is None and real:
+        wp, = real_weight_grad_pack([weight], grad=train)
+    elif wp is None:
         wp = _alloc_weight_pack(weight.shape, x.device, wf=not use8, wf8=use8, grad=train)
         _weight_pack(weight, wp, fmt)
     return use8, act, wp
@@ -960,7 +1023,7 @@ class _ConvBNAddUnit(torch.autograd.Function):
     @_on_device
     def forward(ctx, x, weight, gamma, beta, residual, running_mean, running_var, momentum, eps, stride,
                 padding, res_is_x, sc_weight=None, sc_gamma=None, sc_beta=None, sc_rm=None, sc_rv=None,
-                sc_momentum=None, sc_eps=None, sc_stride=None, sc_pad=None, hardtanh=False):
+                sc_momentum=None, sc_eps=None, sc_stride=None, sc_pad=None, hardtanh=False, real_weight=False):
         _require_cuda(x, "conv_bn_add(x)")
         ctx.hardtanh = bool(hardtanh)
         _same_device(x, weight, gamma, beta, residual, running_mean, running_var, sc_weight)
@@ -1003,13 +1066,14 @@ class _ConvBNAddUnit(torch.autograd.Function):
         key = _shape_key(sh)
         i32 = dict(dtype=torch.int32, device=dev)
         caps = int(L.bdbnn_tc_supported(ctypes.byref(sh)))
-        use8, ap, wp = _unit_operands(x, weight, sh, caps, train=True)
+        use8, ap, wp = _unit_operands(x, weight, sh, caps, train=True, real=real_weight)
         alpha = wp.alpha
         # BN batch statistics of y are accumulated by the conv kernel's epilogue (BDBNN_CONV_STATS=0: separate pass)
         sums = torch.empty((2 * cout,), dtype=torch.float64, device=dev)
         ymax = torch.empty((cout,), **i32)
         in_conv = conv_stats_enabled() and cout <= 512
-        i16 = bool(caps & 16) and in_conv and y_i16_enabled()
+        # a real weight makes y no integer multiple of alpha: fp32 y (and no int16 hand-off to the next unit)
+        i16 = bool(caps & 16) and in_conv and y_i16_enabled() and not real_weight
         if i16:     # y kept as the exact integer accumulator, int16 NHWC (y = alpha * y_int)
             y = torch.empty((n, sh.Ho, sh.Wo, cout), dtype=torch.int16, device=dev)
         else:
@@ -1029,7 +1093,8 @@ class _ConvBNAddUnit(torch.autograd.Function):
         zs = torch.empty((n, sh.Ho, sh.Wo, cout // 32), **i32) if pack else None
         zm = torch.empty((n, sh.Ho, sh.Wo, cout // 32), **i32) if pack else None
         zb = torch.empty((n, sh.Ho, sh.Wo, cout), dtype=torch.int16, device=dev) if pack else None
-        zb8 = torch.empty((n, sh.Ho, sh.Wo, cout), dtype=torch.uint8, device=dev) if (pack and fwd8_enabled()) else None
+        zb8 = (torch.empty((n, sh.Ho, sh.Wo, cout), dtype=torch.uint8, device=dev)
+               if (pack and fwd8_enabled() and not real_weight) else None)
         ybytes = 2 if i16 else 4
         if sc_join is not None:
             torch.cuda.current_stream().wait_stream(sc_join)
@@ -1084,7 +1149,7 @@ class _ConvBNAddUnit(torch.autograd.Function):
     @_on_device
     def backward(ctx, gz, _g1, _g2, _g3, _g4):
         if gz is None:
-            return (None,) * 22
+            return (None,) * 23
         L = _lib.lib()
         sh = ctx.sh
         st = _stream()
@@ -1164,7 +1229,7 @@ class _ConvBNAddUnit(torch.autograd.Function):
             sc_db = sc_db if ctx.needs_input_grad[14] else None
         return (gx, gw, dgamma if ctx.needs_input_grad[2] else None, dbeta if ctx.needs_input_grad[3] else None,
                 gres, None, None, None, None, None, None, None,
-                sc_gw, sc_dg, sc_db, None, None, None, None, None, None, None)
+                sc_gw, sc_dg, sc_db, None, None, None, None, None, None, None, None)
 
 
 PadShortcut = collections.namedtuple("PadShortcut", "pad")
@@ -1180,7 +1245,7 @@ def pad_shortcut_supported(x_shape, w_shape, stride, pad):
 
 
 def conv_bn_add(x, weight, gamma, beta, residual, running_mean, running_var, momentum, eps, stride, padding,
-                shortcut=None, hardtanh=False):
+                shortcut=None, hardtanh=False, real_weight=False):
     """z = BN_train(binconv2d(x, weight)) + residual on the fused kernels.  `shortcut` = (weight[Cout,Cin,1,1],
     gamma, beta, running_mean, running_var, momentum, eps, stride) evaluates the real-valued 1x1 conv + BN
     `downsample` branch of x inside the same node and uses it as the residual; `shortcut` = PadShortcut(pad) uses
@@ -1189,7 +1254,9 @@ def conv_bn_add(x, weight, gamma, beta, residual, running_mean, running_var, mom
     `_bdbnn_pack` = (sign bits, mask bits, +-1 copy, fmt, fp8 copy) of z so that a following conv_bn_add skips its
     own activation pack; x's own `_bdbnn_pack` (if present and of the current format) is consumed.
     `hardtanh`: z = hardtanh(BN_train(binconv2d(x, weight))) without residual (the VGG-Small units, DESIGN.md §4n);
-    the mask bits of z's pack are Hardtanh's strict -1 < u < 1 and the backward applies that mask to gz."""
+    the mask bits of z's pack are Hardtanh's strict -1 < u < 1 and the backward applies that mask to gz.
+    `real_weight`: the conv is binact_conv2d (real weight, +-1 activation, DESIGN.md §4p) instead of binconv2d; its
+    forward runs on fp16 weights with an fp32 y, and z carries no fp8 copy."""
     res_is_x = residual is x and x.shape[1] == weight.shape[0] and int(stride) == 1
     sc, sc_pad = (None,) * 8, None       # the 1x1 shortcut's arguments, the option-A shortcut's pad
     if hardtanh:
@@ -1207,7 +1274,7 @@ def conv_bn_add(x, weight, gamma, beta, residual, running_mean, running_var, mom
                                f"{tuple(x.shape)}, weight {tuple(weight.shape)}, stride {stride}")
     z, zs, zm, zb, zb8 = _ConvBNAddUnit.apply(x, weight, gamma, beta, None if res_is_x else residual, running_mean,
                                               running_var, momentum, eps, int(stride), int(padding), res_is_x, *sc,
-                                              sc_pad, bool(hardtanh))
+                                              sc_pad, bool(hardtanh), bool(real_weight))
     if zs is not None:
         _set_act_pack(z, _ActPack(zs, zm, zb, grad_mode()[3], zb8))
         z._bdbnn_bnctx = _ConvBNAddUnit._last_bnctx      # (y_int, alpha, mean, invstd) of this unit, or None
@@ -1774,7 +1841,7 @@ def eval_unit_supported(x_shape, w_shape, stride, padding):
 
 @_on_x_device
 def conv_bn_add_eval(x, weight, gamma, beta, running_mean, running_var, eps, stride, padding, residual,
-                     shortcut=None):
+                     shortcut=None, real_weight=False):
     """z = BN_eval(binconv2d(x, weight)) + residual in one kernel (bdbnn_binconv_fwd_tc_eval), under no_grad.
     `shortcut` = (weight[Cout,Cin,1,1], gamma, beta, running_mean, running_var, eps, stride) computes the residual as
     the real-valued 1x1 conv + BN_eval `downsample` branch of x; `shortcut` = PadShortcut(pad) takes the option-A
@@ -1782,7 +1849,8 @@ def conv_bn_add_eval(x, weight, gamma, beta, running_mean, running_var, eps, str
     bit-identical to passing F.pad(x[:, :, ::2, ::2], (0, 0, 0, 0, pad, pad)) as `residual`.  The returned z carries
     `_bdbnn_eval_pack` = (format, +-1 copy of z) for the next unit: fp8 bytes (format -1) when Cout % 128 == 0 and
     BDBNN_FWD8 is on, else 16-bit in the grad_mode() format.  x's own `_bdbnn_eval_pack` is used when it matches this
-    conv's operand."""
+    conv's operand.  `real_weight`: the conv is binact_conv2d (DESIGN.md §4p): fp16 weights folded with
+    alpha = 2^-ew, and z's copy is 16-bit."""
     _eval_only("conv_bn_add_eval")
     _require_cuda(x, "conv_bn_add_eval(x)")
     _require_cuda(weight, "conv_bn_add_eval(weight)")
@@ -1808,8 +1876,8 @@ def conv_bn_add_eval(x, weight, gamma, beta, running_mean, running_var, eps, str
     st = _stream()
     key = _shape_key(sh)
     pack = cout % 32 == 0
-    out8 = pack and cout % 128 == 0 and fwd8_enabled()
-    use8, xop, wp = _unit_operands(x, weight, sh, caps, train=False)
+    out8 = pack and cout % 128 == 0 and fwd8_enabled() and not real_weight
+    use8, xop, wp = _unit_operands(x, weight, sh, caps, train=False, real=real_weight)
     if pad_sc and use8:
         raise RuntimeError("bdbnn_b200.conv_bn_add_eval: the option-A shortcut needs 16-bit operands (fp8 forward "
                            f"chosen for {sh.Cin} input channels)")
@@ -1942,18 +2010,16 @@ def _dense(w):
     return w.contiguous()
 
 
-def real_weight_pack(weights):
-    """fp16 operands of real-valued k x k conv weights, all in two launches (bdbnn_real_weight_pack_multi): one
-    power-of-two scale per tensor.  Contiguous and channels_last weights are read in place, through their strides.
-    Returns [(wf [Cout][k*k][Cin] int16, alpha[Cout] = 2^-ew)] in input order, on the weights' device."""
+def _real_pack(weights, grad):
+    """bdbnn_real_weight_pack_multi (grad False) or _multi_grad (grad True) of real-valued k x k conv weights.
+    Returns the dense weights that were packed, wf, alpha and (grad) wt, gscale, inv_gscale, as lists."""
     L = _lib.lib()
-    if not weights:
-        return []
     ws = [_dense(w.detach()) for w in weights]
+    what = "real_weight_grad_pack" if grad else "real_weight_pack"
     for w in ws:
-        _require_cuda(w, "real_weight_pack")
+        _require_cuda(w, what)
         if w.dim() != 4 or w.shape[2] != w.shape[3]:
-            raise RuntimeError(f"bdbnn_b200.real_weight_pack: expected [Cout,Cin,k,k] weights, got {tuple(w.shape)}")
+            raise RuntimeError(f"bdbnn_b200.{what}: expected [Cout,Cin,k,k] weights, got {tuple(w.shape)}")
     _same_device(*ws)
     dev = ws[0].device
     with torch.cuda.device(dev):            # launch on the weights' device, whichever device is current
@@ -1965,13 +2031,70 @@ def real_weight_pack(weights):
         ints = lambda vals: (ctypes.c_int32 * n)(*vals)
         strides = (ctypes.c_int64 * (4 * n))(*[st for w in ws for st in w.stride()])
         n_w = sum(w.numel() for w in ws)
-        with _timed("real_weight_pack", f"n{n}", 4 * n_w * 2 + 2 * n_w):    # amax read, pack read, fp16 write
-            _lib.check(L.bdbnn_real_weight_pack_multi(
-                n, _ptr_array(ws), ints([w.shape[0] for w in ws]), ints([w.shape[1] for w in ws]),
-                ints([w.shape[3] for w in ws]), strides, _p(amax), _ptr_array(wf), _ptr_array(alpha), _stream()),
-                "real_weight_pack_multi")
-    _lib.count(2 * ((n + 47) // 48))
+        args = (n, _ptr_array(ws), ints([w.shape[0] for w in ws]), ints([w.shape[1] for w in ws]),
+                ints([w.shape[3] for w in ws]), strides, _p(amax), _ptr_array(wf), _ptr_array(alpha))
+        if not grad:
+            with _timed("real_weight_pack", f"n{n}", 4 * n_w * 2 + 2 * n_w):    # amax read, pack read, fp16 write
+                _lib.check(L.bdbnn_real_weight_pack_multi(*args, _stream()), "real_weight_pack_multi")
+            _lib.count(2 * ((n + 47) // 48))
+            return ws, wf, alpha
+        wt = [torch.empty((w.shape[1], w.shape[2] * w.shape[3], w.shape[0]), dtype=torch.int16, device=dev)
+              for w in ws]
+        gscale = [torch.empty((w.shape[0],), dtype=torch.float32, device=dev) for w in ws]
+        inv_gscale = [torch.empty((w.shape[0],), dtype=torch.float32, device=dev) for w in ws]
+        # + the transpose: fp16 wf read, fp16 wt write
+        with _timed("real_weight_grad_pack", f"n{n}", 4 * n_w * 2 + 2 * n_w + 4 * n_w):
+            _lib.check(L.bdbnn_real_weight_pack_multi_grad(*args, _ptr_array(wt), _ptr_array(gscale),
+                                                           _ptr_array(inv_gscale), _stream()),
+                       "real_weight_pack_multi_grad")
+        _lib.count(3 * ((n + 47) // 48))
+        return ws, wf, alpha, wt, gscale, inv_gscale
+
+
+def real_weight_pack(weights):
+    """fp16 operands of real-valued k x k conv weights, all in two launches (bdbnn_real_weight_pack_multi): one
+    power-of-two scale per tensor.  Contiguous and channels_last weights are read in place, through their strides.
+    Returns [(wf [Cout][k*k][Cin] int16, alpha[Cout] = 2^-ew)] in input order, on the weights' device."""
+    if not weights:
+        return []
+    _, wf, alpha = _real_pack(weights, grad=False)
     return list(zip(wf, alpha))
+
+
+def real_weight_grad_pack(weights, grad=True):
+    """_WeightPacks of the W32/A1 convs' real weights (DESIGN.md §4p) in one bdbnn_real_weight_pack_multi_grad call:
+    wf = fp16(W * 2^ew) [Cout][k*k][Cin] and alpha = 2^-ew for the forward; with `grad` also the dgrad operand wt
+    [Cin][k*k flipped][Cout], gscale = 2^-ew, inv_gscale = 2^ew and an all-ones weight mask (W is a real parameter:
+    its gradient is not clamped).  No sign bits and no fp8 copy: those exist for +-1 weights only."""
+    if not weights:
+        return []
+    if not grad:
+        _, wf, alpha = _real_pack(weights, grad=False)
+        return [_WeightPack(a, None, None, f, None, None, None, None) for f, a in zip(wf, alpha)]
+    ws, wf, alpha, wt, gscale, inv_gscale = _real_pack(weights, grad=True)
+    out = []
+    for w, f, a, t, g, ig in zip(ws, wf, alpha, wt, gscale, inv_gscale):
+        ones = torch.full(((w.numel() + 31) // 32,), -1, dtype=torch.int32, device=w.device)
+        out.append(_WeightPack(a, None, ones, f, None, t, g, ig))
+    return out
+
+
+def real_prepack_weights(weights, grad):
+    """{weight.data_ptr(): _Prepacked} of the W32/A1 convs of one forward pass (the shells' _prepack), found by the
+    units through _prepacked(weight, FMT_FP16, use8=False)."""
+    if not weights:
+        return {}
+    packs = real_weight_grad_pack(weights, grad)
+    return {w.data_ptr(): _Prepacked(w._version, FMT_FP16, False, w, *pk) for w, pk in zip(weights, packs)}
+
+
+def _require_fp16s(what):
+    """The W32/A1 convs meet a +-1 activation (and the 16-bit gradient) in one wgmma with an fp16 weight: both
+    operands must be fp16, which only the fp16s gradient mode gives."""
+    name = grad_mode()[0]
+    if name != "fp16s":
+        raise RuntimeError(f"bdbnn_b200: {what} needs {_GRAD_ENV}=fp16s; {_GRAD_ENV}={name} has bf16 +-1 and "
+                           "gradient operands, which cannot meet its fp16 real-valued weight in one wgmma")
 
 
 def _real_act_pack(x, x_amax, sh):

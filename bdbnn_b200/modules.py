@@ -17,7 +17,7 @@ forward(x[N,Cin,H,W]) -> [N,Cout,Ho,Wo], differentiable through torch.autograd.
 import torch
 import torch.nn as nn
 
-from .functional import binconv2d, max_pool2d_nhwc
+from .functional import binact_conv2d, binconv2d, max_pool2d_nhwc
 
 
 class BinarizeConv2d(nn.Conv2d):
@@ -104,6 +104,33 @@ class HardBinaryConv_cifar(BinarizeConv2d):
 
     def __init__(self, in_chn, out_chn, kernel_size=3, stride=1, padding=1, **kw):
         super().__init__(in_chn, out_chn, kernel_size, stride, padding, **kw)
+
+
+class BinaryActivationConv2d(nn.Conv2d):
+    """W32/A1 conv2d, step 1 of the two-step ImageNet recipe: y = conv2d(sign(x), W) with a real-valued W, no alpha,
+    no weight STE, and the hard-tanh STE on x (DESIGN.md §4p).  Runs on the wgmma kernels with fp16 weights under a
+    power-of-two scale (TF32-class), in BDBNN_GRAD_MODE=fp16s only; CUDA tensors only.
+
+    Deliberately not a BinarizeConv2d: no code path for +-1 weights (fp8 forward, int16 accumulator, weight sign
+    packs, teacher and KD pairing checks) takes it.  It is an nn.Conv2d with one `weight` and no bias, so its
+    state_dict keys are those of the binary convs (a step-1 checkpoint loads into resnet18 / resnet34 for step 2) and
+    the kurtosis hooks select it.  EDE (`--ede`, a CIFAR recipe) does not apply: assigning `.k` / `.t` just stores
+    the attributes, and the backward ignores them."""
+
+    def __init__(self, in_chn, out_chn, kernel_size=3, stride=1, padding=1, bias=False):
+        if bias:
+            raise ValueError("BinaryActivationConv2d has no bias")
+        super().__init__(in_chn, out_chn, kernel_size, stride, padding, bias=False)
+        if self.stride[0] != self.stride[1] or self.padding[0] != self.padding[1]:
+            raise ValueError("BinaryActivationConv2d needs equal stride/padding in h and w")
+        if self.dilation != (1, 1) or self.groups != 1:
+            raise ValueError("BinaryActivationConv2d supports dilation=1, groups=1 only")
+
+    def forward(self, x):
+        return binact_conv2d(x, self.weight, self.stride[0], self.padding[0])
+
+    def extra_repr(self):
+        return super().extra_repr() + ", binarized=32W/1A"
 
 
 class MaxPool2dNHWC(nn.Module):

@@ -15,22 +15,25 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import functional as F_
-from .modules import BinarizeConv2d, HardBinaryConv, HardBinaryConv_cifar, MaxPool2dNHWC
+from .modules import BinarizeConv2d, BinaryActivationConv2d, HardBinaryConv, HardBinaryConv_cifar, MaxPool2dNHWC
 
 
 def _fused_unit(x, conv, bn, residual, shortcut=None):
     """BN_train(conv(x)) + residual through the fused kernels when the pair qualifies, else None.
-    `shortcut`: argument tuple of a qualifying `downsample` branch (see _shortcut_args) evaluated in the same node."""
-    if not (x.is_cuda and bn.training and isinstance(conv, BinarizeConv2d) and isinstance(bn, nn.BatchNorm2d)):
+    `shortcut`: argument tuple of a qualifying `downsample` branch (see _shortcut_args) evaluated in the same node.
+    A BinaryActivationConv2d takes the same unit with its real-weight operands (DESIGN.md §4p)."""
+    real = isinstance(conv, BinaryActivationConv2d)
+    if not (x.is_cuda and bn.training and (real or isinstance(conv, BinarizeConv2d)) and
+            isinstance(bn, nn.BatchNorm2d)):
         return None
     if not (bn.affine and bn.track_running_stats and bn.momentum is not None and F_.fuse_enabled()):
         return None
-    if conv.impl == "xnor" or x.dtype != torch.float32 or conv.ede_active:
+    if x.dtype != torch.float32 or (not real and (conv.impl == "xnor" or conv.ede_active)):
         return None                       # EDE backward needs fp32 x: module chain
     if not F_.unit_supported(x.shape, conv.weight.shape, conv.stride[0], conv.padding[0]):
         return None
     z = F_.conv_bn_add(x, conv.weight, bn.weight, bn.bias, residual, bn.running_mean, bn.running_var, bn.momentum,
-                       bn.eps, conv.stride[0], conv.padding[0], shortcut=shortcut)
+                       bn.eps, conv.stride[0], conv.padding[0], shortcut=shortcut, real_weight=real)
     bn.num_batches_tracked.add_(1)
     return z
 
@@ -45,17 +48,21 @@ def _eval_unit(x, conv, bn, residual, shortcut=None):
     """BN_eval(conv(x)) + residual through the eval kernels when the pair qualifies, else None.  Applies under
     no_grad / inference_mode only: with grad enabled the module chain keeps its autograd graph.  EDE changes only the
     backward, so it does not exclude a unit.  `shortcut` = functional.PadShortcut: the option-A shortcut of x, read
-    in place, is the residual (the caller checked pad_shortcut_supported)."""
-    if not (_eval_mode(x, bn) and isinstance(conv, BinarizeConv2d) and isinstance(bn, nn.BatchNorm2d)):
+    in place, is the residual (the caller checked pad_shortcut_supported).  A BinaryActivationConv2d takes the eval
+    unit with its real-weight operands."""
+    real = isinstance(conv, BinaryActivationConv2d)
+    if not (_eval_mode(x, bn) and (real or isinstance(conv, BinarizeConv2d)) and isinstance(bn, nn.BatchNorm2d)):
         return None
-    if not (bn.affine and bn.running_mean is not None and bn.running_var is not None) or conv.impl == "xnor":
+    if not (bn.affine and bn.running_mean is not None and bn.running_var is not None):
+        return None
+    if not real and conv.impl == "xnor":
         return None
     if not F_.eval_unit_supported(x.shape, conv.weight.shape, conv.stride[0], conv.padding[0]):
         return None
     if shortcut is not None and F_.use_fwd8(x.shape[1], conv.weight.shape[0], eval_unit=True):
         return None                       # the in-place option-A read has 16-bit operands only
     return F_.conv_bn_add_eval(x, conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps,
-                               conv.stride[0], conv.padding[0], residual, shortcut=shortcut)
+                               conv.stride[0], conv.padding[0], residual, shortcut=shortcut, real_weight=real)
 
 
 def _unit(x, conv, bn, residual, shortcut=None):
@@ -99,22 +106,27 @@ def _prepack(model, x):
     """Pack the weights of every binary conv that will run as a fused (training) or eval unit in this forward, in
     two launches (functional.prepack_weights).  Returns True if functional._PREPACKED was filled (caller clears it).
     Packs are never kept across forwards: the fused optimizers update parameters in place without bumping
-    `_version`, so a cached pack could hold stale signs."""
+    `_version`, so a cached pack could hold stale signs (or, for the real weights of BinaryActivationConv2d, stale
+    values).  Those are packed in one more call (functional.real_prepack_weights) in the fp16s gradient mode; in the
+    others their units raise."""
     if not (x.is_cuda and F_.fuse_enabled() and F_.prepack_enabled() and x.dtype == torch.float32):
         return False
     if not model.training and torch.is_grad_enabled():
         return False
-    items = []
+    items, real = [], []
     for m in model.modules():
         if (isinstance(m, BinarizeConv2d) and m.impl != "xnor" and m.weight.is_cuda and
                 not (model.training and m.ede_active)):
             cout, cin, kh, kw = m.weight.shape
             if (cin * kh * kw) % 32 == 0 and cin % 64 == 0 and cout % 32 == 0:
                 items.append((m.weight, F_.use_fwd8(cin, cout, eval_unit=not model.training)))
-    if not items:
+        elif isinstance(m, BinaryActivationConv2d) and m.weight.is_cuda and F_.grad_mode()[0] == "fp16s":
+            real.append(m.weight)
+    if not items and not real:
         return False
     F_._PREPACKED.clear()
     F_._PREPACKED.update(F_.prepack_weights(items))
+    F_._PREPACKED.update(F_.real_prepack_weights(real, grad=model.training))
     return True
 
 
@@ -365,6 +377,17 @@ def resnet18(pretrained=False, conv_cls=HardBinaryConv, **kw):
 
 def resnet34(pretrained=False, conv_cls=HardBinaryConv, **kw):
     return ResNetImageNet([3, 4, 6, 3], conv_cls=conv_cls, **kw)
+
+
+def resnet18_step1(pretrained=False, **kw):
+    """Step 1 of the two-step ImageNet recipe (DESIGN.md §4p): ResNet-18 with W32/A1 3x3 convs
+    (BinaryActivationConv2d); stem, shortcuts and fc as resnet18, state_dict keys identical to it."""
+    return ResNetImageNet([2, 2, 2, 2], conv_cls=BinaryActivationConv2d, **kw)
+
+
+def resnet34_step1(pretrained=False, **kw):
+    """resnet34's topology with W32/A1 3x3 convs, as resnet18_step1."""
+    return ResNetImageNet([3, 4, 6, 3], conv_cls=BinaryActivationConv2d, **kw)
 
 
 def resnet20(conv_cls=HardBinaryConv_cifar, **kw):

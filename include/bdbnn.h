@@ -588,6 +588,23 @@ BDBNN_API int bdbnn_real_weight_pack_multi(int32_t count, const float* const* W_
                                  const int32_t* Cin_host, const int32_t* kw_host, const int64_t* strides_host,
                                  uint32_t* amax_bits,
                                  uint16_t* const* wf_host, float* const* alpha_host, void* stream);
+/*   real_weight_pack_multi_grad : the same pack (same arguments, same launches, same wf / alpha bits) plus the
+ *                            operands of the data and weight gradients of a conv with real weights and +-1
+ *                            activations (the W32/A1 convs, DESIGN.md §4p), through the existing
+ *                            bdbnn_binconv_dgrad_tc / _wgrad_tc epilogues:
+ *                              wt_l[c][k*k-1-t][o] = wf_l[o][t][c]   (the dgrad operand [Cin][k*k flipped][Cout],
+ *                                                                     wf's fp16 bits, same scale)
+ *                              gscale_l[o] = 2^-ew_l,  inv_gscale_l[o] = 2^ew_l
+ *                            so that grad_pack(gy, gscale) with B = wt gives conv_transpose(gy, W) and the wgrad
+ *                            epilogue's * inv_gscale gives sum(xb * gy).  wt_host, gscale_host and inv_gscale_host
+ *                            are all NULL (then this is bdbnn_real_weight_pack_multi: two launches per 48 tensors)
+ *                            or all given with non-NULL entries (three launches per 48 tensors); anything else is
+ *                            BDBNN_ERR_INVALID_ARG before any launch. */
+BDBNN_API int bdbnn_real_weight_pack_multi_grad(int32_t count, const float* const* W_host, const int32_t* Cout_host,
+                                      const int32_t* Cin_host, const int32_t* kw_host, const int64_t* strides_host,
+                                      uint32_t* amax_bits, uint16_t* const* wf_host, float* const* alpha_host,
+                                      uint16_t* const* wt_host, float* const* gscale_host,
+                                      float* const* inv_gscale_host, void* stream);
 BDBNN_API int bdbnn_real_conv_fwd_eval(const uint16_t* xh, const uint32_t* x_amax_bits, const uint16_t* wf,
                              const float* scale, const float* shift, const float* residual, int32_t act, float* z,
                              uint32_t* z_amax_bits, const bdbnn_conv_shape* s, void* stream);
