@@ -4,9 +4,9 @@ from .modules import BinarizeConv2d, BinaryActivationConv2d, HardBinaryConv, Har
 from .losses import (KurtosisWeight, DistributionLoss, DistributionLoss_layer,
                      kurtosis_regularization, matched_weight_pairs)
 from .functional import binact_conv2d, binconv2d, kurtosis_multi, kd_logits_loss, kd_layer_loss
-from .teacher import FrozenResNetTeacher, FrozenVGGTeacher
+from .teacher import FrozenBottleneckTeacher, FrozenResNetTeacher, FrozenVGGTeacher
 
 __all__ = ["BinarizeConv2d", "BinaryActivationConv2d", "HardBinaryConv", "HardBinaryConv_react", "HardBinaryConv_cifar",
            "KurtosisWeight", "DistributionLoss", "DistributionLoss_layer", "kurtosis_regularization",
            "matched_weight_pairs", "binact_conv2d", "binconv2d", "kurtosis_multi", "kd_logits_loss", "kd_layer_loss",
-           "FrozenResNetTeacher", "FrozenVGGTeacher"]
+           "FrozenBottleneckTeacher", "FrozenResNetTeacher", "FrozenVGGTeacher"]

@@ -84,6 +84,8 @@ SIGNATURES = {
     "bdbnn_real_weight_pack_multi": (c_int, [c_int] + [_P] * 8 + [_P]),
     "bdbnn_real_weight_pack_multi_grad": (c_int, [c_int] + [_P] * 11 + [_P]),
     "bdbnn_real_conv_fwd_eval": (c_int, [_P] * 6 + [c_int, _P, _P, _SH, _P]),
+    "bdbnn_real_gemm1x1_fwd_eval": (c_int, [_P] * 6 + [c_int, _P, _P, _SH, _P]),
+    "bdbnn_real_gemm1x1_supported": (c_int, [_SH]),
     "bdbnn_bn_fwd_pad_shortcut": (c_int, [_P, _P] + [c_int] * 5 + [_P, _P, c_int, ctypes.c_float, ctypes.c_float] +
                                   [_P] * 12 + [c_int, c_int, _P]),
     "bdbnn_bn_fwd_i16_pad_shortcut": (c_int, [_P, _P, _P] + [c_int] * 5 + [_P, _P, c_int, ctypes.c_float,

@@ -1,12 +1,13 @@
 """The frozen fp32 teacher of the KD step (train.py:250-277, run at train.py:603) on this repository's kernels.
 
     teacher = FrozenResNetTeacher(torchvision.models.resnet18())      # or resnet34
+    teacher = FrozenBottleneckTeacher(torchvision.models.resnet50())  # or resnet101/152, wide_resnet50_2/101_2
     teacher = FrozenResNetTeacher(resnet.ResNetCifar(3, conv_cls=nn.Conv2d))   # the CIFAR KD step's ResNet-20
     teacher = FrozenResNetTeacher(resnet.resnet18_cifar(conv_cls=nn.Conv2d))   # ... and its ResNet-18 (the default)
     teacher = FrozenVGGTeacher(vgg.vgg_small(conv_cls=lambda i, o, k, s, p: nn.Conv2d(i, o, k, s, p, bias=False)))
 
-wraps a torchvision BasicBlock ResNet, an fp32 CIFAR ResNet of bdbnn_b200.resnet, or the fp32 VGG-Small of
-bdbnn_b200.vgg, without copying it: the wrapper's children ARE the model's children, so
+wraps a torchvision BasicBlock or Bottleneck ResNet, an fp32 CIFAR ResNet of bdbnn_b200.resnet, or the fp32
+VGG-Small of bdbnn_b200.vgg, without copying it: the wrapper's children ARE the model's children, so
 `named_modules()`, `named_parameters()` and `state_dict()` have exactly the model's names (DistributionLoss_layer pairs
 teacher and student convs by name), the parameters are the same objects, and `.cuda()`, `.to()`, `.eval()` and
 `load_state_dict` act on the model.
@@ -16,8 +17,11 @@ In eval mode on a CUDA fp32 input, with no autograd graph to record, the forward
 §4h); avgpool and fc stay in torch.  The CIFAR ResNet has no ReLU; its stem conv + BatchNorm runs as one fp32
 CUDA-core launch and its option-A shortcuts are read in place by conv1's epilogue (DESIGN.md §4j).  The CIFAR
 ResNet-18 has the same stem and no ReLU; each of its 1x1 `downsample` branches runs on the shortcut eval GEMM and is
-conv1's residual (DESIGN.md §4k).  VGG-Small's Hardtanh is in the epilogue of its stem and of its unpooled convs; its
-pooled convs write their fp32 output and one more kernel takes the 2x2 max, BatchNorm and Hardtanh (DESIGN.md §4o).
+conv1's residual (DESIGN.md §4k).  A Bottleneck ResNet's convs all run as real_conv_bn_eval; with
+BDBNN_TEACHER_F32A=1 its 1x1 convs (conv1, conv3 and the `downsample`) instead read their fp32 input in a GEMM that
+rounds it to fp16 on the way in (real_conv1x1_bn_eval, DESIGN.md §4q).  VGG-Small's Hardtanh is in the epilogue of
+its stem and of its unpooled convs; its pooled convs write their fp32 output and one more kernel takes the 2x2 max,
+BatchNorm and Hardtanh (DESIGN.md §4o).
 Anything else returns the wrapped model's own forward."""
 import ctypes
 from typing import NamedTuple
@@ -43,6 +47,7 @@ class _Family(NamedTuple):
     #                     _PadShortcut that conv1's epilogue reads in place (no launch)
     bireal: bool        # out = bn1(conv1(x)) + shortcut(x); out2 = bn2(conv2(out)) + out (Bi-Real: one shortcut per
     #                     conv); else out = bn1(conv1(x)); out2 = bn2(conv2(out)) + shortcut(x)
+    bottleneck: bool = False   # torchvision Bottleneck blocks: 1x1, 3x3 (the block's stride), 1x1 + shortcut(x)
 
 
 _LAYERS = ("layer1", "layer2", "layer3", "layer4")
@@ -59,9 +64,14 @@ def _family(model):
     from torchvision.models import resnet as tv
     if type(model) is not tv.ResNet:
         raise TypeError(f"FrozenResNetTeacher wraps a torchvision ResNet with BasicBlocks (resnet18/34) or an fp32 "
-                        f"bdbnn_b200.resnet.ResNetCifar / ResNetCifar18, got {type(model).__name__}")
-    return _Family(("conv1", "bn1", "relu", "maxpool") + _LAYERS + ("avgpool", "fc"), tv.BasicBlock, True, True,
-                   "downsample", False)
+                        f"bdbnn_b200.resnet.ResNetCifar / ResNetCifar18, FrozenBottleneckTeacher a torchvision ResNet "
+                        f"with Bottlenecks (resnet50/101/152, wide_resnet50_2/101_2), got {type(model).__name__}")
+    # the kind of layer1's first block; _blocks then asks every block to be exactly that type
+    layer1 = getattr(model, "layer1", None)
+    first = layer1[0] if type(layer1) is nn.Sequential and len(layer1) > 0 else None
+    bottleneck = type(first) is tv.Bottleneck
+    return _Family(("conv1", "bn1", "relu", "maxpool") + _LAYERS + ("avgpool", "fc"),
+                   tv.Bottleneck if bottleneck else tv.BasicBlock, True, True, "downsample", False, bottleneck)
 
 
 def _bn_args(bn):
@@ -128,10 +138,29 @@ def _check_shortcut(blk, where, fam):
         _check_bn(sc[1], where + ".downsample.1")
 
 
+def _check_bottleneck(blk, where):
+    """conv1 1x1, conv2 3x3 with the block's stride (groups 1, dilation 1: no ResNeXt, no replace_stride_with_dilation),
+    conv3 1x1, bn3 BatchNorm2d, and a downsample, if any, with the block's stride."""
+    net = "a Bottleneck ResNet"
+    for name, k in (("conv1", 1), ("conv2", 3), ("conv3", 1)):
+        _check_conv(getattr(blk, name), f"{where}.{name}", k, net=net)
+    s = blk.conv2.stride
+    if s not in ((1, 1), (2, 2)) or blk.conv2.padding != (1, 1):
+        raise TypeError(f"FrozenResNetTeacher: {where}.conv2 must be a pad-1 3x3 conv of stride 1 or 2")
+    for name in ("conv1", "conv3"):
+        c = getattr(blk, name)
+        if c.stride != (1, 1) or c.padding != (0, 0):
+            raise TypeError(f"FrozenResNetTeacher: {where}.{name} must be a stride-1 / pad-0 1x1 conv")
+    _check_bn(blk.bn3, where + ".bn3")
+    ds = blk.downsample
+    if type(ds) is nn.Sequential and len(ds) == 2 and type(ds[0]) is nn.Conv2d and ds[0].stride != s:
+        raise TypeError(f"FrozenResNetTeacher: {where}.downsample.0 must have conv2's stride {s}")
+
+
 def _blocks(model):
-    """(family, [(name, block)] of the residual blocks) after checking that `model` is a torchvision BasicBlock
-    ResNet, or a ResNetCifar or ResNetCifar18 with nn.Conv2d convs throughout: the fp32 teachers.  A CIFAR shell with
-    binary convs is a student, whose eval forward has its own units."""
+    """(family, [(name, block)] of the residual blocks) after checking that `model` is a torchvision BasicBlock or
+    Bottleneck ResNet, or a ResNetCifar or ResNetCifar18 with nn.Conv2d convs throughout: the fp32 teachers.  A CIFAR
+    shell with binary convs is a student, whose eval forward has its own units."""
     fam = _family(model)
     names = [n for n, _ in model.named_children()]
     if names != list(fam.children):
@@ -155,10 +184,13 @@ def _blocks(model):
             if fam is _CIFAR18 and [n for n, _ in blk.named_children()] != ["conv1", "bn1", "conv2", "bn2"] + (
                     ["downsample"] if blk.downsample is not None else []):
                 raise TypeError(f"FrozenResNetTeacher: {where} has unexpected children")
-            _check_conv(blk.conv1, where + ".conv1", 3)
-            _check_conv(blk.conv2, where + ".conv2", 3)
-            if blk.conv2.stride != (1, 1) or blk.conv1.padding != (1, 1) or blk.conv2.padding != (1, 1):
-                raise TypeError(f"FrozenResNetTeacher: {where} convs are not the {fam.block.__name__}'s")
+            if fam.bottleneck:
+                _check_bottleneck(blk, where)
+            else:
+                _check_conv(blk.conv1, where + ".conv1", 3)
+                _check_conv(blk.conv2, where + ".conv2", 3)
+                if blk.conv2.stride != (1, 1) or blk.conv1.padding != (1, 1) or blk.conv2.padding != (1, 1):
+                    raise TypeError(f"FrozenResNetTeacher: {where} convs are not the {fam.block.__name__}'s")
             _check_bn(blk.bn1, where + ".bn1")
             _check_bn(blk.bn2, where + ".bn2")
             if fam.relu and type(blk.relu) is not nn.ReLU:
@@ -221,10 +253,16 @@ class _FrozenTeacher(nn.Module):
 class FrozenResNetTeacher(_FrozenTeacher):
     """A torchvision resnet18 / resnet34 teacher, or an fp32 CIFAR ResNet (ResNetCifar with nn.Conv2d convs, any
     depth and class count, or ResNetCifar18 with nn.Conv2d convs, any class count), whose eval forward runs on the
-    real-valued eval kernels.  Raises TypeError for any other structure (Bottleneck, binary convs, nn.DataParallel,
-    custom blocks)."""
+    real-valued eval kernels.  Raises TypeError for any other structure (a Bottleneck ResNet, which
+    FrozenBottleneckTeacher wraps; binary convs, nn.DataParallel, custom blocks)."""
+    _BOTTLENECK = False     # the block kind this class wraps
 
     def __init__(self, model):
+        if _family(model).bottleneck != self._BOTTLENECK:
+            raise TypeError("FrozenResNetTeacher wraps BasicBlock ResNets and the CIFAR ResNets; wrap a torchvision "
+                            "Bottleneck ResNet in FrozenBottleneckTeacher" if not self._BOTTLENECK else
+                            "FrozenBottleneckTeacher wraps torchvision Bottleneck ResNets (resnet50/101/152, "
+                            "wide_resnet50_2/101_2); wrap a BasicBlock or CIFAR ResNet in FrozenResNetTeacher")
         family, blocks = _blocks(model)
         super().__init__(model)
         self.__dict__["_family"] = family
@@ -278,6 +316,23 @@ class FrozenResNetTeacher(_FrozenTeacher):
             shape = (n, c1.out_channels, h, w)
         L = _lib.lib()
         fwd_ok = lambda sh: sh.Cin % 4 == 0 and bool(int(L.bdbnn_tc_supported(ctypes.byref(sh))) & 1)
+        if fam.bottleneck:
+            # every conv on the pack + GEMM path, and every 1x1 conv on the GEMM that reads fp32 (either arm of
+            # BDBNN_TEACHER_F32A runs)
+            conv_ok = lambda sh: fwd_ok(sh) and (sh.kh != 1 or F_.real_gemm1x1_supported(sh))
+            for blk in self._blocks:
+                if not ok:
+                    break
+                x_shape = shape
+                for conv in (blk.conv1, blk.conv2, blk.conv3):
+                    sh = F_.conv_shape(shape, conv.weight.shape, conv.stride[0], conv.padding[0])
+                    ok = ok and conv_ok(sh)
+                    shape = (n, sh.Cout, sh.Ho, sh.Wo)
+                ds = blk.downsample
+                if ds is not None:
+                    sh = F_.conv_shape(x_shape, ds[0].weight.shape, ds[0].stride[0], 0)
+                    ok = ok and conv_ok(sh) and (n, sh.Cout, sh.Ho, sh.Wo) == shape
+            return ok
         for blk in self._blocks:
             if not ok:
                 break
@@ -304,6 +359,8 @@ class FrozenResNetTeacher(_FrozenTeacher):
             z, z_amax = F_.stem_conv_bn_relu_pool_eval(x, self.conv1.weight, *_bn_args(self.bn1), *self._pool_args())
         else:
             z, z_amax = F_.cifar_stem_conv_bn_eval(x, self.conv1.weight, *_bn_args(self.bn1))
+        if fam.bottleneck:
+            return self._bottleneck_forward(z, z_amax)
         # packed at every forward, never cached: a load_state_dict or an in-place update is always seen
         packs = F_.real_weight_pack([c.weight for c in self._convs])
         for i, blk in enumerate(self._blocks):
@@ -320,6 +377,41 @@ class FrozenResNetTeacher(_FrozenTeacher):
             z, z_amax = F_.real_conv_bn_eval(y, y_amax, packs[2 * i + 1], *_bn_args(blk.bn2), 1, 1, relu=fam.relu,
                                              **(dict(residual=y) if fam.bireal else res))
         return self.fc(torch.flatten(self.avgpool(z), 1))
+
+    def _bottleneck_forward(self, z, z_amax):
+        """out = relu(bn1(conv1(x))); out = relu(bn2(conv2(out))); out = relu(bn3(conv3(out)) + shortcut(x)), the
+        shortcut x or bn(downsample conv(x)).  The 1x1 convs pack their input first, or with BDBNN_TEACHER_F32A=1 read
+        it as fp32 in the GEMM (the same logits bit for bit)."""
+        if F_.teacher_f32a_enabled():
+            conv1x1 = F_.real_conv1x1_bn_eval
+        else:
+            def conv1x1(x, x_amax, pack, *bn, stride, residual=None, relu=True):
+                return F_.real_conv_bn_eval(x, x_amax, pack, *bn, stride, 0, residual=residual, relu=relu)
+        convs = []
+        for blk in self._blocks:
+            convs += [blk.conv1, blk.conv2, blk.conv3] + ([blk.downsample[0]] if blk.downsample is not None else [])
+        # 1x1 and 3x3 weights in one pack, at every forward, never cached
+        packs = iter(F_.real_weight_pack([c.weight for c in convs]))
+        for blk in self._blocks:
+            p1, p2, p3 = next(packs), next(packs), next(packs)
+            ds = blk.downsample
+            if ds is None:
+                res = z
+            else:
+                res, _ = conv1x1(z, z_amax, next(packs), *_bn_args(ds[1]), stride=ds[0].stride[0], relu=False)
+            y, y_amax = conv1x1(z, z_amax, p1, *_bn_args(blk.bn1), stride=1)
+            y, y_amax = F_.real_conv_bn_eval(y, y_amax, p2, *_bn_args(blk.bn2), blk.conv2.stride[0], 1)
+            z, z_amax = conv1x1(y, y_amax, p3, *_bn_args(blk.bn3), stride=1, residual=res)
+        return self.fc(torch.flatten(self.avgpool(z), 1))
+
+
+class FrozenBottleneckTeacher(FrozenResNetTeacher):
+    """A torchvision Bottleneck ResNet teacher (resnet50/101/152, wide_resnet50_2/101_2: every block exactly
+    torchvision's Bottleneck, groups 1, no dilation), whose eval forward runs on the real-valued eval kernels
+    (DESIGN.md §4q), with FrozenResNetTeacher's names, parameters, kernel-path conditions and fallback.  Raises
+    TypeError for any other structure (ResNeXt, dilated ResNets, mixed or subclassed blocks, BasicBlock ResNets,
+    nn.DataParallel)."""
+    _BOTTLENECK = True
 
 
 _VGG_CHILDREN = ("conv0", "bn0", "conv1", "pooling", "bn1", "conv2", "bn2", "conv3", "bn3", "conv4", "bn4", "conv5",
@@ -421,13 +513,21 @@ def launches_per_forward(model):
         `downsample` (x amax, x pack, W amax, W pack, fold, conv);
       CIFAR ResNet (DESIGN.md §4j): 2 for the stem (fold, conv); the option-A shortcuts launch nothing;
       CIFAR ResNet-18 (DESIGN.md §4k): 2 for the stem (fold, conv) and 6 per `downsample`;
-      VGG-Small (DESIGN.md §4o): 2 for the stem (fold, conv) and 1 more per pooled conv (its pool)."""
+      VGG-Small (DESIGN.md §4o): 2 for the stem (fold, conv) and 1 more per pooled conv (its pool);
+      torchvision Bottleneck ResNet (DESIGN.md §4q): 2 per 48 convs of any size (one pack), 6 for the stem, 3 per 3x3
+        conv and per 1x1 conv (conv1, conv3, downsample) 3 (activation pack, fold, conv), or 2 with
+        BDBNN_TEACHER_F32A=1 (fold, the GEMM that reads fp32)."""
     m = model.wrapped if isinstance(model, _FrozenTeacher) else model
     if type(m) is VGGSmall:
         _check_vgg(m)
         return 2 + 2 + sum(4 if pooled else 3 for pooled in _VGG_POOLED)
     fam = _family(m)
     blocks = [b for b in m.modules() if type(b) is fam.block]
+    if fam.bottleneck:
+        n_ds = sum(1 for b in blocks if b.downsample is not None)
+        n1 = 2 * len(blocks) + n_ds
+        return (2 * ((n1 + len(blocks) + 47) // 48) + 6 + 3 * len(blocks) +
+                (2 if F_.teacher_f32a_enabled() else 3) * n1)
     n3 = 2 * len(blocks)
     n_ds = sum(1 for b in blocks if b.downsample is not None) if fam.shortcut == "downsample" else 0
     return 2 * ((n3 + 47) // 48) + (6 if fam.pooled_stem else 2) + 3 * n3 + 6 * n_ds

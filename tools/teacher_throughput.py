@@ -1,31 +1,40 @@
 """Throughput of the KD step's frozen fp32 teacher (train.py:250-277, run at train.py:603): this repository's kernel
-teacher (bdbnn_b200.FrozenResNetTeacher / FrozenVGGTeacher) against the unwrapped model on cuDNN.
+teacher (bdbnn_b200.FrozenResNetTeacher / FrozenBottleneckTeacher / FrozenVGGTeacher) against the unwrapped model on
+cuDNN.
 
-    python tools/teacher_throughput.py [--models resnet18,resnet34,resnet20,resnet18_cifar,vgg_small] [--batch N]
+    python tools/teacher_throughput.py [--models resnet18,resnet34,resnet50,wide_resnet50_2,resnet20,resnet18_cifar,
+                                                 vgg_small] [--batch N]
                                        [--iters 20]
                                        [--warmup 5] [--rounds 3] [--steps 50] [--step-warmup 10] [--no-step]
 
-resnet18 / resnet34: the torchvision models on 224x224 images, batch 256 by default.  resnet20: the fp32 CIFAR
+resnet18 / resnet34 / resnet50 / wide_resnet50_2 (or another torchvision Bottleneck ResNet): the torchvision models on
+224x224 images, batch 256 by default.  resnet20: the fp32 CIFAR
 ResNet-20 (bdbnn_b200.resnet.ResNetCifar(3) with bias-free nn.Conv2d convs) on 32x32 images, batch 128 by default;
 resnet18_cifar: the fp32 CIFAR ResNet-18 (bdbnn_b200.resnet.resnet18_cifar(conv_cls=<bias-free nn.Conv2d>)), the same;
 vgg_small: the fp32 CIFAR VGG-Small (bdbnn_b200.vgg.vgg_small(conv_cls=<bias-free nn.Conv2d>)), the same.
 channels_last images, random weights and BatchNorm statistics.  Teacher forward arms, alternated round by
 round, each warmed up first, images/s from CUDA events over --iters forwards:
 
-    kernel_eager     FrozenResNetTeacher / FrozenVGGTeacher, launched eagerly
+    kernel_eager     FrozenResNetTeacher / FrozenBottleneckTeacher / FrozenVGGTeacher, launched eagerly
     kernel_graphed   the same forward captured once as a CUDA graph and replayed
     cudnn_default    the unwrapped model with TF32 allowed and cudnn.benchmark off (bench.py's timed path)
     cudnn_benchmark  the same with cudnn.benchmark = True (train.py:368)
+    kernel_eager_f32a1, kernel_graphed_f32a1   (Bottleneck teachers) the kernel arms with BDBNN_TEACHER_F32A=1: the 1x1
+                     convs read their fp32 input in the GEMM instead of packing it to fp16 first (DESIGN.md §4q)
 
 The two kernel arms run in this process.  Each cuDNN arm runs in a process of its own, started afresh every round:
 PyTorch caches the cuDNN plan of a conv shape whatever `benchmark` was when it was chosen, so in one process the arm
 that ran first would serve its plans to the other and the benchmark arm would not autotune.
 
-Then one eager kernel-teacher forward under functional.KernelTimer (per-family times), and the full KD step:
+Then one eager kernel-teacher forward under functional.KernelTimer (per-family times; for a Bottleneck teacher also
+per 1x1 shape, the fp32-reading GEMM against real_act_pack + real_conv_fwd_eval, three forwards of each), and the full
+KD step:
 GraphedTrainStep(TrainStep(student, kurtosis + KD config, teacher=...)) with the kernel teacher and with the
 unwrapped teacher (cudnn.benchmark off throughout this process; the student is the binary resnet18, or the binary
-CIFAR net of the teacher's shape for a CIFAR teacher, the binary vgg_small for vgg_small), alternated, --step-warmup steps then --steps
-timed steps per round.  The card name, power limit and maximum SM clock are read (read-only) from nvidia-smi.
+CIFAR net of the teacher's shape for a CIFAR teacher, the binary vgg_small for vgg_small; a Bottleneck teacher runs
+the logit-KD step, react=True, whose layer-wise term would need the student's conv shapes), alternated,
+--step-warmup steps then --steps timed steps per round.  The card name, power limit and maximum SM clock are read
+(read-only) from nvidia-smi.
 Needs a CUDA device."""
 import argparse
 import json
@@ -129,9 +138,41 @@ def _cudnn_round(name, mode, args):
     return json.loads(r.stdout.strip().splitlines()[-1])["img_per_s"]
 
 
+BOTTLENECK = ("resnet50", "resnet101", "resnet152", "wide_resnet50_2", "wide_resnet101_2")
+
+
+def _bottleneck(name):
+    return name in BOTTLENECK
+
+
+class _f32a:
+    """BDBNN_TEACHER_F32A set to `value` for the duration of a call (the teacher reads it at every forward)."""
+    def __init__(self, value):
+        self.value = value
+
+    def __enter__(self):
+        self.prev = os.environ.get("BDBNN_TEACHER_F32A")
+        os.environ["BDBNN_TEACHER_F32A"] = self.value
+
+    def __exit__(self, *exc):
+        if self.prev is None:
+            del os.environ["BDBNN_TEACHER_F32A"]
+        else:
+            os.environ["BDBNN_TEACHER_F32A"] = self.prev
+
+
+def _with_f32a(value, fn):
+    def run():
+        with _f32a(value):
+            return fn()
+    return run
+
+
 def _wrap(name, model):
-    from bdbnn_b200 import FrozenResNetTeacher, FrozenVGGTeacher
-    return (FrozenVGGTeacher if name == "vgg_small" else FrozenResNetTeacher)(model)
+    from bdbnn_b200 import FrozenBottleneckTeacher, FrozenResNetTeacher, FrozenVGGTeacher
+    if name == "vgg_small":
+        return FrozenVGGTeacher(model)
+    return (FrozenBottleneckTeacher if _bottleneck(name) else FrozenResNetTeacher)(model)
 
 
 def forward_arms(torch, name, args, dev):
@@ -142,6 +183,9 @@ def forward_arms(torch, name, args, dev):
     with torch.no_grad():
         assert kt.kernel_path(x)
         arms = {"kernel_eager": lambda: kt(x), "kernel_graphed": _graphed(torch, lambda: kt(x), args.warmup)}
+        if _bottleneck(name):
+            arms["kernel_eager_f32a1"] = _with_f32a("1", lambda: kt(x))
+            arms["kernel_graphed_f32a1"] = _with_f32a("1", lambda: _graphed(torch, lambda: kt(x), args.warmup))()
         for fn in arms.values():
             for _ in range(args.warmup):
                 fn()
@@ -165,6 +209,23 @@ def forward_arms(torch, name, args, dev):
     for fam, f in sorted(fams.items(), key=lambda kv: -kv[1]["ms"]):
         print(json.dumps({"teacher": name, "family": fam, "ms": round(f["ms"], 4), "launches": f["launches"]}))
     print(json.dumps({"teacher": name, "kernel_timer_total_ms": round(total, 4)}), flush=True)
+    if _bottleneck(name):
+        per_shape = {}
+        for value in ("1", "0"):
+            with torch.no_grad(), _f32a(value):
+                kt(x)
+                KernelTimer.start()
+                for _ in range(3):
+                    kt(x)
+                kern = KernelTimer.stop()
+            for (fam, key), d in kern.items():
+                if fam in ("real_gemm1x1_fwd_eval", "real_act_pack", "real_conv_fwd_eval") and "k1" in str(key):
+                    row = per_shape.setdefault(str(key), {})
+                    arm = "gemm1x1" if value == "1" else "pack_gemm"
+                    row[arm + "_ms"] = round(row.get(arm + "_ms", 0.0) + d["ms"] / 3, 4)
+                    row[arm + "_launches"] = row.get(arm + "_launches", 0) + d["launches"] // 3
+        for key, row in per_shape.items():
+            print(json.dumps({"teacher": name, "conv1x1": key, **row}), flush=True)
 
 
 def kd_step_arms(torch, name, args, dev):
@@ -174,6 +235,8 @@ def kd_step_arms(torch, name, args, dev):
     torch.backends.cudnn.benchmark = False
     tv = _teacher(torch, name, dev)
     cfg = StepConfig(w_kurtosis=True, teacher_student=True, alpha=0.9, beta=200.0, w_lambda_ce=1.0)
+    if _bottleneck(name):
+        cfg = StepConfig(teacher_student=True, react=True)
     g = torch.Generator().manual_seed(0)
     batch, hw = _batch(args, name), _hw(name)
     student, classes = {"resnet20": (resnet20, 10), "resnet18_cifar": (resnet18_cifar, 10),
@@ -193,14 +256,15 @@ def kd_step_arms(torch, name, args, dev):
     for _ in range(args.rounds):
         for arm, st in steps.items():
             rates[arm].append(round(batch * args.steps / _timed_loop(torch, lambda: st(x, y), args.steps), 1))
-    print(json.dumps({"kd_step": f"{student.__name__} student, {name} teacher", "batch": batch, "img_per_s": rates}),
+    print(json.dumps({"kd_step": f"{student.__name__} student, {name} teacher", "react": cfg.react, "batch": batch,
+                      "img_per_s": rates}),
           flush=True)
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--models", default="resnet18,resnet34")
-    ap.add_argument("--batch", type=int, default=None, help="default: 256 (resnet18/34), 128 (the CIFAR nets)")
+    ap.add_argument("--batch", type=int, default=None, help="default: 256 (the ImageNet ResNets), 128 (the CIFAR nets)")
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--rounds", type=int, default=3)
