@@ -106,6 +106,12 @@ SIGNATURES = {
     "bdbnn_bn_fwd_hardtanh": (c_int, [_P] * 4 + [c_int64, c_int, ctypes.c_float, ctypes.c_float] + [_P] * 12 +
                               [c_int, c_int, _P]),
     "bdbnn_bn_bwd_pack_hardtanh": (c_int, [_P] * 9 + [c_int64, c_int, c_int] + [_P] * 8),
+    "bdbnn_bn_fwd_relu": (c_int, [_P] * 4 + [c_int64, c_int, ctypes.c_float, ctypes.c_float] + [_P] * 10 + [c_int, _P]),
+    "bdbnn_bn_bwd_pack_relu": (c_int, [_P] * 8 + [c_int64, c_int, c_int] + [_P] * 9),
+    "bdbnn_bn_pool_fwd_relu": (c_int, [_P, _P, _P] + [c_int] * 9 + [ctypes.c_float, ctypes.c_float] + [_P] * 12 +
+                               [c_int, _P]),
+    "bdbnn_bn_pool_bwd_relu": (c_int, [_P] * 10 + [c_int] * 9 + [_P] * 9),
+    "bdbnn_real_scale_fold": (c_int, [_P, _P, _P, c_int, _P, _P, _P]),
     "bdbnn_pool2_i16": (c_int, [_P, _P] + [c_int] * 4 + [_P] * 5),
     "bdbnn_pool2_bn_bwd_pack": (c_int, [_P] * 10 + [c_int] * 5 + [_P] * 8),
     "bdbnn_pool2_bn_eval_hardtanh": (c_int, [_P] * 3 + [c_int] * 4 + [_P] * 3 + [c_int, _P]),

@@ -91,14 +91,35 @@ __device__ __forceinline__ float4 htanh_mask(float4 g, const float4 v, const flo
 // torch.nn.Hardtanh: clamp to [-1, 1], NaN stays NaN
 __device__ __forceinline__ float htanh(float u) { return u != u ? u : fminf(fmaxf(u, -1.0f), 1.0f); }
 
+// torch.relu bit for bit: 0 below 0, u itself otherwise (-0.0 and NaN stay)
+__device__ __forceinline__ float relu_f(float u) { return u < 0.0f ? 0.0f : u; }
+
+// ReLU's gradient bit as torch's threshold_backward takes it from z: 1 <=> !(z <= 0), so 1 at NaN too
+__device__ __forceinline__ uint32_t relu_bits4(const float4 o) {
+  return uint32_t(!(o.x <= 0.0f)) | (uint32_t(!(o.y <= 0.0f)) << 1) | (uint32_t(!(o.z <= 0.0f)) << 2) |
+         (uint32_t(!(o.w <= 0.0f)) << 3);
+}
+
+// ReLU's gradient mask from the bit words [pix][C/32] the forward wrote (relu_bits4), for float4 element i of an
+// NHWC tensor with C % 32 == 0: word i / 8, bits 4 * (i % 8) ..  A select, not a product, as torch's
+// threshold_backward: a NaN or inf of gz where z <= 0 gives 0.
+__device__ __forceinline__ float4 relu_mask(float4 g, const uint32_t* __restrict__ words, int64_t i) {
+  const uint32_t m = __ldg(words + (i >> 3)) >> ((i & 7) * 4);
+  g.x = (m & 1u) ? g.x : 0.0f;
+  g.y = (m & 2u) ? g.y : 0.0f;
+  g.z = (m & 4u) ? g.z : 0.0f;
+  g.w = (m & 8u) ? g.w : 0.0f;
+  return g;
+}
+
 // HT (backward only): gz is first multiplied by Hardtanh's mask on u = fmaf(y, ab[c], ab[C + c]) (ab: the forward's
-// bn_finalize output, alpha folded in for I16).
-template <bool BWD, bool I16 = false, bool HT = false>
+// bn_finalize output, alpha folded in for I16).  RM (backward only): gz is first masked by relu_mask(rmask).
+template <bool BWD, bool I16 = false, bool HT = false, bool RM = false>
 __global__ void __launch_bounds__(kBnThreads)
 bn_reduce_kernel(const float4* __restrict__ p0, const void* __restrict__ p1, const float* __restrict__ mean,
                  const float* __restrict__ invstd, int64_t n_pix, int C4, double* __restrict__ part,
                  uint32_t* __restrict__ maxbits, const float* __restrict__ alpha = nullptr,
-                 const float* __restrict__ ab = nullptr) {
+                 const float* __restrict__ ab = nullptr, const uint32_t* __restrict__ rmask = nullptr) {
   extern __shared__ float4 shs[];             // [2][blockDim] per-thread partials, then [C] max bits
   const int C = C4 * 4;
   uint32_t* shm = reinterpret_cast<uint32_t*>(shs + 2 * blockDim.x);   // non-negative floats order like uints
@@ -131,6 +152,7 @@ bn_reduce_kernel(const float4* __restrict__ p0, const void* __restrict__ p1, con
     if (BWD) {   // u = gz, v = y:  a = gz, b = gz * yhat, c = |gz|
       const float4 v = load_y4<I16>(p1, p * C4 + c4);
       if (HT) u = htanh_mask(u, v, ha, hb);
+      if (RM) u = relu_mask(u, rmask, p * C4 + c4);
       sa.x += u.x; sa.y += u.y; sa.z += u.z; sa.w += u.w;
       if (I16) {
         sb.x += u.x * fmaf(v.x, is.x, -mu.x); sb.y += u.y * fmaf(v.y, is.y, -mu.y);
@@ -212,16 +234,16 @@ int det_sums_finish(double* part, int64_t nparts, int width, double* sums, cudaS
 }
 
 // bn_reduce_kernel over `grid` blocks with its partials summed into sums[2C] (pre-zeroed or accumulated)
-template <bool BWD, bool I16 = false, bool HT = false>
+template <bool BWD, bool I16 = false, bool HT = false, bool RM = false>
 static int bn_reduce_launch(int grid, const float4* p0, const void* p1, const float* mean, const float* invstd,
                             int64_t n_pix, int C4, double* sums, uint32_t* maxbits, const float* alpha,
-                            cudaStream_t st, const float* ab = nullptr) {
+                            cudaStream_t st, const float* ab = nullptr, const uint32_t* rmask = nullptr) {
   double* part = nullptr;
   int rc = det_sums_alloc(&part, grid, 8 * C4, st);
   if (rc) return rc;
-  bn_reduce_kernel<BWD, I16, HT><<<grid, kBnThreads, 2 * kBnThreads * sizeof(float4) +
-                                   size_t(4 * C4) * sizeof(uint32_t), st>>>(p0, p1, mean, invstd, n_pix, C4, part,
-                                                                            maxbits, alpha, ab);
+  bn_reduce_kernel<BWD, I16, HT, RM><<<grid, kBnThreads, 2 * kBnThreads * sizeof(float4) +
+                                       size_t(4 * C4) * sizeof(uint32_t), st>>>(p0, p1, mean, invstd, n_pix, C4, part,
+                                                                                maxbits, alpha, ab, rmask);
   rc = check_launch(BWD ? "bn_reduce_kernel<bwd>" : "bn_reduce_kernel<fwd>");
   if (rc) { cudaFreeAsync(part, st); return rc; }
   return det_sums_finish(part, grid, 8 * C4, sums, st);
@@ -267,13 +289,17 @@ struct PadResidual {
 // pixel from 4 lanes (bits 16-31 zero, as bdbnn_act_pack writes them) instead of one per 32 channels from 8 lanes.
 // HT: z = hardtanh(u) for u = y*a + b, and the mask bits are Hardtanh's strict -1 < u < 1 (the product of its
 // gradient and the next conv's STE indicator, which is 1 on hardtanh's range except at NaN).
-template <bool PACK, bool I16 = false, int U = 4, bool SUB = false, bool P16 = false, bool HT = false>
+// RELU (PACK false, fp32 y): z = relu(y*a + b (+ residual)), mask_bits = ReLU's gradient mask (relu_bits4, one bit per
+// channel as the STE mask), and the bits of max|z| into z_amax (integer atomicMax, NaN on top: run-to-run identical),
+// the word the next real-valued conv's real_act_pack scales its fp16 operand by.
+template <bool PACK, bool I16 = false, int U = 4, bool SUB = false, bool P16 = false, bool HT = false,
+          bool RELU = false>
 __global__ void __launch_bounds__(kBnThreads)
 bn_apply_add_pack_kernel(const void* __restrict__ y, const float4* __restrict__ res,
                          const float* __restrict__ a, const float* __restrict__ b, int64_t n4, int C4,
                          float4* __restrict__ z, uint32_t* __restrict__ sign_bits,
                          uint32_t* __restrict__ mask_bits, uint2* __restrict__ xb4, uint32_t* __restrict__ xb8,
-                         uint32_t one16, const PadResidual sub = PadResidual{}) {
+                         uint32_t one16, const PadResidual sub = PadResidual{}, uint32_t* __restrict__ z_amax = nullptr) {
   constexpr int GL = P16 ? 4 : 8;                                 // lanes (float4 groups) per bit word
   const int lane = threadIdx.x & 31;
   const uint32_t group_mask = (P16 ? 0xfu : 0xffu) << (lane & (32 - GL));
@@ -285,11 +311,19 @@ bn_apply_add_pack_kernel(const void* __restrict__ y, const float4* __restrict__ 
   const float4 av = *reinterpret_cast<const float4*>(a + c4 * 4);
   const float4 bv = *reinterpret_cast<const float4*>(b + c4 * 4);
   const bool sub_on = SUB && c4 >= sub.pad4 && c4 < sub.pad4 + sub.Cin4;   // constant per thread too
+  uint32_t zmax = 0u;
   auto emit = [&](int64_t i, const float4 v, const float4 r) {
     float4 o = make_float4(fmaf(v.x, av.x, bv.x), fmaf(v.y, av.y, bv.y), fmaf(v.z, av.z, bv.z),
                            fmaf(v.w, av.w, bv.w));
     o.x += r.x; o.y += r.y; o.z += r.z; o.w += r.w;
     if (HT) { o.x = htanh(o.x); o.y = htanh(o.y); o.z = htanh(o.z); o.w = htanh(o.w); }
+    if (RELU) {
+      o.x = relu_f(o.x); o.y = relu_f(o.y); o.z = relu_f(o.z); o.w = relu_f(o.w);
+      zmax = max(zmax, max(max(__float_as_uint(fabsf(o.x)), __float_as_uint(fabsf(o.y))),
+                           max(__float_as_uint(fabsf(o.z)), __float_as_uint(fabsf(o.w)))));
+      const uint32_t mw = __reduce_or_sync(group_mask, relu_bits4(o) << sh);
+      if ((lane & (GL - 1)) == 0) mask_bits[i / GL] = mw;
+    }
     // z (4 B/element, re-read only after the next conv has run) is stored evict-first so that the next conv's
     // operands written below (xb / xb8, 1-2 B/element) have a chance to stay in the 126 MB L2
     __stcs(z + i, o);
@@ -339,6 +373,10 @@ bn_apply_add_pack_kernel(const void* __restrict__ y, const float4* __restrict__ 
     for (int u = 0; u < U; ++u) emit(i + u * nthreads, v[u], r[u]);
   }
   for (; i < n4; i += nthreads) emit(i, load_y4<I16>(y, i), load_r(i));
+  if (RELU) {
+    zmax = __reduce_max_sync(0xffffffffu, zmax);      // every lane of the (whole) warp gets here
+    if (lane == 0 && zmax != 0u) atomicMax(z_amax, zmax);
+  }
 }
 
 // [C] math of the backward.  consts[c] = {m1, m2*invstd, mean, a*gscale}; gy*gscale = (gz - m1 -
@@ -385,11 +423,14 @@ __global__ void bn_bwd_bound_kernel(const double* __restrict__ sums, const uint3
 }
 
 // gys = 16-bit operand of the conv backward, straight from gz and y.  HT: gz times Hardtanh's mask (bn_reduce_kernel).
-template <int MODE, bool I16 = false, int U = 4, bool HT = false>
+// RM: gz masked by relu_mask(rmask) first; the masked gradient is also written to g_out when that is non-NULL (the
+// gradient of a residual added before the ReLU).
+template <int MODE, bool I16 = false, int U = 4, bool HT = false, bool RM = false>
 __global__ void __launch_bounds__(kBnThreads)
 bn_bwd_pack_kernel(const float4* __restrict__ gz, const void* __restrict__ y, const float4* __restrict__ consts,
                    const uint32_t* __restrict__ amax_bits, int64_t n4, int C4, uint16_t* __restrict__ out,
-                   const float* __restrict__ ab = nullptr) {
+                   const float* __restrict__ ab = nullptr, const uint32_t* __restrict__ rmask = nullptr,
+                   float4* __restrict__ g_out = nullptr) {
   constexpr int HALVES = MODE == 2 ? 2 : 1;
   const int64_t nthreads = int64_t(gridDim.x) * blockDim.x;       // multiple of C4
   int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -404,8 +445,12 @@ bn_bwd_pack_kernel(const float4* __restrict__ gz, const void* __restrict__ y, co
   }
   int64_t pix = i / C4;
   const int64_t pix_step = nthreads / C4;
-  auto emit = [&](int64_t pix, float4 g, const float4 v) {
+  auto emit = [&](int64_t e, int64_t pix, float4 g, const float4 v) {
     if (HT) g = htanh_mask(g, v, ha, hb);
+    if (RM) {
+      g = relu_mask(g, rmask, e);
+      if (g_out != nullptr) __stcs(g_out + e, g);
+    }
     const float a0 = (g.x - k0.x - (v.x - k0.z) * k0.y) * k0.w * up;
     const float a1 = (g.y - k1.x - (v.y - k1.z) * k1.y) * k1.w * up;
     const float a2 = (g.z - k2.x - (v.z - k2.z) * k2.y) * k2.w * up;
@@ -435,9 +480,9 @@ bn_bwd_pack_kernel(const float4* __restrict__ gz, const void* __restrict__ y, co
 #pragma unroll
     for (int u = 0; u < U; ++u) v[u] = load_y4<I16>(y, i + u * nthreads);
 #pragma unroll
-    for (int u = 0; u < U; ++u) emit(pix + u * pix_step, g[u], v[u]);
+    for (int u = 0; u < U; ++u) emit(i + u * nthreads, pix + u * pix_step, g[u], v[u]);
   }
-  for (; i < n4; i += nthreads, pix += pix_step) emit(pix, __ldcs(gz + i), load_y4<I16>(y, i));
+  for (; i < n4; i += nthreads, pix += pix_step) emit(i, pix, __ldcs(gz + i), load_y4<I16>(y, i));
 }
 
 // Hardtanh units after a 2x2 / stride-2 max-pool (DESIGN.md §4n), int16 conv results y_int [N][H][W][C] (H, W even):
@@ -705,7 +750,12 @@ static int bn_fwd_impl(const void* y, const float* alpha_i16, const float* resid
                        float* running_var, double* sums_ws, uint32_t* ymax_bits, float* mean, float* invstd,
                        float* ab_ws, float* z, uint32_t* sign_bits, uint32_t* mask_bits, uint16_t* xb,
                        uint8_t* xb_fp8, int32_t fmt, int32_t stats_ready, void* stream,
-                       const PadResidual* sub = nullptr, bool ht = false) {
+                       const PadResidual* sub = nullptr, bool ht = false, uint32_t* relu_amax = nullptr) {
+  if (relu_amax != nullptr) {      // bdbnn_bn_fwd_relu: fp32 y, no +-1 packs, the ReLU mask words instead
+    BDBNN_REQUIRE(alpha_i16 == nullptr && sub == nullptr && !ht && sign_bits == nullptr && mask_bits != nullptr,
+                  "bn_fwd_relu: needs fp32 y and mask_bits");
+    BDBNN_REQUIRE((C & 31) == 0, "bn_fwd_relu: the mask words need C %% 32 == 0");
+  }
   const bool pack = sign_bits != nullptr;
   const bool i16 = alpha_i16 != nullptr;
   // 16-channel packs (one word per pixel): the CIFAR stem's BatchNorm, fp32 y only
@@ -736,7 +786,11 @@ static int bn_fwd_impl(const void* y, const float* alpha_i16, const float* resid
   const int grid = bn_grid(n4, C4);
   const float4* r4 = reinterpret_cast<const float4*>(residual);
   float4* z4 = reinterpret_cast<float4*>(z);
-  if (sub != nullptr) {
+  if (relu_amax != nullptr) {
+    BDBNN_CUDA(cudaMemsetAsync(relu_amax, 0, sizeof(uint32_t), st));
+    bn_apply_add_pack_kernel<false, false, 4, false, false, false, true><<<grid, kBnThreads, 0, st>>>(
+        y, r4, a, b, n4, C4, z4, nullptr, mask_bits, nullptr, nullptr, 0u, PadResidual{}, relu_amax);
+  } else if (sub != nullptr) {
     const uint32_t one16 = fmt == BDBNN_FMT_FP16 ? 0x3C00u : 0x3F80u;
     uint2* xb2 = reinterpret_cast<uint2*>(xb);
     uint32_t* xb8 = reinterpret_cast<uint32_t*>(xb_fp8);
@@ -800,6 +854,17 @@ extern "C" int bdbnn_bn_fwd(const float* y, const float* residual, const float* 
                             uint16_t* xb, uint8_t* xb_fp8, int32_t fmt, int32_t stats_ready, void* stream) {
   return bn_fwd_impl(y, nullptr, residual, gamma, beta, n_pix, C, eps, momentum, running_mean, running_var, sums_ws,
                      ymax_bits, mean, invstd, ab_ws, z, sign_bits, mask_bits, xb, xb_fp8, fmt, stats_ready, stream);
+}
+
+extern "C" int bdbnn_bn_fwd_relu(const float* y, const float* residual, const float* gamma, const float* beta,
+                                 int64_t n_pix, int32_t C, float eps, float momentum, float* running_mean,
+                                 float* running_var, double* sums_ws, uint32_t* ymax_bits, float* mean, float* invstd,
+                                 float* ab_ws, float* z, uint32_t* mask_bits, uint32_t* z_amax_bits,
+                                 int32_t stats_ready, void* stream) {
+  BDBNN_REQUIRE(z_amax_bits != nullptr, "bn_fwd_relu: NULL z_amax_bits");
+  return bn_fwd_impl(y, nullptr, residual, gamma, beta, n_pix, C, eps, momentum, running_mean, running_var, sums_ws,
+                     ymax_bits, mean, invstd, ab_ws, z, nullptr, mask_bits, nullptr, nullptr, BDBNN_FMT_FP16,
+                     stats_ready, stream, nullptr, false, z_amax_bits);
 }
 
 extern "C" int bdbnn_bn_fwd_hardtanh(const void* y, const float* alpha, const float* gamma, const float* beta,
@@ -871,10 +936,14 @@ static int bn_bwd_pack_impl(const float* gz, const void* y, const float* alpha_i
                             const float* invstd, const float* gamma, const float* gscale, const uint32_t* ymax_bits,
                             int64_t n_pix, int32_t C, int32_t grad_mode, double* sums_ws, uint32_t* gmax_bits,
                             float* consts_ws, float* dgamma, float* dbeta, uint32_t* amax_bits, uint16_t* gys,
-                            int stats_ready, void* stream, const float* ab_ht = nullptr) {
+                            int stats_ready, void* stream, const float* ab_ht = nullptr,
+                            const uint32_t* rmask = nullptr, float* g_out = nullptr) {
   const bool i16 = alpha_i16 != nullptr;
   const bool ht = ab_ht != nullptr;
+  const bool rm = rmask != nullptr;
   BDBNN_REQUIRE(!(ht && stats_ready), "bn_bwd_pack_hardtanh: the sums are of the masked gradient (stats_ready = 0)");
+  BDBNN_REQUIRE(!rm || (!i16 && !ht && !stats_ready && (C & 31) == 0 && grad_mode == BDBNN_GRAD_FP16S),
+                "bn_bwd_pack_relu: fp32 y, C %% 32 == 0, grad_mode FP16S, and the sums are of the masked gradient");
   int rc = bn_dims_ok(n_pix, C, false);
   if (rc) return rc;
   BDBNN_REQUIRE(gz && y && mean && invstd && gamma && gscale && ymax_bits && sums_ws && gmax_bits && consts_ws &&
@@ -888,7 +957,10 @@ static int bn_bwd_pack_impl(const float* gz, const void* y, const float* alpha_i
     BDBNN_CUDA(cudaMemsetAsync(gmax_bits, 0, size_t(C) * sizeof(uint32_t), st));
     const int rgrid = bn_grid(n_pix * C4 / 8, C4, n_pix * C4 > (int64_t(16) << 20) ? 8 : 3);
     const float4* g4 = reinterpret_cast<const float4*>(gz);
-    if (i16 && ht)
+    if (rm)
+      rc = bn_reduce_launch<true, false, false, true>(rgrid, g4, y, mean, invstd, n_pix, C4, sums_ws, gmax_bits,
+                                                      nullptr, st, nullptr, rmask);
+    else if (i16 && ht)
       rc = bn_reduce_launch<true, true, true>(rgrid, g4, y, mean, invstd, n_pix, C4, sums_ws, gmax_bits, alpha_i16, st,
                                               ab_ht);
     else if (ht)
@@ -912,7 +984,10 @@ static int bn_bwd_pack_impl(const float* gz, const void* y, const float* alpha_i
   const int grid = bn_grid(n4, C4, bwd_per_sm);
   const float4* g4 = reinterpret_cast<const float4*>(gz);
   const float4* k4 = reinterpret_cast<const float4*>(consts_ws);
-  if (ht) {
+  if (rm) {
+    bn_bwd_pack_kernel<3, false, 4, false, true><<<grid, kBnThreads, 0, st>>>(
+        g4, y, k4, amax_bits, n4, C4, gys, nullptr, rmask, reinterpret_cast<float4*>(g_out));
+  } else if (ht) {
     if (i16 && grad_mode == BDBNN_GRAD_FP16S)
       bn_bwd_pack_kernel<3, true, 4, true><<<grid, kBnThreads, 0, st>>>(g4, y, k4, amax_bits, n4, C4, gys, ab_ht);
     else if (i16 && grad_mode == BDBNN_GRAD_BF16X2)
@@ -950,6 +1025,16 @@ extern "C" int bdbnn_bn_bwd_pack(const float* gz, const float* y, const float* m
                                  uint32_t* amax_bits, uint16_t* gys, void* stream) {
   return bn_bwd_pack_impl(gz, y, nullptr, mean, invstd, gamma, gscale, ymax_bits, n_pix, C, grad_mode, sums_ws,
                           gmax_bits, consts_ws, dgamma, dbeta, amax_bits, gys, 0, stream);
+}
+
+extern "C" int bdbnn_bn_bwd_pack_relu(const float* gz, const uint32_t* mask_bits, const float* y, const float* mean,
+                                      const float* invstd, const float* gamma, const float* gscale,
+                                      const uint32_t* ymax_bits, int64_t n_pix, int32_t C, int32_t grad_mode,
+                                      double* sums_ws, uint32_t* gmax_bits, float* consts_ws, float* dgamma,
+                                      float* dbeta, uint32_t* amax_bits, uint16_t* gys, float* g_out, void* stream) {
+  BDBNN_REQUIRE(mask_bits != nullptr, "bn_bwd_pack_relu: NULL mask_bits");
+  return bn_bwd_pack_impl(gz, y, nullptr, mean, invstd, gamma, gscale, ymax_bits, n_pix, C, grad_mode, sums_ws,
+                          gmax_bits, consts_ws, dgamma, dbeta, amax_bits, gys, 0, stream, nullptr, mask_bits, g_out);
 }
 
 extern "C" int bdbnn_bn_bwd_pack_hardtanh(const float* gz, const void* y, const float* alpha, const float* ab,
@@ -1087,6 +1172,25 @@ extern "C" int bdbnn_bn_bwd_pack_i16(const float* gz, const int16_t* y_int, cons
 // ===================================================================================================
 namespace bdbnn {
 
+// RELU of bn_pool_fwd_k3s2_kernel (PACK false): z = relu(max) = max(relu(v)); mask_bits = ReLU's gradient mask
+// (relu_bits4) as bn_apply_add_pack's RELU words, the winner byte 0xff (no tap: the backward gives that window's
+// gradient to no position) where the bit is 0, and the bits of max|z| into z_amax.
+__device__ __forceinline__ void pool_relu(float4& m, uint32_t& w4, uint32_t& zmax, uint32_t* __restrict__ mask_bits,
+                                          int64_t i, uint32_t group_mask, int sh, int lane) {
+  const uint32_t m4 = relu_bits4(m);
+  m.x = relu_f(m.x); m.y = relu_f(m.y); m.z = relu_f(m.z); m.w = relu_f(m.w);
+  w4 |= (m4 & 1u ? 0u : 0xffu) | (m4 & 2u ? 0u : 0xff00u) | (m4 & 4u ? 0u : 0xff0000u) | (m4 & 8u ? 0u : 0xff000000u);
+  zmax = max(zmax, max(max(__float_as_uint(fabsf(m.x)), __float_as_uint(fabsf(m.y))),
+                       max(__float_as_uint(fabsf(m.z)), __float_as_uint(fabsf(m.w)))));
+  const uint32_t mw = __reduce_or_sync(group_mask, m4 << sh);
+  if ((lane & 7) == 0) mask_bits[i >> 3] = mw;
+}
+
+__device__ __forceinline__ void pool_relu_amax(uint32_t zmax, uint32_t* __restrict__ z_amax) {
+  zmax = __reduce_max_sync(0xffffffffu, zmax);      // every lane of the (whole) warp gets here
+  if ((threadIdx.x & 31) == 0 && zmax != 0u) atomicMax(z_amax, zmax);
+}
+
 template <bool PACK>
 __global__ void __launch_bounds__(kBnThreads)
 bn_pool_fwd_kernel(const float4* __restrict__ y, const float* __restrict__ a, const float* __restrict__ b,
@@ -1156,13 +1260,13 @@ bn_pool_fwd_kernel(const float4* __restrict__ y, const float* __restrict__ a, co
 // as four small integers instead of read-modify-write byte lanes — about half the instructions of the
 // generic kernel, which is bound by instruction issue rather than by memory.
 // Same scan order and NaN rule, so outputs are bit-identical.  blockDim.x is a multiple of C4.
-template <bool PACK>
+template <bool PACK, bool RELU = false>
 __global__ void __launch_bounds__(kBnThreads)
 bn_pool_fwd_k3s2_kernel(const float4* __restrict__ y, const float* __restrict__ a, const float* __restrict__ b,
                         int H, int W, int C4, int Ho, int Wo, float4* __restrict__ z, float4* __restrict__ ysel,
                         uint32_t* __restrict__ idx, uint32_t* __restrict__ sign_bits,
                         uint32_t* __restrict__ mask_bits, uint2* __restrict__ xb4, uint32_t* __restrict__ xb8,
-                        uint32_t one16) {
+                        uint32_t one16, uint32_t* __restrict__ z_amax = nullptr) {
   const int lane = threadIdx.x & 31;
   const uint32_t group_mask = 0xffu << (lane & 24);
   const int sh = (lane & 7) * 4;
@@ -1182,6 +1286,7 @@ bn_pool_fwd_k3s2_kernel(const float4* __restrict__ y, const float* __restrict__ 
   }
   const int per_row = Wo * C4;               // multiple of 8 when PACK (C % 32 == 0)
   const int64_t out0 = (int64_t(n) * Ho + ho) * per_row;
+  uint32_t zmax = 0u;
   for (int j = threadIdx.x; j < per_row; j += blockDim.x) {
     const int wo = j / C4;
     const int w0 = 2 * wo - 1;
@@ -1207,9 +1312,11 @@ bn_pool_fwd_k3s2_kernel(const float4* __restrict__ y, const float* __restrict__ 
       }
     }
     const int64_t i = out0 + j;
+    uint32_t w4 = tx | (ty << 8) | (tz << 16) | (tw << 24);
+    if (RELU) pool_relu(m, w4, zmax, mask_bits, i, group_mask, sh, lane);
     z[i] = m;
     ysel[i] = ys;
-    idx[i] = tx | (ty << 8) | (tz << 16) | (tw << 24);
+    idx[i] = w4;
     if (PACK) {
       const uint32_t s0 = m.x >= 0.0f, s1 = m.y >= 0.0f, s2 = m.z >= 0.0f, s3 = m.w >= 0.0f;
       const uint32_t m0 = fabsf(m.x) <= 1.0f, m1 = fabsf(m.y) <= 1.0f, m2 = fabsf(m.z) <= 1.0f,
@@ -1228,6 +1335,7 @@ bn_pool_fwd_k3s2_kernel(const float4* __restrict__ y, const float* __restrict__ 
         xb8[i] = 0x38383838u | ((s0 ? 0u : 0x80u) | (s1 ? 0u : 0x8000u) | (s2 ? 0u : 0x800000u) | (s3 ? 0u : 0x80000000u));
     }
   }
+  if (RELU) pool_relu_amax(zmax, z_amax);
 }
 
 // gy[n,h,w,c] = A*(gz - m1 - (y-mean)*m2'),  gz = sum of g_pool over the windows won by (h,w);
@@ -1367,18 +1475,24 @@ static int pool_geom_ok(int N, int H, int W, int C, int k, int s, int p, int Ho,
   return BDBNN_OK;
 }
 
-extern "C" int bdbnn_bn_pool_fwd(const float* y, const float* gamma, const float* beta, int32_t N, int32_t H,
-                                 int32_t W, int32_t C, int32_t k, int32_t stride, int32_t pad, int32_t Ho,
-                                 int32_t Wo, float eps, float momentum, float* running_mean, float* running_var,
-                                 double* sums_ws, uint32_t* ymax_bits, float* mean, float* invstd, float* ab_ws,
-                                 float* z, float* y_sel, uint8_t* idx, uint32_t* sign_bits, uint32_t* mask_bits,
-                                 uint16_t* xb, uint8_t* xb_fp8, int32_t fmt, int32_t stats_ready, void* stream) {
+// relu_amax != NULL: bdbnn_bn_pool_fwd_relu (mask_bits are ReLU's, no +-1 packs)
+static int bn_pool_fwd_impl(const float* y, const float* gamma, const float* beta, int32_t N, int32_t H, int32_t W,
+                            int32_t C, int32_t k, int32_t stride, int32_t pad, int32_t Ho, int32_t Wo, float eps,
+                            float momentum, float* running_mean, float* running_var, double* sums_ws,
+                            uint32_t* ymax_bits, float* mean, float* invstd, float* ab_ws, float* z, float* y_sel,
+                            uint8_t* idx, uint32_t* sign_bits, uint32_t* mask_bits, uint16_t* xb, uint8_t* xb_fp8,
+                            int32_t fmt, int32_t stats_ready, void* stream, uint32_t* relu_amax = nullptr) {
   int rc = pool_geom_ok(N, H, W, C, k, stride, pad, Ho, Wo);
   if (rc) return rc;
   const bool pack = sign_bits != nullptr;
+  const bool relu = relu_amax != nullptr;
   BDBNN_REQUIRE(y && gamma && beta && sums_ws && ymax_bits && mean && invstd && ab_ws && z && y_sel && idx,
                 "bn_pool_fwd: NULL pointer");
   BDBNN_REQUIRE(!pack || ((C & 31) == 0 && mask_bits && xb), "bn_pool_fwd: packing needs C %% 32 == 0 and all pack outputs");
+  BDBNN_REQUIRE(!relu || (!pack && (C & 31) == 0 && mask_bits), "bn_pool_fwd_relu: needs C %% 32 == 0 and mask_bits");
+  // the ReLU is in the 3x3 / stride-2 / pad-1 kernel only (the pool of the torchvision ResNet stem)
+  BDBNN_REQUIRE(!relu || (k == 3 && stride == 2 && pad == 1 && C <= 4 * kBnThreads && kBnThreads % (C / 4) == 0),
+                "bn_pool_fwd_relu: needs the 3x3 / stride-2 / pad-1 pool and C dividing 1024");
   cudaStream_t st = cudaStream_t(stream);
   const int C4 = C / 4;
   const int64_t n_pix = int64_t(N) * H * W;
@@ -1397,12 +1511,18 @@ extern "C" int bdbnn_bn_pool_fwd(const float* y, const float* gamma, const float
   const int64_t total = int64_t(N) * Ho * Wo * C4;
   const int grid = bn_grid(total, C4);
   const float4* y4 = reinterpret_cast<const float4*>(y);
-  // PACK needs the 8 lanes of a 32-channel word inside one iteration of one warp: per-row work and the
-  // block size must be multiples of 8 quads, which C % 32 == 0 gives when blockDim is a multiple of C4
-  if (k == 3 && stride == 2 && pad == 1 && C4 <= kBnThreads && (!pack || (C4 % 8 == 0 && kBnThreads % C4 == 0))) {
+  if (relu) BDBNN_CUDA(cudaMemsetAsync(relu_amax, 0, sizeof(uint32_t), st));
+  // PACK (and RELU's mask words) need the 8 lanes of a 32-channel word inside one iteration of one warp: per-row work
+  // and the block size must be multiples of 8 quads, which C % 32 == 0 gives when blockDim is a multiple of C4
+  if (k == 3 && stride == 2 && pad == 1 && C4 <= kBnThreads &&
+      (!(pack || relu) || (C4 % 8 == 0 && kBnThreads % C4 == 0))) {
     const int threads = (kBnThreads / C4) * C4;
     const unsigned rows_grid = unsigned(N) * unsigned(Ho);
-    if (pack)
+    if (relu)
+      bn_pool_fwd_k3s2_kernel<false, true><<<rows_grid, threads, 0, st>>>(
+          y4, a, b, H, W, C4, Ho, Wo, reinterpret_cast<float4*>(z), reinterpret_cast<float4*>(y_sel),
+          reinterpret_cast<uint32_t*>(idx), nullptr, mask_bits, nullptr, nullptr, 0u, relu_amax);
+    else if (pack)
       bn_pool_fwd_k3s2_kernel<true><<<rows_grid, threads, 0, st>>>(
           y4, a, b, H, W, C4, Ho, Wo, reinterpret_cast<float4*>(z), reinterpret_cast<float4*>(y_sel),
           reinterpret_cast<uint32_t*>(idx), sign_bits, mask_bits, reinterpret_cast<uint2*>(xb),
@@ -1426,25 +1546,57 @@ extern "C" int bdbnn_bn_pool_fwd(const float* y, const float* gamma, const float
   return check_launch("bn_pool_fwd_kernel");
 }
 
-extern "C" int bdbnn_bn_pool_bwd(const float* g_pool, const uint8_t* idx, const float* y, const float* y_sel,
-                                 const float* mean, const float* invstd, const float* gamma, const float* ones,
-                                 const uint32_t* ymax_bits, int32_t N, int32_t H, int32_t W, int32_t C, int32_t k,
-                                 int32_t stride, int32_t pad, int32_t Ho, int32_t Wo, double* sums_ws,
-                                 uint32_t* gmax_bits, float* consts_ws, float* dgamma, float* dbeta,
-                                 uint32_t* amax_scratch, float* gy, uint16_t* gys, void* stream) {
+extern "C" int bdbnn_bn_pool_fwd(const float* y, const float* gamma, const float* beta, int32_t N, int32_t H,
+                                 int32_t W, int32_t C, int32_t k, int32_t stride, int32_t pad, int32_t Ho,
+                                 int32_t Wo, float eps, float momentum, float* running_mean, float* running_var,
+                                 double* sums_ws, uint32_t* ymax_bits, float* mean, float* invstd, float* ab_ws,
+                                 float* z, float* y_sel, uint8_t* idx, uint32_t* sign_bits, uint32_t* mask_bits,
+                                 uint16_t* xb, uint8_t* xb_fp8, int32_t fmt, int32_t stats_ready, void* stream) {
+  return bn_pool_fwd_impl(y, gamma, beta, N, H, W, C, k, stride, pad, Ho, Wo, eps, momentum, running_mean, running_var,
+                          sums_ws, ymax_bits, mean, invstd, ab_ws, z, y_sel, idx, sign_bits, mask_bits, xb, xb_fp8, fmt,
+                          stats_ready, stream);
+}
+
+extern "C" int bdbnn_bn_pool_fwd_relu(const float* y, const float* gamma, const float* beta, int32_t N, int32_t H,
+                                      int32_t W, int32_t C, int32_t k, int32_t stride, int32_t pad, int32_t Ho,
+                                      int32_t Wo, float eps, float momentum, float* running_mean, float* running_var,
+                                      double* sums_ws, uint32_t* ymax_bits, float* mean, float* invstd, float* ab_ws,
+                                      float* z, float* y_sel, uint8_t* idx, uint32_t* mask_bits, uint32_t* z_amax_bits,
+                                      int32_t stats_ready, void* stream) {
+  BDBNN_REQUIRE(z_amax_bits != nullptr, "bn_pool_fwd_relu: NULL z_amax_bits");
+  return bn_pool_fwd_impl(y, gamma, beta, N, H, W, C, k, stride, pad, Ho, Wo, eps, momentum, running_mean, running_var,
+                          sums_ws, ymax_bits, mean, invstd, ab_ws, z, y_sel, idx, nullptr, mask_bits, nullptr, nullptr,
+                          BDBNN_FMT_FP16, stats_ready, stream, z_amax_bits);
+}
+
+// relu_mask != NULL: bdbnn_bn_pool_bwd_relu (the pooled gradient masked by ReLU's words in the sums; the scatter needs
+// no mask, the forward wrote no winner where z is not > 0)
+static int bn_pool_bwd_impl(const float* g_pool, const uint8_t* idx, const float* y, const float* y_sel,
+                            const float* mean, const float* invstd, const float* gamma, const float* ones,
+                            const uint32_t* ymax_bits, int32_t N, int32_t H, int32_t W, int32_t C, int32_t k,
+                            int32_t stride, int32_t pad, int32_t Ho, int32_t Wo, double* sums_ws, uint32_t* gmax_bits,
+                            float* consts_ws, float* dgamma, float* dbeta, uint32_t* amax_scratch, float* gy,
+                            uint16_t* gys, void* stream, const uint32_t* relu_mask = nullptr) {
   int rc = pool_geom_ok(N, H, W, C, k, stride, pad, Ho, Wo);
   if (rc) return rc;
   BDBNN_REQUIRE(g_pool && idx && y && y_sel && mean && invstd && gamma && ones && ymax_bits && sums_ws && gmax_bits &&
                     consts_ws && dgamma && dbeta && amax_scratch && (gy || gys),
                 "bn_pool_bwd: NULL pointer");
+  BDBNN_REQUIRE(relu_mask == nullptr || (C & 31) == 0, "bn_pool_bwd_relu: the mask words need C %% 32 == 0");
   cudaStream_t st = cudaStream_t(stream);
   const int C4 = C / 4;
   const int64_t n_pool = int64_t(N) * Ho * Wo, n_full = int64_t(N) * H * W;
   BDBNN_CUDA(cudaMemsetAsync(sums_ws, 0, size_t(2 * C) * sizeof(double), st));
   BDBNN_CUDA(cudaMemsetAsync(gmax_bits, 0, size_t(C) * sizeof(uint32_t), st));
-  rc = bn_reduce_launch<true>(bn_grid(n_pool * C4 / 8, C4, 3), reinterpret_cast<const float4*>(g_pool),
-                              reinterpret_cast<const float4*>(y_sel), mean, invstd, n_pool, C4, sums_ws, gmax_bits,
-                              nullptr, st);
+  if (relu_mask != nullptr)
+    rc = bn_reduce_launch<true, false, false, true>(bn_grid(n_pool * C4 / 8, C4, 3),
+                                                    reinterpret_cast<const float4*>(g_pool),
+                                                    reinterpret_cast<const float4*>(y_sel), mean, invstd, n_pool, C4,
+                                                    sums_ws, gmax_bits, nullptr, st, nullptr, relu_mask);
+  else
+    rc = bn_reduce_launch<true>(bn_grid(n_pool * C4 / 8, C4, 3), reinterpret_cast<const float4*>(g_pool),
+                                reinterpret_cast<const float4*>(y_sel), mean, invstd, n_pool, C4, sums_ws, gmax_bits,
+                                nullptr, st);
   if (rc) return rc;
   // means are over the FULL-resolution element count; gscale = 1 (`ones`)
   const int per_dim = (k + stride - 1) / stride;          // pooling windows covering one position, per axis
@@ -1481,4 +1633,26 @@ extern "C" int bdbnn_bn_pool_bwd(const float* g_pool, const uint8_t* idx, const 
         reinterpret_cast<const float4*>(y), reinterpret_cast<const float4*>(consts_ws), N, H, W, C4, Ho, Wo, k,
         stride, pad, total, reinterpret_cast<float4*>(gy), nullptr, nullptr);
   return check_launch("bn_pool_bwd_kernel");
+}
+
+extern "C" int bdbnn_bn_pool_bwd(const float* g_pool, const uint8_t* idx, const float* y, const float* y_sel,
+                                 const float* mean, const float* invstd, const float* gamma, const float* ones,
+                                 const uint32_t* ymax_bits, int32_t N, int32_t H, int32_t W, int32_t C, int32_t k,
+                                 int32_t stride, int32_t pad, int32_t Ho, int32_t Wo, double* sums_ws,
+                                 uint32_t* gmax_bits, float* consts_ws, float* dgamma, float* dbeta,
+                                 uint32_t* amax_scratch, float* gy, uint16_t* gys, void* stream) {
+  return bn_pool_bwd_impl(g_pool, idx, y, y_sel, mean, invstd, gamma, ones, ymax_bits, N, H, W, C, k, stride, pad, Ho,
+                          Wo, sums_ws, gmax_bits, consts_ws, dgamma, dbeta, amax_scratch, gy, gys, stream);
+}
+
+extern "C" int bdbnn_bn_pool_bwd_relu(const float* g_pool, const uint8_t* idx, const uint32_t* mask_bits,
+                                      const float* y, const float* y_sel, const float* mean, const float* invstd,
+                                      const float* gamma, const float* ones, const uint32_t* ymax_bits, int32_t N,
+                                      int32_t H, int32_t W, int32_t C, int32_t k, int32_t stride, int32_t pad,
+                                      int32_t Ho, int32_t Wo, double* sums_ws, uint32_t* gmax_bits, float* consts_ws,
+                                      float* dgamma, float* dbeta, uint32_t* amax_scratch, float* gy, uint16_t* gys,
+                                      void* stream) {
+  BDBNN_REQUIRE(mask_bits != nullptr, "bn_pool_bwd_relu: NULL mask_bits");
+  return bn_pool_bwd_impl(g_pool, idx, y, y_sel, mean, invstd, gamma, ones, ymax_bits, N, H, W, C, k, stride, pad, Ho,
+                          Wo, sums_ws, gmax_bits, consts_ws, dgamma, dbeta, amax_scratch, gy, gys, stream, mask_bits);
 }

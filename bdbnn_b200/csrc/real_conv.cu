@@ -196,9 +196,31 @@ real_wt_multi_kernel(const __grid_constant__ RealWtTable tab, const uint32_t* __
   }
 }
 
+// The activation's scale folded into a 3x3 real x real conv's weight vectors (DESIGN.md §4r): x's fp16 operand is
+// fp16(x * 2^ex) with ex from x_amax_bits, so alpha[o] = alpha_w[o] * 2^-ex and inv_gscale[o] = inv_gscale_w[o] * 2^-ex
+// (powers of two: exact).
+__global__ void real_scale_fold_kernel(const uint32_t* __restrict__ x_amax_bits, const float* __restrict__ alpha_w,
+                                       const float* __restrict__ inv_gscale_w, int C, float* __restrict__ alpha,
+                                       float* __restrict__ inv_gscale) {
+  const int o = blockIdx.x * blockDim.x + threadIdx.x;
+  if (o >= C) return;
+  const float isx = amax_pow2_scale(__ldg(x_amax_bits), true);
+  alpha[o] = alpha_w[o] * isx;
+  inv_gscale[o] = inv_gscale_w[o] * isx;
+}
+
 }  // namespace bdbnn
 
 using namespace bdbnn;
+
+extern "C" int bdbnn_real_scale_fold(const uint32_t* x_amax_bits, const float* alpha_w, const float* inv_gscale_w,
+                                     int32_t C, float* alpha, float* inv_gscale, void* stream) {
+  BDBNN_REQUIRE(C > 0, "real_scale_fold: C must be positive");
+  BDBNN_REQUIRE(x_amax_bits && alpha_w && inv_gscale_w && alpha && inv_gscale, "real_scale_fold: NULL pointer");
+  real_scale_fold_kernel<<<(C + 127) / 128, 128, 0, cudaStream_t(stream)>>>(x_amax_bits, alpha_w, inv_gscale_w, C,
+                                                                            alpha, inv_gscale);
+  return check_launch("real_scale_fold_kernel");
+}
 
 extern "C" int bdbnn_real_act_pack(const float* x, int64_t n_pix, int32_t C, uint32_t* amax_bits, int32_t have_amax,
                                    uint16_t* xh, void* stream) {

@@ -1291,13 +1291,18 @@ def shortcut_supported(x, weight, stride):
     fp16s gradient mode (the operands are fp16), and all three kernels available for the 1x1 geometry."""
     if not (x.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and weight.dim() == 4):
         return False
-    cout, cin, kh, kw = weight.shape
-    if (kh, kw) != (1, 1) or cin != x.shape[1] or grad_mode()[0] != "fp16s":
+    return shortcut_shape_supported(tuple(x.shape), tuple(weight.shape), stride)
+
+
+def shortcut_shape_supported(x_shape, w_shape, stride):
+    """shortcut_supported's conditions on the shapes alone (host-only)."""
+    cout, cin, kh, kw = w_shape
+    if (kh, kw) != (1, 1) or cin != x_shape[1] or grad_mode()[0] != "fp16s":
         return False
-    n, _, h, w = x.shape
+    n, _, h, w = x_shape
     ho, wo = (h - 1) // stride + 1, (w - 1) // stride + 1
-    caps1 = int(_lib.lib().bdbnn_tc_supported(ctypes.byref(conv_shape((n, cin, ho, wo), weight.shape, 1, 0))))
-    capss = int(_lib.lib().bdbnn_tc_supported(ctypes.byref(conv_shape(x.shape, weight.shape, stride, 0))))
+    caps1 = int(_lib.lib().bdbnn_tc_supported(ctypes.byref(conv_shape((n, cin, ho, wo), w_shape, 1, 0))))
+    capss = int(_lib.lib().bdbnn_tc_supported(ctypes.byref(conv_shape(x_shape, w_shape, stride, 0))))
     return (caps1 & 5) == 5 and bool(capss & 2) and cout % 4 == 0 and cout <= 512
 
 
@@ -1404,9 +1409,11 @@ def shortcut_conv_bn(x, weight, gamma, beta, running_mean, running_var, momentum
     return _RealConvBN.apply(x, weight, gamma, beta, running_mean, running_var, momentum, eps, int(stride))
 
 
-def _bn_pool_fwd_impl(yc, gamma, beta, running_mean, running_var, momentum, eps, k, stride, pad, stats=None):
+def _bn_pool_fwd_impl(yc, gamma, beta, running_mean, running_var, momentum, eps, k, stride, pad, stats=None,
+                      relu=False):
     """bn_pool_fwd launch sequence on an NHWC-contiguous y. Returns (outs, saved, geom).
-    stats = (sums, ymax) already filled by the conv that produced y, or None."""
+    stats = (sums, ymax) already filled by the conv that produced y, or None.
+    relu: bn_pool_fwd_relu, z = maxpool(relu(BN(y))); outs = (z, z_amax) and the ReLU mask words are saved last."""
     L = _lib.lib()
     n, c, h, w = yc.shape
     if c % 4:
@@ -1425,6 +1432,19 @@ def _bn_pool_fwd_impl(yc, gamma, beta, running_mean, running_var, momentum, eps,
     z = torch.empty((n, c, ho, wo), memory_format=torch.channels_last, **f32)
     ysel = torch.empty((n, ho, wo, c), **f32)
     idx = torch.empty((n, ho, wo, c), dtype=torch.uint8, device=dev)
+    geom = (n, h, w, c, k, stride, pad, ho, wo)
+    if relu:
+        mask = torch.empty((n, ho, wo, c // 32), **i32)
+        z_amax = torch.empty((1,), **i32)
+        nbytes = 4 * n * h * w * c * (1 if stats is not None else 2) + (4 + 4 + 1 + 0.125) * n * ho * wo * c
+        with _timed("stem_bn_pool_fwd_relu", f"N{n}_{h}x{w}_c{c}", nbytes):
+            _lib.check(L.bdbnn_bn_pool_fwd_relu(_p(yc), _p(gamma.detach()), _p(beta.detach()), n, h, w, c, k, stride,
+                                                pad, ho, wo, float(eps), float(momentum), _p(running_mean),
+                                                _p(running_var), _p(sums), _p(ymax), _p(mean), _p(invstd), _p(ab),
+                                                _p(z), _p(ysel), _p(idx), _p(mask), _p(z_amax),
+                                                1 if stats is not None else 0, _stream()), "bn_pool_fwd_relu")
+        _lib.count(2 if stats is not None else 3)
+        return (z, z_amax), (yc, ysel, idx, mean, invstd, gamma.detach(), ymax, mask), geom
     pack = c % 32 == 0
     zs = torch.empty((n, ho, wo, c // 32), **i32) if pack else None
     zm = torch.empty((n, ho, wo, c // 32), **i32) if pack else None
@@ -1438,14 +1458,16 @@ def _bn_pool_fwd_impl(yc, gamma, beta, running_mean, running_var, momentum, eps,
                                        _p(zs), _p(zm), _p(zb), _p(zb8), fmt, 1 if stats is not None else 0,
                                        _stream()), "bn_pool_fwd")
     _lib.count(2 if stats is not None else 3)
-    return (z, zs, zm, zb, zb8), (yc, ysel, idx, mean, invstd, gamma.detach(), ymax), (n, h, w, c, k, stride, pad, ho, wo)
+    return (z, zs, zm, zb, zb8), (yc, ysel, idx, mean, invstd, gamma.detach(), ymax), geom
 
 
 def _bn_pool_bwd_impl(gz, saved, geom, half):
     """bn_pool_bwd launch sequence. half=False -> (gy fp32 NCHW-shaped channels_last, dgamma, dbeta);
-    half=True -> ((gys fp16 x 2^e [N,H,W,C], amax word), dgamma, dbeta): the fp32 gradient is never written."""
+    half=True -> ((gys fp16 x 2^e [N,H,W,C], amax word), dgamma, dbeta): the fp32 gradient is never written.
+    saved with the ReLU mask words last (_bn_pool_fwd_impl(relu=True)): bn_pool_bwd_relu."""
     L = _lib.lib()
-    yc, ysel, idx, mean, invstd, gamma, ymax = saved
+    yc, ysel, idx, mean, invstd, gamma, ymax = saved[:7]
+    mask = saved[7] if len(saved) > 7 else None
     n, h, w, c, k, stride, pad, ho, wo = geom
     dev = gz.device
     g = _nhwc(gz)
@@ -1462,10 +1484,18 @@ def _bn_pool_bwd_impl(gz, saved, geom, half):
     else:
         gy = torch.empty((n, c, h, w), memory_format=torch.channels_last, **f32)
     nbytes = 8 * n * ho * wo * c + (4 + (2 if half else 4)) * n * h * w * c + 5 * n * ho * wo * c
-    with _timed("stem_bn_pool_bwd", f"N{n}_{h}x{w}_c{c}", nbytes):
-        _lib.check(L.bdbnn_bn_pool_bwd(_p(g), _p(idx), _p(yc), _p(ysel), _p(mean), _p(invstd), _p(gamma), _p(ones),
-                                       _p(ymax), n, h, w, c, k, stride, pad, ho, wo, _p(sums), _p(gmax), _p(consts),
-                                       _p(dgamma), _p(dbeta), _p(amax), _p(gy), _p(gys), _stream()), "bn_pool_bwd")
+    if mask is not None:
+        with _timed("stem_bn_pool_bwd_relu", f"N{n}_{h}x{w}_c{c}", nbytes + n * ho * wo * c / 8):
+            _lib.check(L.bdbnn_bn_pool_bwd_relu(_p(g), _p(idx), _p(mask), _p(yc), _p(ysel), _p(mean), _p(invstd),
+                                                _p(gamma), _p(ones), _p(ymax), n, h, w, c, k, stride, pad, ho, wo,
+                                                _p(sums), _p(gmax), _p(consts), _p(dgamma), _p(dbeta), _p(amax),
+                                                _p(gy), _p(gys), _stream()), "bn_pool_bwd_relu")
+    else:
+        with _timed("stem_bn_pool_bwd", f"N{n}_{h}x{w}_c{c}", nbytes):
+            _lib.check(L.bdbnn_bn_pool_bwd(_p(g), _p(idx), _p(yc), _p(ysel), _p(mean), _p(invstd), _p(gamma),
+                                           _p(ones), _p(ymax), n, h, w, c, k, stride, pad, ho, wo, _p(sums), _p(gmax),
+                                           _p(consts), _p(dgamma), _p(dbeta), _p(amax), _p(gy), _p(gys), _stream()),
+                       "bn_pool_bwd")
     _lib.count(3)
     return ((gys, amax) if half else gy), dgamma, dbeta
 
@@ -1603,15 +1633,16 @@ class _StemConv(torch.autograd.Function):
 
 class _StemFused(torch.autograd.Function):
     """z = maxpool(BN_train(conv7x7/2(x, W))) as ONE autograd node: the conv output's gradient goes from
-    bn_pool_bwd to stem_conv_wgrad as the fp16 operand only (no fp32 gradient of the 112x112x64 tensor)."""
+    bn_pool_bwd to stem_conv_wgrad as the fp16 operand only (no fp32 gradient of the 112x112x64 tensor).
+    relu: z = maxpool(relu(BN_train(conv7x7/2(x, W)))), returned with its max|z| word (DESIGN.md §4r)."""
 
     @staticmethod
     @_on_device
-    def forward(ctx, x, weight, gamma, beta, running_mean, running_var, momentum, eps, k, stride, pad):
+    def forward(ctx, x, weight, gamma, beta, running_mean, running_var, momentum, eps, k, stride, pad, relu=False):
         ctx.set_materialize_grads(False)
         y, xw, x_amax, stats = _stem_conv_fwd_impl(x, weight, want_stats=True)
         outs, saved, ctx.geom = _bn_pool_fwd_impl(y, gamma, beta, running_mean, running_var, momentum, eps, k,
-                                                  stride, pad, stats)
+                                                  stride, pad, stats, relu)
         ctx.xgeom = (x.shape[0], x.shape[2], x.shape[3])
         ctx.w_param = weight if (weight.is_leaf and weight.requires_grad) else None
         ctx.save_for_backward(xw, x_amax, *saved)
@@ -1624,12 +1655,12 @@ class _StemFused(torch.autograd.Function):
     @_on_device
     def backward(ctx, gz, *_unused):
         if gz is None:
-            return (None,) * 11
+            return (None,) * 12
         xw, x_amax = ctx.saved_tensors[:2]
         (gys, g_amax), dgamma, dbeta = _bn_pool_bwd_impl(gz, ctx.saved_tensors[2:], ctx.geom, half=True)
         gw = _stem_wgrad_impl(gys, g_amax, xw, x_amax, *ctx.xgeom, w_param=ctx.w_param) if ctx.needs_input_grad[1] else None
         return (None, gw, dgamma if ctx.needs_input_grad[2] else None, dbeta if ctx.needs_input_grad[3] else None,
-                None, None, None, None, None, None, None)
+                None, None, None, None, None, None, None, None)
 
 
 def stem_conv_bn_pool(x, weight, gamma, beta, running_mean, running_var, momentum, eps, kernel_size, stride, padding):
@@ -2466,3 +2497,136 @@ def conv_pool_bn_eval(x, weight, gamma, beta, running_mean, running_var, eps, pa
     _lib.count(1)
     _set_eval_pack(z, *((-1, zb8) if out8 else (fmt, zb)))
     return z
+
+
+# ---------------------------------------------------------------------------------------------------
+# Training units of torchvision's fp32 ResNet-18/34 (DESIGN.md §4r): a real x real 3x3 conv + BatchNorm(train)
+# (+ residual) + ReLU, and the stem with its ReLU.  fp16 operands under power-of-two scales (TF32-class), the scales
+# folded into the per-channel vectors the wgmma kernels take (as §4f and §4p).
+# ---------------------------------------------------------------------------------------------------
+def real_unit_supported(x_shape, w_shape, stride, padding):
+    """real_conv_bn_relu's geometry (host-only): all three wgmma kernels for the conv, Cin % 4 == 0 (the fp16 operand
+    pack), Cout % 32 == 0 (ReLU's mask words) and Cout <= 512 (the BatchNorm statistics in the conv's epilogue)."""
+    return (x_shape[1] % 4 == 0 and w_shape[0] % 32 == 0 and w_shape[0] <= 512 and
+            unit_supported(x_shape, w_shape, stride, padding))
+
+
+def _real_scale_fold(amax, wp):
+    """(alpha, inv_gscale) of the conv of an activation scaled by `amax`'s exponent and the weight pack wp."""
+    alpha, inv_gscale = torch.empty_like(wp.alpha), torch.empty_like(wp.inv_gscale)
+    _lib.check(_lib.lib().bdbnn_real_scale_fold(_p(amax), _p(wp.alpha), _p(wp.inv_gscale), wp.alpha.numel(),
+                                                _p(alpha), _p(inv_gscale), _stream()), "real_scale_fold")
+    _lib.count(1)
+    return alpha, inv_gscale
+
+
+class _RealConvBNReLU(torch.autograd.Function):
+    """z = relu(BN_train(conv2d(x, W, stride, pad 1)) + residual) of a real-valued 3x3 conv (DESIGN.md §4r).
+    forward : real_act_pack(x, x_amax) -> real_scale_fold -> binconv_fwd_tc (fp16 operands, BatchNorm statistics in
+              the epilogue) -> bn_fwd_relu (z, ReLU's mask words, max|z|)
+    backward: bn_bwd_pack_relu (gz masked, which is also the residual's gradient) -> wgrad_tc, dgrad_tc with all-ones
+              STE masks."""
+
+    @staticmethod
+    @_on_device
+    def forward(ctx, x, weight, gamma, beta, residual, x_amax, wpack, running_mean, running_var, momentum, eps, stride):
+        _require_cuda(x, "real_conv_bn_relu(x)")
+        _same_device(x, weight, gamma, beta, residual, x_amax, running_mean, running_var)
+        _require_fp16s("real_conv_bn_relu")
+        ctx.set_materialize_grads(False)
+        L = _lib.lib()
+        sh = conv_shape(x.shape, weight.shape, stride, 1)
+        if not real_unit_supported(x.shape, weight.shape, stride, 1):
+            raise RuntimeError(f"bdbnn_b200.real_conv_bn_relu: no kernel for input {tuple(x.shape)}, weight "
+                               f"{tuple(weight.shape)}, stride {stride}")
+        z_shape = (sh.N, sh.Cout, sh.Ho, sh.Wo)
+        if residual is not None and tuple(residual.shape) != z_shape:
+            raise RuntimeError(f"real_conv_bn_relu: residual shape {tuple(residual.shape)} != output shape {z_shape}")
+        dev = x.device
+        st = _stream()
+        key = _shape_key(sh)
+        cout, n_pix = sh.Cout, sh.N * sh.Ho * sh.Wo
+        _, xh, amax = _real_act_pack(x, x_amax, sh)
+        alpha, inv_gscale = _real_scale_fold(amax, wpack)
+        f32 = dict(dtype=torch.float32, device=dev)
+        y = torch.empty(z_shape, memory_format=torch.channels_last, **f32)
+        sums = torch.empty((2 * cout,), dtype=torch.float64, device=dev)
+        ymax = torch.empty((cout,), dtype=torch.int32, device=dev)
+        with _timed("real_conv_fwd_tc", key, algorithmic_bytes("fwd_tc", sh)):
+            _lib.check(L.bdbnn_binconv_fwd_tc(_p(xh), _p(wpack.wf), FMT_FP16, _p(alpha), _p(y), ctypes.byref(sh),
+                                              _p(sums), _p(ymax), st), "binconv_fwd_tc(real)")
+        _lib.count(1)
+        rc = _nhwc(residual.detach()) if residual is not None else None
+        z = torch.empty_like(y)
+        mean, invstd, ab = torch.empty((cout,), **f32), torch.empty((cout,), **f32), torch.empty((2 * cout,), **f32)
+        mask = torch.empty((sh.N, sh.Ho, sh.Wo, cout // 32), dtype=torch.int32, device=dev)
+        z_amax = torch.empty((1,), dtype=torch.int32, device=dev)
+        with _timed("real_bn_fwd_relu", key, (8 + (4 if rc is not None else 0) + 0.125) * n_pix * cout):
+            _lib.check(L.bdbnn_bn_fwd_relu(_p(y), _p(rc), _p(gamma.detach()), _p(beta.detach()), n_pix, cout,
+                                           float(eps), float(momentum), _p(running_mean), _p(running_var), _p(sums),
+                                           _p(ymax), _p(mean), _p(invstd), _p(ab), _p(z), _p(mask), _p(z_amax), 1, st),
+                       "bn_fwd_relu")
+        _lib.count(2)
+        ctx.sh = sh
+        ctx.x_shape, ctx.w_shape = tuple(x.shape), tuple(weight.shape)
+        ctx.w_param = weight if (weight.is_leaf and weight.requires_grad) else None
+        ctx.has_res = residual is not None
+        ctx.save_for_backward(y, mean, invstd, gamma.detach(), ymax, mask, xh, wpack.wt, wpack.wmask, wpack.gscale,
+                              inv_gscale)
+        ctx.mark_non_differentiable(z_amax)
+        return z, z_amax
+
+    @staticmethod
+    @_on_device
+    def backward(ctx, gz, _g_amax):
+        if gz is None:
+            return (None,) * 12
+        L = _lib.lib()
+        sh = ctx.sh
+        dev = gz.device
+        y, mean, invstd, gamma, ymax, mask, xh, wt, wmask, gscale, inv_gscale = ctx.saved_tensors
+        key = _shape_key(sh)
+        g = _nhwc(gz)
+        cout, n_pix = sh.Cout, sh.N * sh.Ho * sh.Wo
+        sums, gmax, consts, dgamma, dbeta, amax, gys = _bn_grads(cout, (sh.N, sh.Ho, sh.Wo), 1, dev)
+        gres = None
+        if ctx.has_res and ctx.needs_input_grad[4]:
+            gres = torch.empty((sh.N, cout, sh.Ho, sh.Wo), dtype=torch.float32, device=dev,
+                               memory_format=torch.channels_last)
+        with _timed("real_bn_bwd_pack_relu", key, (16 + 2 + 0.25 + (4 if gres is not None else 0)) * n_pix * cout):
+            _lib.check(L.bdbnn_bn_bwd_pack_relu(_p(g), _p(mask), _p(y), _p(mean), _p(invstd), _p(gamma), _p(gscale),
+                                                _p(ymax), n_pix, cout, GRAD_MODES["fp16s"], _p(sums), _p(gmax),
+                                                _p(consts), _p(dgamma), _p(dbeta), _p(amax), _p(gys), _p(gres),
+                                                _stream()), "bn_bwd_pack_relu")
+        _lib.count(3)
+        gx = gw = None
+        # the weight gradient first: in a wgrad_side scope it forks off here and overlaps the dgrad
+        if ctx.needs_input_grad[1]:
+            gw = _wgrad_tc(sh, gys, GRAD_MODES["fp16s"], amax, xh, wmask, inv_gscale, ctx.w_shape, ctx.w_param,
+                           "real_conv_wgrad_tc", key, algorithmic_bytes("wgrad_tc", sh))
+        if ctx.needs_input_grad[0]:
+            ones = torch.full((sh.N, sh.H, sh.W, (sh.Cin + 31) // 32), -1, dtype=torch.int32, device=dev)
+            gx = torch.empty(ctx.x_shape, dtype=torch.float32, device=dev, memory_format=torch.channels_last)
+            _dgrad_tc(sh, gys, GRAD_MODES["fp16s"], amax, wt, ones, None, gx, "real_conv_dgrad_tc",
+                      algorithmic_bytes("dgrad_tc", sh))
+        return (gx, gw, dgamma if ctx.needs_input_grad[2] else None, dbeta if ctx.needs_input_grad[3] else None, gres,
+                None, None, None, None, None, None, None)
+
+
+def real_conv_bn_relu(x, x_amax, wpack, weight, gamma, beta, running_mean, running_var, momentum, eps, stride,
+                      residual=None):
+    """z = relu(BN_train(conv2d(x, weight, stride, padding 1)) + residual) of a real-valued 3x3 conv on the wgmma
+    kernels, with autograd (DESIGN.md §4r; geometry: real_unit_supported; gradient mode fp16s).  wpack: weight's
+    _WeightPack from real_weight_grad_pack; x_amax: the max|x| word the call that wrote x returned (None: computed
+    here).  Returns (z fp32 channels_last, z_amax int32[1] = bits of max|z|, for the next unit's x_amax)."""
+    return _RealConvBNReLU.apply(x, weight, gamma, beta, residual, x_amax, wpack, running_mean, running_var,
+                                 float(momentum), float(eps), int(stride))
+
+
+def stem_conv_bn_relu_pool(x, weight, gamma, beta, running_mean, running_var, momentum, eps, kernel_size, stride,
+                           padding):
+    """maxpool(relu(BN_train(stem_conv(x)))) with autograd: the training stem of a torchvision ResNet (DESIGN.md §4r),
+    3x3 / stride-2 / pad-1 pool only.  Returns (z fp32 channels_last, z_amax int32[1] = bits of max|z|)."""
+    if (int(kernel_size), int(stride), int(padding)) != (3, 2, 1):
+        raise RuntimeError("bdbnn_b200.stem_conv_bn_relu_pool: the ReLU stem pool is 3x3 / stride 2 / pad 1")
+    return _StemFused.apply(x, weight, gamma, beta, running_mean, running_var, momentum, eps, 3, 2, 1, True)

@@ -1,0 +1,125 @@
+"""Training torchvision's fp32 ResNet-18/34 on this repository's kernels (DESIGN.md §4r).
+
+    model = RealResNet(torchvision.models.resnet18())      # or resnet34
+
+wraps the model without copying it, as FrozenResNetTeacher does: the wrapper's children ARE the model's children, so
+`named_parameters()` and `state_dict()` have the model's names and objects, and `load_state_dict`, `.cuda()` and
+`.train()` act on the model.
+
+In training mode, on a CUDA fp32 input whose geometry every unit takes, the forward runs with autograd as
+
+    z  = maxpool(relu(BN_train(conv1(x))))                  stem_conv_bn_relu_pool
+    z1 = relu(BN1_train(conv1(z)))                          real_conv_bn_relu            per BasicBlock
+    r  = z, or BN_ds_train(conv_ds(z))                      shortcut_conv_bn
+    z  = relu(BN2_train(conv2(z1)) + r)                     real_conv_bn_relu(residual=r)
+    logits = fc(flatten(avgpool(z)))                        torch
+
+In eval mode under no_grad it is FrozenResNetTeacher's eval kernel forward.  Anything else (CPU, other dtypes,
+unsupported geometry, BDBNN_FUSE_BN=0, a gradient mode other than fp16s, eval mode with autograd) returns the wrapped
+model's own forward."""
+import torch
+
+from . import functional as F_
+from .teacher import FrozenResNetTeacher, _family
+
+
+def _bn_train_args(bn):
+    return bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.momentum, bn.eps
+
+
+class RealResNet(FrozenResNetTeacher):
+    """A torchvision resnet18 / resnet34 (exactly torchvision's ResNet with BasicBlocks) trained on the real-valued
+    training units, with FrozenResNetTeacher's structure check, geometry walk and eval forward.  Raises TypeError for
+    any other structure (Bottleneck ResNets, subclasses, nn.DataParallel, custom blocks), naming the module."""
+
+    def __init__(self, model):
+        from torchvision.models import resnet as tv
+        if type(model) is not tv.ResNet:
+            raise TypeError(f"RealResNet wraps a torchvision ResNet with BasicBlocks (resnet18/34), got "
+                            f"{type(model).__name__}")
+        if _family(model).bottleneck:
+            raise TypeError("RealResNet wraps torchvision BasicBlock ResNets (resnet18/34); layer1.0 is a Bottleneck")
+        try:
+            super().__init__(model)
+        except TypeError as e:      # the teacher's structure check: name the class the caller used
+            raise TypeError(str(e).replace("FrozenResNetTeacher", "RealResNet")) from None
+        self.__dict__["_train_ok"] = {}
+
+    def kernel_path(self, x):
+        """True when forward(x) runs on this repository's kernels: the training units in training mode, the eval
+        kernels in eval mode (see the module docstring)."""
+        if not F_.fuse_enabled():
+            return False
+        if self.training:
+            return self._train_supported(x)
+        return super().kernel_path(x)
+
+    def forward(self, x):
+        if not self.training:
+            return super().forward(x)            # the eval kernels through kernel_path, else the model
+        if not self.kernel_path(x):
+            return self._wrapped(x)
+        with torch.cuda.device(x.device):
+            return self._train_forward(x)
+
+    # ---- path selection ----------------------------------------------------------------------------------------
+    def _train_supported(self, x):
+        if not (torch.is_tensor(x) and x.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and x.shape[1] == 3):
+            return False
+        if F_.grad_mode()[0] != "fp16s":
+            return False
+        for bn in self._bns():
+            if not (bn.training and bn.affine and bn.track_running_stats and bn.momentum is not None and
+                    bn.running_mean is not None):
+                return False
+        if any(p.device != x.device or p.dtype != torch.float32 for p in self.parameters()):
+            return False
+        c1 = self.conv1
+        if self._pool_args() != (3, 2, 1) or not F_.stem_conv_supported(x, c1.weight, c1.stride, c1.padding):
+            return False
+        key = (x.device, tuple(x.shape))
+        ok = self._train_ok.get(key)
+        if ok is None:
+            ok = self._train_ok[key] = self._walk_train_geometry(x)
+        return ok
+
+    def _walk_train_geometry(self, x):
+        """Every 3x3 conv has its training unit and every `downsample` its shortcut unit at this input size, and each
+        block's shortcut has its output's shape (host-only)."""
+        n, _, h, w = x.shape
+        ho, wo = (h - 1) // 2 + 1, (w - 1) // 2 + 1
+        shape = (n, self.conv1.out_channels, (ho - 1) // 2 + 1, (wo - 1) // 2 + 1)
+        for blk in self._blocks:
+            x_shape = shape
+            for conv in (blk.conv1, blk.conv2):
+                if not F_.real_unit_supported(shape, conv.weight.shape, conv.stride[0], conv.padding[0]):
+                    return False
+                sh = F_.conv_shape(shape, conv.weight.shape, conv.stride[0], conv.padding[0])
+                shape = (n, sh.Cout, sh.Ho, sh.Wo)
+            ds = blk.downsample
+            if ds is None:
+                if x_shape != shape:
+                    return False
+            else:
+                sd = ds[0].stride[0]
+                if not F_.shortcut_shape_supported(x_shape, tuple(ds[0].weight.shape), sd):
+                    return False
+                if (n, ds[0].out_channels, (x_shape[2] - 1) // sd + 1, (x_shape[3] - 1) // sd + 1) != shape:
+                    return False
+        return True
+
+    # ---- training forward --------------------------------------------------------------------------------------
+    def _train_forward(self, x):
+        # the 3x3 weights in one pack per forward, never cached: the optimizers update them in place
+        packs = F_.real_weight_grad_pack([c.weight for c in self._convs])
+        c1 = self.conv1
+        z, z_amax = F_.stem_conv_bn_relu_pool(x, c1.weight, *_bn_train_args(self.bn1), *self._pool_args())
+        for i, blk in enumerate(self._blocks):
+            ds = blk.downsample
+            res = z if ds is None else F_.shortcut_conv_bn(z, ds[0].weight, *_bn_train_args(ds[1]), ds[0].stride[0])
+            y, y_amax = F_.real_conv_bn_relu(z, z_amax, packs[2 * i], blk.conv1.weight, *_bn_train_args(blk.bn1),
+                                             blk.conv1.stride[0])
+            z, z_amax = F_.real_conv_bn_relu(y, y_amax, packs[2 * i + 1], blk.conv2.weight, *_bn_train_args(blk.bn2),
+                                             1, residual=res)
+        torch._foreach_add_([bn.num_batches_tracked for bn in self._bns()], 1)
+        return self.fc(torch.flatten(self.avgpool(z), 1))

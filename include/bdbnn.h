@@ -396,6 +396,48 @@ BDBNN_API int bdbnn_real_pool2_bn_eval_hardtanh(const float* y, const float* sca
                                       int32_t H, int32_t W, int32_t C, float* z, uint32_t* z_amax_bits,
                                       void* stream);
 
+/* ---- ReLU units of the fp32 ResNet trained on the wgmma kernels (DESIGN.md §4r) ------------------------------------
+ * bn_fwd_relu : bdbnn_bn_fwd on fp32 y (residual may be NULL), then z = relu(u) for u = BatchNorm(y) (+ residual)
+ *          (torch.relu bit for bit: NaN and -0.0 stay).  No +-1 packs; instead mask_bits u32 [n_pix][C/32]
+ *          (C % 32 == 0) = ReLU's gradient mask, bit c % 32 of word c / 32 set <=> !(z <= 0) (so set at NaN: torch's
+ *          relu backward passes the gradient there), and
+ *          z_amax_bits (one word, zeroed here) = bits of max|z| (integer atomicMax, NaN above every number), the word
+ *          bdbnn_real_act_pack takes for the next conv's fp16 operand.
+ * bn_bwd_pack_relu : bdbnn_bn_bwd_pack (grad_mode FP16S) of g = gz where the mask bit is set, 0 elsewhere (a select:
+ *          a NaN of gz where z <= 0 gives 0); the sums are always computed here.  g_out (may be NULL) receives g, fp32
+ *          like gz: the gradient of the residual added before the ReLU.
+ * bn_pool_fwd_relu : bdbnn_bn_pool_fwd with z = relu(maxpool(u)) = maxpool(relu(u)) and no +-1 packs; mask_bits and
+ *          z_amax_bits as bn_fwd_relu (on the pooled z, C % 32 == 0); where the mask bit is 0 the winner byte is 0xff,
+ *          so that bn_pool_bwd_relu sends that window's gradient nowhere (a NaN window keeps its winner).
+ * bn_pool_bwd_relu : bdbnn_bn_pool_bwd with g_pool masked by mask_bits (bn_pool_fwd_relu's) in the sums and, through
+ *          idx, in the scatter.
+ * real_scale_fold : alpha[o] = alpha_w[o] * 2^-ex, inv_gscale[o] = inv_gscale_w[o] * 2^-ex for o < C, ex the exponent
+ *          bdbnn_real_act_pack scales x by (x_amax_bits): the vectors bdbnn_binconv_fwd_tc and bdbnn_binconv_wgrad_tc
+ *          take for a 3x3 conv of fp16 x by the weight pack of bdbnn_real_weight_pack_multi_grad.  One launch. */
+BDBNN_API int bdbnn_bn_fwd_relu(const float* y, const float* residual, const float* gamma, const float* beta,
+                      int64_t n_pix, int32_t C, float eps, float momentum, float* running_mean, float* running_var,
+                      double* sums_ws, uint32_t* ymax_bits, float* mean, float* invstd, float* ab_ws, float* z,
+                      uint32_t* mask_bits, uint32_t* z_amax_bits, int32_t stats_ready, void* stream);
+BDBNN_API int bdbnn_bn_bwd_pack_relu(const float* gz, const uint32_t* mask_bits, const float* y, const float* mean,
+                           const float* invstd, const float* gamma, const float* gscale, const uint32_t* ymax_bits,
+                           int64_t n_pix, int32_t C, int32_t grad_mode, double* sums_ws, uint32_t* gmax_bits,
+                           float* consts_ws, float* dgamma, float* dbeta, uint32_t* amax_bits, uint16_t* gys,
+                           float* g_out, void* stream);
+BDBNN_API int bdbnn_bn_pool_fwd_relu(const float* y, const float* gamma, const float* beta, int32_t N, int32_t H,
+                           int32_t W, int32_t C, int32_t k, int32_t stride, int32_t pad, int32_t Ho, int32_t Wo,
+                           float eps, float momentum, float* running_mean, float* running_var, double* sums_ws,
+                           uint32_t* ymax_bits, float* mean, float* invstd, float* ab_ws, float* z, float* y_sel,
+                           uint8_t* idx, uint32_t* mask_bits, uint32_t* z_amax_bits, int32_t stats_ready,
+                           void* stream);
+BDBNN_API int bdbnn_bn_pool_bwd_relu(const float* g_pool, const uint8_t* idx, const uint32_t* mask_bits, const float* y,
+                           const float* y_sel, const float* mean, const float* invstd, const float* gamma,
+                           const float* ones, const uint32_t* ymax_bits, int32_t N, int32_t H, int32_t W, int32_t C,
+                           int32_t k, int32_t stride, int32_t pad, int32_t Ho, int32_t Wo, double* sums_ws,
+                           uint32_t* gmax_bits, float* consts_ws, float* dgamma, float* dbeta,
+                           uint32_t* amax_scratch, float* gy, uint16_t* gys, void* stream);
+BDBNN_API int bdbnn_real_scale_fold(const uint32_t* x_amax_bits, const float* alpha_w, const float* inv_gscale_w,
+                          int32_t C, float* alpha, float* inv_gscale, void* stream);
+
 /* ---- CIFAR stem: 3x3 / stride 1 / pad 1, 3 -> Cout channels (Cout in {16, 32, 48, 64, 128}), fp32, CUDA cores -
  * Replaces the fp32 nn.Conv2d `conv1` of the CIFAR ResNets (models/cifar10; model(images), train.py:492 and its
  * weight gradient under loss.backward(), train.py:528), which the reference runs on cuDNN.
