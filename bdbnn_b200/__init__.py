@@ -5,9 +5,10 @@ from .losses import (KurtosisWeight, DistributionLoss, DistributionLoss_layer,
                      kurtosis_regularization, matched_weight_pairs)
 from .functional import binact_conv2d, binconv2d, kurtosis_multi, kd_logits_loss, kd_layer_loss
 from .teacher import FrozenBottleneckTeacher, FrozenResNetTeacher, FrozenVGGTeacher
-from .realnet import RealResNet
+from .realnet import RealBottleneckResNet, RealResNet
 
 __all__ = ["BinarizeConv2d", "BinaryActivationConv2d", "HardBinaryConv", "HardBinaryConv_react", "HardBinaryConv_cifar",
            "KurtosisWeight", "DistributionLoss", "DistributionLoss_layer", "kurtosis_regularization",
            "matched_weight_pairs", "binact_conv2d", "binconv2d", "kurtosis_multi", "kd_logits_loss", "kd_layer_loss",
-           "FrozenBottleneckTeacher", "FrozenResNetTeacher", "FrozenVGGTeacher", "RealResNet"]
+           "FrozenBottleneckTeacher", "FrozenResNetTeacher", "FrozenVGGTeacher", "RealBottleneckResNet",
+           "RealResNet"]

@@ -2500,14 +2500,18 @@ def conv_pool_bn_eval(x, weight, gamma, beta, running_mean, running_var, eps, pa
 
 
 # ---------------------------------------------------------------------------------------------------
-# Training units of torchvision's fp32 ResNet-18/34 (DESIGN.md §4r): a real x real 3x3 conv + BatchNorm(train)
-# (+ residual) + ReLU, and the stem with its ReLU.  fp16 operands under power-of-two scales (TF32-class), the scales
-# folded into the per-channel vectors the wgmma kernels take (as §4f and §4p).
+# Training units of torchvision's fp32 ResNets (DESIGN.md §4r, §4s): a real x real conv + BatchNorm(train)
+# (+ residual) (+ ReLU).  fp16 operands under power-of-two scales (TF32-class), the scales folded into the per-channel
+# vectors the wgmma kernels take (as §4f and §4p).
 # ---------------------------------------------------------------------------------------------------
-def real_unit_supported(x_shape, w_shape, stride, padding):
+REAL_MAX_COUT = 4096     # the BatchNorm kernels' channel limit (csrc/bn.cu)
+
+
+def real_unit_supported(x_shape, w_shape, stride, padding, max_cout=512):
     """real_conv_bn_relu's geometry (host-only): all three wgmma kernels for the conv, Cin % 4 == 0 (the fp16 operand
-    pack), Cout % 32 == 0 (ReLU's mask words) and Cout <= 512 (the BatchNorm statistics in the conv's epilogue)."""
-    return (x_shape[1] % 4 == 0 and w_shape[0] % 32 == 0 and w_shape[0] <= 512 and
+    pack), Cout % 32 == 0 (ReLU's mask words) and Cout <= max_cout.  512 is ResNet-18/34's widest conv; the unit itself
+    takes up to REAL_MAX_COUT, which the Bottleneck ResNets' walk asks for (their conv3 and downsample reach 2048)."""
+    return (x_shape[1] % 4 == 0 and w_shape[0] % 32 == 0 and w_shape[0] <= max_cout and
             unit_supported(x_shape, w_shape, stride, padding))
 
 
@@ -2520,45 +2524,40 @@ def _real_scale_fold(amax, wp):
     return alpha, inv_gscale
 
 
-class _RealConvBNReLU(torch.autograd.Function):
-    """z = relu(BN_train(conv2d(x, W, stride, pad 1)) + residual) of a real-valued 3x3 conv (DESIGN.md §4r).
-    forward : real_act_pack(x, x_amax) -> real_scale_fold -> binconv_fwd_tc (fp16 operands, BatchNorm statistics in
-              the epilogue) -> bn_fwd_relu (z, ReLU's mask words, max|z|)
-    backward: bn_bwd_pack_relu (gz masked, which is also the residual's gradient) -> wgrad_tc, dgrad_tc with all-ones
-              STE masks."""
-
-    @staticmethod
-    @_on_device
-    def forward(ctx, x, weight, gamma, beta, residual, x_amax, wpack, running_mean, running_var, momentum, eps, stride):
-        _require_cuda(x, "real_conv_bn_relu(x)")
-        _same_device(x, weight, gamma, beta, residual, x_amax, running_mean, running_var)
-        _require_fp16s("real_conv_bn_relu")
-        ctx.set_materialize_grads(False)
-        L = _lib.lib()
-        sh = conv_shape(x.shape, weight.shape, stride, 1)
-        if not real_unit_supported(x.shape, weight.shape, stride, 1):
-            raise RuntimeError(f"bdbnn_b200.real_conv_bn_relu: no kernel for input {tuple(x.shape)}, weight "
-                               f"{tuple(weight.shape)}, stride {stride}")
-        z_shape = (sh.N, sh.Cout, sh.Ho, sh.Wo)
-        if residual is not None and tuple(residual.shape) != z_shape:
-            raise RuntimeError(f"real_conv_bn_relu: residual shape {tuple(residual.shape)} != output shape {z_shape}")
-        dev = x.device
-        st = _stream()
-        key = _shape_key(sh)
-        cout, n_pix = sh.Cout, sh.N * sh.Ho * sh.Wo
-        _, xh, amax = _real_act_pack(x, x_amax, sh)
-        alpha, inv_gscale = _real_scale_fold(amax, wpack)
-        f32 = dict(dtype=torch.float32, device=dev)
-        y = torch.empty(z_shape, memory_format=torch.channels_last, **f32)
-        sums = torch.empty((2 * cout,), dtype=torch.float64, device=dev)
-        ymax = torch.empty((cout,), dtype=torch.int32, device=dev)
-        with _timed("real_conv_fwd_tc", key, algorithmic_bytes("fwd_tc", sh)):
-            _lib.check(L.bdbnn_binconv_fwd_tc(_p(xh), _p(wpack.wf), FMT_FP16, _p(alpha), _p(y), ctypes.byref(sh),
-                                              _p(sums), _p(ymax), st), "binconv_fwd_tc(real)")
-        _lib.count(1)
+def _real_unit_fwd(x, x_amax, op, wpack, w_shape, gamma, beta, residual, running_mean, running_var, momentum, eps,
+                   stride, padding, relu=True):
+    """Forward of one real-valued conv + BatchNorm(train) (+ residual) (+ ReLU) unit:
+    real_act_pack(x, x_amax) -> real_scale_fold -> binconv_fwd_tc (fp16 operands, BatchNorm statistics in the
+    epilogue) -> bn_fwd_relu (z, ReLU's mask words, max|z|), or without `relu` bn_fwd (z only; no residual).
+    op: (xh, amax), x's fp16 operand and the amax word it was scaled by when another unit already made it, else None.
+    Returns (z, z_amax or None, the tensors the backward reads, the conv's shape)."""
+    L = _lib.lib()
+    sh = conv_shape(x.shape, w_shape, stride, padding)
+    if not real_unit_supported(x.shape, w_shape, stride, padding, REAL_MAX_COUT):
+        raise RuntimeError(f"bdbnn_b200.real_conv_bn_relu: no kernel for input {tuple(x.shape)}, weight "
+                           f"{tuple(w_shape)}, stride {stride}, padding {padding}")
+    z_shape = (sh.N, sh.Cout, sh.Ho, sh.Wo)
+    if residual is not None and tuple(residual.shape) != z_shape:
+        raise RuntimeError(f"real_conv_bn_relu: residual shape {tuple(residual.shape)} != output shape {z_shape}")
+    dev = x.device
+    st = _stream()
+    key = _shape_key(sh)
+    cout, n_pix = sh.Cout, sh.N * sh.Ho * sh.Wo
+    xh, amax = op if op is not None else _real_act_pack(x, x_amax, sh)[1:]
+    alpha, inv_gscale = _real_scale_fold(amax, wpack)
+    f32 = dict(dtype=torch.float32, device=dev)
+    y = torch.empty(z_shape, memory_format=torch.channels_last, **f32)
+    sums = torch.empty((2 * cout,), dtype=torch.float64, device=dev)
+    ymax = torch.empty((cout,), dtype=torch.int32, device=dev)
+    with _timed("real_conv_fwd_tc", key, algorithmic_bytes("fwd_tc", sh)):
+        _lib.check(L.bdbnn_binconv_fwd_tc(_p(xh), _p(wpack.wf), FMT_FP16, _p(alpha), _p(y), ctypes.byref(sh),
+                                          _p(sums), _p(ymax), st), "binconv_fwd_tc(real)")
+    _lib.count(1)
+    z = torch.empty_like(y)
+    mean, invstd, ab = torch.empty((cout,), **f32), torch.empty((cout,), **f32), torch.empty((2 * cout,), **f32)
+    mask = z_amax = None
+    if relu:
         rc = _nhwc(residual.detach()) if residual is not None else None
-        z = torch.empty_like(y)
-        mean, invstd, ab = torch.empty((cout,), **f32), torch.empty((cout,), **f32), torch.empty((2 * cout,), **f32)
         mask = torch.empty((sh.N, sh.Ho, sh.Wo, cout // 32), dtype=torch.int32, device=dev)
         z_amax = torch.empty((1,), dtype=torch.int32, device=dev)
         with _timed("real_bn_fwd_relu", key, (8 + (4 if rc is not None else 0) + 0.125) * n_pix * cout):
@@ -2566,31 +2565,35 @@ class _RealConvBNReLU(torch.autograd.Function):
                                            float(eps), float(momentum), _p(running_mean), _p(running_var), _p(sums),
                                            _p(ymax), _p(mean), _p(invstd), _p(ab), _p(z), _p(mask), _p(z_amax), 1, st),
                        "bn_fwd_relu")
-        _lib.count(2)
-        ctx.sh = sh
-        ctx.x_shape, ctx.w_shape = tuple(x.shape), tuple(weight.shape)
-        ctx.w_param = weight if (weight.is_leaf and weight.requires_grad) else None
-        ctx.has_res = residual is not None
-        ctx.save_for_backward(y, mean, invstd, gamma.detach(), ymax, mask, xh, wpack.wt, wpack.wmask, wpack.gscale,
-                              inv_gscale)
-        ctx.mark_non_differentiable(z_amax)
-        return z, z_amax
+    else:
+        if residual is not None:
+            raise RuntimeError("real_conv_bn: the unit without ReLU takes no residual")
+        with _timed("real_bn_fwd", key, 8 * n_pix * cout):
+            _lib.check(L.bdbnn_bn_fwd(_p(y), None, _p(gamma.detach()), _p(beta.detach()), n_pix, cout, float(eps),
+                                      float(momentum), _p(running_mean), _p(running_var), _p(sums), _p(ymax),
+                                      _p(mean), _p(invstd), _p(ab), _p(z), None, None, None, None, 0, 1, st),
+                       "bn_fwd(real)")
+    _lib.count(2)
+    saved = (y, mean, invstd, gamma.detach(), ymax, mask, xh, wpack.wt, wpack.wmask, wpack.gscale, inv_gscale)
+    return z, z_amax, saved, sh
 
-    @staticmethod
-    @_on_device
-    def backward(ctx, gz, _g_amax):
-        if gz is None:
-            return (None,) * 12
-        L = _lib.lib()
-        sh = ctx.sh
-        dev = gz.device
-        y, mean, invstd, gamma, ymax, mask, xh, wt, wmask, gscale, inv_gscale = ctx.saved_tensors
-        key = _shape_key(sh)
-        g = _nhwc(gz)
-        cout, n_pix = sh.Cout, sh.N * sh.Ho * sh.Wo
-        sums, gmax, consts, dgamma, dbeta, amax, gys = _bn_grads(cout, (sh.N, sh.Ho, sh.Wo), 1, dev)
-        gres = None
-        if ctx.has_res and ctx.needs_input_grad[4]:
+
+def _real_unit_bwd(gz, saved, sh, x_shape, w_shape, w_param, need_x, need_w, need_res, relu=True, add=None,
+                   out=None):
+    """Backward of _real_unit_fwd: bn_bwd_pack_relu (gz masked, which is also the residual's gradient), or without
+    `relu` bn_bwd_pack -> wgrad_tc, dgrad_tc with all-ones STE masks.  add: an fp32 NHWC tensor of x's shape that
+    dgrad's epilogue adds into gx; out: the tensor gx is written to (may be `add`), else a fresh one.
+    Returns (gx, gw, dgamma, dbeta, gres)."""
+    L = _lib.lib()
+    y, mean, invstd, gamma, ymax, mask, xh, wt, wmask, gscale, inv_gscale = saved
+    dev = gz.device
+    key = _shape_key(sh)
+    g = _nhwc(gz)
+    cout, n_pix = sh.Cout, sh.N * sh.Ho * sh.Wo
+    sums, gmax, consts, dgamma, dbeta, amax, gys = _bn_grads(cout, (sh.N, sh.Ho, sh.Wo), 1, dev)
+    gres = None
+    if relu:
+        if need_res:
             gres = torch.empty((sh.N, cout, sh.Ho, sh.Wo), dtype=torch.float32, device=dev,
                                memory_format=torch.channels_last)
         with _timed("real_bn_bwd_pack_relu", key, (16 + 2 + 0.25 + (4 if gres is not None else 0)) * n_pix * cout):
@@ -2598,29 +2601,159 @@ class _RealConvBNReLU(torch.autograd.Function):
                                                 _p(ymax), n_pix, cout, GRAD_MODES["fp16s"], _p(sums), _p(gmax),
                                                 _p(consts), _p(dgamma), _p(dbeta), _p(amax), _p(gys), _p(gres),
                                                 _stream()), "bn_bwd_pack_relu")
-        _lib.count(3)
-        gx = gw = None
-        # the weight gradient first: in a wgrad_side scope it forks off here and overlaps the dgrad
-        if ctx.needs_input_grad[1]:
-            gw = _wgrad_tc(sh, gys, GRAD_MODES["fp16s"], amax, xh, wmask, inv_gscale, ctx.w_shape, ctx.w_param,
-                           "real_conv_wgrad_tc", key, algorithmic_bytes("wgrad_tc", sh))
-        if ctx.needs_input_grad[0]:
-            ones = torch.full((sh.N, sh.H, sh.W, (sh.Cin + 31) // 32), -1, dtype=torch.int32, device=dev)
-            gx = torch.empty(ctx.x_shape, dtype=torch.float32, device=dev, memory_format=torch.channels_last)
-            _dgrad_tc(sh, gys, GRAD_MODES["fp16s"], amax, wt, ones, None, gx, "real_conv_dgrad_tc",
-                      algorithmic_bytes("dgrad_tc", sh))
-        return (gx, gw, dgamma if ctx.needs_input_grad[2] else None, dbeta if ctx.needs_input_grad[3] else None, gres,
-                None, None, None, None, None, None, None)
+    else:
+        with _timed("real_bn_bwd_pack", key, 18 * n_pix * cout):
+            _lib.check(L.bdbnn_bn_bwd_pack(_p(g), _p(y), _p(mean), _p(invstd), _p(gamma), _p(gscale), _p(ymax), n_pix,
+                                           cout, GRAD_MODES["fp16s"], _p(sums), _p(gmax), _p(consts), _p(dgamma),
+                                           _p(dbeta), _p(amax), _p(gys), _stream()), "bn_bwd_pack(real)")
+    _lib.count(3)
+    gx = gw = None
+    # the weight gradient first: in a wgrad_side scope it forks off here and overlaps the dgrad
+    if need_w:
+        gw = _wgrad_tc(sh, gys, GRAD_MODES["fp16s"], amax, xh, wmask, inv_gscale, w_shape, w_param,
+                       "real_conv_wgrad_tc", key, algorithmic_bytes("wgrad_tc", sh))
+    if need_x:
+        ones = torch.full((sh.N, sh.H, sh.W, (sh.Cin + 31) // 32), -1, dtype=torch.int32, device=dev)
+        gx = out if out is not None else torch.empty(x_shape, dtype=torch.float32, device=dev,
+                                                     memory_format=torch.channels_last)
+        _dgrad_tc(sh, gys, GRAD_MODES["fp16s"], amax, wt, ones, add, gx, "real_conv_dgrad_tc",
+                  algorithmic_bytes("dgrad_tc", sh) + (4 * gx.numel() if add is not None else 0))
+    return gx, gw, dgamma, dbeta, gres
+
+
+class _RealConvBNReLU(torch.autograd.Function):
+    """z = relu(BN_train(conv2d(x, W, stride, padding)) + residual) of a real-valued 3x3 (padding 1) or 1x1
+    (padding 0) conv (DESIGN.md §4r, §4s): _real_unit_fwd and _real_unit_bwd as one autograd node."""
+
+    @staticmethod
+    @_on_device
+    def forward(ctx, x, weight, gamma, beta, residual, x_amax, wpack, running_mean, running_var, momentum, eps, stride,
+                padding=1):
+        _require_cuda(x, "real_conv_bn_relu(x)")
+        _same_device(x, weight, gamma, beta, residual, x_amax, running_mean, running_var)
+        _require_fp16s("real_conv_bn_relu")
+        ctx.set_materialize_grads(False)
+        z, z_amax, saved, ctx.sh = _real_unit_fwd(x, x_amax, None, wpack, tuple(weight.shape), gamma, beta, residual,
+                                                  running_mean, running_var, momentum, eps, stride, padding)
+        ctx.x_shape, ctx.w_shape = tuple(x.shape), tuple(weight.shape)
+        ctx.w_param = weight if (weight.is_leaf and weight.requires_grad) else None
+        ctx.has_res = residual is not None
+        ctx.save_for_backward(*saved)
+        ctx.mark_non_differentiable(z_amax)
+        return z, z_amax
+
+    @staticmethod
+    @_on_device
+    def backward(ctx, gz, _g_amax):
+        if gz is None:
+            return (None,) * 13
+        need = ctx.needs_input_grad
+        gx, gw, dgamma, dbeta, gres = _real_unit_bwd(gz, ctx.saved_tensors, ctx.sh, ctx.x_shape, ctx.w_shape,
+                                                     ctx.w_param, need[0], need[1], ctx.has_res and need[4])
+        return (gx, gw, dgamma if need[2] else None, dbeta if need[3] else None, gres,
+                None, None, None, None, None, None, None, None)
 
 
 def real_conv_bn_relu(x, x_amax, wpack, weight, gamma, beta, running_mean, running_var, momentum, eps, stride,
-                      residual=None):
-    """z = relu(BN_train(conv2d(x, weight, stride, padding 1)) + residual) of a real-valued 3x3 conv on the wgmma
-    kernels, with autograd (DESIGN.md §4r; geometry: real_unit_supported; gradient mode fp16s).  wpack: weight's
-    _WeightPack from real_weight_grad_pack; x_amax: the max|x| word the call that wrote x returned (None: computed
-    here).  Returns (z fp32 channels_last, z_amax int32[1] = bits of max|z|, for the next unit's x_amax)."""
+                      residual=None, padding=1):
+    """z = relu(BN_train(conv2d(x, weight, stride, padding)) + residual) of a real-valued conv on the wgmma kernels,
+    with autograd (DESIGN.md §4r; 3x3 / padding 1, or 1x1 / padding 0 as in §4s; geometry:
+    real_unit_supported(..., max_cout=REAL_MAX_COUT); gradient mode fp16s).  wpack: weight's _WeightPack from
+    real_weight_grad_pack; x_amax: the max|x| word the call that wrote x returned (None: computed here).  Returns
+    (z fp32 channels_last, z_amax int32[1] = bits of max|z|, for the next unit's x_amax)."""
     return _RealConvBNReLU.apply(x, weight, gamma, beta, residual, x_amax, wpack, running_mean, running_var,
-                                 float(momentum), float(eps), int(stride))
+                                 float(momentum), float(eps), int(stride), int(padding))
+
+
+class _RealBottleneck(torch.autograd.Function):
+    """One torchvision Bottleneck block in training mode as ONE autograd node (DESIGN.md §4s):
+
+        xh = real_act_pack(x)                         x's fp16 operand, read by conv1 and the downsample
+        r  = x, or BN_ds(conv_ds 1x1 / stride s (x))  no ReLU
+        y1 = relu(BN1(conv1 1x1 (x)))
+        y2 = relu(BN2(conv2 3x3 / stride s (y1)))
+        z  = relu(BN3(conv3 1x1 (y2)) + r)
+
+    x reaches two convs (or a conv and the identity path) inside this node, so autograd never holds two gradients of
+    x to sum: conv3's masked gradient gres is the identity path's gradient and conv1's dgrad epilogue adds it in place
+    (add = out = gres); with a downsample, gres is its BatchNorm's incoming gradient and its dgrad adds into conv1's gx.
+    params: w1, gamma1, beta1, w2, gamma2, beta2, w3, gamma3, beta3 [, w_ds, gamma_ds, beta_ds]; packs: their weights'
+    _WeightPacks; bn_state: (running_mean, running_var, momentum, eps) of each BatchNorm in the same order."""
+
+    @staticmethod
+    @_on_device
+    def forward(ctx, x, x_amax, packs, bn_state, stride, *params):
+        _require_cuda(x, "real_bottleneck(x)")
+        _same_device(x, x_amax, *params)
+        _require_fp16s("real_bottleneck")
+        ctx.set_materialize_grads(False)
+        ws = params[0::3]
+        has_ds = len(ws) == 4
+        sh1 = conv_shape(x.shape, ws[0].shape, 1, 0)
+        _, xh, amax = _real_act_pack(x, x_amax, sh1)
+        units = [((x, None, (xh, amax)), 1, 0), (None, stride, 1), (None, 1, 0)] + (
+            [((x, None, (xh, amax)), stride, 0)] if has_ds else [])
+        saved, geoms = [None] * len(ws), [None] * len(ws)
+
+        def unit(i, inp, residual=None, relu=True):
+            z, za, saved[i], sh = _real_unit_fwd(*inp, packs[i], tuple(ws[i].shape), params[3 * i + 1],
+                                                 params[3 * i + 2], residual, *bn_state[i], units[i][1], units[i][2],
+                                                 relu=relu)
+            geoms[i] = sh
+            return z, za
+
+        r = unit(3, units[3][0], relu=False)[0] if has_ds else x.detach()
+        y1, a1 = unit(0, units[0][0])
+        y2, a2 = unit(1, (y1, a1, None))
+        z, z_amax = unit(2, (y2, a2, None), residual=r)
+        ctx.geoms, ctx.has_ds, ctx.x_shape = geoms, has_ds, tuple(x.shape)
+        ctx.w_shapes = [tuple(w.shape) for w in ws]
+        ctx.w_params = [w if (w.is_leaf and w.requires_grad) else None for w in ws]
+        ctx.in_shapes = [tuple(x.shape), tuple(y1.shape), tuple(y2.shape), tuple(x.shape)]
+        ctx.save_for_backward(*[t for s in saved for t in s])
+        ctx.mark_non_differentiable(z_amax)
+        return z, z_amax
+
+    @staticmethod
+    @_on_device
+    def backward(ctx, gz, _g_amax):
+        n_params = 3 * len(ctx.w_shapes)
+        if gz is None:
+            return (None,) * (5 + n_params)
+        need = ctx.needs_input_grad
+        need_x = need[0]
+        st = ctx.saved_tensors
+        saved = [st[11 * i:11 * i + 11] for i in range(len(ctx.w_shapes))]
+
+        def unit(i, g, need_in, need_res=False, relu=True, add=None, out=None):
+            return _real_unit_bwd(g, saved[i], ctx.geoms[i], ctx.in_shapes[i], ctx.w_shapes[i], ctx.w_params[i],
+                                  need_in, need[5 + 3 * i], need_res, relu=relu, add=add, out=out)
+
+        grads = [None] * len(ctx.w_shapes)
+        g2, *grads[2], gres = unit(2, gz, True, need_res=need_x or ctx.has_ds)
+        g1, *grads[1], _ = unit(1, g2, True)
+        if ctx.has_ds:
+            gx, *grads[0], _ = unit(0, g1, need_x)
+            _, *grads[3], _ = unit(3, gres, need_x, relu=False, add=gx, out=gx)
+        else:
+            gx, *grads[0], _ = unit(0, g1, need_x, add=gres, out=gres)
+        out = [gx if need_x else None, None, None, None, None]
+        for i, (gw, dgamma, dbeta) in enumerate(grads):
+            out += [gw, dgamma if need[6 + 3 * i] else None, dbeta if need[7 + 3 * i] else None]
+        return tuple(out)
+
+
+def real_bottleneck(x, x_amax, packs, params, bn_state, stride):
+    """z = relu(BN3(conv3(relu(BN2(conv2(relu(BN1(conv1(x)))))))) + shortcut(x)) of a torchvision Bottleneck block in
+    training mode on the wgmma kernels, with autograd (DESIGN.md §4s; geometry: real_unit_supported(...,
+    max_cout=REAL_MAX_COUT) for every conv; gradient mode fp16s).  params: [w1, gamma1, beta1, w2, gamma2, beta2, w3,
+    gamma3, beta3] and, with a downsample, [w_ds, gamma_ds, beta_ds] after them; packs: the weights' _WeightPacks from
+    real_weight_grad_pack, in the same order; bn_state: (running_mean, running_var, momentum, eps) per BatchNorm, in
+    the same order; stride: conv2's and the downsample's.  Returns (z fp32 channels_last, z_amax int32[1])."""
+    if len(params) not in (9, 12) or len(packs) != len(params) // 3 or len(bn_state) != len(packs):
+        raise RuntimeError("bdbnn_b200.real_bottleneck: expects 3 or 4 convs with their packs and BatchNorm states")
+    return _RealBottleneck.apply(x, x_amax, list(packs),
+                                 [(rm, rv, float(m), float(e)) for rm, rv, m, e in bn_state], int(stride), *params)
 
 
 def stem_conv_bn_relu_pool(x, weight, gamma, beta, running_mean, running_var, momentum, eps, kernel_size, stride,

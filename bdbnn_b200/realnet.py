@@ -1,6 +1,7 @@
-"""Training torchvision's fp32 ResNet-18/34 on this repository's kernels (DESIGN.md §4r).
+"""Training torchvision's fp32 ResNets on this repository's kernels (DESIGN.md §4r, §4s).
 
-    model = RealResNet(torchvision.models.resnet18())      # or resnet34
+    model = RealResNet(torchvision.models.resnet18())                # or resnet34
+    model = RealBottleneckResNet(torchvision.models.resnet50())      # or resnet101/152, wide_resnet50_2/101_2
 
 wraps the model without copying it, as FrozenResNetTeacher does: the wrapper's children ARE the model's children, so
 `named_parameters()` and `state_dict()` have the model's names and objects, and `load_state_dict`, `.cuda()` and
@@ -14,13 +15,15 @@ In training mode, on a CUDA fp32 input whose geometry every unit takes, the forw
     z  = relu(BN2_train(conv2(z1)) + r)                     real_conv_bn_relu(residual=r)
     logits = fc(flatten(avgpool(z)))                        torch
 
-In eval mode under no_grad it is FrozenResNetTeacher's eval kernel forward.  Anything else (CPU, other dtypes,
-unsupported geometry, BDBNN_FUSE_BN=0, a gradient mode other than fp16s, eval mode with autograd) returns the wrapped
-model's own forward."""
+and each Bottleneck block of RealBottleneckResNet as one real_bottleneck node (its 1x1, 3x3 and 1x1 units and the
+downsample).  In eval mode under no_grad it is FrozenResNetTeacher's (FrozenBottleneckTeacher's) eval kernel forward.
+Anything else (CPU, other dtypes, unsupported geometry, BDBNN_FUSE_BN=0, a gradient mode other than fp16s, eval mode
+with autograd) returns the wrapped model's own forward."""
 import torch
+import torch.nn as nn
 
 from . import functional as F_
-from .teacher import FrozenResNetTeacher, _family
+from .teacher import FrozenBottleneckTeacher, FrozenResNetTeacher, _family
 
 
 def _bn_train_args(bn):
@@ -38,7 +41,8 @@ class RealResNet(FrozenResNetTeacher):
             raise TypeError(f"RealResNet wraps a torchvision ResNet with BasicBlocks (resnet18/34), got "
                             f"{type(model).__name__}")
         if _family(model).bottleneck:
-            raise TypeError("RealResNet wraps torchvision BasicBlock ResNets (resnet18/34); layer1.0 is a Bottleneck")
+            raise TypeError("RealResNet wraps torchvision BasicBlock ResNets (resnet18/34); layer1.0 is a Bottleneck: "
+                            "wrap a Bottleneck ResNet in RealBottleneckResNet")
         try:
             super().__init__(model)
         except TypeError as e:      # the teacher's structure check: name the class the caller used
@@ -121,5 +125,71 @@ class RealResNet(FrozenResNetTeacher):
                                              blk.conv1.stride[0])
             z, z_amax = F_.real_conv_bn_relu(y, y_amax, packs[2 * i + 1], blk.conv2.weight, *_bn_train_args(blk.bn2),
                                              1, residual=res)
+        torch._foreach_add_([bn.num_batches_tracked for bn in self._bns()], 1)
+        return self.fc(torch.flatten(self.avgpool(z), 1))
+
+
+class RealBottleneckResNet(RealResNet, FrozenBottleneckTeacher):
+    """A torchvision Bottleneck ResNet (exactly torchvision's ResNet with Bottleneck blocks, groups 1, no dilation:
+    resnet50/101/152, wide_resnet50_2/101_2) trained on the real-valued training units (DESIGN.md §4s), with
+    RealResNet's kernel-path conditions and fallback and FrozenBottleneckTeacher's structure check and eval forward.
+    Raises TypeError for any other structure (BasicBlock ResNets, ResNeXt, replace_stride_with_dilation, subclassed
+    models or blocks, mixed blocks, nn.DataParallel), naming the module."""
+
+    def __init__(self, model):
+        from torchvision.models import resnet as tv
+        who = "RealBottleneckResNet"
+        if type(model) is not tv.ResNet:
+            raise TypeError(f"{who} wraps a torchvision ResNet with Bottlenecks (resnet50/101/152, "
+                            f"wide_resnet50_2/101_2), got {type(model).__name__}")
+        layer1 = getattr(model, "layer1", None)
+        first = layer1[0] if type(layer1) is nn.Sequential and len(layer1) > 0 else None
+        if type(first) is not tv.Bottleneck:
+            hint = ": wrap a BasicBlock ResNet in RealResNet" if type(first) is tv.BasicBlock else ""
+            raise TypeError(f"{who} wraps torchvision Bottleneck ResNets (resnet50/101/152, wide_resnet50_2/101_2); "
+                            f"layer1.0 is a {type(first).__name__}{hint}")
+        try:
+            FrozenBottleneckTeacher.__init__(self, model)
+        except TypeError as e:      # the teacher's structure check: name the class the caller used
+            raise TypeError(str(e).replace("FrozenResNetTeacher", who)) from None
+        self.__dict__["_train_ok"] = {}
+
+    def _walk_train_geometry(self, x):
+        """Every conv has its training unit at this input size (up to F_.REAL_MAX_COUT output channels), and each
+        block's shortcut has its output's shape (host-only)."""
+        n, _, h, w = x.shape
+        ho, wo = (h - 1) // 2 + 1, (w - 1) // 2 + 1
+        shape = (n, self.conv1.out_channels, (ho - 1) // 2 + 1, (wo - 1) // 2 + 1)
+
+        def unit(x_shape, conv):
+            s, p = conv.stride[0], conv.padding[0]
+            if not F_.real_unit_supported(x_shape, tuple(conv.weight.shape), s, p, F_.REAL_MAX_COUT):
+                return None
+            sh = F_.conv_shape(x_shape, conv.weight.shape, s, p)
+            return (n, sh.Cout, sh.Ho, sh.Wo)
+
+        for blk in self._blocks:
+            x_shape = shape
+            for conv in (blk.conv1, blk.conv2, blk.conv3):
+                shape = unit(shape, conv)
+                if shape is None:
+                    return False
+            r_shape = x_shape if blk.downsample is None else unit(x_shape, blk.downsample[0])
+            if r_shape != shape:
+                return False
+        return True
+
+    def _train_forward(self, x):
+        # (conv, BatchNorm) pairs of each block: conv1, conv2, conv3 and the downsample's
+        units = [[(blk.conv1, blk.bn1), (blk.conv2, blk.bn2), (blk.conv3, blk.bn3)] +
+                 ([tuple(blk.downsample)] if blk.downsample is not None else []) for blk in self._blocks]
+        # 1x1 and 3x3 weights in one pack per forward, never cached: the optimizers update them in place
+        packs = iter(F_.real_weight_grad_pack([c.weight for u in units for c, _ in u]))
+        c1 = self.conv1
+        z, z_amax = F_.stem_conv_bn_relu_pool(x, c1.weight, *_bn_train_args(self.bn1), *self._pool_args())
+        for blk, u in zip(self._blocks, units):
+            params = [t for c, bn in u for t in (c.weight, bn.weight, bn.bias)]
+            z, z_amax = F_.real_bottleneck(z, z_amax, [next(packs) for _ in u], params,
+                                           [_bn_train_args(bn)[2:] for _, bn in u], blk.conv2.stride[0])
         torch._foreach_add_([bn.num_batches_tracked for bn in self._bns()], 1)
         return self.fc(torch.flatten(self.avgpool(z), 1))

@@ -1,17 +1,18 @@
-"""Throughput of the fp32 ResNet-18/34 training step on this repository's kernels (RealResNet, DESIGN.md §4r):
-CE + kurtosis (avg over the hooked convs), Adam, batch 256, 224x224, channels_last.
+"""Throughput of the fp32 torchvision ResNet training step on this repository's kernels (RealResNet, DESIGN.md §4r;
+RealBottleneckResNet, §4s): CE + kurtosis (avg over the hooked convs), Adam, batch 256, 224x224, channels_last.
 
     python tools/real_resnet_throughput.py [--batch 256] [--steps 20] [--warmup 5] [--rounds 3] [--nets resnet18,resnet34]
+    python tools/real_resnet_throughput.py --nets resnet50,wide_resnet50_2
 
 Arms:
-    kernels       RealResNet(torchvision model), the step captured by GraphedTrainStep
+    kernels       RealResNet / RealBottleneckResNet(torchvision model), the step captured by GraphedTrainStep
     fuse_off      the same with BDBNN_FUSE_BN=0: the torchvision model's own forward (cuDNN, ATen), graphed
     cudnn         the torchvision model in plain TrainStep, eager, TF32 defaults
     cudnn_bench   the same with torch.backends.cudnn.benchmark = True (the reference's train.py:368)
 Every (arm, net) pair runs in a fresh process of its own; the arms alternate within each of --rounds rounds.
 Images/s = batch * steps / (CUDA-event time of the timed steps).  The kernels arm also prints its per-family kernel
-times (KernelTimer, one eager step).  The card name and power limit are read (read-only) from nvidia-smi in the same
-run.  Needs a CUDA device."""
+times (KernelTimer, one eager step); every arm prints its peak torch.cuda.max_memory_allocated.  The card name and
+power limit are read (read-only) from nvidia-smi in the same run.  Needs a CUDA device."""
 import argparse
 import json
 import os
@@ -22,13 +23,14 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 ARMS = ("kernels", "fuse_off", "cudnn", "cudnn_bench")
-NETS = ("resnet18", "resnet34")
+NETS = ("resnet18", "resnet34")                                      # the default --nets
+BOTTLENECK_NETS = ("resnet50", "resnet101", "resnet152", "wide_resnet50_2", "wide_resnet101_2")
 
 
 def _child(arm, net, batch, steps, warmup):
     import torch
     import torchvision
-    from bdbnn_b200 import RealResNet
+    from bdbnn_b200 import RealBottleneckResNet, RealResNet
     from bdbnn_b200.functional import KernelTimer
     from bdbnn_b200.step import GraphedTrainStep, StepConfig, TrainStep, make_optimizer
     if not torch.cuda.is_available():
@@ -37,7 +39,7 @@ def _child(arm, net, batch, steps, warmup):
     torch.manual_seed(0)
     model = getattr(torchvision.models, net)().cuda().to(memory_format=torch.channels_last)
     if arm in ("kernels", "fuse_off"):
-        model = RealResNet(model)
+        model = (RealBottleneckResNet if net in BOTTLENECK_NETS else RealResNet)(model)
     model.train()
     cfg = StepConfig(w_kurtosis=True)
     eager = TrainStep(model, make_optimizer(model, "imagenet", lr=1e-4), cfg)
@@ -55,7 +57,8 @@ def _child(arm, net, batch, steps, warmup):
     e1.record()
     e1.synchronize()
     ms = e0.elapsed_time(e1) / steps
-    rec = {"arm": arm, "net": net, "ms_per_step": ms, "img_per_s": batch * 1e3 / ms, "loss": float(out["loss"])}
+    rec = {"arm": arm, "net": net, "ms_per_step": ms, "img_per_s": batch * 1e3 / ms, "loss": float(out["loss"]),
+           "max_memory_allocated_gib": round(torch.cuda.max_memory_allocated() / 2 ** 30, 2)}
     if arm == "kernels":
         KernelTimer.start()
         eager(x, y)
@@ -81,14 +84,18 @@ def main():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--rounds", type=int, default=3)
-    ap.add_argument("--nets", default=",".join(NETS), help="comma-separated subset of " + ",".join(NETS))
+    ap.add_argument("--nets", default=",".join(NETS),
+                    help="comma-separated subset of " + ",".join(NETS + BOTTLENECK_NETS))
     ap.add_argument("--child", nargs=2, metavar=("ARM", "NET"))
     a = ap.parse_args()
     if a.child:
         _child(a.child[0], a.child[1], a.batch, a.steps, a.warmup)
         return
+    bad = [n for n in a.nets.split(",") if n not in NETS + BOTTLENECK_NETS]
+    if bad:
+        ap.error(f"unknown nets {bad}")
     print(json.dumps({"card": _card()}), flush=True)
-    results = {}
+    results, peak = {}, {}
     for r in range(a.rounds):
         for net in a.nets.split(","):
             for arm in ARMS:
@@ -106,7 +113,9 @@ def main():
                 rec["round"] = r
                 print(json.dumps(rec), flush=True)
                 results.setdefault(f"{net}/{arm}", []).append(rec["img_per_s"])
-    print(json.dumps({"card": _card(), "img_per_s": {k: [round(v) for v in vs] for k, vs in results.items()}}))
+                peak[f"{net}/{arm}"] = max(peak.get(f"{net}/{arm}", 0.0), rec["max_memory_allocated_gib"])
+    print(json.dumps({"card": _card(), "img_per_s": {k: [round(v) for v in vs] for k, vs in results.items()},
+                      "max_memory_allocated_gib": peak}))
 
 
 if __name__ == "__main__":
