@@ -4,11 +4,11 @@ from .modules import BinarizeConv2d, BinaryActivationConv2d, HardBinaryConv, Har
 from .losses import (KurtosisWeight, DistributionLoss, DistributionLoss_layer,
                      kurtosis_regularization, matched_weight_pairs)
 from .functional import binact_conv2d, binconv2d, kurtosis_multi, kd_logits_loss, kd_layer_loss
-from .teacher import FrozenBottleneckTeacher, FrozenResNetTeacher, FrozenVGGTeacher
-from .realnet import RealBottleneckResNet, RealResNet
+from .teacher import FrozenBottleneckTeacher, FrozenResNetTeacher, FrozenResNeXtTeacher, FrozenVGGTeacher
+from .realnet import RealBottleneckResNet, RealResNet, RealResNeXt
 
 __all__ = ["BinarizeConv2d", "BinaryActivationConv2d", "HardBinaryConv", "HardBinaryConv_react", "HardBinaryConv_cifar",
            "KurtosisWeight", "DistributionLoss", "DistributionLoss_layer", "kurtosis_regularization",
            "matched_weight_pairs", "binact_conv2d", "binconv2d", "kurtosis_multi", "kd_logits_loss", "kd_layer_loss",
-           "FrozenBottleneckTeacher", "FrozenResNetTeacher", "FrozenVGGTeacher", "RealBottleneckResNet",
-           "RealResNet"]
+           "FrozenBottleneckTeacher", "FrozenResNetTeacher", "FrozenResNeXtTeacher", "FrozenVGGTeacher",
+           "RealBottleneckResNet", "RealResNet", "RealResNeXt"]

@@ -86,6 +86,13 @@ SIGNATURES = {
     "bdbnn_real_conv_fwd_eval": (c_int, [_P] * 6 + [c_int, _P, _P, _SH, _P]),
     "bdbnn_real_gemm1x1_fwd_eval": (c_int, [_P] * 6 + [c_int, _P, _P, _SH, _P]),
     "bdbnn_real_gemm1x1_supported": (c_int, [_SH]),
+    "bdbnn_real_gconv_supported": (c_int, [_SH, c_int]),
+    "bdbnn_real_gconv_fwd": (c_int, [_P, _P, _P, _P, _SH, c_int, _P, _P, _P]),
+    "bdbnn_real_gconv_fwd_eval": (c_int, [_P] * 6 + [c_int, _P, _P, _SH, c_int, _P]),
+    "bdbnn_real_gconv_dgrad": (c_int, [_P] * 6 + [_SH, c_int, _P]),
+    "bdbnn_real_gconv_wgrad_workspace_bytes": (c_size_t, [_SH, c_int]),
+    "bdbnn_real_gconv_wgrad": (c_int, [_P] * 6 + [_SH, c_int, _P, c_size_t, _P]),
+    "bdbnn_real_weight_pack_multi_grouped": (c_int, [c_int] + [_P] * 12 + [_P]),
     "bdbnn_bn_fwd_pad_shortcut": (c_int, [_P, _P] + [c_int] * 5 + [_P, _P, c_int, ctypes.c_float, ctypes.c_float] +
                                   [_P] * 12 + [c_int, c_int, _P]),
     "bdbnn_bn_fwd_i16_pad_shortcut": (c_int, [_P, _P, _P] + [c_int] * 5 + [_P, _P, c_int, ctypes.c_float,

@@ -13,6 +13,8 @@
 //             bdbnn_binconv_wgrad_tc(gys, xh, all-ones mask)        inv_gscale[o] = 2^ew * 2^-ex
 #include <cuda_fp16.h>
 
+#include <vector>
+
 #include "common.cuh"
 
 namespace bdbnn {
@@ -209,6 +211,73 @@ __global__ void real_scale_fold_kernel(const uint32_t* __restrict__ x_amax_bits,
   inv_gscale[o] = inv_gscale_w[o] * isx;
 }
 
+// Grouped 3x3 weights (DESIGN.md §4t): the banded operands of bdbnn_real_weight_pack_multi_grouped.  Tensor l has
+// band B[l] and Cin[l] = Cg channels per group (the weight's second dimension); its wf and wt both have Cout*T*B
+// entries, blk0 counts their blocks.
+struct RealGroupTable {
+  int32_t B[kRealPackMax];
+  int32_t blk0[kRealPackMax + 1];
+};
+
+__device__ __forceinline__ int real_group_find(const RealGroupTable& gt, int n, int b) {
+  int l = 0;
+  while (l + 1 < n && b >= gt.blk0[l + 1]) ++l;
+  return l;
+}
+
+// wf[o][t][cl] = fp16(W[o][c - g(o)][t] * 2^ew) for c = b(o) + cl in o's group, else +0 (b, g: o's band and group
+// starts); alpha[o] = 2^-ew.  Coalesced along the output.
+__global__ void __launch_bounds__(256)
+real_gwpack_multi_kernel(const __grid_constant__ RealWPackTable tab, const __grid_constant__ RealGroupTable gt,
+                         const uint32_t* __restrict__ amax) {
+  const int l = real_group_find(gt, tab.n, int(blockIdx.x));
+  const int Cg = tab.Cin[l], T = tab.T[l], KW = tab.KW[l], B = gt.B[l], n = tab.Cout[l] * T * B;
+  const int sO = tab.sO[l], sC = tab.sC[l], sR = tab.sR[l], sS = tab.sS[l];
+  const int base = (int(blockIdx.x) - gt.blk0[l]) * kRealPackPerBlock;
+  const int end = base + kRealPackPerBlock < n ? base + kRealPackPerBlock : n;
+  const uint32_t a = __ldg(amax + l);
+  const float sw = amax_pow2_scale(a, false), isw = amax_pow2_scale(a, true);
+  const float* W = tab.W[l];
+  __half* wf = reinterpret_cast<__half*>(tab.wf[l]);
+  for (int j = base + threadIdx.x; j < end; j += blockDim.x) {
+    const int cl = j % B, q = j / B;
+    const int t = q % T, o = q / T;
+    const int cg = (o - o % B) + cl - (o - o % Cg);
+    const int r = t / KW, sx = t - r * KW;
+    __half v = __float2half_rn(0.f);
+    if (cg >= 0 && cg < Cg)
+      v = __float2half_rn(__ldg(W + int64_t(o) * sO + int64_t(cg) * sC + int64_t(r) * sR + int64_t(sx) * sS) * sw);
+    wf[j] = v;
+    if (cl == 0 && t == 0) tab.alpha[l][o] = isw;
+  }
+}
+
+// wt[c][T-1-t][ol] = wf[b(c) + ol][t][c - b(c)] (wf's bits: the band's transpose, taps flipped); gscale[c] = 2^-ew,
+// inv_gscale[c] = 2^ew (Cin = Cout).  Coalesced along the output; wf is read in 2-byte gathers (a band operand is at
+// most C * 9 * 64 * 2 bytes).
+__global__ void __launch_bounds__(256)
+real_gwt_multi_kernel(const __grid_constant__ RealWtTable tab, const __grid_constant__ RealGroupTable gt,
+                      const uint32_t* __restrict__ amax) {
+  const int l = real_group_find(gt, tab.n, int(blockIdx.x));
+  const int T = tab.T[l], B = gt.B[l], n = tab.Cout[l] * T * B;
+  const int base = (int(blockIdx.x) - gt.blk0[l]) * kRealPackPerBlock;
+  const int end = base + kRealPackPerBlock < n ? base + kRealPackPerBlock : n;
+  const uint32_t a = __ldg(amax + l);
+  const float sw = amax_pow2_scale(a, false), isw = amax_pow2_scale(a, true);
+  const uint16_t* wf = tab.wf[l];
+  uint16_t* wt = tab.wt[l];
+  for (int j = base + threadIdx.x; j < end; j += blockDim.x) {
+    const int ol = j % B, q = j / B;
+    const int tt = q % T, c = q / T;
+    const int b = c - c % B;
+    wt[j] = wf[(int64_t(b + ol) * T + (T - 1 - tt)) * B + (c - b)];
+    if (ol == 0 && tt == 0) {
+      tab.gscale[l][c] = isw;
+      tab.inv_gscale[l][c] = sw;
+    }
+  }
+}
+
 }  // namespace bdbnn
 
 using namespace bdbnn;
@@ -245,6 +314,34 @@ extern "C" int bdbnn_real_act_pack(const float* x, int64_t n_pix, int32_t C, uin
   return check_launch("real_pack_x_kernel");
 }
 
+// Tensor l of a pack's host tables: non-NULL pointers, positive dims and a dense weight.
+static int check_weight_tensor(int l, const float* const* W_host, const int32_t* Cout_host, const int32_t* Cin_host,
+                               const int32_t* kw_host, const int64_t* strides_host, uint16_t* const* wf_host,
+                               float* const* alpha_host, uint16_t* const* wt_host, float* const* gscale_host,
+                               float* const* inv_gscale_host) {
+  const bool grad = wt_host != nullptr;
+  const int k = kw_host[l];
+  const int64_t n = int64_t(Cout_host[l]) * Cin_host[l] * k * k;
+  const int64_t* st4 = strides_host + 4 * int64_t(l);
+  BDBNN_REQUIRE(W_host[l] && wf_host[l] && alpha_host[l], "real_weight_pack_multi: NULL pointer in tensor %d", l);
+  BDBNN_REQUIRE(!grad || (wt_host[l] && gscale_host[l] && inv_gscale_host[l]),
+                "real_weight_pack_multi: NULL gradient output in tensor %d", l);
+  BDBNN_REQUIRE(Cout_host[l] > 0 && Cin_host[l] > 0 && k > 0 && n < (int64_t(1) << 30),
+                "real_weight_pack_multi: bad dims in tensor %d", l);
+  // dense: the strides are a permutation of the contiguous strides of some dimension order
+  int64_t dims[4] = {Cout_host[l], Cin_host[l], k, k}, span = 1;
+  bool dense = true;
+  for (int d = 0; d < 4; ++d) {
+    BDBNN_REQUIRE(st4[d] >= 0 && st4[d] < (int64_t(1) << 30), "real_weight_pack_multi: bad strides in tensor %d", l);
+    span += (dims[d] - 1) * st4[d];
+  }
+  for (int d = 0; d < 4 && dense; ++d)
+    for (int e = d + 1; e < 4; ++e)
+      if (dims[d] > 1 && dims[e] > 1 && st4[d] == st4[e]) dense = false;
+  BDBNN_REQUIRE(dense && span == n, "real_weight_pack_multi: tensor %d is not dense", l);
+  return BDBNN_OK;
+}
+
 // One host body for both entry points: the gradient outputs (wt, gscale, inv_gscale) come as a group, all NULL or
 // all given.  NULL: the two launches and their results are those of the forward-only pack.
 static int real_weight_pack_multi(int32_t count, const float* const* W_host, const int32_t* Cout_host,
@@ -261,25 +358,9 @@ static int real_weight_pack_multi(int32_t count, const float* const* W_host, con
                 "real_weight_pack_multi: wt, gscale and inv_gscale are given together or not at all");
   // every tensor is checked before the first launch
   for (int l = 0; l < count; ++l) {
-    const int k = kw_host[l];
-    const int64_t n = int64_t(Cout_host[l]) * Cin_host[l] * k * k;
-    const int64_t* st4 = strides_host + 4 * int64_t(l);
-    BDBNN_REQUIRE(W_host[l] && wf_host[l] && alpha_host[l], "real_weight_pack_multi: NULL pointer in tensor %d", l);
-    BDBNN_REQUIRE(!grad || (wt_host[l] && gscale_host[l] && inv_gscale_host[l]),
-                  "real_weight_pack_multi: NULL gradient output in tensor %d", l);
-    BDBNN_REQUIRE(Cout_host[l] > 0 && Cin_host[l] > 0 && k > 0 && n < (int64_t(1) << 30),
-                  "real_weight_pack_multi: bad dims in tensor %d", l);
-    // dense: the strides are a permutation of the contiguous strides of some dimension order
-    int64_t dims[4] = {Cout_host[l], Cin_host[l], k, k}, span = 1;
-    bool dense = true;
-    for (int d = 0; d < 4; ++d) {
-      BDBNN_REQUIRE(st4[d] >= 0 && st4[d] < (int64_t(1) << 30), "real_weight_pack_multi: bad strides in tensor %d", l);
-      span += (dims[d] - 1) * st4[d];
-    }
-    for (int d = 0; d < 4 && dense; ++d)
-      for (int e = d + 1; e < 4; ++e)
-        if (dims[d] > 1 && dims[e] > 1 && st4[d] == st4[e]) dense = false;
-    BDBNN_REQUIRE(dense && span == n, "real_weight_pack_multi: tensor %d is not dense", l);
+    const int rc = check_weight_tensor(l, W_host, Cout_host, Cin_host, kw_host, strides_host, wf_host, alpha_host,
+                                       wt_host, gscale_host, inv_gscale_host);
+    if (rc) return rc;
   }
   cudaStream_t st = cudaStream_t(stream);
   if (count > 0) BDBNN_CUDA(cudaMemsetAsync(amax_bits, 0, size_t(count) * sizeof(uint32_t), st));
@@ -378,4 +459,106 @@ extern "C" int bdbnn_real_conv_pack(const float* x, int32_t N, int32_t H, int32_
   real_pack_w_kernel<<<wblocks, 1024, 0, st>>>(weight, Cout, Cin, x_amax_bits, x_amax_bits + 1, reinterpret_cast<__half*>(wf),
                                          reinterpret_cast<__half*>(wt), alpha, gscale, inv_gscale);
   return check_launch("real_pack_w_kernel");
+}
+
+// Dense tensors (groups 1) go through real_weight_pack_multi in their order, their amax words first; the grouped ones
+// through the banded kernels, their words after.
+extern "C" int bdbnn_real_weight_pack_multi_grouped(int32_t count, const float* const* W_host,
+                                                    const int32_t* Cout_host, const int32_t* Cin_host,
+                                                    const int32_t* kw_host, const int64_t* strides_host,
+                                                    const int32_t* groups_host, uint32_t* amax_bits,
+                                                    uint16_t* const* wf_host, float* const* alpha_host,
+                                                    uint16_t* const* wt_host, float* const* gscale_host,
+                                                    float* const* inv_gscale_host, void* stream) {
+  BDBNN_REQUIRE(count >= 0, "real_weight_pack_multi_grouped: bad count");
+  BDBNN_REQUIRE(count == 0 || (W_host && Cout_host && Cin_host && kw_host && strides_host && groups_host && amax_bits &&
+                               wf_host && alpha_host),
+                "real_weight_pack_multi_grouped: NULL table");
+  const bool grad = wt_host != nullptr;
+  BDBNN_REQUIRE((gscale_host != nullptr) == grad && (inv_gscale_host != nullptr) == grad,
+                "real_weight_pack_multi_grouped: wt, gscale and inv_gscale are given together or not at all");
+  std::vector<int> dense, grouped;
+  for (int l = 0; l < count; ++l) {
+    const int g = groups_host[l];
+    BDBNN_REQUIRE(g >= 1, "real_weight_pack_multi_grouped: groups must be >= 1 in tensor %d", l);
+    if (g == 1) { dense.push_back(l); continue; }
+    const int rc = check_weight_tensor(l, W_host, Cout_host, Cin_host, kw_host, strides_host, wf_host, alpha_host,
+                                       wt_host, gscale_host, inv_gscale_host);
+    if (rc) return rc;
+    const int cg = Cin_host[l], B = cg < 16 ? 16 : cg;
+    BDBNN_REQUIRE(kw_host[l] == 3 && int64_t(cg) * g == Cout_host[l] && (B == 16 || B == 32 || B == 64) &&
+                      B % cg == 0 && Cout_host[l] % B == 0,
+                  "real_weight_pack_multi_grouped: tensor %d ([%d, %d, %d, %d], groups %d) has no banded operand", l,
+                  Cout_host[l], cg, kw_host[l], kw_host[l], g);
+    grouped.push_back(l);
+  }
+  cudaStream_t st = cudaStream_t(stream);
+  const int nd = int(dense.size());
+  {
+    // the dense tensors' host tables, in order (real_weight_pack_multi checks them before its first launch; a
+    // grouped tensor launches nothing before that)
+    std::vector<const float*> W(nd);
+    std::vector<int32_t> co(nd), ci(nd), kw(nd);
+    std::vector<int64_t> str(4 * size_t(nd));
+    std::vector<uint16_t*> wf(nd), wt(nd);
+    std::vector<float*> al(nd), gs(nd), igs(nd);
+    for (int i = 0; i < nd; ++i) {
+      const int l = dense[i];
+      W[i] = W_host[l]; co[i] = Cout_host[l]; ci[i] = Cin_host[l]; kw[i] = kw_host[l];
+      for (int d = 0; d < 4; ++d) str[4 * i + d] = strides_host[4 * int64_t(l) + d];
+      wf[i] = wf_host[l]; al[i] = alpha_host[l];
+      if (grad) { wt[i] = wt_host[l]; gs[i] = gscale_host[l]; igs[i] = inv_gscale_host[l]; }
+    }
+    const int rc = real_weight_pack_multi(nd, W.data(), co.data(), ci.data(), kw.data(), str.data(), amax_bits,
+                                          wf.data(), al.data(), grad ? wt.data() : nullptr,
+                                          grad ? gs.data() : nullptr, grad ? igs.data() : nullptr, stream);
+    if (rc) return rc;
+  }
+  const int ng = int(grouped.size());
+  uint32_t* gamax = amax_bits + nd;
+  if (ng > 0) BDBNN_CUDA(cudaMemsetAsync(gamax, 0, size_t(ng) * sizeof(uint32_t), st));
+  for (int off = 0; off < ng; off += kRealPackMax) {
+    const int cnt = ng - off < kRealPackMax ? ng - off : kRealPackMax;
+    RealWPackTable tab;
+    memset(&tab, 0, sizeof(tab));
+    RealWtTable wtab;
+    memset(&wtab, 0, sizeof(wtab));
+    RealGroupTable gt;
+    memset(&gt, 0, sizeof(gt));
+    tab.n = wtab.n = cnt;
+    int64_t wblocks = 0, blocks = 0;
+    for (int i = 0; i < cnt; ++i) {
+      const int l = grouped[off + i];
+      const int cg = Cin_host[l], B = cg < 16 ? 16 : cg;
+      const int64_t* st4 = strides_host + 4 * int64_t(l);
+      tab.W[i] = W_host[l]; tab.wf[i] = wf_host[l]; tab.alpha[i] = alpha_host[l];
+      tab.Cout[i] = Cout_host[l]; tab.Cin[i] = cg; tab.T[i] = 9; tab.KW[i] = 3;
+      tab.sO[i] = int32_t(st4[0]); tab.sC[i] = int32_t(st4[1]); tab.sR[i] = int32_t(st4[2]); tab.sS[i] = int32_t(st4[3]);
+      tab.blk0[i] = int32_t(wblocks);
+      wblocks += (int64_t(Cout_host[l]) * cg * 9 + kRealPackPerBlock - 1) / kRealPackPerBlock;
+      gt.B[i] = B;
+      gt.blk0[i] = int32_t(blocks);
+      blocks += (int64_t(Cout_host[l]) * 9 * B + kRealPackPerBlock - 1) / kRealPackPerBlock;
+      if (grad) {
+        wtab.wf[i] = wf_host[l]; wtab.wt[i] = wt_host[l];
+        wtab.gscale[i] = gscale_host[l]; wtab.inv_gscale[i] = inv_gscale_host[l];
+        wtab.Cout[i] = Cout_host[l]; wtab.Cin[i] = cg; wtab.T[i] = 9;
+      }
+    }
+    BDBNN_REQUIRE(blocks < (int64_t(1) << 31), "real_weight_pack_multi_grouped: too many weights");
+    tab.blk0[cnt] = int32_t(wblocks);
+    gt.blk0[cnt] = int32_t(blocks);
+    real_wamax_multi_kernel<<<unsigned(wblocks), 256, 0, st>>>(tab, gamax + off);
+    int rc = check_launch("real_wamax_multi_kernel");
+    if (rc) return rc;
+    real_gwpack_multi_kernel<<<unsigned(blocks), 256, 0, st>>>(tab, gt, gamax + off);
+    rc = check_launch("real_gwpack_multi_kernel");
+    if (rc) return rc;
+    if (grad) {
+      real_gwt_multi_kernel<<<unsigned(blocks), 256, 0, st>>>(wtab, gt, gamax + off);
+      rc = check_launch("real_gwt_multi_kernel");
+      if (rc) return rc;
+    }
+  }
+  return BDBNN_OK;
 }

@@ -391,6 +391,10 @@ struct TcConvLaunch {
   // stem conv: A is an overlapping-window view (make_window_map) instead of a dense NHWC tensor
   int win;                       // 0 = dense NHWC
   uint64_t win_stride, win_row_stride, win_img_stride;
+  // grouped conv as a banded GEMM (DESIGN.md §4t): band = B > 0 makes the N tile one band [n0, n0 + B) of Nout,
+  // Kc = B, and the activation box's channel coordinate n0 + k over A's a_chans channels (tc_conv_kernel's BANDED
+  // instances); 0 = dense
+  int band, a_chans;
 };
 
 // Geometry of the stem's packed input (stem.cu): fp16 [N][HP][WP][4] zero-padded by 3 on every side,
@@ -431,5 +435,9 @@ int launch_stem_wgrad(const uint16_t* gys, const uint16_t* xw, float* ws, size_t
 void set_tc_trace(long long* buf);
 long long* get_tc_trace();
 bool wgrad_tc_ok(const bdbnn_conv_shape* s);
+// grouped 3x3 convs (DESIGN.md §4t): the band B of the banded kernels (0 = not supported), and whether the banded
+// weight gradient has a plan
+int gconv_band(const bdbnn_conv_shape* s, int groups);
+bool gwgrad_tc_ok(const bdbnn_conv_shape* s, int band);
 
 }  // namespace bdbnn

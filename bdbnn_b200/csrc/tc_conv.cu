@@ -83,7 +83,9 @@ __device__ __forceinline__ void wgmma_k_block(float (&acc)[NW / 2], uint32_t a_s
 // an instance of its own so that the dense-residual instances keep their code.
 // HARDTANH (MODE 2, fp16 operands, no PADRES): z = hardtanh(z) where relu would apply (p.relu is not read), the
 // VGG-Small teacher's unpooled convs; instances of their own for the same reason.
-template <int MODE, int KIND, int NW, bool PADRES = false, bool HARDTANH = false>
+// BANDED (fp16 operands, no PADRES / HARDTANH): a grouped conv as a banded GEMM (DESIGN.md §4t): the N tile is one
+// band of BN = Kc channels and the activation box reads channels [nn0, nn0 + Kc) of A; instances of their own too.
+template <int MODE, int KIND, int NW, bool PADRES = false, bool HARDTANH = false, bool BANDED = false>
 __global__ void __launch_bounds__(kTcThreads, MODE == 0 ? 0 : 2)
 tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const TcConvParams p) {
@@ -146,8 +148,12 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           mbar_expect_tx(fb, tx);
           const uint32_t a_dst = tiles_base + stage * stage_bytes;
           const int kbb = kb >= p.n_kb ? kb - p.n_kb : kb;       // hi and lo halves share B
-          if (p.cn == 1) tma_load_4d(a_dst, &tmA, fb, kb * p.KB, dw, h0 * p.in_step + dh, n0);
-          else if (it % p.cn == ry) tma_load_4d_mc(a_dst, &tmA, fb, kb * p.KB, dw, h0 * p.in_step + dh, n0, a_mask);
+          if constexpr (BANDED) {   // this band's channels of A (no multicast: cn == 1)
+            tma_load_4d(a_dst, &tmA, fb, nn0 + kb * p.KB, dw, h0 * p.in_step + dh, n0);
+          } else {
+            if (p.cn == 1) tma_load_4d(a_dst, &tmA, fb, kb * p.KB, dw, h0 * p.in_step + dh, n0);
+            else if (it % p.cn == ry) tma_load_4d_mc(a_dst, &tmA, fb, kb * p.KB, dw, h0 * p.in_step + dh, n0, a_mask);
+          }
           if (p.cm == 1) tma_load_2d(a_dst + a_bytes, &tmB, fb, tb * p.Kc + kbb * p.KB, nn0);
           else if (it % p.cm == rx) tma_load_2d_mc(a_dst + a_bytes, &tmB, fb, tb * p.Kc + kbb * p.KB, nn0, b_mask);
         }
@@ -391,6 +397,12 @@ static bool plan_tc_conv(const TcConvLaunch& L, int mode, TcConvParams* pp, size
   p.Nout = L.Nout;
   p.BN = pick_bn(L.Nout);
   if (L.fmt < 0 && p.BN < 64) return false;
+  if (L.band) {   // one band per N tile: Kc = B channels of A starting at the tile's first output channel
+    if (L.band != L.Kc || L.Nout % L.band != 0 || L.fmt != BDBNN_FMT_FP16 || L.a_halves != 1 || L.pad_res ||
+        L.hardtanh || L.out_i16 || (mode == 1 && L.bn_sums) || L.win)
+      return false;
+    p.BN = L.band;
+  }
   p.alpha = L.alpha; p.mask = L.mask; p.out = L.out; p.out_i16 = mode == 0 ? L.out_i16 : nullptr;
   p.shift = L.shift; p.zb = L.zb; p.zb8 = L.zb8; p.zb_one = L.fmt == BDBNN_FMT_BF16 ? 0x3F80u : 0x3C00u;
   p.amax_bits = L.amax_bits; p.add = L.add; p.relu = L.relu; p.z_amax = L.z_amax;
@@ -416,7 +428,7 @@ static bool plan_tc_conv(const TcConvLaunch& L, int mode, TcConvParams* pp, size
   p.cm = p.cn = 1;
   if (tc_cluster_enabled()) {
     if (*tiles_out % 2 == 0) p.cm = 2;
-    if ((L.Nout / p.BN) % 2 == 0) p.cn = 2;
+    if ((L.Nout / p.BN) % 2 == 0 && !L.band) p.cn = 2;   // the bands of a row read different activation boxes
   }
   return true;
 }
@@ -440,6 +452,13 @@ static int launch_one(K kern, dim3 grid, size_t smem, cudaStream_t st, const CUt
 
 // The instance for an N tile of bn columns (16, 32, 64 or 128).
 using TcConvKernel = decltype(&tc_conv_kernel<0, 0, 16, false>);
+// The banded instance for a band of bn channels (16, 32 or 64), fp16 operands.
+template <int MODE>
+static TcConvKernel banded_kernel_for(int bn) {
+  return bn == 16 ? tc_conv_kernel<MODE, 0, 16, false, false, true>
+         : bn == 32 ? tc_conv_kernel<MODE, 0, 32, false, false, true>
+                    : tc_conv_kernel<MODE, 0, 64, false, false, true>;
+}
 template <int MODE, int KIND, bool PADRES = false, bool HARDTANH = false>
 static TcConvKernel kernel_for(int bn) {
   return bn == 16   ? tc_conv_kernel<MODE, KIND, 16, PADRES, HARDTANH>
@@ -448,10 +467,10 @@ static TcConvKernel kernel_for(int bn) {
                     : tc_conv_kernel<MODE, KIND, 128, PADRES, HARDTANH>;
 }
 
-template <int MODE, int KIND, bool PADRES = false, bool HARDTANH = false>
+template <int MODE, int KIND, bool PADRES = false, bool HARDTANH = false, bool BANDED = false>
 static int launch_kind(const CUtensorMap& tmA, const CUtensorMap& tmB, const TcConvParams& p, size_t smem, dim3 grid,
                        cudaStream_t st) {
-  const TcConvKernel kern = kernel_for<MODE, KIND, PADRES, HARDTANH>(p.BN);
+  const TcConvKernel kern = BANDED ? banded_kernel_for<MODE>(p.BN) : kernel_for<MODE, KIND, PADRES, HARDTANH>(p.BN);
   BDBNN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
   if (p.bn_sums == nullptr) return launch_one(kern, grid, smem, st, tmA, tmB, p);
   TcConvParams q = p;
@@ -478,14 +497,17 @@ static int launch_tc_conv(const TcConvLaunch& L, cudaStream_t st) {
     rc = make_window_map(&tmA, L.A, L.NIMG, L.IH, L.IW, p.KB, L.win_stride, L.win_row_stride, L.win_img_stride,
                          p.BW, p.BH, p.BNI, L.in_step);
   else
-    rc = make_act_map(&tmA, L.A, L.NIMG, L.IH, L.IW, L.Kc * L.a_halves, p.KB, p.BW, p.BH, p.BNI, L.in_step, esize);
+    rc = make_act_map(&tmA, L.A, L.NIMG, L.IH, L.IW, L.band ? L.a_chans : L.Kc * L.a_halves, p.KB, p.BW, p.BH, p.BNI,
+                      L.in_step, esize);
   if (rc) return rc;
   rc = make_weight_map(&tmB, L.B, L.Nout, L.b_taps * L.Kc, p.KB, p.BN, esize);
   if (rc) return rc;
   const dim3 grid(unsigned(tiles), unsigned(L.Nout / p.BN));
-  // forward statistics of the narrow (16/32-channel) GEMMs: one pass over the fp32 result after the kernel
-  const bool stats_pass = MODE == 0 && L.bn_sums != nullptr && !wide_gemm(L) && L.out != nullptr;
+  // forward statistics of the narrow (16/32-channel) GEMMs: one pass over the fp32 result after the kernel; the
+  // banded GEMMs keep them in the epilogue (DESIGN.md §4t)
+  const bool stats_pass = MODE == 0 && L.bn_sums != nullptr && !wide_gemm(L) && L.out != nullptr && !L.band;
   if (stats_pass) { p.bn_sums = nullptr; p.bn_ymax = nullptr; }
+  if (L.band) return launch_kind<MODE, 0, false, false, true>(tmA, tmB, p, smem, grid, st);
   if (L.fmt < 0) {
     if constexpr (MODE == 1) {
       set_error("tc_conv: fp8 operands are forward only");
@@ -850,9 +872,10 @@ struct DgradStats {      // backward statistics of the BatchNorm unit that produ
   double* sums; uint32_t* gmax;
 };
 
+// band > 0: the grouped conv's banded dgrad (DESIGN.md §4t), wt = [Cin][k*k flipped][band]
 static int dgrad_tc_impl(const uint16_t* gys_bf16, int32_t grad_mode, const uint32_t* amax_bits,
                          const uint16_t* wt_bf16, const uint32_t* mask_bits, const float* add, float* gx,
-                         const bdbnn_conv_shape* s, const DgradStats* stats, void* stream) {
+                         const bdbnn_conv_shape* s, const DgradStats* stats, void* stream, int band = 0) {
   int rc = validate_shape(s);
   if (rc) return rc;
   BDBNN_REQUIRE(gys_bf16 && wt_bf16 && mask_bits && gx, "binconv_dgrad_tc: NULL pointer");
@@ -885,7 +908,8 @@ static int dgrad_tc_impl(const uint16_t* gys_bf16, int32_t grad_mode, const uint
       L.OH = (s->H - a + sd - 1) / sd; L.OW = (s->W - b + sd - 1) / sd;
       if (L.OH <= 0 || L.OW <= 0) continue;
       if (L.n_taps == 0) { empty_phase = true; continue; }
-      L.A = gys_bf16; L.IH = s->Ho; L.IW = s->Wo; L.Kc = s->Cout; L.a_halves = grad_halves; L.in_step = 1;
+      L.A = gys_bf16; L.IH = s->Ho; L.IW = s->Wo; L.Kc = band ? band : s->Cout; L.a_halves = grad_halves; L.in_step = 1;
+      L.band = band; L.a_chans = s->Cout;
       L.B = wt_bf16; L.b_taps = T; L.Nout = s->Cin;
       L.NIMG = s->N;
       L.out_step = sd; L.off_h = a; L.off_w = b; L.OHf = s->H; L.OWf = s->W;
@@ -938,3 +962,123 @@ extern "C" int bdbnn_binconv_dgrad_tc_stats(const uint16_t* gys_bf16, int32_t gr
   return dgrad_tc_impl(gys_bf16, grad_mode, amax_bits, wt_bf16, mask_bits, add, gx, s, &stats, stream);
 }
 
+
+// ---- grouped 3x3 convs as banded GEMMs (DESIGN.md §4t) -------------------------------------------------------
+// The band B = max(16, Cg) of a grouped conv the banded kernels take (Cin = Cout, Cg = Cin / groups divides B, B in
+// {16, 32, 64} and divides Cout, 3x3 / pad 1, the dense kernels' spatial limits), else 0.  No CUDA call.
+namespace bdbnn {
+int gconv_band(const bdbnn_conv_shape* s, int groups) {
+  if (!s || groups < 2 || s->Cin != s->Cout || s->Cin % groups != 0) return 0;
+  const int cg = s->Cin / groups, B = cg < 16 ? 16 : cg;
+  if ((B != 16 && B != 32 && B != 64) || B % cg != 0 || s->Cout % B != 0) return 0;
+  if (s->kh != 3 || s->kw != 3 || s->pad != 1 || !tc_shape_ok(s)) return 0;
+  return B;
+}
+}  // namespace bdbnn
+
+// The forward GEMM of a grouped conv: A = xh (fp16 NHWC, Cin channels), B = wf [Cout][9][B] block-diagonal per band.
+static void gconv_fwd_launch(TcConvLaunch* L, const void* xh, const void* wf, const bdbnn_conv_shape* s, int B) {
+  fwd_launch(L, xh, wf, BDBNN_FMT_FP16, s);
+  L->Kc = B; L->band = B; L->a_chans = s->Cin;
+}
+
+static int gconv_check(const bdbnn_conv_shape* s, int32_t groups, const char* what, int* band) {
+  int rc = validate_shape(s);
+  if (rc) return rc;
+  *band = gconv_band(s, groups);
+  if (*band == 0) {
+    set_error("%s: grouped conv (Cin %d, Cout %d, groups %d, %dx%d, pad %d) not supported", what, s->Cin, s->Cout,
+              groups, s->kh, s->kw, s->pad);
+    return BDBNN_ERR_UNSUPPORTED;
+  }
+  return BDBNN_OK;
+}
+
+extern "C" int bdbnn_real_gconv_supported(const bdbnn_conv_shape* s, int32_t groups) {
+  if (!s || s->N <= 0 || s->H <= 0 || s->W <= 0 || s->stride <= 0 || s->Ho != (s->H + 2 * s->pad - s->kh) / s->stride + 1 ||
+      s->Wo != (s->W + 2 * s->pad - s->kw) / s->stride + 1 || s->Ho <= 0 || s->Wo <= 0)
+    return 0;
+  const int B = gconv_band(s, groups);
+  if (B == 0) return 0;
+  TcConvParams p;
+  size_t smem = 0;
+  int tiles = 0, caps = 0;
+  TcConvLaunch L;
+  gconv_fwd_launch(&L, nullptr, nullptr, s, B);
+  double sums = 0.0;
+  uint32_t ymax = 0;
+  L.bn_sums = &sums; L.bn_ymax = &ymax;          // the training forward keeps its statistics in the epilogue
+  if (plan_tc_conv(L, 0, &p, &smem, &tiles)) caps |= BDBNN_TC_FWD;
+  L.bn_sums = nullptr; L.bn_ymax = nullptr;
+  if (plan_tc_conv(L, 2, &p, &smem, &tiles)) caps |= BDBNN_TC_EVAL;
+  // every phase of the dgrad (the taps of phase (a, b) as dgrad_tc_impl builds them)
+  bool dg = true;
+  const int sd = s->stride;
+  for (int a = 0; a < sd; ++a)
+    for (int b = 0; b < sd; ++b) {
+      memset(&L, 0, sizeof(L));
+      for (int r = 0; r < 3; ++r)
+        for (int q = 0; q < 3; ++q)
+          if ((a + 1 - r) % sd == 0 && (b + 1 - q) % sd == 0) {
+            L.dh[L.n_taps] = int8_t((a + 1 - r) / sd); L.dw[L.n_taps] = int8_t((b + 1 - q) / sd);
+            L.tb[L.n_taps] = uint8_t(8 - (r * 3 + q));
+            ++L.n_taps;
+          }
+      L.OH = (s->H - a + sd - 1) / sd; L.OW = (s->W - b + sd - 1) / sd;
+      if (L.OH <= 0 || L.OW <= 0) continue;
+      L.IH = s->Ho; L.IW = s->Wo; L.Kc = B; L.a_halves = 1; L.in_step = 1; L.b_taps = 9; L.Nout = s->Cin;
+      L.NIMG = s->N; L.out_step = sd; L.off_h = a; L.off_w = b; L.OHf = s->H; L.OWf = s->W;
+      L.fmt = BDBNN_FMT_FP16; L.band = B; L.a_chans = s->Cout;
+      dg = dg && plan_tc_conv(L, 1, &p, &smem, &tiles);
+    }
+  if (dg) caps |= BDBNN_TC_DGRAD;
+  if (gwgrad_tc_ok(s, B)) caps |= BDBNN_TC_WGRAD;
+  return caps;
+}
+
+extern "C" int bdbnn_real_gconv_fwd(const uint16_t* xh, const uint16_t* wf, const float* alpha, float* y,
+                                    const bdbnn_conv_shape* s, int32_t groups, double* bn_sums, uint32_t* bn_ymax,
+                                    void* stream) {
+  int band = 0;
+  int rc = gconv_check(s, groups, "real_gconv_fwd", &band);
+  if (rc) return rc;
+  BDBNN_REQUIRE(xh && wf && alpha && y, "real_gconv_fwd: NULL pointer");
+  BDBNN_REQUIRE((bn_sums == nullptr) == (bn_ymax == nullptr), "real_gconv_fwd: bn_sums and bn_ymax go together");
+  TcConvLaunch L;
+  gconv_fwd_launch(&L, xh, wf, s, band);
+  L.alpha = alpha; L.out = y;
+  L.bn_sums = bn_sums; L.bn_ymax = bn_ymax;
+  rc = bn_stats_zero(bn_sums, bn_ymax, s->Cout, cudaStream_t(stream));
+  if (rc) return rc;
+  return launch_tc_conv<0>(L, cudaStream_t(stream));
+}
+
+extern "C" int bdbnn_real_gconv_fwd_eval(const uint16_t* xh, const uint32_t* x_amax_bits, const uint16_t* wf,
+                                         const float* scale, const float* shift, const float* residual, int32_t act,
+                                         float* z, uint32_t* z_amax_bits, const bdbnn_conv_shape* s, int32_t groups,
+                                         void* stream) {
+  int band = 0;
+  int rc = gconv_check(s, groups, "real_gconv_fwd_eval", &band);
+  if (rc) return rc;
+  BDBNN_REQUIRE(xh && x_amax_bits && wf && scale && shift && z, "real_gconv_fwd_eval: NULL pointer");
+  BDBNN_REQUIRE(act == BDBNN_ACT_NONE || act == BDBNN_ACT_RELU,
+                "real_gconv_fwd_eval: act must be 0 (none) or 1 (ReLU), got %d", act);
+  BDBNN_REQUIRE(residual != z, "real_gconv_fwd_eval: residual must not alias z");
+  cudaStream_t st = cudaStream_t(stream);
+  TcConvLaunch L;
+  gconv_fwd_launch(&L, xh, wf, s, band);
+  L.amax_bits = x_amax_bits;
+  L.alpha = scale; L.shift = shift; L.add = residual; L.out = z; L.z_amax = z_amax_bits;
+  L.relu = act == BDBNN_ACT_RELU;
+  if (z_amax_bits) BDBNN_CUDA(cudaMemsetAsync(z_amax_bits, 0, sizeof(uint32_t), st));
+  return launch_tc_conv<2>(L, st);
+}
+
+extern "C" int bdbnn_real_gconv_dgrad(const uint16_t* gys, const uint32_t* amax_bits, const uint16_t* wt,
+                                      const uint32_t* mask_bits, const float* add, float* gx,
+                                      const bdbnn_conv_shape* s, int32_t groups, void* stream) {
+  int band = 0;
+  int rc = gconv_check(s, groups, "real_gconv_dgrad", &band);
+  if (rc) return rc;
+  return dgrad_tc_impl(gys, BDBNN_GRAD_FP16S, amax_bits, wt, mask_bits, add, gx, s, nullptr, stream, band);
+}

@@ -83,7 +83,9 @@ __host__ __device__ inline int wgrad_a_loads(const TcWgradParams& p, int mg) {
 // NS > 0: the plan's G slots, all issued unconditionally (a CTA of the last M group with fewer M tiles multiplies a
 // duplicate unit into the extra slots and does not store them), so the wgmma chain of a K step has no branch and
 // ptxas does not fence between its wgmmas.  NS = 0: up to 256 / NW slots, predicated on the CTA's count.
-template <int KIND, int NW, int NS>
+// BANDED (box mode): a grouped conv's banded weight gradient (DESIGN.md §4t): N tile blockIdx.z is one band of
+// BN = UW channels, and its units read the activation channels [nn0, nn0 + UW) of that band; instances of their own.
+template <int KIND, int NW, int NS, bool BANDED = false>
 __global__ void __launch_bounds__(kTcThreads)
 tc_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmG,
                 const TcWgradParams p) {
@@ -197,7 +199,7 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
         } else {
           const int hs = h0 * p.stride;
           for (int i = 0; i < n_loads; ++i)
-            tma_load_4d(dst0 + unit_off[i], &tmX, fb, unit_c[i], unit_dw[i], hs + unit_dh[i], n0);
+            tma_load_4d(dst0 + unit_off[i], &tmX, fb, unit_c[i] + (BANDED ? nn0 : 0), unit_dw[i], hs + unit_dh[i], n0);
         }
         uint32_t bdst = dst0 + a_bytes;
         for (int hf = 0; hf < p.g_halves; ++hf)
@@ -268,12 +270,27 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
   }
 }
 
-// Launch with the template arguments of the plan (operand format, wgmma N).
+// Launch with the template arguments of the plan (operand format, wgmma N); `banded`: the BANDED instances (fp16).
 static int launch_wgrad_kernel(const CUtensorMap& tmX, const CUtensorMap& tmG, const TcWgradParams& p, size_t smem,
-                               dim3 grid, cudaStream_t st) {
+                               dim3 grid, cudaStream_t st, bool banded = false) {
   const int nw = p.BN, ns = nw >= 64 ? p.G : 0;
   if (nw >= 64 && ns * nw > 256) { set_error("tc_wgrad_kernel: %d accumulators of %d columns", ns, nw); return BDBNN_ERR_UNSUPPORTED; }
   using Kern = void (*)(CUtensorMap, CUtensorMap, TcWgradParams);
+  if (banded) {
+    if (p.fmt != BDBNN_FMT_FP16 || p.patch || (nw != 16 && nw != 32 && nw != 64) || (nw == 64 && (ns < 1 || ns > 4))) {
+      set_error("tc_wgrad_kernel: no banded instance for N %d, %d accumulators", nw, ns);
+      return BDBNN_ERR_UNSUPPORTED;
+    }
+    const Kern kern = nw == 16   ? tc_wgrad_kernel<0, 16, 0, true>
+                      : nw == 32 ? tc_wgrad_kernel<0, 32, 0, true>
+                      : ns == 1  ? tc_wgrad_kernel<0, 64, 1, true>
+                      : ns == 2  ? tc_wgrad_kernel<0, 64, 2, true>
+                      : ns == 3  ? tc_wgrad_kernel<0, 64, 3, true>
+                                 : tc_wgrad_kernel<0, 64, 4, true>;
+    BDBNN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+    kern<<<grid, kTcThreads, smem, st>>>(tmX, tmG, p);
+    return check_launch("tc_wgrad_kernel(banded)");
+  }
   auto pick = [&](auto kind) -> Kern {
     constexpr int K = decltype(kind)::value;
     if (nw == 16) return tc_wgrad_kernel<K, 16, 0>;
@@ -557,6 +574,67 @@ static WgradPlan plan_wgrad_small(const bdbnn_conv_shape* s, int halves) {
 
 bool wgrad_tc_ok(const bdbnn_conv_shape* s) { return s && plan_wgrad(s, 2).ok; }
 
+// ---- grouped conv weight gradient (DESIGN.md §4t) ----------------------------------------------------------------
+// Each band of B channels is a dense B -> B conv: the narrow-unit box plan of that conv (plan_wgrad_small, UW = BN =
+// B), with one N tile per band (grid z) and the split recomputed for the band count.  Workspace [ksplit][9*B][Cout]:
+// row t*B + cl holds, for output channel o, the sum of x[channel band0(o) + cl] * gy[o], band0(o) = o - o % B.
+static WgradPlan plan_gwgrad(const bdbnn_conv_shape* s, int band) {
+  WgradPlan pl;
+  memset(&pl, 0, sizeof(pl));
+  if (!s || band == 0) return pl;
+  bdbnn_conv_shape sb = *s;
+  sb.Cin = sb.Cout = band;
+  pl = plan_wgrad_small(&sb, 1);
+  if (!pl.ok) return pl;
+  TcWgradParams& p = pl.p;
+  p.Cout = s->Cout;
+  pl.ntiles = s->Cout / band;
+  int ks = kWgradWaves * num_sms() / (pl.mgroups * pl.ntiles);
+  if (ks < 1) ks = 1;
+  pl.ks_cap = ks;
+  if (ks > p.n_kboxes) ks = p.n_kboxes;
+  p.kboxes_per_cta = (p.n_kboxes + ks - 1) / ks;
+  pl.ksplit = (p.n_kboxes + p.kboxes_per_cta - 1) / p.kboxes_per_cta;
+  pl.l2_bytes = wgrad_l2_bytes(pl);
+  return pl;
+}
+
+bool gwgrad_tc_ok(const bdbnn_conv_shape* s, int band) { return plan_gwgrad(s, band).ok; }
+
+// gW[o][cg][t] (OIHW of the grouped weight [Cout][Cg][3][3]) = wmask ? inv_gscale[o] * 2^-e * sum_k ws[k][(t*B + cl)
+// * Cout + o] : 0 for the in-group entries cl = cg + o - o % Cg - (o - o % B); one thread per workspace entry (read
+// coalesced along o), the out-of-group ones (the band's exact zeros) skipped.
+__global__ void __launch_bounds__(256)
+gwgrad_finalize_kernel(const float* __restrict__ ws, int ksplit, const uint32_t* __restrict__ wmask,
+                       const float* __restrict__ inv_gscale, const uint32_t* __restrict__ amax_bits,
+                       float* __restrict__ gW, int Cout, int Cg, int B, int T) {
+  const int64_t n = int64_t(T) * B * Cout;
+  const float post = amax_bits ? amax_pow2_scale(__ldg(amax_bits), true) : 1.0f;
+  for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
+       i += int64_t(gridDim.x) * blockDim.x) {
+    const int o = int(i % Cout);
+    const int64_t q = i / Cout;
+    const int cl = int(q % B), t = int(q / B);
+    const int cg = (o - o % B) + cl - (o - o % Cg);     // input channel minus the first channel of o's group
+    if (cg < 0 || cg >= Cg) continue;
+    const int64_t e = (int64_t(o) * Cg + cg) * T + t;
+    float acc = 0.f;
+    if ((wmask[e >> 5] >> (e & 31)) & 1u) {
+      float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+      int k = 0;
+      for (; k + 3 < ksplit; k += 4) {
+        a0 += ws[int64_t(k) * n + i];
+        a1 += ws[int64_t(k + 1) * n + i];
+        a2 += ws[int64_t(k + 2) * n + i];
+        a3 += ws[int64_t(k + 3) * n + i];
+      }
+      for (; k < ksplit; ++k) a0 += ws[int64_t(k) * n + i];
+      acc = ((a0 + a1) + (a2 + a3)) * post * inv_gscale[o];
+    }
+    gW[e] = acc;
+  }
+}
+
 // ---- stem conv weight gradient ------------------------------------------------------------------
 // D[(r, j), o] = sum_pix xw[window(pix) of row 2*oh + r][j] * gys[pix, o]: 7 units (rows r of the 7x7
 // filter) of 32 window values (8 pixels x 4 halves; j = s*4 + c), box mode, one K stage per output row
@@ -709,4 +787,50 @@ extern "C" int bdbnn_binconv_wgrad_tc(const uint16_t* gys_bf16, int32_t grad_mod
       pl.p.ws, pl.ksplit, wmask_bits, inv_gscale, grad_mode == BDBNN_GRAD_FP16S ? amax_bits : nullptr, gW, s->Cout, s->Cin,
       s->kh * s->kw);
   return check_launch("wgrad_finalize_kernel");
+}
+
+extern "C" size_t bdbnn_real_gconv_wgrad_workspace_bytes(const bdbnn_conv_shape* s, int32_t groups) {
+  const int band = gconv_band(s, groups);
+  const WgradPlan pl = plan_gwgrad(s, band);
+  if (!pl.ok) return 0;
+  return size_t(pl.ks_cap) * 9 * band * s->Cout * sizeof(float);
+}
+
+extern "C" int bdbnn_real_gconv_wgrad(const uint16_t* gys, const uint32_t* amax_bits, const uint16_t* xh,
+                                      const uint32_t* wmask_bits, const float* inv_gscale, float* gW,
+                                      const bdbnn_conv_shape* s, int32_t groups, void* workspace,
+                                      size_t workspace_bytes, void* stream) {
+  int rc = validate_shape(s);
+  if (rc) return rc;
+  BDBNN_REQUIRE(gys && amax_bits && xh && wmask_bits && inv_gscale && gW && workspace, "real_gconv_wgrad: NULL pointer");
+  const int band = gconv_band(s, groups);
+  WgradPlan pl = plan_gwgrad(s, band);
+  if (!pl.ok) {
+    set_error("real_gconv_wgrad: grouped conv (Cin %d, Cout %d, groups %d) not supported", s->Cin, s->Cout, groups);
+    return BDBNN_ERR_UNSUPPORTED;
+  }
+  const size_t need = bdbnn_real_gconv_wgrad_workspace_bytes(s, groups);
+  if (workspace_bytes < need) {
+    set_error("real_gconv_wgrad: workspace %zu B < required %zu B", workspace_bytes, need);
+    return BDBNN_ERR_WORKSPACE;
+  }
+  cudaStream_t st = cudaStream_t(stream);
+  pl.p.fmt = BDBNN_FMT_FP16;
+  pl.p.ws = static_cast<float*>(workspace);
+  pl.p.trace = nullptr;
+  CUtensorMap tmX, tmG;
+  rc = make_act_map(&tmX, xh, s->N, s->H, s->W, s->Cin, band, pl.p.BW, pl.p.BH, pl.p.BNI, s->stride);
+  if (rc) return rc;
+  rc = make_act_map(&tmG, gys, s->N, s->Ho, s->Wo, s->Cout, band, pl.p.BW, pl.p.BH, pl.p.BNI);
+  if (rc) return rc;
+  rc = launch_wgrad_kernel(tmX, tmG, pl.p, pl.smem,
+                           dim3(unsigned(pl.ksplit), unsigned(pl.mgroups), unsigned(pl.ntiles)), st, true);
+  if (rc) return rc;
+  const int cg = s->Cin / groups;
+  const int64_t n = int64_t(9) * band * s->Cout;
+  int64_t blocks = (n + 255) / 256;
+  if (blocks > 2048) blocks = 2048;
+  gwgrad_finalize_kernel<<<unsigned(blocks), 256, 0, st>>>(pl.p.ws, pl.ksplit, wmask_bits, inv_gscale, amax_bits, gW,
+                                                           s->Cout, cg, band, 9);
+  return check_launch("gwgrad_finalize_kernel");
 }

@@ -136,6 +136,27 @@ def algorithmic_bytes(kernel, sh, gh=1):
     }[kernel]
 
 
+def gconv_algorithmic_bytes(kernel, sh, groups):
+    """algorithmic_bytes of the banded grouped-conv kernels (DESIGN.md §4t): the fp16 activations and gradients as the
+    dense kernels, the banded fp16 weight operand [Cout][k*k][B], and the fp32 [Cout][Cg][k][k] weight gradient."""
+    n_in = sh.N * sh.H * sh.W * sh.Cin
+    n_out = sh.N * sh.Ho * sh.Wo * sh.Cout
+    T = sh.kh * sh.kw
+    n_band = sh.Cout * T * gconv_band(sh.Cin, groups)
+    n_w = sh.Cout * (sh.Cin // groups) * T
+    return {
+        "gconv_fwd": 2 * n_in + 2 * n_band + 4 * n_out,       # read fp16 x and the band operand, write fp32 y
+        "gconv_fwd_eval": 2 * n_in + 2 * n_band + 4 * n_out,  # ... write fp32 z (+ residual)
+        "gconv_dgrad": 2 * n_out + 2 * n_band + n_in // 8 + 4 * n_in,
+        "gconv_wgrad": 2 * n_out + 2 * n_in + n_w // 8 + 4 * n_w,
+    }[kernel]
+
+
+def gconv_band(channels, groups):
+    """The band B = max(16, Cg) of a grouped conv over `channels` channels (DESIGN.md §4t)."""
+    return max(16, channels // groups)
+
+
 def _p(t):
     return ctypes.c_void_p(t.data_ptr()) if t is not None else ctypes.c_void_p(0)
 
@@ -2041,11 +2062,18 @@ def _dense(w):
     return w.contiguous()
 
 
-def _real_pack(weights, grad):
-    """bdbnn_real_weight_pack_multi (grad False) or _multi_grad (grad True) of real-valued k x k conv weights.
+def _real_pack(weights, grad, groups=None):
+    """bdbnn_real_weight_pack_multi (grad False) or _multi_grad (grad True) of real-valued k x k conv weights, or with a
+    group count above 1 in `groups` (one per weight) bdbnn_real_weight_pack_multi_grouped, whose grouped weights get
+    the banded operands wf [Cout][k*k][B] and wt [Cin][k*k][B] (DESIGN.md §4t).
     Returns the dense weights that were packed, wf, alpha and (grad) wt, gscale, inv_gscale, as lists."""
     L = _lib.lib()
     ws = [_dense(w.detach()) for w in weights]
+    groups = [int(g) for g in groups] if groups is not None else [1] * len(ws)
+    if len(groups) != len(ws):
+        raise RuntimeError(f"bdbnn_b200.real_weight_pack: {len(groups)} group counts for {len(ws)} weights")
+    if any(g != 1 for g in groups):
+        return _real_pack_grouped(ws, grad, groups)
     what = "real_weight_grad_pack" if grad else "real_weight_pack"
     for w in ws:
         _require_cuda(w, what)
@@ -2082,27 +2110,74 @@ def _real_pack(weights, grad):
         return ws, wf, alpha, wt, gscale, inv_gscale
 
 
-def real_weight_pack(weights):
+def _real_pack_grouped(ws, grad, groups):
+    """_real_pack through bdbnn_real_weight_pack_multi_grouped: groups[l] > 1 gives weight l's banded operands."""
+    L = _lib.lib()
+    what = "real_weight_grad_pack" if grad else "real_weight_pack"
+    for w, g in zip(ws, groups):
+        _require_cuda(w, what)
+        if w.dim() != 4 or w.shape[2] != w.shape[3]:
+            raise RuntimeError(f"bdbnn_b200.{what}: expected [Cout,Cin,k,k] weights, got {tuple(w.shape)}")
+        if g > 1 and (w.shape[2] != 3 or w.shape[0] != w.shape[1] * g or w.shape[0] % gconv_band(w.shape[0], g) or
+                      gconv_band(w.shape[0], g) % w.shape[1] or gconv_band(w.shape[0], g) > 64):
+            raise RuntimeError(f"bdbnn_b200.{what}: weight {tuple(w.shape)} with groups {g} has no banded operand")
+    _same_device(*ws)
+    dev = ws[0].device
+    # the operand width: Cin for a dense weight, the band for a grouped one
+    width = [w.shape[1] if g == 1 else gconv_band(w.shape[0], g) for w, g in zip(ws, groups)]
+    with torch.cuda.device(dev):
+        i16 = dict(dtype=torch.int16, device=dev)
+        wf = [torch.empty((w.shape[0], w.shape[2] * w.shape[3], k), **i16) for w, k in zip(ws, width)]
+        alpha = [torch.empty((w.shape[0],), dtype=torch.float32, device=dev) for w in ws]
+        amax = torch.empty((len(ws),), dtype=torch.int32, device=dev)
+        n = len(ws)
+        ints = lambda vals: (ctypes.c_int32 * n)(*vals)
+        strides = (ctypes.c_int64 * (4 * n))(*[st for w in ws for st in w.stride()])
+        wt = gscale = inv_gscale = None
+        if grad:
+            wt = [torch.empty((w.shape[1] * g, w.shape[2] * w.shape[3], w.shape[0] if g == 1 else k), **i16)
+                  for w, g, k in zip(ws, groups, width)]
+            gscale = [torch.empty((w.shape[0],), dtype=torch.float32, device=dev) for w in ws]
+            inv_gscale = [torch.empty((w.shape[0],), dtype=torch.float32, device=dev) for w in ws]
+        n_w = sum(w.numel() for w in ws)
+        n_op = sum(t.numel() for t in wf)
+        # amax read, pack read, fp16 operand write (+ the dgrad operand's read and write)
+        with _timed("real_weight_grouped_pack", f"n{n}", 4 * n_w * 2 + 2 * n_op + (4 * n_op if grad else 0)):
+            _lib.check(L.bdbnn_real_weight_pack_multi_grouped(
+                n, _ptr_array(ws), ints([w.shape[0] for w in ws]), ints([w.shape[1] for w in ws]),
+                ints([w.shape[3] for w in ws]), strides, ints(groups), _p(amax), _ptr_array(wf), _ptr_array(alpha),
+                _ptr_array(wt) if grad else None, _ptr_array(gscale) if grad else None,
+                _ptr_array(inv_gscale) if grad else None, _stream()), "real_weight_pack_multi_grouped")
+        n_dense = sum(1 for g in groups if g == 1)
+        per = 3 if grad else 2
+        _lib.count(per * ((n_dense + 47) // 48) + per * ((n - n_dense + 47) // 48))
+    return (ws, wf, alpha, wt, gscale, inv_gscale) if grad else (ws, wf, alpha)
+
+
+def real_weight_pack(weights, groups=None):
     """fp16 operands of real-valued k x k conv weights, all in two launches (bdbnn_real_weight_pack_multi): one
     power-of-two scale per tensor.  Contiguous and channels_last weights are read in place, through their strides.
+    `groups` (one count per weight, None = all 1): a grouped 3x3 weight [Cout][Cin/groups][3][3] gets the banded
+    operand wf [Cout][9][B] of DESIGN.md §4t (bdbnn_real_weight_pack_multi_grouped, same call for all weights).
     Returns [(wf [Cout][k*k][Cin] int16, alpha[Cout] = 2^-ew)] in input order, on the weights' device."""
     if not weights:
         return []
-    _, wf, alpha = _real_pack(weights, grad=False)
+    _, wf, alpha = _real_pack(weights, False, groups)
     return list(zip(wf, alpha))
 
 
-def real_weight_grad_pack(weights, grad=True):
+def real_weight_grad_pack(weights, grad=True, groups=None):
     """_WeightPacks of the W32/A1 convs' real weights (DESIGN.md §4p) in one bdbnn_real_weight_pack_multi_grad call:
     wf = fp16(W * 2^ew) [Cout][k*k][Cin] and alpha = 2^-ew for the forward; with `grad` also the dgrad operand wt
     [Cin][k*k flipped][Cout], gscale = 2^-ew, inv_gscale = 2^ew and an all-ones weight mask (W is a real parameter:
-    its gradient is not clamped).  No sign bits and no fp8 copy: those exist for +-1 weights only."""
+    its gradient is not clamped).  No sign bits and no fp8 copy: those exist for +-1 weights only.  `groups` as
+    real_weight_pack: a grouped weight's wf and wt are its banded operands [Cout][9][B], [Cin][9 flipped][B]."""
     if not weights:
         return []
     if not grad:
-        _, wf, alpha = _real_pack(weights, grad=False)
+        _, wf, alpha = _real_pack(weights, False, groups)
         return [_WeightPack(a, None, None, f, None, None, None, None) for f, a in zip(wf, alpha)]
-    ws, wf, alpha, wt, gscale, inv_gscale = _real_pack(weights, grad=True)
+    ws, wf, alpha, wt, gscale, inv_gscale = _real_pack(weights, True, groups)
     out = []
     for w, f, a, t, g, ig in zip(ws, wf, alpha, wt, gscale, inv_gscale):
         ones = torch.full(((w.numel() + 31) // 32,), -1, dtype=torch.int32, device=w.device)
@@ -2145,7 +2220,7 @@ def _real_act_pack(x, x_amax, sh):
 
 @_on_x_device
 def real_conv_bn_eval(x, x_amax, wpack, gamma, beta, running_mean, running_var, eps, stride, padding, residual=None,
-                      relu=True, shortcut=None, hardtanh=False):
+                      relu=True, shortcut=None, hardtanh=False, groups=1):
     """z = relu(BN_eval(conv2d(x, W)) + residual) of a real-valued conv under no_grad, with wpack = (wf, alpha) of
     real_weight_pack(W): real_act_pack -> fold(alpha) -> real_conv_fwd_eval.  x fp32 CUDA (channels_last avoids a
     copy); x_amax = the device word of max|x| a previous call returned (None: computed here, one more pass over x).
@@ -2154,8 +2229,13 @@ def real_conv_bn_eval(x, x_amax, wpack, gamma, beta, running_mean, running_var, 
     padded tensor is written, and z is bit-identical to passing that tensor as `residual`.
     `hardtanh` (with relu=False, without `shortcut`): z = hardtanh(BN_eval(conv2d(x, W)) + residual) in the same
     epilogue, torch.nn.Hardtanh() bit for bit.
+    `groups` > 1: a grouped 3x3 conv (Cin = Cout) with wpack from real_weight_pack(..., groups), on the banded GEMM
+    (real_gconv_fwd_eval, DESIGN.md §4t); no shortcut, no Hardtanh.
     Returns (z fp32 channels_last, z_amax int32[1] = bits of max|z|)."""
     _eval_only("real_conv_bn_eval")
+    if groups != 1:
+        return _real_gconv_bn_eval(x, x_amax, wpack, gamma, beta, running_mean, running_var, eps, stride, padding,
+                                   residual, relu, shortcut, hardtanh, int(groups))
     if hardtanh and relu:
         raise ValueError("bdbnn_b200.real_conv_bn_eval: pass relu=False with hardtanh=True")
     if hardtanh and shortcut is not None:
@@ -2195,6 +2275,49 @@ def real_conv_bn_eval(x, x_amax, wpack, gamma, beta, running_mean, running_var, 
             act = ACT_HARDTANH if hardtanh else (ACT_RELU if relu else ACT_NONE)
             _lib.check(L.bdbnn_real_conv_fwd_eval(_p(xh), _p(amax), _p(wf), _p(scale), _p(shift), _p(rc), act, _p(z),
                                                   _p(z_amax), ctypes.byref(sh), st), "real_conv_fwd_eval")
+    _lib.count(1)
+    return z, z_amax
+
+
+def gconv_shape(x_shape, w_shape, stride, padding, groups):
+    """The ConvShape of a conv of groups `groups` with weight shape [Cout][Cin/groups][kh][kw]."""
+    return conv_shape(x_shape, (w_shape[0], w_shape[1] * groups, *w_shape[2:]), stride, padding)
+
+
+def real_gconv_supported(sh, groups):
+    """bdbnn_real_gconv_supported of a ConvShape (host-only): BDBNN_TC_FWD 1 | DGRAD 2 | WGRAD 4 | EVAL 32, or 0."""
+    return int(_lib.lib().bdbnn_real_gconv_supported(ctypes.byref(sh), int(groups)))
+
+
+def _real_gconv_bn_eval(x, x_amax, wpack, gamma, beta, running_mean, running_var, eps, stride, padding, residual,
+                        relu, shortcut, hardtanh, groups):
+    if shortcut is not None or hardtanh:
+        raise ValueError("bdbnn_b200.real_conv_bn_eval: a grouped conv takes no option-A shortcut and no Hardtanh")
+    _require_cuda(x, "real_conv_bn_eval(x)")
+    wf, alpha = wpack
+    _same_device(x, wf, gamma, beta, running_mean, running_var, residual)
+    L = _lib.lib()
+    n, cin, h, w = x.shape
+    cout, taps, band = wf.shape
+    k = int(round(taps ** 0.5))
+    sh = gconv_shape(x.shape, (cout, cin // groups, k, k), stride, padding, groups)
+    if cin % groups or band != gconv_band(cin, groups) or not real_gconv_supported(sh, groups) & 32:
+        raise RuntimeError(f"bdbnn_b200.real_conv_bn_eval: no banded kernel for input {tuple(x.shape)}, operand "
+                           f"{tuple(wf.shape)}, groups {groups}, stride {stride}, padding {padding}")
+    z_shape = (n, cout, sh.Ho, sh.Wo)
+    if residual is not None and tuple(residual.shape) != z_shape:
+        raise RuntimeError(f"real_conv_bn_eval: residual shape {tuple(residual.shape)} != output shape {z_shape}")
+    dev = x.device
+    _, xh, amax = _real_act_pack(x, x_amax, sh)
+    scale, shift = bn_eval_fold(gamma, beta, running_mean, running_var, eps, alpha)
+    rc = _nhwc(residual.detach()) if residual is not None else None
+    z = torch.empty(z_shape, dtype=torch.float32, device=dev, memory_format=torch.channels_last)
+    z_amax = torch.empty((1,), dtype=torch.int32, device=dev)
+    with _timed("real_gconv_fwd_eval", _shape_key(sh) + f"_g{groups}",
+                gconv_algorithmic_bytes("gconv_fwd_eval", sh, groups) + (4 * z.numel() if rc is not None else 0)):
+        _lib.check(L.bdbnn_real_gconv_fwd_eval(_p(xh), _p(amax), _p(wf), _p(scale), _p(shift), _p(rc),
+                                               ACT_RELU if relu else ACT_NONE, _p(z), _p(z_amax), ctypes.byref(sh),
+                                               groups, _stream()), "real_gconv_fwd_eval")
     _lib.count(1)
     return z, z_amax
 
@@ -2507,12 +2630,18 @@ def conv_pool_bn_eval(x, weight, gamma, beta, running_mean, running_var, eps, pa
 REAL_MAX_COUT = 4096     # the BatchNorm kernels' channel limit (csrc/bn.cu)
 
 
-def real_unit_supported(x_shape, w_shape, stride, padding, max_cout=512):
+def real_unit_supported(x_shape, w_shape, stride, padding, max_cout=512, groups=1):
     """real_conv_bn_relu's geometry (host-only): all three wgmma kernels for the conv, Cin % 4 == 0 (the fp16 operand
     pack), Cout % 32 == 0 (ReLU's mask words) and Cout <= max_cout.  512 is ResNet-18/34's widest conv; the unit itself
-    takes up to REAL_MAX_COUT, which the Bottleneck ResNets' walk asks for (their conv3 and downsample reach 2048)."""
-    return (x_shape[1] % 4 == 0 and w_shape[0] % 32 == 0 and w_shape[0] <= max_cout and
-            unit_supported(x_shape, w_shape, stride, padding))
+    takes up to REAL_MAX_COUT, which the Bottleneck ResNets' walk asks for (their conv3 and downsample reach 2048).
+    groups > 1 (w_shape [Cout][Cin/groups][3][3]): the banded kernels' forward, dgrad and wgrad (DESIGN.md §4t)."""
+    if not (x_shape[1] % 4 == 0 and w_shape[0] % 32 == 0 and w_shape[0] <= max_cout):
+        return False
+    if groups != 1:
+        if x_shape[1] != w_shape[1] * groups:
+            return False
+        return real_gconv_supported(gconv_shape(x_shape, w_shape, stride, padding, groups), groups) & 7 == 7
+    return unit_supported(x_shape, w_shape, stride, padding)
 
 
 def _real_scale_fold(amax, wp):
@@ -2525,15 +2654,16 @@ def _real_scale_fold(amax, wp):
 
 
 def _real_unit_fwd(x, x_amax, op, wpack, w_shape, gamma, beta, residual, running_mean, running_var, momentum, eps,
-                   stride, padding, relu=True):
+                   stride, padding, relu=True, groups=1):
     """Forward of one real-valued conv + BatchNorm(train) (+ residual) (+ ReLU) unit:
     real_act_pack(x, x_amax) -> real_scale_fold -> binconv_fwd_tc (fp16 operands, BatchNorm statistics in the
     epilogue) -> bn_fwd_relu (z, ReLU's mask words, max|z|), or without `relu` bn_fwd (z only; no residual).
     op: (xh, amax), x's fp16 operand and the amax word it was scaled by when another unit already made it, else None.
+    groups > 1: a grouped conv on the banded GEMM (real_gconv_fwd, DESIGN.md §4t), wpack its banded operands.
     Returns (z, z_amax or None, the tensors the backward reads, the conv's shape)."""
     L = _lib.lib()
-    sh = conv_shape(x.shape, w_shape, stride, padding)
-    if not real_unit_supported(x.shape, w_shape, stride, padding, REAL_MAX_COUT):
+    sh = gconv_shape(x.shape, w_shape, stride, padding, groups)
+    if not real_unit_supported(x.shape, w_shape, stride, padding, REAL_MAX_COUT, groups):
         raise RuntimeError(f"bdbnn_b200.real_conv_bn_relu: no kernel for input {tuple(x.shape)}, weight "
                            f"{tuple(w_shape)}, stride {stride}, padding {padding}")
     z_shape = (sh.N, sh.Cout, sh.Ho, sh.Wo)
@@ -2549,9 +2679,14 @@ def _real_unit_fwd(x, x_amax, op, wpack, w_shape, gamma, beta, residual, running
     y = torch.empty(z_shape, memory_format=torch.channels_last, **f32)
     sums = torch.empty((2 * cout,), dtype=torch.float64, device=dev)
     ymax = torch.empty((cout,), dtype=torch.int32, device=dev)
-    with _timed("real_conv_fwd_tc", key, algorithmic_bytes("fwd_tc", sh)):
-        _lib.check(L.bdbnn_binconv_fwd_tc(_p(xh), _p(wpack.wf), FMT_FP16, _p(alpha), _p(y), ctypes.byref(sh),
-                                          _p(sums), _p(ymax), st), "binconv_fwd_tc(real)")
+    if groups != 1:
+        with _timed("real_gconv_fwd_tc", key + f"_g{groups}", gconv_algorithmic_bytes("gconv_fwd", sh, groups)):
+            _lib.check(L.bdbnn_real_gconv_fwd(_p(xh), _p(wpack.wf), _p(alpha), _p(y), ctypes.byref(sh), groups,
+                                              _p(sums), _p(ymax), st), "real_gconv_fwd")
+    else:
+        with _timed("real_conv_fwd_tc", key, algorithmic_bytes("fwd_tc", sh)):
+            _lib.check(L.bdbnn_binconv_fwd_tc(_p(xh), _p(wpack.wf), FMT_FP16, _p(alpha), _p(y), ctypes.byref(sh),
+                                              _p(sums), _p(ymax), st), "binconv_fwd_tc(real)")
     _lib.count(1)
     z = torch.empty_like(y)
     mean, invstd, ab = torch.empty((cout,), **f32), torch.empty((cout,), **f32), torch.empty((2 * cout,), **f32)
@@ -2579,10 +2714,11 @@ def _real_unit_fwd(x, x_amax, op, wpack, w_shape, gamma, beta, residual, running
 
 
 def _real_unit_bwd(gz, saved, sh, x_shape, w_shape, w_param, need_x, need_w, need_res, relu=True, add=None,
-                   out=None):
+                   out=None, groups=1):
     """Backward of _real_unit_fwd: bn_bwd_pack_relu (gz masked, which is also the residual's gradient), or without
     `relu` bn_bwd_pack -> wgrad_tc, dgrad_tc with all-ones STE masks.  add: an fp32 NHWC tensor of x's shape that
-    dgrad's epilogue adds into gx; out: the tensor gx is written to (may be `add`), else a fresh one.
+    dgrad's epilogue adds into gx; out: the tensor gx is written to (may be `add`), else a fresh one.  groups > 1: the
+    banded dgrad and wgrad (real_gconv_dgrad / _wgrad, DESIGN.md §4t).
     Returns (gx, gw, dgamma, dbeta, gres)."""
     L = _lib.lib()
     y, mean, invstd, gamma, ymax, mask, xh, wt, wmask, gscale, inv_gscale = saved
@@ -2609,15 +2745,30 @@ def _real_unit_bwd(gz, saved, sh, x_shape, w_shape, w_param, need_x, need_w, nee
     _lib.count(3)
     gx = gw = None
     # the weight gradient first: in a wgrad_side scope it forks off here and overlaps the dgrad
-    if need_w:
+    if need_w and groups != 1:
+        gw = _wgrad_launch(
+            lambda gwp, ws, ws_bytes, st: _lib.check(L.bdbnn_real_gconv_wgrad(
+                _p(gys), _p(amax), _p(xh), _p(wmask), _p(inv_gscale), gwp, ctypes.byref(sh), groups, ws, ws_bytes, st),
+                "real_gconv_wgrad"),
+            int(L.bdbnn_real_gconv_wgrad_workspace_bytes(ctypes.byref(sh), groups)), w_shape, w_param,
+            (gys, amax, xh, wmask, inv_gscale), "real_gconv_wgrad_tc", key + f"_g{groups}",
+            gconv_algorithmic_bytes("gconv_wgrad", sh, groups))
+    elif need_w:
         gw = _wgrad_tc(sh, gys, GRAD_MODES["fp16s"], amax, xh, wmask, inv_gscale, w_shape, w_param,
                        "real_conv_wgrad_tc", key, algorithmic_bytes("wgrad_tc", sh))
     if need_x:
         ones = torch.full((sh.N, sh.H, sh.W, (sh.Cin + 31) // 32), -1, dtype=torch.int32, device=dev)
         gx = out if out is not None else torch.empty(x_shape, dtype=torch.float32, device=dev,
                                                      memory_format=torch.channels_last)
-        _dgrad_tc(sh, gys, GRAD_MODES["fp16s"], amax, wt, ones, add, gx, "real_conv_dgrad_tc",
-                  algorithmic_bytes("dgrad_tc", sh) + (4 * gx.numel() if add is not None else 0))
+        if groups != 1:
+            with _timed("real_gconv_dgrad_tc", key + f"_g{groups}", gconv_algorithmic_bytes("gconv_dgrad", sh, groups)
+                        + (4 * gx.numel() if add is not None else 0)):
+                _lib.check(L.bdbnn_real_gconv_dgrad(_p(gys), _p(amax), _p(wt), _p(ones), _p(add), _p(gx),
+                                                    ctypes.byref(sh), groups, _stream()), "real_gconv_dgrad")
+            _lib.count(_dgrad_launches(sh))
+        else:
+            _dgrad_tc(sh, gys, GRAD_MODES["fp16s"], amax, wt, ones, add, gx, "real_conv_dgrad_tc",
+                      algorithmic_bytes("dgrad_tc", sh) + (4 * gx.numel() if add is not None else 0))
     return gx, gw, dgamma, dbeta, gres
 
 
@@ -2628,13 +2779,15 @@ class _RealConvBNReLU(torch.autograd.Function):
     @staticmethod
     @_on_device
     def forward(ctx, x, weight, gamma, beta, residual, x_amax, wpack, running_mean, running_var, momentum, eps, stride,
-                padding=1):
+                padding=1, groups=1):
         _require_cuda(x, "real_conv_bn_relu(x)")
         _same_device(x, weight, gamma, beta, residual, x_amax, running_mean, running_var)
         _require_fp16s("real_conv_bn_relu")
         ctx.set_materialize_grads(False)
         z, z_amax, saved, ctx.sh = _real_unit_fwd(x, x_amax, None, wpack, tuple(weight.shape), gamma, beta, residual,
-                                                  running_mean, running_var, momentum, eps, stride, padding)
+                                                  running_mean, running_var, momentum, eps, stride, padding,
+                                                  groups=groups)
+        ctx.groups = groups
         ctx.x_shape, ctx.w_shape = tuple(x.shape), tuple(weight.shape)
         ctx.w_param = weight if (weight.is_leaf and weight.requires_grad) else None
         ctx.has_res = residual is not None
@@ -2646,23 +2799,25 @@ class _RealConvBNReLU(torch.autograd.Function):
     @_on_device
     def backward(ctx, gz, _g_amax):
         if gz is None:
-            return (None,) * 13
+            return (None,) * 14
         need = ctx.needs_input_grad
         gx, gw, dgamma, dbeta, gres = _real_unit_bwd(gz, ctx.saved_tensors, ctx.sh, ctx.x_shape, ctx.w_shape,
-                                                     ctx.w_param, need[0], need[1], ctx.has_res and need[4])
+                                                     ctx.w_param, need[0], need[1], ctx.has_res and need[4],
+                                                     groups=ctx.groups)
         return (gx, gw, dgamma if need[2] else None, dbeta if need[3] else None, gres,
-                None, None, None, None, None, None, None, None)
+                None, None, None, None, None, None, None, None, None)
 
 
 def real_conv_bn_relu(x, x_amax, wpack, weight, gamma, beta, running_mean, running_var, momentum, eps, stride,
-                      residual=None, padding=1):
+                      residual=None, padding=1, groups=1):
     """z = relu(BN_train(conv2d(x, weight, stride, padding)) + residual) of a real-valued conv on the wgmma kernels,
     with autograd (DESIGN.md §4r; 3x3 / padding 1, or 1x1 / padding 0 as in §4s; geometry:
     real_unit_supported(..., max_cout=REAL_MAX_COUT); gradient mode fp16s).  wpack: weight's _WeightPack from
     real_weight_grad_pack; x_amax: the max|x| word the call that wrote x returned (None: computed here).  Returns
-    (z fp32 channels_last, z_amax int32[1] = bits of max|z|, for the next unit's x_amax)."""
+    (z fp32 channels_last, z_amax int32[1] = bits of max|z|, for the next unit's x_amax).  groups > 1: a grouped 3x3
+    conv with wpack from real_weight_grad_pack(..., groups), on the banded kernels (DESIGN.md §4t)."""
     return _RealConvBNReLU.apply(x, weight, gamma, beta, residual, x_amax, wpack, running_mean, running_var,
-                                 float(momentum), float(eps), int(stride), int(padding))
+                                 float(momentum), float(eps), int(stride), int(padding), int(groups))
 
 
 class _RealBottleneck(torch.autograd.Function):
@@ -2682,7 +2837,7 @@ class _RealBottleneck(torch.autograd.Function):
 
     @staticmethod
     @_on_device
-    def forward(ctx, x, x_amax, packs, bn_state, stride, *params):
+    def forward(ctx, x, x_amax, packs, bn_state, stride, groups, *params):
         _require_cuda(x, "real_bottleneck(x)")
         _same_device(x, x_amax, *params)
         _require_fp16s("real_bottleneck")
@@ -2698,7 +2853,7 @@ class _RealBottleneck(torch.autograd.Function):
         def unit(i, inp, residual=None, relu=True):
             z, za, saved[i], sh = _real_unit_fwd(*inp, packs[i], tuple(ws[i].shape), params[3 * i + 1],
                                                  params[3 * i + 2], residual, *bn_state[i], units[i][1], units[i][2],
-                                                 relu=relu)
+                                                 relu=relu, groups=groups if i == 1 else 1)
             geoms[i] = sh
             return z, za
 
@@ -2706,7 +2861,7 @@ class _RealBottleneck(torch.autograd.Function):
         y1, a1 = unit(0, units[0][0])
         y2, a2 = unit(1, (y1, a1, None))
         z, z_amax = unit(2, (y2, a2, None), residual=r)
-        ctx.geoms, ctx.has_ds, ctx.x_shape = geoms, has_ds, tuple(x.shape)
+        ctx.geoms, ctx.has_ds, ctx.x_shape, ctx.groups = geoms, has_ds, tuple(x.shape), groups
         ctx.w_shapes = [tuple(w.shape) for w in ws]
         ctx.w_params = [w if (w.is_leaf and w.requires_grad) else None for w in ws]
         ctx.in_shapes = [tuple(x.shape), tuple(y1.shape), tuple(y2.shape), tuple(x.shape)]
@@ -2719,7 +2874,7 @@ class _RealBottleneck(torch.autograd.Function):
     def backward(ctx, gz, _g_amax):
         n_params = 3 * len(ctx.w_shapes)
         if gz is None:
-            return (None,) * (5 + n_params)
+            return (None,) * (6 + n_params)
         need = ctx.needs_input_grad
         need_x = need[0]
         st = ctx.saved_tensors
@@ -2727,7 +2882,8 @@ class _RealBottleneck(torch.autograd.Function):
 
         def unit(i, g, need_in, need_res=False, relu=True, add=None, out=None):
             return _real_unit_bwd(g, saved[i], ctx.geoms[i], ctx.in_shapes[i], ctx.w_shapes[i], ctx.w_params[i],
-                                  need_in, need[5 + 3 * i], need_res, relu=relu, add=add, out=out)
+                                  need_in, need[6 + 3 * i], need_res, relu=relu, add=add, out=out,
+                                  groups=ctx.groups if i == 1 else 1)
 
         grads = [None] * len(ctx.w_shapes)
         g2, *grads[2], gres = unit(2, gz, True, need_res=need_x or ctx.has_ds)
@@ -2737,23 +2893,26 @@ class _RealBottleneck(torch.autograd.Function):
             _, *grads[3], _ = unit(3, gres, need_x, relu=False, add=gx, out=gx)
         else:
             gx, *grads[0], _ = unit(0, g1, need_x, add=gres, out=gres)
-        out = [gx if need_x else None, None, None, None, None]
+        out = [gx if need_x else None, None, None, None, None, None]
         for i, (gw, dgamma, dbeta) in enumerate(grads):
-            out += [gw, dgamma if need[6 + 3 * i] else None, dbeta if need[7 + 3 * i] else None]
+            out += [gw, dgamma if need[7 + 3 * i] else None, dbeta if need[8 + 3 * i] else None]
         return tuple(out)
 
 
-def real_bottleneck(x, x_amax, packs, params, bn_state, stride):
+def real_bottleneck(x, x_amax, packs, params, bn_state, stride, groups=1):
     """z = relu(BN3(conv3(relu(BN2(conv2(relu(BN1(conv1(x)))))))) + shortcut(x)) of a torchvision Bottleneck block in
     training mode on the wgmma kernels, with autograd (DESIGN.md §4s; geometry: real_unit_supported(...,
     max_cout=REAL_MAX_COUT) for every conv; gradient mode fp16s).  params: [w1, gamma1, beta1, w2, gamma2, beta2, w3,
     gamma3, beta3] and, with a downsample, [w_ds, gamma_ds, beta_ds] after them; packs: the weights' _WeightPacks from
     real_weight_grad_pack, in the same order; bn_state: (running_mean, running_var, momentum, eps) per BatchNorm, in
-    the same order; stride: conv2's and the downsample's.  Returns (z fp32 channels_last, z_amax int32[1])."""
+    the same order; stride: conv2's and the downsample's; groups: conv2's (> 1: a ResNeXt block, conv2 on the banded
+    kernels of DESIGN.md §4t, its pack from real_weight_grad_pack(..., groups)).  Returns (z fp32 channels_last,
+    z_amax int32[1])."""
     if len(params) not in (9, 12) or len(packs) != len(params) // 3 or len(bn_state) != len(packs):
         raise RuntimeError("bdbnn_b200.real_bottleneck: expects 3 or 4 convs with their packs and BatchNorm states")
     return _RealBottleneck.apply(x, x_amax, list(packs),
-                                 [(rm, rv, float(m), float(e)) for rm, rv, m, e in bn_state], int(stride), *params)
+                                 [(rm, rv, float(m), float(e)) for rm, rv, m, e in bn_state], int(stride), int(groups),
+                                 *params)
 
 
 def stem_conv_bn_relu_pool(x, weight, gamma, beta, running_mean, running_var, momentum, eps, kernel_size, stride,

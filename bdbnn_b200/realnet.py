@@ -2,6 +2,7 @@
 
     model = RealResNet(torchvision.models.resnet18())                # or resnet34
     model = RealBottleneckResNet(torchvision.models.resnet50())      # or resnet101/152, wide_resnet50_2/101_2
+    model = RealResNeXt(torchvision.models.resnext50_32x4d())        # or resnext101_32x8d, resnext101_64x4d
 
 wraps the model without copying it, as FrozenResNetTeacher does: the wrapper's children ARE the model's children, so
 `named_parameters()` and `state_dict()` have the model's names and objects, and `load_state_dict`, `.cuda()` and
@@ -16,14 +17,15 @@ In training mode, on a CUDA fp32 input whose geometry every unit takes, the forw
     logits = fc(flatten(avgpool(z)))                        torch
 
 and each Bottleneck block of RealBottleneckResNet as one real_bottleneck node (its 1x1, 3x3 and 1x1 units and the
-downsample).  In eval mode under no_grad it is FrozenResNetTeacher's (FrozenBottleneckTeacher's) eval kernel forward.
+downsample); RealResNeXt's the same, with the grouped conv2 on the banded kernels (DESIGN.md §4t).  In eval mode under
+no_grad it is FrozenResNetTeacher's (FrozenBottleneckTeacher's, FrozenResNeXtTeacher's) eval kernel forward.
 Anything else (CPU, other dtypes, unsupported geometry, BDBNN_FUSE_BN=0, a gradient mode other than fp16s, eval mode
 with autograd) returns the wrapped model's own forward."""
 import torch
 import torch.nn as nn
 
 from . import functional as F_
-from .teacher import FrozenBottleneckTeacher, FrozenResNetTeacher, _family
+from .teacher import FrozenBottleneckTeacher, FrozenResNetTeacher, FrozenResNeXtTeacher, _check_resnext, _family
 
 
 def _bn_train_args(bn):
@@ -162,10 +164,10 @@ class RealBottleneckResNet(RealResNet, FrozenBottleneckTeacher):
         shape = (n, self.conv1.out_channels, (ho - 1) // 2 + 1, (wo - 1) // 2 + 1)
 
         def unit(x_shape, conv):
-            s, p = conv.stride[0], conv.padding[0]
-            if not F_.real_unit_supported(x_shape, tuple(conv.weight.shape), s, p, F_.REAL_MAX_COUT):
+            s, p, g = conv.stride[0], conv.padding[0], conv.groups
+            if not F_.real_unit_supported(x_shape, tuple(conv.weight.shape), s, p, F_.REAL_MAX_COUT, g):
                 return None
-            sh = F_.conv_shape(x_shape, conv.weight.shape, s, p)
+            sh = F_.gconv_shape(x_shape, conv.weight.shape, s, p, g)
             return (n, sh.Cout, sh.Ho, sh.Wo)
 
         for blk in self._blocks:
@@ -183,13 +185,35 @@ class RealBottleneckResNet(RealResNet, FrozenBottleneckTeacher):
         # (conv, BatchNorm) pairs of each block: conv1, conv2, conv3 and the downsample's
         units = [[(blk.conv1, blk.bn1), (blk.conv2, blk.bn2), (blk.conv3, blk.bn3)] +
                  ([tuple(blk.downsample)] if blk.downsample is not None else []) for blk in self._blocks]
-        # 1x1 and 3x3 weights in one pack per forward, never cached: the optimizers update them in place
-        packs = iter(F_.real_weight_grad_pack([c.weight for u in units for c, _ in u]))
+        # 1x1 and 3x3 weights in one pack per forward, never cached: the optimizers update them in place (a ResNeXt's
+        # conv2 as its banded operands)
+        packs = iter(F_.real_weight_grad_pack([c.weight for u in units for c, _ in u],
+                                              groups=[c.groups for u in units for c, _ in u]))
         c1 = self.conv1
         z, z_amax = F_.stem_conv_bn_relu_pool(x, c1.weight, *_bn_train_args(self.bn1), *self._pool_args())
         for blk, u in zip(self._blocks, units):
             params = [t for c, bn in u for t in (c.weight, bn.weight, bn.bias)]
             z, z_amax = F_.real_bottleneck(z, z_amax, [next(packs) for _ in u], params,
-                                           [_bn_train_args(bn)[2:] for _, bn in u], blk.conv2.stride[0])
+                                           [_bn_train_args(bn)[2:] for _, bn in u], blk.conv2.stride[0],
+                                           blk.conv2.groups)
         torch._foreach_add_([bn.num_batches_tracked for bn in self._bns()], 1)
         return self.fc(torch.flatten(self.avgpool(z), 1))
+
+
+class RealResNeXt(RealBottleneckResNet, FrozenResNeXtTeacher):
+    """A torchvision ResNeXt (resnext50_32x4d, resnext101_32x8d, resnext101_64x4d: exactly torchvision's ResNet with
+    Bottleneck blocks whose conv2 all have groups == model.groups > 1) trained on the real-valued training units, each
+    grouped conv2 on the banded kernels (DESIGN.md §4t), with RealBottleneckResNet's kernel-path conditions, fallback
+    and training forward and FrozenResNeXtTeacher's structure check and eval forward.  Raises TypeError, naming the
+    module, for any other structure (groups-1 Bottleneck ResNets, which RealBottleneckResNet wraps; BasicBlock ResNets,
+    replace_stride_with_dilation, a conv2 with another group count, subclassed models or blocks, mixed blocks,
+    nn.DataParallel)."""
+
+    def __init__(self, model):
+        who = "RealResNeXt"
+        _check_resnext(model, who, "RealBottleneckResNet")
+        try:
+            FrozenResNeXtTeacher.__init__(self, model)
+        except TypeError as e:      # the teacher's structure check: name the class the caller used
+            raise TypeError(str(e).replace("FrozenResNeXtTeacher", who)) from None
+        self.__dict__["_train_ok"] = {}

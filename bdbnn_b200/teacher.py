@@ -2,6 +2,7 @@
 
     teacher = FrozenResNetTeacher(torchvision.models.resnet18())      # or resnet34
     teacher = FrozenBottleneckTeacher(torchvision.models.resnet50())  # or resnet101/152, wide_resnet50_2/101_2
+    teacher = FrozenResNeXtTeacher(torchvision.models.resnext101_32x8d())   # or resnext50_32x4d, resnext101_64x4d
     teacher = FrozenResNetTeacher(resnet.ResNetCifar(3, conv_cls=nn.Conv2d))   # the CIFAR KD step's ResNet-20
     teacher = FrozenResNetTeacher(resnet.resnet18_cifar(conv_cls=nn.Conv2d))   # ... and its ResNet-18 (the default)
     teacher = FrozenVGGTeacher(vgg.vgg_small(conv_cls=lambda i, o, k, s, p: nn.Conv2d(i, o, k, s, p, bias=False)))
@@ -19,7 +20,8 @@ CUDA-core launch and its option-A shortcuts are read in place by conv1's epilogu
 ResNet-18 has the same stem and no ReLU; each of its 1x1 `downsample` branches runs on the shortcut eval GEMM and is
 conv1's residual (DESIGN.md §4k).  A Bottleneck ResNet's convs all run as real_conv_bn_eval; with
 BDBNN_TEACHER_F32A=1 its 1x1 convs (conv1, conv3 and the `downsample`) instead read their fp32 input in a GEMM that
-rounds it to fp16 on the way in (real_conv1x1_bn_eval, DESIGN.md §4q).  VGG-Small's Hardtanh is in the epilogue of
+rounds it to fp16 on the way in (real_conv1x1_bn_eval, DESIGN.md §4q).  A ResNeXt's grouped conv2 runs on the banded
+GEMM (real_conv_bn_eval(groups=...), DESIGN.md §4t).  VGG-Small's Hardtanh is in the epilogue of
 its stem and of its unpooled convs; its pooled convs write their fp32 output and one more kernel takes the 2x2 max,
 BatchNorm and Hardtanh (DESIGN.md §4o).
 Anything else returns the wrapped model's own forward."""
@@ -83,10 +85,10 @@ def _check_bn(bn, where, who="FrozenResNetTeacher"):
         raise TypeError(f"{who}: {where} must be nn.BatchNorm2d, got {type(bn).__name__}")
 
 
-def _check_conv(conv, where, k, bias=False, who="FrozenResNetTeacher", net="a BasicBlock ResNet"):
+def _check_conv(conv, where, k, bias=False, who="FrozenResNetTeacher", net="a BasicBlock ResNet", groups=1):
     if type(conv) is not nn.Conv2d:
         raise TypeError(f"{who}: {where} must be nn.Conv2d, got {type(conv).__name__}")
-    if (conv.kernel_size != (k, k) or conv.groups != 1 or conv.dilation != (1, 1) or (conv.bias is not None) != bias
+    if (conv.kernel_size != (k, k) or conv.groups != groups or conv.dilation != (1, 1) or (conv.bias is not None) != bias
             or conv.padding_mode != "zeros" or conv.stride[0] != conv.stride[1] or conv.padding[0] != conv.padding[1]):
         raise TypeError(f"{who}: {where} is not a {k}x{k} conv of {net}")
 
@@ -138,12 +140,19 @@ def _check_shortcut(blk, where, fam):
         _check_bn(sc[1], where + ".downsample.1")
 
 
-def _check_bottleneck(blk, where):
-    """conv1 1x1, conv2 3x3 with the block's stride (groups 1, dilation 1: no ResNeXt, no replace_stride_with_dilation),
-    conv3 1x1, bn3 BatchNorm2d, and a downsample, if any, with the block's stride."""
-    net = "a Bottleneck ResNet"
+def _check_bottleneck(blk, where, groups=1):
+    """conv1 1x1, conv2 3x3 with the block's stride (`groups` groups, dilation 1: no replace_stride_with_dilation;
+    groups 1 refuses ResNeXt), conv3 1x1, bn3 BatchNorm2d, and a downsample, if any, with the block's stride.  A
+    grouped conv2 maps C channels to C with a group width the banded kernels take (DESIGN.md §4t)."""
+    net = "a Bottleneck ResNet" if groups == 1 else f"a ResNeXt with {groups} groups"
     for name, k in (("conv1", 1), ("conv2", 3), ("conv3", 1)):
-        _check_conv(getattr(blk, name), f"{where}.{name}", k, net=net)
+        _check_conv(getattr(blk, name), f"{where}.{name}", k, net=net, groups=groups if name == "conv2" else 1)
+    if groups != 1:
+        c = blk.conv2.in_channels
+        band = F_.gconv_band(c, groups)
+        if blk.conv2.out_channels != c or c % groups or band > 64 or band % (c // groups) or c % band:
+            raise TypeError(f"FrozenResNetTeacher: {where}.conv2 ({c} -> {blk.conv2.out_channels} channels, {groups} "
+                            "groups) has no banded kernel: it needs Cin = Cout and a group width dividing 16, 32 or 64")
     s = blk.conv2.stride
     if s not in ((1, 1), (2, 2)) or blk.conv2.padding != (1, 1):
         raise TypeError(f"FrozenResNetTeacher: {where}.conv2 must be a pad-1 3x3 conv of stride 1 or 2")
@@ -157,10 +166,11 @@ def _check_bottleneck(blk, where):
         raise TypeError(f"FrozenResNetTeacher: {where}.downsample.0 must have conv2's stride {s}")
 
 
-def _blocks(model):
+def _blocks(model, groups=1):
     """(family, [(name, block)] of the residual blocks) after checking that `model` is a torchvision BasicBlock or
     Bottleneck ResNet, or a ResNetCifar or ResNetCifar18 with nn.Conv2d convs throughout: the fp32 teachers.  A CIFAR
-    shell with binary convs is a student, whose eval forward has its own units."""
+    shell with binary convs is a student, whose eval forward has its own units.  groups > 1: a ResNeXt, every
+    Bottleneck's conv2 with exactly that many groups."""
     fam = _family(model)
     names = [n for n, _ in model.named_children()]
     if names != list(fam.children):
@@ -185,7 +195,7 @@ def _blocks(model):
                     ["downsample"] if blk.downsample is not None else []):
                 raise TypeError(f"FrozenResNetTeacher: {where} has unexpected children")
             if fam.bottleneck:
-                _check_bottleneck(blk, where)
+                _check_bottleneck(blk, where, groups)
             else:
                 _check_conv(blk.conv1, where + ".conv1", 3)
                 _check_conv(blk.conv2, where + ".conv2", 3)
@@ -263,11 +273,16 @@ class FrozenResNetTeacher(_FrozenTeacher):
                             "Bottleneck ResNet in FrozenBottleneckTeacher" if not self._BOTTLENECK else
                             "FrozenBottleneckTeacher wraps torchvision Bottleneck ResNets (resnet50/101/152, "
                             "wide_resnet50_2/101_2); wrap a BasicBlock or CIFAR ResNet in FrozenResNetTeacher")
-        family, blocks = _blocks(model)
+        family, blocks = _blocks(model, self._conv2_groups(model))
         super().__init__(model)
         self.__dict__["_family"] = family
         self.__dict__["_blocks"] = [blk for _, blk in blocks]
         self.__dict__["_convs"] = [c for blk in self._blocks for c in (blk.conv1, blk.conv2)]
+
+    @staticmethod
+    def _conv2_groups(model):
+        """The group count every Bottleneck conv2 must have: 1 (FrozenResNeXtTeacher asks for the model's)."""
+        return 1
 
     @property
     def _cifar(self):
@@ -325,8 +340,9 @@ class FrozenResNetTeacher(_FrozenTeacher):
                     break
                 x_shape = shape
                 for conv in (blk.conv1, blk.conv2, blk.conv3):
-                    sh = F_.conv_shape(shape, conv.weight.shape, conv.stride[0], conv.padding[0])
-                    ok = ok and conv_ok(sh)
+                    g = conv.groups
+                    sh = F_.gconv_shape(shape, conv.weight.shape, conv.stride[0], conv.padding[0], g)
+                    ok = ok and (conv_ok(sh) if g == 1 else sh.Cin % 4 == 0 and bool(F_.real_gconv_supported(sh, g) & 32))
                     shape = (n, sh.Cout, sh.Ho, sh.Wo)
                 ds = blk.downsample
                 if ds is not None:
@@ -390,8 +406,8 @@ class FrozenResNetTeacher(_FrozenTeacher):
         convs = []
         for blk in self._blocks:
             convs += [blk.conv1, blk.conv2, blk.conv3] + ([blk.downsample[0]] if blk.downsample is not None else [])
-        # 1x1 and 3x3 weights in one pack, at every forward, never cached
-        packs = iter(F_.real_weight_pack([c.weight for c in convs]))
+        # 1x1 and 3x3 weights in one pack, at every forward, never cached (a ResNeXt's conv2 as its banded operand)
+        packs = iter(F_.real_weight_pack([c.weight for c in convs], [c.groups for c in convs]))
         for blk in self._blocks:
             p1, p2, p3 = next(packs), next(packs), next(packs)
             ds = blk.downsample
@@ -400,7 +416,8 @@ class FrozenResNetTeacher(_FrozenTeacher):
             else:
                 res, _ = conv1x1(z, z_amax, next(packs), *_bn_args(ds[1]), stride=ds[0].stride[0], relu=False)
             y, y_amax = conv1x1(z, z_amax, p1, *_bn_args(blk.bn1), stride=1)
-            y, y_amax = F_.real_conv_bn_eval(y, y_amax, p2, *_bn_args(blk.bn2), blk.conv2.stride[0], 1)
+            y, y_amax = F_.real_conv_bn_eval(y, y_amax, p2, *_bn_args(blk.bn2), blk.conv2.stride[0], 1,
+                                             groups=blk.conv2.groups)
             z, z_amax = conv1x1(y, y_amax, p3, *_bn_args(blk.bn3), stride=1, residual=res)
         return self.fc(torch.flatten(self.avgpool(z), 1))
 
@@ -412,6 +429,42 @@ class FrozenBottleneckTeacher(FrozenResNetTeacher):
     TypeError for any other structure (ResNeXt, dilated ResNets, mixed or subclassed blocks, BasicBlock ResNets,
     nn.DataParallel)."""
     _BOTTLENECK = True
+
+
+class FrozenResNeXtTeacher(FrozenBottleneckTeacher):
+    """A torchvision ResNeXt teacher (resnext50_32x4d, resnext101_32x8d, resnext101_64x4d: exactly torchvision's ResNet
+    with Bottleneck blocks whose conv2 all have groups == model.groups > 1, a group width dividing 16, 32 or 64, no
+    dilation), whose eval forward runs on the real-valued eval kernels with each grouped conv2 on the banded GEMM
+    (DESIGN.md §4t), with FrozenBottleneckTeacher's names, parameters, kernel-path conditions and fallback.  Raises
+    TypeError, naming the module, for any other structure (groups-1 Bottleneck ResNets, which FrozenBottleneckTeacher
+    wraps; replace_stride_with_dilation, a conv2 with another group count, mixed or subclassed blocks, subclassed
+    models, nn.DataParallel)."""
+
+    def __init__(self, model):
+        _check_resnext(model, "FrozenResNeXtTeacher", "FrozenBottleneckTeacher")
+        try:
+            super().__init__(model)
+        except TypeError as e:      # the structure check: name the class the caller used
+            raise TypeError(str(e).replace("FrozenResNetTeacher", "FrozenResNeXtTeacher")) from None
+
+    @staticmethod
+    def _conv2_groups(model):
+        return model.groups
+
+
+def _check_resnext(model, who, dense_who):
+    """Raise TypeError unless `model` is exactly a torchvision ResNet of Bottlenecks with model.groups > 1."""
+    from torchvision.models import resnet as tv
+    if type(model) is not tv.ResNet:
+        raise TypeError(f"{who} wraps a torchvision ResNeXt (resnext50_32x4d, resnext101_32x8d, resnext101_64x4d), got "
+                        f"{type(model).__name__}")
+    layer1 = getattr(model, "layer1", None)
+    first = layer1[0] if type(layer1) is nn.Sequential and len(layer1) > 0 else None
+    if type(first) is not tv.Bottleneck:
+        raise TypeError(f"{who} wraps torchvision ResNeXts; layer1.0 is a {type(first).__name__}")
+    if getattr(model, "groups", 1) <= 1:
+        raise TypeError(f"{who} wraps torchvision ResNeXts; this ResNet has groups 1 (layer1.0.conv2 is not grouped): "
+                        f"wrap it in {dense_who}")
 
 
 _VGG_CHILDREN = ("conv0", "bn0", "conv1", "pooling", "bn1", "conv2", "bn2", "conv3", "bn3", "conv4", "bn4", "conv5",
@@ -526,8 +579,10 @@ def launches_per_forward(model):
     if fam.bottleneck:
         n_ds = sum(1 for b in blocks if b.downsample is not None)
         n1 = 2 * len(blocks) + n_ds
-        return (2 * ((n1 + len(blocks) + 47) // 48) + 6 + 3 * len(blocks) +
-                (2 if F_.teacher_f32a_enabled() else 3) * n1)
+        # a ResNeXt's pack: its dense weights and its grouped conv2s each 2 launches per 48 (DESIGN.md §4t)
+        n_pack = (2 * ((n1 + 47) // 48) + 2 * ((len(blocks) + 47) // 48) if m.groups > 1 else
+                  2 * ((n1 + len(blocks) + 47) // 48))
+        return n_pack + 6 + 3 * len(blocks) + (2 if F_.teacher_f32a_enabled() else 3) * n1
     n3 = 2 * len(blocks)
     n_ds = sum(1 for b in blocks if b.downsample is not None) if fam.shortcut == "downsample" else 0
     return 2 * ((n3 + 47) // 48) + (6 if fam.pooled_stem else 2) + 3 * n3 + 6 * n_ds

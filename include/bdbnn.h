@@ -72,6 +72,7 @@ BDBNN_API int bdbnn_debug_trace(long long* device_buf);
 #define BDBNN_TC_WGRAD 4
 #define BDBNN_TC_FWD8 8   /* fp8 (e4m3 +-1) forward: bdbnn_binconv_fwd_tc8 */
 #define BDBNN_TC_FWD_I16 16 /* forward can store the integer accumulator as int16: bdbnn_binconv_fwd_tc_i16 */
+#define BDBNN_TC_EVAL 32    /* eval-mode forward of a grouped conv: bdbnn_real_gconv_supported only */
 BDBNN_API int bdbnn_tc_supported(const bdbnn_conv_shape* s);
 
 /* ---- activation sign/pack ---------------------------------------------------------------------
@@ -665,6 +666,63 @@ BDBNN_API int bdbnn_real_gemm1x1_fwd_eval(const float* x, const uint32_t* x_amax
                                 const float* scale, const float* shift, const float* residual, int32_t act, float* z,
                                 uint32_t* z_amax_bits, const bdbnn_conv_shape* s, void* stream);
 BDBNN_API int bdbnn_real_gemm1x1_supported(const bdbnn_conv_shape* s);
+
+/* ---- grouped 3x3 real-valued convs as banded GEMMs (ResNeXt conv2, DESIGN.md §4t) -------------------------------
+ * A grouped conv with Cin = Cout = C, `groups` groups of Cg = C / groups channels, 3x3 / pad 1 / stride 1 or 2.  The
+ * output channels are split into bands of B = max(16, Cg) channels (B in {16, 32, 64}, Cg divides B, B divides C);
+ * every group lies inside one band, and a band is a dense B -> B conv whose weight is block-diagonal (exact zeros
+ * between its groups).  x, gy: fp16 NHWC operands as for the dense kernels; fp16 weights as packed by
+ * bdbnn_real_weight_pack_multi_grouped.  Since the band multiplies the other groups' activations by exact zeros, an
+ * Inf or NaN of x (or of gy) in one group reaches the outputs of the other groups of its band (Inf * 0 = NaN), where
+ * torch's grouped conv keeps it inside its group.
+ *   real_gconv_supported   : host-only, no CUDA call: for a valid shape s (Cin = Cout = C) and `groups`,
+ *                            BDBNN_TC_FWD (the training forward, statistics in the epilogue) | BDBNN_TC_EVAL |
+ *                            BDBNN_TC_DGRAD | BDBNN_TC_WGRAD when the banded kernels take it, else 0.
+ *   real_gconv_fwd         : y = acc * alpha[o] (fp32 NHWC [N][Ho][Wo][C]) of xh by wf [C][9][B], with the BatchNorm
+ *                            statistics of y (sum y, sum y^2 as doubles [2C], max|y| bits [C], zeroed here) in the
+ *                            epilogue when bn_sums / bn_ymax are given.  One launch (+ one statistics sum).
+ *   real_gconv_fwd_eval    : bdbnn_real_conv_fwd_eval's epilogue (act BDBNN_ACT_NONE or BDBNN_ACT_RELU) on the
+ *                            banded GEMM.  One launch.
+ *   real_gconv_dgrad       : bdbnn_binconv_dgrad_tc in the BDBNN_GRAD_FP16S mode (gys fp16 [N][Ho][Wo][C] with its
+ *                            amax word; mask_bits, add as there) with wt [C][9 flipped][B].  One launch per stride
+ *                            phase.
+ *   real_gconv_wgrad       : bdbnn_binconv_wgrad_tc in the BDBNN_GRAD_FP16S mode: gW [C][Cg][3][3] = the in-group
+ *                            sums (wmask over gW's OIHW index), with a workspace of
+ *                            real_gconv_wgrad_workspace_bytes(s, groups) bytes (0 = not supported).  Two launches. */
+BDBNN_API int bdbnn_real_gconv_supported(const bdbnn_conv_shape* s, int32_t groups);
+BDBNN_API int bdbnn_real_gconv_fwd(const uint16_t* xh, const uint16_t* wf, const float* alpha, float* y,
+                                   const bdbnn_conv_shape* s, int32_t groups, double* bn_sums, uint32_t* bn_ymax,
+                                   void* stream);
+BDBNN_API int bdbnn_real_gconv_fwd_eval(const uint16_t* xh, const uint32_t* x_amax_bits, const uint16_t* wf,
+                                        const float* scale, const float* shift, const float* residual, int32_t act,
+                                        float* z, uint32_t* z_amax_bits, const bdbnn_conv_shape* s, int32_t groups,
+                                        void* stream);
+BDBNN_API int bdbnn_real_gconv_dgrad(const uint16_t* gys, const uint32_t* amax_bits, const uint16_t* wt,
+                                     const uint32_t* mask_bits, const float* add, float* gx, const bdbnn_conv_shape* s,
+                                     int32_t groups, void* stream);
+BDBNN_API size_t bdbnn_real_gconv_wgrad_workspace_bytes(const bdbnn_conv_shape* s, int32_t groups);
+BDBNN_API int bdbnn_real_gconv_wgrad(const uint16_t* gys, const uint32_t* amax_bits, const uint16_t* xh,
+                                     const uint32_t* wmask_bits, const float* inv_gscale, float* gW,
+                                     const bdbnn_conv_shape* s, int32_t groups, void* workspace,
+                                     size_t workspace_bytes, void* stream);
+/*   real_weight_pack_multi_grouped : bdbnn_real_weight_pack_multi_grad with a group count per tensor (groups_host[l]
+ *                            >= 1; Cin_host[l] = the weight's second dimension, Cin / groups).  A tensor with groups 1
+ *                            gets exactly that entry's wf / alpha / wt / gscale / inv_gscale bits.  A grouped tensor
+ *                            (Cout = Cin_host * groups, k = 3, B = max(16, Cin_host) as in real_gconv_supported)
+ *                            gets the banded operands
+ *                              wf_l[o][t][cl] = fp16(W_l[o][c - g(o)][t] * 2^ew_l) if c and o share a group, else +0
+ *                              wt_l[c][8-t][ol] = wf_l[b(c) + ol][t][c - b(c)]
+ *                            for c = b(o) + cl, b(o) = o - o % B, g(o) = o - o % Cin_host, and the same alpha, gscale
+ *                            and inv_gscale (the zeros do not move max|W_l|).  wt_host, gscale_host and
+ *                            inv_gscale_host are all NULL (forward operands only) or all given.  amax_bits: device
+ *                            scratch of `count` words.  Every tensor is checked before the first launch. */
+BDBNN_API int bdbnn_real_weight_pack_multi_grouped(int32_t count, const float* const* W_host,
+                                                   const int32_t* Cout_host, const int32_t* Cin_host,
+                                                   const int32_t* kw_host, const int64_t* strides_host,
+                                                   const int32_t* groups_host, uint32_t* amax_bits,
+                                                   uint16_t* const* wf_host, float* const* alpha_host,
+                                                   uint16_t* const* wt_host, float* const* gscale_host,
+                                                   float* const* inv_gscale_host, void* stream);
 
 /* ---- eval forward with the CIFAR option-A shortcut as the residual, read in place ------------------------------
  * Replaces F.pad(x[:, :, ::2, ::2], (0, 0, 0, 0, pad, pad)) (models/cifar10's LambdaLayer, the `shortcut` of a

@@ -1,11 +1,13 @@
 """Throughput of the fp32 torchvision ResNet training step on this repository's kernels (RealResNet, DESIGN.md §4r;
-RealBottleneckResNet, §4s): CE + kurtosis (avg over the hooked convs), Adam, batch 256, 224x224, channels_last.
+RealBottleneckResNet, §4s; RealResNeXt, §4t): CE + kurtosis (avg over the hooked convs), Adam, batch 256, 224x224,
+channels_last.
 
     python tools/real_resnet_throughput.py [--batch 256] [--steps 20] [--warmup 5] [--rounds 3] [--nets resnet18,resnet34]
     python tools/real_resnet_throughput.py --nets resnet50,wide_resnet50_2
+    python tools/real_resnet_throughput.py --nets resnext50_32x4d,resnext101_32x8d,resnext101_64x4d
 
 Arms:
-    kernels       RealResNet / RealBottleneckResNet(torchvision model), the step captured by GraphedTrainStep
+    kernels       RealResNet / RealBottleneckResNet / RealResNeXt(torchvision model), the step captured by GraphedTrainStep
     fuse_off      the same with BDBNN_FUSE_BN=0: the torchvision model's own forward (cuDNN, ATen), graphed
     cudnn         the torchvision model in plain TrainStep, eager, TF32 defaults
     cudnn_bench   the same with torch.backends.cudnn.benchmark = True (the reference's train.py:368)
@@ -25,12 +27,13 @@ sys.path.insert(0, ROOT)
 ARMS = ("kernels", "fuse_off", "cudnn", "cudnn_bench")
 NETS = ("resnet18", "resnet34")                                      # the default --nets
 BOTTLENECK_NETS = ("resnet50", "resnet101", "resnet152", "wide_resnet50_2", "wide_resnet101_2")
+RESNEXT_NETS = ("resnext50_32x4d", "resnext101_32x8d", "resnext101_64x4d")
 
 
 def _child(arm, net, batch, steps, warmup):
     import torch
     import torchvision
-    from bdbnn_b200 import RealBottleneckResNet, RealResNet
+    from bdbnn_b200 import RealBottleneckResNet, RealResNet, RealResNeXt
     from bdbnn_b200.functional import KernelTimer
     from bdbnn_b200.step import GraphedTrainStep, StepConfig, TrainStep, make_optimizer
     if not torch.cuda.is_available():
@@ -39,7 +42,8 @@ def _child(arm, net, batch, steps, warmup):
     torch.manual_seed(0)
     model = getattr(torchvision.models, net)().cuda().to(memory_format=torch.channels_last)
     if arm in ("kernels", "fuse_off"):
-        model = (RealBottleneckResNet if net in BOTTLENECK_NETS else RealResNet)(model)
+        model = (RealResNeXt if net in RESNEXT_NETS else
+                 RealBottleneckResNet if net in BOTTLENECK_NETS else RealResNet)(model)
     model.train()
     cfg = StepConfig(w_kurtosis=True)
     eager = TrainStep(model, make_optimizer(model, "imagenet", lr=1e-4), cfg)
@@ -62,10 +66,14 @@ def _child(arm, net, batch, steps, warmup):
     if arm == "kernels":
         KernelTimer.start()
         eager(x, y)
-        fam = {}
-        for (family, _key), d in KernelTimer.stop().items():
+        fam, grouped = {}, {}
+        for (family, key), d in KernelTimer.stop().items():
             fam[family] = round(fam.get(family, 0.0) + d["ms"], 3)
+            if family.startswith("real_gconv"):       # the banded kernels per grouped shape (DESIGN.md §4t)
+                grouped[f"{family} {key}"] = round(d["ms"], 3)
         rec["kernel_ms_per_family"] = dict(sorted(fam.items(), key=lambda kv: -kv[1]))
+        if grouped:
+            rec["grouped_conv_ms_per_shape"] = grouped
     print(json.dumps(rec))
 
 
@@ -85,13 +93,13 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--nets", default=",".join(NETS),
-                    help="comma-separated subset of " + ",".join(NETS + BOTTLENECK_NETS))
+                    help="comma-separated subset of " + ",".join(NETS + BOTTLENECK_NETS + RESNEXT_NETS))
     ap.add_argument("--child", nargs=2, metavar=("ARM", "NET"))
     a = ap.parse_args()
     if a.child:
         _child(a.child[0], a.child[1], a.batch, a.steps, a.warmup)
         return
-    bad = [n for n in a.nets.split(",") if n not in NETS + BOTTLENECK_NETS]
+    bad = [n for n in a.nets.split(",") if n not in NETS + BOTTLENECK_NETS + RESNEXT_NETS]
     if bad:
         ap.error(f"unknown nets {bad}")
     print(json.dumps({"card": _card()}), flush=True)

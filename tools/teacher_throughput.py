@@ -138,7 +138,8 @@ def _cudnn_round(name, mode, args):
     return json.loads(r.stdout.strip().splitlines()[-1])["img_per_s"]
 
 
-BOTTLENECK = ("resnet50", "resnet101", "resnet152", "wide_resnet50_2", "wide_resnet101_2")
+BOTTLENECK = ("resnet50", "resnet101", "resnet152", "wide_resnet50_2", "wide_resnet101_2", "resnext50_32x4d",
+              "resnext101_32x8d", "resnext101_64x4d")
 
 
 def _bottleneck(name):
@@ -169,9 +170,11 @@ def _with_f32a(value, fn):
 
 
 def _wrap(name, model):
-    from bdbnn_b200 import FrozenBottleneckTeacher, FrozenResNetTeacher, FrozenVGGTeacher
+    from bdbnn_b200 import FrozenBottleneckTeacher, FrozenResNetTeacher, FrozenResNeXtTeacher, FrozenVGGTeacher
     if name == "vgg_small":
         return FrozenVGGTeacher(model)
+    if name.startswith("resnext"):
+        return FrozenResNeXtTeacher(model)
     return (FrozenBottleneckTeacher if _bottleneck(name) else FrozenResNetTeacher)(model)
 
 
