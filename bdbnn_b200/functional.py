@@ -2063,56 +2063,16 @@ def _dense(w):
 
 
 def _real_pack(weights, grad, groups=None):
-    """bdbnn_real_weight_pack_multi (grad False) or _multi_grad (grad True) of real-valued k x k conv weights, or with a
-    group count above 1 in `groups` (one per weight) bdbnn_real_weight_pack_multi_grouped, whose grouped weights get
-    the banded operands wf [Cout][k*k][B] and wt [Cin][k*k][B] (DESIGN.md §4t).
-    Returns the dense weights that were packed, wf, alpha and (grad) wt, gscale, inv_gscale, as lists."""
+    """bdbnn_real_weight_pack_multi (grad False) or _multi_grad (grad True) of real-valued k x k conv weights, or, when
+    a group count in `groups` (one per weight) is above 1, bdbnn_real_weight_pack_multi_grouped of them all: a grouped
+    weight gets the banded operands wf [Cout][k*k][B] and wt [Cin][k*k][B] (DESIGN.md §4t), a dense one the bits of
+    the dense pack.  Returns the dense weights that were packed, wf, alpha and (grad) wt, gscale, inv_gscale, as
+    lists."""
     L = _lib.lib()
     ws = [_dense(w.detach()) for w in weights]
     groups = [int(g) for g in groups] if groups is not None else [1] * len(ws)
     if len(groups) != len(ws):
         raise RuntimeError(f"bdbnn_b200.real_weight_pack: {len(groups)} group counts for {len(ws)} weights")
-    if any(g != 1 for g in groups):
-        return _real_pack_grouped(ws, grad, groups)
-    what = "real_weight_grad_pack" if grad else "real_weight_pack"
-    for w in ws:
-        _require_cuda(w, what)
-        if w.dim() != 4 or w.shape[2] != w.shape[3]:
-            raise RuntimeError(f"bdbnn_b200.{what}: expected [Cout,Cin,k,k] weights, got {tuple(w.shape)}")
-    _same_device(*ws)
-    dev = ws[0].device
-    with torch.cuda.device(dev):            # launch on the weights' device, whichever device is current
-        wf = [torch.empty((w.shape[0], w.shape[2] * w.shape[3], w.shape[1]), dtype=torch.int16, device=dev)
-              for w in ws]
-        alpha = [torch.empty((w.shape[0],), dtype=torch.float32, device=dev) for w in ws]
-        amax = torch.empty((len(ws),), dtype=torch.int32, device=dev)
-        n = len(ws)
-        ints = lambda vals: (ctypes.c_int32 * n)(*vals)
-        strides = (ctypes.c_int64 * (4 * n))(*[st for w in ws for st in w.stride()])
-        n_w = sum(w.numel() for w in ws)
-        args = (n, _ptr_array(ws), ints([w.shape[0] for w in ws]), ints([w.shape[1] for w in ws]),
-                ints([w.shape[3] for w in ws]), strides, _p(amax), _ptr_array(wf), _ptr_array(alpha))
-        if not grad:
-            with _timed("real_weight_pack", f"n{n}", 4 * n_w * 2 + 2 * n_w):    # amax read, pack read, fp16 write
-                _lib.check(L.bdbnn_real_weight_pack_multi(*args, _stream()), "real_weight_pack_multi")
-            _lib.count(2 * ((n + 47) // 48))
-            return ws, wf, alpha
-        wt = [torch.empty((w.shape[1], w.shape[2] * w.shape[3], w.shape[0]), dtype=torch.int16, device=dev)
-              for w in ws]
-        gscale = [torch.empty((w.shape[0],), dtype=torch.float32, device=dev) for w in ws]
-        inv_gscale = [torch.empty((w.shape[0],), dtype=torch.float32, device=dev) for w in ws]
-        # + the transpose: fp16 wf read, fp16 wt write
-        with _timed("real_weight_grad_pack", f"n{n}", 4 * n_w * 2 + 2 * n_w + 4 * n_w):
-            _lib.check(L.bdbnn_real_weight_pack_multi_grad(*args, _ptr_array(wt), _ptr_array(gscale),
-                                                           _ptr_array(inv_gscale), _stream()),
-                       "real_weight_pack_multi_grad")
-        _lib.count(3 * ((n + 47) // 48))
-        return ws, wf, alpha, wt, gscale, inv_gscale
-
-
-def _real_pack_grouped(ws, grad, groups):
-    """_real_pack through bdbnn_real_weight_pack_multi_grouped: groups[l] > 1 gives weight l's banded operands."""
-    L = _lib.lib()
     what = "real_weight_grad_pack" if grad else "real_weight_pack"
     for w, g in zip(ws, groups):
         _require_cuda(w, what)
@@ -2123,9 +2083,10 @@ def _real_pack_grouped(ws, grad, groups):
             raise RuntimeError(f"bdbnn_b200.{what}: weight {tuple(w.shape)} with groups {g} has no banded operand")
     _same_device(*ws)
     dev = ws[0].device
+    grouped = any(g != 1 for g in groups)
     # the operand width: Cin for a dense weight, the band for a grouped one
     width = [w.shape[1] if g == 1 else gconv_band(w.shape[0], g) for w, g in zip(ws, groups)]
-    with torch.cuda.device(dev):
+    with torch.cuda.device(dev):            # launch on the weights' device, whichever device is current
         i16 = dict(dtype=torch.int16, device=dev)
         wf = [torch.empty((w.shape[0], w.shape[2] * w.shape[3], k), **i16) for w, k in zip(ws, width)]
         alpha = [torch.empty((w.shape[0],), dtype=torch.float32, device=dev) for w in ws]
@@ -2141,14 +2102,25 @@ def _real_pack_grouped(ws, grad, groups):
             inv_gscale = [torch.empty((w.shape[0],), dtype=torch.float32, device=dev) for w in ws]
         n_w = sum(w.numel() for w in ws)
         n_op = sum(t.numel() for t in wf)
-        # amax read, pack read, fp16 operand write (+ the dgrad operand's read and write)
-        with _timed("real_weight_grouped_pack", f"n{n}", 4 * n_w * 2 + 2 * n_op + (4 * n_op if grad else 0)):
-            _lib.check(L.bdbnn_real_weight_pack_multi_grouped(
-                n, _ptr_array(ws), ints([w.shape[0] for w in ws]), ints([w.shape[1] for w in ws]),
-                ints([w.shape[3] for w in ws]), strides, ints(groups), _p(amax), _ptr_array(wf), _ptr_array(alpha),
-                _ptr_array(wt) if grad else None, _ptr_array(gscale) if grad else None,
-                _ptr_array(inv_gscale) if grad else None, _stream()), "real_weight_pack_multi_grouped")
-        n_dense = sum(1 for g in groups if g == 1)
+        # amax read, pack read, fp16 operand write (+ the dgrad operand: fp16 wf read, fp16 wt write)
+        nbytes = 4 * n_w * 2 + 2 * n_op + (4 * n_op if grad else 0)
+        shapes = (n, _ptr_array(ws), ints([w.shape[0] for w in ws]), ints([w.shape[1] for w in ws]),
+                  ints([w.shape[3] for w in ws]), strides)
+        outs = (_p(amax), _ptr_array(wf), _ptr_array(alpha))
+        grad_outs = (_ptr_array(wt), _ptr_array(gscale), _ptr_array(inv_gscale)) if grad else (None, None, None)
+        if grouped:
+            with _timed("real_weight_grouped_pack", f"n{n}", nbytes):
+                _lib.check(L.bdbnn_real_weight_pack_multi_grouped(*shapes, ints(groups), *outs, *grad_outs, _stream()),
+                           "real_weight_pack_multi_grouped")
+        elif grad:
+            with _timed("real_weight_grad_pack", f"n{n}", nbytes):
+                _lib.check(L.bdbnn_real_weight_pack_multi_grad(*shapes, *outs, *grad_outs, _stream()),
+                           "real_weight_pack_multi_grad")
+        else:
+            with _timed("real_weight_pack", f"n{n}", nbytes):
+                _lib.check(L.bdbnn_real_weight_pack_multi(*shapes, *outs, _stream()), "real_weight_pack_multi")
+        # each entry point: 2 launches (3 with grad) per 48 dense weights and per 48 grouped ones
+        n_dense = groups.count(1)
         per = 3 if grad else 2
         _lib.count(per * ((n_dense + 47) // 48) + per * ((n - n_dense + 47) // 48))
     return (ws, wf, alpha, wt, gscale, inv_gscale) if grad else (ws, wf, alpha)
@@ -2233,9 +2205,9 @@ def real_conv_bn_eval(x, x_amax, wpack, gamma, beta, running_mean, running_var, 
     (real_gconv_fwd_eval, DESIGN.md §4t); no shortcut, no Hardtanh.
     Returns (z fp32 channels_last, z_amax int32[1] = bits of max|z|)."""
     _eval_only("real_conv_bn_eval")
-    if groups != 1:
-        return _real_gconv_bn_eval(x, x_amax, wpack, gamma, beta, running_mean, running_var, eps, stride, padding,
-                                   residual, relu, shortcut, hardtanh, int(groups))
+    groups = int(groups)
+    if groups != 1 and (shortcut is not None or hardtanh):
+        raise ValueError("bdbnn_b200.real_conv_bn_eval: a grouped conv takes no option-A shortcut and no Hardtanh")
     if hardtanh and relu:
         raise ValueError("bdbnn_b200.real_conv_bn_eval: pass relu=False with hardtanh=True")
     if hardtanh and shortcut is not None:
@@ -2245,13 +2217,19 @@ def real_conv_bn_eval(x, x_amax, wpack, gamma, beta, running_mean, running_var, 
     _same_device(x, wf, gamma, beta, running_mean, running_var, residual)
     L = _lib.lib()
     n, cin, h, w = x.shape
-    cout, taps, cin_w = wf.shape
+    cout, taps, width = wf.shape        # width: Cin, or a grouped conv's band
     k = int(round(taps ** 0.5))
-    sh = conv_shape(x.shape, (cout, cin_w, k, k), stride, padding)
-    if not int(L.bdbnn_tc_supported(ctypes.byref(sh))) & 1:
-        raise RuntimeError("bdbnn_b200.real_conv_bn_eval: the wgmma forward does not support this shape")
-    if shortcut is not None:
-        _check_pad_shortcut("real_conv_bn_eval", x, (cout, cin_w, k, k), stride, residual, shortcut)
+    if groups == 1:
+        sh = conv_shape(x.shape, (cout, width, k, k), stride, padding)
+        if not int(L.bdbnn_tc_supported(ctypes.byref(sh))) & 1:
+            raise RuntimeError("bdbnn_b200.real_conv_bn_eval: the wgmma forward does not support this shape")
+        if shortcut is not None:
+            _check_pad_shortcut("real_conv_bn_eval", x, (cout, width, k, k), stride, residual, shortcut)
+    else:
+        sh = gconv_shape(x.shape, (cout, cin // groups, k, k), stride, padding, groups)
+        if cin % groups or width != gconv_band(cin, groups) or not real_gconv_supported(sh, groups) & 32:
+            raise RuntimeError(f"bdbnn_b200.real_conv_bn_eval: no banded kernel for input {tuple(x.shape)}, operand "
+                               f"{tuple(wf.shape)}, groups {groups}, stride {stride}, padding {padding}")
     z_shape = (n, cout, sh.Ho, sh.Wo)
     if residual is not None and tuple(residual.shape) != z_shape:
         raise RuntimeError(f"real_conv_bn_eval: residual shape {tuple(residual.shape)} != output shape {z_shape}")
@@ -2263,18 +2241,23 @@ def real_conv_bn_eval(x, x_amax, wpack, gamma, beta, running_mean, running_var, 
     rc = _nhwc(residual.detach()) if residual is not None else None
     z = torch.empty(z_shape, dtype=torch.float32, device=dev, memory_format=torch.channels_last)
     z_amax = torch.empty((1,), dtype=torch.int32, device=dev)
-    n_out = z.numel()
+    res_bytes = 4 * z.numel() if rc is not None else 0
     if shortcut is not None:
         with _timed("real_conv_fwd_eval_pad_shortcut", key, algorithmic_bytes("fwd_tc_eval", sh) + _pad_res_bytes(sh)):
             _lib.check(L.bdbnn_real_conv_fwd_eval_pad_shortcut(
                 _p(xh), _p(amax), _p(wf), _p(scale), _p(shift), _p(xc), h, w, cin, int(shortcut.pad), int(bool(relu)),
                 _p(z), _p(z_amax), ctypes.byref(sh), st), "real_conv_fwd_eval_pad_shortcut")
-    else:
-        with _timed("real_conv_fwd_eval", key,
-                    algorithmic_bytes("fwd_tc_eval", sh) + (4 * n_out if rc is not None else 0)):
+    elif groups == 1:
+        with _timed("real_conv_fwd_eval", key, algorithmic_bytes("fwd_tc_eval", sh) + res_bytes):
             act = ACT_HARDTANH if hardtanh else (ACT_RELU if relu else ACT_NONE)
             _lib.check(L.bdbnn_real_conv_fwd_eval(_p(xh), _p(amax), _p(wf), _p(scale), _p(shift), _p(rc), act, _p(z),
                                                   _p(z_amax), ctypes.byref(sh), st), "real_conv_fwd_eval")
+    else:
+        with _timed("real_gconv_fwd_eval", key + f"_g{groups}",
+                    gconv_algorithmic_bytes("gconv_fwd_eval", sh, groups) + res_bytes):
+            _lib.check(L.bdbnn_real_gconv_fwd_eval(_p(xh), _p(amax), _p(wf), _p(scale), _p(shift), _p(rc),
+                                                   ACT_RELU if relu else ACT_NONE, _p(z), _p(z_amax), ctypes.byref(sh),
+                                                   groups, st), "real_gconv_fwd_eval")
     _lib.count(1)
     return z, z_amax
 
@@ -2287,39 +2270,6 @@ def gconv_shape(x_shape, w_shape, stride, padding, groups):
 def real_gconv_supported(sh, groups):
     """bdbnn_real_gconv_supported of a ConvShape (host-only): BDBNN_TC_FWD 1 | DGRAD 2 | WGRAD 4 | EVAL 32, or 0."""
     return int(_lib.lib().bdbnn_real_gconv_supported(ctypes.byref(sh), int(groups)))
-
-
-def _real_gconv_bn_eval(x, x_amax, wpack, gamma, beta, running_mean, running_var, eps, stride, padding, residual,
-                        relu, shortcut, hardtanh, groups):
-    if shortcut is not None or hardtanh:
-        raise ValueError("bdbnn_b200.real_conv_bn_eval: a grouped conv takes no option-A shortcut and no Hardtanh")
-    _require_cuda(x, "real_conv_bn_eval(x)")
-    wf, alpha = wpack
-    _same_device(x, wf, gamma, beta, running_mean, running_var, residual)
-    L = _lib.lib()
-    n, cin, h, w = x.shape
-    cout, taps, band = wf.shape
-    k = int(round(taps ** 0.5))
-    sh = gconv_shape(x.shape, (cout, cin // groups, k, k), stride, padding, groups)
-    if cin % groups or band != gconv_band(cin, groups) or not real_gconv_supported(sh, groups) & 32:
-        raise RuntimeError(f"bdbnn_b200.real_conv_bn_eval: no banded kernel for input {tuple(x.shape)}, operand "
-                           f"{tuple(wf.shape)}, groups {groups}, stride {stride}, padding {padding}")
-    z_shape = (n, cout, sh.Ho, sh.Wo)
-    if residual is not None and tuple(residual.shape) != z_shape:
-        raise RuntimeError(f"real_conv_bn_eval: residual shape {tuple(residual.shape)} != output shape {z_shape}")
-    dev = x.device
-    _, xh, amax = _real_act_pack(x, x_amax, sh)
-    scale, shift = bn_eval_fold(gamma, beta, running_mean, running_var, eps, alpha)
-    rc = _nhwc(residual.detach()) if residual is not None else None
-    z = torch.empty(z_shape, dtype=torch.float32, device=dev, memory_format=torch.channels_last)
-    z_amax = torch.empty((1,), dtype=torch.int32, device=dev)
-    with _timed("real_gconv_fwd_eval", _shape_key(sh) + f"_g{groups}",
-                gconv_algorithmic_bytes("gconv_fwd_eval", sh, groups) + (4 * z.numel() if rc is not None else 0)):
-        _lib.check(L.bdbnn_real_gconv_fwd_eval(_p(xh), _p(amax), _p(wf), _p(scale), _p(shift), _p(rc),
-                                               ACT_RELU if relu else ACT_NONE, _p(z), _p(z_amax), ctypes.byref(sh),
-                                               groups, _stream()), "real_gconv_fwd_eval")
-    _lib.count(1)
-    return z, z_amax
 
 
 def teacher_f32a_enabled():
@@ -2653,6 +2603,55 @@ def _real_scale_fold(amax, wp):
     return alpha, inv_gscale
 
 
+def _real_conv_launches(sh, groups):
+    """(fwd, dgrad, wgrad): the launches of a real-valued unit's conv sh, each with its entry point, _timed family, key
+    and algorithmic bytes: the dense wgmma kernels, or with groups > 1 the banded ones (real_gconv_*, DESIGN.md §4t).
+      fwd(xh, wf, alpha, y, sums, ymax)                            y, with its BatchNorm statistics
+      dgrad(gys, amax, wt, ones, add, gx)                          gx (+ add, in the epilogue)
+      wgrad(gys, amax, xh, wmask, inv_gscale, w_shape, w_param)    gw through _wgrad_launch"""
+    L = _lib.lib()
+    key = _shape_key(sh)
+    fp16s = GRAD_MODES["fp16s"]
+    add_bytes = lambda add, gx: 4 * gx.numel() if add is not None else 0
+    if groups == 1:
+        def fwd(xh, wf, alpha, y, sums, ymax):
+            with _timed("real_conv_fwd_tc", key, algorithmic_bytes("fwd_tc", sh)):
+                _lib.check(L.bdbnn_binconv_fwd_tc(_p(xh), _p(wf), FMT_FP16, _p(alpha), _p(y), ctypes.byref(sh),
+                                                  _p(sums), _p(ymax), _stream()), "binconv_fwd_tc(real)")
+
+        def dgrad(gys, amax, wt, ones, add, gx):
+            _dgrad_tc(sh, gys, fp16s, amax, wt, ones, add, gx, "real_conv_dgrad_tc",
+                      algorithmic_bytes("dgrad_tc", sh) + add_bytes(add, gx))
+
+        def wgrad(gys, amax, xh, wmask, inv_gscale, w_shape, w_param):
+            return _wgrad_tc(sh, gys, fp16s, amax, xh, wmask, inv_gscale, w_shape, w_param, "real_conv_wgrad_tc", key,
+                             algorithmic_bytes("wgrad_tc", sh))
+        return fwd, dgrad, wgrad
+    key += f"_g{groups}"
+
+    def fwd(xh, wf, alpha, y, sums, ymax):
+        with _timed("real_gconv_fwd_tc", key, gconv_algorithmic_bytes("gconv_fwd", sh, groups)):
+            _lib.check(L.bdbnn_real_gconv_fwd(_p(xh), _p(wf), _p(alpha), _p(y), ctypes.byref(sh), groups, _p(sums),
+                                              _p(ymax), _stream()), "real_gconv_fwd")
+
+    def dgrad(gys, amax, wt, ones, add, gx):
+        with _timed("real_gconv_dgrad_tc", key,
+                    gconv_algorithmic_bytes("gconv_dgrad", sh, groups) + add_bytes(add, gx)):
+            _lib.check(L.bdbnn_real_gconv_dgrad(_p(gys), _p(amax), _p(wt), _p(ones), _p(add), _p(gx), ctypes.byref(sh),
+                                                groups, _stream()), "real_gconv_dgrad")
+        _lib.count(_dgrad_launches(sh))
+
+    def wgrad(gys, amax, xh, wmask, inv_gscale, w_shape, w_param):
+        return _wgrad_launch(
+            lambda gwp, ws, ws_bytes, st: _lib.check(L.bdbnn_real_gconv_wgrad(
+                _p(gys), _p(amax), _p(xh), _p(wmask), _p(inv_gscale), gwp, ctypes.byref(sh), groups, ws, ws_bytes, st),
+                "real_gconv_wgrad"),
+            int(L.bdbnn_real_gconv_wgrad_workspace_bytes(ctypes.byref(sh), groups)), w_shape, w_param,
+            (gys, amax, xh, wmask, inv_gscale), "real_gconv_wgrad_tc", key,
+            gconv_algorithmic_bytes("gconv_wgrad", sh, groups))
+    return fwd, dgrad, wgrad
+
+
 def _real_unit_fwd(x, x_amax, op, wpack, w_shape, gamma, beta, residual, running_mean, running_var, momentum, eps,
                    stride, padding, relu=True, groups=1):
     """Forward of one real-valued conv + BatchNorm(train) (+ residual) (+ ReLU) unit:
@@ -2679,14 +2678,8 @@ def _real_unit_fwd(x, x_amax, op, wpack, w_shape, gamma, beta, residual, running
     y = torch.empty(z_shape, memory_format=torch.channels_last, **f32)
     sums = torch.empty((2 * cout,), dtype=torch.float64, device=dev)
     ymax = torch.empty((cout,), dtype=torch.int32, device=dev)
-    if groups != 1:
-        with _timed("real_gconv_fwd_tc", key + f"_g{groups}", gconv_algorithmic_bytes("gconv_fwd", sh, groups)):
-            _lib.check(L.bdbnn_real_gconv_fwd(_p(xh), _p(wpack.wf), _p(alpha), _p(y), ctypes.byref(sh), groups,
-                                              _p(sums), _p(ymax), st), "real_gconv_fwd")
-    else:
-        with _timed("real_conv_fwd_tc", key, algorithmic_bytes("fwd_tc", sh)):
-            _lib.check(L.bdbnn_binconv_fwd_tc(_p(xh), _p(wpack.wf), FMT_FP16, _p(alpha), _p(y), ctypes.byref(sh),
-                                              _p(sums), _p(ymax), st), "binconv_fwd_tc(real)")
+    fwd, _, _ = _real_conv_launches(sh, groups)
+    fwd(xh, wpack.wf, alpha, y, sums, ymax)
     _lib.count(1)
     z = torch.empty_like(y)
     mean, invstd, ab = torch.empty((cout,), **f32), torch.empty((cout,), **f32), torch.empty((2 * cout,), **f32)
@@ -2743,32 +2736,16 @@ def _real_unit_bwd(gz, saved, sh, x_shape, w_shape, w_param, need_x, need_w, nee
                                            cout, GRAD_MODES["fp16s"], _p(sums), _p(gmax), _p(consts), _p(dgamma),
                                            _p(dbeta), _p(amax), _p(gys), _stream()), "bn_bwd_pack(real)")
     _lib.count(3)
+    _, dgrad, wgrad = _real_conv_launches(sh, groups)
     gx = gw = None
     # the weight gradient first: in a wgrad_side scope it forks off here and overlaps the dgrad
-    if need_w and groups != 1:
-        gw = _wgrad_launch(
-            lambda gwp, ws, ws_bytes, st: _lib.check(L.bdbnn_real_gconv_wgrad(
-                _p(gys), _p(amax), _p(xh), _p(wmask), _p(inv_gscale), gwp, ctypes.byref(sh), groups, ws, ws_bytes, st),
-                "real_gconv_wgrad"),
-            int(L.bdbnn_real_gconv_wgrad_workspace_bytes(ctypes.byref(sh), groups)), w_shape, w_param,
-            (gys, amax, xh, wmask, inv_gscale), "real_gconv_wgrad_tc", key + f"_g{groups}",
-            gconv_algorithmic_bytes("gconv_wgrad", sh, groups))
-    elif need_w:
-        gw = _wgrad_tc(sh, gys, GRAD_MODES["fp16s"], amax, xh, wmask, inv_gscale, w_shape, w_param,
-                       "real_conv_wgrad_tc", key, algorithmic_bytes("wgrad_tc", sh))
+    if need_w:
+        gw = wgrad(gys, amax, xh, wmask, inv_gscale, w_shape, w_param)
     if need_x:
         ones = torch.full((sh.N, sh.H, sh.W, (sh.Cin + 31) // 32), -1, dtype=torch.int32, device=dev)
         gx = out if out is not None else torch.empty(x_shape, dtype=torch.float32, device=dev,
                                                      memory_format=torch.channels_last)
-        if groups != 1:
-            with _timed("real_gconv_dgrad_tc", key + f"_g{groups}", gconv_algorithmic_bytes("gconv_dgrad", sh, groups)
-                        + (4 * gx.numel() if add is not None else 0)):
-                _lib.check(L.bdbnn_real_gconv_dgrad(_p(gys), _p(amax), _p(wt), _p(ones), _p(add), _p(gx),
-                                                    ctypes.byref(sh), groups, _stream()), "real_gconv_dgrad")
-            _lib.count(_dgrad_launches(sh))
-        else:
-            _dgrad_tc(sh, gys, GRAD_MODES["fp16s"], amax, wt, ones, add, gx, "real_conv_dgrad_tc",
-                      algorithmic_bytes("dgrad_tc", sh) + (4 * gx.numel() if add is not None else 0))
+        dgrad(gys, amax, wt, ones, add, gx)
     return gx, gw, dgamma, dbeta, gres
 
 

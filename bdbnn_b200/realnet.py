@@ -6,7 +6,10 @@
 
 wraps the model without copying it, as FrozenResNetTeacher does: the wrapper's children ARE the model's children, so
 `named_parameters()` and `state_dict()` have the model's names and objects, and `load_state_dict`, `.cuda()` and
-`.train()` act on the model.
+`.train()` act on the model.  Each is a subclass of the teacher of the same kind (FrozenResNetTeacher,
+FrozenBottleneckTeacher, FrozenResNeXtTeacher), whose structure check and eval forward it uses; RealResNet holds the
+training path for both block kinds, and RealBottleneckResNet and RealResNeXt are subclasses whose body is the _KINDS
+they take.
 
 In training mode, on a CUDA fp32 input whose geometry every unit takes, the forward runs with autograd as
 
@@ -22,10 +25,9 @@ no_grad it is FrozenResNetTeacher's (FrozenBottleneckTeacher's, FrozenResNeXtTea
 Anything else (CPU, other dtypes, unsupported geometry, BDBNN_FUSE_BN=0, a gradient mode other than fp16s, eval mode
 with autograd) returns the wrapped model's own forward."""
 import torch
-import torch.nn as nn
 
 from . import functional as F_
-from .teacher import FrozenBottleneckTeacher, FrozenResNetTeacher, FrozenResNeXtTeacher, _check_resnext, _family
+from .teacher import FrozenBottleneckTeacher, FrozenResNetTeacher, FrozenResNeXtTeacher
 
 
 def _bn_train_args(bn):
@@ -35,21 +37,12 @@ def _bn_train_args(bn):
 class RealResNet(FrozenResNetTeacher):
     """A torchvision resnet18 / resnet34 (exactly torchvision's ResNet with BasicBlocks) trained on the real-valued
     training units, with FrozenResNetTeacher's structure check, geometry walk and eval forward.  Raises TypeError for
-    any other structure (Bottleneck ResNets, subclasses, nn.DataParallel, custom blocks), naming the module."""
-
-    def __init__(self, model):
-        from torchvision.models import resnet as tv
-        if type(model) is not tv.ResNet:
-            raise TypeError(f"RealResNet wraps a torchvision ResNet with BasicBlocks (resnet18/34), got "
-                            f"{type(model).__name__}")
-        if _family(model).bottleneck:
-            raise TypeError("RealResNet wraps torchvision BasicBlock ResNets (resnet18/34); layer1.0 is a Bottleneck: "
-                            "wrap a Bottleneck ResNet in RealBottleneckResNet")
-        try:
-            super().__init__(model)
-        except TypeError as e:      # the teacher's structure check: name the class the caller used
-            raise TypeError(str(e).replace("FrozenResNetTeacher", "RealResNet")) from None
-        self.__dict__["_train_ok"] = {}
+    any other structure (Bottleneck ResNets, subclasses, nn.DataParallel, custom blocks), naming the module.  Its
+    subclasses share its kernel-path conditions, training walk and training forward, each for the kinds of network in
+    its _KINDS."""
+    _KINDS = ("basic",)
+    # the trainer of each kind, which a refusal names instead (no trainer takes the CIFAR ResNets)
+    _WRAPPER_OF = {"basic": "RealResNet", "bottleneck": "RealBottleneckResNet", "resnext": "RealResNeXt"}
 
     def kernel_path(self, x):
         """True when forward(x) runs on this repository's kernels: the training units in training mode, the eval
@@ -83,137 +76,93 @@ class RealResNet(FrozenResNetTeacher):
         c1 = self.conv1
         if self._pool_args() != (3, 2, 1) or not F_.stem_conv_supported(x, c1.weight, c1.stride, c1.padding):
             return False
-        key = (x.device, tuple(x.shape))
-        ok = self._train_ok.get(key)
+        key = (x.device, tuple(x.shape), "train")      # in the eval walk's cache, apart from its keys
+        ok = self._geom_ok.get(key)
         if ok is None:
-            ok = self._train_ok[key] = self._walk_train_geometry(x)
+            ok = self._geom_ok[key] = self._walk_train_geometry(x)
         return ok
 
     def _walk_train_geometry(self, x):
-        """Every 3x3 conv has its training unit and every `downsample` its shortcut unit at this input size, and each
-        block's shortcut has its output's shape (host-only)."""
-        n, _, h, w = x.shape
-        ho, wo = (h - 1) // 2 + 1, (w - 1) // 2 + 1
-        shape = (n, self.conv1.out_channels, (ho - 1) // 2 + 1, (wo - 1) // 2 + 1)
-        for blk in self._blocks:
-            x_shape = shape
-            for conv in (blk.conv1, blk.conv2):
-                if not F_.real_unit_supported(shape, conv.weight.shape, conv.stride[0], conv.padding[0]):
-                    return False
-                sh = F_.conv_shape(shape, conv.weight.shape, conv.stride[0], conv.padding[0])
-                shape = (n, sh.Cout, sh.Ho, sh.Wo)
-            ds = blk.downsample
-            if ds is None:
-                if x_shape != shape:
-                    return False
-            else:
-                sd = ds[0].stride[0]
-                if not F_.shortcut_shape_supported(x_shape, tuple(ds[0].weight.shape), sd):
-                    return False
-                if (n, ds[0].out_channels, (x_shape[2] - 1) // sd + 1, (x_shape[3] - 1) // sd + 1) != shape:
-                    return False
-        return True
-
-    # ---- training forward --------------------------------------------------------------------------------------
-    def _train_forward(self, x):
-        # the 3x3 weights in one pack per forward, never cached: the optimizers update them in place
-        packs = F_.real_weight_grad_pack([c.weight for c in self._convs])
-        c1 = self.conv1
-        z, z_amax = F_.stem_conv_bn_relu_pool(x, c1.weight, *_bn_train_args(self.bn1), *self._pool_args())
-        for i, blk in enumerate(self._blocks):
-            ds = blk.downsample
-            res = z if ds is None else F_.shortcut_conv_bn(z, ds[0].weight, *_bn_train_args(ds[1]), ds[0].stride[0])
-            y, y_amax = F_.real_conv_bn_relu(z, z_amax, packs[2 * i], blk.conv1.weight, *_bn_train_args(blk.bn1),
-                                             blk.conv1.stride[0])
-            z, z_amax = F_.real_conv_bn_relu(y, y_amax, packs[2 * i + 1], blk.conv2.weight, *_bn_train_args(blk.bn2),
-                                             1, residual=res)
-        torch._foreach_add_([bn.num_batches_tracked for bn in self._bns()], 1)
-        return self.fc(torch.flatten(self.avgpool(z), 1))
-
-
-class RealBottleneckResNet(RealResNet, FrozenBottleneckTeacher):
-    """A torchvision Bottleneck ResNet (exactly torchvision's ResNet with Bottleneck blocks, groups 1, no dilation:
-    resnet50/101/152, wide_resnet50_2/101_2) trained on the real-valued training units (DESIGN.md §4s), with
-    RealResNet's kernel-path conditions and fallback and FrozenBottleneckTeacher's structure check and eval forward.
-    Raises TypeError for any other structure (BasicBlock ResNets, ResNeXt, replace_stride_with_dilation, subclassed
-    models or blocks, mixed blocks, nn.DataParallel), naming the module."""
-
-    def __init__(self, model):
-        from torchvision.models import resnet as tv
-        who = "RealBottleneckResNet"
-        if type(model) is not tv.ResNet:
-            raise TypeError(f"{who} wraps a torchvision ResNet with Bottlenecks (resnet50/101/152, "
-                            f"wide_resnet50_2/101_2), got {type(model).__name__}")
-        layer1 = getattr(model, "layer1", None)
-        first = layer1[0] if type(layer1) is nn.Sequential and len(layer1) > 0 else None
-        if type(first) is not tv.Bottleneck:
-            hint = ": wrap a BasicBlock ResNet in RealResNet" if type(first) is tv.BasicBlock else ""
-            raise TypeError(f"{who} wraps torchvision Bottleneck ResNets (resnet50/101/152, wide_resnet50_2/101_2); "
-                            f"layer1.0 is a {type(first).__name__}{hint}")
-        try:
-            FrozenBottleneckTeacher.__init__(self, model)
-        except TypeError as e:      # the teacher's structure check: name the class the caller used
-            raise TypeError(str(e).replace("FrozenResNetTeacher", who)) from None
-        self.__dict__["_train_ok"] = {}
-
-    def _walk_train_geometry(self, x):
-        """Every conv has its training unit at this input size (up to F_.REAL_MAX_COUT output channels), and each
-        block's shortcut has its output's shape (host-only)."""
+        """Every conv has its training unit at this input size, a BasicBlock's `downsample` its shortcut unit and a
+        Bottleneck's its conv unit, and each block's shortcut has its output's shape (host-only)."""
+        bottleneck = self._family.bottleneck
+        # a Bottleneck ResNet's conv3 and downsample reach 2048 channels, up to the BatchNorm kernels' limit; a
+        # BasicBlock ResNet's units keep real_unit_supported's default cap of 512 channels, ResNet-18/34's widest
+        max_cout = F_.REAL_MAX_COUT if bottleneck else 512
         n, _, h, w = x.shape
         ho, wo = (h - 1) // 2 + 1, (w - 1) // 2 + 1
         shape = (n, self.conv1.out_channels, (ho - 1) // 2 + 1, (wo - 1) // 2 + 1)
 
         def unit(x_shape, conv):
             s, p, g = conv.stride[0], conv.padding[0], conv.groups
-            if not F_.real_unit_supported(x_shape, tuple(conv.weight.shape), s, p, F_.REAL_MAX_COUT, g):
+            if not F_.real_unit_supported(x_shape, tuple(conv.weight.shape), s, p, max_cout, g):
                 return None
             sh = F_.gconv_shape(x_shape, conv.weight.shape, s, p, g)
             return (n, sh.Cout, sh.Ho, sh.Wo)
 
-        for blk in self._blocks:
+        for units, ds in self._units:
             x_shape = shape
-            for conv in (blk.conv1, blk.conv2, blk.conv3):
+            for conv, _ in units:
                 shape = unit(shape, conv)
                 if shape is None:
                     return False
-            r_shape = x_shape if blk.downsample is None else unit(x_shape, blk.downsample[0])
+            if ds is None:
+                r_shape = x_shape
+            elif bottleneck:
+                r_shape = unit(x_shape, ds[0])
+            else:
+                sd = ds[0].stride[0]
+                if not F_.shortcut_shape_supported(x_shape, tuple(ds[0].weight.shape), sd):
+                    return False
+                r_shape = (n, ds[0].out_channels, (x_shape[2] - 1) // sd + 1, (x_shape[3] - 1) // sd + 1)
             if r_shape != shape:
                 return False
         return True
 
+    # ---- training forward --------------------------------------------------------------------------------------
     def _train_forward(self, x):
-        # (conv, BatchNorm) pairs of each block: conv1, conv2, conv3 and the downsample's
-        units = [[(blk.conv1, blk.bn1), (blk.conv2, blk.bn2), (blk.conv3, blk.bn3)] +
-                 ([tuple(blk.downsample)] if blk.downsample is not None else []) for blk in self._blocks]
-        # 1x1 and 3x3 weights in one pack per forward, never cached: the optimizers update them in place (a ResNeXt's
-        # conv2 as its banded operands)
-        packs = iter(F_.real_weight_grad_pack([c.weight for u in units for c, _ in u],
-                                              groups=[c.groups for u in units for c, _ in u]))
+        # every weight in one pack per forward, never cached: the optimizers update them in place (a ResNeXt's conv2 as
+        # its banded operands)
+        packs = iter(F_.real_weight_grad_pack([c.weight for c in self._convs], groups=[c.groups for c in self._convs]))
         c1 = self.conv1
         z, z_amax = F_.stem_conv_bn_relu_pool(x, c1.weight, *_bn_train_args(self.bn1), *self._pool_args())
-        for blk, u in zip(self._blocks, units):
-            params = [t for c, bn in u for t in (c.weight, bn.weight, bn.bias)]
-            z, z_amax = F_.real_bottleneck(z, z_amax, [next(packs) for _ in u], params,
-                                           [_bn_train_args(bn)[2:] for _, bn in u], blk.conv2.stride[0],
-                                           blk.conv2.groups)
+        if self._family.bottleneck:
+            # each block one real_bottleneck node: its conv1, conv2, conv3 and downsample units
+            for units, ds in self._units:
+                units = units + ([tuple(ds)] if ds is not None else [])
+                params = [t for c, bn in units for t in (c.weight, bn.weight, bn.bias)]
+                conv2 = units[1][0]
+                z, z_amax = F_.real_bottleneck(z, z_amax, [next(packs) for _ in units], params,
+                                               [_bn_train_args(bn)[2:] for _, bn in units], conv2.stride[0],
+                                               conv2.groups)
+        else:
+            # a node per conv, the downsample on the shortcut unit
+            for ((conv1, bn1), (conv2, bn2)), ds in self._units:
+                res = z if ds is None else F_.shortcut_conv_bn(z, ds[0].weight, *_bn_train_args(ds[1]),
+                                                               ds[0].stride[0])
+                y, y_amax = F_.real_conv_bn_relu(z, z_amax, next(packs), conv1.weight, *_bn_train_args(bn1),
+                                                 conv1.stride[0])
+                z, z_amax = F_.real_conv_bn_relu(y, y_amax, next(packs), conv2.weight, *_bn_train_args(bn2), 1,
+                                                 residual=res)
         torch._foreach_add_([bn.num_batches_tracked for bn in self._bns()], 1)
         return self.fc(torch.flatten(self.avgpool(z), 1))
+
+
+class RealBottleneckResNet(RealResNet, FrozenBottleneckTeacher):
+    """A torchvision Bottleneck ResNet (exactly torchvision's ResNet with Bottleneck blocks, groups 1, no dilation:
+    resnet50/101/152, wide_resnet50_2/101_2) trained on the real-valued training units (DESIGN.md §4s), each block one
+    real_bottleneck node, with RealResNet's kernel-path conditions and fallback and FrozenBottleneckTeacher's eval
+    forward.  Raises TypeError for any other structure (BasicBlock ResNets, ResNeXt, replace_stride_with_dilation,
+    subclassed models or blocks, mixed blocks, nn.DataParallel), naming the module."""
+    _KINDS = ("bottleneck",)
 
 
 class RealResNeXt(RealBottleneckResNet, FrozenResNeXtTeacher):
     """A torchvision ResNeXt (resnext50_32x4d, resnext101_32x8d, resnext101_64x4d: exactly torchvision's ResNet with
     Bottleneck blocks whose conv2 all have groups == model.groups > 1) trained on the real-valued training units, each
     grouped conv2 on the banded kernels (DESIGN.md §4t), with RealBottleneckResNet's kernel-path conditions, fallback
-    and training forward and FrozenResNeXtTeacher's structure check and eval forward.  Raises TypeError, naming the
-    module, for any other structure (groups-1 Bottleneck ResNets, which RealBottleneckResNet wraps; BasicBlock ResNets,
+    and training forward and FrozenResNeXtTeacher's eval forward.  Raises TypeError, naming the module, for any other
+    structure (groups-1 Bottleneck ResNets, which RealBottleneckResNet wraps; BasicBlock ResNets,
     replace_stride_with_dilation, a conv2 with another group count, subclassed models or blocks, mixed blocks,
     nn.DataParallel)."""
-
-    def __init__(self, model):
-        who = "RealResNeXt"
-        _check_resnext(model, who, "RealBottleneckResNet")
-        try:
-            FrozenResNeXtTeacher.__init__(self, model)
-        except TypeError as e:      # the teacher's structure check: name the class the caller used
-            raise TypeError(str(e).replace("FrozenResNeXtTeacher", who)) from None
-        self.__dict__["_train_ok"] = {}
+    _KINDS = ("resnext",)

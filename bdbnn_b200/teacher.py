@@ -24,7 +24,12 @@ rounds it to fp16 on the way in (real_conv1x1_bn_eval, DESIGN.md §4q).  A ResNe
 GEMM (real_conv_bn_eval(groups=...), DESIGN.md §4t).  VGG-Small's Hardtanh is in the epilogue of
 its stem and of its unpooled convs; its pooled convs write their fp32 output and one more kernel takes the 2x2 max,
 BatchNorm and Hardtanh (DESIGN.md §4o).
-Anything else returns the wrapped model's own forward."""
+Anything else returns the wrapped model's own forward.
+
+The three ResNet teachers are one class for five kinds of network (_Family.kind: torchvision BasicBlock, CIFAR ResNet,
+CIFAR ResNet-18, Bottleneck, ResNeXt): FrozenResNetTeacher holds the structure check, the geometry walk and the kernel
+forward, which read each block's (conv, BatchNorm) units from one list, and FrozenBottleneckTeacher and
+FrozenResNeXtTeacher are subclasses whose body is the _KINDS they take.  _check_kind refuses any other kind."""
 import ctypes
 from typing import NamedTuple
 
@@ -39,6 +44,7 @@ from .vgg import VGGSmall
 
 class _Family(NamedTuple):
     """What the structure check, the geometry walk, the kernel forward and the launch count know of a network."""
+    kind: str           # the key of _KIND_TEXT; each wrapper class takes the kinds in its _KINDS
     children: tuple     # names of the model's children, in order
     block: type         # of every residual block
     pooled_stem: bool   # 7x7 / stride-2 conv + BatchNorm + ReLU + max-pool (stem_conv_bn_relu_pool_eval, 6 launches);
@@ -49,43 +55,89 @@ class _Family(NamedTuple):
     #                     _PadShortcut that conv1's epilogue reads in place (no launch)
     bireal: bool        # out = bn1(conv1(x)) + shortcut(x); out2 = bn2(conv2(out)) + out (Bi-Real: one shortcut per
     #                     conv); else out = bn1(conv1(x)); out2 = bn2(conv2(out)) + shortcut(x)
-    bottleneck: bool = False   # torchvision Bottleneck blocks: 1x1, 3x3 (the block's stride), 1x1 + shortcut(x)
+    bottleneck: bool = False   # torchvision Bottleneck blocks: 1x1, 3x3 (the block's stride), 1x1 + shortcut(x); the
+    #                            downsample runs as one more conv + BatchNorm unit, in the blocks' weight pack
+    groups: int = 1     # of every Bottleneck's conv2: 1, or a ResNeXt's model.groups (conv2 on the banded kernels)
 
 
+# what the refusals call each kind
+_KIND_TEXT = {"basic": "torchvision BasicBlock ResNets (resnet18/34)",
+              "cifar": "the fp32 bdbnn_b200.resnet.ResNetCifar",
+              "cifar18": "the fp32 bdbnn_b200.resnet.ResNetCifar18",
+              "bottleneck": "torchvision Bottleneck ResNets (resnet50/101/152, wide_resnet50_2/101_2)",
+              "resnext": "torchvision ResNeXts (resnext50_32x4d, resnext101_32x8d, resnext101_64x4d)"}
 _LAYERS = ("layer1", "layer2", "layer3", "layer4")
-_CIFAR = _Family(("conv1", "bn1") + _LAYERS[:3] + ("avgpool", "fc"), BasicBlockCifar, False, False, "shortcut", True)
-_CIFAR18 = _Family(("conv1", "bn1") + _LAYERS + ("avgpool", "fc"), BasicBlock, False, False, "downsample", True)
+_CIFAR = _Family("cifar", ("conv1", "bn1") + _LAYERS[:3] + ("avgpool", "fc"), BasicBlockCifar, False, False,
+                 "shortcut", True)
+_CIFAR18 = _Family("cifar18", ("conv1", "bn1") + _LAYERS + ("avgpool", "fc"), BasicBlock, False, False, "downsample",
+                   True)
+
+
+def _first_block(model):
+    layer1 = getattr(model, "layer1", None)
+    return layer1[0] if type(layer1) is nn.Sequential and len(layer1) > 0 else None
 
 
 def _family(model):
-    """The _Family of `model` by its exact type: a subclass or a wrapper (nn.DataParallel) is refused."""
+    """The _Family of `model` by its exact type, or None: a subclass or a wrapper (nn.DataParallel) is no family.  A
+    torchvision ResNet's kind is that of layer1's first block (_blocks then asks every block to be exactly that type):
+    for a Bottleneck "bottleneck", or "resnext" when its conv2 is grouped, every conv2 then with model.groups groups;
+    else "basic"."""
     if type(model) is ResNetCifar:
         return _CIFAR
     if type(model) is ResNetCifar18:
         return _CIFAR18
     from torchvision.models import resnet as tv
     if type(model) is not tv.ResNet:
-        raise TypeError(f"FrozenResNetTeacher wraps a torchvision ResNet with BasicBlocks (resnet18/34) or an fp32 "
-                        f"bdbnn_b200.resnet.ResNetCifar / ResNetCifar18, FrozenBottleneckTeacher a torchvision ResNet "
-                        f"with Bottlenecks (resnet50/101/152, wide_resnet50_2/101_2), got {type(model).__name__}")
-    # the kind of layer1's first block; _blocks then asks every block to be exactly that type
-    layer1 = getattr(model, "layer1", None)
-    first = layer1[0] if type(layer1) is nn.Sequential and len(layer1) > 0 else None
-    bottleneck = type(first) is tv.Bottleneck
-    return _Family(("conv1", "bn1", "relu", "maxpool") + _LAYERS + ("avgpool", "fc"),
-                   tv.Bottleneck if bottleneck else tv.BasicBlock, True, True, "downsample", False, bottleneck)
+        return None
+    children = ("conv1", "bn1", "relu", "maxpool") + _LAYERS + ("avgpool", "fc")
+    first = _first_block(model)
+    if type(first) is not tv.Bottleneck:
+        return _Family("basic", children, tv.BasicBlock, True, True, "downsample", False)
+    if getattr(getattr(first, "conv2", None), "groups", 1) == 1:
+        return _Family("bottleneck", children, tv.Bottleneck, True, True, "downsample", False, True)
+    return _Family("resnext", children, tv.Bottleneck, True, True, "downsample", False, True,
+                   max(getattr(model, "groups", 1), 1))
+
+
+# the kinds in the order the ResNet wrappers derive from one another: a refusal points one step along it only (a change
+# of block, BasicBlock <-> Bottleneck, or of groups, Bottleneck <-> ResNeXt)
+_STEP = {"basic": 0, "cifar": 0, "cifar18": 0, "bottleneck": 1, "resnext": 2}
+
+
+def _check_kind(model, cls):
+    """The _Family of `model` when its kind is one of cls._KINDS, else TypeError naming cls, what it wraps, what
+    `model` is and, when there is one, the class to wrap it in instead (cls._WRAPPER_OF, one step away, and only when
+    layer1.0 is exactly the block of the model's kind, so that the class named takes that kind)."""
+    fam = _family(model)
+    if fam is not None and fam.kind in cls._KINDS:
+        return fam
+    first = _first_block(model)
+    if fam is None or not fam.pooled_stem:
+        what = f"got {type(model).__name__}"
+    elif fam.bottleneck:
+        groups = getattr(getattr(first, "conv2", None), "groups", 1)
+        what = f"layer1.0 is a Bottleneck and layer1.0.conv2 has groups {groups}"
+    else:
+        what = f"layer1.0 is a {type(first).__name__}"
+    use = None
+    if fam is not None and type(first) is fam.block and min(abs(_STEP[fam.kind] - _STEP[k])
+                                                            for k in cls._KINDS) == 1:
+        use = cls._WRAPPER_OF.get(fam.kind)
+    raise TypeError(f"{cls.__name__} wraps {', '.join(_KIND_TEXT[k] for k in cls._KINDS)}; {what}" +
+                    (f": wrap it in {use}" if use else ""))
 
 
 def _bn_args(bn):
     return bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps
 
 
-def _check_bn(bn, where, who="FrozenResNetTeacher"):
+def _check_bn(bn, where, who):
     if type(bn) is not nn.BatchNorm2d:
         raise TypeError(f"{who}: {where} must be nn.BatchNorm2d, got {type(bn).__name__}")
 
 
-def _check_conv(conv, where, k, bias=False, who="FrozenResNetTeacher", net="a BasicBlock ResNet", groups=1):
+def _check_conv(conv, where, k, who, bias=False, net="a BasicBlock ResNet", groups=1):
     if type(conv) is not nn.Conv2d:
         raise TypeError(f"{who}: {where} must be nn.Conv2d, got {type(conv).__name__}")
     if (conv.kernel_size != (k, k) or conv.groups != groups or conv.dilation != (1, 1) or (conv.bias is not None) != bias
@@ -93,29 +145,29 @@ def _check_conv(conv, where, k, bias=False, who="FrozenResNetTeacher", net="a Ba
         raise TypeError(f"{who}: {where} is not a {k}x{k} conv of {net}")
 
 
-def _check_stem(model, fam):
+def _check_stem(model, fam, who):
     c1 = model.conv1
     if fam.pooled_stem:
-        _check_conv(c1, "conv1", 7)
+        _check_conv(c1, "conv1", 7, who)
         if c1.stride != (2, 2) or c1.padding != (3, 3) or c1.in_channels != 3:
-            raise TypeError("FrozenResNetTeacher: conv1 must be the 7x7 / stride-2 / pad-3 stem on 3 channels")
-        _check_bn(model.bn1, "bn1")
+            raise TypeError(f"{who}: conv1 must be the 7x7 / stride-2 / pad-3 stem on 3 channels")
+        _check_bn(model.bn1, "bn1", who)
         mp = model.maxpool
         if type(model.relu) is not nn.ReLU or type(mp) is not nn.MaxPool2d or mp.ceil_mode or mp.dilation != 1 \
                 or mp.return_indices:
-            raise TypeError("FrozenResNetTeacher: the stem must end in nn.ReLU and nn.MaxPool2d")
+            raise TypeError(f"{who}: the stem must end in nn.ReLU and nn.MaxPool2d")
     else:
-        _check_conv(c1, "conv1", 3)
+        _check_conv(c1, "conv1", 3, who)
         if c1.in_channels != 3 or not F_.cifar_stem_supported((1, 3, 1, 1), tuple(c1.weight.shape), c1.stride,
                                                               c1.padding):
-            raise TypeError("FrozenResNetTeacher: conv1 must be the 3x3 / stride-1 / pad-1 CIFAR stem on 3 channels "
-                            "with 16, 32, 48 or 64 outputs")
-        _check_bn(model.bn1, "bn1")
+            raise TypeError(f"{who}: conv1 must be the 3x3 / stride-1 / pad-1 CIFAR stem on 3 channels with 16, 32, 48 "
+                            "or 64 outputs")
+        _check_bn(model.bn1, "bn1", who)
         if fam is _CIFAR18 and c1.out_channels != 64:
-            raise TypeError("FrozenResNetTeacher: the CIFAR ResNet-18 stem must have 64 outputs")
+            raise TypeError(f"{who}: the CIFAR ResNet-18 stem must have 64 outputs")
 
 
-def _check_shortcut(blk, where, fam):
+def _check_shortcut(blk, where, fam, who):
     sc = getattr(blk, fam.shortcut)
     conv1 = blk.conv1
     cin, cout = conv1.in_channels, conv1.out_channels
@@ -123,91 +175,97 @@ def _check_shortcut(blk, where, fam):
     own = fam is _CIFAR or fam is _CIFAR18
     if sc is None:
         if own and (conv1.stride != (1, 1) or cin != cout):
-            raise TypeError(f"FrozenResNetTeacher: {where} changes shape but has no {fam.shortcut}")
+            raise TypeError(f"{who}: {where} changes shape but has no {fam.shortcut}")
     elif fam.shortcut == "shortcut":
         if type(sc) is not _PadShortcut or not F_.pad_shortcut_supported((1, cin, 1, 1), tuple(conv1.weight.shape),
                                                                          conv1.stride[0], sc.pad):
-            raise TypeError(f"FrozenResNetTeacher: {where}.shortcut must be the option-A _PadShortcut of a stride-2 "
-                            "conv1 with Cout = Cin + 2 * pad (multiples of 4)")
+            raise TypeError(f"{who}: {where}.shortcut must be the option-A _PadShortcut of a stride-2 conv1 with "
+                            "Cout = Cin + 2 * pad (multiples of 4)")
     else:
         if type(sc) is not nn.Sequential or len(sc) != 2:
-            raise TypeError(f"FrozenResNetTeacher: {where}.downsample must be Sequential(1x1 Conv2d, BatchNorm2d)")
-        _check_conv(sc[0], where + ".downsample.0", 1)
+            raise TypeError(f"{who}: {where}.downsample must be Sequential(1x1 Conv2d, BatchNorm2d)")
+        _check_conv(sc[0], where + ".downsample.0", 1, who)
         if sc[0].padding != (0, 0):
-            raise TypeError(f"FrozenResNetTeacher: {where}.downsample.0 must have no padding")
+            raise TypeError(f"{who}: {where}.downsample.0 must have no padding")
         if own and (sc[0].stride != conv1.stride or sc[0].in_channels != cin or sc[0].out_channels != cout):
-            raise TypeError(f"FrozenResNetTeacher: {where}.downsample.0 must map conv1's input to its output shape")
-        _check_bn(sc[1], where + ".downsample.1")
+            raise TypeError(f"{who}: {where}.downsample.0 must map conv1's input to its output shape")
+        _check_bn(sc[1], where + ".downsample.1", who)
 
 
-def _check_bottleneck(blk, where, groups=1):
+def _check_bottleneck(blk, where, groups, who):
     """conv1 1x1, conv2 3x3 with the block's stride (`groups` groups, dilation 1: no replace_stride_with_dilation;
     groups 1 refuses ResNeXt), conv3 1x1, bn3 BatchNorm2d, and a downsample, if any, with the block's stride.  A
     grouped conv2 maps C channels to C with a group width the banded kernels take (DESIGN.md §4t)."""
     net = "a Bottleneck ResNet" if groups == 1 else f"a ResNeXt with {groups} groups"
     for name, k in (("conv1", 1), ("conv2", 3), ("conv3", 1)):
-        _check_conv(getattr(blk, name), f"{where}.{name}", k, net=net, groups=groups if name == "conv2" else 1)
+        _check_conv(getattr(blk, name), f"{where}.{name}", k, who, net=net, groups=groups if name == "conv2" else 1)
     if groups != 1:
         c = blk.conv2.in_channels
         band = F_.gconv_band(c, groups)
         if blk.conv2.out_channels != c or c % groups or band > 64 or band % (c // groups) or c % band:
-            raise TypeError(f"FrozenResNetTeacher: {where}.conv2 ({c} -> {blk.conv2.out_channels} channels, {groups} "
-                            "groups) has no banded kernel: it needs Cin = Cout and a group width dividing 16, 32 or 64")
+            raise TypeError(f"{who}: {where}.conv2 ({c} -> {blk.conv2.out_channels} channels, {groups} groups) has no "
+                            "banded kernel: it needs Cin = Cout and a group width dividing 16, 32 or 64")
     s = blk.conv2.stride
     if s not in ((1, 1), (2, 2)) or blk.conv2.padding != (1, 1):
-        raise TypeError(f"FrozenResNetTeacher: {where}.conv2 must be a pad-1 3x3 conv of stride 1 or 2")
+        raise TypeError(f"{who}: {where}.conv2 must be a pad-1 3x3 conv of stride 1 or 2")
     for name in ("conv1", "conv3"):
         c = getattr(blk, name)
         if c.stride != (1, 1) or c.padding != (0, 0):
-            raise TypeError(f"FrozenResNetTeacher: {where}.{name} must be a stride-1 / pad-0 1x1 conv")
-    _check_bn(blk.bn3, where + ".bn3")
+            raise TypeError(f"{who}: {where}.{name} must be a stride-1 / pad-0 1x1 conv")
+    _check_bn(blk.bn3, where + ".bn3", who)
     ds = blk.downsample
     if type(ds) is nn.Sequential and len(ds) == 2 and type(ds[0]) is nn.Conv2d and ds[0].stride != s:
-        raise TypeError(f"FrozenResNetTeacher: {where}.downsample.0 must have conv2's stride {s}")
+        raise TypeError(f"{who}: {where}.downsample.0 must have conv2's stride {s}")
 
 
-def _blocks(model, groups=1):
-    """(family, [(name, block)] of the residual blocks) after checking that `model` is a torchvision BasicBlock or
-    Bottleneck ResNet, or a ResNetCifar or ResNetCifar18 with nn.Conv2d convs throughout: the fp32 teachers.  A CIFAR
-    shell with binary convs is a student, whose eval forward has its own units.  groups > 1: a ResNeXt, every
-    Bottleneck's conv2 with exactly that many groups."""
-    fam = _family(model)
+def _blocks(model, fam, who):
+    """[(name, block)] of the residual blocks after checking that `model`, of family `fam`, is a torchvision BasicBlock
+    or Bottleneck ResNet or ResNeXt (every conv2 with fam.groups groups), or a ResNetCifar or ResNetCifar18 with
+    nn.Conv2d convs throughout: the fp32 teachers.  A CIFAR shell with binary convs is a student, whose eval forward has
+    its own units.  `who` is the class the refusals name."""
     names = [n for n, _ in model.named_children()]
     if names != list(fam.children):
-        raise TypeError(f"FrozenResNetTeacher: unexpected children {names}")
+        raise TypeError(f"{who}: unexpected children {names}")
     if list(model.named_parameters(recurse=False)) or list(model.named_buffers(recurse=False)):
-        raise TypeError("FrozenResNetTeacher: the model itself must hold no parameters or buffers")
-    _check_stem(model, fam)
+        raise TypeError(f"{who}: the model itself must hold no parameters or buffers")
+    _check_stem(model, fam, who)
     if type(model.avgpool) is not nn.AdaptiveAvgPool2d or type(model.fc) is not nn.Linear:
-        raise TypeError("FrozenResNetTeacher: the head must be nn.AdaptiveAvgPool2d and nn.Linear")
+        raise TypeError(f"{who}: the head must be nn.AdaptiveAvgPool2d and nn.Linear")
     out = []
     for lname in (n for n in fam.children if n in _LAYERS):
         layer = getattr(model, lname)
         if type(layer) is not nn.Sequential:
-            raise TypeError(f"FrozenResNetTeacher: {lname} must be nn.Sequential")
+            raise TypeError(f"{who}: {lname} must be nn.Sequential")
         for bi, blk in layer.named_children():
             where = f"{lname}.{bi}"
             if type(blk) is not fam.block:
-                raise TypeError(f"FrozenResNetTeacher: {where} is a {type(blk).__name__}; only "
+                raise TypeError(f"{who}: {where} is a {type(blk).__name__}; only "
                                 f"{fam.block.__module__}.{fam.block.__name__} is supported")
             # the Bi-Real BasicBlock has no other child (a `relu`, say, would never run on the kernel path)
             if fam is _CIFAR18 and [n for n, _ in blk.named_children()] != ["conv1", "bn1", "conv2", "bn2"] + (
                     ["downsample"] if blk.downsample is not None else []):
-                raise TypeError(f"FrozenResNetTeacher: {where} has unexpected children")
+                raise TypeError(f"{who}: {where} has unexpected children")
             if fam.bottleneck:
-                _check_bottleneck(blk, where, groups)
+                _check_bottleneck(blk, where, fam.groups, who)
             else:
-                _check_conv(blk.conv1, where + ".conv1", 3)
-                _check_conv(blk.conv2, where + ".conv2", 3)
+                _check_conv(blk.conv1, where + ".conv1", 3, who)
+                _check_conv(blk.conv2, where + ".conv2", 3, who)
                 if blk.conv2.stride != (1, 1) or blk.conv1.padding != (1, 1) or blk.conv2.padding != (1, 1):
-                    raise TypeError(f"FrozenResNetTeacher: {where} convs are not the {fam.block.__name__}'s")
-            _check_bn(blk.bn1, where + ".bn1")
-            _check_bn(blk.bn2, where + ".bn2")
+                    raise TypeError(f"{who}: {where} convs are not the {fam.block.__name__}'s")
+            _check_bn(blk.bn1, where + ".bn1", who)
+            _check_bn(blk.bn2, where + ".bn2", who)
             if fam.relu and type(blk.relu) is not nn.ReLU:
-                raise TypeError(f"FrozenResNetTeacher: {where}.relu must be nn.ReLU")
-            _check_shortcut(blk, where, fam)
+                raise TypeError(f"{who}: {where}.relu must be nn.ReLU")
+            _check_shortcut(blk, where, fam, who)
             out.append((where, blk))
-    return fam, out
+    return out
+
+
+def _units(blk, fam):
+    """([(conv, BatchNorm)] of `blk`'s main path, in the order the kernels run them, and its shortcut: None, the
+    option-A _PadShortcut, or the `downsample` Sequential(conv, BatchNorm))."""
+    names = ("1", "2", "3") if fam.bottleneck else ("1", "2")
+    return [(getattr(blk, "conv" + i), getattr(blk, "bn" + i)) for i in names], getattr(blk, fam.shortcut)
 
 
 class _FrozenTeacher(nn.Module):
@@ -264,25 +322,27 @@ class FrozenResNetTeacher(_FrozenTeacher):
     """A torchvision resnet18 / resnet34 teacher, or an fp32 CIFAR ResNet (ResNetCifar with nn.Conv2d convs, any
     depth and class count, or ResNetCifar18 with nn.Conv2d convs, any class count), whose eval forward runs on the
     real-valued eval kernels.  Raises TypeError for any other structure (a Bottleneck ResNet, which
-    FrozenBottleneckTeacher wraps; binary convs, nn.DataParallel, custom blocks)."""
-    _BOTTLENECK = False     # the block kind this class wraps
+    FrozenBottleneckTeacher wraps; binary convs, nn.DataParallel, custom blocks).  Its subclasses share its structure
+    check, geometry walk and eval forward, each for the kinds of network in its _KINDS."""
+    _KINDS = ("basic", "cifar", "cifar18")     # the _Family kinds this class wraps
+    # the teacher of each kind, which a refusal names instead
+    _WRAPPER_OF = {"basic": "FrozenResNetTeacher", "cifar": "FrozenResNetTeacher", "cifar18": "FrozenResNetTeacher",
+                   "bottleneck": "FrozenBottleneckTeacher", "resnext": "FrozenResNeXtTeacher"}
 
     def __init__(self, model):
-        if _family(model).bottleneck != self._BOTTLENECK:
-            raise TypeError("FrozenResNetTeacher wraps BasicBlock ResNets and the CIFAR ResNets; wrap a torchvision "
-                            "Bottleneck ResNet in FrozenBottleneckTeacher" if not self._BOTTLENECK else
-                            "FrozenBottleneckTeacher wraps torchvision Bottleneck ResNets (resnet50/101/152, "
-                            "wide_resnet50_2/101_2); wrap a BasicBlock or CIFAR ResNet in FrozenResNetTeacher")
-        family, blocks = _blocks(model, self._conv2_groups(model))
+        family = _check_kind(model, type(self))
+        blocks = _blocks(model, family, type(self).__name__)
         super().__init__(model)
         self.__dict__["_family"] = family
         self.__dict__["_blocks"] = [blk for _, blk in blocks]
-        self.__dict__["_convs"] = [c for blk in self._blocks for c in (blk.conv1, blk.conv2)]
-
-    @staticmethod
-    def _conv2_groups(model):
-        """The group count every Bottleneck conv2 must have: 1 (FrozenResNeXtTeacher asks for the model's)."""
-        return 1
+        self.__dict__["_units"] = [_units(blk, family) for blk in self._blocks]
+        # the weights of the one real-valued weight pack per forward, in pack order: each block's main path, and a
+        # Bottleneck's downsample, which runs as one more unit (a BasicBlock's runs on the shortcut GEMM, which packs
+        # its own weight)
+        convs = []
+        for units, sc in self._units:
+            convs += [c for c, _ in units] + ([sc[0]] if family.bottleneck and sc is not None else [])
+        self.__dict__["_convs"] = convs
 
     @property
     def _cifar(self):
@@ -306,7 +366,7 @@ class FrozenResNetTeacher(_FrozenTeacher):
         return tuple(out)
 
     def _geometry_supported(self, x):
-        """The stem, every 3x3 conv and every shortcut of the network have their kernel at this input size (host-only
+        """The stem, every conv and every shortcut of the network have their kernel at this input size (host-only
         checks, cached).  The max-pool's arguments are part of the key: they are read at every forward, so a
         `maxpool` assigned after wrapping is seen."""
         pool = self._pool_args() if self._family.pooled_stem else ()
@@ -331,37 +391,26 @@ class FrozenResNetTeacher(_FrozenTeacher):
             shape = (n, c1.out_channels, h, w)
         L = _lib.lib()
         fwd_ok = lambda sh: sh.Cin % 4 == 0 and bool(int(L.bdbnn_tc_supported(ctypes.byref(sh))) & 1)
-        if fam.bottleneck:
-            # every conv on the pack + GEMM path, and every 1x1 conv on the GEMM that reads fp32 (either arm of
-            # BDBNN_TEACHER_F32A runs)
-            conv_ok = lambda sh: fwd_ok(sh) and (sh.kh != 1 or F_.real_gemm1x1_supported(sh))
-            for blk in self._blocks:
-                if not ok:
-                    break
-                x_shape = shape
-                for conv in (blk.conv1, blk.conv2, blk.conv3):
-                    g = conv.groups
-                    sh = F_.gconv_shape(shape, conv.weight.shape, conv.stride[0], conv.padding[0], g)
-                    ok = ok and (conv_ok(sh) if g == 1 else sh.Cin % 4 == 0 and bool(F_.real_gconv_supported(sh, g) & 32))
-                    shape = (n, sh.Cout, sh.Ho, sh.Wo)
-                ds = blk.downsample
-                if ds is not None:
-                    sh = F_.conv_shape(x_shape, ds[0].weight.shape, ds[0].stride[0], 0)
-                    ok = ok and conv_ok(sh) and (n, sh.Cout, sh.Ho, sh.Wo) == shape
-            return ok
-        for blk in self._blocks:
+        # every conv on the pack + GEMM path, and every 1x1 conv (a Bottleneck's) on the GEMM that reads fp32 too
+        # (either arm of BDBNN_TEACHER_F32A runs); a grouped conv on the banded GEMM
+        conv_ok = lambda sh: fwd_ok(sh) and (sh.kh != 1 or F_.real_gemm1x1_supported(sh))
+        for units, sc in self._units:
             if not ok:
                 break
             x_shape = shape
-            for conv in (blk.conv1, blk.conv2):
-                sh = F_.conv_shape(shape, conv.weight.shape, conv.stride[0], conv.padding[0])
-                ok = ok and fwd_ok(sh)
+            for conv, _ in units:
+                g = conv.groups
+                sh = F_.gconv_shape(shape, conv.weight.shape, conv.stride[0], conv.padding[0], g)
+                ok = ok and (conv_ok(sh) if g == 1 else sh.Cin % 4 == 0 and bool(F_.real_gconv_supported(sh, g) & 32))
                 shape = (n, sh.Cout, sh.Ho, sh.Wo)
-            sc = getattr(blk, fam.shortcut)
             if sc is None:
                 continue
             if fam.shortcut == "shortcut":       # the option-A residual of conv1, read in place
-                ok = ok and F_.pad_shortcut_supported(x_shape, blk.conv1.weight.shape, blk.conv1.stride[0], sc.pad)
+                conv1 = units[0][0]
+                ok = ok and F_.pad_shortcut_supported(x_shape, conv1.weight.shape, conv1.stride[0], sc.pad)
+            elif fam.bottleneck:                 # one more conv on the pack + GEMM path, to the block's output shape
+                sh = F_.conv_shape(x_shape, sc[0].weight.shape, sc[0].stride[0], 0)
+                ok = ok and conv_ok(sh) and (n, sh.Cout, sh.Ho, sh.Wo) == shape
             else:                                # the 1x1 GEMM over the strided samples (shortcut_eval_supported)
                 sd = sc[0].stride[0]
                 sampled = (n, x_shape[1], (x_shape[2] - 1) // sd + 1, (x_shape[3] - 1) // sd + 1)
@@ -375,12 +424,12 @@ class FrozenResNetTeacher(_FrozenTeacher):
             z, z_amax = F_.stem_conv_bn_relu_pool_eval(x, self.conv1.weight, *_bn_args(self.bn1), *self._pool_args())
         else:
             z, z_amax = F_.cifar_stem_conv_bn_eval(x, self.conv1.weight, *_bn_args(self.bn1))
+        # packed at every forward, never cached: a load_state_dict or an in-place update is always seen (a ResNeXt's
+        # conv2 as its banded operand)
+        packs = iter(F_.real_weight_pack([c.weight for c in self._convs], [c.groups for c in self._convs]))
         if fam.bottleneck:
-            return self._bottleneck_forward(z, z_amax)
-        # packed at every forward, never cached: a load_state_dict or an in-place update is always seen
-        packs = F_.real_weight_pack([c.weight for c in self._convs])
-        for i, blk in enumerate(self._blocks):
-            sc = getattr(blk, fam.shortcut)
+            return self._bottleneck_forward(z, z_amax, packs)
+        for ((conv1, bn1), (_, bn2)), sc in self._units:
             if sc is None:
                 res = dict(residual=z)
             elif fam.shortcut == "shortcut":
@@ -388,13 +437,13 @@ class FrozenResNetTeacher(_FrozenTeacher):
             else:
                 res = dict(residual=F_._shortcut_eval_impl(z, sc[0].weight, *_bn_args(sc[1]), sc[0].stride[0]))
             # the shortcut is conv1's residual and conv1's output is conv2's on a Bi-Real block, else it is conv2's
-            y, y_amax = F_.real_conv_bn_eval(z, z_amax, packs[2 * i], *_bn_args(blk.bn1), blk.conv1.stride[0],
-                                             blk.conv1.padding[0], relu=fam.relu, **(res if fam.bireal else {}))
-            z, z_amax = F_.real_conv_bn_eval(y, y_amax, packs[2 * i + 1], *_bn_args(blk.bn2), 1, 1, relu=fam.relu,
+            y, y_amax = F_.real_conv_bn_eval(z, z_amax, next(packs), *_bn_args(bn1), conv1.stride[0], conv1.padding[0],
+                                             relu=fam.relu, **(res if fam.bireal else {}))
+            z, z_amax = F_.real_conv_bn_eval(y, y_amax, next(packs), *_bn_args(bn2), 1, 1, relu=fam.relu,
                                              **(dict(residual=y) if fam.bireal else res))
         return self.fc(torch.flatten(self.avgpool(z), 1))
 
-    def _bottleneck_forward(self, z, z_amax):
+    def _bottleneck_forward(self, z, z_amax, packs):
         """out = relu(bn1(conv1(x))); out = relu(bn2(conv2(out))); out = relu(bn3(conv3(out)) + shortcut(x)), the
         shortcut x or bn(downsample conv(x)).  The 1x1 convs pack their input first, or with BDBNN_TEACHER_F32A=1 read
         it as fp32 in the GEMM (the same logits bit for bit)."""
@@ -403,22 +452,15 @@ class FrozenResNetTeacher(_FrozenTeacher):
         else:
             def conv1x1(x, x_amax, pack, *bn, stride, residual=None, relu=True):
                 return F_.real_conv_bn_eval(x, x_amax, pack, *bn, stride, 0, residual=residual, relu=relu)
-        convs = []
-        for blk in self._blocks:
-            convs += [blk.conv1, blk.conv2, blk.conv3] + ([blk.downsample[0]] if blk.downsample is not None else [])
-        # 1x1 and 3x3 weights in one pack, at every forward, never cached (a ResNeXt's conv2 as its banded operand)
-        packs = iter(F_.real_weight_pack([c.weight for c in convs], [c.groups for c in convs]))
-        for blk in self._blocks:
+        for ((_, bn1), (c2, bn2), (_, bn3)), ds in self._units:
             p1, p2, p3 = next(packs), next(packs), next(packs)
-            ds = blk.downsample
             if ds is None:
                 res = z
             else:
                 res, _ = conv1x1(z, z_amax, next(packs), *_bn_args(ds[1]), stride=ds[0].stride[0], relu=False)
-            y, y_amax = conv1x1(z, z_amax, p1, *_bn_args(blk.bn1), stride=1)
-            y, y_amax = F_.real_conv_bn_eval(y, y_amax, p2, *_bn_args(blk.bn2), blk.conv2.stride[0], 1,
-                                             groups=blk.conv2.groups)
-            z, z_amax = conv1x1(y, y_amax, p3, *_bn_args(blk.bn3), stride=1, residual=res)
+            y, y_amax = conv1x1(z, z_amax, p1, *_bn_args(bn1), stride=1)
+            y, y_amax = F_.real_conv_bn_eval(y, y_amax, p2, *_bn_args(bn2), c2.stride[0], 1, groups=c2.groups)
+            z, z_amax = conv1x1(y, y_amax, p3, *_bn_args(bn3), stride=1, residual=res)
         return self.fc(torch.flatten(self.avgpool(z), 1))
 
 
@@ -428,7 +470,7 @@ class FrozenBottleneckTeacher(FrozenResNetTeacher):
     (DESIGN.md §4q), with FrozenResNetTeacher's names, parameters, kernel-path conditions and fallback.  Raises
     TypeError for any other structure (ResNeXt, dilated ResNets, mixed or subclassed blocks, BasicBlock ResNets,
     nn.DataParallel)."""
-    _BOTTLENECK = True
+    _KINDS = ("bottleneck",)
 
 
 class FrozenResNeXtTeacher(FrozenBottleneckTeacher):
@@ -439,32 +481,8 @@ class FrozenResNeXtTeacher(FrozenBottleneckTeacher):
     TypeError, naming the module, for any other structure (groups-1 Bottleneck ResNets, which FrozenBottleneckTeacher
     wraps; replace_stride_with_dilation, a conv2 with another group count, mixed or subclassed blocks, subclassed
     models, nn.DataParallel)."""
+    _KINDS = ("resnext",)
 
-    def __init__(self, model):
-        _check_resnext(model, "FrozenResNeXtTeacher", "FrozenBottleneckTeacher")
-        try:
-            super().__init__(model)
-        except TypeError as e:      # the structure check: name the class the caller used
-            raise TypeError(str(e).replace("FrozenResNetTeacher", "FrozenResNeXtTeacher")) from None
-
-    @staticmethod
-    def _conv2_groups(model):
-        return model.groups
-
-
-def _check_resnext(model, who, dense_who):
-    """Raise TypeError unless `model` is exactly a torchvision ResNet of Bottlenecks with model.groups > 1."""
-    from torchvision.models import resnet as tv
-    if type(model) is not tv.ResNet:
-        raise TypeError(f"{who} wraps a torchvision ResNeXt (resnext50_32x4d, resnext101_32x8d, resnext101_64x4d), got "
-                        f"{type(model).__name__}")
-    layer1 = getattr(model, "layer1", None)
-    first = layer1[0] if type(layer1) is nn.Sequential and len(layer1) > 0 else None
-    if type(first) is not tv.Bottleneck:
-        raise TypeError(f"{who} wraps torchvision ResNeXts; layer1.0 is a {type(first).__name__}")
-    if getattr(model, "groups", 1) <= 1:
-        raise TypeError(f"{who} wraps torchvision ResNeXts; this ResNet has groups 1 (layer1.0.conv2 is not grouped): "
-                        f"wrap it in {dense_who}")
 
 
 _VGG_CHILDREN = ("conv0", "bn0", "conv1", "pooling", "bn1", "conv2", "bn2", "conv3", "bn3", "conv4", "bn4", "conv5",
@@ -575,12 +593,14 @@ def launches_per_forward(model):
         _check_vgg(m)
         return 2 + 2 + sum(4 if pooled else 3 for pooled in _VGG_POOLED)
     fam = _family(m)
+    if fam is None:
+        raise TypeError(f"launches_per_forward: no kernel forward for a {type(m).__name__}")
     blocks = [b for b in m.modules() if type(b) is fam.block]
     if fam.bottleneck:
         n_ds = sum(1 for b in blocks if b.downsample is not None)
         n1 = 2 * len(blocks) + n_ds
         # a ResNeXt's pack: its dense weights and its grouped conv2s each 2 launches per 48 (DESIGN.md §4t)
-        n_pack = (2 * ((n1 + 47) // 48) + 2 * ((len(blocks) + 47) // 48) if m.groups > 1 else
+        n_pack = (2 * ((n1 + 47) // 48) + 2 * ((len(blocks) + 47) // 48) if fam.groups > 1 else
                   2 * ((n1 + len(blocks) + 47) // 48))
         return n_pack + 6 + 3 * len(blocks) + (2 if F_.teacher_f32a_enabled() else 3) * n1
     n3 = 2 * len(blocks)

@@ -1,5 +1,6 @@
-"""Seeded workloads of the binary-conv units, the train steps, the eval forwards and the frozen teachers, and the
-recorder of what they ask of the C ABI (tests/golden/make_launch_trace.py, tests/test_gpu_launch_trace.py).
+"""Seeded workloads of the binary-conv units, the train steps, the eval forwards, the frozen teachers and the
+torchvision fp32 ResNet wrappers (training forward + backward, eval forward), and the recorder of what they ask of
+the C ABI (tests/golden/make_launch_trace.py, tests/test_gpu_launch_trace.py).
 
 The trace lists, in host order:
   ["call", name, args]     every bdbnn_* call made through _lib.lib(): integer and float arguments as they are, the
@@ -22,6 +23,7 @@ SETTINGS = {
     "conv_stats_0": {"BDBNN_CONV_STATS": "0"},
     "fwd8_0": {"BDBNN_FWD8": "0"},
     "bf16x2": {"BDBNN_GRAD_MODE": "bf16x2"},
+    "teacher_f32a": {"BDBNN_TEACHER_F32A": "1"},
 }
 
 _BYREF = type(ctypes.byref(ctypes.c_int()))
@@ -198,6 +200,46 @@ def _teacher_forward(net, n):
     return run
 
 
+# torchvision's fp32 ResNets: the smallest input every unit of resnet18, resnet50 and resnext50_32x4d takes (the stem's
+# minimum), 10 classes
+_TV_N, _TV_HW = 1, 7
+
+
+def _tv_wrapped(wrapper, net, seed):
+    import torchvision
+    import bdbnn_b200
+    torch.manual_seed(seed)
+    m = _random_bn_(getattr(torchvision.models, net)(num_classes=10), seed + 1)
+    return getattr(bdbnn_b200, wrapper)(m.cuda().to(memory_format=torch.channels_last))
+
+
+def _tv_input(seed):
+    return _cl(torch.randn(_TV_N, 3, _TV_HW, _TV_HW, generator=torch.Generator().manual_seed(seed)))
+
+
+def _tv_train(wrapper, net):
+    def run():
+        from bdbnn_b200.functional import grad_mode
+        model = _tv_wrapped(wrapper, net, 11).train()
+        x = _tv_input(12)
+        if grad_mode()[0] != "fp16s":       # the training units take the fp16s gradient mode only
+            assert not model.kernel_path(x)
+            return
+        assert model.kernel_path(x)
+        model(x).square().sum().backward()
+    return run
+
+
+def _tv_eval(wrapper, net):
+    def run():
+        model = _tv_wrapped(wrapper, net, 13).eval()
+        x = _tv_input(14)
+        with torch.no_grad():
+            assert model.kernel_path(x)
+            model(x)
+    return run
+
+
 WORKLOADS = {
     "binconv2d_tc": _binconv((4, 64, 14, 14), (64, 64, 3, 3)),
     "binconv2d_tc_stride2": _binconv((4, 64, 14, 14), (128, 64, 3, 3), stride=2),
@@ -214,6 +256,13 @@ WORKLOADS = {
     "teacher_resnet20": _teacher_forward("resnet20", 8),
     "teacher_resnet18_cifar": _teacher_forward("resnet18_cifar", 8),
     "teacher_vgg_small": _teacher_forward("vgg_small", 8),
+    "train_real_resnet18": _tv_train("RealResNet", "resnet18"),
+    "train_real_resnet50": _tv_train("RealBottleneckResNet", "resnet50"),
+    "train_real_resnext50": _tv_train("RealResNeXt", "resnext50_32x4d"),
+    "teacher_resnet18": _tv_eval("FrozenResNetTeacher", "resnet18"),
+    "teacher_resnet50": _tv_eval("FrozenBottleneckTeacher", "resnet50"),
+    "teacher_resnext50": _tv_eval("FrozenResNeXtTeacher", "resnext50_32x4d"),
+    "eval_real_resnext50": _tv_eval("RealResNeXt", "resnext50_32x4d"),
 }
 
 

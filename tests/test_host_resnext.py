@@ -158,3 +158,81 @@ def test_launches_per_forward_counts_the_grouped_pack():
     m = tv.resnext101_32x8d()           # 33 blocks, 4 downsamples: 70 dense weights, 33 grouped
     n1 = 2 * 33 + 4
     assert launches_per_forward(FrozenResNeXtTeacher(m)) == 2 * 2 + 2 * 1 + 6 + 3 * 33 + 3 * n1
+
+
+def _small(block=tv.Bottleneck, **kw):
+    return lambda: tv.ResNet(block, [1, 1, 1, 1], **kw)
+
+
+def _empty_layer1():
+    m = tv.resnet18()
+    m.layer1 = nn.Sequential()
+    return m
+
+
+def _dense_conv2s():
+    """A ResNeXt whose grouped conv2s were replaced by dense ones (model.groups stays 32)."""
+    m = tv.ResNet(tv.Bottleneck, [1, 1, 1, 1], groups=32, width_per_group=4)
+    for blk in m.modules():
+        if type(blk) is tv.Bottleneck:
+            c = blk.conv2
+            blk.conv2 = nn.Conv2d(c.in_channels, c.out_channels, 3, c.stride, 1, bias=False)
+    return m
+
+
+def _groups_attr():
+    m = tv.ResNet(tv.Bottleneck, [1, 1, 1, 1])
+    m.groups = 32
+    return m
+
+
+def _cifar():
+    from bdbnn_b200.resnet import ResNetCifar
+    return ResNetCifar(1, conv_cls=lambda i, o, k, s, p: nn.Conv2d(i, o, k, s, p, bias=False))
+
+
+_CLASSES = ["FrozenResNetTeacher", "FrozenBottleneckTeacher", "FrozenResNeXtTeacher", "RealResNet",
+            "RealBottleneckResNet", "RealResNeXt"]
+_MODELS = {"basic": (_small(tv.BasicBlock), {"FrozenResNetTeacher", "RealResNet"}),
+           "bottleneck": (_small(), {"FrozenBottleneckTeacher", "RealBottleneckResNet"}),
+           "resnext": (_small(groups=32, width_per_group=4), {"FrozenResNeXtTeacher", "RealResNeXt"}),
+           "cifar": (_cifar, {"FrozenResNetTeacher"}),
+           "sub_block": (_small(_Bottleneck), set()),
+           "sub_basic_block": (lambda: tv.ResNet(type("_Basic", (tv.BasicBlock,), {}), [1, 1, 1, 1]), set()),
+           "empty_layer1": (_empty_layer1, {"FrozenResNetTeacher", "RealResNet"}),       # layer2 takes its input
+           "dense_conv2s": (_dense_conv2s, {"FrozenBottleneckTeacher", "RealBottleneckResNet"}),
+           "groups_attr": (_groups_attr, {"FrozenBottleneckTeacher", "RealBottleneckResNet"})}
+
+
+@pytest.mark.parametrize("name", list(_MODELS))
+def test_each_wrapper_takes_its_kind_and_every_hint_names_a_class_that_takes_the_model(name):
+    """Every wrapper accepts exactly the models of its kind; a refusal that says 'wrap it in X' names an X that
+    accepts the model."""
+    import bdbnn_b200
+    make, takers = _MODELS[name]
+    for cls in _CLASSES:
+        try:
+            getattr(bdbnn_b200, cls)(make())
+        except TypeError as e:
+            assert cls not in takers, (cls, str(e))
+            msg = str(e)
+            assert msg.startswith(cls), msg
+            if ": wrap it in " in msg:
+                other = msg.rsplit(": wrap it in ", 1)[1]
+                assert other in takers, msg
+                getattr(bdbnn_b200, other)(make())
+        else:
+            assert cls in takers, cls
+
+
+@pytest.mark.parametrize("cls", _CLASSES)
+def test_a_subclass_of_a_wrapper_keeps_its_refusals(cls):
+    import bdbnn_b200
+    sub = type("MyWrapper", (getattr(bdbnn_b200, cls),), {})
+    for name in ("basic", "bottleneck", "resnext", "cifar", "sub_block", "empty_layer1"):
+        make, takers = _MODELS[name]
+        if cls in takers:
+            sub(make())
+        else:
+            with pytest.raises(TypeError, match="MyWrapper"):
+                sub(make())
