@@ -1,6 +1,6 @@
 // Fused multi-tensor loss kernels: kurtosis regulariser, KD logits loss, KD per-layer weight loss.
 // All are tiny-tensor, launch-latency-bound in the reference (≈400 ATen launches per step, SURVEY.md
-// §2.1); here each is 1-2 launches regardless of the number of layers.  Contracts: include/bdbnn.h.
+// §2.1); here each is 1-2 launches per BDBNN_MAX_TENSORS layers (one table).  Contracts: include/bdbnn.h.
 #include "common.cuh"
 
 namespace bdbnn {
@@ -198,11 +198,15 @@ kd_layer_fwd_kernel(TensorTable tab, double* __restrict__ part) {   // part: [gr
   }
 }
 
-__global__ void kd_layer_finalize_kernel(TensorTable tab, const double* __restrict__ partial,
+// partial[off + l] = sum of layer l of this table -> its mean (reduction='mean' per layer).  The call's last table
+// (out != NULL) then adds the means of all off + L layers in layer order: one sum, whatever the number of tables.
+__global__ void kd_layer_finalize_kernel(TensorTable tab, double* __restrict__ partial, int32_t off,
                                          float* __restrict__ out) {
   if (threadIdx.x != 0) return;
+  for (int l = 0; l < tab.L; ++l) partial[off + l] /= double(tab.n[l]);
+  if (out == nullptr) return;
   double t = 0.0;
-  for (int l = 0; l < tab.L; ++l) t += partial[l] / double(tab.n[l]);  // reduction='mean' per layer
+  for (int l = 0; l < off + tab.L; ++l) t += partial[l];
   out[0] = float(t);
 }
 
@@ -220,34 +224,43 @@ kd_layer_bwd_kernel(TensorTable tab, const float* __restrict__ gout, int accumul
   }
 }
 
-static int fill_table(TensorTable& tab, const float* const* a, const float* const* b,
-                      float* const* g, const int64_t* n, const float* targets, int32_t L,
-                      int64_t* max_n) {
-  BDBNN_REQUIRE(L >= 0 && L <= BDBNN_MAX_TENSORS, "tensor count %d outside [0,%d]", L,
-                BDBNN_MAX_TENSORS);
-  memset(&tab, 0, sizeof(tab));
-  tab.L = L;
-  int64_t mx = 0;
-  for (int l = 0; l < L; ++l) {
-    BDBNN_REQUIRE(n[l] > 0, "tensor %d has numel %lld", l, (long long)n[l]);
-    BDBNN_REQUIRE(a[l] != nullptr, "tensor %d pointer is NULL", l);
-    tab.a[l] = a[l];
-    tab.b[l] = b ? b[l] : nullptr;
-    tab.g[l] = g ? g[l] : nullptr;
-    tab.n[l] = n[l];
-    tab.target[l] = targets ? targets[l] : 0.f;
-    if (n[l] > mx) mx = n[l];
-  }
-  *max_n = mx;
-  return BDBNN_OK;
-}
-
 static unsigned blocks_for(int64_t max_n, int L) {
   int64_t bx = (max_n + int64_t(kLossThreads) * 4 - 1) / (int64_t(kLossThreads) * 4);
   const int64_t cap = (int64_t(num_sms()) * 8 + L - 1) / (L > 0 ? L : 1);
   if (bx > cap) bx = cap;
   if (bx < 1) bx = 1;
   return unsigned(bx);
+}
+
+// Every entry of a call's host arrays checked (b and g where given) before anything is enqueued.
+static int check_entries(const float* const* a, const float* const* b, float* const* g, const int64_t* n,
+                         int32_t L) {
+  for (int i = 0; i < L; ++i) {
+    BDBNN_REQUIRE(n[i] > 0, "tensor %d has numel %lld", i, (long long)n[i]);
+    BDBNN_REQUIRE(a[i] != nullptr, "tensor %d pointer is NULL", i);
+    BDBNN_REQUIRE(!b || b[i], "student pointer %d is NULL", i);
+    BDBNN_REQUIRE(!g || g[i], "grad pointer %d is NULL", i);
+  }
+  return BDBNN_OK;
+}
+
+// Tensors [off, min(off + BDBNN_MAX_TENSORS, L)) as one table; returns its grid.x.  An entry point launches its
+// kernels once per table, tables in order.
+static unsigned fill_table(TensorTable& tab, const float* const* a, const float* const* b, float* const* g,
+                           const int64_t* n, const float* targets, int32_t off, int32_t L) {
+  memset(&tab, 0, sizeof(tab));
+  tab.L = L - off < BDBNN_MAX_TENSORS ? L - off : BDBNN_MAX_TENSORS;
+  int64_t mx = 0;
+  for (int l = 0; l < tab.L; ++l) {
+    const int i = off + l;
+    tab.a[l] = a[i];
+    tab.b[l] = b ? b[i] : nullptr;
+    tab.g[l] = g ? g[i] : nullptr;
+    tab.n[l] = n[i];
+    tab.target[l] = targets ? targets[i] : 0.f;
+    if (n[i] > mx) mx = n[i];
+  }
+  return blocks_for(mx, tab.L);
 }
 
 }  // namespace bdbnn
@@ -257,46 +270,57 @@ using namespace bdbnn;
 extern "C" int bdbnn_kurtosis_multi_fwd(const float* const* w_ptrs_host, const int64_t* numel_host,
                                         const float* targets_host, int32_t L, double* moments,
                                         float* kurt_out, float* loss_out, void* stream) {
+  BDBNN_REQUIRE(L >= 0, "kurtosis_multi_fwd: tensor count %d", L);
   if (L == 0) return BDBNN_OK;
   BDBNN_REQUIRE(w_ptrs_host && numel_host && targets_host && moments && kurt_out && loss_out,
                 "kurtosis_multi_fwd: NULL pointer");
-  TensorTable tab;
-  int64_t max_n;
-  int rc = fill_table(tab, w_ptrs_host, nullptr, nullptr, numel_host, targets_host, L, &max_n);
+  int rc = check_entries(w_ptrs_host, nullptr, nullptr, numel_host, L);
   if (rc) return rc;
   cudaStream_t st = cudaStream_t(stream);
   BDBNN_CUDA(cudaMemsetAsync(moments, 0, size_t(L) * kMomentStride * sizeof(double), st));
-  dim3 grid(blocks_for(max_n, L), unsigned(L));
-  const int width = L * kMomentStride;
-  double* part = nullptr;
-  rc = det_sums_alloc(&part, grid.x, width, st);
-  if (rc) return rc;
-  const cudaError_t em = cudaMemsetAsync(part, 0, size_t(grid.x) * width * sizeof(double), st);
-  kurt_moments_kernel<<<grid, kLossThreads, 0, st>>>(tab, part);
-  rc = em != cudaSuccess ? (set_error("kurtosis: cudaMemsetAsync failed: %s", cudaGetErrorString(em)), BDBNN_ERR_CUDA)
-                         : check_launch("kurt_moments_kernel");
-  if (rc) { cudaFreeAsync(part, st); return rc; }
-  rc = det_sums_finish(part, grid.x, width, moments, st);
-  if (rc) return rc;
-  kurt_finalize_kernel<<<1, BDBNN_MAX_TENSORS, 0, st>>>(tab, moments, kurt_out, loss_out);
-  return check_launch("kurt_finalize_kernel");
+  for (int32_t off = 0; off < L; off += BDBNN_MAX_TENSORS) {
+    TensorTable tab;
+    const unsigned bx = fill_table(tab, w_ptrs_host, nullptr, nullptr, numel_host, targets_host, off, L);
+    dim3 grid(bx, unsigned(tab.L));
+    double* m = moments + int64_t(off) * kMomentStride;
+    const int width = tab.L * kMomentStride;
+    double* part = nullptr;
+    rc = det_sums_alloc(&part, grid.x, width, st);
+    if (rc) return rc;
+    const cudaError_t em = cudaMemsetAsync(part, 0, size_t(grid.x) * width * sizeof(double), st);
+    kurt_moments_kernel<<<grid, kLossThreads, 0, st>>>(tab, part);
+    rc = em != cudaSuccess ? (set_error("kurtosis: cudaMemsetAsync failed: %s", cudaGetErrorString(em)), BDBNN_ERR_CUDA)
+                           : check_launch("kurt_moments_kernel");
+    if (rc) { cudaFreeAsync(part, st); return rc; }
+    rc = det_sums_finish(part, grid.x, width, m, st);
+    if (rc) return rc;
+    kurt_finalize_kernel<<<1, BDBNN_MAX_TENSORS, 0, st>>>(tab, m, kurt_out + off, loss_out + off);
+    rc = check_launch("kurt_finalize_kernel");
+    if (rc) return rc;
+  }
+  return BDBNN_OK;
 }
 
 extern "C" int bdbnn_kurtosis_multi_bwd(const float* const* w_ptrs_host, const int64_t* numel_host,
                                         const float* targets_host, int32_t L, const double* moments,
                                         const float* gout, float* const* grad_ptrs_host,
                                         int32_t accumulate, void* stream) {
+  BDBNN_REQUIRE(L >= 0, "kurtosis_multi_bwd: tensor count %d", L);
   if (L == 0) return BDBNN_OK;
   BDBNN_REQUIRE(w_ptrs_host && numel_host && targets_host && moments && gout && grad_ptrs_host,
                 "kurtosis_multi_bwd: NULL pointer");
-  TensorTable tab;
-  int64_t max_n;
-  int rc = fill_table(tab, w_ptrs_host, nullptr, grad_ptrs_host, numel_host, targets_host, L, &max_n);
+  int rc = check_entries(w_ptrs_host, nullptr, grad_ptrs_host, numel_host, L);
   if (rc) return rc;
-  for (int l = 0; l < L; ++l) BDBNN_REQUIRE(tab.g[l] != nullptr, "grad pointer %d is NULL", l);
-  dim3 grid(blocks_for(max_n, L), unsigned(L));
-  kurt_bwd_kernel<<<grid, kLossThreads, 0, cudaStream_t(stream)>>>(tab, moments, gout, accumulate);
-  return check_launch("kurt_bwd_kernel");
+  for (int32_t off = 0; off < L; off += BDBNN_MAX_TENSORS) {
+    TensorTable tab;
+    const unsigned bx = fill_table(tab, w_ptrs_host, nullptr, grad_ptrs_host, numel_host, targets_host, off, L);
+    dim3 grid(bx, unsigned(tab.L));
+    kurt_bwd_kernel<<<grid, kLossThreads, 0, cudaStream_t(stream)>>>(tab, moments + int64_t(off) * kMomentStride,
+                                                                     gout + off, accumulate);
+    rc = check_launch("kurt_bwd_kernel");
+    if (rc) return rc;
+  }
+  return BDBNN_OK;
 }
 
 extern "C" int bdbnn_kd_logits_fwd_bwd(const float* s, const float* t, int32_t N, int32_t C,
@@ -315,6 +339,7 @@ extern "C" int bdbnn_kd_layer_multi_fwd(const float* const* ws_ptrs_host,
                                         const float* const* wt_ptrs_host, const int64_t* numel_host,
                                         int32_t L, double* partial, float* loss_out, void* stream) {
   BDBNN_REQUIRE(loss_out != nullptr, "kd_layer_multi_fwd: NULL loss_out");
+  BDBNN_REQUIRE(L >= 0, "kd_layer_multi_fwd: tensor count %d", L);
   cudaStream_t st = cudaStream_t(stream);
   if (L == 0) {
     BDBNN_CUDA(cudaMemsetAsync(loss_out, 0, sizeof(float), st));
@@ -322,37 +347,45 @@ extern "C" int bdbnn_kd_layer_multi_fwd(const float* const* ws_ptrs_host,
   }
   BDBNN_REQUIRE(ws_ptrs_host && wt_ptrs_host && numel_host && partial,
                 "kd_layer_multi_fwd: NULL pointer");
-  TensorTable tab;
-  int64_t max_n;
-  int rc = fill_table(tab, wt_ptrs_host, ws_ptrs_host, nullptr, numel_host, nullptr, L, &max_n);
+  int rc = check_entries(wt_ptrs_host, ws_ptrs_host, nullptr, numel_host, L);
   if (rc) return rc;
-  for (int l = 0; l < L; ++l) BDBNN_REQUIRE(tab.b[l] != nullptr, "student pointer %d is NULL", l);
   BDBNN_CUDA(cudaMemsetAsync(partial, 0, size_t(L) * sizeof(double), st));
-  dim3 grid(blocks_for(max_n, L), unsigned(L));
-  double* part = nullptr;
-  rc = det_sums_alloc(&part, grid.x, L, st);
-  if (rc) return rc;
-  kd_layer_fwd_kernel<<<grid, kLossThreads, 0, st>>>(tab, part);
-  rc = check_launch("kd_layer_fwd_kernel");
-  if (rc) { cudaFreeAsync(part, st); return rc; }
-  rc = det_sums_finish(part, grid.x, L, partial, st);
-  if (rc) return rc;
-  kd_layer_finalize_kernel<<<1, 32, 0, st>>>(tab, partial, loss_out);
-  return check_launch("kd_layer_finalize_kernel");
+  for (int32_t off = 0; off < L; off += BDBNN_MAX_TENSORS) {
+    TensorTable tab;
+    const unsigned bx = fill_table(tab, wt_ptrs_host, ws_ptrs_host, nullptr, numel_host, nullptr, off, L);
+    const int32_t cnt = tab.L;
+    dim3 grid(bx, unsigned(cnt));
+    double* part = nullptr;
+    rc = det_sums_alloc(&part, grid.x, cnt, st);
+    if (rc) return rc;
+    kd_layer_fwd_kernel<<<grid, kLossThreads, 0, st>>>(tab, part);
+    rc = check_launch("kd_layer_fwd_kernel");
+    if (rc) { cudaFreeAsync(part, st); return rc; }
+    rc = det_sums_finish(part, grid.x, cnt, partial + off, st);
+    if (rc) return rc;
+    kd_layer_finalize_kernel<<<1, 32, 0, st>>>(tab, partial, off, off + cnt == L ? loss_out : nullptr);
+    rc = check_launch("kd_layer_finalize_kernel");
+    if (rc) return rc;
+  }
+  return BDBNN_OK;
 }
 
 extern "C" int bdbnn_kd_layer_multi_bwd(const float* const* wt_ptrs_host, const int64_t* numel_host,
                                         int32_t L, const float* gout, float* const* grad_ptrs_host,
                                         int32_t accumulate, void* stream) {
+  BDBNN_REQUIRE(L >= 0, "kd_layer_multi_bwd: tensor count %d", L);
   if (L == 0) return BDBNN_OK;
   BDBNN_REQUIRE(wt_ptrs_host && numel_host && gout && grad_ptrs_host,
                 "kd_layer_multi_bwd: NULL pointer");
-  TensorTable tab;
-  int64_t max_n;
-  int rc = fill_table(tab, wt_ptrs_host, nullptr, grad_ptrs_host, numel_host, nullptr, L, &max_n);
+  int rc = check_entries(wt_ptrs_host, nullptr, grad_ptrs_host, numel_host, L);
   if (rc) return rc;
-  for (int l = 0; l < L; ++l) BDBNN_REQUIRE(tab.g[l] != nullptr, "grad pointer %d is NULL", l);
-  dim3 grid(blocks_for(max_n, L), unsigned(L));
-  kd_layer_bwd_kernel<<<grid, kLossThreads, 0, cudaStream_t(stream)>>>(tab, gout, accumulate);
-  return check_launch("kd_layer_bwd_kernel");
+  for (int32_t off = 0; off < L; off += BDBNN_MAX_TENSORS) {
+    TensorTable tab;
+    const unsigned bx = fill_table(tab, wt_ptrs_host, nullptr, grad_ptrs_host, numel_host, nullptr, off, L);
+    dim3 grid(bx, unsigned(tab.L));
+    kd_layer_bwd_kernel<<<grid, kLossThreads, 0, cudaStream_t(stream)>>>(tab, gout, accumulate);
+    rc = check_launch("kd_layer_bwd_kernel");
+    if (rc) return rc;
+  }
+  return BDBNN_OK;
 }

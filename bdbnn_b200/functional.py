@@ -556,8 +556,13 @@ def _ptr_array(tensors):
     return (ctypes.c_void_p * len(tensors))(*[t.data_ptr() for t in tensors])
 
 
+def _loss_tables(n):
+    """Kernel-parameter tables the multi-tensor loss calls launch once each: one per BDBNN_MAX_TENSORS (64) tensors."""
+    return (n + 63) // 64
+
+
 class _KurtosisMulti(torch.autograd.Function):
-    """All hooked layers' kurtosis losses in two launches (fwd) + one (bwd).
+    """All hooked layers' kurtosis losses in two launches (fwd) + one (bwd) per 64 layers.
     Replaces 19x KurtosisWeight.kurtosis_calc (kurtosis.py:23-39)."""
 
     @staticmethod
@@ -565,8 +570,8 @@ class _KurtosisMulti(torch.autograd.Function):
     def forward(ctx, targets, *weights):
         L = _lib.lib()
         n = len(weights)
-        if n == 0 or n > 64:
-            raise RuntimeError(f"kurtosis_multi: need 1..64 tensors, got {n}")
+        if n == 0:
+            raise RuntimeError("kurtosis_multi: need at least one tensor")
         ws = []
         for w in weights:
             _require_cuda(w, "kurtosis_multi")
@@ -581,7 +586,7 @@ class _KurtosisMulti(torch.autograd.Function):
         with _timed("kurtosis_fwd", f"L{n}_n{tot}", 4 * tot):
             _lib.check(L.bdbnn_kurtosis_multi_fwd(_ptr_array(ws), numel, tg, n, _p(moments), _p(kurt),
                                                   _p(loss), _stream()), "kurtosis_multi_fwd")
-        _lib.count(2)
+        _lib.count(2 * _loss_tables(n))
         ctx.targets = tuple(float(t) for t in targets)
         ctx.save_for_backward(moments, *ws)
         ctx.mark_non_differentiable(kurt)
@@ -601,7 +606,7 @@ class _KurtosisMulti(torch.autograd.Function):
         with _timed("kurtosis_bwd", f"L{n}_n{tot}", 8 * tot):
             _lib.check(L.bdbnn_kurtosis_multi_bwd(_ptr_array(ws), numel, tg, n, _p(moments), _p(gout),
                                                   _ptr_array(grads), 0, _stream()), "kurtosis_multi_bwd")
-        _lib.count(1)
+        _lib.count(_loss_tables(n))
         return (None, *grads)
 
 
@@ -695,7 +700,7 @@ def cross_entropy_topk(logits, target, topk=(1, 5), meters=None):
 
 
 class _KDLayerMulti(torch.autograd.Function):
-    """sum_l KLDivLoss(log_target=True)(Ws_l, Wt_l) (utils/KD_loss.py:52-67) in two launches."""
+    """sum_l KLDivLoss(log_target=True)(Ws_l, Wt_l) (utils/KD_loss.py:52-67) in two launches per 64 pairs."""
 
     @staticmethod
     @_on_device
@@ -703,8 +708,8 @@ class _KDLayerMulti(torch.autograd.Function):
         L = _lib.lib()
         ws = [t.detach().contiguous() for t in tensors[:n_pairs]]
         wt = [t.detach().contiguous() for t in tensors[n_pairs:]]
-        if len(wt) != n_pairs or n_pairs == 0 or n_pairs > 64:
-            raise RuntimeError("kd_layer_multi: need 1..64 (student, teacher) pairs")
+        if len(wt) != n_pairs or n_pairs == 0:
+            raise RuntimeError("kd_layer_multi: need one or more (student, teacher) pairs")
         for a, b in zip(ws, wt):
             _require_cuda(a, "kd_layer_multi")
             _require_cuda(b, "kd_layer_multi")
@@ -718,7 +723,7 @@ class _KDLayerMulti(torch.autograd.Function):
         with _timed("kd_layer_fwd", f"L{n_pairs}_n{tot}", 8 * tot):
             _lib.check(L.bdbnn_kd_layer_multi_fwd(_ptr_array(ws), _ptr_array(wt), numel, n_pairs, _p(partial),
                                                   _p(loss), _stream()), "kd_layer_multi_fwd")
-        _lib.count(2)
+        _lib.count(2 * _loss_tables(n_pairs))
         ctx.n_pairs = n_pairs
         ctx.save_for_backward(*wt)
         return loss
@@ -736,7 +741,7 @@ class _KDLayerMulti(torch.autograd.Function):
         with _timed("kd_layer_bwd", f"L{n}_n{tot}", 8 * tot):
             _lib.check(L.bdbnn_kd_layer_multi_bwd(_ptr_array(wt), numel, n, _p(g), _ptr_array(grads), 0,
                                                   _stream()), "kd_layer_multi_bwd")
-        _lib.count(1)
+        _lib.count(_loss_tables(n))
         return (None, *grads, *([None] * n))
 
 

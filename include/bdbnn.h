@@ -241,8 +241,10 @@ BDBNN_API int bdbnn_binconv_wgrad_tc(const uint16_t* gys, int32_t grad_mode, con
 /* ---- kurtosis regulariser, multi-tensor --------------------------------------------------------
  * Replaces KurtosisWeight.kurtosis_calc (kurtosis.py:23-39) called per hooked layer at
  * train.py:501-504 / 622-625, and the scalar reduction at train.py:505-512.
- * For each tensor l<L (L <= BDBNN_MAX_TENSORS): mu=mean(w), s=std(w) UNBIASED (n-1),
+ * For each tensor l<L (any L >= 0): mu=mean(w), s=std(w) UNBIASED (n-1),
  * K=mean(((w-mu)/s)^4), loss=(K-target)^2.
+ * The multi-tensor loss calls launch their kernels once per BDBNN_MAX_TENSORS tensors (one kernel-parameter
+ * table each); with L <= BDBNN_MAX_TENSORS that is one set of launches.
  *   w_ptrs_host / numel_host / targets_host : HOST arrays of length L
  *   moments  : device double[L*8] scratch that the backward reads (mu, s, K, mean z^3, ...)
  *   kurt_out, loss_out : device float[L]
@@ -267,7 +269,8 @@ BDBNN_API int bdbnn_kd_logits_fwd_bwd(const float* s, const float* t, int32_t N,
 /* ---- KD per-layer weight loss (DistributionLoss_layer.forward, utils/KD_loss.py:52-67) ---------
  * loss = sum_l mean_l( exp(Wt_l) * (Wt_l - Ws_l) )   == sum_l KLDivLoss(log_target=True)(Ws,Wt)
  * bwd : gWs_l[j] (+)= -gout[0] * exp(Wt_l[j]) / numel_l
- * partial: device double[L] scratch. */
+ * partial: device double[L] scratch, left holding mean_l(...) per layer; loss adds them in layer order, one sum
+ * for any L (the same bits in every run). */
 BDBNN_API int bdbnn_kd_layer_multi_fwd(const float* const* ws_ptrs_host, const float* const* wt_ptrs_host,
                              const int64_t* numel_host, int32_t L, double* partial,
                              float* loss_out, void* stream);
