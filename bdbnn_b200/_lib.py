@@ -84,8 +84,6 @@ SIGNATURES = {
     "bdbnn_real_weight_pack_multi": (c_int, [c_int] + [_P] * 8 + [_P]),
     "bdbnn_real_weight_pack_multi_grad": (c_int, [c_int] + [_P] * 11 + [_P]),
     "bdbnn_real_conv_fwd_eval": (c_int, [_P] * 6 + [c_int, _P, _P, _SH, _P]),
-    "bdbnn_real_gemm1x1_fwd_eval": (c_int, [_P] * 6 + [c_int, _P, _P, _SH, _P]),
-    "bdbnn_real_gemm1x1_supported": (c_int, [_SH]),
     "bdbnn_real_gconv_supported": (c_int, [_SH, c_int]),
     "bdbnn_real_gconv_fwd": (c_int, [_P, _P, _P, _P, _SH, c_int, _P, _P, _P]),
     "bdbnn_real_gconv_fwd_eval": (c_int, [_P] * 6 + [c_int, _P, _P, _SH, c_int, _P]),

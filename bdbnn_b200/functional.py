@@ -2277,58 +2277,6 @@ def real_gconv_supported(sh, groups):
     return int(_lib.lib().bdbnn_real_gconv_supported(ctypes.byref(sh), int(groups)))
 
 
-def teacher_f32a_enabled():
-    """BDBNN_TEACHER_F32A (default 0): 1 runs the Bottleneck teacher's 1x1 convs on the GEMM that reads their fp32
-    input (real_conv1x1_bn_eval); 0 packs the input to fp16 first (real_conv_bn_eval), which measured faster on an H100
-    (DESIGN.md §4q).  The logits are the same bit for bit."""
-    return os.environ.get("BDBNN_TEACHER_F32A", "0") == "1"
-
-
-def real_gemm1x1_supported(sh):
-    """bdbnn_real_gemm1x1_supported of a ConvShape (host-only)."""
-    return bool(int(_lib.lib().bdbnn_real_gemm1x1_supported(ctypes.byref(sh))))
-
-
-@_on_x_device
-def real_conv1x1_bn_eval(x, x_amax, wpack, gamma, beta, running_mean, running_var, eps, stride, residual=None,
-                         relu=True):
-    """real_conv_bn_eval of a 1x1 / pad-0 conv (stride 1 or 2) in one launch: bdbnn_real_gemm1x1_fwd_eval reads x
-    fp32 and rounds it to fp16 in the kernel by real_act_pack's rule, so no fp16 copy of x is written.  x_amax is
-    required (the device word a previous call returned).  Bit-identical to real_conv_bn_eval(x, x_amax, wpack, ...,
-    stride, 0, residual, relu).  Returns (z fp32 channels_last, z_amax int32[1] = bits of max|z|)."""
-    _eval_only("real_conv1x1_bn_eval")
-    _require_cuda(x, "real_conv1x1_bn_eval(x)")
-    if x_amax is None:
-        raise ValueError("bdbnn_b200.real_conv1x1_bn_eval: needs x_amax, the max|x| word of the call that wrote x")
-    wf, alpha = wpack
-    _same_device(x, x_amax, wf, gamma, beta, running_mean, running_var, residual)
-    L = _lib.lib()
-    n = x.shape[0]
-    cout, taps, cin_w = wf.shape
-    if taps != 1:
-        raise RuntimeError(f"bdbnn_b200.real_conv1x1_bn_eval: expected the pack of a 1x1 weight, got {taps} taps")
-    sh = conv_shape(x.shape, (cout, cin_w, 1, 1), stride, 0)
-    if not real_gemm1x1_supported(sh):
-        raise RuntimeError("bdbnn_b200.real_conv1x1_bn_eval: the 1x1 GEMM does not support this shape")
-    z_shape = (n, cout, sh.Ho, sh.Wo)
-    if residual is not None and tuple(residual.shape) != z_shape:
-        raise RuntimeError(f"real_conv1x1_bn_eval: residual shape {tuple(residual.shape)} != output shape {z_shape}")
-    dev = x.device
-    xc = _nhwc(x.detach())
-    scale, shift = bn_eval_fold(gamma, beta, running_mean, running_var, eps, alpha)
-    rc = _nhwc(residual.detach()) if residual is not None else None
-    z = torch.empty(z_shape, dtype=torch.float32, device=dev, memory_format=torch.channels_last)
-    z_amax = torch.empty((1,), dtype=torch.int32, device=dev)
-    n_out = z.numel()
-    nbytes = 4 * n * sh.Ho * sh.Wo * sh.Cin + 2 * wf.numel() + 4 * n_out + (4 * n_out if rc is not None else 0)
-    with _timed("real_gemm1x1_fwd_eval", _shape_key(sh), nbytes):
-        _lib.check(L.bdbnn_real_gemm1x1_fwd_eval(_p(xc), _p(x_amax), _p(wf), _p(scale), _p(shift), _p(rc),
-                                                 ACT_RELU if relu else ACT_NONE, _p(z), _p(z_amax), ctypes.byref(sh),
-                                                 _stream()), "real_gemm1x1_fwd_eval")
-    _lib.count(1)
-    return z, z_amax
-
-
 @_on_x_device
 def real_conv_pool_bn_eval(x, x_amax, wpack, gamma, beta, running_mean, running_var, eps, padding=1):
     """z = hardtanh(BN_eval(max_pool2d(conv2d(x, W, stride 1), 2, 2))) of a real-valued conv under no_grad, the pooled

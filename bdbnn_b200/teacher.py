@@ -18,12 +18,10 @@ In eval mode on a CUDA fp32 input, with no autograd graph to record, the forward
 §4h); avgpool and fc stay in torch.  The CIFAR ResNet has no ReLU; its stem conv + BatchNorm runs as one fp32
 CUDA-core launch and its option-A shortcuts are read in place by conv1's epilogue (DESIGN.md §4j).  The CIFAR
 ResNet-18 has the same stem and no ReLU; each of its 1x1 `downsample` branches runs on the shortcut eval GEMM and is
-conv1's residual (DESIGN.md §4k).  A Bottleneck ResNet's convs all run as real_conv_bn_eval; with
-BDBNN_TEACHER_F32A=1 its 1x1 convs (conv1, conv3 and the `downsample`) instead read their fp32 input in a GEMM that
-rounds it to fp16 on the way in (real_conv1x1_bn_eval, DESIGN.md §4q).  A ResNeXt's grouped conv2 runs on the banded
-GEMM (real_conv_bn_eval(groups=...), DESIGN.md §4t).  VGG-Small's Hardtanh is in the epilogue of
-its stem and of its unpooled convs; its pooled convs write their fp32 output and one more kernel takes the 2x2 max,
-BatchNorm and Hardtanh (DESIGN.md §4o).
+conv1's residual (DESIGN.md §4k).  A Bottleneck ResNet's convs all run as real_conv_bn_eval (DESIGN.md §4q).  A
+ResNeXt's grouped conv2 runs on the banded GEMM (real_conv_bn_eval(groups=...), DESIGN.md §4t).  VGG-Small's Hardtanh
+is in the epilogue of its stem and of its unpooled convs; its pooled convs write their fp32 output and one more kernel
+takes the 2x2 max, BatchNorm and Hardtanh (DESIGN.md §4o).
 Anything else returns the wrapped model's own forward.
 
 The three ResNet teachers are one class for five kinds of network (_Family.kind: torchvision BasicBlock, CIFAR ResNet,
@@ -390,10 +388,8 @@ class FrozenResNetTeacher(_FrozenTeacher):
             ok = F_.cifar_stem_supported(tuple(x.shape), tuple(c1.weight.shape), c1.stride, c1.padding)
             shape = (n, c1.out_channels, h, w)
         L = _lib.lib()
+        # every conv on the pack + GEMM path, a grouped conv on the banded GEMM
         fwd_ok = lambda sh: sh.Cin % 4 == 0 and bool(int(L.bdbnn_tc_supported(ctypes.byref(sh))) & 1)
-        # every conv on the pack + GEMM path, and every 1x1 conv (a Bottleneck's) on the GEMM that reads fp32 too
-        # (either arm of BDBNN_TEACHER_F32A runs); a grouped conv on the banded GEMM
-        conv_ok = lambda sh: fwd_ok(sh) and (sh.kh != 1 or F_.real_gemm1x1_supported(sh))
         for units, sc in self._units:
             if not ok:
                 break
@@ -401,7 +397,7 @@ class FrozenResNetTeacher(_FrozenTeacher):
             for conv, _ in units:
                 g = conv.groups
                 sh = F_.gconv_shape(shape, conv.weight.shape, conv.stride[0], conv.padding[0], g)
-                ok = ok and (conv_ok(sh) if g == 1 else sh.Cin % 4 == 0 and bool(F_.real_gconv_supported(sh, g) & 32))
+                ok = ok and (fwd_ok(sh) if g == 1 else sh.Cin % 4 == 0 and bool(F_.real_gconv_supported(sh, g) & 32))
                 shape = (n, sh.Cout, sh.Ho, sh.Wo)
             if sc is None:
                 continue
@@ -410,7 +406,7 @@ class FrozenResNetTeacher(_FrozenTeacher):
                 ok = ok and F_.pad_shortcut_supported(x_shape, conv1.weight.shape, conv1.stride[0], sc.pad)
             elif fam.bottleneck:                 # one more conv on the pack + GEMM path, to the block's output shape
                 sh = F_.conv_shape(x_shape, sc[0].weight.shape, sc[0].stride[0], 0)
-                ok = ok and conv_ok(sh) and (n, sh.Cout, sh.Ho, sh.Wo) == shape
+                ok = ok and fwd_ok(sh) and (n, sh.Cout, sh.Ho, sh.Wo) == shape
             else:                                # the 1x1 GEMM over the strided samples (shortcut_eval_supported)
                 sd = sc[0].stride[0]
                 sampled = (n, x_shape[1], (x_shape[2] - 1) // sd + 1, (x_shape[3] - 1) // sd + 1)
@@ -445,22 +441,16 @@ class FrozenResNetTeacher(_FrozenTeacher):
 
     def _bottleneck_forward(self, z, z_amax, packs):
         """out = relu(bn1(conv1(x))); out = relu(bn2(conv2(out))); out = relu(bn3(conv3(out)) + shortcut(x)), the
-        shortcut x or bn(downsample conv(x)).  The 1x1 convs pack their input first, or with BDBNN_TEACHER_F32A=1 read
-        it as fp32 in the GEMM (the same logits bit for bit)."""
-        if F_.teacher_f32a_enabled():
-            conv1x1 = F_.real_conv1x1_bn_eval
-        else:
-            def conv1x1(x, x_amax, pack, *bn, stride, residual=None, relu=True):
-                return F_.real_conv_bn_eval(x, x_amax, pack, *bn, stride, 0, residual=residual, relu=relu)
+        shortcut x or bn(downsample conv(x))."""
         for ((_, bn1), (c2, bn2), (_, bn3)), ds in self._units:
             p1, p2, p3 = next(packs), next(packs), next(packs)
             if ds is None:
                 res = z
             else:
-                res, _ = conv1x1(z, z_amax, next(packs), *_bn_args(ds[1]), stride=ds[0].stride[0], relu=False)
-            y, y_amax = conv1x1(z, z_amax, p1, *_bn_args(bn1), stride=1)
+                res, _ = F_.real_conv_bn_eval(z, z_amax, next(packs), *_bn_args(ds[1]), ds[0].stride[0], 0, relu=False)
+            y, y_amax = F_.real_conv_bn_eval(z, z_amax, p1, *_bn_args(bn1), 1, 0)
             y, y_amax = F_.real_conv_bn_eval(y, y_amax, p2, *_bn_args(bn2), c2.stride[0], 1, groups=c2.groups)
-            z, z_amax = conv1x1(y, y_amax, p3, *_bn_args(bn3), stride=1, residual=res)
+            z, z_amax = F_.real_conv_bn_eval(y, y_amax, p3, *_bn_args(bn3), 1, 0, residual=res)
         return self.fc(torch.flatten(self.avgpool(z), 1))
 
 
@@ -586,8 +576,7 @@ def launches_per_forward(model):
       CIFAR ResNet-18 (DESIGN.md §4k): 2 for the stem (fold, conv) and 6 per `downsample`;
       VGG-Small (DESIGN.md §4o): 2 for the stem (fold, conv) and 1 more per pooled conv (its pool);
       torchvision Bottleneck ResNet (DESIGN.md §4q): 2 per 48 convs of any size (one pack), 6 for the stem, 3 per 3x3
-        conv and per 1x1 conv (conv1, conv3, downsample) 3 (activation pack, fold, conv), or 2 with
-        BDBNN_TEACHER_F32A=1 (fold, the GEMM that reads fp32)."""
+        conv and per 1x1 conv (conv1, conv3, downsample): activation pack, fold, conv."""
     m = model.wrapped if isinstance(model, _FrozenTeacher) else model
     if type(m) is VGGSmall:
         _check_vgg(m)
@@ -602,7 +591,7 @@ def launches_per_forward(model):
         # a ResNeXt's pack: its dense weights and its grouped conv2s each 2 launches per 48 (DESIGN.md §4t)
         n_pack = (2 * ((n1 + 47) // 48) + 2 * ((len(blocks) + 47) // 48) if fam.groups > 1 else
                   2 * ((n1 + len(blocks) + 47) // 48))
-        return n_pack + 6 + 3 * len(blocks) + (2 if F_.teacher_f32a_enabled() else 3) * n1
+        return n_pack + 6 + 3 * len(blocks) + 3 * n1
     n3 = 2 * len(blocks)
     n_ds = sum(1 for b in blocks if b.downsample is not None) if fam.shortcut == "downsample" else 0
     return 2 * ((n3 + 47) // 48) + (6 if fam.pooled_stem else 2) + 3 * n3 + 6 * n_ds

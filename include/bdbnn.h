@@ -654,21 +654,6 @@ BDBNN_API int bdbnn_real_weight_pack_multi_grad(int32_t count, const float* cons
 BDBNN_API int bdbnn_real_conv_fwd_eval(const uint16_t* xh, const uint32_t* x_amax_bits, const uint16_t* wf,
                              const float* scale, const float* shift, const float* residual, int32_t act, float* z,
                              uint32_t* z_amax_bits, const bdbnn_conv_shape* s, void* stream);
-/*   real_gemm1x1_fwd_eval  : a 1x1 / pad-0 conv of stride 1 or 2 that reads x fp32 NHWC [N][H][W][Cin] itself
- *                            (16-byte aligned, not aliasing z): each sampled element is rounded in the kernel to
- *                            fp16(x * 2^ex), real_act_pack's rule with ex from x_amax_bits (read, not computed), and
- *                            the GEMM takes the same k16 steps in the same order as real_conv_fwd_eval.  wf, scale,
- *                            shift, residual, act, z and z_amax_bits as real_conv_fwd_eval, whose result this is bit
- *                            for bit (DESIGN.md §4q).  One launch; no allocation, no synchronisation.
- *                            BDBNN_ERR_INVALID_ARG for NULL pointers, a bad act code, aliasing or misalignment, and
- *                            BDBNN_ERR_UNSUPPORTED for a shape bdbnn_real_gemm1x1_supported refuses, both before any
- *                            launch.
- *   real_gemm1x1_supported : host-only, no CUDA call: 1 when s is a valid 1x1 / pad-0 conv of stride 1 or 2 with Cin
- *                            64 or a multiple of 128, Cout 16, 32, 64 or a multiple of 128 and N*H*W < 2^31, else 0. */
-BDBNN_API int bdbnn_real_gemm1x1_fwd_eval(const float* x, const uint32_t* x_amax_bits, const uint16_t* wf,
-                                const float* scale, const float* shift, const float* residual, int32_t act, float* z,
-                                uint32_t* z_amax_bits, const bdbnn_conv_shape* s, void* stream);
-BDBNN_API int bdbnn_real_gemm1x1_supported(const bdbnn_conv_shape* s);
 
 /* ---- grouped 3x3 real-valued convs as banded GEMMs (ResNeXt conv2, DESIGN.md §4t) -------------------------------
  * A grouped conv with Cin = Cout = C, `groups` groups of Cg = C / groups channels, 3x3 / pad 1 / stride 1 or 2.  The

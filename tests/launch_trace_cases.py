@@ -23,7 +23,6 @@ SETTINGS = {
     "conv_stats_0": {"BDBNN_CONV_STATS": "0"},
     "fwd8_0": {"BDBNN_FWD8": "0"},
     "bf16x2": {"BDBNN_GRAD_MODE": "bf16x2"},
-    "teacher_f32a": {"BDBNN_TEACHER_F32A": "1"},
 }
 
 _BYREF = type(ctypes.byref(ctypes.c_int()))

@@ -1,7 +1,7 @@
-"""GPU: the Bottleneck ResNet teacher (DESIGN.md §4q).  The 1x1 GEMM that reads fp32 is checked bit for bit against
-the pack + real_conv_fwd_eval pair it replaces (and the downsample against _shortcut_eval_impl) at every distinct
-ResNet-50 / Wide-ResNet-50 1x1 shape, the mixed-k weight pack bit for bit, and the whole teacher against float64 next
-to cuDNN's TF32 forward, across BDBNN_TEACHER_F32A, CUDA graphs, load_state_dict, the fallback and the KD step."""
+"""GPU: the Bottleneck ResNet teacher (DESIGN.md §4q).  The pack + real_conv_fwd_eval pair of a 1x1 conv is checked
+against float64 (and the downsample bit for bit against _shortcut_eval_impl) at every distinct ResNet-50 /
+Wide-ResNet-50 1x1 shape, the mixed-k weight pack bit for bit, and the whole teacher against float64 next to cuDNN's
+TF32 forward, under CUDA graphs, load_state_dict, the fallback and the KD step."""
 import copy
 import ctypes
 
@@ -30,9 +30,9 @@ def _pow2_scale(amax_bits, inverse=False):
     return 2.0 ** (-e if inverse else e)
 
 
-def _teacher(arch, seed=0):
+def _teacher(arch, seed=0, **kw):
     torch.manual_seed(seed)
-    m = getattr(torchvision.models, arch)()
+    m = getattr(torchvision.models, arch)(**kw)
     g = torch.Generator().manual_seed(seed + 1)
     for mod in m.modules():                  # random BatchNorm buffers and affine parameters, some gamma < 0
         if isinstance(mod, nn.BatchNorm2d):
@@ -82,16 +82,7 @@ def _shapes_1x1():
 SHAPES = _shapes_1x1()
 
 
-def _gemm1x1(x, amax, wf, scale, shift, res, act, sh):
-    from bdbnn_b200.functional import _p, _stream
-    z = torch.empty((sh.N, sh.Ho, sh.Wo, sh.Cout), device="cuda")
-    zmax = torch.empty(1, dtype=torch.int32, device="cuda")
-    assert _lib().bdbnn_real_gemm1x1_fwd_eval(_p(x), _p(amax), _p(wf), _p(scale), _p(shift), _p(res), act, _p(z),
-                                              _p(zmax), ctypes.byref(sh), _stream()) == 0
-    return z, zmax
-
-
-def _mirror(xh, amax, wf, scale, shift, res, act, sh):
+def _conv_fwd_eval(xh, amax, wf, scale, shift, res, act, sh):
     from bdbnn_b200.functional import _p, _stream
     z = torch.empty((sh.N, sh.Ho, sh.Wo, sh.Cout), device="cuda")
     zmax = torch.empty(1, dtype=torch.int32, device="cuda")
@@ -101,14 +92,14 @@ def _mirror(xh, amax, wf, scale, shift, res, act, sh):
 
 
 @pytest.mark.parametrize("idx", range(len(SHAPES)), ids=[f"{c}x{h}to{o}s{s}" for c, h, _, o, s, _ in SHAPES])
-def test_gemm1x1_bitwise_vs_pack_and_gemm_and_vs_fp64(idx):
+def test_conv1x1_pack_and_gemm_vs_fp64(idx):
     from bdbnn_b200 import functional as F_
     from bdbnn_b200.functional import _p, _stream, bn_eval_fold, conv_shape, real_weight_pack
     cin, h, w, cout, stride, is_ds = SHAPES[idx]
     n = 8
     g = torch.Generator().manual_seed(1000 + idx)
     x = (torch.randn(n, h, w, cin, generator=g) * 1.7).cuda()
-    x[0, 0, 0, 0] = 9.5                       # max|x| on a sampled pixel: the downsample mirror scales by the same 2^ex
+    x[0, 0, 0, 0] = 9.5                       # max|x| on a sampled pixel: _shortcut_eval_impl scales by the same 2^ex
     x.view(-1)[7::997] = -0.0
     wt = (torch.randn(cout, cin, 1, 1, generator=g) * 0.05).cuda()
     amax = torch.empty(1, dtype=torch.int32, device="cuda")
@@ -117,7 +108,6 @@ def test_gemm1x1_bitwise_vs_pack_and_gemm_and_vs_fp64(idx):
     with torch.no_grad():
         (wf, alpha), = real_weight_pack([wt])
     sh = conv_shape((n, cin, h, w), (cout, cin, 1, 1), stride, 0)
-    assert F_.real_gemm1x1_supported(sh)
     gamma, beta, rm, rv = _random_bn(cout, g)
     with torch.no_grad():
         scale, shift = bn_eval_fold(gamma, beta, rm, rv, 1e-5, alpha)
@@ -129,26 +119,23 @@ def test_gemm1x1_bitwise_vs_pack_and_gemm_and_vs_fp64(idx):
     res_nan[n - 1, sh.Ho - 1, sh.Wo - 1, 1] = -0.0
     for r in (None, res, res_nan):
         for act in (0, 1, 2):
-            z, zmax = _gemm1x1(x, amax, wf, scale, shift, r, act, sh)
-            ref, ref_max = _mirror(xh, amax, wf, scale, shift, r, act, sh)
-            assert torch.equal(_bits(z), _bits(ref)), (r is None, act)
-            assert int(zmax.item()) == int(ref_max.item()), (r is None, act)
+            z, zmax = _conv_fwd_eval(xh, amax, wf, scale, shift, r, act, sh)
             if r is not res_nan:
-                assert int(zmax.item()) == int(_bits(z.abs().max().reshape(1)))
+                assert int(zmax.item()) == int(_bits(z.abs().max().reshape(1))), (r is None, act)
             else:
                 assert torch.isnan(z[0, 0, 0, 3])
-    if is_ds:                                 # the downsample against the path it replaces
+    if is_ds:                                 # the downsample against the BasicBlock teachers' shortcut GEMM
         x_nchw = x.permute(0, 3, 1, 2)
         with torch.no_grad():
             ds = F_._shortcut_eval_impl(x_nchw, wt, gamma, beta, rm, rv, 1e-5, stride)
-        z, _ = _gemm1x1(x, amax, wf, scale, shift, None, 0, sh)
+        z, _ = _conv_fwd_eval(xh, amax, wf, scale, shift, None, 0, sh)
         assert torch.equal(_bits(z), _bits(ds.permute(0, 2, 3, 1)))
     with torch.no_grad():                     # conv + BN + residual + ReLU in float64
         y64 = torch.nn.functional.conv2d(x.permute(0, 3, 1, 2).double(), wt.double(), None, stride, 0)
         k = gamma.double() / torch.sqrt(rv.double() + 1e-5)
         r64 = (y64 - rm.double().view(1, -1, 1, 1)) * k.view(1, -1, 1, 1) + beta.double().view(1, -1, 1, 1)
         r64 = torch.relu(r64 + res.permute(0, 3, 1, 2).double())
-        z, _ = _gemm1x1(x, amax, wf, scale, shift, res, 1, sh)
+        z, _ = _conv_fwd_eval(xh, amax, wf, scale, shift, res, 1, sh)
         err = (z.permute(0, 3, 1, 2).double() - r64).abs().max().item()
     assert err <= 2e-3 * r64.abs().max().item(), err
 
@@ -174,10 +161,12 @@ def test_mixed_k_weight_pack_bitwise():
 # ---- whole teacher --------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("arch,n,layout", [("resnet50", 8, "nchw"), ("resnet50", 8, "channels_last"),
                                            ("wide_resnet50_2", 8, "nchw"), ("wide_resnet50_2", 8, "channels_last"),
-                                           ("resnet101", 4, "channels_last")])
-def test_teacher_logits_vs_fp64_and_tf32_and_across_f32a(arch, n, layout, monkeypatch, tmp_path):
+                                           ("resnet101", 4, "channels_last"),
+                                           # width_per_group 32: layer1's conv3 reads 32 channels
+                                           ("resnet50_w32", 8, "channels_last")])
+def test_teacher_logits_vs_fp64_and_tf32(arch, n, layout, tmp_path):
     from bdbnn_b200 import FrozenBottleneckTeacher
-    m = _teacher(arch).cuda()
+    m = (_teacher("resnet50", width_per_group=32) if arch == "resnet50_w32" else _teacher(arch)).cuda()
     t = FrozenBottleneckTeacher(m)
     g = torch.Generator().manual_seed(9)
     x = torch.randn(n, 3, 224, 224, generator=g).cuda()
@@ -185,11 +174,7 @@ def test_teacher_logits_vs_fp64_and_tf32_and_across_f32a(arch, n, layout, monkey
         x = x.contiguous(memory_format=torch.channels_last)
     assert t.kernel_path(x)
     with torch.no_grad():
-        monkeypatch.setenv("BDBNN_TEACHER_F32A", "1")
         out = t(x)
-        monkeypatch.setenv("BDBNN_TEACHER_F32A", "0")
-        out_packed = t(x)
-        monkeypatch.delenv("BDBNN_TEACHER_F32A")
         ref = copy.deepcopy(m).double()(x.double())
         prev = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
         torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = True
@@ -197,7 +182,6 @@ def test_teacher_logits_vs_fp64_and_tf32_and_across_f32a(arch, n, layout, monkey
             tf32 = m(x)
         finally:
             torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = prev
-    assert torch.equal(_bits(out), _bits(out_packed))
     err = (out.double() - ref).abs().max().item()
     err_tf32 = (tf32.double() - ref).abs().max().item()
     scale = ref.abs().max().item()
@@ -206,19 +190,17 @@ def test_teacher_logits_vs_fp64_and_tf32_and_across_f32a(arch, n, layout, monkey
     assert err <= max(2 * err_tf32, 2e-3 * scale), (err, err_tf32, scale)
 
 
-@pytest.mark.parametrize("f32a", ["1", "0"])
-def test_teacher_determinism_graph_state_and_launches(f32a, monkeypatch):
+def test_teacher_determinism_graph_state_and_launches():
     from bdbnn_b200 import FrozenBottleneckTeacher, _lib as lib
     from bdbnn_b200.teacher import launches_per_forward
-    monkeypatch.setenv("BDBNN_TEACHER_F32A", f32a)
-    m = _teacher("resnet50").cuda().to(memory_format=torch.channels_last)
+    m =_teacher("resnet50").cuda().to(memory_format=torch.channels_last)
     t = FrozenBottleneckTeacher(m)
     x = torch.randn(8, 3, 224, 224, generator=torch.Generator().manual_seed(2)).cuda()
     x = x.contiguous(memory_format=torch.channels_last)
     buffers = {k: v.clone() for k, v in m.named_buffers()}
     n0 = lib.launch_count()
     a = t(x)                          # grad mode on, nothing requires grad: the kernel path
-    assert lib.launch_count() - n0 == launches_per_forward(t) == (130 if f32a == "1" else 166)
+    assert lib.launch_count() - n0 == launches_per_forward(t) == 166
     b = t(x)
     assert not a.requires_grad and torch.equal(_bits(a), _bits(b))
     for k, v in m.named_buffers():
@@ -268,12 +250,10 @@ def test_teacher_falls_back_to_the_models_forward():
         assert torch.equal(v, w), k
 
 
-@pytest.mark.parametrize("f32a", ["1", "0"])
-def test_profiled_forward_has_no_cudnn_conv_or_aten_bn_relu_add(f32a, monkeypatch):
+def test_profiled_forward_has_no_cudnn_conv_or_aten_bn_relu_add():
     from torch.profiler import ProfilerActivity, profile
     from bdbnn_b200 import FrozenBottleneckTeacher
-    monkeypatch.setenv("BDBNN_TEACHER_F32A", f32a)
-    t = FrozenBottleneckTeacher(_teacher("resnet50").cuda())
+    t =FrozenBottleneckTeacher(_teacher("resnet50").cuda())
     x = torch.randn(4, 3, 224, 224, generator=torch.Generator().manual_seed(3)).cuda()
     t(x)
     torch.cuda.synchronize()
@@ -286,7 +266,6 @@ def test_profiled_forward_has_no_cudnn_conv_or_aten_bn_relu_add(f32a, monkeypatc
               "aten::add_"}
     assert not (names & banned), names & banned
     assert not [nm for nm in names if "cudnn" in nm.lower()]
-    assert any("real_gemm1x1_kernel" in nm for nm in names) == (f32a == "1")
 
 
 # ---- in the logit-KD step -------------------------------------------------------------------------------------------

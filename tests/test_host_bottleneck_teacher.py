@@ -1,8 +1,6 @@
 """Host-only checks of the Bottleneck ResNet teacher (DESIGN.md §4q): the structures FrozenBottleneckTeacher accepts
-and refuses, names and parameters, the geometry walk, the launch formula, the fallback to the model's forward, and the
-argument validation of bdbnn_real_gemm1x1_fwd_eval (error codes before anything is launched, no CUDA device needed)."""
+and refuses, names and parameters, the geometry walk, the launch formula and the fallback to the model's forward."""
 import copy
-import ctypes
 
 import pytest
 import torch
@@ -11,9 +9,6 @@ import torch.nn as nn
 torchvision = pytest.importorskip("torchvision")
 tv = torchvision.models.resnet
 
-BDBNN_ERR_INVALID_ARG, BDBNN_ERR_UNSUPPORTED = -1, -3
-NULL = ctypes.c_void_p(0)
-PTR = ctypes.c_void_p(4096)       # any non-NULL, 16-byte aligned value: validation fails before it is dereferenced
 ARCHS = ["resnet50", "resnet101", "resnet152", "wide_resnet50_2", "wide_resnet101_2"]
 
 
@@ -133,44 +128,26 @@ def test_geometry_walk(L, arch, monkeypatch):
     t = FrozenBottleneckTeacher(getattr(torchvision.models, arch)())
     assert t._walk_geometry(torch.empty(8, 3, 224, 224), (3, 2, 1))
     assert t._walk_geometry(torch.empty(256, 3, 224, 224), (3, 2, 1))
-    # 48 channels inside the blocks: neither the 3x3 GEMM nor the 1x1 GEMM takes them
+    # 48 channels inside the blocks: the 3x3 GEMM does not take them
     narrow = FrozenBottleneckTeacher(tv.ResNet(tv.Bottleneck, [1, 1, 1, 1], width_per_group=48))
     assert not narrow._walk_geometry(torch.empty(8, 3, 224, 224), (3, 2, 1))
+    # 32 channels into layer1's conv3 (a 1x1 conv): the pack + GEMM path takes every conv
+    slim = FrozenBottleneckTeacher(torchvision.models.resnet50(width_per_group=32))
+    assert slim._walk_geometry(torch.empty(8, 3, 224, 224), (3, 2, 1))
 
 
-def test_gemm1x1_support_query(L):
-    from bdbnn_b200.functional import conv_shape, real_gemm1x1_supported
-    ok = [((8, 64, 56, 56), (64, 64, 1, 1), 1), ((8, 64, 56, 56), (256, 64, 1, 1), 1),
-          ((8, 256, 56, 56), (512, 256, 1, 1), 2), ((8, 1024, 14, 14), (2048, 1024, 1, 1), 2),
-          ((8, 128, 28, 28), (32, 128, 1, 1), 1)]
-    bad = [((8, 64, 56, 56), (64, 64, 3, 3), 1),          # not 1x1
-           ((8, 64, 56, 56), (64, 64, 1, 1), 3),          # stride 3
-           ((8, 96, 56, 56), (64, 96, 1, 1), 1),          # Cin not 64 or a multiple of 128
-           ((8, 32, 56, 56), (64, 32, 1, 1), 1),
-           ((8, 64, 56, 56), (96, 64, 1, 1), 1)]          # Cout 96
-    for x, w, s in ok:
-        assert real_gemm1x1_supported(conv_shape(x, w, s, 0)), (x, w, s)
-    for x, w, s in bad:
-        assert not real_gemm1x1_supported(conv_shape(x, w, s, 0)), (x, w, s)
-    assert not real_gemm1x1_supported(conv_shape((8, 64, 56, 56), (64, 64, 1, 1), 1, 1))     # padded
-    assert L.bdbnn_real_gemm1x1_supported(None) == 0
-
-
-def test_launch_formula(monkeypatch):
+def test_launch_formula():
     from bdbnn_b200 import FrozenBottleneckTeacher
     from bdbnn_b200.teacher import launches_per_forward
     # blocks, downsamples: 1x1 convs = 2 * blocks + downsamples, all convs = 3 * blocks + downsamples
     depth = {"resnet50": (16, 4), "resnet101": (33, 4), "resnet152": (50, 4), "wide_resnet50_2": (16, 4)}
-    for f32a, per_1x1 in (("1", 2), ("0", 3)):
-        monkeypatch.setenv("BDBNN_TEACHER_F32A", f32a)
-        for arch, (nb, nd) in depth.items():
-            m = getattr(torchvision.models, arch)()
-            n_all, n1 = 3 * nb + nd, 2 * nb + nd
-            want = 2 * ((n_all + 47) // 48) + 6 + 3 * nb + per_1x1 * n1
-            assert launches_per_forward(m) == want, (arch, f32a)
-            assert launches_per_forward(FrozenBottleneckTeacher(m)) == want
-    monkeypatch.delenv("BDBNN_TEACHER_F32A")
-    assert launches_per_forward(torchvision.models.resnet50()) == 4 + 6 + 48 + 3 * 36      # default: the pack path
+    for arch, (nb, nd) in depth.items():
+        m = getattr(torchvision.models, arch)()
+        n_all, n1 = 3 * nb + nd, 2 * nb + nd
+        want = 2 * ((n_all + 47) // 48) + 6 + 3 * nb + 3 * n1
+        assert launches_per_forward(m) == want, arch
+        assert launches_per_forward(FrozenBottleneckTeacher(m)) == want
+    assert launches_per_forward(torchvision.models.resnet50()) == 4 + 6 + 48 + 3 * 36
     # the BasicBlock families are counted as before
     assert launches_per_forward(torchvision.models.resnet18()) == 2 + 6 + 3 * 16 + 6 * 3
 
@@ -212,30 +189,3 @@ def test_load_state_dict_round_trips():
     x = torch.randn(1, 3, 64, 64)
     with torch.no_grad():
         assert torch.equal(t(x), b(x))
-
-
-def _shape(n=8, h=56, w=56, cin=256, cout=128, stride=1):
-    from bdbnn_b200.functional import conv_shape
-    return conv_shape((n, cin, h, w), (cout, cin, 1, 1), stride, 0)
-
-
-def test_gemm1x1_rejects_bad_arguments(L):
-    ok = dict(x=PTR, amax=PTR, wf=PTR, scale=PTR, shift=PTR, res=NULL, act=1, z=ctypes.c_void_p(8192), zmax=NULL,
-              sh=_shape())
-
-    def call(**kw):
-        a = {**ok, **kw}
-        sh = a["sh"]
-        return L.bdbnn_real_gemm1x1_fwd_eval(a["x"], a["amax"], a["wf"], a["scale"], a["shift"], a["res"], a["act"],
-                                             a["z"], a["zmax"], ctypes.byref(sh) if sh is not None else None, NULL)
-    bad_shape = _shape()
-    bad_shape.Ho = 55
-    for bad in (dict(x=NULL), dict(amax=NULL), dict(wf=NULL), dict(scale=NULL), dict(shift=NULL), dict(z=NULL),
-                dict(act=3), dict(act=-1), dict(res=ctypes.c_void_p(8192)), dict(x=ctypes.c_void_p(8192)),
-                dict(x=ctypes.c_void_p(4104)), dict(sh=None), dict(sh=bad_shape)):
-        assert call(**bad) == BDBNN_ERR_INVALID_ARG, bad
-    from bdbnn_b200.functional import conv_shape
-    for sh in (conv_shape((8, 256, 56, 56), (128, 256, 3, 3), 1, 1), _shape(cin=96), _shape(cout=96),
-               _shape(stride=3)):
-        assert call(sh=sh) == BDBNN_ERR_UNSUPPORTED
-        assert b"real_gemm1x1_fwd_eval" in L.bdbnn_last_error_string()

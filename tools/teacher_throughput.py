@@ -19,16 +19,12 @@ round, each warmed up first, images/s from CUDA events over --iters forwards:
     kernel_graphed   the same forward captured once as a CUDA graph and replayed
     cudnn_default    the unwrapped model with TF32 allowed and cudnn.benchmark off (bench.py's timed path)
     cudnn_benchmark  the same with cudnn.benchmark = True (train.py:368)
-    kernel_eager_f32a1, kernel_graphed_f32a1   (Bottleneck teachers) the kernel arms with BDBNN_TEACHER_F32A=1: the 1x1
-                     convs read their fp32 input in the GEMM instead of packing it to fp16 first (DESIGN.md §4q)
 
 The two kernel arms run in this process.  Each cuDNN arm runs in a process of its own, started afresh every round:
 PyTorch caches the cuDNN plan of a conv shape whatever `benchmark` was when it was chosen, so in one process the arm
 that ran first would serve its plans to the other and the benchmark arm would not autotune.
 
-Then one eager kernel-teacher forward under functional.KernelTimer (per-family times; for a Bottleneck teacher also
-per 1x1 shape, the fp32-reading GEMM against real_act_pack + real_conv_fwd_eval, three forwards of each), and the full
-KD step:
+Then one eager kernel-teacher forward under functional.KernelTimer (per-family times), and the full KD step:
 GraphedTrainStep(TrainStep(student, kurtosis + KD config, teacher=...)) with the kernel teacher and with the
 unwrapped teacher (cudnn.benchmark off throughout this process; the student is the binary resnet18, or the binary
 CIFAR net of the teacher's shape for a CIFAR teacher, the binary vgg_small for vgg_small; a Bottleneck teacher runs
@@ -146,29 +142,6 @@ def _bottleneck(name):
     return name in BOTTLENECK
 
 
-class _f32a:
-    """BDBNN_TEACHER_F32A set to `value` for the duration of a call (the teacher reads it at every forward)."""
-    def __init__(self, value):
-        self.value = value
-
-    def __enter__(self):
-        self.prev = os.environ.get("BDBNN_TEACHER_F32A")
-        os.environ["BDBNN_TEACHER_F32A"] = self.value
-
-    def __exit__(self, *exc):
-        if self.prev is None:
-            del os.environ["BDBNN_TEACHER_F32A"]
-        else:
-            os.environ["BDBNN_TEACHER_F32A"] = self.prev
-
-
-def _with_f32a(value, fn):
-    def run():
-        with _f32a(value):
-            return fn()
-    return run
-
-
 def _wrap(name, model):
     from bdbnn_b200 import FrozenBottleneckTeacher, FrozenResNetTeacher, FrozenResNeXtTeacher, FrozenVGGTeacher
     if name == "vgg_small":
@@ -186,9 +159,6 @@ def forward_arms(torch, name, args, dev):
     with torch.no_grad():
         assert kt.kernel_path(x)
         arms = {"kernel_eager": lambda: kt(x), "kernel_graphed": _graphed(torch, lambda: kt(x), args.warmup)}
-        if _bottleneck(name):
-            arms["kernel_eager_f32a1"] = _with_f32a("1", lambda: kt(x))
-            arms["kernel_graphed_f32a1"] = _with_f32a("1", lambda: _graphed(torch, lambda: kt(x), args.warmup))()
         for fn in arms.values():
             for _ in range(args.warmup):
                 fn()
@@ -212,23 +182,6 @@ def forward_arms(torch, name, args, dev):
     for fam, f in sorted(fams.items(), key=lambda kv: -kv[1]["ms"]):
         print(json.dumps({"teacher": name, "family": fam, "ms": round(f["ms"], 4), "launches": f["launches"]}))
     print(json.dumps({"teacher": name, "kernel_timer_total_ms": round(total, 4)}), flush=True)
-    if _bottleneck(name):
-        per_shape = {}
-        for value in ("1", "0"):
-            with torch.no_grad(), _f32a(value):
-                kt(x)
-                KernelTimer.start()
-                for _ in range(3):
-                    kt(x)
-                kern = KernelTimer.stop()
-            for (fam, key), d in kern.items():
-                if fam in ("real_gemm1x1_fwd_eval", "real_act_pack", "real_conv_fwd_eval") and "k1" in str(key):
-                    row = per_shape.setdefault(str(key), {})
-                    arm = "gemm1x1" if value == "1" else "pack_gemm"
-                    row[arm + "_ms"] = round(row.get(arm + "_ms", 0.0) + d["ms"] / 3, 4)
-                    row[arm + "_launches"] = row.get(arm + "_launches", 0) + d["launches"] // 3
-        for key, row in per_shape.items():
-            print(json.dumps({"teacher": name, "conv1x1": key, **row}), flush=True)
 
 
 def kd_step_arms(torch, name, args, dev):
