@@ -321,8 +321,7 @@ def test_stem_conv_module_path_and_fallback(monkeypatch):
 @pytest.mark.parametrize("geom", [(4, 64, 64), (2, 224, 224), (3, 38, 50)])
 def test_stem_fused_conv_bn_pool(geom):
     """One-node stem (conv -> BN(train) -> maxpool, gradient handed to the wgrad as fp16 only) vs the two-node
-    path on the same kernels (identical forward; weight gradient within fp16-rounding distance) and vs an
-    fp64 torch stem."""
+    path on the same kernels (statistics from a different reduction: last-bit distance) and vs an fp64 torch stem."""
     import torch.nn as nn
     from bdbnn_b200 import functional as F_
     n, h, w = geom
@@ -347,11 +346,15 @@ def test_stem_fused_conv_bn_pool(geom):
 
     zf, gwf, ggf, gbf, rmf, rvf, gz = run(True)
     zu, gwu, ggu, gbu, rmu, rvu, _ = run(False)
-    # same kernels; the BN statistics are summed with atomics (fp32 per CTA, then fp64), so the last bits of mean /
-    # invstd differ run to run and dgamma / dbeta (sums over 1e5 terms) move by a few 1e-5 relative
-    for a, b in ((zf, zu), (rmf, rmu), (rvf, rvu), (ggf, ggu), (gbf, gbu)):
-        torch.testing.assert_close(a, b, rtol=1e-4, atol=1e-4)
-    assert (gwf - gwu).abs().max().item() <= 2e-3 * gwu.abs().max().item()
+    # each path is run-to-run deterministic, but the two take the BatchNorm sums from different reductions: the
+    # one-node path from the conv epilogue's per-CTA rows, the two-node path from bn_stats_launch's per-block rows.
+    # The fp64 sums then differ in their last bits, and so do the fp32 mean / invstd made from them: z, the running
+    # statistics and dgamma / dbeta move by about 1e-7 of their max (measured: up to 2.2e-7), and the fp16 gradient
+    # operand rounds a few entries the other way, which moves gW by a few 1e-6 of its max (measured: 3.6e-6)
+    for name, a, b in (("z", zf, zu), ("running_mean", rmf, rmu), ("running_var", rvf, rvu), ("dgamma", ggf, ggu),
+                       ("dbeta", gbf, gbu)):
+        assert (a - b).abs().max().item() <= 1e-6 * b.abs().max().item(), name
+    assert (gwf - gwu).abs().max().item() <= 2e-5 * gwu.abs().max().item()
     assert hasattr(zf, "shape") and zf.shape == (n, 64, ((h - 1) // 2) // 2 + 1, ((w - 1) // 2) // 2 + 1)
     # fp64 torch BN + max-pool + conv weight gradient, evaluated on the GPU conv's own output y (pooling
     # winners are discrete: an fp64 conv would flip a few near-ties and move whole gradient entries)
@@ -440,10 +443,10 @@ def test_unit_with_in_node_shortcut_equals_two_nodes(geom):
 
     o1, g1, rm1 = run(True)
     o2, g2, rm2 = run(False)
-    torch.testing.assert_close(o1, o2, rtol=1e-5, atol=1e-5)       # BN statistics use fp64 atomics: last-bit noise
-    torch.testing.assert_close(rm1, rm2, rtol=1e-5, atol=1e-6)
-    for a, b in zip(g1, g2):
-        assert (a - b).abs().max().item() <= 2e-4 * b.abs().max().item() + 1e-7
+    # the same kernels on the same data, every sum in a fixed order: the same bits
+    assert torch.equal(o1, o2) and torch.equal(rm1, rm2)
+    for i, (a, b) in enumerate(zip(g1, g2)):
+        assert torch.equal(a, b), i
 
 
 FULL_SIZE = [  # BASELINE.json config-2 layer geometries at N=256 (cin, hw, cout, stride)
