@@ -121,6 +121,10 @@ SIGNATURES = {
     "bdbnn_pool2_bn_bwd_pack": (c_int, [_P] * 10 + [c_int] * 5 + [_P] * 8),
     "bdbnn_pool2_bn_eval_hardtanh": (c_int, [_P] * 3 + [c_int] * 4 + [_P] * 3 + [c_int, _P]),
     "bdbnn_real_pool2_bn_eval_hardtanh": (c_int, [_P] * 3 + [c_int] * 4 + [_P] * 3),
+    "bdbnn_real_bn_fwd_hardtanh": (c_int, [_P] * 3 + [c_int64, c_int, ctypes.c_float, ctypes.c_float] + [_P] * 9 +
+                                   [c_int, _P]),
+    "bdbnn_real_pool2": (c_int, [_P] + [c_int] * 4 + [_P] * 5),
+    "bdbnn_real_pool2_bn_bwd_pack": (c_int, [_P] * 9 + [c_int] * 4 + [_P] * 8),
     "bdbnn_cifar_batch": (c_int, [_P, _P, c_int64, ctypes.c_uint64, ctypes.c_uint32, c_int64, c_int, c_int, _P, _P, _P,
                                   c_int64, c_int64, c_int64, c_int64, _P, _P]),
     "bdbnn_imagenet_batch": (c_int, [_P, _P, c_int, _P, _P, _P, c_int64, c_int64, c_int64, c_int64, _P, _P]),

@@ -292,6 +292,9 @@ struct PadResidual {
 // RELU (PACK false, fp32 y): z = relu(y*a + b (+ residual)), mask_bits = ReLU's gradient mask (relu_bits4, one bit per
 // channel as the STE mask), and the bits of max|z| into z_amax (integer atomicMax, NaN on top: run-to-run identical),
 // the word the next real-valued conv's real_act_pack scales its fp16 operand by.
+// HT with PACK false (fp32 y, no residual, the real-valued Hardtanh units): z = hardtanh(u) for u = fmaf(y, a, b) as it
+// stands (adding a zero residual would turn a -0.0 into +0.0), no mask words (the backward recomputes u with the same
+// fmaf, htanh_mask), and max|z| into z_amax as RELU.
 template <bool PACK, bool I16 = false, int U = 4, bool SUB = false, bool P16 = false, bool HT = false,
           bool RELU = false>
 __global__ void __launch_bounds__(kBnThreads)
@@ -300,6 +303,7 @@ bn_apply_add_pack_kernel(const void* __restrict__ y, const float4* __restrict__ 
                          float4* __restrict__ z, uint32_t* __restrict__ sign_bits,
                          uint32_t* __restrict__ mask_bits, uint2* __restrict__ xb4, uint32_t* __restrict__ xb8,
                          uint32_t one16, const PadResidual sub = PadResidual{}, uint32_t* __restrict__ z_amax = nullptr) {
+  constexpr bool HT_REAL = HT && !PACK;
   constexpr int GL = P16 ? 4 : 8;                                 // lanes (float4 groups) per bit word
   const int lane = threadIdx.x & 31;
   const uint32_t group_mask = (P16 ? 0xfu : 0xffu) << (lane & (32 - GL));
@@ -315,12 +319,13 @@ bn_apply_add_pack_kernel(const void* __restrict__ y, const float4* __restrict__ 
   auto emit = [&](int64_t i, const float4 v, const float4 r) {
     float4 o = make_float4(fmaf(v.x, av.x, bv.x), fmaf(v.y, av.y, bv.y), fmaf(v.z, av.z, bv.z),
                            fmaf(v.w, av.w, bv.w));
-    o.x += r.x; o.y += r.y; o.z += r.z; o.w += r.w;
+    if (!HT_REAL) { o.x += r.x; o.y += r.y; o.z += r.z; o.w += r.w; }
     if (HT) { o.x = htanh(o.x); o.y = htanh(o.y); o.z = htanh(o.z); o.w = htanh(o.w); }
-    if (RELU) {
-      o.x = relu_f(o.x); o.y = relu_f(o.y); o.z = relu_f(o.z); o.w = relu_f(o.w);
+    if (RELU) { o.x = relu_f(o.x); o.y = relu_f(o.y); o.z = relu_f(o.z); o.w = relu_f(o.w); }
+    if (RELU || HT_REAL)
       zmax = max(zmax, max(max(__float_as_uint(fabsf(o.x)), __float_as_uint(fabsf(o.y))),
                            max(__float_as_uint(fabsf(o.z)), __float_as_uint(fabsf(o.w)))));
+    if (RELU) {
       const uint32_t mw = __reduce_or_sync(group_mask, relu_bits4(o) << sh);
       if ((lane & (GL - 1)) == 0) mask_bits[i / GL] = mw;
     }
@@ -373,7 +378,7 @@ bn_apply_add_pack_kernel(const void* __restrict__ y, const float4* __restrict__ 
     for (int u = 0; u < U; ++u) emit(i + u * nthreads, v[u], r[u]);
   }
   for (; i < n4; i += nthreads) emit(i, load_y4<I16>(y, i), load_r(i));
-  if (RELU) {
+  if (RELU || HT_REAL) {
     zmax = __reduce_max_sync(0xffffffffu, zmax);      // every lane of the (whole) warp gets here
     if (lane == 0 && zmax != 0u) atomicMax(z_amax, zmax);
   }
@@ -493,6 +498,9 @@ bn_bwd_pack_kernel(const float4* __restrict__ gz, const void* __restrict__ y, co
 //                           backward's 16-bit operand at the conv-output resolution: the value at the winner, 0 elsewhere
 //   pool2_eval_kernel     : z = hardtanh(fp32(fp32(max * scale) + shift)) from the folded eval BatchNorm, + the +-1 copy
 //   real_pool2_eval_kernel: the same on the fp32 output of a real-valued conv (the fp32 VGG-Small teacher), + max|z|
+//   real_pool2_kernel     : pool2_i16_kernel on the fp32 output of a real-valued conv (the fp32 VGG-Small in training),
+//                           F.max_pool2d's winner, statistics and max|p| of p itself; pool2_bwd_pack_kernel<MODE, false>
+//                           is its backward
 __device__ __forceinline__ int4 pool2_quad(const int16_t* __restrict__ y, int64_t off) {
   const uint2 r = __ldcs(reinterpret_cast<const uint2*>(y + off));
   return make_int4(int16_t(r.x & 0xffffu), int16_t(r.x >> 16), int16_t(r.y & 0xffffu), int16_t(r.y >> 16));
@@ -516,11 +524,38 @@ __device__ __forceinline__ int4 pool2_max(const int16_t* __restrict__ y, int64_t
   return m;
 }
 
-// thread = one channel group, strided over pooled pixels as bn_reduce_kernel (grid * blockDim a multiple of C4)
-__global__ void __launch_bounds__(kBnThreads)
-pool2_i16_kernel(const int16_t* __restrict__ y, const float* __restrict__ alpha, int H, int W, int C4, int64_t n_pool,
-                 int16_t* __restrict__ p, uint32_t* __restrict__ idx, double* __restrict__ part,
-                 uint32_t* __restrict__ maxbits) {
+// fp32 y: the max of the window as F.max_pool2d takes it (scan order, `v > m || v is NaN`): NaN if the window holds
+// one, and of equal values (+0.0 / -0.0) the first.  win != NULL: the winner's tap bytes as pool2_max (the last NaN
+// of a window, as torch's index)
+__device__ __forceinline__ bool pool2_wins(float m, float v) { return v > m || v != v; }
+
+__device__ __forceinline__ float4 pool2_max_f32(const float* __restrict__ y, int64_t n, int ho, int wo, int H, int W,
+                                                int C, int c4, uint32_t* win = nullptr) {
+  float4 m;
+  uint32_t tx = 0, ty = 0, tz = 0, tw = 0;
+#pragma unroll
+  for (int t = 0; t < 4; ++t) {
+    const int64_t off = ((n * H + 2 * ho + (t >> 1)) * W + 2 * wo + (t & 1)) * C + 4 * c4;
+    const float4 v = __ldcs(reinterpret_cast<const float4*>(y + off));
+    if (t == 0) {
+      m = v;
+    } else {
+      if (pool2_wins(m.x, v.x)) { m.x = v.x; tx = t; }
+      if (pool2_wins(m.y, v.y)) { m.y = v.y; ty = t; }
+      if (pool2_wins(m.z, v.z)) { m.z = v.z; tz = t; }
+      if (pool2_wins(m.w, v.w)) { m.w = v.w; tw = t; }
+    }
+  }
+  if (win != nullptr) *win = tx | (ty << 8) | (tz << 16) | (tw << 24);
+  return m;
+}
+
+// thread = one channel group, strided over pooled pixels as bn_reduce_kernel (grid * blockDim a multiple of C4).
+// F32: y and p fp32 (real_pool2_kernel, the statistics of p itself), else int16 (pool2_i16_kernel, those of alpha*p).
+template <bool F32>
+__device__ __forceinline__ void pool2_stats(const void* __restrict__ y, const float* __restrict__ alpha, int H, int W,
+                                            int C4, int64_t n_pool, void* __restrict__ p, uint32_t* __restrict__ idx,
+                                            double* __restrict__ part, uint32_t* __restrict__ maxbits) {
   extern __shared__ float4 shs[];
   const int C = C4 * 4;
   uint32_t* shm = reinterpret_cast<uint32_t*>(shs + 2 * blockDim.x);
@@ -531,20 +566,26 @@ pool2_i16_kernel(const int16_t* __restrict__ y, const float* __restrict__ alpha,
   const int64_t nthreads = int64_t(gridDim.x) * blockDim.x;
   const int c4 = int(gtid % C4);
   const int64_t p_step = nthreads / C4;
-  const float4 al = *reinterpret_cast<const float4*>(alpha + c4 * 4);
+  const float4 al = F32 ? make_float4(1, 1, 1, 1) : *reinterpret_cast<const float4*>(alpha + c4 * 4);
   float4 sa = make_float4(0, 0, 0, 0), sb = sa, mx = sa;
   for (int64_t q = gtid / C4; q < n_pool; q += p_step) {
     const int wo = int(q % Wo);
     const int64_t r = q / Wo;
     const int ho = int(r % Ho);
     uint32_t win;
-    const int4 m = pool2_max(y, r / Ho, ho, wo, H, W, C, c4, &win);
     const int64_t o = q * C4 + c4;
-    *reinterpret_cast<uint2*>(p + 4 * o) = make_uint2((uint32_t(m.x) & 0xffffu) | (uint32_t(m.y) << 16),
-                                                      (uint32_t(m.z) & 0xffffu) | (uint32_t(m.w) << 16));
+    float4 v;
+    if (F32) {
+      v = pool2_max_f32(static_cast<const float*>(y), r / Ho, ho, wo, H, W, C, c4, &win);
+      static_cast<float4*>(p)[o] = v;
+    } else {
+      const int4 m = pool2_max(static_cast<const int16_t*>(y), r / Ho, ho, wo, H, W, C, c4, &win);
+      *reinterpret_cast<uint2*>(static_cast<int16_t*>(p) + 4 * o) =
+          make_uint2((uint32_t(m.x) & 0xffffu) | (uint32_t(m.y) << 16), (uint32_t(m.z) & 0xffffu) | (uint32_t(m.w) << 16));
+      // alpha * p is the conv's fp32 output at the winner (one fp32 multiply, as the conv epilogue)
+      v = make_float4(float(m.x) * al.x, float(m.y) * al.y, float(m.z) * al.z, float(m.w) * al.w);
+    }
     idx[o] = win;
-    // alpha * p is the conv's fp32 output at the winner (one fp32 multiply, as the conv epilogue)
-    const float4 v = make_float4(float(m.x) * al.x, float(m.y) * al.y, float(m.z) * al.z, float(m.w) * al.w);
     sa.x += v.x; sa.y += v.y; sa.z += v.z; sa.w += v.w;
     sb.x += v.x * v.x; sb.y += v.y * v.y; sb.z += v.z * v.z; sb.w += v.w * v.w;
     mx.x = fmaxf(mx.x, fabsf(v.x)); mx.y = fmaxf(mx.y, fabsf(v.y));
@@ -553,9 +594,23 @@ pool2_i16_kernel(const int16_t* __restrict__ y, const float* __restrict__ alpha,
   block_partials(shs, shm, C4, c4, sa, sb, mx, part, maxbits);
 }
 
-template <int MODE>
 __global__ void __launch_bounds__(kBnThreads)
-pool2_bwd_pack_kernel(const float4* __restrict__ gz, const int16_t* __restrict__ p, const uint32_t* __restrict__ idx,
+pool2_i16_kernel(const int16_t* __restrict__ y, const float* __restrict__ alpha, int H, int W, int C4, int64_t n_pool,
+                 int16_t* __restrict__ p, uint32_t* __restrict__ idx, double* __restrict__ part,
+                 uint32_t* __restrict__ maxbits) {
+  pool2_stats<false>(y, alpha, H, W, C4, n_pool, p, idx, part, maxbits);
+}
+
+__global__ void __launch_bounds__(kBnThreads)
+real_pool2_kernel(const float* __restrict__ y, int H, int W, int C4, int64_t n_pool, float* __restrict__ p,
+                  uint32_t* __restrict__ idx, double* __restrict__ part, uint32_t* __restrict__ maxbits) {
+  pool2_stats<true>(y, nullptr, H, W, C4, n_pool, p, idx, part, maxbits);
+}
+
+// I16: p is the int16 p_int of pool2_i16_kernel (consts carry alpha), else the fp32 p of real_pool2_kernel
+template <int MODE, bool I16 = true>
+__global__ void __launch_bounds__(kBnThreads)
+pool2_bwd_pack_kernel(const float4* __restrict__ gz, const void* __restrict__ p, const uint32_t* __restrict__ idx,
                       const float4* __restrict__ consts, const float* __restrict__ ab,
                       const uint32_t* __restrict__ amax_bits, int H, int W, int C4, int64_t n4,
                       uint16_t* __restrict__ out) {
@@ -569,7 +624,7 @@ pool2_bwd_pack_kernel(const float4* __restrict__ gz, const int16_t* __restrict__
   const float4 ha = *reinterpret_cast<const float4*>(ab + c4 * 4);
   const float4 hb = *reinterpret_cast<const float4*>(ab + C + c4 * 4);
   for (; i < n4; i += nthreads) {
-    const float4 v = load_y4<true>(p, i);
+    const float4 v = load_y4<I16>(p, i);
     const float4 g = htanh_mask(__ldcs(gz + i), v, ha, hb);
     const uint32_t win = __ldcs(idx + i);
     const float a0 = (g.x - k0.x - (v.x - k0.z) * k0.y) * k0.w * up;
@@ -606,26 +661,6 @@ pool2_bwd_pack_kernel(const float4* __restrict__ gz, const int16_t* __restrict__
       }
     }
   }
-}
-
-// fp32 y: the max of the window as F.max_pool2d takes it (scan order, `v > m || v is NaN`): NaN if the window holds
-// one, and of equal values (+0.0 / -0.0) the first
-__device__ __forceinline__ float pool2_fmax(float m, float v) { return (v > m || v != v) ? v : m; }
-
-__device__ __forceinline__ float4 pool2_max_f32(const float* __restrict__ y, int64_t n, int ho, int wo, int H, int W,
-                                                int C, int c4) {
-  float4 m;
-#pragma unroll
-  for (int t = 0; t < 4; ++t) {
-    const int64_t off = ((n * H + 2 * ho + (t >> 1)) * W + 2 * wo + (t & 1)) * C + 4 * c4;
-    const float4 v = __ldcs(reinterpret_cast<const float4*>(y + off));
-    if (t == 0) {
-      m = v;
-    } else {
-      m.x = pool2_fmax(m.x, v.x); m.y = pool2_fmax(m.y, v.y); m.z = pool2_fmax(m.z, v.z); m.w = pool2_fmax(m.w, v.w);
-    }
-  }
-  return m;
 }
 
 __global__ void __launch_bounds__(kBnThreads)
@@ -751,18 +786,25 @@ static int bn_fwd_impl(const void* y, const float* alpha_i16, const float* resid
                        float* ab_ws, float* z, uint32_t* sign_bits, uint32_t* mask_bits, uint16_t* xb,
                        uint8_t* xb_fp8, int32_t fmt, int32_t stats_ready, void* stream,
                        const PadResidual* sub = nullptr, bool ht = false, uint32_t* relu_amax = nullptr) {
-  if (relu_amax != nullptr) {      // bdbnn_bn_fwd_relu: fp32 y, no +-1 packs, the ReLU mask words instead
+  // bdbnn_real_bn_fwd_hardtanh: fp32 y, no +-1 packs and no mask words, max|z| into relu_amax
+  const bool ht_real = ht && relu_amax != nullptr;
+  if (relu_amax != nullptr && !ht) {      // bdbnn_bn_fwd_relu: fp32 y, no +-1 packs, the ReLU mask words instead
     BDBNN_REQUIRE(alpha_i16 == nullptr && sub == nullptr && !ht && sign_bits == nullptr && mask_bits != nullptr,
                   "bn_fwd_relu: needs fp32 y and mask_bits");
     BDBNN_REQUIRE((C & 31) == 0, "bn_fwd_relu: the mask words need C %% 32 == 0");
   }
+  if (ht_real)
+    BDBNN_REQUIRE(alpha_i16 == nullptr && sub == nullptr && residual == nullptr && sign_bits == nullptr &&
+                      mask_bits == nullptr && stats_ready,
+                  "real_bn_fwd_hardtanh: fp32 y, no residual, and the statistics ready (stats_ready = 1)");
   const bool pack = sign_bits != nullptr;
   const bool i16 = alpha_i16 != nullptr;
   // 16-channel packs (one word per pixel): the CIFAR stem's BatchNorm, fp32 y only
   const bool p16 = pack && C == 16;
   BDBNN_REQUIRE(!i16 || stats_ready, "bn_fwd_i16: the statistics must come from the conv epilogue (stats_ready = 1)");
   BDBNN_REQUIRE(!(p16 && (i16 || sub)), "bn_fwd: 16-channel packs only without int16 y and option-A residual");
-  BDBNN_REQUIRE(!ht || (pack && !p16 && !sub && !residual), "bn_fwd_hardtanh: needs the packs, C %% 32 == 0 and no residual");
+  BDBNN_REQUIRE(!ht || ht_real || (pack && !p16 && !sub && !residual),
+                "bn_fwd_hardtanh: needs the packs, C %% 32 == 0 and no residual");
   int rc = bn_dims_ok(n_pix, C, pack && !p16);
   if (rc) return rc;
   BDBNN_REQUIRE(y && gamma && beta && sums_ws && ymax_bits && mean && invstd && ab_ws && z, "bn_fwd: NULL pointer");
@@ -786,7 +828,11 @@ static int bn_fwd_impl(const void* y, const float* alpha_i16, const float* resid
   const int grid = bn_grid(n4, C4);
   const float4* r4 = reinterpret_cast<const float4*>(residual);
   float4* z4 = reinterpret_cast<float4*>(z);
-  if (relu_amax != nullptr) {
+  if (ht_real) {
+    BDBNN_CUDA(cudaMemsetAsync(relu_amax, 0, sizeof(uint32_t), st));
+    bn_apply_add_pack_kernel<false, false, 4, false, false, true><<<grid, kBnThreads, 0, st>>>(
+        y, nullptr, a, b, n4, C4, z4, nullptr, nullptr, nullptr, nullptr, 0u, PadResidual{}, relu_amax);
+  } else if (relu_amax != nullptr) {
     BDBNN_CUDA(cudaMemsetAsync(relu_amax, 0, sizeof(uint32_t), st));
     bn_apply_add_pack_kernel<false, false, 4, false, false, false, true><<<grid, kBnThreads, 0, st>>>(
         y, r4, a, b, n4, C4, z4, nullptr, mask_bits, nullptr, nullptr, 0u, PadResidual{}, relu_amax);
@@ -876,6 +922,17 @@ extern "C" int bdbnn_bn_fwd_hardtanh(const void* y, const float* alpha, const fl
   return bn_fwd_impl(y, alpha, nullptr, gamma, beta, n_pix, C, eps, momentum, running_mean, running_var, sums_ws,
                      ymax_bits, mean, invstd, ab_ws, z, sign_bits, mask_bits, xb, xb_fp8, fmt, stats_ready, stream,
                      nullptr, true);
+}
+
+extern "C" int bdbnn_real_bn_fwd_hardtanh(const float* y, const float* gamma, const float* beta, int64_t n_pix,
+                                          int32_t C, float eps, float momentum, float* running_mean,
+                                          float* running_var, double* sums_ws, uint32_t* ymax_bits, float* mean,
+                                          float* invstd, float* ab_ws, float* z, uint32_t* z_amax_bits,
+                                          int32_t stats_ready, void* stream) {
+  BDBNN_REQUIRE(z_amax_bits != nullptr, "real_bn_fwd_hardtanh: NULL z_amax_bits");
+  return bn_fwd_impl(y, nullptr, nullptr, gamma, beta, n_pix, C, eps, momentum, running_mean, running_var, sums_ws,
+                     ymax_bits, mean, invstd, ab_ws, z, nullptr, nullptr, nullptr, nullptr, BDBNN_FMT_FP16,
+                     stats_ready, stream, nullptr, true, z_amax_bits);
 }
 
 extern "C" int bdbnn_bn_fwd_i16(const int16_t* y_int, const float* alpha, const float* residual, const float* gamma,
@@ -1056,11 +1113,12 @@ static int pool2_dims_ok(const char* what, int32_t N, int32_t H, int32_t W, int3
   return BDBNN_OK;
 }
 
-extern "C" int bdbnn_pool2_i16(const int16_t* y_int, const float* alpha, int32_t N, int32_t H, int32_t W, int32_t C,
-                               int16_t* p_int, uint8_t* idx, double* sums, uint32_t* ymax_bits, void* stream) {
-  int rc = pool2_dims_ok("pool2_i16", N, H, W, C);
+// pool2_i16 (alpha != NULL: int16 y and p) and real_pool2 (alpha NULL: fp32 y and p)
+static int pool2_stats_impl(const char* what, const void* y, const float* alpha, int32_t N, int32_t H, int32_t W,
+                            int32_t C, void* p, uint8_t* idx, double* sums, uint32_t* ymax_bits, void* stream) {
+  int rc = pool2_dims_ok(what, N, H, W, C);
   if (rc) return rc;
-  BDBNN_REQUIRE(y_int && alpha && p_int && idx && sums && ymax_bits, "pool2_i16: NULL pointer");
+  BDBNN_REQUIRE(y && p && idx && sums && ymax_bits, "%s: NULL pointer", what);
   cudaStream_t st = cudaStream_t(stream);
   const int C4 = C / 4;
   const int64_t n_pool = int64_t(N) * (H / 2) * (W / 2);
@@ -1070,11 +1128,80 @@ extern "C" int bdbnn_pool2_i16(const int16_t* y_int, const float* alpha, int32_t
   double* part = nullptr;
   rc = det_sums_alloc(&part, grid, 2 * C, st);
   if (rc) return rc;
-  pool2_i16_kernel<<<grid, kBnThreads, 2 * kBnThreads * sizeof(float4) + size_t(C) * sizeof(uint32_t), st>>>(
-      y_int, alpha, H, W, C4, n_pool, p_int, reinterpret_cast<uint32_t*>(idx), part, ymax_bits);
-  rc = check_launch("pool2_i16_kernel");
+  const size_t smem = 2 * kBnThreads * sizeof(float4) + size_t(C) * sizeof(uint32_t);
+  uint32_t* win = reinterpret_cast<uint32_t*>(idx);
+  if (alpha != nullptr) {
+    pool2_i16_kernel<<<grid, kBnThreads, smem, st>>>(static_cast<const int16_t*>(y), alpha, H, W, C4, n_pool,
+                                                     static_cast<int16_t*>(p), win, part, ymax_bits);
+    rc = check_launch("pool2_i16_kernel");
+  } else {
+    real_pool2_kernel<<<grid, kBnThreads, smem, st>>>(static_cast<const float*>(y), H, W, C4, n_pool,
+                                                      static_cast<float*>(p), win, part, ymax_bits);
+    rc = check_launch("real_pool2_kernel");
+  }
   if (rc) { cudaFreeAsync(part, st); return rc; }
   return det_sums_finish(part, grid, 2 * C, sums, st);
+}
+
+extern "C" int bdbnn_pool2_i16(const int16_t* y_int, const float* alpha, int32_t N, int32_t H, int32_t W, int32_t C,
+                               int16_t* p_int, uint8_t* idx, double* sums, uint32_t* ymax_bits, void* stream) {
+  int rc = pool2_dims_ok("pool2_i16", N, H, W, C);
+  if (rc) return rc;
+  BDBNN_REQUIRE(y_int && alpha && p_int && idx && sums && ymax_bits, "pool2_i16: NULL pointer");
+  return pool2_stats_impl("pool2_i16", y_int, alpha, N, H, W, C, p_int, idx, sums, ymax_bits, stream);
+}
+
+extern "C" int bdbnn_real_pool2(const float* y, int32_t N, int32_t H, int32_t W, int32_t C, float* p, uint8_t* idx,
+                                double* sums, uint32_t* pmax_bits, void* stream) {
+  return pool2_stats_impl("real_pool2", y, nullptr, N, H, W, C, p, idx, sums, pmax_bits, stream);
+}
+
+// pool2_bn_bwd_pack (alpha != NULL: int16 p) and real_pool2_bn_bwd_pack (alpha NULL: fp32 p)
+static int pool2_bn_bwd_pack_impl(const char* what, const float* gz, const void* p, const uint8_t* idx,
+                                  const float* alpha, const float* ab, const float* mean, const float* invstd,
+                                  const float* gamma, const float* gscale, const uint32_t* ymax_bits, int32_t N,
+                                  int32_t H, int32_t W, int32_t C, int32_t grad_mode, double* sums_ws,
+                                  uint32_t* gmax_bits, float* consts_ws, float* dgamma, float* dbeta,
+                                  uint32_t* amax_bits, uint16_t* gys, void* stream) {
+  int rc = pool2_dims_ok(what, N, H, W, C);
+  if (rc) return rc;
+  BDBNN_REQUIRE(gz && p && idx && ab && mean && invstd && gamma && gscale && ymax_bits && sums_ws && gmax_bits &&
+                    consts_ws && dgamma && dbeta && amax_bits && gys,
+                "%s: NULL pointer", what);
+  BDBNN_REQUIRE(grad_mode >= BDBNN_GRAD_BF16 && grad_mode <= BDBNN_GRAD_FP16S, "%s: bad grad_mode", what);
+  const bool i16 = alpha != nullptr;
+  cudaStream_t st = cudaStream_t(stream);
+  const int C4 = C / 4;
+  const int64_t n_pool = int64_t(N) * (H / 2) * (W / 2);
+  BDBNN_CUDA(cudaMemsetAsync(sums_ws, 0, size_t(2 * C) * sizeof(double), st));
+  BDBNN_CUDA(cudaMemsetAsync(gmax_bits, 0, size_t(C) * sizeof(uint32_t), st));
+  // BatchNorm's backward over the pooled tensor (it normalised the pooled values); each conv-output position takes at
+  // most one pooled gradient, so the FP16S bound needs no multiplier
+  const int rgrid = bn_grid(n_pool * C4 / 8, C4, 3);
+  const float4* g4 = reinterpret_cast<const float4*>(gz);
+  if (i16)
+    rc = bn_reduce_launch<true, true, true>(rgrid, g4, p, mean, invstd, n_pool, C4, sums_ws, gmax_bits, alpha, st, ab);
+  else
+    rc = bn_reduce_launch<true, false, true>(rgrid, g4, p, mean, invstd, n_pool, C4, sums_ws, gmax_bits, nullptr, st,
+                                             ab);
+  if (rc) return rc;
+  bn_bwd_bound_kernel<<<1, 256, 0, st>>>(sums_ws, gmax_bits, ymax_bits, n_pool, C, mean, invstd, gamma, gscale,
+                                         reinterpret_cast<float4*>(consts_ws), dgamma, dbeta, amax_bits, 1.0f, alpha);
+  rc = check_launch("bn_bwd_bound_kernel");
+  if (rc) return rc;
+  const int64_t n4 = n_pool * C4;
+  const int grid = bn_grid(n4, C4);
+  const float4* k4 = reinterpret_cast<const float4*>(consts_ws);
+  const uint32_t* w4 = reinterpret_cast<const uint32_t*>(idx);
+  if (!i16)
+    pool2_bwd_pack_kernel<3, false><<<grid, kBnThreads, 0, st>>>(g4, p, w4, k4, ab, amax_bits, H, W, C4, n4, gys);
+  else if (grad_mode == BDBNN_GRAD_FP16S)
+    pool2_bwd_pack_kernel<3><<<grid, kBnThreads, 0, st>>>(g4, p, w4, k4, ab, amax_bits, H, W, C4, n4, gys);
+  else if (grad_mode == BDBNN_GRAD_BF16X2)
+    pool2_bwd_pack_kernel<2><<<grid, kBnThreads, 0, st>>>(g4, p, w4, k4, ab, amax_bits, H, W, C4, n4, gys);
+  else
+    pool2_bwd_pack_kernel<1><<<grid, kBnThreads, 0, st>>>(g4, p, w4, k4, ab, amax_bits, H, W, C4, n4, gys);
+  return check_launch("pool2_bwd_pack_kernel");
 }
 
 extern "C" int bdbnn_pool2_bn_bwd_pack(const float* gz, const int16_t* p_int, const uint8_t* idx, const float* alpha,
@@ -1085,36 +1212,21 @@ extern "C" int bdbnn_pool2_bn_bwd_pack(const float* gz, const int16_t* p_int, co
                                        uint16_t* gys, void* stream) {
   int rc = pool2_dims_ok("pool2_bn_bwd_pack", N, H, W, C);
   if (rc) return rc;
-  BDBNN_REQUIRE(gz && p_int && idx && alpha && ab && mean && invstd && gamma && gscale && ymax_bits && sums_ws &&
-                    gmax_bits && consts_ws && dgamma && dbeta && amax_bits && gys,
-                "pool2_bn_bwd_pack: NULL pointer");
-  BDBNN_REQUIRE(grad_mode >= BDBNN_GRAD_BF16 && grad_mode <= BDBNN_GRAD_FP16S, "pool2_bn_bwd_pack: bad grad_mode");
-  cudaStream_t st = cudaStream_t(stream);
-  const int C4 = C / 4;
-  const int64_t n_pool = int64_t(N) * (H / 2) * (W / 2);
-  BDBNN_CUDA(cudaMemsetAsync(sums_ws, 0, size_t(2 * C) * sizeof(double), st));
-  BDBNN_CUDA(cudaMemsetAsync(gmax_bits, 0, size_t(C) * sizeof(uint32_t), st));
-  // BatchNorm's backward over the pooled tensor (it normalised the pooled values); each conv-output position takes at
-  // most one pooled gradient, so the FP16S bound needs no multiplier
-  rc = bn_reduce_launch<true, true, true>(bn_grid(n_pool * C4 / 8, C4, 3), reinterpret_cast<const float4*>(gz), p_int,
-                                          mean, invstd, n_pool, C4, sums_ws, gmax_bits, alpha, st, ab);
-  if (rc) return rc;
-  bn_bwd_bound_kernel<<<1, 256, 0, st>>>(sums_ws, gmax_bits, ymax_bits, n_pool, C, mean, invstd, gamma, gscale,
-                                         reinterpret_cast<float4*>(consts_ws), dgamma, dbeta, amax_bits, 1.0f, alpha);
-  rc = check_launch("bn_bwd_bound_kernel");
-  if (rc) return rc;
-  const int64_t n4 = n_pool * C4;
-  const int grid = bn_grid(n4, C4);
-  const float4* g4 = reinterpret_cast<const float4*>(gz);
-  const float4* k4 = reinterpret_cast<const float4*>(consts_ws);
-  const uint32_t* w4 = reinterpret_cast<const uint32_t*>(idx);
-  if (grad_mode == BDBNN_GRAD_FP16S)
-    pool2_bwd_pack_kernel<3><<<grid, kBnThreads, 0, st>>>(g4, p_int, w4, k4, ab, amax_bits, H, W, C4, n4, gys);
-  else if (grad_mode == BDBNN_GRAD_BF16X2)
-    pool2_bwd_pack_kernel<2><<<grid, kBnThreads, 0, st>>>(g4, p_int, w4, k4, ab, amax_bits, H, W, C4, n4, gys);
-  else
-    pool2_bwd_pack_kernel<1><<<grid, kBnThreads, 0, st>>>(g4, p_int, w4, k4, ab, amax_bits, H, W, C4, n4, gys);
-  return check_launch("pool2_bwd_pack_kernel");
+  BDBNN_REQUIRE(alpha != nullptr, "pool2_bn_bwd_pack: NULL pointer");
+  return pool2_bn_bwd_pack_impl("pool2_bn_bwd_pack", gz, p_int, idx, alpha, ab, mean, invstd, gamma, gscale,
+                                ymax_bits, N, H, W, C, grad_mode, sums_ws, gmax_bits, consts_ws, dgamma, dbeta,
+                                amax_bits, gys, stream);
+}
+
+extern "C" int bdbnn_real_pool2_bn_bwd_pack(const float* gz, const float* p, const uint8_t* idx, const float* ab,
+                                            const float* mean, const float* invstd, const float* gamma,
+                                            const float* gscale, const uint32_t* pmax_bits, int32_t N, int32_t H,
+                                            int32_t W, int32_t C, double* sums_ws, uint32_t* gmax_bits,
+                                            float* consts_ws, float* dgamma, float* dbeta, uint32_t* amax_bits,
+                                            uint16_t* gys, void* stream) {
+  return pool2_bn_bwd_pack_impl("real_pool2_bn_bwd_pack", gz, p, idx, nullptr, ab, mean, invstd, gamma, gscale,
+                                pmax_bits, N, H, W, C, BDBNN_GRAD_FP16S, sums_ws, gmax_bits, consts_ws, dgamma, dbeta,
+                                amax_bits, gys, stream);
 }
 
 extern "C" int bdbnn_pool2_bn_eval_hardtanh(const int16_t* y_int, const float* scale, const float* shift, int32_t N,

@@ -1739,15 +1739,18 @@ class _CifarStem(torch.autograd.Function):
     """z = BN_train(conv3x3(x, W)) for the CIFAR stem (csrc/cifar_stem.cu, csrc/bn.cu).
     forward : cifar_stem_fwd (fp32 direct conv + BN statistics) -> bn_fwd (z + the first binary conv's packs)
     backward: bn_bwd_pack (dgamma, dbeta, fp16 x 2^e gradient operand) -> cifar_stem_wgrad ; no input gradient.
-    Saved for backward: the images, y and the BN constants."""
+    `real` (with hardtanh, real_cifar_stem_conv_bn): the apply is real_bn_fwd_hardtanh, z and its max|z| word, no
+    packs.  Saved for backward: the images, y and the BN constants."""
 
     @staticmethod
     @_on_device
-    def forward(ctx, x, weight, gamma, beta, running_mean, running_var, momentum, eps, hardtanh=False):
+    def forward(ctx, x, weight, gamma, beta, running_mean, running_var, momentum, eps, hardtanh=False, real=False):
         _require_cuda(x, "cifar_stem_conv_bn(x)")
         _require_cuda(weight, "cifar_stem_conv_bn(weight)")
         _same_device(x, weight, gamma, beta, running_mean, running_var)
         ctx.hardtanh = bool(hardtanh)
+        if real and not hardtanh:
+            raise RuntimeError("bdbnn_b200.cifar_stem_conv_bn: the real-output stem is the Hardtanh one")
         if not cifar_stem_supported(x.shape, weight.shape, (1, 1), (1, 1), ctx.hardtanh):
             raise RuntimeError(f"bdbnn_b200.cifar_stem_conv_bn: unsupported input {tuple(x.shape)} / weight "
                                f"{tuple(weight.shape)}")
@@ -1769,7 +1772,7 @@ class _CifarStem(torch.autograd.Function):
                                               _p(y), _p(sums), _p(ymax), st), "cifar_stem_fwd")
         _lib.count(2)       # conv, statistics sum
         fmt = grad_mode()[3]
-        pack = cout % 32 == 0 or cout == 16
+        pack = not real and (cout % 32 == 0 or cout == 16)
         i32 = dict(dtype=torch.int32, device=dev)
         cw = (cout + 31) // 32
         zs = torch.empty((n, h, w, cw), **i32) if pack else None
@@ -1779,8 +1782,14 @@ class _CifarStem(torch.autograd.Function):
                                                                                 fwd8_enabled()) else None
         z = torch.empty_like(y)
         mean, invstd, ab = torch.empty((cout,), **f32), torch.empty((cout,), **f32), torch.empty((2 * cout,), **f32)
+        z_amax = torch.empty((1,), **i32) if real else None
         with _timed("cifar_stem_bn_fwd", key, (8 + (2.25 if pack else 0) + (1 if zb8 is not None else 0)) * y.numel()):
-            if ctx.hardtanh:
+            if real:
+                _lib.check(L.bdbnn_real_bn_fwd_hardtanh(_p(y), _p(gamma.detach()), _p(beta.detach()), n_pix, cout,
+                                                        float(eps), float(momentum), _p(running_mean), _p(running_var),
+                                                        _p(sums), _p(ymax), _p(mean), _p(invstd), _p(ab), _p(z),
+                                                        _p(z_amax), 1, st), "real_bn_fwd_hardtanh(cifar stem)")
+            elif ctx.hardtanh:
                 _lib.check(L.bdbnn_bn_fwd_hardtanh(_p(y), None, _p(gamma.detach()), _p(beta.detach()), n_pix, cout,
                                                    float(eps), float(momentum), _p(running_mean), _p(running_var),
                                                    _p(sums), _p(ymax), _p(mean), _p(invstd), _p(ab), _p(z), _p(zs),
@@ -1794,16 +1803,16 @@ class _CifarStem(torch.autograd.Function):
         ctx.geom = (n, h, w, cout)
         ctx.w_param = weight if (weight.is_leaf and weight.requires_grad) else None
         ctx.save_for_backward(xd, y, mean, invstd, gamma.detach(), ymax, *((ab,) if ctx.hardtanh else ()))
-        nd = [t for t in (zs, zm, zb, zb8) if t is not None]
+        nd = [t for t in (zs, zm, zb, zb8, z_amax) if t is not None]
         if nd:
             ctx.mark_non_differentiable(*nd)
-        return z, zs, zm, zb, zb8
+        return z, zs, zm, zb, zb8, z_amax
 
     @staticmethod
     @_on_device
     def backward(ctx, gz, *_unused):
         if gz is None or not (ctx.needs_input_grad[1] or ctx.needs_input_grad[2] or ctx.needs_input_grad[3]):
-            return (None,) * 9
+            return (None,) * 10
         L = _lib.lib()
         xd, y, mean, invstd, gamma, ymax = ctx.saved_tensors[:6]
         n, h, w, cout = ctx.geom
@@ -1832,7 +1841,7 @@ class _CifarStem(torch.autograd.Function):
                 int(L.bdbnn_cifar_stem_wgrad_workspace_bytes(n, h, w, cout)), (cout, 3, 3, 3), ctx.w_param,
                 (xd, gys, amax), "cifar_stem_wgrad", key, 4 * xd.numel() + 2 * gys.numel())
         return (None, gw, dgamma if ctx.needs_input_grad[2] else None, dbeta if ctx.needs_input_grad[3] else None,
-                None, None, None, None, None)
+                None, None, None, None, None, None)
 
 
 def cifar_stem_conv_bn(x, weight, gamma, beta, running_mean, running_var, momentum, eps, hardtanh=False):
@@ -1840,11 +1849,20 @@ def cifar_stem_conv_bn(x, weight, gamma, beta, running_mean, running_var, moment
     conv, BatchNorm with its running-statistics update (the caller adds 1 to num_batches_tracked), TF32-class weight
     gradient, no input gradient.  The result carries `_bdbnn_pack` for the first binary conv.  `hardtanh`: the result
     is hardtanh(BN_train(...)) with Hardtanh's strict mask in the pack (conv_bn_add(hardtanh=True))."""
-    z, zs, zm, zb, zb8 = _CifarStem.apply(x, weight, gamma, beta, running_mean, running_var, momentum, eps,
-                                          bool(hardtanh))
+    z, zs, zm, zb, zb8, _ = _CifarStem.apply(x, weight, gamma, beta, running_mean, running_var, momentum, eps,
+                                             bool(hardtanh))
     if zs is not None:
         _set_act_pack(z, _ActPack(zs, zm, zb, grad_mode()[3], zb8))
     return z
+
+
+def real_cifar_stem_conv_bn(x, weight, gamma, beta, running_mean, running_var, momentum, eps):
+    """hardtanh(BN_train(conv2d(x, weight, stride 1, pad 1))) of the fp32 VGG-Small's stem (DESIGN.md §4u;
+    cifar_stem_supported(..., hardtanh=True)) as one node: cifar_stem_conv_bn(hardtanh=True) whose BatchNorm apply
+    writes no +-1 packs but the max|z| word of the next real-valued conv (real_bn_fwd_hardtanh).  No input gradient.
+    Returns (z fp32 channels_last, z_amax int32[1] = bits of max|z|)."""
+    z, *_, z_amax = _CifarStem.apply(x, weight, gamma, beta, running_mean, running_var, momentum, eps, True, True)
+    return z, z_amax
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -2606,10 +2624,14 @@ def _real_conv_launches(sh, groups):
 
 
 def _real_unit_fwd(x, x_amax, op, wpack, w_shape, gamma, beta, residual, running_mean, running_var, momentum, eps,
-                   stride, padding, relu=True, groups=1):
-    """Forward of one real-valued conv + BatchNorm(train) (+ residual) (+ ReLU) unit:
+                   stride, padding, relu=True, groups=1, hardtanh=False, pool=False):
+    """Forward of one real-valued conv (+ 2x2 max-pool) + BatchNorm(train) (+ residual) (+ ReLU or Hardtanh) unit:
     real_act_pack(x, x_amax) -> real_scale_fold -> binconv_fwd_tc (fp16 operands, BatchNorm statistics in the
     epilogue) -> bn_fwd_relu (z, ReLU's mask words, max|z|), or without `relu` bn_fwd (z only; no residual).
+    `hardtanh` (relu False, no residual, groups 1): real_bn_fwd_hardtanh (z = hardtanh(u), max|z|; the backward
+    recomputes Hardtanh's mask from y and ab).  `pool` (with hardtanh, DESIGN.md §4u): the conv writes y without
+    statistics, real_pool2 takes its 2x2 max p, the winner bytes and p's statistics, the BatchNorm and Hardtanh apply
+    to p, and y is freed: the backward reads p and the winners.
     op: (xh, amax), x's fp16 operand and the amax word it was scaled by when another unit already made it, else None.
     groups > 1: a grouped conv on the banded GEMM (real_gconv_fwd, DESIGN.md §4t), wpack its banded operands.
     Returns (z, z_amax or None, the tensors the backward reads, the conv's shape)."""
@@ -2618,6 +2640,11 @@ def _real_unit_fwd(x, x_amax, op, wpack, w_shape, gamma, beta, residual, running
     if not real_unit_supported(x.shape, w_shape, stride, padding, REAL_MAX_COUT, groups):
         raise RuntimeError(f"bdbnn_b200.real_conv_bn_relu: no kernel for input {tuple(x.shape)}, weight "
                            f"{tuple(w_shape)}, stride {stride}, padding {padding}")
+    if hardtanh and (relu or residual is not None or groups != 1):
+        raise RuntimeError("bdbnn_b200.real_conv_bn_hardtanh: the Hardtanh unit takes no ReLU, residual or groups")
+    if pool and not (hardtanh and sh.Ho % 2 == 0 and sh.Wo % 2 == 0):
+        raise RuntimeError(f"bdbnn_b200.real_conv_bn_hardtanh: the 2x2 pool follows a Hardtanh unit's conv with an even "
+                           f"output, got {sh.Ho}x{sh.Wo}")
     z_shape = (sh.N, sh.Cout, sh.Ho, sh.Wo)
     if residual is not None and tuple(residual.shape) != z_shape:
         raise RuntimeError(f"real_conv_bn_relu: residual shape {tuple(residual.shape)} != output shape {z_shape}")
@@ -2632,12 +2659,31 @@ def _real_unit_fwd(x, x_amax, op, wpack, w_shape, gamma, beta, residual, running
     sums = torch.empty((2 * cout,), dtype=torch.float64, device=dev)
     ymax = torch.empty((cout,), dtype=torch.int32, device=dev)
     fwd, _, _ = _real_conv_launches(sh, groups)
-    fwd(xh, wpack.wf, alpha, y, sums, ymax)
+    fwd(xh, wpack.wf, alpha, y, *((None, None) if pool else (sums, ymax)))
     _lib.count(1)
+    idx = None
+    if pool:
+        # y -> p, the winners and p's statistics (max|p| in ymax); the BatchNorm and the backward read p
+        p = torch.empty((sh.N, cout, sh.Ho // 2, sh.Wo // 2), memory_format=torch.channels_last, **f32)
+        idx = torch.empty((sh.N, sh.Ho // 2, sh.Wo // 2, cout), dtype=torch.uint8, device=dev)
+        with _timed("real_pool2", key, 4 * y.numel() + 5 * p.numel()):
+            _lib.check(L.bdbnn_real_pool2(_p(y), sh.N, sh.Ho, sh.Wo, cout, _p(p), _p(idx), _p(sums), _p(ymax), st),
+                       "real_pool2")
+        _lib.count(2)       # pool, statistics sum
+        y = p
+        n_pix = y.numel() // cout
     z = torch.empty_like(y)
     mean, invstd, ab = torch.empty((cout,), **f32), torch.empty((cout,), **f32), torch.empty((2 * cout,), **f32)
     mask = z_amax = None
-    if relu:
+    if hardtanh:
+        z_amax = torch.empty((1,), dtype=torch.int32, device=dev)
+        with _timed("real_bn_fwd_hardtanh", key, 8 * n_pix * cout):
+            _lib.check(L.bdbnn_real_bn_fwd_hardtanh(_p(y), _p(gamma.detach()), _p(beta.detach()), n_pix, cout,
+                                                    float(eps), float(momentum), _p(running_mean), _p(running_var),
+                                                    _p(sums), _p(ymax), _p(mean), _p(invstd), _p(ab), _p(z),
+                                                    _p(z_amax), 1, st), "real_bn_fwd_hardtanh")
+        mask = ab       # the backward's Hardtanh mask is recomputed from y and the forward's ab
+    elif relu:
         rc = _nhwc(residual.detach()) if residual is not None else None
         mask = torch.empty((sh.N, sh.Ho, sh.Wo, cout // 32), dtype=torch.int32, device=dev)
         z_amax = torch.empty((1,), dtype=torch.int32, device=dev)
@@ -2655,26 +2701,44 @@ def _real_unit_fwd(x, x_amax, op, wpack, w_shape, gamma, beta, residual, running
                                       _p(mean), _p(invstd), _p(ab), _p(z), None, None, None, None, 0, 1, st),
                        "bn_fwd(real)")
     _lib.count(2)
-    saved = (y, mean, invstd, gamma.detach(), ymax, mask, xh, wpack.wt, wpack.wmask, wpack.gscale, inv_gscale)
+    saved = (y, mean, invstd, gamma.detach(), ymax, mask, xh, wpack.wt, wpack.wmask, wpack.gscale, inv_gscale, idx)
     return z, z_amax, saved, sh
 
 
+REAL_UNIT_SAVED = 12     # tensors (or None) _real_unit_fwd saves per unit
+
+
 def _real_unit_bwd(gz, saved, sh, x_shape, w_shape, w_param, need_x, need_w, need_res, relu=True, add=None,
-                   out=None, groups=1):
+                   out=None, groups=1, hardtanh=False, pool=False):
     """Backward of _real_unit_fwd: bn_bwd_pack_relu (gz masked, which is also the residual's gradient), or without
-    `relu` bn_bwd_pack -> wgrad_tc, dgrad_tc with all-ones STE masks.  add: an fp32 NHWC tensor of x's shape that
-    dgrad's epilogue adds into gx; out: the tensor gx is written to (may be `add`), else a fresh one.  groups > 1: the
-    banded dgrad and wgrad (real_gconv_dgrad / _wgrad, DESIGN.md §4t).
+    `relu` bn_bwd_pack, or with `hardtanh` bn_bwd_pack_hardtanh (gz times the strict mask recomputed from y and ab)
+    and with `pool` real_pool2_bn_bwd_pack (the same over p, gys at the conv resolution: the value at the winner, 0
+    elsewhere) -> wgrad_tc, dgrad_tc with all-ones STE masks.  add: an fp32 NHWC tensor of x's shape that dgrad's
+    epilogue adds into gx; out: the tensor gx is written to (may be `add`), else a fresh one.  groups > 1: the banded
+    dgrad and wgrad (real_gconv_dgrad / _wgrad, DESIGN.md §4t).
     Returns (gx, gw, dgamma, dbeta, gres)."""
     L = _lib.lib()
-    y, mean, invstd, gamma, ymax, mask, xh, wt, wmask, gscale, inv_gscale = saved
+    y, mean, invstd, gamma, ymax, mask, xh, wt, wmask, gscale, inv_gscale, idx = saved
     dev = gz.device
     key = _shape_key(sh)
     g = _nhwc(gz)
     cout, n_pix = sh.Cout, sh.N * sh.Ho * sh.Wo
     sums, gmax, consts, dgamma, dbeta, amax, gys = _bn_grads(cout, (sh.N, sh.Ho, sh.Wo), 1, dev)
     gres = None
-    if relu:
+    if pool:
+        n_pool = y.numel() // cout
+        with _timed("real_pool2_bn_bwd_pack", key, (4 + 4 + 1) * n_pool * cout + 2 * gys.numel()):
+            _lib.check(L.bdbnn_real_pool2_bn_bwd_pack(_p(g), _p(y), _p(idx), _p(mask), _p(mean), _p(invstd), _p(gamma),
+                                                      _p(gscale), _p(ymax), sh.N, sh.Ho, sh.Wo, cout, _p(sums),
+                                                      _p(gmax), _p(consts), _p(dgamma), _p(dbeta), _p(amax), _p(gys),
+                                                      _stream()), "real_pool2_bn_bwd_pack")
+    elif hardtanh:
+        with _timed("real_bn_bwd_pack_hardtanh", key, 18 * n_pix * cout):
+            _lib.check(L.bdbnn_bn_bwd_pack_hardtanh(_p(g), _p(y), None, _p(mask), _p(mean), _p(invstd), _p(gamma),
+                                                    _p(gscale), _p(ymax), n_pix, cout, GRAD_MODES["fp16s"], _p(sums),
+                                                    _p(gmax), _p(consts), _p(dgamma), _p(dbeta), _p(amax), _p(gys),
+                                                    _stream()), "bn_bwd_pack_hardtanh(real)")
+    elif relu:
         if need_res:
             gres = torch.empty((sh.N, cout, sh.Ho, sh.Wo), dtype=torch.float32, device=dev,
                                memory_format=torch.channels_last)
@@ -2704,20 +2768,22 @@ def _real_unit_bwd(gz, saved, sh, x_shape, w_shape, w_param, need_x, need_w, nee
 
 class _RealConvBNReLU(torch.autograd.Function):
     """z = relu(BN_train(conv2d(x, W, stride, padding)) + residual) of a real-valued 3x3 (padding 1) or 1x1
-    (padding 0) conv (DESIGN.md §4r, §4s): _real_unit_fwd and _real_unit_bwd as one autograd node."""
+    (padding 0) conv (DESIGN.md §4r, §4s), or with `hardtanh` z = hardtanh(BN_train([maxpool2x2](conv2d(x, W))))
+    (DESIGN.md §4u): _real_unit_fwd and _real_unit_bwd as one autograd node."""
 
     @staticmethod
     @_on_device
     def forward(ctx, x, weight, gamma, beta, residual, x_amax, wpack, running_mean, running_var, momentum, eps, stride,
-                padding=1, groups=1):
-        _require_cuda(x, "real_conv_bn_relu(x)")
+                padding=1, groups=1, hardtanh=False, pool=False):
+        what = "real_conv_bn_hardtanh" if hardtanh else "real_conv_bn_relu"
+        _require_cuda(x, f"{what}(x)")
         _same_device(x, weight, gamma, beta, residual, x_amax, running_mean, running_var)
-        _require_fp16s("real_conv_bn_relu")
+        _require_fp16s(what)
         ctx.set_materialize_grads(False)
         z, z_amax, saved, ctx.sh = _real_unit_fwd(x, x_amax, None, wpack, tuple(weight.shape), gamma, beta, residual,
                                                   running_mean, running_var, momentum, eps, stride, padding,
-                                                  groups=groups)
-        ctx.groups = groups
+                                                  relu=not hardtanh, groups=groups, hardtanh=hardtanh, pool=pool)
+        ctx.groups, ctx.hardtanh, ctx.pool = groups, hardtanh, pool
         ctx.x_shape, ctx.w_shape = tuple(x.shape), tuple(weight.shape)
         ctx.w_param = weight if (weight.is_leaf and weight.requires_grad) else None
         ctx.has_res = residual is not None
@@ -2729,13 +2795,14 @@ class _RealConvBNReLU(torch.autograd.Function):
     @_on_device
     def backward(ctx, gz, _g_amax):
         if gz is None:
-            return (None,) * 14
+            return (None,) * 16
         need = ctx.needs_input_grad
         gx, gw, dgamma, dbeta, gres = _real_unit_bwd(gz, ctx.saved_tensors, ctx.sh, ctx.x_shape, ctx.w_shape,
                                                      ctx.w_param, need[0], need[1], ctx.has_res and need[4],
-                                                     groups=ctx.groups)
+                                                     relu=not ctx.hardtanh, groups=ctx.groups, hardtanh=ctx.hardtanh,
+                                                     pool=ctx.pool)
         return (gx, gw, dgamma if need[2] else None, dbeta if need[3] else None, gres,
-                None, None, None, None, None, None, None, None, None)
+                None, None, None, None, None, None, None, None, None, None, None)
 
 
 def real_conv_bn_relu(x, x_amax, wpack, weight, gamma, beta, running_mean, running_var, momentum, eps, stride,
@@ -2748,6 +2815,16 @@ def real_conv_bn_relu(x, x_amax, wpack, weight, gamma, beta, running_mean, runni
     conv with wpack from real_weight_grad_pack(..., groups), on the banded kernels (DESIGN.md §4t)."""
     return _RealConvBNReLU.apply(x, weight, gamma, beta, residual, x_amax, wpack, running_mean, running_var,
                                  float(momentum), float(eps), int(stride), int(padding), int(groups))
+
+
+def real_conv_bn_hardtanh(x, x_amax, wpack, weight, gamma, beta, running_mean, running_var, momentum, eps, pool=False):
+    """z = hardtanh(BN_train(conv2d(x, weight, stride 1, padding 1))) of a real-valued 3x3 conv on the wgmma kernels,
+    with autograd: a unit of the fp32 VGG-Small (DESIGN.md §4u; geometry: real_unit_supported; gradient mode fp16s).
+    `pool`: z = hardtanh(BN_train(max_pool2d(conv2d(...), 2, 2))), the conv output even and Cout % 32 == 0; the
+    BatchNorm follows the max, as in the model.  wpack, x_amax as real_conv_bn_relu.  Returns (z fp32 channels_last,
+    z_amax int32[1] = bits of max|z|)."""
+    return _RealConvBNReLU.apply(x, weight, gamma, beta, None, x_amax, wpack, running_mean, running_var,
+                                 float(momentum), float(eps), 1, 1, 1, True, bool(pool))
 
 
 class _RealBottleneck(torch.autograd.Function):
@@ -2808,7 +2885,8 @@ class _RealBottleneck(torch.autograd.Function):
         need = ctx.needs_input_grad
         need_x = need[0]
         st = ctx.saved_tensors
-        saved = [st[11 * i:11 * i + 11] for i in range(len(ctx.w_shapes))]
+        k = REAL_UNIT_SAVED
+        saved = [st[k * i:k * i + k] for i in range(len(ctx.w_shapes))]
 
         def unit(i, g, need_in, need_res=False, relu=True, add=None, out=None):
             return _real_unit_bwd(g, saved[i], ctx.geoms[i], ctx.in_shapes[i], ctx.w_shapes[i], ctx.w_params[i],

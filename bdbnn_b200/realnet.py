@@ -3,13 +3,14 @@
     model = RealResNet(torchvision.models.resnet18())                # or resnet34
     model = RealBottleneckResNet(torchvision.models.resnet50())      # or resnet101/152, wide_resnet50_2/101_2
     model = RealResNeXt(torchvision.models.resnext50_32x4d())        # or resnext101_32x8d, resnext101_64x4d
+    model = RealVGGSmall(vgg.vgg_small(conv_cls=<bias-free nn.Conv2d>))   # the CIFAR KD step's fp32 teacher
 
 wraps the model without copying it, as FrozenResNetTeacher does: the wrapper's children ARE the model's children, so
 `named_parameters()` and `state_dict()` have the model's names and objects, and `load_state_dict`, `.cuda()` and
 `.train()` act on the model.  Each is a subclass of the teacher of the same kind (FrozenResNetTeacher,
 FrozenBottleneckTeacher, FrozenResNeXtTeacher), whose structure check and eval forward it uses; RealResNet holds the
 training path for both block kinds, and RealBottleneckResNet and RealResNeXt are subclasses whose body is the _KINDS
-they take.
+they take.  RealVGGSmall is FrozenVGGTeacher's subclass, with its own training walk and forward (DESIGN.md §4u).
 
 In training mode, on a CUDA fp32 input whose geometry every unit takes, the forward runs with autograd as
 
@@ -27,7 +28,9 @@ with autograd) returns the wrapped model's own forward."""
 import torch
 
 from . import functional as F_
-from .teacher import FrozenBottleneckTeacher, FrozenResNetTeacher, FrozenResNeXtTeacher
+from .teacher import (_VGG_POOLED, FrozenBottleneckTeacher, FrozenResNetTeacher, FrozenResNeXtTeacher,
+                      FrozenVGGTeacher)
+from .vgg import VGGSmall
 
 
 def _bn_train_args(bn):
@@ -166,3 +169,88 @@ class RealResNeXt(RealBottleneckResNet, FrozenResNeXtTeacher):
     replace_stride_with_dilation, a conv2 with another group count, subclassed models or blocks, mixed blocks,
     nn.DataParallel)."""
     _KINDS = ("resnext",)
+
+
+class RealVGGSmall(FrozenVGGTeacher):
+    """The fp32 CIFAR VGG-Small (bdbnn_b200.vgg.VGGSmall with bias-free nn.Conv2d convs, any class count: the model
+    FrozenVGGTeacher wraps) trained on the real-valued training units (DESIGN.md §4u), with FrozenVGGTeacher's
+    structure check, names, parameters and eval forward.  In training mode, on a CUDA fp32 input that requires no
+    gradient and whose geometry every unit takes, the forward runs with autograd as
+
+        z = hardtanh(BN0_train(conv0(x)))                   real_cifar_stem_conv_bn (no input gradient)
+        z = hardtanh(BN_train(maxpool2x2(conv(z))))         conv1, conv3, conv5: real_conv_bn_hardtanh(pool=True)
+        z = hardtanh(BN_train(conv(z)))                     conv2, conv4: real_conv_bn_hardtanh
+        logits = fc(flatten(z))                             torch, NCHW flattening as VGGSmall.forward
+
+    while `nonlinear` and `pooling` are nn.Hardtanh(-1, 1) and nn.MaxPool2d(2, 2).  Anything else (CPU, other dtypes,
+    BDBNN_FUSE_BN=0, a gradient mode other than fp16s, other shared modules, unsupported geometry, an input that
+    requires grad) returns the wrapped model's own forward.  Raises TypeError for any other structure, as
+    FrozenVGGTeacher."""
+
+    def kernel_path(self, x):
+        """True when forward(x) runs on this repository's kernels: the training units in training mode, the eval
+        kernels in eval mode (FrozenVGGTeacher.kernel_path)."""
+        if self.training:
+            return self._train_supported(x)
+        return super().kernel_path(x)
+
+    def forward(self, x):
+        if not self.training:
+            return super().forward(x)            # the eval kernels through kernel_path, else the model
+        if not self.kernel_path(x):
+            return self._wrapped(x)
+        with torch.cuda.device(x.device):
+            return self._train_forward(x)
+
+    # ---- path selection ----------------------------------------------------------------------------------------
+    def _train_supported(self, x):
+        if not F_.fuse_enabled():
+            return False
+        if not (torch.is_tensor(x) and x.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and x.shape[1] == 3 and
+                not x.requires_grad):
+            return False
+        if F_.grad_mode()[0] != "fp16s":
+            return False
+        for bn in self._bns():
+            if not (bn.training and bn.affine and bn.track_running_stats and bn.momentum is not None and
+                    bn.running_mean is not None):
+                return False
+        if any(p.device != x.device or p.dtype != torch.float32 for p in self.parameters()):
+            return False
+        if not (VGGSmall._modules_standard(self) and self._wrapped._modules_standard()):
+            return False
+        key = (x.device, tuple(x.shape), "train")      # in the eval walk's cache, apart from its keys
+        ok = self._geom_ok.get(key)
+        if ok is None:
+            ok = self._geom_ok[key] = self._walk_train_geometry(x)
+        return ok
+
+    def _walk_train_geometry(self, x):
+        """The stem's kernel takes x, every conv has all three wgmma kernels (real_unit_supported), and every pooled
+        conv output is even (host-only)."""
+        n, _, h, w = x.shape
+        c0 = self.conv0
+        if not F_.cifar_stem_supported(tuple(x.shape), tuple(c0.weight.shape), c0.stride, c0.padding, True):
+            return False
+        shape = (n, c0.out_channels, h, w)
+        for i, pooled in enumerate(_VGG_POOLED):
+            w_shape = tuple(getattr(self, f"conv{i + 1}").weight.shape)
+            if not F_.real_unit_supported(shape, w_shape, 1, 1):
+                return False
+            sh = F_.conv_shape(shape, w_shape, 1, 1)
+            if pooled and (sh.Ho % 2 or sh.Wo % 2):
+                return False
+            shape = (n, sh.Cout, sh.Ho // 2, sh.Wo // 2) if pooled else (n, sh.Cout, sh.Ho, sh.Wo)
+        return True
+
+    # ---- training forward --------------------------------------------------------------------------------------
+    def _train_forward(self, x):
+        convs = [getattr(self, f"conv{i}") for i in range(1, 6)]
+        # one pack per forward, never cached: the optimizers update the weights in place
+        packs = F_.real_weight_grad_pack([c.weight for c in convs])
+        z, z_amax = F_.real_cifar_stem_conv_bn(x, self.conv0.weight, *_bn_train_args(self.bn0))
+        for i, (conv, pack, pooled) in enumerate(zip(convs, packs, _VGG_POOLED)):
+            bn = getattr(self, f"bn{i + 1}")
+            z, z_amax = F_.real_conv_bn_hardtanh(z, z_amax, pack, conv.weight, *_bn_train_args(bn), pool=pooled)
+        torch._foreach_add_([bn.num_batches_tracked for bn in self._bns()], 1)
+        return self.fc(torch.flatten(z, 1))

@@ -480,10 +480,9 @@ _VGG_CHILDREN = ("conv0", "bn0", "conv1", "pooling", "bn1", "conv2", "bn2", "con
 _VGG_POOLED = (True, False, True, False, True)     # a 2x2 max-pool follows conv1, conv3, conv5
 
 
-def _check_vgg(model):
-    """Raise TypeError unless `model` is a VGGSmall whose six convs are bias-free 3x3 / stride-1 / pad-1 nn.Conv2d: the
-    fp32 teacher.  The binary VGG-Small is a student, whose eval forward has its own units."""
-    who = "FrozenVGGTeacher"
+def _check_vgg(model, who="FrozenVGGTeacher"):
+    """Raise TypeError, naming `who`, unless `model` is a VGGSmall whose six convs are bias-free 3x3 / stride-1 / pad-1
+    nn.Conv2d: the fp32 teacher.  The binary VGG-Small is a student, whose eval forward has its own units."""
     if type(model) is not VGGSmall:
         raise TypeError(f"{who} wraps a bdbnn_b200.vgg.VGGSmall with nn.Conv2d convs, got {type(model).__name__}")
     names = [n for n, _ in model.named_children()]
@@ -521,7 +520,7 @@ class FrozenVGGTeacher(_FrozenTeacher):
     structure (binary convs, biased convs, extra children, nn.DataParallel, subclasses, other BatchNorms)."""
 
     def __init__(self, model):
-        _check_vgg(model)
+        _check_vgg(model, type(self).__name__)
         super().__init__(model)
 
     def _geometry_supported(self, x):

@@ -400,6 +400,33 @@ BDBNN_API int bdbnn_real_pool2_bn_eval_hardtanh(const float* y, const float* sca
                                       int32_t H, int32_t W, int32_t C, float* z, uint32_t* z_amax_bits,
                                       void* stream);
 
+/* ---- Hardtanh units of the fp32 VGG-Small trained on the wgmma kernels (DESIGN.md §4u) ------------------------------
+ * real_bn_fwd_hardtanh : BatchNorm(train) + Hardtanh on fp32 y NHWC [n_pix][C] (C % 4 == 0) with the statistics
+ *          ready in sums_ws / ymax_bits (stats_ready must be 1: from the conv epilogue, real_pool2 or the stem):
+ *          bn_finalize (mean, invstd, ab_ws, running statistics), then z = hardtanh(u) for u = fmaf(y, a, b), torch's
+ *          Hardtanh (clamp to [-1, 1], NaN and -0.0 stay), no +-1 packs.  u is the u bn_bwd_pack_hardtanh recomputes
+ *          from y and ab_ws, so its strict mask (-1 < u < 1, 0 at NaN) is this forward's decision.  z_amax_bits (one
+ *          word, zeroed here) = bits of max|z| (integer atomicMax, NaN on top) for the next bdbnn_real_act_pack.
+ * real_pool2 : pool2_i16 on the fp32 output of a real-valued conv: p fp32 NHWC [N,H/2,W/2,C] = 2x2 / stride-2 max of y
+ *          [N,H,W,C] as F.max_pool2d takes it (scan order, `v > m || v is NaN`: the first of equal values, NaN wins),
+ *          idx uint8 = the winner's tap dy*2 + dx (torch's index), the BatchNorm statistics of p into sums double[2C]
+ *          and pmax_bits u32[C] = max|p| per channel (both zeroed here; per-block partials summed in a fixed order) for
+ *          real_bn_fwd_hardtanh(p, n_pix = N*H/2*W/2, stats_ready = 1).  H, W even, C % 32 == 0.
+ * real_pool2_bn_bwd_pack : pool2_bn_bwd_pack of that unit with fp32 p (no alpha), grad_mode FP16S: the BatchNorm +
+ *          Hardtanh backward over the pooled tensor written as gys fp16 [N,H,W,C] at the conv-output resolution, the
+ *          value at the winner and 0 elsewhere; pmax_bits is real_pool2's. */
+BDBNN_API int bdbnn_real_bn_fwd_hardtanh(const float* y, const float* gamma, const float* beta, int64_t n_pix, int32_t C,
+                               float eps, float momentum, float* running_mean, float* running_var, double* sums_ws,
+                               uint32_t* ymax_bits, float* mean, float* invstd, float* ab_ws, float* z,
+                               uint32_t* z_amax_bits, int32_t stats_ready, void* stream);
+BDBNN_API int bdbnn_real_pool2(const float* y, int32_t N, int32_t H, int32_t W, int32_t C, float* p, uint8_t* idx,
+                     double* sums, uint32_t* pmax_bits, void* stream);
+BDBNN_API int bdbnn_real_pool2_bn_bwd_pack(const float* gz, const float* p, const uint8_t* idx, const float* ab,
+                                 const float* mean, const float* invstd, const float* gamma, const float* gscale,
+                                 const uint32_t* pmax_bits, int32_t N, int32_t H, int32_t W, int32_t C,
+                                 double* sums_ws, uint32_t* gmax_bits, float* consts_ws, float* dgamma, float* dbeta,
+                                 uint32_t* amax_bits, uint16_t* gys, void* stream);
+
 /* ---- ReLU units of the fp32 ResNet trained on the wgmma kernels (DESIGN.md §4r) ------------------------------------
  * bn_fwd_relu : bdbnn_bn_fwd on fp32 y (residual may be NULL), then z = relu(u) for u = BatchNorm(y) (+ residual)
  *          (torch.relu bit for bit: NaN and -0.0 stay).  No +-1 packs; instead mask_bits u32 [n_pix][C/32]
