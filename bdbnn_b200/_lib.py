@@ -135,6 +135,11 @@ SIGNATURES = {
     "bdbnn_jpeg_check_batch": (c_int, [_P, c_int, _P, c_int, c_int64, c_int64, c_size_t]),
     "bdbnn_jpeg_decode_batch": (c_int, [_P, _P, c_int, _P, _P, c_int, _P, _P, c_int64, _P, c_size_t, _P, c_int64, _P,
                                         _P, _P, _P]),
+    "bdbnn_jpeg_index_scratch_bytes": (c_size_t, [c_int64]),
+    "bdbnn_debug_jpeg_index_entry": (c_int, [c_int, c_int, c_int, c_int, c_int, _P, _P]),
+    "bdbnn_jpeg_index_file": (c_int, [ctypes.c_char_p, c_int64, c_int, _P, c_size_t, _P, c_int64, _P, _P]),
+    "bdbnn_jpeg_decode_batch_indexed": (c_int, [_P, _P, c_int, _P, _P, c_int, _P, _P, c_int64, _P, _P, c_int64, _P,
+                                                c_size_t, _P, c_int64, _P, _P, _P, _P]),
 }
 
 

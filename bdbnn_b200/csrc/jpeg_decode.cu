@@ -284,14 +284,14 @@ static int jp_parse(const uint8_t* d, int64_t n, bdbnn_jpeg_desc* o, uint8_t* ou
   return BDBNN_OK;
 }
 
-// ---- device: Huffman -----------------------------------------------------------------------------------------------
+// ---- Huffman, on the device and in the host index builder (bdbnn_jpeg_index_file) ----------------------------------
 struct JpBits {
   const uint8_t* p;
   int32_t nbytes;
   uint64_t buf;                                   // left-aligned
   int32_t have, next, pos;
 
-  __device__ void init(const uint8_t* data, int32_t nb, int32_t bitpos) {
+  __host__ __device__ void init(const uint8_t* data, int32_t nb, int32_t bitpos) {
     p = data;
     nbytes = nb;
     next = bitpos >> 3;
@@ -301,30 +301,34 @@ struct JpBits {
     fill();
     skip(bitpos & 7);
   }
-  __device__ __forceinline__ void fill() {
+  __host__ __device__ __forceinline__ void fill() {
     while (have <= 56) {
+#ifdef __CUDA_ARCH__
       const uint32_t b = next < nbytes ? uint32_t(__ldg(p + next)) : 0u;   // zeros past the end
+#else
+      const uint32_t b = next < nbytes ? uint32_t(p[next]) : 0u;
+#endif
       buf |= uint64_t(b) << (56 - have);
       ++next;
       have += 8;
     }
   }
-  __device__ __forceinline__ void skip(int n) {
+  __host__ __device__ __forceinline__ void skip(int n) {
     buf <<= n;
     have -= n;
     pos += n;
   }
 };
 
-__device__ __forceinline__ uint64_t jp_pack(int32_t pos, int b, int k) {
+__host__ __device__ __forceinline__ uint64_t jp_pack(int32_t pos, int b, int k) {
   return (uint64_t(uint32_t(pos)) << 16) | (uint64_t(b) << 8) | uint64_t(k);
 }
 
 // Decode codewords from (pos, b, k) until pos >= stop_pos or stop_blocks blocks are complete.  WRITE stores each
 // value at coef[block * 64 + natural index] (DC differences at index 0).  Returns the status bits of the first fault
-// (decoding stops there); `done` counts the completed blocks.
+// (decoding stops there); `done` counts the completed blocks.  The host (index builder) runs only jp_run<false>.
 template <bool WRITE>
-__device__ int jp_run(const bdbnn_jpeg_desc* __restrict__ d, const uint8_t* seg, int32_t nbits, int32_t& pos,
+__host__ __device__ int jp_run(const bdbnn_jpeg_desc* __restrict__ d, const uint8_t* seg, int32_t nbits, int32_t& pos,
                       int& b, int& k, int32_t stop_pos, int32_t stop_blocks, int32_t& done, int16_t* coef) {
   done = 0;
   if (pos >= stop_pos || stop_blocks <= 0) return 0;
@@ -377,7 +381,13 @@ __device__ int jp_run(const bdbnn_jpeg_desc* __restrict__ d, const uint8_t* seg,
         pos = br.pos;
         return BDBNN_JPEG_K_OVERFLOW;
       }
-      if (WRITE) coef[int64_t(done) * 64 + c_zigzag[k]] = int16_t(v);
+      if constexpr (WRITE) {
+#ifdef __CUDA_ARCH__
+        coef[int64_t(done) * 64 + c_zigzag[k]] = int16_t(v);
+#else
+        coef[int64_t(done) * 64 + kZigzag[k]] = int16_t(v);
+#endif
+      }
       ++k;
     } else if (r == 15) {
       k += 16;
@@ -520,6 +530,58 @@ jpeg_sync_kernel(const bdbnn_jpeg_desc* __restrict__ descs, const bdbnn_jpeg_seg
     atomicExch(ready + tile, 1);
     atomicMax(rounds_max, rounds);
   }
+}
+
+// Index entry of subsequence j >= 1 of a segment (bdbnn_jpeg_index_file): its start state, the exit of subsequence
+// j - 1, as bits 0-4 the overshoot pos - j S past its first bit, bits 5-7 the block in the MCU, bits 8-13 the
+// zig-zag index.  Bits 14-15 are zero.
+constexpr int kJpEntryOvershoot = 31;
+
+__host__ __device__ __forceinline__ bool jp_entry_pack(int32_t pos, int b, int k, int32_t j, int S, uint16_t* e) {
+  const int64_t ov = int64_t(pos) - int64_t(j) * S;
+  if (ov < 0 || ov >= kJpEntryOvershoot || b < 0 || b > 7 || k < 0 || k > 63) return false;
+  *e = uint16_t(ov | (b << 5) | (k << 8));
+  return true;
+}
+
+__host__ __device__ __forceinline__ uint64_t jp_entry_state(uint16_t e, int32_t j, int S) {
+  return jp_pack(j * S + (e & 31), (e >> 5) & 7, (e >> 8) & 63);
+}
+
+// Replaces phases 1-2 when the starts come from an index: thread i takes its start from the entries (the segment's
+// first subsequence starts at (0, 0, 0); segment s's entries begin at sub0 - s), decodes to its exit as phase 1 does
+// and writes start[i] and cnt[i] for phases 3-4.  If the exit is not the segment's next stored start, or a stored
+// start is malformed, the image gets BDBNN_JPEG_INDEX.  No waits: when every exit equals the next stored start, the
+// stored starts are the sequential decode's states by induction from the segment's first, so phases 3-4 see what
+// they see after phase 2.  A malformed start is replaced by the guess (j S, 0, 0) so that the later kernels stay in
+// bounds.  (Four blocks per SM lift ptxas's default register budget, which spilled.)
+__global__ void __launch_bounds__(kJpThreads, 4)
+jpeg_index_check_kernel(const bdbnn_jpeg_desc* __restrict__ descs, const bdbnn_jpeg_seg* __restrict__ segs, int nseg,
+                        const uint8_t* __restrict__ data, int64_t n_sub, int S, const uint16_t* __restrict__ entries,
+                        uint64_t* __restrict__ start, int32_t* __restrict__ cnt, int32_t* __restrict__ status) {
+  const int64_t i = int64_t(blockIdx.x) * kJpThreads + threadIdx.x;
+  if (i >= n_sub) return;
+  int s;
+  const JpSub q = jp_sub(descs, segs, nseg, data, i, S, &s);
+  const bdbnn_jpeg_seg g = segs[s];
+  const int32_t j = int32_t(i - g.sub0);
+  bool bad = false;
+  uint64_t st = 0;
+  if (j > 0) {
+    const uint16_t e = entries[i - s - 1];
+    st = jp_entry_state(e, j, S);
+    if ((e >> 14) != 0 || ((e >> 5) & 7) >= q.d->bpm) {
+      bad = true;
+      st = jp_pack(j * S, 0, 0);
+    }
+  }
+  int32_t pos = int32_t(st >> 16), nb = 0;
+  int b = int((st >> 8) & 255), k = int(st & 255);
+  jp_run<false>(q.d, q.data, q.nbits, pos, b, k, q.end, INT_MAX, nb, nullptr);
+  start[i] = st;
+  cnt[i] = nb;
+  if (j + 1 < g.nsub && jp_pack(pos, b, k) != jp_entry_state(entries[i - s], j + 1, S)) bad = true;
+  if (bad) atomicOr(status + g.img, BDBNN_JPEG_INDEX);
 }
 
 // Phase 3: first[i] = blocks completed by the segment's earlier subsequences (one warp per segment).
@@ -812,6 +874,85 @@ extern "C" int bdbnn_jpeg_parse(const uint8_t* file_host, int64_t file_bytes, bd
   return jp_parse(file_host, file_bytes, desc_host, data_host, data_cap, seg_off_host, seg_cap);
 }
 
+// Scratch of bdbnn_jpeg_index_file: the descriptor, the segment offsets, the unstuffed data.
+static size_t jp_index_scratch(int64_t file_bytes, size_t* seg_at, size_t* data_at) {
+  *seg_at = jp_align(sizeof(bdbnn_jpeg_desc));
+  *data_at = *seg_at + jp_align(size_t(file_bytes / 3 + 2) * 4);
+  return *data_at + size_t(file_bytes);
+}
+
+extern "C" int bdbnn_debug_jpeg_index_entry(int32_t pos, int32_t b, int32_t k, int32_t j, int32_t S, uint16_t* entry,
+                                            int32_t* state) {
+  BDBNN_REQUIRE(entry && state, "debug_jpeg_index_entry: NULL pointer");
+  BDBNN_REQUIRE(j >= 1 && S >= 8 && S <= (1 << 20) && int64_t(j) * S + 31 < INT_MAX,
+                "debug_jpeg_index_entry: j = %d, S = %d outside range", j, S);
+  if (!jp_entry_pack(pos, b, k, j, S, entry)) return BDBNN_ERR_UNSUPPORTED;
+  const uint64_t st = jp_entry_state(*entry, j, S);
+  state[0] = int32_t(st >> 16);
+  state[1] = int32_t((st >> 8) & 255);
+  state[2] = int32_t(st & 255);
+  return BDBNN_OK;
+}
+
+extern "C" size_t bdbnn_jpeg_index_scratch_bytes(int64_t file_bytes) {
+  if (file_bytes < 0 || file_bytes >= (int64_t(1) << 31)) return 0;
+  size_t seg_at, data_at;
+  return jp_index_scratch(file_bytes, &seg_at, &data_at);
+}
+
+// The sequential decode of each segment, cut at the same subsequence ends with the same unlimited block count as
+// phase 1, so each recorded exit is the start phase 2 converges to.  The last subsequence is decoded to the segment's
+// last block, as phase 4 decodes it, so that a stream the device would flag (cut short, corrupt, padded by more than
+// 7 bits) is refused here and goes to the host decoder without a trip through the device.
+extern "C" int bdbnn_jpeg_index_file(const uint8_t* file_host, int64_t file_bytes, int32_t S, void* scratch,
+                                     size_t scratch_cap, uint16_t* entries, int64_t entry_cap, int64_t* n_entries,
+                                     int32_t* n_seg) {
+  BDBNN_REQUIRE(file_host && scratch && entries && n_entries && n_seg, "jpeg_index_file: NULL pointer");
+  BDBNN_REQUIRE(file_bytes >= 0 && file_bytes < (int64_t(1) << 31) && entry_cap >= 0,
+                "jpeg_index_file: file of %lld bytes or entry_cap %lld outside range", (long long)file_bytes,
+                (long long)entry_cap);
+  BDBNN_REQUIRE(S >= 8 && S <= (1 << 20), "jpeg_index_file: S = %d outside [8, 2^20]", S);
+  BDBNN_REQUIRE((reinterpret_cast<uintptr_t>(scratch) & 7) == 0, "jpeg_index_file: scratch not 8-byte aligned");
+  size_t seg_at, data_at;
+  BDBNN_REQUIRE(scratch_cap >= jp_index_scratch(file_bytes, &seg_at, &data_at),
+                "jpeg_index_file: scratch of %zu bytes, need %zu", scratch_cap,
+                jp_index_scratch(file_bytes, &seg_at, &data_at));
+  uint8_t* base = static_cast<uint8_t*>(scratch);
+  bdbnn_jpeg_desc* d = reinterpret_cast<bdbnn_jpeg_desc*>(base);
+  uint32_t* seg_off = reinterpret_cast<uint32_t*>(base + seg_at);
+  uint8_t* data = base + data_at;
+  if (int rc = jp_parse(file_host, file_bytes, d, data, file_bytes, seg_off, int32_t(file_bytes / 3 + 2))) return rc;
+  const int64_t total = int64_t(d->mcux) * d->mcuy, R = d->restart ? d->restart : total;
+  int64_t n = 0;
+  for (int sg = 0; sg < d->nseg; ++sg) {
+    const uint32_t off = seg_off[sg];
+    const int32_t nbytes = int32_t((sg + 1 < d->nseg ? seg_off[sg + 1] : uint32_t(d->data_bytes)) - off);
+    const int32_t nbits = nbytes * 8;
+    const int32_t nsub = std::max(1, int32_t((int64_t(nbits) + S - 1) / S));
+    const int64_t nblk = std::min(R, total - sg * R) * d->bpm;
+    int32_t pos = 0, done = 0;
+    int b = 0, k = 0;
+    int64_t blocks = 0;
+    for (int32_t j = 1; j < nsub; ++j) {
+      if (int f = jp_run<false>(d, data + off, nbits, pos, b, k, j * S, INT_MAX, done, nullptr))
+        JP_REJECT("jpeg_index_file: segment %d: status %d before bit %lld", sg, f, (long long)j * S);
+      blocks += done;
+      BDBNN_REQUIRE(n < entry_cap, "jpeg_index_file: more than entry_cap = %lld entries", (long long)entry_cap);
+      if (!jp_entry_pack(pos, b, k, j, S, entries + n))
+        JP_REJECT("jpeg_index_file: segment %d: state (%d, %d, %d) at subsequence %d has no entry", sg, pos, b, k, j);
+      ++n;
+    }
+    if (blocks > nblk) JP_REJECT("jpeg_index_file: segment %d: data past its last block", sg);
+    const int f = jp_run<false>(d, data + off, nbits, pos, b, k, INT_MAX, int32_t(nblk - blocks), done, nullptr);
+    if (f || blocks + done != nblk || nbits - pos > 7)
+      JP_REJECT("jpeg_index_file: segment %d: status %d, %lld of %lld blocks, %d bits left", sg, f,
+                (long long)(blocks + done), (long long)nblk, nbits - pos);
+  }
+  *n_entries = n;
+  *n_seg = d->nseg;
+  return BDBNN_OK;
+}
+
 extern "C" int bdbnn_jpeg_subseq_bits(void) { return jp_sub_bits(); }
 
 extern "C" int bdbnn_debug_jpeg_subseq_bits(int32_t bits) {
@@ -902,18 +1043,20 @@ extern "C" int bdbnn_jpeg_check_batch(const bdbnn_jpeg_desc* desc_host, int32_t 
   return jp_check(desc_host, n_img, seg_host, n_seg, data_bytes, rgb_bytes, work_bytes, &blocks, &pix, &n_sub);
 }
 
-extern "C" int bdbnn_jpeg_decode_batch(const bdbnn_jpeg_desc* desc_host, bdbnn_jpeg_desc* desc_dev, int32_t n_img,
-                                       const bdbnn_jpeg_seg* seg_host, bdbnn_jpeg_seg* seg_dev, int32_t n_seg,
-                                       const uint8_t* data_host, uint8_t* data_dev, int64_t data_bytes, void* work,
-                                       size_t work_bytes, uint8_t* rgb, int64_t rgb_bytes, int32_t* status_dev,
-                                       int32_t* status_host, int32_t* rounds_host, void* stream) {
-  BDBNN_REQUIRE(desc_host && desc_dev && seg_host && seg_dev && data_host && data_dev && work && rgb && status_dev &&
-                    status_host,
-                "jpeg_decode_batch: NULL pointer");
+// bdbnn_jpeg_decode_batch, or with entries_dev set bdbnn_jpeg_decode_batch_indexed: jpeg_index_check_kernel
+// in place of jpeg_sync_kernel, the rest as it is.
+static int jp_decode(const bdbnn_jpeg_desc* desc_host, bdbnn_jpeg_desc* desc_dev, int32_t n_img,
+                     const bdbnn_jpeg_seg* seg_host, bdbnn_jpeg_seg* seg_dev, int32_t n_seg, const uint8_t* data_host,
+                     uint8_t* data_dev, int64_t data_bytes, const uint16_t* entries_host, uint16_t* entries_dev,
+                     int64_t n_entries, void* work, size_t work_bytes, uint8_t* rgb, int64_t rgb_bytes,
+                     int32_t* status_dev, int32_t* status_host, int32_t* rounds_host, void* stream) {
   int64_t blocks, pix, n_sub;
   if (int rc = jp_check(desc_host, n_img, seg_host, n_seg, data_bytes, rgb_bytes, work_bytes, &blocks, &pix, &n_sub))
     return rc;
   const int S = jp_sub_bits();
+  BDBNN_REQUIRE(!entries_dev || n_entries == n_sub - n_seg,
+                "jpeg_decode_batch_indexed: %lld entries, the segments' nsub - 1 sum to %lld", (long long)n_entries,
+                (long long)(n_sub - n_seg));
   BDBNN_REQUIRE((reinterpret_cast<uintptr_t>(work) & 255) == 0, "jpeg_decode_batch: workspace not 256-byte aligned");
 
   const cudaStream_t st = cudaStream_t(stream);
@@ -926,11 +1069,20 @@ extern "C" int bdbnn_jpeg_decode_batch(const bdbnn_jpeg_desc* desc_host, bdbnn_j
   BDBNN_CUDA(cudaMemsetAsync(status_dev, 0, size_t(n_img) * 4, st));
 
   const unsigned sub_grid = unsigned((n_sub + kJpThreads - 1) / kJpThreads);
-  BDBNN_CUDA(cudaMemsetAsync(w.ready, 0, size_t(sub_grid) * 4, st));
-  BDBNN_CUDA(cudaMemsetAsync(w.counters, 0, 8, st));
-  jpeg_sync_kernel<<<sub_grid, kJpThreads, 0, st>>>(desc_dev, seg_dev, n_seg, data_dev, n_sub, S, w.start, w.exit,
-                                                     w.cnt, w.counters, w.ready, w.counters + 1);
-  if (int rc = check_launch("jpeg_sync_kernel")) return rc;
+  if (entries_dev) {
+    BDBNN_CUDA(cudaMemsetAsync(w.counters, 0, 8, st));         // rounds_host receives 0
+    if (n_entries > 0)
+      BDBNN_CUDA(cudaMemcpyAsync(entries_dev, entries_host, size_t(n_entries) * 2, cudaMemcpyHostToDevice, st));
+    jpeg_index_check_kernel<<<sub_grid, kJpThreads, 0, st>>>(desc_dev, seg_dev, n_seg, data_dev, n_sub, S,
+                                                              entries_dev, w.start, w.cnt, status_dev);
+    if (int rc = check_launch("jpeg_index_check_kernel")) return rc;
+  } else {
+    BDBNN_CUDA(cudaMemsetAsync(w.ready, 0, size_t(sub_grid) * 4, st));
+    BDBNN_CUDA(cudaMemsetAsync(w.counters, 0, 8, st));
+    jpeg_sync_kernel<<<sub_grid, kJpThreads, 0, st>>>(desc_dev, seg_dev, n_seg, data_dev, n_sub, S, w.start, w.exit,
+                                                       w.cnt, w.counters, w.ready, w.counters + 1);
+    if (int rc = check_launch("jpeg_sync_kernel")) return rc;
+  }
   jpeg_scan_kernel<<<unsigned((int64_t(n_seg) * 32 + 255) / 256), 256, 0, st>>>(seg_dev, n_seg, w.cnt, w.first);
   if (int rc = check_launch("jpeg_scan_kernel")) return rc;
   jpeg_write_kernel<<<sub_grid, kJpThreads, 0, st>>>(desc_dev, seg_dev, n_seg, data_dev, n_sub, S, w.start, w.first,
@@ -947,4 +1099,32 @@ extern "C" int bdbnn_jpeg_decode_batch(const bdbnn_jpeg_desc* desc_host, bdbnn_j
   BDBNN_CUDA(cudaMemcpyAsync(status_host, status_dev, size_t(n_img) * 4, cudaMemcpyDeviceToHost, st));
   if (rounds_host) BDBNN_CUDA(cudaMemcpyAsync(rounds_host, w.counters + 1, 4, cudaMemcpyDeviceToHost, st));
   return BDBNN_OK;
+}
+
+extern "C" int bdbnn_jpeg_decode_batch(const bdbnn_jpeg_desc* desc_host, bdbnn_jpeg_desc* desc_dev, int32_t n_img,
+                                       const bdbnn_jpeg_seg* seg_host, bdbnn_jpeg_seg* seg_dev, int32_t n_seg,
+                                       const uint8_t* data_host, uint8_t* data_dev, int64_t data_bytes, void* work,
+                                       size_t work_bytes, uint8_t* rgb, int64_t rgb_bytes, int32_t* status_dev,
+                                       int32_t* status_host, int32_t* rounds_host, void* stream) {
+  BDBNN_REQUIRE(desc_host && desc_dev && seg_host && seg_dev && data_host && data_dev && work && rgb && status_dev &&
+                    status_host,
+                "jpeg_decode_batch: NULL pointer");
+  return jp_decode(desc_host, desc_dev, n_img, seg_host, seg_dev, n_seg, data_host, data_dev, data_bytes, nullptr,
+                   nullptr, 0, work, work_bytes, rgb, rgb_bytes, status_dev, status_host, rounds_host, stream);
+}
+
+extern "C" int bdbnn_jpeg_decode_batch_indexed(const bdbnn_jpeg_desc* desc_host, bdbnn_jpeg_desc* desc_dev,
+                                               int32_t n_img, const bdbnn_jpeg_seg* seg_host, bdbnn_jpeg_seg* seg_dev,
+                                               int32_t n_seg, const uint8_t* data_host, uint8_t* data_dev,
+                                               int64_t data_bytes, const uint16_t* entries_host,
+                                               uint16_t* entries_dev, int64_t n_entries, void* work,
+                                               size_t work_bytes, uint8_t* rgb, int64_t rgb_bytes,
+                                               int32_t* status_dev, int32_t* status_host, int32_t* rounds_host,
+                                               void* stream) {
+  BDBNN_REQUIRE(desc_host && desc_dev && seg_host && seg_dev && data_host && data_dev && entries_host &&
+                    entries_dev && work && rgb && status_dev && status_host,
+                "jpeg_decode_batch_indexed: NULL pointer");
+  return jp_decode(desc_host, desc_dev, n_img, seg_host, seg_dev, n_seg, data_host, data_dev, data_bytes,
+                   entries_host, entries_dev, n_entries, work, work_bytes, rgb, rgb_bytes, status_dev, status_host,
+                   rounds_host, stream);
 }

@@ -385,6 +385,7 @@ assert _JDESC.itemsize == 6152
 _JSEG = np.dtype([("off", "<i8"), ("img", "<i4"), ("nbytes", "<i4"), ("mcu0", "<i4"), ("nmcu", "<i4"),
                   ("sub0", "<i4"), ("nsub", "<i4")])
 assert _JSEG.itemsize == 32
+BDBNN_JPEG_INDEX = 64                            # status bit of bdbnn_jpeg_decode_batch_indexed
 
 
 def jpeg_parse(data):
@@ -437,11 +438,12 @@ def jpeg_batch_layout(descs):
     return int(blocks.sum()), int(pix.sum())
 
 
-def jpeg_decode_batch(descs, segs, staging, device, stream):
+def jpeg_decode_batch(descs, segs, staging, device, stream, entries=None):
     """bdbnn_jpeg_decode_batch on `stream`: descs (_JDESC, every offset set), segs (_JSEG), staging the uint8 host
     tensor (pinned) holding the images' unstuffed data.  Returns (rgb uint8 device tensor, pinned int32 status per
     image, pinned int32 [1] synchronisation rounds, workspace tensor); all are ready, and staging may be rewritten,
-    once `stream` has run the queued work."""
+    once `stream` has run the queued work.  entries (uint16, each segment's nsub - 1 index entries, segments in order;
+    bdbnn_b200.jpeg_index): bdbnn_jpeg_decode_batch_indexed instead, which reports 0 rounds."""
     lib = _lib.lib()
     n_blocks, n_pix = int((descs["mcux"].astype(np.int64) * descs["mcuy"] * descs["bpm"]).sum()), \
         int((descs["H"].astype(np.int64) * descs["W"]).sum())
@@ -454,14 +456,27 @@ def jpeg_decode_batch(descs, segs, staging, device, stream):
         work = torch.empty(lib.bdbnn_jpeg_workspace_bytes(n_blocks, n_sub), dtype=torch.uint8, device=device)
         rgb = torch.empty(3 * n_pix, dtype=torch.uint8, device=device)
         status_dev = torch.empty(len(descs), dtype=torch.int32, device=device)
-        status = torch.empty(len(descs) + 1, dtype=torch.int32, pin_memory=True)
-        _lib.check(lib.bdbnn_jpeg_decode_batch(
-            descs.ctypes.data, desc_dev.data_ptr(), len(descs), segs.ctypes.data, seg_dev.data_ptr(), len(segs),
-            staging.data_ptr(), data_dev.data_ptr(), data_bytes, work.data_ptr(), work.numel(), rgb.data_ptr(),
-            rgb.numel(), status_dev.data_ptr(), status.data_ptr(), status.data_ptr() + 4 * len(descs),
-            ctypes.c_void_p(stream.cuda_stream)), "jpeg_decode_batch")
+        if entries is None:
+            status = torch.empty(len(descs) + 1, dtype=torch.int32, pin_memory=True)
+            _lib.check(lib.bdbnn_jpeg_decode_batch(
+                descs.ctypes.data, desc_dev.data_ptr(), len(descs), segs.ctypes.data, seg_dev.data_ptr(), len(segs),
+                staging.data_ptr(), data_dev.data_ptr(), data_bytes, work.data_ptr(), work.numel(), rgb.data_ptr(),
+                rgb.numel(), status_dev.data_ptr(), status.data_ptr(), status.data_ptr() + 4 * len(descs),
+                ctypes.c_void_p(stream.cuda_stream)), "jpeg_decode_batch")
+        else:
+            # the entries' pinned copy lives in the status buffer's tail, so it stays alive while status is held
+            n_ent = len(entries)
+            status = torch.empty(len(descs) + 1 + (n_ent + 1) // 2, dtype=torch.int32, pin_memory=True)
+            ent_host = status[len(descs) + 1:].view(torch.int16)[:n_ent]
+            ent_host.numpy()[:] = np.asarray(entries, np.uint16).view(np.int16)
+            ent_dev = torch.empty(max(n_ent, 1), dtype=torch.int16, device=device)
+            _lib.check(lib.bdbnn_jpeg_decode_batch_indexed(
+                descs.ctypes.data, desc_dev.data_ptr(), len(descs), segs.ctypes.data, seg_dev.data_ptr(), len(segs),
+                staging.data_ptr(), data_dev.data_ptr(), data_bytes, ent_host.data_ptr(), ent_dev.data_ptr(), n_ent,
+                work.data_ptr(), work.numel(), rgb.data_ptr(), rgb.numel(), status_dev.data_ptr(), status.data_ptr(),
+                status.data_ptr() + 4 * len(descs), ctypes.c_void_p(stream.cuda_stream)), "jpeg_decode_batch_indexed")
     _lib.count(6)
-    return rgb, status[:len(descs)], status[len(descs):], work
+    return rgb, status[:len(descs)], status[len(descs):len(descs) + 1], work
 
 
 def _pil_decode(data):
@@ -567,7 +582,13 @@ class ImageNetDeviceLoader:
     decode, IDCT, upsampling and colour conversion of the batch run on the loader's stream, with libjpeg-turbo's
     integer arithmetic, so the batches are bit-identical to decode='cpu' (and to the PIL chain).  Files the device
     decoder does not take (progressive, CMYK, PNG, other sampling, ...; include/bdbnn.h) or flags while decoding
-    (corrupt data) are decoded as in decode='cpu', one at a time; decode_stats counts them.
+    (corrupt data) are decoded as in decode='cpu', one at a time; decode_stats counts them.  jpeg_index (only with
+    decode='kernel'; a path or a bdbnn_b200.jpeg_index.JpegIndex, built by `python -m bdbnn_b200.jpeg_index ROOT OUT`
+    at the library's subsequence length) supplies the Huffman synchronisation points, so the device checks them in one
+    pass instead of finding them: every indexed file of a batch goes through one bdbnn_jpeg_decode_batch_indexed call,
+    with the same pixels.  A file with no record for its path, or whose size, segment count or entry count differs from
+    its record, is unindexed and decoded on the host, as is a file whose stored points the device finds inconsistent
+    with its bytes (BDBNN_JPEG_INDEX); decode_stats counts them as "unindexed" and "index_flagged".
 
     The training split is shuffled by the epoch permutation of §4l and sharded as CifarDeviceLoader (shard_spans);
     the validation split is read in order, as the reference's (shuffle=train_flag).  Crop and flip are pure functions
@@ -576,9 +597,11 @@ class ImageNetDeviceLoader:
     orders its launch after that decode with an event, without a host synchronisation on the device's work."""
 
     def __init__(self, root, batch_size, train, seed=None, drop_last=False, rank=0, world_size=1, device=None, *,
-                 decode="cpu", workers=16, mean=IMAGENET_MEAN, std=IMAGENET_STD):
+                 decode="cpu", workers=16, mean=IMAGENET_MEAN, std=IMAGENET_STD, jpeg_index=None):
         if decode not in ("cuda", "cpu", "kernel"):
             raise ValueError(f"ImageNetDeviceLoader: decode must be 'cpu', 'cuda' or 'kernel', got {decode!r}")
+        if jpeg_index is not None and decode != "kernel":
+            raise ValueError(f"ImageNetDeviceLoader: jpeg_index needs decode='kernel', got decode={decode!r}")
         if int(batch_size) < 1 or int(world_size) < 1 or not 0 <= int(rank) < int(world_size) or int(workers) < 1:
             raise ValueError(f"ImageNetDeviceLoader: need batch_size >= 1, workers >= 1 and 0 <= rank < world_size, "
                              f"got {batch_size}, {workers}, {rank}, {world_size}")
@@ -609,6 +632,14 @@ class ImageNetDeviceLoader:
         # decode='kernel': files decoded on the device, parse rejections, device flags, most synchronisation rounds
         # of a block
         self.decode_stats = {"device": 0, "rejected": 0, "flagged": 0, "rounds": 0}
+        self._jindex = None                      # (JpegIndex, record of each sample or -1) with jpeg_index
+        if jpeg_index is not None:
+            from . import jpeg_index as JI
+            index = jpeg_index if isinstance(jpeg_index, JI.JpegIndex) else JI.JpegIndex(jpeg_index)
+            hashes = [JI.path_hash(r) for r in JI.relative_paths(root, self.samples)]
+            self._jindex = (index, index.find(hashes))
+            # files parsed but without a matching record, files whose stored points the device rejected
+            self.decode_stats.update(unindexed=0, index_flagged=0)
         self._turn = 0
         self._lock = threading.Lock()
         self._next_epoch = 0
@@ -705,10 +736,29 @@ class ImageNetDeviceLoader:
         st[1].record(self._stream)
         return [(buf[int(offs[i]):int(offs[i + 1])].view(t.shape), hwc) for i, (t, hwc) in enumerate(dec)]
 
-    def _decode_kernel(self, blobs):
+    def _indexed(self, idx, blobs, descs, acc, seg_off, seg_base):
+        """(the accepted files whose index record matches, their concatenated entries)."""
+        index, rec_of = self._jindex
+        if not acc:
+            return [], np.zeros(0, np.uint16)
+        a = descs[acc]
+        segs = jpeg_segment_table(a, [seg_off[seg_base[k]:seg_base[k] + descs["nseg"][k]] for k in acc],
+                                  index.S)
+        want = np.bincount(segs["img"], weights=segs["nsub"] - 1, minlength=len(acc)).astype(np.int64)
+        keep, ent = [], []
+        for j, k in enumerate(acc):
+            r = int(rec_of[int(idx[k])])
+            if r >= 0 and int(index.records["size"][r]) == len(blobs[k]) and \
+                    int(index.records["nseg"][r]) == int(a["nseg"][j]) and int(index.records["n_entries"][r]) == want[j]:
+                keep.append(k)
+                ent.append(index.file_entries(r))
+        return keep, (np.concatenate(ent) if ent else np.zeros(0, np.uint16))
+
+    def _decode_kernel(self, blobs, idx=None):
         """[(device tensor, hwc)] of the batch's files: header parse and unstuffing in the pool, one
-        bdbnn_jpeg_decode_batch on self._stream, then a wait for its status words (this runs in the read-ahead
-        thread) and _host_decode for the files the parse rejected or the device flagged."""
+        bdbnn_jpeg_decode_batch on self._stream (bdbnn_jpeg_decode_batch_indexed for the indexed files with
+        jpeg_index), then a wait for its status words (this runs in the read-ahead thread) and _host_decode for the
+        files the parse rejected, the index lacks or the device flagged."""
         lib = _lib.lib()
         B = len(blobs)
         size = np.array([len(b) for b in blobs], np.int64)
@@ -731,6 +781,10 @@ class ImageNetDeviceLoader:
             if rc[k] not in (0, -3):             # -3: BDBNN_ERR_UNSUPPORTED, the host decodes the file
                 _lib.check(rc[k], "jpeg_parse")
         acc = [k for k in range(B) if rc[k] == 0]
+        parsed, entries = len(acc), None
+        if self._jindex is not None:
+            acc, entries = self._indexed(idx, blobs, descs, acc, seg_off, seg_base)
+            self.decode_stats["unindexed"] += parsed - len(acc)
         out = [None] * B
         if acc:
             a = descs[acc]
@@ -738,7 +792,8 @@ class ImageNetDeviceLoader:
             jpeg_batch_layout(a)
             segs = jpeg_segment_table(a, [seg_off[seg_base[k]:seg_base[k] + descs["nseg"][k]] for k in acc],
                                       lib.bdbnn_jpeg_subseq_bits())
-            rgb, status, rounds, _ = jpeg_decode_batch(a, segs, stage[:int(data_off[-1])], self.device, self._stream)
+            rgb, status, rounds, _ = jpeg_decode_batch(a, segs, stage[:int(data_off[-1])], self.device, self._stream,
+                                                       entries)
             done = torch.cuda.Event()
             done.record(self._stream)
             done.synchronize()
@@ -750,7 +805,9 @@ class ImageNetDeviceLoader:
             self.decode_stats["flagged"] += int((st != 0).sum())
             self.decode_stats["device"] += int((st == 0).sum())
             self.decode_stats["rounds"] = max(self.decode_stats["rounds"], int(rounds[0]))
-        self.decode_stats["rejected"] += B - len(acc)
+            if entries is not None:
+                self.decode_stats["index_flagged"] += int((st & BDBNN_JPEG_INDEX != 0).sum())
+        self.decode_stats["rejected"] += B - parsed
         rest = [k for k in range(B) if out[k] is None]
         for k, (t, hwc) in zip(rest, self._pool.map(self._host_decode, [blobs[k] for k in rest])):
             out[k] = (t.pin_memory().to(self.device, non_blocking=True), hwc)
@@ -761,8 +818,10 @@ class ImageNetDeviceLoader:
         idx = self.indices(epoch, batch_index)
         blobs = list(self._pool.map(_read, [self.samples[int(k)][0] for k in idx]))
         with self._lock, torch.cuda.device(self.device), torch.cuda.stream(self._stream):
-            srcs = {"cuda": self._decode_cuda, "cpu": self._decode_cpu, "kernel": self._decode_kernel}[self.decode](
-                blobs)
+            if self.decode == "kernel":
+                srcs = self._decode_kernel(blobs, idx)
+            else:
+                srcs = {"cuda": self._decode_cuda, "cpu": self._decode_cpu}[self.decode](blobs)
             ev = torch.cuda.Event()
             ev.record(self._stream)
         return idx, srcs, ev

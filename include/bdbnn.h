@@ -867,6 +867,8 @@ typedef struct bdbnn_jpeg_seg {
 #define BDBNN_JPEG_IDCT_RANGE 32  /* IDCT inputs or intermediates outside the range where libjpeg-turbo's SIMD and
                                      C paths agree (dequantised or pass-1 values outside int16, pass-2 outside
                                      [-512, 511]) */
+#define BDBNN_JPEG_INDEX 64       /* bdbnn_jpeg_decode_batch_indexed: a subsequence's exit differs from the segment's
+                                     next stored start, or a stored start is malformed */
 /* Subsequence length S in bits (1024, or the bdbnn_debug_jpeg_subseq_bits override). */
 BDBNN_API int bdbnn_jpeg_subseq_bits(void);
 /* Tests only: sets S to bits in [8, 2^20], 0 restores the default.  Process-wide. */
@@ -893,6 +895,44 @@ BDBNN_API int bdbnn_jpeg_decode_batch(const bdbnn_jpeg_desc* desc_host, bdbnn_jp
                                       const uint8_t* data_host, uint8_t* data_dev, int64_t data_bytes, void* work,
                                       size_t work_bytes, uint8_t* rgb, int64_t rgb_bytes, int32_t* status_dev,
                                       int32_t* status_host, int32_t* rounds_host, void* stream);
+
+/* ---- Index of the synchronisation points (DESIGN.md §4m) ------------------------------------------------------------
+ * The state of the sequential decode at every subsequence boundary of a file, computed once on the host so that the
+ * device needs no synchronisation pass.  One uint16 entry per subsequence j >= 1 of each segment, segments in order
+ * (the first subsequence of a segment starts at bit 0, block 0, DC, and is not stored): the state (pos, b, k) where
+ * the sequential decode crosses bit j S, i.e. its first codeword boundary at or past j S, as bits 0-4 pos - j S,
+ * bits 5-7 the block in the MCU b, bits 8-13 the zig-zag index k; bits 14-15 zero.
+ *
+ * bdbnn_jpeg_index_file (host only, thread-safe, allocates nothing): the entries of file_host at subsequences of
+ * S bits, S in [8, 2^20].  scratch: 8-byte aligned, scratch_cap >= bdbnn_jpeg_index_scratch_bytes(file_bytes);
+ * entry_cap >= 8 file_bytes / S suffices.  On success *n_entries entries and *n_seg = desc->nseg of
+ * bdbnn_jpeg_parse.  Returns 0; BDBNN_ERR_UNSUPPORTED for a file bdbnn_jpeg_parse does not take, a segment whose
+ * sequential decode raises a BDBNN_JPEG_* status bit (a fault, fewer blocks than its MCUs hold, or more than 7 bits
+ * after them), or a state that does not fit an entry; BDBNN_ERR_INVALID_ARG for NULL pointers, sizes out of range
+ * or too small a scratch or entry_cap. */
+BDBNN_API size_t bdbnn_jpeg_index_scratch_bytes(int64_t file_bytes);
+/* Tests only: packs state (pos, b, k) as the entry of subsequence j at S bits into *entry and unpacks it into
+ * state[0..2]; BDBNN_ERR_UNSUPPORTED if the state has no entry. */
+BDBNN_API int bdbnn_debug_jpeg_index_entry(int32_t pos, int32_t b, int32_t k, int32_t j, int32_t S, uint16_t* entry,
+                                           int32_t* state);
+BDBNN_API int bdbnn_jpeg_index_file(const uint8_t* file_host, int64_t file_bytes, int32_t S, void* scratch,
+                                    size_t scratch_cap, uint16_t* entries, int64_t entry_cap, int64_t* n_entries,
+                                    int32_t* n_seg);
+/* bdbnn_jpeg_decode_batch with the starts taken from an index instead of the synchronisation pass.  entries_host
+ * (n_entries uint16, pinned for an asynchronous copy) holds, segment by segment in the order of seg_host, each
+ * segment's nsub - 1 entries at the current S (segment s's begin at entry sub0 - s); they are copied to entries_dev
+ * on `stream`.  Returns BDBNN_ERR_INVALID_ARG before any launch if n_entries is not the sum of nsub - 1.  One pass,
+ * one thread per subsequence, decodes from each stored start and compares the exit with the next stored start: an
+ * image with a mismatch or a malformed entry gets BDBNN_JPEG_INDEX (and its pixels are not to be used, as with any
+ * status bit).  When no image is flagged, the coefficients and pixels are those of bdbnn_jpeg_decode_batch.
+ * rounds_host (may be NULL) receives 0. */
+BDBNN_API int bdbnn_jpeg_decode_batch_indexed(const bdbnn_jpeg_desc* desc_host, bdbnn_jpeg_desc* desc_dev,
+                                              int32_t n_img, const bdbnn_jpeg_seg* seg_host, bdbnn_jpeg_seg* seg_dev,
+                                              int32_t n_seg, const uint8_t* data_host, uint8_t* data_dev,
+                                              int64_t data_bytes, const uint16_t* entries_host, uint16_t* entries_dev,
+                                              int64_t n_entries, void* work, size_t work_bytes, uint8_t* rgb,
+                                              int64_t rgb_bytes, int32_t* status_dev, int32_t* status_host,
+                                              int32_t* rounds_host, void* stream);
 
 #ifdef __cplusplus
 }

@@ -1,5 +1,5 @@
 """Throughput of the graphed ImageNet ResNet-18 CE step (batch 256, bench.py's workload) when it is fed real JPEG
-batches from disk, five ways:
+batches from disk, six ways:
 
     a  the reference pipeline (loader.py:52-85, train.py:488-491): torchvision ImageFolder with RandomResizedCrop(224),
        RandomHorizontalFlip, ToTensor, Normalize on PIL images in a 16-worker DataLoader with pin_memory, .cuda()
@@ -8,19 +8,23 @@ batches from disk, five ways:
     d  one batch resident in device memory, never rewritten
     e  ImageNetDeviceLoader(decode='kernel', workers=16).fill (header parse in 16 host threads, Huffman decode, IDCT,
        upsampling and colour conversion on the device, csrc/jpeg_decode.cu)
+    f  e with jpeg_index: the Huffman synchronisation points read from an index built once before the rounds
+       (bdbnn_b200/jpeg_index.py; its wall time and size are reported), checked on the device in one pass
 
-    python tools/imagenet_input_throughput.py [--rounds 3] [--steps 70] [--warmup 20] [--images 23040]
+    python tools/imagenet_input_throughput.py [--rounds 3] [--steps 70] [--warmup 20] [--images 23040] [--arms abcdef]
+                                              [--skip-extras]
 
 The data is a synthetic ImageFolder written to a temporary directory (removed at the end): --images JPEGs (quality 90,
 textured so that a 500 x 375 file is about 100 KB) in 100 classes, sized like ImageNet's 500 x 375 / 375 x 500 /
 500 x 333 with one image in 200 of 2 000-4 000 px.  Every file is read once before timing, so the timed passes read
 from the page cache (warm files).  Every arm runs in a process of its own, started afresh every round, the arms
-alternated (a, b, c, d, e per round); each process captures the step, runs --warmup steps and times --steps steps with
+alternated (a, b, c, d, e, f per round, or the --arms given); each process captures the step, runs --warmup steps and times --steps steps with
 a host clock between two device synchronisations, and the step's own device time with CUDA events around each replay.  Then, once: each loader alone (img/s, no step; for e the share of
-files sent to the host decoder and the synchronisation launches), the batch kernel alone (CUDA events around 200
-launches on one decoded batch of 256), the device JPEG decode of one batch of 256 by kernel (torch.profiler, CUDA
-activities) and one evaluation pass (Resize(256) + CenterCrop(224) through ImageNetDeviceLoader with decode="cpu" and
-decode="kernel" into the eval-mode forward).  The card name, power limit and maximum SM
+files sent to the host decoder and the synchronisation launches, likewise for f), the batch kernel alone (CUDA events
+around 200 launches on one decoded batch of 256), the device JPEG decode of one batch of 256 by kernel without and
+with the index (torch.profiler, CUDA activities) and one evaluation pass (Resize(256) + CenterCrop(224) through
+ImageNetDeviceLoader with decode="cpu", decode="kernel" and decode="kernel" with the index into the eval-mode
+forward).  The card name, power limit and maximum SM
 clock are read (read-only) from nvidia-smi.  Needs a CUDA device."""
 import argparse
 import json
@@ -72,6 +76,10 @@ def _warm(root):
                 fh.read()
 
 
+def _index_path(args):
+    return os.path.join(args.root, "train.jpeg_index")
+
+
 def _step(torch):
     from bdbnn_b200.resnet import resnet18
     from bdbnn_b200.step import GraphedTrainStep, StepConfig, TrainStep, make_optimizer
@@ -103,7 +111,8 @@ def _feeder(torch, args):
                     y.cuda(non_blocking=True))
         return nxt
     loader = ImageNetDeviceLoader(os.path.join(args.root, "train"), BATCH, True, seed=0, drop_last=True,
-                                  decode={"b": "cuda", "c": "cpu", "e": "kernel"}[args.arm], workers=16)
+                                  decode={"b": "cuda", "c": "cpu", "e": "kernel", "f": "kernel"}[args.arm], workers=16,
+                                  jpeg_index=_index_path(args) if args.arm == "f" else None)
     state = {"epoch": 0, "i": 0}
 
     def nxt(gstep):
@@ -162,7 +171,7 @@ def arm(torch, args):
 def loaders_alone(torch, args):
     """img/s of each loader with nothing else on the device: 5 warm-up batches, then 30 timed."""
     res = {}
-    for which in "abce":
+    for which in "abcef":
         args.arm = which
         nxt = _feeder(torch, args)
         for _ in range(5):
@@ -173,27 +182,34 @@ def loaders_alone(torch, args):
             nxt(None)
         torch.cuda.synchronize()
         res[which] = round(30 * BATCH / (time.perf_counter() - t0), 1)
-        if which == "e":
+        if which in "ef":
             st = dict(nxt.loader.decode_stats)
-            files = st["device"] + st["rejected"] + st["flagged"]
-            st["host_share"] = round((st["rejected"] + st["flagged"]) / files, 4)
-            print(json.dumps({"kernel_decode_stats": st}), flush=True)
+            files = st["device"] + st["rejected"] + st["flagged"] + st.get("unindexed", 0)
+            st["host_share"] = round((files - st["device"]) / files, 4)
+            print(json.dumps({"kernel_decode_stats" if which == "e" else "indexed_decode_stats": st}), flush=True)
     print(json.dumps({"loader_alone_img_per_s": res}), flush=True)
 
 
-def decode_phases(torch, args):
-    """The device JPEG decode of one training batch of 256 (bdbnn_jpeg_decode_batch) by kernel: torch.profiler with
-    CUDA activities over 5 decodes after 2 warm-up decodes; plus the host's wall time per decode call (parse excluded)
-    and the whole _decode_kernel (parse, decode, wait) per batch."""
+def decode_phases(torch, args, indexed=False):
+    """The device JPEG decode of one training batch of 256 (bdbnn_jpeg_decode_batch, or with indexed=True
+    bdbnn_jpeg_decode_batch_indexed) by kernel: torch.profiler with CUDA activities over 5 decodes after 2 warm-up
+    decodes; plus the host's wall time per decode call (parse excluded) and the whole _decode_kernel (parse, decode,
+    wait) per batch."""
     import numpy as np
     from torch.profiler import ProfilerActivity, profile
     from bdbnn_b200 import _lib
     from bdbnn_b200 import data as D
+    from bdbnn_b200 import jpeg_index as JI
     loader = D.ImageNetDeviceLoader(os.path.join(args.root, "train"), BATCH, True, seed=0, drop_last=True,
-                                    decode="kernel", workers=16)
+                                    decode="kernel", workers=16, jpeg_index=_index_path(args) if indexed else None)
     idx = loader.indices(0, 0)
     blobs = [D._read(loader.samples[int(k)][0]) for k in idx]
     parsed = [D.jpeg_parse(b) for b in blobs]
+    ent = None
+    if indexed:
+        got = [JI.index_file(b) for b in blobs]
+        parsed = [p if g is not None else None for p, g in zip(parsed, got)]
+        ent = np.concatenate([g[0] for p, g in zip(parsed, got) if p is not None])
     acc = [p for p in parsed if p is not None]
     descs = np.concatenate([p[0][None] for p in acc])
     descs["data_off"] = np.concatenate([[0], np.cumsum([len(p[1]) for p in acc])[:-1]])
@@ -202,17 +218,17 @@ def decode_phases(torch, args):
     segs = D.jpeg_segment_table(descs, [np.array(p[2]) for p in acc], _lib.lib().bdbnn_jpeg_subseq_bits())
     dev, st = torch.device("cuda", torch.cuda.current_device()), torch.cuda.current_stream()
     for _ in range(2):
-        D.jpeg_decode_batch(descs, segs, staging, dev, st)
+        D.jpeg_decode_batch(descs, segs, staging, dev, st, ent)
     torch.cuda.synchronize()
     t0 = time.perf_counter()
     for _ in range(5):
-        _, status, rounds, _ = D.jpeg_decode_batch(descs, segs, staging, dev, st)
+        _, status, rounds, _ = D.jpeg_decode_batch(descs, segs, staging, dev, st, ent)
         torch.cuda.synchronize()
         rounds = int(rounds[0])
     call_ms = (time.perf_counter() - t0) * 1e3 / 5
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         for _ in range(5):
-            D.jpeg_decode_batch(descs, segs, staging, dev, st)
+            D.jpeg_decode_batch(descs, segs, staging, dev, st, ent)
         torch.cuda.synchronize()
     us = {}
     for e in prof.key_averages():
@@ -222,9 +238,9 @@ def decode_phases(torch, args):
     t0 = time.perf_counter()
     for _ in range(5):
         with torch.cuda.stream(loader._stream):
-            loader._decode_kernel(blobs)
+            loader._decode_kernel(blobs, idx)
     whole_ms = (time.perf_counter() - t0) * 1e3 / 5
-    print(json.dumps({"kernel_decode_batch": {
+    print(json.dumps({"indexed_decode_batch" if indexed else "kernel_decode_batch": {
         "files_on_device": len(acc), "entropy_MB": round(staging.numel() / 1e6, 2),
         "subsequences": int(segs["nsub"].sum()), "max_block_rounds": rounds, "flagged": int((status.numpy() != 0).sum()),
         "us_per_batch_by_kernel": us, "decode_call_ms": round(call_ms, 2),
@@ -260,14 +276,15 @@ def kernel_time(torch, args):
     loader.close()
 
 
-def eval_pass(torch, args, decode):
+def eval_pass(torch, args, decode, indexed=False):
     """One pass of Resize(256) + CenterCrop(224) batches through the eval-mode forward, against the same number of
     forwards on a resident batch."""
     from bdbnn_b200.data import ImageNetDeviceLoader
     from bdbnn_b200.resnet import resnet18
     torch.manual_seed(0)
     model = resnet18().cuda().eval()
-    loader = ImageNetDeviceLoader(os.path.join(args.root, "train"), BATCH, False, drop_last=True, decode=decode)
+    loader = ImageNetDeviceLoader(os.path.join(args.root, "train"), BATCH, False, drop_last=True, decode=decode,
+                                  jpeg_index=_index_path(args) if indexed else None)
     n = min(len(loader), 40)
     x = torch.empty(BATCH, 3, 224, 224, device="cuda").contiguous(memory_format=torch.channels_last)
     y = torch.empty(BATCH, dtype=torch.int64, device="cuda")
@@ -285,7 +302,8 @@ def eval_pass(torch, args, decode):
             model(x)
         torch.cuda.synchronize()
         resident = n * BATCH / (time.perf_counter() - t0)
-    print(json.dumps({"eval_img_per_s": {f"loader_{decode}": round(fed, 1), "resident": round(resident, 1),
+    print(json.dumps({"eval_img_per_s": {f"loader_{decode}{'_indexed' if indexed else ''}": round(fed, 1),
+                                         "resident": round(resident, 1),
                                          "batches": n}}), flush=True)
     loader.close()
 
@@ -305,7 +323,9 @@ def main():
     ap.add_argument("--steps", type=int, default=70)
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--images", type=int, default=90 * BATCH)
-    ap.add_argument("--arm", choices=("a", "b", "c", "d", "e", "extras"), help=argparse.SUPPRESS)
+    ap.add_argument("--arms", default="abcdef", help="the arms to alternate, a subset of abcdef")
+    ap.add_argument("--skip-extras", action="store_true", help="skip the once-only measurements after the rounds")
+    ap.add_argument("--arm", choices=("a", "b", "c", "d", "e", "f", "extras"), help=argparse.SUPPRESS)
     ap.add_argument("--root", help=argparse.SUPPRESS)
     args = ap.parse_args()
     import torch
@@ -315,8 +335,10 @@ def main():
         loaders_alone(torch, args)
         kernel_time(torch, args)
         decode_phases(torch, args)
+        decode_phases(torch, args, indexed=True)
         eval_pass(torch, args, "cpu")
         eval_pass(torch, args, "kernel")
+        eval_pass(torch, args, "kernel", indexed=True)
         return
     if args.arm:
         arm(torch, args)
@@ -331,18 +353,27 @@ def main():
         mean_bytes = write_folder(tmp, args.images)
         _warm(tmp)
         args.root = tmp
+        from bdbnn_b200.jpeg_index import build_jpeg_index
+        built = build_jpeg_index(os.path.join(tmp, "train"), _index_path(args), workers=16)
+        built["bytes_per_image"] = round(built["bytes"] / built["files"], 1)
+        built["host_cpus"] = os.cpu_count()
         print(json.dumps({"gpu": q.stdout.strip().splitlines()[0] if q.returncode == 0 else None, "batch": BATCH,
                           "images": args.images, "mean_file_KB": round(mean_bytes / 1e3, 1), "steps": args.steps,
                           "warmup": args.warmup, "rounds": args.rounds, "host_cpus": os.cpu_count(),
                           "write_s": round(time.perf_counter() - t0, 1), "page_cache": "warm"}), flush=True)
-        res = {a: [] for a in "abcde"}
+        print(json.dumps({"index_build": built}), flush=True)
+        res = {a: [] for a in args.arms}
         for _ in range(args.rounds):
-            for a in "abcde":
+            for a in args.arms:
                 r = _run(args, a)
                 print(json.dumps(r), flush=True)
                 res[a].append(r["img_per_s"])
         med = {a: sorted(v)[len(v) // 2] for a, v in res.items() if v}
-        if len(med) == 5:
+        print(json.dumps({"img_per_s_median": med}), flush=True)
+        if "f" in med and "c" in med and "e" in med:
+            print(json.dumps({"f_over_c_median": round(med["f"] / med["c"], 3),
+                              "f_over_e_median": round(med["f"] / med["e"], 3)}), flush=True)
+        if len(med) >= 5 and all(a in med for a in "abcde"):
             print(json.dumps({"img_per_s": res, "b_over_d_median": round(med["b"] / med["d"], 4),
                               "c_over_d_median": round(med["c"] / med["d"], 4),
                               "b_over_a_median": round(med["b"] / med["a"], 3),
@@ -350,7 +381,7 @@ def main():
                               "e_over_d_median": round(med["e"] / med["d"], 4),
                               "e_over_c_median": round(med["e"] / med["c"], 3)}), flush=True)
         cmd = [sys.executable, os.path.abspath(__file__), "--arm", "extras", "--root", tmp]
-        if subprocess.run(cmd).returncode != 0:                 # its results stream to stdout as they come
+        if not args.skip_extras and subprocess.run(cmd).returncode != 0:     # its results stream to stdout
             print("extras failed", flush=True)
     finally:
         shutil.rmtree(tmp, ignore_errors=True)
