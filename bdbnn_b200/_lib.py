@@ -140,6 +140,8 @@ SIGNATURES = {
     "bdbnn_jpeg_index_file": (c_int, [ctypes.c_char_p, c_int64, c_int, _P, c_size_t, _P, c_int64, _P, _P]),
     "bdbnn_jpeg_decode_batch_indexed": (c_int, [_P, _P, c_int, _P, _P, c_int, _P, _P, c_int64, _P, _P, c_int64, _P,
                                                 c_size_t, _P, c_int64, _P, _P, _P, _P]),
+    "bdbnn_jpeg_decode_batch_files": (c_int, [_P, _P, c_int64, _P, _P, _P, _P, c_int, _P, _P, c_int, _P, c_int64, _P,
+                                              _P, c_int64, _P, c_size_t, _P, c_int64, _P, _P, _P]),
 }
 
 

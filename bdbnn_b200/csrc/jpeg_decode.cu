@@ -22,6 +22,7 @@
 // Every bit read, table index and coefficient index is bounds-checked; an image whose stream is malformed, or whose
 // values leave the range where libjpeg-turbo's SIMD and C arithmetic agree, gets a nonzero status word.
 #include <limits.h>
+#include <stddef.h>
 #include <stdarg.h>
 
 #include <algorithm>
@@ -50,26 +51,39 @@ static int jp_sub_bits() {
 static const uint8_t kZigzag[64] = JP_ZIGZAG;
 __constant__ uint8_t c_zigzag[64] = JP_ZIGZAG;
 
-// ---- host parse ----------------------------------------------------------------------------------------------------
-#define JP_REJECT(...)                \
-  do {                                \
-    ::bdbnn::set_error(__VA_ARGS__);  \
-    return BDBNN_ERR_UNSUPPORTED;     \
-  } while (0)
+// ---- header parse, on the host (jp_parse) and on the device (jpeg_parse_kernel) ---------------------------------
+// Why jp_parse_head refused a file: the host reports kJpWhy[why], the device sets BDBNN_JPEG_RECORD.
+enum {
+  kJpOk, kJpNotJpeg, kJpBadMarker, kJpTruncated, kJpMarkerBeforeScan, kJpFrameHeader, kJpFrameParams, kJpSof, kJpDht,
+  kJpDqt, kJpDri, kJpShortJfif, kJpShortAdobe, kJpMarker, kJpNoFrame, kJpScanHeader, kJpScanOrder, kJpUndefTable,
+  kJpSpectral, kJpSampling, kJpAdobeTransform, kJpComponentIds, kJpDcTables, kJpAcTables, kJpHuffOverflow, kJpDcSymbol
+};
+static const char* const kJpWhy[] = {
+    "ok", "not a JPEG", "bad marker", "truncated", "marker before the scan", "frame header", "frame parameters",
+    "SOF other than 0 / 1", "DHT", "DQT", "DRI", "short JFIF marker", "short Adobe marker", "unknown marker",
+    "no frame header", "scan header", "scan component order", "a component uses an undefined table",
+    "spectral selection", "sampling", "Adobe transform", "component ids", "more than two DC tables",
+    "more than two AC tables", "Huffman code overflow", "DC symbol > 15"};
 
-struct JpRawHuff {
-  uint8_t bits[16];
-  uint8_t vals[256];
-  int n;
-  bool defined;
+// What the header fixes besides the descriptor's tables; scan: offset of the entropy-coded data (after SOS).
+struct JpHead {
+  int32_t H, W, ncomp, hmax, vmax, mcux, mcuy, bpm, restart;
+  int64_t scan;
 };
 
-// Canonical code assignment as jpeg_make_d_derived_tbl (which rejects the same tables).
-static int jp_build_huff(const JpRawHuff& r, bool is_dc, bdbnn_jpeg_huff* h) {
+__host__ __device__ __forceinline__ bool jp_same(const uint8_t* s, const char* lit, int n) {
+  for (int i = 0; i < n; ++i)
+    if (s[i] != uint8_t(lit[i])) return false;
+  return true;
+}
+
+// Canonical code assignment as jpeg_make_d_derived_tbl (which rejects the same tables); bits: the 16 code counts of
+// a DHT table, vals: its symbols.
+__host__ __device__ int jp_build_huff(const uint8_t* bits, const uint8_t* vals, bool is_dc, bdbnn_jpeg_huff* h) {
   memset(h, 0, sizeof(*h));
   int code = 0, i = 0;
   for (int L = 1; L <= 16; ++L) {
-    const int cnt = r.bits[L - 1];
+    const int cnt = bits[L - 1];
     if (cnt) {
       h->valoff[L] = i - code;
       h->maxcode[L] = code + cnt - 1;
@@ -79,56 +93,54 @@ static int jp_build_huff(const JpRawHuff& r, bool is_dc, bdbnn_jpeg_huff* h) {
     for (int c = 0; c < cnt; ++c, ++code, ++i) {
       if (L <= 9) {
         const int lo = code << (9 - L), span = 1 << (9 - L);
-        for (int x = 0; x < span; ++x) h->lut[lo + x] = uint16_t((L << 8) | r.vals[i]);
+        for (int x = 0; x < span; ++x) h->lut[lo + x] = uint16_t((L << 8) | vals[i]);
       }
     }
-    if (code >= (1 << L)) JP_REJECT("jpeg_parse: Huffman code overflow");
+    if (code >= (1 << L)) return kJpHuffOverflow;
     code <<= 1;
   }
   h->maxcode[0] = -1;
   h->maxcode[17] = INT_MAX;
-  for (int k = 0; k < r.n; ++k) {
-    if (is_dc && r.vals[k] > 15) JP_REJECT("jpeg_parse: DC symbol %d > 15", r.vals[k]);
-    h->vals[k] = r.vals[k];
+  for (int k = 0; k < i; ++k) {
+    if (is_dc && vals[k] > 15) return kJpDcSymbol;
+    h->vals[k] = vals[k];
   }
-  return BDBNN_OK;
+  return kJpOk;
 }
 
-static int jp_parse(const uint8_t* d, int64_t n, bdbnn_jpeg_desc* o, uint8_t* out, int64_t out_cap,
-                    uint32_t* seg_off, int32_t seg_cap) {
-  if (n < 4 || d[0] != 0xFF || d[1] != 0xD8) JP_REJECT("jpeg_parse: not a JPEG");
+// The markers of file d[0, n) up to SOS: *g and the descriptor's tables (blk_comp onwards; the fields before them are
+// not touched).  Returns kJpOk or why the file is refused.  Every read stays inside [0, n).
+__host__ __device__ int jp_parse_head(const uint8_t* d, int64_t n, JpHead* g, bdbnn_jpeg_desc* o) {
+  if (n < 4 || d[0] != 0xFF || d[1] != 0xD8) return kJpNotJpeg;
   int64_t p = 2;
-  uint16_t qt[4][64];
-  bool q_def[4] = {false, false, false, false};
-  JpRawHuff raw[2][4];                            // [DC / AC][slot]
-  for (int c = 0; c < 2; ++c)
-    for (int t = 0; t < 4; ++t) raw[c][t].defined = false;
+  int32_t q_at[4] = {-1, -1, -1, -1};            // offset of each quantisation table's values, -1 = undefined
+  int q_prec[4] = {0, 0, 0, 0};
+  int32_t h_at[2][4] = {{-1, -1, -1, -1}, {-1, -1, -1, -1}};   // [DC / AC][slot]: offset of the 16 code counts
   bool have_frame = false, jfif = false;
   int adobe = -1, restart = 0, H = 0, W = 0, nf = 0;
   int cid[3] = {0, 0, 0}, ch[3] = {0, 0, 0}, cv[3] = {0, 0, 0}, cq[3] = {0, 0, 0};
   const uint8_t* sos = nullptr;
   int sos_len = 0;
   while (sos == nullptr) {
-    if (p + 2 > n || d[p] != 0xFF) JP_REJECT("jpeg_parse: bad marker at %lld", (long long)p);
+    if (p + 2 > n || d[p] != 0xFF) return kJpBadMarker;
     while (p + 1 < n && d[p + 1] == 0xFF) ++p;
-    if (p + 2 > n) JP_REJECT("jpeg_parse: truncated");
+    if (p + 2 > n) return kJpTruncated;
     const int m = d[p + 1];
     p += 2;
-    if (m == 0xD8 || m == 0xD9 || (m >= 0xD0 && m <= 0xD7) || m == 0x01 || m == 0x00)
-      JP_REJECT("jpeg_parse: marker 0x%02x before the scan", m);
-    if (p + 2 > n) JP_REJECT("jpeg_parse: truncated");
+    if (m == 0xD8 || m == 0xD9 || (m >= 0xD0 && m <= 0xD7) || m == 0x01 || m == 0x00) return kJpMarkerBeforeScan;
+    if (p + 2 > n) return kJpTruncated;
     const int L = (d[p] << 8) | d[p + 1];
-    if (L < 2 || p + L > n) JP_REJECT("jpeg_parse: truncated segment");
+    if (L < 2 || p + L > n) return kJpTruncated;
     const uint8_t* s = d + p + 2;
     const int ls = L - 2;
     if (m == 0xC0 || m == 0xC1) {
-      if (have_frame || ls < 6) JP_REJECT("jpeg_parse: frame header");
+      if (have_frame || ls < 6) return kJpFrameHeader;
       H = (s[1] << 8) | s[2];
       W = (s[3] << 8) | s[4];
       nf = s[5];
       if (s[0] != 8 || (nf != 1 && nf != 3) || ls != 6 + 3 * nf || H < 1 || W < 1 || H > kJpMaxSide ||
           W > kJpMaxSide)
-        JP_REJECT("jpeg_parse: frame parameters (precision %d, %d components, %d x %d)", s[0], nf, H, W);
+        return kJpFrameParams;
       for (int i = 0; i < nf; ++i) {
         cid[i] = s[6 + 3 * i];
         ch[i] = s[7 + 3 * i] >> 4;
@@ -137,20 +149,16 @@ static int jp_parse(const uint8_t* d, int64_t n, bdbnn_jpeg_desc* o, uint8_t* ou
       }
       have_frame = true;
     } else if (m >= 0xC2 && m <= 0xCF && m != 0xC4 && m != 0xC8 && m != 0xCC) {
-      JP_REJECT("jpeg_parse: SOF%d", m - 0xC0);
+      return kJpSof;
     } else if (m == 0xC4) {
       int q = 0;
       while (q < ls) {
-        if (q + 17 > ls) JP_REJECT("jpeg_parse: DHT");
+        if (q + 17 > ls) return kJpDht;
         const int tc = s[q] >> 4, th = s[q] & 15;
         int cnt = 0;
         for (int i = 0; i < 16; ++i) cnt += s[q + 1 + i];
-        if (tc > 1 || th > 3 || cnt > 256 || q + 17 + cnt > ls) JP_REJECT("jpeg_parse: DHT");
-        JpRawHuff& r = raw[tc][th];
-        memcpy(r.bits, s + q + 1, 16);
-        memcpy(r.vals, s + q + 17, size_t(cnt));
-        r.n = cnt;
-        r.defined = true;
+        if (tc > 1 || th > 3 || cnt > 256 || q + 17 + cnt > ls) return kJpDht;
+        h_at[tc][th] = int32_t(s + q + 1 - d);
         q += 17 + cnt;
       }
     } else if (m == 0xDB) {
@@ -158,92 +166,126 @@ static int jp_parse(const uint8_t* d, int64_t n, bdbnn_jpeg_desc* o, uint8_t* ou
       while (q < ls) {
         const int pq = s[q] >> 4, tq = s[q] & 15;
         const int len = 64 * (pq + 1);
-        if (pq > 1 || tq > 3 || q + 1 + len > ls) JP_REJECT("jpeg_parse: DQT");
-        for (int k = 0; k < 64; ++k)
-          qt[tq][kZigzag[k]] = pq ? uint16_t((s[q + 1 + 2 * k] << 8) | s[q + 2 + 2 * k]) : s[q + 1 + k];
-        q_def[tq] = true;
+        if (pq > 1 || tq > 3 || q + 1 + len > ls) return kJpDqt;
+        q_at[tq] = int32_t(s + q + 1 - d);
+        q_prec[tq] = pq;
         q += 1 + len;
       }
     } else if (m == 0xDD) {
-      if (ls != 2) JP_REJECT("jpeg_parse: DRI");
+      if (ls != 2) return kJpDri;
       restart = (s[0] << 8) | s[1];
     } else if (m == 0xE0) {
-      if (ls >= 5 && memcmp(s, "JFIF\0", 5) == 0) {
-        if (ls < 14) JP_REJECT("jpeg_parse: short JFIF marker");
+      if (ls >= 5 && jp_same(s, "JFIF\0", 5)) {
+        if (ls < 14) return kJpShortJfif;
         jfif = true;
       }
     } else if (m == 0xEE) {
-      if (ls >= 5 && memcmp(s, "Adobe", 5) == 0) {
-        if (ls < 12) JP_REJECT("jpeg_parse: short Adobe marker");
+      if (ls >= 5 && jp_same(s, "Adobe", 5)) {
+        if (ls < 12) return kJpShortAdobe;
         adobe = s[11];
       }
     } else if (m == 0xDA) {
       sos = s;
       sos_len = ls;
     } else if (!((m >= 0xE0 && m <= 0xEF) || m == 0xFE)) {
-      JP_REJECT("jpeg_parse: marker 0x%02x", m);
+      return kJpMarker;
     }
     p += L;
   }
-  if (!have_frame) JP_REJECT("jpeg_parse: no frame header");
-  if (sos_len != 4 + 2 * nf || sos[0] != nf) JP_REJECT("jpeg_parse: scan header");
+  if (!have_frame) return kJpNoFrame;
+  if (sos_len != 4 + 2 * nf || sos[0] != nf) return kJpScanHeader;
   int td[3], ta[3];
   for (int i = 0; i < nf; ++i) {
-    if (sos[1 + 2 * i] != cid[i]) JP_REJECT("jpeg_parse: scan component order");
+    if (sos[1 + 2 * i] != cid[i]) return kJpScanOrder;
     td[i] = sos[2 + 2 * i] >> 4;
     ta[i] = sos[2 + 2 * i] & 15;
-    if (cq[i] > 3 || !q_def[cq[i]] || td[i] > 3 || ta[i] > 3 || !raw[0][td[i]].defined || !raw[1][ta[i]].defined)
-      JP_REJECT("jpeg_parse: component %d uses an undefined table", i);
+    if (cq[i] > 3 || q_at[cq[i]] < 0 || td[i] > 3 || ta[i] > 3 || h_at[0][td[i]] < 0 || h_at[1][ta[i]] < 0)
+      return kJpUndefTable;
   }
-  if (sos[1 + 2 * nf] != 0 || sos[2 + 2 * nf] != 63 || sos[3 + 2 * nf] != 0)
-    JP_REJECT("jpeg_parse: spectral selection");
+  if (sos[1 + 2 * nf] != 0 || sos[2 + 2 * nf] != 63 || sos[3 + 2 * nf] != 0) return kJpSpectral;
   int hmax = 1, vmax = 1;
   if (nf == 1) {
     // one component, non-interleaved: the MCU is one block whatever the declared factors
-    if (ch[0] < 1 || ch[0] > 4 || cv[0] < 1 || cv[0] > 4) JP_REJECT("jpeg_parse: sampling");
+    if (ch[0] < 1 || ch[0] > 4 || cv[0] < 1 || cv[0] > 4) return kJpSampling;
   } else {
     const bool y_ok = (ch[0] == 1 && cv[0] == 1) || (ch[0] == 2 && cv[0] == 1) || (ch[0] == 2 && cv[0] == 2);
-    if (!y_ok || ch[1] != 1 || cv[1] != 1 || ch[2] != 1 || cv[2] != 1)
-      JP_REJECT("jpeg_parse: sampling %dx%d,%dx%d,%dx%d", ch[0], cv[0], ch[1], cv[1], ch[2], cv[2]);
+    if (!y_ok || ch[1] != 1 || cv[1] != 1 || ch[2] != 1 || cv[2] != 1) return kJpSampling;
     if (!jfif) {
-      if (adobe >= 0 && adobe != 1) JP_REJECT("jpeg_parse: Adobe transform %d", adobe);
-      if (adobe < 0 && !(cid[0] == 1 && cid[1] == 2 && cid[2] == 3)) JP_REJECT("jpeg_parse: component ids");
+      if (adobe >= 0 && adobe != 1) return kJpAdobeTransform;
+      if (adobe < 0 && !(cid[0] == 1 && cid[1] == 2 && cid[2] == 3)) return kJpComponentIds;
     }
     hmax = ch[0];
     vmax = cv[0];
   }
-  // descriptor
-  memset(o, 0, sizeof(*o));
-  o->H = H;
-  o->W = W;
-  o->ncomp = nf;
-  o->hmax = hmax;
-  o->vmax = vmax;
-  o->mcux = (W + 8 * hmax - 1) / (8 * hmax);
-  o->mcuy = (H + 8 * vmax - 1) / (8 * vmax);
-  o->restart = restart;
+  // descriptor tables
+  memset(o->blk_comp, 0, sizeof(*o) - offsetof(bdbnn_jpeg_desc, blk_comp));
+  g->H = H;
+  g->W = W;
+  g->ncomp = nf;
+  g->hmax = hmax;
+  g->vmax = vmax;
+  g->mcux = (W + 8 * hmax - 1) / (8 * hmax);
+  g->mcuy = (H + 8 * vmax - 1) / (8 * vmax);
+  g->restart = restart;
+  g->scan = p;
   int bpm = 0;
   for (int i = 0; i < hmax * vmax; ++i) o->blk_comp[bpm++] = 0;
   for (int c = 1; c < nf; ++c) o->blk_comp[bpm++] = uint8_t(c);
-  o->bpm = bpm;
+  g->bpm = bpm;
   int dslot[4] = {-1, -1, -1, -1}, aslot[4] = {-1, -1, -1, -1}, nd = 0, na = 0;
   for (int i = 0; i < nf; ++i) {
-    memcpy(o->qt[i], qt[cq[i]], sizeof(o->qt[i]));
+    const uint8_t* qv = d + q_at[cq[i]];
+    for (int k = 0; k < 64; ++k) {
+#ifdef __CUDA_ARCH__
+      const int z = c_zigzag[k];
+#else
+      const int z = kZigzag[k];
+#endif
+      o->qt[i][z] = q_prec[cq[i]] ? uint16_t((qv[2 * k] << 8) | qv[2 * k + 1]) : qv[k];
+    }
     if (dslot[td[i]] < 0) {
-      if (nd == 2) JP_REJECT("jpeg_parse: more than two DC tables");
+      if (nd == 2) return kJpDcTables;
       dslot[td[i]] = nd;
-      if (int rc = jp_build_huff(raw[0][td[i]], true, &o->dc[nd])) return rc;
+      const uint8_t* b = d + h_at[0][td[i]];
+      if (int why = jp_build_huff(b, b + 16, true, &o->dc[nd])) return why;
       ++nd;
     }
     if (aslot[ta[i]] < 0) {
-      if (na == 2) JP_REJECT("jpeg_parse: more than two AC tables");
+      if (na == 2) return kJpAcTables;
       aslot[ta[i]] = na;
-      if (int rc = jp_build_huff(raw[1][ta[i]], false, &o->ac[na])) return rc;
+      const uint8_t* b = d + h_at[1][ta[i]];
+      if (int why = jp_build_huff(b, b + 16, false, &o->ac[na])) return why;
       ++na;
     }
     o->comp_dc[i] = uint8_t(dslot[td[i]]);
     o->comp_ac[i] = uint8_t(aslot[ta[i]]);
   }
+  return kJpOk;
+}
+
+// ---- host parse ----------------------------------------------------------------------------------------------------
+#define JP_REJECT(...)                \
+  do {                                \
+    ::bdbnn::set_error(__VA_ARGS__);  \
+    return BDBNN_ERR_UNSUPPORTED;     \
+  } while (0)
+
+static int jp_parse(const uint8_t* d, int64_t n, bdbnn_jpeg_desc* o, uint8_t* out, int64_t out_cap,
+                    uint32_t* seg_off, int32_t seg_cap) {
+  memset(o, 0, sizeof(*o));
+  JpHead g;
+  if (int why = jp_parse_head(d, n, &g, o)) JP_REJECT("jpeg_parse: %s", kJpWhy[why]);
+  o->H = g.H;
+  o->W = g.W;
+  o->ncomp = g.ncomp;
+  o->hmax = g.hmax;
+  o->vmax = g.vmax;
+  o->mcux = g.mcux;
+  o->mcuy = g.mcuy;
+  o->bpm = g.bpm;
+  o->restart = g.restart;
+  const int restart = g.restart;
+  int64_t p = g.scan;
   // entropy-coded data: unstuff, split at RSTn, end at EOI
   const int64_t total = int64_t(o->mcux) * o->mcuy;
   int64_t w = 0;
@@ -582,6 +624,147 @@ jpeg_index_check_kernel(const bdbnn_jpeg_desc* __restrict__ descs, const bdbnn_j
   cnt[i] = nb;
   if (j + 1 < g.nsub && jp_pack(pos, b, k) != jp_entry_state(entries[i - s], j + 1, S)) bad = true;
   if (bad) atomicOr(status + g.img, BDBNN_JPEG_INDEX);
+}
+
+// ---- device: parse and unstuff of the original files (bdbnn_jpeg_decode_batch_files) -------------------------------
+// One thread per image: the header half of the host parse, building the descriptor's tables in place.  The
+// geometry the host took from the image's record stays as it is and is compared with the file's; any difference, or
+// anything the host parse refuses, flags the image with BDBNN_JPEG_RECORD and sets its scan offset to -1.
+__global__ void __launch_bounds__(128)
+jpeg_parse_kernel(const uint8_t* __restrict__ files, bdbnn_jpeg_file* __restrict__ ftab,
+                  bdbnn_jpeg_desc* __restrict__ descs, int n_img, int32_t* __restrict__ status) {
+  const int i = int(blockIdx.x) * 128 + int(threadIdx.x);
+  if (i >= n_img) return;
+  const bdbnn_jpeg_file f = ftab[i];
+  bdbnn_jpeg_desc* o = descs + i;
+  JpHead g;
+  const int why = jp_parse_head(files + f.off, f.size, &g, o);
+  const bool bad = why != kJpOk || g.H != o->H || g.W != o->W || g.ncomp != o->ncomp || g.hmax != o->hmax ||
+                   g.vmax != o->vmax || g.mcux != o->mcux || g.mcuy != o->mcuy || g.bpm != o->bpm ||
+                   g.restart != o->restart;
+  ftab[i].scan = bad ? -1 : int32_t(g.scan);
+  if (bad) atomicOr(status + i, BDBNN_JPEG_RECORD);
+}
+
+constexpr int kJpUnBytes = 16;                    // scan bytes per thread per tile of jpeg_unstuff_kernel
+
+__device__ __forceinline__ int jp_first_seg(const bdbnn_jpeg_seg* segs, int nseg, int img) {
+  int lo = 0, hi = nseg;                          // first segment of an image >= img
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (segs[mid].img < img) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo;
+}
+
+// Block-wide exclusive sum of v (every thread of a kJpThreads block calls it); *total receives the sum.
+__device__ __forceinline__ uint64_t jp_block_scan(uint64_t v, uint64_t* sh_warp, uint64_t* total) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  uint64_t incl = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint64_t u = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += u;
+  }
+  if (lane == 31) sh_warp[wid] = incl;
+  __syncthreads();
+  uint64_t before = 0, all = 0;
+#pragma unroll
+  for (int w = 0; w < kJpThreads / 32; ++w) {
+    const uint64_t x = sh_warp[w];
+    before += w < wid ? x : 0;
+    all += x;
+  }
+  __syncthreads();
+  *total = all;
+  return before + incl - v;
+}
+
+// One CUDA block per image: the host parse's unstuff and RST split, in parallel over tiles of kJpThreads x
+// kJpUnBytes scan bytes.  Within the scan an FF pairs with the next byte (00: a data FF, D0-D7: a segment end, D9:
+// the end of the scan, anything else refused), so a byte's fate follows from its predecessor: each thread counts the
+// data bytes and RST markers of its bytes before the scan's end, a block scan gives their positions, and a second
+// walk writes the bytes to data at the image's data_off.  The RST sequence, each segment's start (the record's, in
+// segs) and the total against data_bytes are checked; any difference sets BDBNN_JPEG_RECORD.  No byte is written at
+// or past data_off + data_bytes, and no byte past the file is read.
+__global__ void __launch_bounds__(kJpThreads)
+jpeg_unstuff_kernel(const uint8_t* __restrict__ files, const bdbnn_jpeg_file* __restrict__ ftab,
+                    const bdbnn_jpeg_desc* __restrict__ descs, const bdbnn_jpeg_seg* __restrict__ segs, int nseg,
+                    uint8_t* __restrict__ data, int32_t* __restrict__ status) {
+  __shared__ uint64_t sh_warp[kJpThreads / 32];
+  __shared__ unsigned long long sh_end;
+  const int img = blockIdx.x, t = threadIdx.x;
+  const bdbnn_jpeg_file f = ftab[img];
+  if (f.scan < 0) return;                         // the parse flagged the image
+  const bdbnn_jpeg_desc* d = descs + img;
+  const uint8_t* src = files + f.off;
+  const int s0 = jp_first_seg(segs, nseg, img), s1 = jp_first_seg(segs, nseg, img + 1);
+  const int64_t size = f.size, scan = f.scan, nbytes = d->data_bytes;
+  uint8_t* out = data + d->data_off;
+  int64_t out0 = 0, rst0 = 0;
+  bool bad = false, ended = false;
+  for (int64_t base = scan; base < size; base += int64_t(kJpThreads) * kJpUnBytes) {
+    const int64_t p0 = base + int64_t(t) * kJpUnBytes;
+    uint8_t b[kJpUnBytes + 1];
+#pragma unroll
+    for (int j = 0; j <= kJpUnBytes; ++j) b[j] = p0 + j < size ? __ldg(src + p0 + j) : 0;
+    const bool prev_ff = p0 > scan && p0 - 1 < size && __ldg(src + p0 - 1) == 0xFF;
+    // pair starts: an FF whose predecessor is not an FF; the end is the first pair start followed by D9
+    if (t == 0) sh_end = ULLONG_MAX;
+    __syncthreads();
+    int64_t end = INT64_MAX;
+#pragma unroll
+    for (int j = 0; j < kJpUnBytes; ++j) {
+      const bool tail = j == 0 ? prev_ff : b[j - 1] == 0xFF;
+      if (end == INT64_MAX && p0 + j + 1 < size && b[j] == 0xFF && !tail && b[j + 1] == 0xD9) end = p0 + j;
+    }
+    if (end != INT64_MAX) atomicMin(&sh_end, (unsigned long long)end);
+    __syncthreads();
+    const int64_t e = sh_end == ULLONG_MAX ? INT64_MAX : int64_t(sh_end);
+    uint32_t n_data = 0, n_rst = 0;
+#pragma unroll
+    for (int j = 0; j < kJpUnBytes; ++j) {
+      const int64_t p = p0 + j;
+      const bool tail = j == 0 ? prev_ff : b[j - 1] == 0xFF;
+      if (p >= e || p >= size || tail) continue;
+      if (b[j] != 0xFF) {
+        ++n_data;
+      } else if (p + 1 < size) {
+        const uint8_t c2 = b[j + 1];
+        if (c2 == 0x00) ++n_data;
+        else if (c2 >= 0xD0 && c2 <= 0xD7) ++n_rst;
+        else bad = true;                          // FF FF, or a foreign marker, before the end
+      }
+    }
+    uint64_t tile;
+    const uint64_t before = jp_block_scan((uint64_t(n_rst) << 32) | n_data, sh_warp, &tile);
+    int64_t w = out0 + int64_t(before & 0xFFFFFFFFu), k = rst0 + int64_t(before >> 32);
+#pragma unroll
+    for (int j = 0; j < kJpUnBytes; ++j) {
+      const int64_t p = p0 + j;
+      const bool tail = j == 0 ? prev_ff : b[j - 1] == 0xFF;
+      if (p >= e || p >= size || tail) continue;
+      if (b[j] != 0xFF || (p + 1 < size && b[j + 1] == 0x00)) {
+        if (w < nbytes) out[w] = b[j];
+        ++w;
+      } else if (p + 1 < size && b[j + 1] >= 0xD0 && b[j + 1] <= 0xD7) {
+        // RST k ends segment k: it must be D0 + k mod 8, and segment k + 1 must start where the record says
+        if (d->restart == 0 || b[j + 1] - 0xD0 != int(k & 7) || s0 + k + 1 >= s1 ||
+            segs[s0 + k + 1].off - d->data_off != w)
+          bad = true;
+        ++k;
+      }
+    }
+    out0 += int64_t(tile & 0xFFFFFFFFu);
+    rst0 += int64_t(tile >> 32);
+    if (e != INT64_MAX) {
+      ended = true;
+      break;
+    }
+  }
+  bad = __syncthreads_or(bad);
+  if (t == 0 && (bad || !ended || out0 != nbytes || rst0 + 1 != s1 - s0)) atomicOr(status + img, BDBNN_JPEG_RECORD);
 }
 
 // Phase 3: first[i] = blocks completed by the segment's earlier subsequences (one warp per segment).
@@ -1043,16 +1226,37 @@ extern "C" int bdbnn_jpeg_check_batch(const bdbnn_jpeg_desc* desc_host, int32_t 
   return jp_check(desc_host, n_img, seg_host, n_seg, data_bytes, rgb_bytes, work_bytes, &blocks, &pix, &n_sub);
 }
 
+// The original files of bdbnn_jpeg_decode_batch_files, parsed and unstuffed on the device.
+struct JpFiles {
+  const uint8_t* host;
+  uint8_t* dev;
+  int64_t bytes;
+  const bdbnn_jpeg_file* tab_host;
+  bdbnn_jpeg_file* tab_dev;
+};
+
 // bdbnn_jpeg_decode_batch, or with entries_dev set bdbnn_jpeg_decode_batch_indexed: jpeg_index_check_kernel
-// in place of jpeg_sync_kernel, the rest as it is.
+// in place of jpeg_sync_kernel, the rest as it is.  With files set (bdbnn_jpeg_decode_batch_files, entries_dev set
+// too), jpeg_parse_kernel and jpeg_unstuff_kernel build the tables and data_dev from the files first, and data_host
+// is NULL.
 static int jp_decode(const bdbnn_jpeg_desc* desc_host, bdbnn_jpeg_desc* desc_dev, int32_t n_img,
                      const bdbnn_jpeg_seg* seg_host, bdbnn_jpeg_seg* seg_dev, int32_t n_seg, const uint8_t* data_host,
                      uint8_t* data_dev, int64_t data_bytes, const uint16_t* entries_host, uint16_t* entries_dev,
                      int64_t n_entries, void* work, size_t work_bytes, uint8_t* rgb, int64_t rgb_bytes,
-                     int32_t* status_dev, int32_t* status_host, int32_t* rounds_host, void* stream) {
+                     int32_t* status_dev, int32_t* status_host, int32_t* rounds_host, void* stream,
+                     const JpFiles* files = nullptr) {
   int64_t blocks, pix, n_sub;
   if (int rc = jp_check(desc_host, n_img, seg_host, n_seg, data_bytes, rgb_bytes, work_bytes, &blocks, &pix, &n_sub))
     return rc;
+  if (files) {
+    BDBNN_REQUIRE(files->bytes >= 0, "jpeg_decode_batch_files: negative files_bytes");
+    for (int i = 0; i < n_img; ++i) {
+      const bdbnn_jpeg_file& f = files->tab_host[i];
+      BDBNN_REQUIRE(f.off >= 0 && f.size >= 0 && f.off <= files->bytes - f.size,
+                    "jpeg_decode_batch_files: image %d: file [%lld, +%d) outside the %lld bytes of files", i,
+                    (long long)f.off, f.size, (long long)files->bytes);
+    }
+  }
   const int S = jp_sub_bits();
   BDBNN_REQUIRE(!entries_dev || n_entries == n_sub - n_seg,
                 "jpeg_decode_batch_indexed: %lld entries, the segments' nsub - 1 sum to %lld", (long long)n_entries,
@@ -1064,9 +1268,21 @@ static int jp_decode(const bdbnn_jpeg_desc* desc_host, bdbnn_jpeg_desc* desc_dev
   jp_layout(blocks, n_sub, static_cast<uint8_t*>(work), &w);
   BDBNN_CUDA(cudaMemcpyAsync(desc_dev, desc_host, size_t(n_img) * sizeof(bdbnn_jpeg_desc), cudaMemcpyHostToDevice, st));
   BDBNN_CUDA(cudaMemcpyAsync(seg_dev, seg_host, size_t(n_seg) * sizeof(bdbnn_jpeg_seg), cudaMemcpyHostToDevice, st));
-  BDBNN_CUDA(cudaMemcpyAsync(data_dev, data_host, size_t(data_bytes), cudaMemcpyHostToDevice, st));
+  if (!files)
+    BDBNN_CUDA(cudaMemcpyAsync(data_dev, data_host, size_t(data_bytes), cudaMemcpyHostToDevice, st));
   BDBNN_CUDA(cudaMemsetAsync(w.coef, 0, size_t(blocks) * 128, st));
   BDBNN_CUDA(cudaMemsetAsync(status_dev, 0, size_t(n_img) * 4, st));
+  if (files) {
+    BDBNN_CUDA(cudaMemcpyAsync(files->dev, files->host, size_t(files->bytes), cudaMemcpyHostToDevice, st));
+    BDBNN_CUDA(cudaMemcpyAsync(files->tab_dev, files->tab_host, size_t(n_img) * sizeof(bdbnn_jpeg_file),
+                               cudaMemcpyHostToDevice, st));
+    jpeg_parse_kernel<<<unsigned((n_img + 127) / 128), 128, 0, st>>>(files->dev, files->tab_dev, desc_dev, n_img,
+                                                                     status_dev);
+    if (int rc = check_launch("jpeg_parse_kernel")) return rc;
+    jpeg_unstuff_kernel<<<unsigned(n_img), kJpThreads, 0, st>>>(files->dev, files->tab_dev, desc_dev, seg_dev, n_seg,
+                                                                data_dev, status_dev);
+    if (int rc = check_launch("jpeg_unstuff_kernel")) return rc;
+  }
 
   const unsigned sub_grid = unsigned((n_sub + kJpThreads - 1) / kJpThreads);
   if (entries_dev) {
@@ -1127,4 +1343,21 @@ extern "C" int bdbnn_jpeg_decode_batch_indexed(const bdbnn_jpeg_desc* desc_host,
   return jp_decode(desc_host, desc_dev, n_img, seg_host, seg_dev, n_seg, data_host, data_dev, data_bytes,
                    entries_host, entries_dev, n_entries, work, work_bytes, rgb, rgb_bytes, status_dev, status_host,
                    rounds_host, stream);
+}
+
+extern "C" int bdbnn_jpeg_decode_batch_files(const uint8_t* files_host, uint8_t* files_dev, int64_t files_bytes,
+                                             const bdbnn_jpeg_file* file_host, bdbnn_jpeg_file* file_dev,
+                                             const bdbnn_jpeg_desc* desc_host, bdbnn_jpeg_desc* desc_dev,
+                                             int32_t n_img, const bdbnn_jpeg_seg* seg_host, bdbnn_jpeg_seg* seg_dev,
+                                             int32_t n_seg, uint8_t* data_dev, int64_t data_bytes,
+                                             const uint16_t* entries_host, uint16_t* entries_dev, int64_t n_entries,
+                                             void* work, size_t work_bytes, uint8_t* rgb, int64_t rgb_bytes,
+                                             int32_t* status_dev, int32_t* status_host, void* stream) {
+  BDBNN_REQUIRE(files_host && files_dev && file_host && file_dev && desc_host && desc_dev && seg_host && seg_dev &&
+                    data_dev && entries_host && entries_dev && work && rgb && status_dev && status_host,
+                "jpeg_decode_batch_files: NULL pointer");
+  const JpFiles files{files_host, files_dev, files_bytes, file_host, file_dev};
+  return jp_decode(desc_host, desc_dev, n_img, seg_host, seg_dev, n_seg, nullptr, data_dev, data_bytes, entries_host,
+                   entries_dev, n_entries, work, work_bytes, rgb, rgb_bytes, status_dev, status_host, nullptr, stream,
+                   &files);
 }

@@ -386,6 +386,8 @@ _JSEG = np.dtype([("off", "<i8"), ("img", "<i4"), ("nbytes", "<i4"), ("mcu0", "<
                   ("sub0", "<i4"), ("nsub", "<i4")])
 assert _JSEG.itemsize == 32
 BDBNN_JPEG_INDEX = 64                            # status bit of bdbnn_jpeg_decode_batch_indexed
+BDBNN_JPEG_RECORD = 128                          # status bit of bdbnn_jpeg_decode_batch_files
+_JFILE = np.dtype([("off", "<i8"), ("size", "<i4"), ("scan", "<i4")])     # bdbnn_jpeg_file
 
 
 def jpeg_parse(data):
@@ -404,7 +406,7 @@ def jpeg_parse(data):
 
 def jpeg_segment_table(descs, rel_off, subseq_bits):
     """bdbnn_jpeg_seg rows of a batch: descs (_JDESC, data_off set), rel_off[i] the segment start offsets of image i
-    (relative to its data).  Segment k of image i holds MCUs [k R, min((k + 1) R, total)), R the restart interval
+    (relative to its data; the list is concatenated, so one array of every image's offsets in turn does too).  Segment k of image i holds MCUs [k R, min((k + 1) R, total)), R the restart interval
     (total without one), and max(1, ceil(8 bytes / subseq_bits)) subsequences."""
     nseg = descs["nseg"].astype(np.int64)
     n = int(nseg.sum())
@@ -477,6 +479,41 @@ def jpeg_decode_batch(descs, segs, staging, device, stream, entries=None):
                 status.data_ptr() + 4 * len(descs), ctypes.c_void_p(stream.cuda_stream)), "jpeg_decode_batch_indexed")
     _lib.count(6)
     return rgb, status[:len(descs)], status[len(descs):len(descs) + 1], work
+
+
+def jpeg_decode_batch_files(files, ftab, descs, segs, entries, data_bytes, device, stream):
+    """bdbnn_jpeg_decode_batch_files on `stream`: files the pinned uint8 host tensor holding the batch's original
+    files, ftab (_JFILE, off and size set), descs (_JDESC: the records' geometry, blk_comp and every offset set,
+    tables zero), segs (_JSEG), entries (uint16, as jpeg_decode_batch), data_bytes the size of the unstuffed-data
+    buffer.  Returns (rgb uint8 device tensor, pinned int32 status per image, desc_dev, data_dev, workspace); all are
+    ready, and files may be rewritten, once `stream` has run the queued work."""
+    lib = _lib.lib()
+    n_blocks = int((descs["mcux"].astype(np.int64) * descs["mcuy"] * descs["bpm"]).sum())
+    n_pix = int((descs["H"].astype(np.int64) * descs["W"]).sum())
+    n_sub = int(segs["nsub"].astype(np.int64).sum())
+    n_ent = len(entries)
+    with torch.cuda.device(device), torch.cuda.stream(stream):
+        files_dev = torch.empty(max(files.numel(), 1), dtype=torch.uint8, device=device)
+        ftab_dev = torch.empty(ftab.nbytes, dtype=torch.uint8, device=device)
+        data_dev = torch.empty(max(int(data_bytes), 1), dtype=torch.uint8, device=device)
+        desc_dev = torch.empty(descs.nbytes, dtype=torch.uint8, device=device)
+        seg_dev = torch.empty(segs.nbytes, dtype=torch.uint8, device=device)
+        work = torch.empty(lib.bdbnn_jpeg_workspace_bytes(n_blocks, n_sub), dtype=torch.uint8, device=device)
+        rgb = torch.empty(3 * n_pix, dtype=torch.uint8, device=device)
+        status_dev = torch.empty(len(descs), dtype=torch.int32, device=device)
+        # the entries' pinned copy lives in the status buffer's tail, so it stays alive while status is held
+        status = torch.empty(len(descs) + (n_ent + 1) // 2, dtype=torch.int32, pin_memory=True)
+        ent_host = status[len(descs):].view(torch.int16)[:n_ent]
+        ent_host.numpy()[:] = np.asarray(entries, np.uint16).view(np.int16)
+        ent_dev = torch.empty(max(n_ent, 1), dtype=torch.int16, device=device)
+        _lib.check(lib.bdbnn_jpeg_decode_batch_files(
+            files.data_ptr(), files_dev.data_ptr(), files.numel(), ftab.ctypes.data, ftab_dev.data_ptr(),
+            descs.ctypes.data, desc_dev.data_ptr(), len(descs), segs.ctypes.data, seg_dev.data_ptr(), len(segs),
+            data_dev.data_ptr(), int(data_bytes), ent_host.data_ptr(), ent_dev.data_ptr(), n_ent, work.data_ptr(),
+            work.numel(), rgb.data_ptr(), rgb.numel(), status_dev.data_ptr(), status.data_ptr(),
+            ctypes.c_void_p(stream.cuda_stream)), "jpeg_decode_batch_files")
+    _lib.count(8)
+    return rgb, status[:len(descs)], desc_dev, data_dev, work
 
 
 def _pil_decode(data):
@@ -878,15 +915,197 @@ class ImageNetDeviceLoader:
         self._pool.shutdown()
 
 
-def dataloader_imagenet(split='train', batch_size=128, data_path='./', distributed=False, **kwargs):
+def _ranges(first, count):
+    """Concatenated arange(first[k], first[k] + count[k]) over k, and the exclusive cumsum of count."""
+    count = np.asarray(count, np.int64)
+    start = np.concatenate([[0], np.cumsum(count)[:-1]]).astype(np.int64)
+    return np.repeat(np.asarray(first, np.int64) - start, count) + np.arange(int(count.sum())), start
+
+
+def _record_ok(r, seglens, n_entries_total, S):
+    """Mask of the device records of r that are consistent with themselves, as bdbnn_jpeg_check_batch and the
+    segment table need them (sides, sampling, MCU grid, segment count, ranges, segment lengths summing to data_bytes,
+    entry count); the loader host-decodes the others.  Vectorised over r."""
+    from .jpeg_pack import KIND_DEVICE, _MAX_DATA
+    i64 = lambda f: r[f].astype(np.int64)
+    H, W, nc, h, v, bpm = i64("H"), i64("W"), i64("ncomp"), i64("hmax"), i64("vmax"), i64("bpm")
+    mx, my, rst, nseg, nb = i64("mcux"), i64("mcuy"), i64("restart"), i64("nseg"), i64("data_bytes")
+    ok = (r["kind"] == KIND_DEVICE) & (H >= 1) & (W >= 1) & (H <= IMAGENET_MAX_SIDE) & (W <= IMAGENET_MAX_SIDE)
+    samp1 = (nc == 1) & (h == 1) & (v == 1) & (bpm == 1)
+    samp3 = (nc == 3) & (bpm == h * v + 2) & (((h == 1) & (v == 1)) | ((h == 2) & ((v == 1) | (v == 2))))
+    ok &= samp1 | samp3
+    ok &= (h >= 1) & (v >= 1)
+    hs, vs = np.maximum(h, 1), np.maximum(v, 1)
+    ok &= (mx == (W + 8 * hs - 1) // (8 * hs)) & (my == (H + 8 * vs - 1) // (8 * vs))
+    total = mx * my
+    R = np.where(rst > 0, rst, np.maximum(total, 1))
+    ok &= (rst >= 0) & (nseg >= 1) & (nseg == (total + R - 1) // R) & (nb >= 0) & (nb < _MAX_DATA)
+    sf, ef, ne = r["seg_first"].astype(np.uint64), r["entry_first"].astype(np.uint64), r["n_entries"].astype(np.int64)
+    ok &= (sf + nseg.clip(0).astype(np.uint64) <= np.uint64(len(seglens)))
+    ok &= (ef + ne.astype(np.uint64) <= np.uint64(n_entries_total))
+    k = np.nonzero(ok)[0]
+    if k.size:
+        at, start = _ranges(sf[k].astype(np.int64), nseg[k])
+        lens = seglens[at].astype(np.int64)
+        nsub = np.maximum(1, (8 * lens + S - 1) // S)
+        img = np.repeat(np.arange(k.size), nseg[k])
+        got = np.bincount(img, weights=lens, minlength=k.size).astype(np.int64)
+        want = np.bincount(img, weights=nsub - 1, minlength=k.size).astype(np.int64)
+        ok[k] = (got == nb[k]) & (want == ne[k])
+    return ok
+
+
+class PackedImageNetLoader(ImageNetDeviceLoader):
+    """ImageNetDeviceLoader over a pack file (bdbnn_b200.jpeg_pack: `python -m bdbnn_b200.jpeg_pack ROOT OUT`), with
+    the same surface, epoch permutation, sharding, crop and flip draws, eval geometry, read-ahead thread and batch
+    kernel, and batches bit-identical to ImageNetDeviceLoader(ROOT, decode='cpu').
+
+    pack: a path or a JpegPack built at the library's subsequence length.  Per batch the host only copies the
+    images' bytes out of the pack's memory map into a reused pinned arena (in `workers` threads) and builds the
+    descriptors, segment table and entries from the records with numpy; one bdbnn_jpeg_decode_batch_files call then
+    parses the markers, unstuffs the scans and decodes every device-kind image on the loader's stream.  Host-kind
+    files (progressive, CMYK, PNG, ...), records inconsistent with themselves and images the device flags (a record
+    that differs from its bytes: BDBNN_JPEG_RECORD; entries that do not fit: BDBNN_JPEG_INDEX; corrupt data) are
+    decoded on the host from the pack's bytes, as decode='cpu' decodes them.  decode_stats counts "device", "host"
+    (host-kind), "record" (inconsistent records), "flagged" (any device status), "record_flagged" and
+    "index_flagged".  samples holds (path relative to the packed folder, label) pairs."""
+
+    def __init__(self, pack, batch_size, train, seed=None, drop_last=False, rank=0, world_size=1, device=None, *,
+                 workers=16, mean=IMAGENET_MEAN, std=IMAGENET_STD):
+        from .jpeg_pack import JpegPack
+        if int(batch_size) < 1 or int(world_size) < 1 or not 0 <= int(rank) < int(world_size) or int(workers) < 1:
+            raise ValueError(f"PackedImageNetLoader: need batch_size >= 1, workers >= 1 and 0 <= rank < world_size, "
+                             f"got {batch_size}, {workers}, {rank}, {world_size}")
+        if seed is None:
+            seed = int(torch.randint(0, 2 ** 62, (), dtype=torch.int64))
+        if not 0 <= int(seed) < 2 ** 64:
+            raise ValueError(f"PackedImageNetLoader: seed must be in [0, 2^64), got {seed}")
+        device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        if device.type != "cuda":
+            raise ValueError(f"PackedImageNetLoader: the batch kernel needs a CUDA device, got {device}")
+        if device.index is None:
+            device = torch.device("cuda", torch.cuda.current_device())
+        self.pack = pack if isinstance(pack, JpegPack) else JpegPack(pack)
+        self.n = self.pack.count
+        if not 1 <= self.n < 2 ** 31:
+            raise ValueError(f"PackedImageNetLoader: need 1 <= n < 2^31 images in {self.pack.path}, found {self.n}")
+        self.labels = self.pack.records["label"].astype(np.int64)
+        self.samples = list(zip(self.pack.paths, self.labels.tolist()))
+        self.class_to_idx = dict(self.pack.class_to_idx)
+        self.batch_size, self.train, self.seed, self.drop_last = int(batch_size), bool(train), int(seed), bool(drop_last)
+        self.rank, self.world_size, self.device, self.decode = int(rank), int(world_size), device, "pack"
+        self.spans = shard_spans(self.n, self.batch_size, self.rank, self.world_size, self.drop_last)
+        self.kernel = ImageNetBatchKernel(device, mean, std)
+        self._workers = int(workers)
+        self._pool = ThreadPoolExecutor(self._workers)
+        self._ahead = ThreadPoolExecutor(1)
+        self._pending = None
+        self._stream = torch.cuda.Stream(device)
+        self._arena = None                       # pinned copy of a batch's files, reused
+        self.decode_stats = {"device": 0, "host": 0, "record": 0, "flagged": 0, "record_flagged": 0,
+                             "index_flagged": 0}
+        self._lock = threading.Lock()
+        self._next_epoch = 0
+
+    def gather(self, idx):
+        """(records of dataset indices idx, offsets of their files in the pinned arena, the arena): the files'
+        bytes copied out of the pack's map in the pool.  The previous batch's decode has been waited for, so nothing
+        reads the arena any more."""
+        r = self.pack.records[np.asarray(idx, np.int64)]
+        size = r["size"].astype(np.int64)
+        foff = np.concatenate([[0], np.cumsum((size + 15) // 16 * 16)])
+        if self._arena is None or self._arena.numel() < foff[-1]:
+            self._arena = torch.empty(int(foff[-1] * 1.25) + 4096, dtype=torch.uint8, pin_memory=True)
+        dst, src = self._arena.numpy(), self.pack.blobs
+        boff = r["blob_off"].astype(np.int64)
+
+        def copy(ks):
+            for k in ks:
+                dst[foff[k]:foff[k] + size[k]] = src[boff[k]:boff[k] + size[k]]
+        list(self._pool.map(copy, np.array_split(np.arange(len(r)), min(self._workers, len(r)))))
+        return r, foff[:-1], self._arena
+
+    def tables(self, r, foff):
+        """(device positions, _JFILE, _JDESC, _JSEG, entries, unstuffed bytes) of the records r whose files are at
+        foff in the arena: the positions k of r that _record_ok takes, with their descriptors laid out back to back."""
+        S = self.pack.S
+        j = np.nonzero(_record_ok(r, self.pack.seglens, self.pack.entries.size, S))[0]
+        a = r[j]
+        ftab = np.zeros(len(j), _JFILE)
+        ftab["off"], ftab["size"] = foff[j], a["size"]
+        descs = np.zeros(len(j), _JDESC)
+        from .jpeg_pack import GEOMETRY
+        for g in GEOMETRY:
+            descs[g] = a[g]
+        nb = a["data_bytes"].astype(np.int64)
+        doff = np.concatenate([[0], np.cumsum((nb + 16) // 16 * 16)])
+        descs["data_off"] = doff[:-1]
+        hv = (a["hmax"].astype(np.int64) * a["vmax"])[:, None]
+        col = np.arange(8)[None, :]
+        descs["blk_comp"] = np.where(col < hv, 0, np.where(col < a["bpm"][:, None], col - hv + 1, 0))
+        jpeg_batch_layout(descs)
+        nseg = a["nseg"].astype(np.int64)
+        at, start = _ranges(a["seg_first"], nseg)
+        lens = self.pack.seglens[at].astype(np.int64)
+        cum = np.cumsum(lens) - lens
+        rel = cum - np.repeat(cum[start], nseg) if len(j) else cum
+        segs = jpeg_segment_table(descs, [rel], S)
+        ent_at, _ = _ranges(a["entry_first"], a["n_entries"])
+        return j, ftab, descs, segs, self.pack.entries[ent_at], int(doff[-1])
+
+    def _prepare(self, epoch, batch_index):
+        """Gather and decode one batch on self._stream: (dataset indices, [(device tensor, hwc)], event)."""
+        idx = self.indices(epoch, batch_index)
+        r, foff, arena = self.gather(idx)
+        B = len(r)
+        out = [None] * B
+        with self._lock, torch.cuda.device(self.device), torch.cuda.stream(self._stream):
+            j, ftab, descs, segs, entries, nbytes = self.tables(r, foff)
+            if len(j):
+                end = int(foff[-1] + r["size"][-1]) if B else 0
+                rgb, status, _, _, _ = jpeg_decode_batch_files(arena[:end], ftab, descs, segs, entries, nbytes,
+                                                               self.device, self._stream)
+                done = torch.cuda.Event()
+                done.record(self._stream)
+                done.synchronize()
+                st = status.numpy()
+                for q, k in enumerate(j.tolist()):
+                    if st[q] == 0:
+                        H, W, o = int(descs["H"][q]), int(descs["W"][q]), int(descs["rgb_off"][q])
+                        out[k] = (rgb[o:o + H * W * 3].view(H, W, 3), True)
+                s = self.decode_stats
+                s["device"] += int((st == 0).sum())
+                s["flagged"] += int((st != 0).sum())
+                s["record_flagged"] += int((st & BDBNN_JPEG_RECORD != 0).sum())
+                s["index_flagged"] += int((st & BDBNN_JPEG_INDEX != 0).sum())
+            from .jpeg_pack import KIND_DEVICE
+            host_kind = int((r["kind"] != KIND_DEVICE).sum())
+            self.decode_stats["host"] += host_kind
+            self.decode_stats["record"] += B - len(j) - host_kind
+            rest = [k for k in range(B) if out[k] is None]
+            a = arena.numpy()
+            blobs = [bytes(a[foff[k]:foff[k] + int(r["size"][k])]) for k in rest]
+            for k, (t, hwc) in zip(rest, self._pool.map(self._host_decode, blobs)):
+                out[k] = (t.pin_memory().to(self.device, non_blocking=True), hwc)
+            ev = torch.cuda.Event()
+            ev.record(self._stream)
+        return idx, out, ev
+
+
+def dataloader_imagenet(split='train', batch_size=128, data_path='./', distributed=False, pack=None, **kwargs):
     """loader.py:52-85 on the device: ImageFolder data_path/train (RandomResizedCrop(224) + RandomHorizontalFlip,
     shuffled) or data_path/val (Resize(256) + CenterCrop(224), in order), normalised with loader.py's constants.
     distributed=True shards the training split over torch.distributed's ranks (the validation split is read whole by
-    every rank, as the reference's, which has no sampler there).  Keyword arguments go to ImageNetDeviceLoader."""
+    every rank, as the reference's, which has no sampler there).  Keyword arguments go to ImageNetDeviceLoader.
+    pack: a directory holding train.pack and val.pack (bdbnn_b200.jpeg_pack); the split is then read from its pack by
+    a PackedImageNetLoader, with the same batches, and data_path is not read."""
     train = split == 'train'
     rank, world = 0, 1
     if distributed and train:
         import torch.distributed as dist
         rank, world = dist.get_rank(), dist.get_world_size()
+    if pack is not None:
+        return PackedImageNetLoader(os.path.join(pack, 'train.pack' if train else 'val.pack'), batch_size, train,
+                                    rank=rank, world_size=world, **kwargs)
     return ImageNetDeviceLoader(os.path.join(data_path, 'train' if train else 'val'), batch_size, train, rank=rank,
                                 world_size=world, **kwargs)

@@ -869,6 +869,9 @@ typedef struct bdbnn_jpeg_seg {
                                      [-512, 511]) */
 #define BDBNN_JPEG_INDEX 64       /* bdbnn_jpeg_decode_batch_indexed: a subsequence's exit differs from the segment's
                                      next stored start, or a stored start is malformed */
+#define BDBNN_JPEG_RECORD 128     /* bdbnn_jpeg_decode_batch_files: the file differs from its record (geometry,
+                                     restart interval, segment count or lengths, data_bytes), or the host parse
+                                     refuses it */
 /* Subsequence length S in bits (1024, or the bdbnn_debug_jpeg_subseq_bits override). */
 BDBNN_API int bdbnn_jpeg_subseq_bits(void);
 /* Tests only: sets S to bits in [8, 2^20], 0 restores the default.  Process-wide. */
@@ -933,6 +936,35 @@ BDBNN_API int bdbnn_jpeg_decode_batch_indexed(const bdbnn_jpeg_desc* desc_host, 
                                               int64_t n_entries, void* work, size_t work_bytes, uint8_t* rgb,
                                               int64_t rgb_bytes, int32_t* status_dev, int32_t* status_host,
                                               int32_t* rounds_host, void* stream);
+
+/* ---- Decode from the original files (DESIGN.md §4m, bdbnn_b200/jpeg_pack.py) ----------------------------------------
+ * bdbnn_jpeg_decode_batch_indexed with the header parse and the unstuffing on the device.  files_host (files_bytes,
+ * pinned) holds the batch's original JPEG files; image i's is bytes [file[i].off, + file[i].size) (16-byte aligned
+ * offsets read fastest).  desc_host holds the image's record: H, W, ncomp, hmax, vmax, mcux, mcuy, bpm, restart, nseg,
+ * data_bytes, blk_comp as bdbnn_jpeg_check_batch requires, and the caller's data_off, coef_off and rgb_off; its
+ * other tables are zero.  seg_host, entries and every other
+ * argument as bdbnn_jpeg_decode_batch_indexed, except that data_dev is written by the device and has no host copy.
+ * On `stream`: files_host and file_host are copied to files_dev and file_dev; jpeg_parse_kernel (one thread per image)
+ * builds desc_dev's quantisation and Huffman tables, blk_comp, comp_dc and comp_ac from the file's markers and sets
+ * file_dev[i].scan; jpeg_unstuff_kernel (one CUDA block per image) writes the scan's unstuffed bytes to data_dev at
+ * data_off, segment k at the segment table's offset; then the indexed decode.  A file that the host parse refuses,
+ * or that differs from its record in geometry, restart interval, RST sequence, segment lengths or data_bytes, gets
+ * BDBNN_JPEG_RECORD; no kernel reads or writes outside the buffers whatever the records say.  When every record
+ * is true, desc_dev equals bdbnn_jpeg_parse's descriptor with the caller's offsets, data_dev its data, and the
+ * pixels those of bdbnn_jpeg_decode_batch. */
+typedef struct bdbnn_jpeg_file {
+  int64_t off;          /* caller: the file's first byte in files */
+  int32_t size;         /* caller: its bytes */
+  int32_t scan;         /* device: offset of its entropy-coded data, -1 if the parse flagged it */
+} bdbnn_jpeg_file;
+BDBNN_API int bdbnn_jpeg_decode_batch_files(const uint8_t* files_host, uint8_t* files_dev, int64_t files_bytes,
+                                            const bdbnn_jpeg_file* file_host, bdbnn_jpeg_file* file_dev,
+                                            const bdbnn_jpeg_desc* desc_host, bdbnn_jpeg_desc* desc_dev, int32_t n_img,
+                                            const bdbnn_jpeg_seg* seg_host, bdbnn_jpeg_seg* seg_dev, int32_t n_seg,
+                                            uint8_t* data_dev, int64_t data_bytes, const uint16_t* entries_host,
+                                            uint16_t* entries_dev, int64_t n_entries, void* work, size_t work_bytes,
+                                            uint8_t* rgb, int64_t rgb_bytes, int32_t* status_dev,
+                                            int32_t* status_host, void* stream);
 
 #ifdef __cplusplus
 }
