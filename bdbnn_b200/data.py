@@ -216,23 +216,23 @@ def _default_root(name):
     return os.path.join(base, "Data", name)
 
 
-def _dataloader(name, split, batch_size, root):
+def _dataloader(name, split, batch_size, root, seed):
     root = _default_root(name) if root is None else root
     train = split == "train"
     images, labels = load_cifar(root, name, train)
-    return CifarDeviceLoader(images, labels, batch_size, train, classes=_SPLITS[name][4])
+    return CifarDeviceLoader(images, labels, batch_size, train, seed=seed, classes=_SPLITS[name][4])
 
 
-def dataloader_cifar10(split='train', batch_size=128, root=None):
+def dataloader_cifar10(split='train', batch_size=128, root=None, seed=None):
     """loader.py:7-28 on the device: CIFAR-10 from root (default <script dir>/Data/cifar10), shuffled, augmented
-    for split == 'train', normalised with loader.py's constants.  Returns a CifarDeviceLoader."""
-    return _dataloader("cifar10", split, batch_size, root)
+    for split == 'train', normalised with loader.py's constants.  Returns a CifarDeviceLoader (seed: its seed)."""
+    return _dataloader("cifar10", split, batch_size, root, seed)
 
 
-def dataloader_cifar100(split='train', batch_size=128, root=None):
+def dataloader_cifar100(split='train', batch_size=128, root=None, seed=None):
     """loader.py:31-50 on the device (CIFAR-100 fine labels, normalised with the CIFAR-10 statistics as the reference
-    does).  Returns a CifarDeviceLoader."""
-    return _dataloader("cifar100", split, batch_size, root)
+    does).  Returns a CifarDeviceLoader (seed: its seed)."""
+    return _dataloader("cifar100", split, batch_size, root, seed)
 
 
 # ---------------------------------------------------------------------------------------------------------------------

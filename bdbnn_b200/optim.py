@@ -73,6 +73,26 @@ class _GraphMode:
             self._lr_dev.copy_(torch.tensor(lrs, dtype=torch.float32), non_blocking=False)
             self._lr_host = lrs
 
+    def state_dict(self):
+        """torch's layout.  In graph mode every parameter's `step` is the device step count (one host read), as a
+        CPU float32 scalar of its own, like torch.optim.Adam's: a checkpoint taken after replays carries the count the
+        replays reached, and loads into torch's optimizers and into these in either mode."""
+        sd = super().state_dict()
+        if self.graph_mode and self._step_dev is not None:
+            step = self._step_dev.detach().to("cpu", torch.float32).reshape(())
+            sd["state"] = {k: (dict(v, step=step.clone()) if "step" in v else v) for k, v in sd["state"].items()}
+        return sd
+
+    def load_state_dict(self, state_dict):
+        """torch's, then the device step count restarts from the loaded `step` (graph mode now, or at the next
+        enable_graph_mode())."""
+        super().load_state_dict(state_dict)
+        steps = [float(s["step"]) for s in self.state.values() if "step" in s]
+        if not self.graph_mode:
+            self._step_dev = None
+        elif self._step_dev is not None:
+            self._step_dev.fill_(max(steps) if steps else 0.0)
+
 
 def _device_of_params(param_groups):
     for group in param_groups:

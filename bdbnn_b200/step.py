@@ -314,6 +314,8 @@ class GraphedTrainStep:
         self.static_images = self.static_target = None
         self.launches_per_replay = 0
         self.out = None
+        self._warmed = 0                 # warm_step() calls since the last capture
+        self._side = None                # the stream of the warm-up steps and of the capture
 
     @property
     def meters(self):
@@ -341,28 +343,64 @@ class GraphedTrainStep:
         self.static_target = target.clone()
         opt.enable_graph_mode()
         cur = torch.cuda.current_stream()
-        # the capture stream, by default above the second stream's priority: where both have blocks pending, the
-        # chain the step waits for goes first (BDBNN_GRAPH_PRIO=0: equal priorities)
-        side = torch.cuda.Stream(priority=int(os.environ.get("BDBNN_GRAPH_PRIO", "-1")))
+        side = self._side_stream()
         side.wait_stream(cur)
         with torch.cuda.stream(side):
             # eager warm-up on the capture side stream: lazy initialisation (kernel attributes, tensor-map
-            # encoder, cuDNN algorithm choice for an fp32 teacher), optimizer / meter state, allocator pools
-            for _ in range(self.warmup):
+            # encoder, cuDNN algorithm choice for an fp32 teacher), optimizer / meter state, allocator pools;
+            # the warm_step() calls since the last capture count toward it
+            for _ in range(self.warmup - self._warmed):
                 self.step(self.static_images, self.static_target, epoch)
         cur.wait_stream(side)
+        self._warmed = 0
         torch.cuda.synchronize()
         self.graph = torch.cuda.CUDAGraph()
         n0 = _lib.launch_count()
         with torch.cuda.graph(self.graph, stream=side, capture_error_mode="thread_local"):
             self.out = self.step(self.static_images, self.static_target, epoch)
         self.launches_per_replay = _lib.launch_count() - n0
-        self._key = (tuple(images.shape), tuple(target.shape),
-                     bool(self.step.cfg.w_kurtosis and self.step.cfg.kurtepoch <= epoch))
+        self._key = self._key_of(images, target, epoch)
+
+    def _side_stream(self):
+        if self._side is None:
+            # the capture stream, by default above the second stream's priority: where both have blocks pending, the
+            # chain the step waits for goes first (BDBNN_GRAPH_PRIO=0: equal priorities)
+            self._side = torch.cuda.Stream(priority=int(os.environ.get("BDBNN_GRAPH_PRIO", "-1")))
+        return self._side
+
+    def _key_of(self, images, target, epoch):
+        return (tuple(images.shape), tuple(target.shape),
+                bool(self.step.cfg.w_kurtosis and self.step.cfg.kurtepoch <= epoch))
+
+    def wants_warm_step(self, images, target, epoch=0):
+        """True when a call with this batch would capture and fewer than `warmup` warm_step() calls precede it."""
+        return (self.graph is None or self._key_of(images, target, epoch) != self._key) and \
+            self._warmed < self.warmup
+
+    def warm_step(self, images, target, epoch=0):
+        """One eager optimisation step on this batch, on the capture stream, counted toward the warm-up of the next
+        capture.  A caller that feeds an epoch's batches in order, through warm_step() while wants_warm_step() and
+        through __call__ after, takes exactly one step per batch (no batch is repeated for the warm-up), so a
+        graphed run computes what the same run of the eager TrainStep computes.  The optimizer is in graph mode
+        from the first warm step on, as in the replays, and its learning rates are synced as before a replay.
+        Returns the step's (non-static) output dict."""
+        opt = self._optimizer()
+        if not hasattr(opt, "enable_graph_mode"):
+            raise RuntimeError("GraphedTrainStep needs bdbnn_b200.optim.FusedAdam / FusedSGD (graph mode)")
+        if not opt.graph_mode:
+            opt.enable_graph_mode()
+        opt.sync_lr()                       # the step reads the device learning rates, as a replay does
+        cur = torch.cuda.current_stream()
+        side = self._side_stream()
+        side.wait_stream(cur)
+        with torch.cuda.stream(side):
+            out = self.step(images, target, epoch)
+        cur.wait_stream(side)
+        self._warmed += 1
+        return out
 
     def __call__(self, images, target, epoch=0):
-        key = (tuple(images.shape), tuple(target.shape),
-               bool(self.step.cfg.w_kurtosis and self.step.cfg.kurtepoch <= epoch))
+        key = self._key_of(images, target, epoch)
         if self.graph is None or key != self._key:
             self.graph = None
             self._capture(images, target, epoch)        # the warm-up steps are real optimisation steps;
