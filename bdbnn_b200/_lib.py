@@ -32,6 +32,7 @@ SIGNATURES = {
     "bdbnn_act_pack": (c_int, [_P, c_int64, c_int, _P, _P, _P, c_int, _P]),
     "bdbnn_weight_pack": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, c_int, _P]),
     "bdbnn_weight_pack_multi": (c_int, [c_int] + [_P] * 12 + [c_int, _P]),
+    "bdbnn_weight_unpack_multi": (c_int, [c_int] + [_P] * 6 + [c_int, _P]),
     "bdbnn_bits_to_fp8": (c_int, [_P, c_int64, c_int, _P, _P]),
     "bdbnn_ede_scale": (c_int, [_P, _P, _P, _P, c_int64, _P]),
     "bdbnn_ce_topk_fwd_bwd": (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P]),

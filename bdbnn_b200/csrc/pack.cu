@@ -208,6 +208,35 @@ weight_wt_multi_kernel(const __grid_constant__ WPackTable tab, uint16_t one16) {
   weight_wt_body(tab.W[l], tab.alpha[l], tab.Cout[l], tab.Cin[l], tab.T[l], tab.wt[l], one16, t % tiles_x, t / tiles_x);
 }
 
+// ---- sign words of all binary convs of a loaded 1-bit model -> their forward operands, one launch ----
+// One block per filter (blk0 as in WPackTable).  Element i = t*Cin + c of filter o reads bit c%32 of word
+// [o][t][c/32]: the 32 lanes of a warp share one word, and the writes of a block run along the filter's row.
+// Per layer exactly one of wf (16-bit, one16 / one16|0x8000) or wf8 (e4m3 0x38 / 0xB8) is non-NULL.
+struct WUnpackTable {
+  const uint32_t* wsign[kPackMaxLayers];
+  uint16_t* wf[kPackMaxLayers];
+  uint8_t* wf8[kPackMaxLayers];
+  int32_t Cin[kPackMaxLayers], T[kPackMaxLayers];
+  int32_t blk0[kPackMaxLayers + 1];
+  int32_t n;
+};
+
+__global__ void __launch_bounds__(256)
+weight_unpack_multi_kernel(const __grid_constant__ WUnpackTable tab, uint16_t one16) {
+  const int l = wpack_find(tab.blk0, tab.n, int(blockIdx.x));
+  const int o = int(blockIdx.x) - tab.blk0[l];
+  const int Cin = tab.Cin[l], T = tab.T[l], Cw = (Cin + 31) / 32, per = Cin * T;
+  const uint32_t* ws = tab.wsign[l] + int64_t(o) * T * Cw;
+  uint16_t* wf = tab.wf[l];
+  uint8_t* wf8 = tab.wf8[l];
+  for (int i = threadIdx.x; i < per; i += blockDim.x) {
+    const int t = i / Cin, c = i - t * Cin;
+    const bool pos = (__ldg(ws + t * Cw + (c >> 5)) >> (c & 31)) & 1u;
+    if (wf8) wf8[int64_t(o) * per + i] = pos ? uint8_t(0x38) : uint8_t(0xB8);
+    else wf[int64_t(o) * per + i] = pos ? one16 : uint16_t(one16 | 0x8000u);
+  }
+}
+
 // sign bits -> fp8 e4m3 +-1 bytes (0x38 / 0xB8), C % 32 == 0: word w expands to 32 consecutive bytes.
 __global__ void __launch_bounds__(256)
 bits_to_fp8_kernel(const uint32_t* __restrict__ bits, int64_t n_words, uint4* __restrict__ out) {
@@ -433,6 +462,41 @@ extern "C" int bdbnn_weight_pack_multi(int32_t count, const float* const* W_host
     if (rc) return rc;
     weight_wt_multi_kernel<<<unsigned(tiles), dim3(32, 8), 0, st>>>(tab, one_bits(fmt));
     rc = check_launch("weight_wt_multi_kernel");
+    if (rc) return rc;
+  }
+  return BDBNN_OK;
+}
+
+extern "C" int bdbnn_weight_unpack_multi(int32_t count, const uint32_t* const* wsign_host, const int32_t* Cout_host,
+                                         const int32_t* Cin_host, const int32_t* taps_host, uint16_t* const* wf_host,
+                                         uint8_t* const* wf8_host, int32_t fmt, void* stream) {
+  BDBNN_REQUIRE(fmt == BDBNN_FMT_FP16 || fmt == BDBNN_FMT_BF16, "weight_unpack_multi: bad operand format");
+  BDBNN_REQUIRE(count >= 0, "weight_unpack_multi: bad count");
+  BDBNN_REQUIRE(count == 0 || (wsign_host && Cout_host && Cin_host && taps_host && wf_host && wf8_host),
+                "weight_unpack_multi: NULL table");
+  cudaStream_t st = cudaStream_t(stream);
+  for (int off = 0; off < count; off += kPackMaxLayers) {
+    const int cnt = count - off < kPackMaxLayers ? count - off : kPackMaxLayers;
+    WUnpackTable tab;
+    memset(&tab, 0, sizeof(tab));
+    tab.n = cnt;
+    int blocks = 0;
+    for (int i = 0; i < cnt; ++i) {
+      const int l = off + i;
+      BDBNN_REQUIRE(wsign_host[l] && ((wf_host[l] != nullptr) != (wf8_host[l] != nullptr)),
+                    "weight_unpack_multi: layer %d needs its sign words and exactly one of wf / wf8", l);
+      BDBNN_REQUIRE(Cout_host[l] > 0 && Cin_host[l] > 0 && taps_host[l] > 0 &&
+                        int64_t(Cin_host[l]) * taps_host[l] <= INT32_MAX,
+                    "weight_unpack_multi: bad dims in layer %d", l);
+      BDBNN_REQUIRE(int64_t(blocks) + Cout_host[l] <= INT32_MAX, "weight_unpack_multi: too many filters");
+      tab.wsign[i] = wsign_host[l]; tab.wf[i] = wf_host[l]; tab.wf8[i] = wf8_host[l];
+      tab.Cin[i] = Cin_host[l]; tab.T[i] = taps_host[l];
+      tab.blk0[i] = blocks;
+      blocks += Cout_host[l];
+    }
+    tab.blk0[cnt] = blocks;
+    weight_unpack_multi_kernel<<<unsigned(blocks), 256, 0, st>>>(tab, one_bits(fmt));
+    const int rc = check_launch("weight_unpack_multi_kernel");
     if (rc) return rc;
   }
   return BDBNN_OK;

@@ -884,15 +884,91 @@ def _prepacked(weight, fmt, use8):
     return _WeightPack._make(getattr(pre, f) for f in _WeightPack._fields)
 
 
+def _version_guard(t):
+    """(address, version) of t; an inference tensor has no version counter, so its guard is the address alone."""
+    return t.data_ptr(), (None if t.is_inference() else t._version)
+
+
+class PackedWeight:
+    """A binary conv's weight as a 1-bit model file holds it (bdbnn_b200.export, DESIGN.md §4v), in place of the fp32
+    weight: `sign` int32 [Cout][kh*kw][ceil(Cin/32)] (bit j of word k = 1 for +1, bdbnn_weight_pack's wsign layout) and
+    `alpha` fp32 [Cout], both on the device; `shape` is the fp32 weight's.  The eval units take it as their `weight`:
+    the forward operand is unpacked from the sign words (bdbnn_weight_unpack_multi) once per (format, operand width),
+    and kept in `cache` (a dict the owning module holds) under the guard of the words, as _Prepacked's.  No training
+    unit, module chain or weight pack takes it: there is no fp32 weight to give them."""
+
+    def __init__(self, sign, alpha, shape, cache):
+        self.sign, self.alpha, self.shape, self.cache = sign, alpha, torch.Size(shape), cache
+
+    @property
+    def device(self):
+        return self.sign.device
+
+    def cached(self, fmt, use8):
+        """The unpacked operand (wf int16 or wf8 uint8 [Cout, kh*kw, Cin]) for (fmt, use8) if it is current, else
+        None."""
+        hit = self.cache.get((fmt, bool(use8)))
+        if hit is None or hit[0] != (_version_guard(self.sign), _version_guard(self.alpha)):
+            return None
+        return hit[1]
+
+    def operands(self, fmt, use8):
+        """The _WeightPack the eval units read: alpha, the sign words and the forward operand for (fmt, use8)."""
+        if self.cached(fmt, use8) is None:
+            unpack_weights([(self, use8)])
+        op = self.cached(fmt, use8)
+        return _WeightPack(self.alpha, self.sign, None, None if use8 else op, op if use8 else None, None, None, None)
+
+
+def unpack_weights(items):
+    """items: list of (PackedWeight, use8).  Unpacks the forward operands of those not yet cached for the current
+    grad_mode() format in one bdbnn_weight_unpack_multi call (one launch per 32 layers) and caches them."""
+    fmt = grad_mode()[3]
+    todo = [(pw, bool(use8)) for pw, use8 in items if pw.cached(fmt, use8) is None]
+    if not todo:
+        return
+    for pw, _ in todo:
+        if not pw.sign.is_cuda:
+            raise RuntimeError(f"bdbnn_b200.unpack_weights: expected CUDA sign words, got device={pw.device}")
+    ops = []
+    for pw, use8 in todo:
+        cout, cin, kh, kw = pw.shape
+        ops.append(torch.empty((cout, kh * kw, cin), dtype=torch.uint8 if use8 else torch.int16, device=pw.device))
+    n = len(todo)
+    P, I = ctypes.c_void_p * n, ctypes.c_int32 * n
+    _lib.check(_lib.lib().bdbnn_weight_unpack_multi(
+        n, P(*[pw.sign.data_ptr() for pw, _ in todo]), I(*[pw.shape[0] for pw, _ in todo]),
+        I(*[pw.shape[1] for pw, _ in todo]), I(*[pw.shape[2] * pw.shape[3] for pw, _ in todo]),
+        P(*[0 if u8 else op.data_ptr() for (_, u8), op in zip(todo, ops)]),
+        P(*[op.data_ptr() if u8 else 0 for (_, u8), op in zip(todo, ops)]), fmt, _stream()), "weight_unpack_multi")
+    _lib.count((n + 31) // 32)
+    for (pw, use8), op in zip(todo, ops):
+        pw.cache[(fmt, use8)] = ((_version_guard(pw.sign), _version_guard(pw.alpha)), op)
+
+
+def _require_weight(weight, what):
+    """_require_cuda for a conv weight an eval unit takes: an fp32 tensor or a PackedWeight.  Returns the tensor that
+    gives its device."""
+    if isinstance(weight, PackedWeight):
+        if not weight.sign.is_cuda:
+            raise RuntimeError(f"bdbnn_b200.{what}: expected CUDA sign words, got device={weight.device}")
+        return weight.sign
+    _require_cuda(weight, what)
+    return weight
+
+
 def _unit_operands(x, weight, sh, caps, train, real=False):
     """(use8, activation, _WeightPack) of a fused unit's binary conv, caps = bdbnn_tc_supported(sh).
     train: the activation is x's _ActPack with the 16-bit copy (the backward reads it and the mask bits), completed
     from the packs its producer attached when they are current; the weight pack has the gradient operands.
     eval: the activation is the one operand the forward reads, x's `_bdbnn_eval_pack` when it matches.
-    The weights come from prepack_weights (real_prepack_weights) when it packed them for this forward.
+    The weights come from prepack_weights (real_prepack_weights) when it packed them for this forward, and from the
+    unpacked sign words when `weight` is a PackedWeight (eval only).
     real: W32/A1 conv (DESIGN.md §4p): fp16 real weights from real_weight_grad_pack, never fp8."""
     if real:
         _require_fp16s("the W32/A1 conv unit")
+    if train and isinstance(weight, PackedWeight):
+        raise RuntimeError("bdbnn_b200: a packed binary conv has no fp32 weight to train")
     fmt = grad_mode()[3]
     use8 = not real and bool(caps & 8) and use_fwd8(sh.Cin, sh.Cout, eval_unit=not train)
     if train:
@@ -902,6 +978,8 @@ def _unit_operands(x, weight, sh, caps, train, real=False):
         if act is None:
             ap = _act_pack(x, sh, fmt, xb=not use8, xb8=use8)
             act = ap.xb8 if use8 else ap.xb
+    if isinstance(weight, PackedWeight):
+        return use8, act, weight.operands(fmt, use8)
     wp = _prepacked(weight, fmt, use8)
     if wp is None and real:
         wp, = real_weight_grad_pack([weight], grad=train)
@@ -1928,8 +2006,8 @@ def conv_bn_add_eval(x, weight, gamma, beta, running_mean, running_var, eps, str
     alpha = 2^-ew, and z's copy is 16-bit."""
     _eval_only("conv_bn_add_eval")
     _require_cuda(x, "conv_bn_add_eval(x)")
-    _require_cuda(weight, "conv_bn_add_eval(weight)")
-    _same_device(x, weight, gamma, beta, running_mean, running_var, residual)
+    _same_device(x, _require_weight(weight, "conv_bn_add_eval(weight)"), gamma, beta, running_mean, running_var,
+                 residual)
     pad_sc = isinstance(shortcut, PadShortcut)
     if pad_sc:
         _check_pad_shortcut("conv_bn_add_eval", x, weight.shape, stride, residual, shortcut)
@@ -2515,8 +2593,7 @@ def conv_pool_bn_eval(x, weight, gamma, beta, running_mean, running_var, eps, pa
     rounded once), Hardtanh and the +-1 copy of z for the next unit (`_bdbnn_eval_pack`, as conv_bn_add_eval)."""
     _eval_only("conv_pool_bn_eval")
     _require_cuda(x, "conv_pool_bn_eval(x)")
-    _require_cuda(weight, "conv_pool_bn_eval(weight)")
-    _same_device(x, weight, gamma, beta, running_mean, running_var)
+    _same_device(x, _require_weight(weight, "conv_pool_bn_eval(weight)"), gamma, beta, running_mean, running_var)
     if not pool_unit_supported(x.shape, weight.shape, 1, padding):
         raise RuntimeError(f"bdbnn_b200.conv_pool_bn_eval: unsupported input {tuple(x.shape)} / weight "
                            f"{tuple(weight.shape)}")

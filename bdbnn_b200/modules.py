@@ -17,7 +17,7 @@ forward(x[N,Cin,H,W]) -> [N,Cout,Ho,Wo], differentiable through torch.autograd.
 import torch
 import torch.nn as nn
 
-from .functional import binact_conv2d, binconv2d, max_pool2d_nhwc
+from .functional import PackedWeight, binact_conv2d, binconv2d, max_pool2d_nhwc
 
 
 class BinarizeConv2d(nn.Conv2d):
@@ -131,6 +131,38 @@ class BinaryActivationConv2d(nn.Conv2d):
 
     def extra_repr(self):
         return super().extra_repr() + ", binarized=32W/1A"
+
+
+class PackedBinaryConv2d(nn.Module):
+    """A 1W/1A conv loaded from a 1-bit model file (bdbnn_b200.export, DESIGN.md §4v): the buffers `sign`, int32
+    [Cout][kh*kw][ceil(Cin/32)] in bdbnn_weight_pack's sign-word layout, and `alpha`, fp32 [Cout], and no fp32 weight.
+    `weight` is a functional.PackedWeight over them that only the eval units take (resnet._eval_unit, the VGG-Small
+    eval units), with its unpacked forward operands cached on this module.  Eval only: calling the module itself, the
+    module chain's conv, raises, since it would need the fp32 weight."""
+
+    impl = None
+
+    def __init__(self, in_chn, out_chn, kernel_size=3, stride=1, padding=1):
+        super().__init__()
+        self.in_channels, self.out_channels = in_chn, out_chn
+        self.kernel_size, self.stride, self.padding = (kernel_size,) * 2, (stride,) * 2, (padding,) * 2
+        self.register_buffer("sign", torch.zeros((out_chn, kernel_size * kernel_size, (in_chn + 31) // 32),
+                                                 dtype=torch.int32))
+        self.register_buffer("alpha", torch.zeros((out_chn,), dtype=torch.float32))
+        self._operands = {}
+
+    @property
+    def weight(self):
+        return PackedWeight(self.sign, self.alpha, (self.out_channels, self.in_channels, *self.kernel_size),
+                            self._operands)
+
+    def forward(self, x):
+        raise RuntimeError("PackedBinaryConv2d runs only inside the eval units (a CUDA fp32 input, eval mode, no grad, "
+                           "BDBNN_FUSE_BN on): it has no fp32 weight for the module chain")
+
+    def extra_repr(self):
+        return (f"{self.in_channels}, {self.out_channels}, kernel_size={self.kernel_size}, stride={self.stride}, "
+                f"padding={self.padding}, binarized=1W/1A packed")
 
 
 class MaxPool2dNHWC(nn.Module):

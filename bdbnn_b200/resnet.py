@@ -15,7 +15,8 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import functional as F_
-from .modules import BinarizeConv2d, BinaryActivationConv2d, HardBinaryConv, HardBinaryConv_cifar, MaxPool2dNHWC
+from .modules import (BinarizeConv2d, BinaryActivationConv2d, HardBinaryConv, HardBinaryConv_cifar, MaxPool2dNHWC,
+                      PackedBinaryConv2d)
 
 
 def _fused_unit(x, conv, bn, residual, shortcut=None):
@@ -49,9 +50,10 @@ def _eval_unit(x, conv, bn, residual, shortcut=None):
     no_grad / inference_mode only: with grad enabled the module chain keeps its autograd graph.  EDE changes only the
     backward, so it does not exclude a unit.  `shortcut` = functional.PadShortcut: the option-A shortcut of x, read
     in place, is the residual (the caller checked pad_shortcut_supported).  A BinaryActivationConv2d takes the eval
-    unit with its real-weight operands."""
+    unit with its real-weight operands, a PackedBinaryConv2d the unit with the operands unpacked from its sign words."""
     real = isinstance(conv, BinaryActivationConv2d)
-    if not (_eval_mode(x, bn) and (real or isinstance(conv, BinarizeConv2d)) and isinstance(bn, nn.BatchNorm2d)):
+    if not (_eval_mode(x, bn) and (real or isinstance(conv, (BinarizeConv2d, PackedBinaryConv2d))) and
+            isinstance(bn, nn.BatchNorm2d)):
         return None
     if not (bn.affine and bn.running_mean is not None and bn.running_var is not None):
         return None
@@ -108,20 +110,24 @@ def _prepack(model, x):
     Packs are never kept across forwards: the fused optimizers update parameters in place without bumping
     `_version`, so a cached pack could hold stale signs (or, for the real weights of BinaryActivationConv2d, stale
     values).  Those are packed in one more call (functional.real_prepack_weights) in the fp16s gradient mode; in the
-    others their units raise."""
+    others their units raise.  The PackedBinaryConv2d of a loaded 1-bit model have their operands unpacked from the
+    sign words in one launch (functional.unpack_weights) the first time, and cached on the modules after that."""
     if not (x.is_cuda and F_.fuse_enabled() and F_.prepack_enabled() and x.dtype == torch.float32):
         return False
     if not model.training and torch.is_grad_enabled():
         return False
-    items, real = [], []
+    items, real, packed = [], [], []
     for m in model.modules():
-        if (isinstance(m, BinarizeConv2d) and m.impl != "xnor" and m.weight.is_cuda and
+        if isinstance(m, PackedBinaryConv2d) and m.sign.is_cuda and not model.training:
+            packed.append((m.weight, F_.use_fwd8(m.in_channels, m.out_channels, eval_unit=True)))
+        elif (isinstance(m, BinarizeConv2d) and m.impl != "xnor" and m.weight.is_cuda and
                 not (model.training and m.ede_active)):
             cout, cin, kh, kw = m.weight.shape
             if (cin * kh * kw) % 32 == 0 and cin % 64 == 0 and cout % 32 == 0:
                 items.append((m.weight, F_.use_fwd8(cin, cout, eval_unit=not model.training)))
         elif isinstance(m, BinaryActivationConv2d) and m.weight.is_cuda and F_.grad_mode()[0] == "fp16s":
             real.append(m.weight)
+    F_.unpack_weights(packed)       # the sign words of a loaded 1-bit model: one launch, then cached
     if not items and not real:
         return False
     F_._PREPACKED.clear()

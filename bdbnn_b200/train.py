@@ -37,6 +37,7 @@ import torch.nn as nn
 import torchvision.models as tv_models
 
 from . import data as _data
+from . import export as _export
 from .realnet import RealBottleneckResNet, RealResNet, RealResNeXt
 from .step import (CIFAR_DIFFKURT, IMAGENET_DIFFKURT, TS_DIFFKURT, EvalStep, GraphedTrainStep, StepConfig, TrainStep,
                    cpt_tk, make_optimizer)
@@ -147,10 +148,30 @@ def check_args(args):
         raise ValueError("--jpeg-index needs --decode kernel")
     if args.dataset != 'imagenet' and (args.jpeg_index or args.pack or args.decode != 'cpu'):
         raise ValueError("--decode / --jpeg-index / --pack apply to --dataset imagenet only")
+    packed_resume(args)
     if args.gpu is not None and not 0 <= args.gpu < torch.cuda.device_count():
         raise ValueError(f"--gpu {args.gpu}: no such device ({torch.cuda.device_count()} visible)")
     if not torch.cuda.is_available():
         raise ValueError("training needs a CUDA device")
+
+
+def packed_resume(args):
+    """(family, arch, num_classes) of the file --resume names when it is a 1-bit model file (bdbnn_b200.export,
+    recognised by its magic), else None.  ValueError when that file cannot serve this run: it is eval-only (-e), and
+    its network must be the one -a / --dataset / --custom_resnet build (build_model)."""
+    if not (args.resume and os.path.isfile(args.resume) and _export.is_packed(args.resume)):
+        return None
+    with open(args.resume, "rb") as fh:
+        family, arch, num_classes, _ = _export.read_header(fh.read(_export.HEADER.size))
+    if not args.evaluate:
+        raise ValueError(f"--resume {args.resume}: a 1-bit model file is eval-only; evaluate it with -e")
+    want = (_export.family_of(args.dataset), args.arch, 10 if args.dataset == "cifar10" else 1000)
+    if not args.custom_resnet or (family, arch, num_classes) != want:
+        raise ValueError(f"--resume {args.resume}: the 1-bit model file holds {family} {arch} with {num_classes} "
+                         f"classes, but -a {args.arch} --dataset {args.dataset}"
+                         f"{' --custom_resnet' if args.custom_resnet else ''} builds "
+                         f"{'%s %s with %d classes' % want if args.custom_resnet else 'a torchvision network'}")
+    return family, arch, num_classes
 
 
 def _wrap_first(model, wrappers):
@@ -332,6 +353,15 @@ def main(argv=None):
             teacher.eval()
             teacher.module = _wrap_first(teacher.module, (FrozenResNeXtTeacher, FrozenBottleneckTeacher,
                                                           FrozenResNetTeacher, FrozenVGGTeacher)).eval()
+
+        if packed_resume(args) is not None:
+            model = data_parallel(_export.load_packed(args.resume, device), device)
+            log.info(model)
+            log.info(f"=> loaded 1-bit model '{args.resume}'")
+            train_loader, val_loader = make_loaders(args, device)
+            acc = validate(val_loader, EvalStep(model), 0, log, args.print_freq)
+            log.info(f'test acc : {acc["acc1"]}')
+            return {"log_path": log_path, "val": acc, "model": model, "optimizer": None}
 
         model = data_parallel(build_model(args), device)
         log.info(model)

@@ -18,7 +18,7 @@ import torch
 import torch.nn as nn
 
 from . import functional as F_
-from .modules import BinarizeConv2d, HardBinaryConv_cifar
+from .modules import BinarizeConv2d, HardBinaryConv_cifar, PackedBinaryConv2d
 from .resnet import _cifar_stem_qualifies, _eval_mode, _prepacked_weights
 
 
@@ -32,9 +32,10 @@ def _fused_ok(x, conv, bn):
 
 
 def _eval_ok(x, conv, bn):
-    """Eval unit: eval-mode BatchNorm under no_grad (resnet._eval_mode) on a binary conv."""
-    return (_eval_mode(x, bn) and isinstance(conv, BinarizeConv2d) and isinstance(bn, nn.BatchNorm2d) and
-            bn.affine and bn.running_mean is not None and bn.running_var is not None and conv.impl != "xnor")
+    """Eval unit: eval-mode BatchNorm under no_grad (resnet._eval_mode) on a binary conv, packed ones included."""
+    return (_eval_mode(x, bn) and isinstance(conv, (BinarizeConv2d, PackedBinaryConv2d)) and
+            isinstance(bn, nn.BatchNorm2d) and bn.affine and bn.running_mean is not None and
+            bn.running_var is not None and conv.impl != "xnor")
 
 
 class VGGSmall(nn.Module):

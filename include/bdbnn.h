@@ -107,6 +107,16 @@ BDBNN_API int bdbnn_weight_pack_multi(int32_t count, const float* const* W_host,
                             uint32_t* const* wsign_host, uint32_t* const* wmask_host, uint16_t* const* wf_host,
                             uint16_t* const* wt_host, uint8_t* const* wf8_host, float* const* gscale_host,
                             float* const* inv_gscale_host, int32_t fmt, void* stream);
+/* The inverse for the forward operands of a loaded 1-bit model (bdbnn_b200/export.py): per layer, the sign words
+ * wsign_bits [Cout][T][ceil(Cin/32)] (bit j of word k = 1 for +1, as bdbnn_weight_pack writes them) become
+ *   wf [(o*T+t)*Cin+c] = +-1 in format fmt (fp16 0x3C00/0xBC00, bf16 0x3F80/0xBF80)   or
+ *   wf8[(o*T+t)*Cin+c] = +-1 as e4m3 byte (0x38 / 0xB8),
+ * exactly one of wf_host[l] / wf8_host[l] non-NULL; byte-identical to bdbnn_weight_pack's wf / wf8 of a weight with
+ * those signs.  Any Cin (also the 16-channel convs bdbnn_weight_pack_multi does not take); taps = kh*kw.  One launch
+ * per 32 layers (one grid of sum(Cout) filter blocks). */
+BDBNN_API int bdbnn_weight_unpack_multi(int32_t count, const uint32_t* const* wsign_host, const int32_t* Cout_host,
+                              const int32_t* Cin_host, const int32_t* taps_host, uint16_t* const* wf_host,
+                              uint8_t* const* wf8_host, int32_t fmt, void* stream);
 /* sign bits -> fp8 e4m3 +-1 bytes [n_pix][C] (0x38 = +1, 0xB8 = -1), C % 32 == 0: operand of fwd_tc8. */
 BDBNN_API int bdbnn_bits_to_fp8(const uint32_t* sign_bits, int64_t n_pix, int32_t C, uint8_t* xb_fp8, void* stream);
 
