@@ -64,6 +64,8 @@ SIGNATURES = {
     "bdbnn_binconv_wgrad_tc": (c_int, [_P, c_int, _P, _P, _P, _P, _P, _SH, _P, c_size_t, _P]),
     "bdbnn_kurtosis_multi_fwd": (c_int, [_P, _P, _P, c_int, _P, _P, _P, _P]),
     "bdbnn_kurtosis_multi_bwd": (c_int, [_P, _P, _P, c_int, _P, _P, _P, c_int, _P]),
+    "bdbnn_sign_flips_multi": (c_int, [_P, _P, _P, c_int, _P, _P, c_int, _P]),
+    "bdbnn_weight_stats_multi": (c_int, [_P, _P, _P, c_int, _P, _P, _P, _P, _P]),
     "bdbnn_kd_logits_fwd_bwd": (c_int, [_P, _P, c_int, c_int, _P, _P, _P, _P]),
     "bdbnn_kd_layer_multi_fwd": (c_int, [_P, _P, _P, c_int, _P, _P, _P]),
     "bdbnn_kd_layer_multi_bwd": (c_int, [_P, _P, c_int, _P, _P, c_int, _P]),

@@ -11,7 +11,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libbdbnn_b200.so")
 STAMP = os.path.join(HERE, ".libbdbnn_b200.stamp")
 SOURCES = ["api.cu", "pack.cu", "binconv.cu", "losses.cu", "tc_conv.cu", "tc_wgrad.cu", "pool.cu", "bn.cu", "stem.cu", "step_ops.cu", "real_conv.cu",
-           "cifar_stem.cu", "cifar_data.cu", "imagenet_data.cu", "jpeg_decode.cu"]
+           "cifar_stem.cu", "cifar_data.cu", "imagenet_data.cu", "jpeg_decode.cu", "weight_stats.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--use_fast_math=false", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",

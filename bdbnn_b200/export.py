@@ -235,10 +235,10 @@ def load_packed(path, device="cuda"):
     return net
 
 
-def _identify(net):
-    """(family, arch) of a binary network this format describes; ValueError for any other model."""
+def _identify(net, what="save_packed"):
+    """(family, arch) of a binary network this format describes; ValueError, prefixed `what`, for any other model."""
     if any(isinstance(m, BinaryActivationConv2d) for m in net.modules()):
-        raise ValueError("save_packed: a step-1 network (BinaryActivationConv2d) has real-valued weights; only 1W/1A "
+        raise ValueError(f"{what}: a step-1 network (BinaryActivationConv2d) has real-valued weights; only 1W/1A "
                          "networks have a 1-bit form")
     if isinstance(net, R.ResNetImageNet):
         arch = {(2, 2, 2, 2): "resnet18", (3, 4, 6, 3): "resnet34"}.get(
@@ -251,7 +251,7 @@ def _identify(net):
         return "cifar", "resnet18"
     elif isinstance(net, V.VGGSmall):
         return "cifar", "vgg_small"
-    raise ValueError(f"save_packed: {type(net).__name__} is not one of the binary networks a 1-bit model file "
+    raise ValueError(f"{what}: {type(net).__name__} is not one of the binary networks a 1-bit model file "
                      f"describes ({', '.join(f'{f} {a}' for f, a in sorted(ARCHS))})")
 
 

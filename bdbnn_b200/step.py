@@ -49,6 +49,7 @@ class StepConfig:
     beta: float = 200.0                                          # train.py:169
     temperature: float = 4.0                                     # train.py:170 (unused by the layer loss)
     w_lambda_ce: float = 1.0                                     # undefined upstream unless --react (B2)
+    weight_flips: bool = False       # count the binary weights' sign flips of every update (DESIGN.md §4w)
 
 
 def select_hooked_weights(model, cfg: StepConfig):
@@ -180,6 +181,10 @@ class TrainStep:
         self._loss_sum = None       # device float64 sum of total loss*N (train.py:519 / 638 `losses` meter)
         self._t_stream = None       # second stream of the teacher forward
         self.hooked = select_hooked_weights(model, self.cfg)
+        self.flip_counter = None
+        if self.cfg.weight_flips:
+            from .weight_stats import SignFlipCounter
+            self.flip_counter = SignFlipCounter.for_model(model)
         if self.cfg.teacher_student and teacher is None:
             raise ValueError("teacher_student step needs a teacher model")
         if self.cfg.w_kurtosis:
@@ -220,6 +225,8 @@ class TrainStep:
         cfg = self.cfg
         output_teacher = None
         t_stream = None
+        if self.flip_counter is not None and not self.flip_counter.initialized:
+            self.flip_counter.init()          # the sign bits of the weights before the first update
         if cfg.teacher_student and images.is_cuda and os.environ.get("BDBNN_TEACHER_SIDE", "1") != "0":
             from .functional import KernelTimer
             if not KernelTimer.enabled:
@@ -284,6 +291,8 @@ class TrainStep:
         if self.grad_sync is not None:
             self.grad_sync()
         self.optimizer.step()                                                     # train.py:529
+        if self.flip_counter is not None:
+            self.flip_counter()                                                   # this update's sign flips
         det = lambda v: v.detach() if torch.is_tensor(v) else v
         return {"loss": loss.detach(), "ce": orig_loss.detach(), "kurt": det(kurt_reg), "kl": det(loss_kl),
                 "kl_c": det(loss_kl_c), "acc1": acc1, "acc5": acc5, "output": output.detach()}

@@ -8,7 +8,8 @@ models, graphed step, eval pass and fused optimizers.
 The flags are the reference's (train.py:64-171), with its names and defaults; INTEGRATION.md §4 has the table of
 what is honoured, what deviates and what is refused.  Per epoch: training steps over the loader, validation with
 EvalStep (one host read), the learning-rate schedule, `checkpoint.pth.tar` (and `model_best.pth.tar`) in the
-format of utils.save_checkpoint, `log.txt` and one row of `metrics.csv` under the log directory.
+format of utils.save_checkpoint, `log.txt` and one row of `metrics.csv` under the log directory; with --weight-stats
+also the binary layers' weight statistics (bdbnn_b200.weight_stats) in `weights.csv` and `weight_hist.csv`.
 
 Where this differs from train.py, and why:
   * the teacher checkpoint is loaded when the file named by --resume_teacher exists; train.py:260 tests the
@@ -38,6 +39,7 @@ import torchvision.models as tv_models
 
 from . import data as _data
 from . import export as _export
+from . import weight_stats as _wstats
 from .realnet import RealBottleneckResNet, RealResNet, RealResNeXt
 from .step import (CIFAR_DIFFKURT, IMAGENET_DIFFKURT, TS_DIFFKURT, EvalStep, GraphedTrainStep, StepConfig, TrainStep,
                    cpt_tk, make_optimizer)
@@ -134,6 +136,17 @@ def make_parser():
     p.add_argument('--pack', default=None, metavar='DIR',
                    help='ImageNet: directory holding train.pack / val.pack (bdbnn_b200.jpeg_pack)')
     p.add_argument('--eager', action='store_true', help='run the plain TrainStep instead of the CUDA-graphed step')
+    p.set_defaults(weight_stats=False)              # the option that sets it is run_parser()'s
+    return p
+
+
+def run_parser():
+    """The command line of `python -m bdbnn_b200.train`: make_parser()'s flags, which keep train.py's surface, plus
+    --weight-stats, which only adds files to the run's log directory (DESIGN.md §4w)."""
+    p = make_parser()
+    p.add_argument('--weight-stats', action='store_true',
+                   help='per epoch, the binary layers\' sign flips, kurtosis, STE share, alpha, binarisation error '
+                        'and histogram to weights.csv / weight_hist.csv (binary networks only)')
     return p
 
 
@@ -149,6 +162,13 @@ def check_args(args):
     if args.dataset != 'imagenet' and (args.jpeg_index or args.pack or args.decode != 'cpu'):
         raise ValueError("--decode / --jpeg-index / --pack apply to --dataset imagenet only")
     packed_resume(args)
+    if args.weight_stats:
+        if args.evaluate:
+            raise ValueError("--weight-stats records training; -e trains nothing")
+        if not args.custom_resnet:
+            raise ValueError("--weight-stats: torchvision's fp32 networks have no binary weights")
+        with torch.device("meta"):
+            _wstats.binary_layers(build_model(args))
     if args.gpu is not None and not 0 <= args.gpu < torch.cuda.device_count():
         raise ValueError(f"--gpu {args.gpu}: no such device ({torch.cuda.device_count()} visible)")
     if not torch.cuda.is_available():
@@ -224,7 +244,8 @@ def step_config(args):
                       w_lambda_kurtosis=args.w_lambda_kurtosis, kurtosis_mode=args.kurtosis_mode,
                       kurtepoch=args.kurtepoch, weight_name=tuple(args.weight_name or ('all',)),
                       remove_weight_name=args.remove_weight_name, teacher_student=args.imagenet_setting_step_2_ts,
-                      react=args.react, alpha=args.alpha, beta=args.beta, temperature=args.temperature)
+                      react=args.react, alpha=args.alpha, beta=args.beta, temperature=args.temperature,
+                      weight_flips=args.weight_stats)
 
 
 def make_scheduler(optimizer, dataset, epochs, start_epoch=0):
@@ -298,6 +319,49 @@ def validate(val_loader, evaluator, epoch, log=None, print_freq=10):
 
 
 METRICS = ("epoch", "lr", "train_loss", "train_acc1", "train_acc5", "val_loss", "val_acc1", "val_acc5", "best_acc1")
+WEIGHTS = ("epoch", "layer", "numel", "kurtosis", "kurtosis_target", "flips", "flip_rate", "ste_active", "alpha_mean",
+           "bin_error")
+WEIGHT_HIST = ("epoch", "layer", *_wstats.HIST_NAMES)
+
+
+class WeightStatsLog:
+    """--weight-stats: per epoch, one row per binary layer in weights.csv and weight_hist.csv, and one line in the
+    log.  The step's SignFlipCounter counts the epoch's updates; reset() zeroes it at the epoch's start."""
+
+    def __init__(self, log_path, model, tstep):
+        self.model, self.counter = model, tstep.flip_counter
+        targets = {}
+        if tstep.cfg.w_kurtosis:
+            targets = {id(p): t for p, t in zip(tstep.hooked.values(), tstep.targets)}
+        self.targets = [targets.get(id(m.weight)) for _, m in _wstats.binary_layers(model)]
+        self._fh = [open(os.path.join(log_path, name), 'w', newline='') for name in ('weights.csv', 'weight_hist.csv')]
+        self._csv = [csv.writer(fh) for fh in self._fh]
+        self._csv[0].writerow(WEIGHTS)
+        self._csv[1].writerow(WEIGHT_HIST)
+
+    def reset(self):
+        self.counter.reset()
+
+    def write(self, epoch, log):
+        rows = _wstats.layer_stats(self.model, self.counter)
+        for r, t in zip(rows, self.targets):
+            self._csv[0].writerow([epoch, r["layer"], r["numel"], repr(r["kurtosis"]), "" if t is None else repr(t),
+                                   r["flips"], repr(r["flip_rate"]), repr(r["ste_active"]), repr(r["alpha_mean"]),
+                                   repr(r["bin_error"])])
+            self._csv[1].writerow([epoch, r["layer"], *r["hist"]])
+        for fh in self._fh:
+            fh.flush()
+        n = sum(r["numel"] for r in rows)
+        rate = sum(r["flip_rate"] * r["numel"] for r in rows) / n
+        active = sum(r["ste_active"] * r["numel"] for r in rows) / n
+        kurt = [r["kurtosis"] for r in rows]
+        log.info(f"Weights: {len(rows)} binary layers, {sum(r['flips'] for r in rows)} sign flips ({rate:.3e} per "
+                 f"weight and step), kurtosis {min(kurt):.3f}-{max(kurt):.3f}, ste_active {active:.4f}, bin_error "
+                 f"{sum(r['bin_error'] for r in rows) / len(rows):.4f} (layer mean)")
+
+    def close(self):
+        for fh in self._fh:
+            fh.close()
 
 
 def _logger(log_path):
@@ -315,7 +379,7 @@ def main(argv=None):
     """Run the recipe the flags describe.  Returns {'log_path', 'best_acc1', 'best_epoch', 'epochs_run',
     'epoch_seconds', 'model', 'optimizer'}: epoch_seconds is the wall time of each epoch (training, validation,
     checkpoint); model and optimizer as trained, for callers that go on using them."""
-    args = make_parser().parse_args(argv)
+    args = run_parser().parse_args(argv)
     check_args(args)
     from utils.utils import save_checkpoint
     device = torch.device("cuda", args.gpu if args.gpu is not None else torch.cuda.current_device())
@@ -327,7 +391,7 @@ def main(argv=None):
     log_path = os.path.join(args.log_path, str(args.w_kurtosis_target), stamp)
     os.makedirs(log_path, exist_ok=True)
     log = _logger(log_path)
-    train_loader = val_loader = None
+    train_loader = val_loader = wlog = None
     # train.py:368 turns cuDNN autotuning on; a layer left on cuDNN would then pick algorithms by timing and two runs
     # could round differently, so it stays off and resume stays exact (the caller's settings come back at the end)
     cudnn_flags = torch.backends.cudnn.benchmark, torch.backends.cudnn.deterministic
@@ -392,6 +456,7 @@ def main(argv=None):
         ede = EdeSchedule(model, args.epochs, device) if args.ede else None
         tstep = TrainStep(model, optimizer, step_config(args), teacher=teacher)
         gstep = None if args.eager else GraphedTrainStep(tstep)
+        wlog = WeightStatsLog(log_path, model, tstep) if args.weight_stats else None
         full = None                                    # the shape of a full batch: the one the graph is captured at
         with open(os.path.join(log_path, 'metrics.csv'), 'w', newline='') as fh:
             metrics = csv.writer(fh)
@@ -407,6 +472,8 @@ def main(argv=None):
                 optimizer.sync_lr()
                 model.train()
                 tstep.reset_meters()
+                if wlog is not None:
+                    wlog.reset()
                 train_loader.set_epoch(epoch)
                 n, t0, out = len(train_loader), time.time(), None
                 for i, (images, target) in enumerate(train_loader):
@@ -427,6 +494,8 @@ def main(argv=None):
                                  f"Acc@5 {a['acc5']:6.2f}")
                 train = tstep.averages()
                 train_loss = float(out["loss"])                 # train.py:552: the last batch's loss
+                if wlog is not None:
+                    wlog.write(epoch, log)
                 val = validate(val_loader, evaluator, epoch, log, args.print_freq)
                 scheduler.step()
                 acc1 = val["acc1"]
@@ -447,6 +516,8 @@ def main(argv=None):
                 "optimizer": optimizer}
     finally:
         torch.backends.cudnn.benchmark, torch.backends.cudnn.deterministic = cudnn_flags
+        if wlog is not None:
+            wlog.close()
         for loader in (train_loader, val_loader):
             if hasattr(loader, "close"):
                 loader.close()

@@ -269,6 +269,31 @@ BDBNN_API int bdbnn_kurtosis_multi_bwd(const float* const* w_ptrs_host, const in
                              const float* gout, float* const* grad_ptrs_host, int32_t accumulate,
                              void* stream);
 
+/* ---- binary-weight statistics for the training log (DESIGN.md §4w) ----------------------------
+ * Both take L >= 0 layers, launched once per BDBNN_MAX_TENSORS of them; the pointer / numel / Cout arrays are HOST
+ * arrays of length L, each weight a dense fp32 tensor whose filters (dim 0) are contiguous runs of numel/Cout
+ * elements (NCHW or channels_last).
+ * sign_flips: the sign bits of each weight (bit 1 = -1: v < 0 or NaN; -0 is +1), packed 32 per uint32 word into
+ *   bits[l] (device, ceil(numel/32) words, tail bits 0).  init != 0 writes the bits and counts nothing (flips and
+ *   steps may be NULL).  Otherwise flips[l] (device uint64) += popcount(new bits ^ stored bits), the new bits are
+ *   stored, and steps[0] (device uint64, may be NULL) += 1.  Allocates nothing and never synchronises, so it can be
+ *   captured in a CUDA graph; the counts are integers, the same in every run.
+ * weight_stats: one block per (layer, filter), alpha_o = mean|W_o| in fp64.  Per layer l:
+ *   stats_out[l*3 + 0] = #(|W| <= 1) / numel,  [1] = mean_o alpha_o,
+ *   [2] = sum (W - alpha_o sign W)^2 / sum W^2 (0 when sum W^2 == 0);
+ *   hist_out[l*68 + c] (uint64): c < 64 counts q = fp32(W / alpha_o) with floor(8q) + 32 == c (q in [-4, 4)),
+ *   64 q < -4, 65 q >= 4, 66 weights of filters with alpha_o == 0, 67 q NaN.
+ *   filter_sums (double[F*4]) and filter_hist (uint32[F*68]) are device scratch, F = sum of Cout.  Filters are
+ *   added in filter order, so every output has the same bits in every run. */
+#define BDBNN_WSTAT_VALUES 3
+#define BDBNN_WSTAT_HIST 68
+BDBNN_API int bdbnn_sign_flips_multi(const float* const* w_ptrs_host, const int64_t* numel_host,
+                                     uint32_t* const* bits_ptrs_host, int32_t L, uint64_t* flips, uint64_t* steps,
+                                     int32_t init, void* stream);
+BDBNN_API int bdbnn_weight_stats_multi(const float* const* w_ptrs_host, const int64_t* numel_host,
+                                       const int32_t* cout_host, int32_t L, double* filter_sums,
+                                       uint32_t* filter_hist, double* stats_out, uint64_t* hist_out, void* stream);
+
 /* ---- KD logits loss (DistributionLoss.forward, utils/KD_loss.py:16-43; train.py:612) -----------
  * loss = -(1/N) sum_n sum_c softmax(t)[n,c] * log_softmax(s)[n,c]
  * grad_s[n,c] = (softmax(s) - softmax(t))[n,c] / N          (written when grad_s != NULL)
