@@ -66,6 +66,10 @@ SIGNATURES = {
     "bdbnn_kurtosis_multi_bwd": (c_int, [_P, _P, _P, c_int, _P, _P, _P, c_int, _P]),
     "bdbnn_sign_flips_multi": (c_int, [_P, _P, _P, c_int, _P, _P, c_int, _P]),
     "bdbnn_weight_stats_multi": (c_int, [_P, _P, _P, c_int, _P, _P, _P, _P, _P]),
+    "bdbnn_binconv_fwd_b1_eval": (c_int, [_P] * 8 + [_SH, _P]),
+    "bdbnn_binconv_fwd_b1_i16": (c_int, [_P] * 4 + [_SH, _P]),
+    "bdbnn_b1_popc_table": (c_int, [_P, c_int, c_int, c_int, _P, _P]),
+    "bdbnn_debug_b1_mma": (c_int, [_P] * 4),
     "bdbnn_kd_logits_fwd_bwd": (c_int, [_P, _P, c_int, c_int, _P, _P, _P, _P]),
     "bdbnn_kd_layer_multi_fwd": (c_int, [_P, _P, _P, c_int, _P, _P, _P]),
     "bdbnn_kd_layer_multi_bwd": (c_int, [_P, _P, c_int, _P, _P, c_int, _P]),

@@ -435,6 +435,8 @@ int launch_stem_wgrad(const uint16_t* gys, const uint16_t* xw, float* ws, size_t
 void set_tc_trace(long long* buf);
 long long* get_tc_trace();
 bool wgrad_tc_ok(const bdbnn_conv_shape* s);
+// shapes of the binary tensor-core conv (b1_conv.cu, DESIGN.md §4x)
+bool b1_shape_ok(const bdbnn_conv_shape* s);
 // grouped 3x3 convs (DESIGN.md §4t): the band B of the banded kernels (0 = not supported), and whether the banded
 // weight gradient has a plan
 int gconv_band(const bdbnn_conv_shape* s, int groups);

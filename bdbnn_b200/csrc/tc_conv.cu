@@ -678,7 +678,7 @@ extern "C" int bdbnn_tc_supported(const bdbnn_conv_shape* s) {
     if (i16 && v2) i16 = bdbnn_debug_conv_plan(s, 2, 1, plan, 12) == BDBNN_OK && plan[0] == 1;   // fp8 forward
   }
   return BDBNN_TC_FWD | BDBNN_TC_DGRAD | (wgrad_tc_ok(s) ? BDBNN_TC_WGRAD : 0) | (v2 ? BDBNN_TC_FWD8 : 0) |
-         (i16 ? BDBNN_TC_FWD_I16 : 0);
+         (i16 ? BDBNN_TC_FWD_I16 : 0) | (b1_shape_ok(s) ? BDBNN_TC_B1 : 0);
 }
 
 // The implicit GEMM of a forward conv: A = the +-1 activations (NHWC, fmt), B = the +-1 weights [Cout][T][Cin].

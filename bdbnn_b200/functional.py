@@ -127,6 +127,8 @@ def algorithmic_bytes(kernel, sh, gh=1):
         "fwd_tc8": n_in + n_w + 4 * n_out,                    # read fp8 +-1, write fp32 y
         "fwd_tc_eval": 2 * n_in + 2 * n_w + 4 * n_out,        # read bf16 +-1, write fp32 z (+ residual, copy)
         "fwd_tc8_eval": n_in + n_w + 4 * n_out,               # read fp8 +-1, write fp32 z (+ residual, copy)
+        "fwd_b1_eval": n_in // 8 + n_w // 8 + 4 * n_out,      # read sign bits, write fp32 z (+ residual, bits)
+        "fwd_b1_i16": n_in // 8 + n_w // 8 + 2 * n_out,       # read sign bits, write int16 y
         "dgrad": 4 * n_out + n_w // 8 + n_in // 8 + 4 * n_in,  # read gy, bits; write gx
         "wgrad": 4 * n_out + n_in // 8 + n_w // 8 + 4 * n_w,
         "grad_pack": 4 * n_out + 2 * gh * n_out,
@@ -242,8 +244,12 @@ def _get_act_pack(x, fmt):
     return None
 
 
+EVAL_BITS = -2      # `_bdbnn_eval_pack` format of sign words [N,H,W,C/32] (bdbnn_act_pack's sign bits)
+
+
 def _set_eval_pack(z, fmt, zb):
-    """Attach the eval units' +-1 copy of z (format fmt, -1 = fp8 bytes) for the next unit, stamped with z's version.
+    """Attach the eval units' +-1 copy of z (format fmt, -1 = fp8 bytes, EVAL_BITS = sign words) for the next unit,
+    stamped with z's version.
     Inference tensors have no version counter to guard the copy with, so they get none."""
     if not z.is_inference():
         z._bdbnn_eval_pack = (fmt, zb)
@@ -809,6 +815,41 @@ def use_fwd8(cin, cout, eval_unit):
     return cout % 128 == 0 or (cout == 64 and not eval_unit)
 
 
+TC_B1 = 64                      # bdbnn_tc_supported's BDBNN_TC_B1
+_B1_ENV = "BDBNN_B1"            # 1 (default): a 1-bit model's qualifying convs run on the binary tensor cores | 0
+
+
+def b1_enabled():
+    return os.environ.get(_B1_ENV, "1") != "0"
+
+
+def b1_selected(cin, cout, kernel, stride, padding):
+    """Whether a loaded 1-bit model's conv of this geometry runs on the binary tensor-core kernel (BDBNN_B1 on): the
+    shapes bdbnn_tc_supported marks BDBNN_TC_B1 (3x3, pad 1, stride 1 or 2, Cin 128/256/512, Cout % 64 == 0), where
+    the kernel was faster than the unpacked fp8 / 16-bit unit at every measured shape and batch (DESIGN.md §4x)."""
+    return (b1_enabled() and kernel == 3 and padding == 1 and stride in (1, 2) and cin in (128, 256, 512) and
+            cout % 64 == 0)
+
+
+def use_b1(sh, weight):
+    """The eval units' choice for conv sh: the binary tensor-core kernel for a PackedWeight of a selected geometry
+    (b1_selected) whose shape has bdbnn_tc_supported's BDBNN_TC_B1 bit.  An fp32 weight never takes it: its sign
+    words would have to be packed every forward."""
+    if not (isinstance(weight, PackedWeight) and sh.kh == sh.kw and
+            b1_selected(sh.Cin, sh.Cout, sh.kh, sh.stride, sh.pad)):
+        return False
+    return bool(int(_lib.lib().bdbnn_tc_supported(ctypes.byref(sh))) & TC_B1)
+
+
+def _b1_operands(x, sh):
+    """x's sign words [N,H,W,Cin/32] for the binary tensor-core conv: the ones its producer attached
+    (`_bdbnn_eval_pack` in format EVAL_BITS) when current, else bdbnn_act_pack's sign bits of x."""
+    xbits = _get_eval_pack(x, EVAL_BITS)
+    if xbits is None:
+        xbits = _act_pack(x, sh, grad_mode()[3], xb=False, xb8=False).sign
+    return xbits
+
+
 def conv_stats_enabled():
     return os.environ.get("BDBNN_CONV_STATS", "1") != "0"
 
@@ -904,13 +945,29 @@ class PackedWeight:
     def device(self):
         return self.sign.device
 
-    def cached(self, fmt, use8):
-        """The unpacked operand (wf int16 or wf8 uint8 [Cout, kh*kw, Cin]) for (fmt, use8) if it is current, else
-        None."""
-        hit = self.cache.get((fmt, bool(use8)))
+    def _current(self, key):
+        hit = self.cache.get(key)
         if hit is None or hit[0] != (_version_guard(self.sign), _version_guard(self.alpha)):
             return None
         return hit[1]
+
+    def cached(self, fmt, use8):
+        """The unpacked operand (wf int16 or wf8 uint8 [Cout, kh*kw, Cin]) for (fmt, use8) if it is current, else
+        None."""
+        return self._current((fmt, bool(use8)))
+
+    def popc_table(self):
+        """int32 [Cout][kh*kw]: the set bits of each (filter, tap)'s sign words, which the binary tensor-core conv
+        reads (bdbnn_b1_popc_table, DESIGN.md §4x).  Built once and cached under the same guard as the operands."""
+        table = self._current("b1")
+        if table is None:
+            cout, cin, kh, kw = self.shape
+            table = torch.empty((cout, kh * kw), dtype=torch.int32, device=self.device)
+            _lib.check(_lib.lib().bdbnn_b1_popc_table(_p(self.sign), cout, cin, kh * kw, _p(table), _stream()),
+                       "b1_popc_table")
+            _lib.count(1)
+            self.cache["b1"] = ((_version_guard(self.sign), _version_guard(self.alpha)), table)
+        return table
 
     def operands(self, fmt, use8):
         """The _WeightPack the eval units read: alpha, the sign words and the forward operand for (fmt, use8)."""
@@ -2003,7 +2060,8 @@ def conv_bn_add_eval(x, weight, gamma, beta, running_mean, running_var, eps, str
     `_bdbnn_eval_pack` = (format, +-1 copy of z) for the next unit: fp8 bytes (format -1) when Cout % 128 == 0 and
     BDBNN_FWD8 is on, else 16-bit in the grad_mode() format.  x's own `_bdbnn_eval_pack` is used when it matches this
     conv's operand.  `real_weight`: the conv is binact_conv2d (DESIGN.md §4p): fp16 weights folded with
-    alpha = 2^-ew, and z's copy is 16-bit."""
+    alpha = 2^-ew, and z's copy is 16-bit.  A PackedWeight that use_b1 selects runs on the binary tensor-core kernel
+    (bdbnn_binconv_fwd_b1_eval, DESIGN.md §4x) from x's sign words, and z carries its sign words (format EVAL_BITS)."""
     _eval_only("conv_bn_add_eval")
     _require_cuda(x, "conv_bn_add_eval(x)")
     _same_device(x, _require_weight(weight, "conv_bn_add_eval(weight)"), gamma, beta, running_mean, running_var,
@@ -2028,6 +2086,20 @@ def conv_bn_add_eval(x, weight, gamma, beta, running_mean, running_var, eps, str
     fmt = grad_mode()[3]
     st = _stream()
     key = _shape_key(sh)
+    if not pad_sc and not real_weight and use_b1(sh, weight):
+        xbits = _b1_operands(x, sh)
+        scale, shift = bn_eval_fold(gamma, beta, running_mean, running_var, eps, weight.alpha)
+        rc = _nhwc(residual.detach()) if residual is not None else None
+        z = torch.empty(z_shape, dtype=torch.float32, device=dev, memory_format=torch.channels_last)
+        zbits = torch.empty((n, sh.Ho, sh.Wo, cout // 32), dtype=torch.int32, device=dev)
+        nbytes = algorithmic_bytes("fwd_b1_eval", sh) + (4 * z.numel() if rc is not None else 0) + zbits.numel() * 4
+        with _timed("binconv_fwd_b1_eval", key, nbytes):
+            _lib.check(L.bdbnn_binconv_fwd_b1_eval(_p(xbits), _p(weight.sign), _p(weight.popc_table()), _p(scale),
+                                                   _p(shift), _p(rc), _p(z), _p(zbits), ctypes.byref(sh), st),
+                       "binconv_fwd_b1_eval")
+        _lib.count(1)
+        _set_eval_pack(z, EVAL_BITS, zbits)
+        return z
     pack = cout % 32 == 0
     out8 = pack and cout % 128 == 0 and fwd8_enabled() and not real_weight
     use8, xop, wp = _unit_operands(x, weight, sh, caps, train=False, real=real_weight)
@@ -2590,7 +2662,8 @@ def conv_pool_bn(x, weight, gamma, beta, running_mean, running_var, momentum, ep
 def conv_pool_bn_eval(x, weight, gamma, beta, running_mean, running_var, eps, padding=1):
     """hardtanh(BN_eval(max_pool2d(binconv2d(x, weight), 2, 2))) under no_grad: the int16 forward, then one kernel for
     the 2x2 integer max, the folded BatchNorm z = fp32(fp32(max * scale) + shift) (bn_eval_fold with alpha, each step
-    rounded once), Hardtanh and the +-1 copy of z for the next unit (`_bdbnn_eval_pack`, as conv_bn_add_eval)."""
+    rounded once), Hardtanh and the +-1 copy of z for the next unit (`_bdbnn_eval_pack`, as conv_bn_add_eval).  A
+    PackedWeight that use_b1 selects takes its int16 forward from bdbnn_binconv_fwd_b1_i16."""
     _eval_only("conv_pool_bn_eval")
     _require_cuda(x, "conv_pool_bn_eval(x)")
     _same_device(x, _require_weight(weight, "conv_pool_bn_eval(weight)"), gamma, beta, running_mean, running_var)
@@ -2604,10 +2677,19 @@ def conv_pool_bn_eval(x, weight, gamma, beta, running_mean, running_var, eps, pa
     fmt = grad_mode()[3]
     st = _stream()
     key = _shape_key(sh)
-    use8, xop, wp = _unit_operands(x, weight, sh, int(L.bdbnn_tc_supported(ctypes.byref(sh))), train=False)
     y = torch.empty((n, sh.Ho, sh.Wo, cout), dtype=torch.int16, device=dev)
-    _fwd_tc(sh, use8, xop, wp, fmt, y)
-    scale, shift = bn_eval_fold(gamma, beta, running_mean, running_var, eps, wp.alpha)
+    if use_b1(sh, weight):
+        xbits = _b1_operands(x, sh)
+        with _timed("binconv_fwd_b1_i16", key, algorithmic_bytes("fwd_b1_i16", sh)):
+            _lib.check(L.bdbnn_binconv_fwd_b1_i16(_p(xbits), _p(weight.sign), _p(weight.popc_table()), _p(y),
+                                                  ctypes.byref(sh), st), "binconv_fwd_b1_i16")
+        _lib.count(1)
+        alpha = weight.alpha
+    else:
+        use8, xop, wp = _unit_operands(x, weight, sh, int(L.bdbnn_tc_supported(ctypes.byref(sh))), train=False)
+        _fwd_tc(sh, use8, xop, wp, fmt, y)
+        alpha = wp.alpha
+    scale, shift = bn_eval_fold(gamma, beta, running_mean, running_var, eps, alpha)
     out8 = cout % 128 == 0 and fwd8_enabled()
     z = torch.empty((n, cout, ho, wo), dtype=torch.float32, device=dev, memory_format=torch.channels_last)
     zb = None if out8 else torch.empty((n, ho, wo, cout), dtype=torch.int16, device=dev)

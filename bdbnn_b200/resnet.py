@@ -111,7 +111,8 @@ def _prepack(model, x):
     `_version`, so a cached pack could hold stale signs (or, for the real weights of BinaryActivationConv2d, stale
     values).  Those are packed in one more call (functional.real_prepack_weights) in the fp16s gradient mode; in the
     others their units raise.  The PackedBinaryConv2d of a loaded 1-bit model have their operands unpacked from the
-    sign words in one launch (functional.unpack_weights) the first time, and cached on the modules after that."""
+    sign words in one launch (functional.unpack_weights) the first time, and cached on the modules after that; those
+    that run on the binary tensor-core kernel (functional.b1_selected) read the sign words and get no operand."""
     if not (x.is_cuda and F_.fuse_enabled() and F_.prepack_enabled() and x.dtype == torch.float32):
         return False
     if not model.training and torch.is_grad_enabled():
@@ -119,7 +120,8 @@ def _prepack(model, x):
     items, real, packed = [], [], []
     for m in model.modules():
         if isinstance(m, PackedBinaryConv2d) and m.sign.is_cuda and not model.training:
-            packed.append((m.weight, F_.use_fwd8(m.in_channels, m.out_channels, eval_unit=True)))
+            if not F_.b1_selected(m.in_channels, m.out_channels, m.kernel_size[0], m.stride[0], m.padding[0]):
+                packed.append((m.weight, F_.use_fwd8(m.in_channels, m.out_channels, eval_unit=True)))
         elif (isinstance(m, BinarizeConv2d) and m.impl != "xnor" and m.weight.is_cuda and
                 not (model.training and m.ede_active)):
             cout, cin, kh, kw = m.weight.shape

@@ -73,6 +73,8 @@ BDBNN_API int bdbnn_debug_trace(long long* device_buf);
 #define BDBNN_TC_FWD8 8   /* fp8 (e4m3 +-1) forward: bdbnn_binconv_fwd_tc8 */
 #define BDBNN_TC_FWD_I16 16 /* forward can store the integer accumulator as int16: bdbnn_binconv_fwd_tc_i16 */
 #define BDBNN_TC_EVAL 32    /* eval-mode forward of a grouped conv: bdbnn_real_gconv_supported only */
+#define BDBNN_TC_B1 64      /* binary tensor-core forward on sign bits: bdbnn_binconv_fwd_b1_eval / _i16 (3x3, pad 1,
+                             * stride 1 or 2, Cin 128, 256 or 512, Cout % 64 == 0) */
 BDBNN_API int bdbnn_tc_supported(const bdbnn_conv_shape* s);
 
 /* ---- activation sign/pack ---------------------------------------------------------------------
@@ -1000,6 +1002,32 @@ BDBNN_API int bdbnn_jpeg_decode_batch_files(const uint8_t* files_host, uint8_t* 
                                             uint16_t* entries_dev, int64_t n_entries, void* work, size_t work_bytes,
                                             uint8_t* rgb, int64_t rgb_bytes, int32_t* status_dev,
                                             int32_t* status_host, void* stream);
+
+/* ---- binary tensor-core conv (csrc/b1_conv.cu, DESIGN.md §4x) -----------------------------------------------
+ * A 3x3 conv (pad 1, stride 1 or 2) on wgmma .b1.and.popc, from sign bits only:
+ *   xbits  [N*H*W][Cin/32]  activation sign words, bdbnn_act_pack's sign_bits (bit j of word k = channel 32k+j,
+ *                           1 = +1); 16-byte aligned
+ *   wsign  [Cout][9][Cin/32] weight sign words, bdbnn_weight_pack's wsign_bits; 16-byte aligned
+ *   popc   [Cout][9]        bdbnn_b1_popc_table of wsign
+ * The integer y_int = sum over the valid taps of (+-1)(+-1) equals the other forward kernels' bit for bit
+ * (|y_int| <= 9*Cin).  Requires bdbnn_tc_supported(s) & BDBNN_TC_B1.  One launch each; nothing is allocated.
+ * fwd_b1_eval: z[p][o] = fp32(fp32(y_int * scale[o]) + shift[o]) (+ residual[p][o] in a third rounding), fp32 NHWC,
+ *              as bdbnn_binconv_fwd_tc_eval computes it; zbits (may be NULL) [N*Ho*Wo][Cout/32] = the sign words of z
+ *              as bdbnn_act_pack(z) writes them (bit = z >= 0: -0.0 -> 1, NaN -> 0).  residual may be NULL and must
+ *              not alias z.
+ * fwd_b1_i16:  y_int as int16 NHWC [N*Ho*Wo][Cout].
+ * b1_popc_table: table[o*T+t] = popcount of wsign's ceil(Cin/32) words of (o, t).
+ * debug_b1_mma: one m64n8k256 AND-popcount tile through the kernel's shared-memory layout: a [64][8] u32 and
+ *              b [8][8] u32 (device, 16-byte aligned; K element 32k+j = bit j of word k), d[m][n] =
+ *              sum_k popcount(a[m][k] & b[n][k]) as int32 [64][8]. */
+BDBNN_API int bdbnn_binconv_fwd_b1_eval(const uint32_t* xbits, const uint32_t* wsign, const int32_t* popc,
+                                        const float* scale, const float* shift, const float* residual, float* z,
+                                        uint32_t* zbits, const bdbnn_conv_shape* s, void* stream);
+BDBNN_API int bdbnn_binconv_fwd_b1_i16(const uint32_t* xbits, const uint32_t* wsign, const int32_t* popc,
+                                       int16_t* y_int, const bdbnn_conv_shape* s, void* stream);
+BDBNN_API int bdbnn_b1_popc_table(const uint32_t* wsign, int32_t Cout, int32_t Cin, int32_t T, int32_t* table,
+                                  void* stream);
+BDBNN_API int bdbnn_debug_b1_mma(const uint32_t* a, const uint32_t* b, int32_t* d, void* stream);
 
 #ifdef __cplusplus
 }

@@ -8,7 +8,9 @@ Arms, alternated round by round in one process, model.eval() under torch.no_grad
 (224x224 ImageNet, 32x32 CIFAR):
 
     ckpt_eager / ckpt_graphed      the source network (fp32 weights; the weight pack runs in every forward)
-    packed_eager / packed_graphed  the loaded 1-bit model (operands unpacked once, then cached)
+    packed_eager / packed_graphed  the loaded 1-bit model (operands unpacked once, then cached; its qualifying
+                                   convs on the binary tensor-core kernel, DESIGN.md §4x)
+    nob1_eager / nob1_graphed      the loaded 1-bit model with BDBNN_B1=0 (every conv on unpacked operands)
 
 Each arm's images/s is timed with CUDA events over --iters forwards.  Also printed: the checkpoint's size
 (torch.save of the state_dict) and the 1-bit file's, and the wall time of load_packed (read, check, build, copy to the
@@ -37,6 +39,21 @@ def _graphed(torch, model, x, warmup):
     with torch.cuda.graph(g):
         model(x)
     return g.replay
+
+
+def _b1_off(fn):
+    """fn run (or captured) with BDBNN_B1=0."""
+    def run(*a):
+        old = os.environ.get("BDBNN_B1")
+        os.environ["BDBNN_B1"] = "0"
+        try:
+            return fn(*a)
+        finally:
+            if old is None:
+                del os.environ["BDBNN_B1"]
+            else:
+                os.environ["BDBNN_B1"] = old
+    return run
 
 
 def main():
@@ -80,10 +97,12 @@ def main():
         torch.cuda.synchronize()
         load_s = time.perf_counter() - t0
         with torch.no_grad():
-            same = bool(torch.equal(out, src(x)))
+            same = bool(torch.equal(out, src(x))) and bool(torch.equal(_b1_off(net)(x), out))
             arms = {"ckpt_eager": lambda: src(x), "packed_eager": lambda: net(x),
                     "ckpt_graphed": _graphed(torch, src, x, args.warmup),
-                    "packed_graphed": _graphed(torch, net, x, args.warmup)}
+                    "packed_graphed": _graphed(torch, net, x, args.warmup),
+                    "nob1_eager": _b1_off(lambda: net(x)),
+                    "nob1_graphed": _b1_off(_graphed)(torch, net, x, args.warmup)}
             for fn in arms.values():
                 for _ in range(args.warmup):
                     fn()
